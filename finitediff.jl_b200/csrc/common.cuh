@@ -46,6 +46,57 @@ template <> __device__ __forceinline__ void ld_color_pair<int32_t>(const int32_t
   a = (uint32_t)v.x; b = (uint32_t)v.y;
 }
 
+// j / d and j mod d for a divisor fixed at plan time, j < 2^32: one multiply-high, two shifts and a multiply-add instead
+// of a division loop (Granlund & Montgomery, "Division by invariant integers using multiplication", PLDI 1994, fig. 4.1)
+struct FastDiv {
+  uint32_t d, magic, s1, s2;
+  __device__ __forceinline__ uint32_t div(uint32_t j) const {
+    const uint32_t t = __umulhi(j, magic);
+    return (t + ((j - t) >> s1)) >> s2;
+  }
+  __device__ __forceinline__ uint32_t mod(uint32_t j) const { return j - div(j) * d; }
+};
+inline FastDiv make_fastdiv(uint32_t d) {   // d >= 1
+  uint32_t l = 0;
+  while ((1ull << l) < d) ++l;
+  FastDiv f;
+  f.d = d;
+  f.magic = (uint32_t)(((1ull << 32) * ((1ull << l) - d)) / d + 1);
+  f.s1 = l > 0 ? 1 : 0;
+  f.s2 = l > 0 ? l - 1 : 0;
+  return f;
+}
+
+// Colour sources: where a kernel finds the 0-based colour of element j (a column, or a structural entry).
+//   TableColors<CT>  the plan's array, one CT per element (all-ones = no valid colour);
+//   CyclicColors     colorvec[j] == j mod P + 1 (what matrix_colors gives banded / tridiagonal matrices): the closed form,
+//                    no array is read.
+// tile(base, tid2, ...) yields the colours of the two element pairs a lane owns in the tile at `base` (common tile shape).
+template <typename CT> struct TableColors {
+  const CT *p;
+  __device__ __forceinline__ uint32_t at(int64_t j) const { return (uint32_t)__ldg(p + j); }
+  __device__ __forceinline__ void tile(int64_t base, int tid2, uint32_t &a0, uint32_t &a1, uint32_t &b0, uint32_t &b1) const {
+    ld_color_pair<CT>(p + base + tid2, a0, a1);
+    ld_color_pair<CT>(p + base + kTile / 2 + tid2, b0, b1);
+  }
+};
+struct CyclicColors {
+  FastDiv P;                                          // P = maximum(colorvec); element indices are < 2^31
+  __device__ __forceinline__ uint32_t at(int64_t j) const { return P.mod((uint32_t)j); }
+  __device__ __forceinline__ uint32_t plus(uint32_t a, uint32_t b) const {   // (a + b) mod P for a < P, b <= P
+    const uint32_t s = a + b;
+    return s >= P.d ? s - P.d : s;
+  }
+  // one modulo per tile; the lane offsets mod P do not depend on the tile (hoisted out of the tile loops)
+  __device__ __forceinline__ void tile(int64_t base, int tid2, uint32_t &a0, uint32_t &a1, uint32_t &b0, uint32_t &b1) const {
+    const uint32_t b = P.mod((uint32_t)base);
+    a0 = plus(b, P.mod((uint32_t)tid2));
+    a1 = plus(a0, 1u);
+    b0 = plus(b, P.mod((uint32_t)(kTile / 2 + tid2)));
+    b1 = plus(b0, 1u);
+  }
+};
+
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -100,6 +100,7 @@ struct fdb_plan {
   int32_t C = 0;
   int color_bits = 8;
   bool has_invalid = false;
+  bool cyclic = false;        // colorvec[j] == j mod C + 1 for every j: kernels use the closed form, jcolor is not read
   // compressed index streams (device)
   void *jcolor = nullptr;     // [n] CT
   int32_t *row32 = nullptr;   // [E]
@@ -134,7 +135,7 @@ struct fdb_plan {
   // A/B switches (environment, read ONCE when the plan is created — never on the hot path; DESIGN.md §4)
   struct Tunables {
     bool no_staged = false, no_eps_lists = false, no_eps_overlap = false, cm_prefetch = false, force_overlap = false;
-    bool no_fx_cm = false, force_fx_cm = false, no_pack = false;
+    bool no_fx_cm = false, force_fx_cm = false, no_pack = false, no_band = false;
     int hi_stream = -1;                // -1: by pattern (random => evict-first slab gathers), 0 / 1: forced
     // walk direction: bit 0 the staged scatter
     // starts at the END of J's storage, bit 1 the perturbation pass at the end of x — each reads first what the kernel
@@ -163,6 +164,8 @@ struct fdb_plan {
   int32_t *tile_w0 = nullptr;
   int32_t stage_W = 0;
   bool staged = false, stage_packed = false;
+  bool stage_band = false;             // exact clipped band: the staged pass derives rows and columns, reads no index stream
+  int32_t band_l = 0, band_col_a = 0, band_col_b = 0, band_e_a = 0, band_e_b = 0, band_w = 1;
   std::vector<int64_t> bucket_start;   // [C+2] offsets into cols_by_color; bucket C = columns without a valid colour
   int lanes = 1;
   double mean_row_jump = 0.0;
@@ -255,6 +258,12 @@ template <typename F> static fdb_status dispatch_ct(int bits, F &&fn) {
   return fn((int32_t)0);
 }
 
+// the per-column colour source of a plan whose table has type CT: the cyclic closed form when it holds, else the table
+template <typename CT, typename F> static fdb_status dispatch_colors(const fdb_plan *P, F &&fn) {
+  if (P->cyclic) return fn(CyclicColors{make_fastdiv((uint32_t)P->C)});
+  return fn(TableColors<CT>{(const CT *)P->jcolor});
+}
+
 static const char *plan_err_text(uint32_t e) {
   if (e & kErrColptr) return "colptr is not a valid CSC column pointer (must start at 1, be non-decreasing, end at nnz+1)";
   if (e & kErrRowRange) return "row index outside 1..m";
@@ -290,27 +299,29 @@ static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or de
   P->color_bits = mx <= 255 ? 8 : (mx <= 65535 ? 16 : 32);
   TRY(P->alloc(&P->jcolor, (size_t)std::max<int64_t>(n, 1) * (P->color_bits / 8)));
   if (n > 0) {
-    uint32_t *d_flags = nullptr;
+    uint32_t *d_flags = nullptr;   // [0] lane conflicts (window path), [1] not cyclic
     const bool window_path = P->C > kEpsRegColors;
-    if (window_path) {
-      CU(cudaMalloc((void **)&d_flags, sizeof(uint32_t)));
-      CU(cudaMemset(d_flags, 0, sizeof(uint32_t)));
-    }
+    CU(cudaMalloc((void **)&d_flags, 2 * sizeof(uint32_t)));
+    CU(cudaMemset(d_flags, 0, 2 * sizeof(uint32_t)));
     fdb_status st = dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
       convert_colors<CT><<<P->grid(n), kThreads>>>(cv.d, n, (CT *)P->jcolor);
       if (window_path) color_lane_conflicts<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags);
+      if (P->C > 0) check_cyclic<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags + 1);
       CU(cudaGetLastError());
       return FDB_OK;
     });
-    if (st == FDB_OK && window_path) {
-      uint32_t flags = 0;
-      cudaError_t e = cudaMemcpy(&flags, d_flags, sizeof flags, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) st = fail(FDB_ERR_CUDA, "colour conflict flags: %s", cudaGetErrorString(e));
-      P->eps_group = 1;
-      for (int lg = 1; lg <= 5 && !(flags & (1u << lg)); ++lg) P->eps_group = 1 << lg;
+    if (st == FDB_OK) {
+      uint32_t flags[2] = {0, 0};
+      cudaError_t e = cudaMemcpy(flags, d_flags, sizeof flags, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) st = fail(FDB_ERR_CUDA, "colour flags: %s", cudaGetErrorString(e));
+      P->cyclic = P->C > 0 && flags[1] == 0;
+      if (window_path) {
+        P->eps_group = 1;
+        for (int lg = 1; lg <= 5 && !(flags[0] & (1u << lg)); ++lg) P->eps_group = 1 << lg;
+      }
     }
-    if (d_flags) cudaFree(d_flags);
+    cudaFree(d_flags);
     if (st != FDB_OK) return st;
   }
   return FDB_OK;
@@ -580,6 +591,41 @@ static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long lo
   return FDB_OK;
 }
 
+// Band form of the staged pass: the pattern is exactly the clipped band of some (l, u) — column c holds the rows
+// max(0, c-l) .. min(m-1, c+u), in order — so every entry's row and column follow from its position.
+static fdb_status try_band_form(fdb_plan *P) {
+  P->stage_band = false;
+  const int64_t m = P->m, n = P->n;
+  int *d_lu = nullptr;
+  uint32_t *d_flag = nullptr;
+  TRY(P->alloc_t(&d_lu, 2));
+  TRY(P->alloc_t(&d_flag, 1));
+  const int init[2] = {INT_MIN, INT_MIN};
+  CU(cudaMemcpy(d_lu, init, sizeof init, cudaMemcpyHostToDevice));
+  CU(cudaMemset(d_flag, 0, 4));
+  band_extent<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, n, d_lu);
+  int lu[2];
+  CU(cudaMemcpy(lu, d_lu, sizeof lu, cudaMemcpyDeviceToHost));
+  const int l = lu[0], u = lu[1];
+  band_check<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, m, n, l, u, d_flag);
+  uint32_t bad = 1;
+  CU(cudaMemcpy(&bad, d_flag, 4, cudaMemcpyDeviceToHost));
+  if (bad) return FDB_OK;
+  // interior columns [a, b): c - l >= 0 and c + u <= m - 1 — every one holds all w = l + u + 1 rows
+  const int64_t a = std::min<int64_t>(std::max(l, 0), n), b = std::max<int64_t>(a, std::min<int64_t>(n, m - u));
+  int32_t ea = 0, eb = 0;
+  CU(cudaMemcpy(&ea, P->colptr32 + a, 4, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(&eb, P->colptr32 + b, 4, cudaMemcpyDeviceToHost));
+  P->band_l = l;
+  P->band_w = l + u + 1;
+  P->band_col_a = (int32_t)a;
+  P->band_col_b = (int32_t)b;
+  P->band_e_a = ea;
+  P->band_e_b = eb;
+  P->stage_band = true;
+  return FDB_OK;
+}
+
 // TMA-staged fused pass: eligible when the whole Jacobian is one resident group on one rank, the destination is the
 // identity (CSC nzval) and every 1024-entry tile touches a short row window (row-local pattern).
 static fdb_status try_stage_plan(fdb_plan *P) {
@@ -615,6 +661,7 @@ static fdb_status try_stage_plan(fdb_plan *P) {
   if (span == 0 || span > 65535 || smem > (size_t)kStageMaxSmem) return FDB_OK;   // not row-local enough: keep the gather form
   P->stage_W = (int32_t)W;
   P->staged = true;
+  if (!P->tune.no_band) TRY(try_band_form(P));
   return FDB_OK;
 }
 
@@ -643,6 +690,7 @@ static void read_tunables(fdb_plan *P) {
   t.no_fx_cm = env_is("FDB_NO_FX_CM", '1');
   t.force_fx_cm = env_is("FDB_FORCE_FX_CM", '1');
   t.no_pack = env_is("FDB_NO_PACK", '1');
+  t.no_band = env_is("FDB_NO_BAND", '1');
   if (const char *hs = getenv("FDB_HI_STREAM")) t.hi_stream = hs[0] == '1' ? 1 : 0;
   if (const char *v = getenv("FDB_REVERSE")) { if (v[0] >= '0' && v[0] <= '3') t.reverse = v[0] - '0'; }
   if (env_is("FDB_CM_HINT", '0')) t.cm_slab_stream = 0;
@@ -1126,8 +1174,11 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
         const int64_t C = std::max<int32_t>(P->C, 1);
         const int64_t owned = P->world > 1 ? P->E * (int64_t)P->local_colors.size() / C : P->E;   // approx. share
         info->moved_bytes_scatter = P->E * (4 + ct) * std::max<int64_t>(P->n_groups, 1) + owned * (8 * slabs_read + 8 + (P->dest ? 8 : 0)) + fx_once;
-        if (P->staged)   // 16-bit row offsets; every slab row and f(x) row staged once
-          info->moved_bytes_scatter = P->E * (2 + (P->stage_packed ? 0 : ct) + 8) + 8 * P->m * (int64_t)(P->fdtype == FDB_CENTRAL ? 2 * P->C : P->C + 1);
+        const int64_t staged_rows = 8 * P->m * (int64_t)(P->fdtype == FDB_CENTRAL ? 2 * P->C : P->C + 1);
+        if (P->staged && P->stage_band)   // no index stream; the column colour table unless the colouring is cyclic
+          info->moved_bytes_scatter = 8 * P->E + staged_rows + (P->cyclic ? 0 : P->n * ct);
+        else if (P->staged)   // 16-bit row offsets; every slab row and f(x) row staged once
+          info->moved_bytes_scatter = P->E * (2 + (P->stage_packed ? 0 : ct) + 8) + staged_rows;
       }
     } else {
       info->moved_bytes_scatter = P->alg_bytes;
@@ -1292,12 +1343,16 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
   if (C <= kEpsRegColors) {
     const int64_t ntiles = (P->n + kTile - 1) / kTile;
     const int aligned = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-    auto go = [&](auto kern) {
-      const int grid = std::min(resident_grid(P, kern, 0, ntiles), P->eps_blocks);  // partial capacity
-      kern<<<grid, kThreads, 0, s>>>(x, (const CT *)P->jcolor, P->n, aligned, C, prm, P->partial, P->ticket, P->eps, P->sumsq);
-    };
-    if (C <= 4) { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CT, 4, 2>); else go(color_sumsq_reg<CT, 4, 1>); }
-    else { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CT, 8, 2>); else go(color_sumsq_reg<CT, 8, 1>); }
+    TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+      using CS = decltype(cs);
+      auto go = [&](auto kern) {
+        const int grid = std::min(resident_grid(P, kern, 0, ntiles), P->eps_blocks);  // partial capacity
+        kern<<<grid, kThreads, 0, s>>>(x, cs, P->n, aligned, C, prm, P->partial, P->ticket, P->eps, P->sumsq);
+      };
+      if (C <= 4) { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CS, 4, 2>); else go(color_sumsq_reg<CS, 4, 1>); }
+      else { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CS, 8, 2>); else go(color_sumsq_reg<CS, 8, 1>); }
+      return FDB_OK;
+    }));
     P->cnt.kernel_launches += 1;
   } else {
     for (int32_t k0 = 0; k0 < C; k0 += kEpsWindow) {
@@ -1365,7 +1420,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   auto perturb_window = [&](int64_t li0, int64_t kc) -> fdb_status {
       for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
         PerturbArgs pa{};
-        pa.x = x; pa.jcolor = P->jcolor; pa.eps = P->eps;
+        pa.x = x; pa.eps = P->eps;
         pa.xp = P->xp + q0 * sX; pa.xm = CENTRAL ? P->xm + q0 * sX : nullptr;
         pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = P->no_drift ? 0 : 1;
         pa.reverse = (P->tune.reverse >> 1) & 1;
@@ -1375,19 +1430,23 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
                        reinterpret_cast<uintptr_t>(P->xm)) & 15) == 0 && (P->ldx & 1) == 0;
         const size_t sm = P->C <= kPerturbSmemColors ? (size_t)P->C * sizeof(double) : 0;
         const int64_t tiles = (P->n + kTile - 1) / kTile;
-        if (COMPLEX) {
-          if (pa.kcount == 1) perturb_complex<CT, 1><<<P->grid(P->n), kThreads, 0, s>>>(pa);
-          else perturb_complex<CT, kPerturbMaxPoints><<<P->grid(P->n), kThreads, 0, s>>>(pa);
-        } else {
-          // store-heavy (NP points written per element read): an oversubscribed grid (16x the resident wave), like the
-          // band and dense-column kernels
-          constexpr int kPerturbGridOver = 16;
-          auto over = [&](int g) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)g * kPerturbGridOver, tiles)); };
-          if (pa.kcount == 1)
-            perturb_colors<CT, CENTRAL, 1><<<over(resident_grid(P, perturb_colors<CT, CENTRAL, 1>, sm, tiles)), kThreads, sm, s>>>(pa);
-          else
-            perturb_colors<CT, CENTRAL, kPerturbMaxPoints><<<over(resident_grid(P, perturb_colors<CT, CENTRAL, kPerturbMaxPoints>, sm, tiles)), kThreads, sm, s>>>(pa);
-        }
+        TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+          using CS = decltype(cs);
+          if (COMPLEX) {
+            if (pa.kcount == 1) perturb_complex<CS, 1><<<P->grid(P->n), kThreads, 0, s>>>(pa, cs);
+            else perturb_complex<CS, kPerturbMaxPoints><<<P->grid(P->n), kThreads, 0, s>>>(pa, cs);
+          } else {
+            // store-heavy (NP points written per element read): an oversubscribed grid (16x the resident wave), like the
+            // band and dense-column kernels
+            constexpr int kPerturbGridOver = 16;
+            auto over = [&](int g) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)g * kPerturbGridOver, tiles)); };
+            if (pa.kcount == 1)
+              perturb_colors<CS, CENTRAL, 1><<<over(resident_grid(P, perturb_colors<CS, CENTRAL, 1>, sm, tiles)), kThreads, sm, s>>>(pa, cs);
+            else
+              perturb_colors<CS, CENTRAL, kPerturbMaxPoints><<<over(resident_grid(P, perturb_colors<CS, CENTRAL, kPerturbMaxPoints>, sm, tiles)), kThreads, sm, s>>>(pa, cs);
+          }
+          return FDB_OK;
+        }));
         P->cnt.kernel_launches += 1;
       }
       return FDB_OK;
@@ -1520,26 +1579,41 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
         if (staged) {
           if constexpr (MODE != kComplex) {
             StagedArgs sa{};
-            sa.row16 = P->row16; sa.ecolor = P->ecolor; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
+            sa.row16 = P->row16; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
             sa.fx = vfx; sa.Fp = P->Fp; sa.Fm = P->Fm; sa.eps = P->eps; sa.J = J; sa.C = P->C; sa.W = P->stage_W;
             sa.ldF = sF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned;
             sa.reverse = P->tune.reverse & 1;
+            sa.colptr32 = P->colptr32; sa.l = P->band_l; sa.n = (int32_t)P->n;
+            sa.col_a = P->band_col_a; sa.col_b = P->band_col_b; sa.e_a = P->band_e_a; sa.e_b = P->band_e_b;
+            sa.w = make_fastdiv((uint32_t)P->band_w);
             const int nwin = CENTRAL ? 2 * P->C : P->C + 1;
             int stages = P->tune.stages;
             if ((size_t)stages * nwin * P->stage_W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8 > (size_t)kStageMaxSmem) stages = 2;
             sa.stages = stages;
             const size_t ssm = (size_t)stages * nwin * P->stage_W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8;
-            // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n): resident blocks per SM x index prefetch
+            // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n | 6e): resident blocks per SM x index prefetch / empty mbarrier
             const char v0 = P->tune.staged_variant[0], v1 = P->tune.staged_variant[1];
-            auto go = [&](auto kern) {
+            auto go = [&](auto kern, auto cs) {
               const int grid = resident_grid(P, kern, ssm, tiles);
-              kern<<<grid, kThreads, ssm, s>>>(sa);
+              kern<<<grid, kThreads, ssm, s>>>(sa, cs);
             };
-            if (P->stage_packed && v1 == 'e') go(diff_scatter_staged<CT, MODE, 6, false, true, true>);
-            else if (P->stage_packed) go(diff_scatter_staged<CT, MODE, 6, false, true>);
-            else if (v0 == '8') go(diff_scatter_staged<CT, MODE, 8, false, false>);
-            else if (v1 == 'n') go(diff_scatter_staged<CT, MODE, 6, false, false>);
-            else go(diff_scatter_staged<CT, MODE, 6, true, false>);
+            if (P->stage_band) {
+              TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+                using CS = decltype(cs);
+                if (v0 == '8') go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs);
+                else if (v1 == 'e') go(diff_scatter_staged<CS, MODE, 6, false, false, true, true>, cs);
+                else go(diff_scatter_staged<CS, MODE, 6, false, false, false, true>, cs);
+                return FDB_OK;
+              }));
+            } else {
+              using CS = TableColors<CT>;          // per-entry colours
+              const CS ec{(const CT *)P->ecolor};
+              if (P->stage_packed && v1 == 'e') go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec);
+              else if (P->stage_packed) go(diff_scatter_staged<CS, MODE, 6, false, true>, ec);
+              else if (v0 == '8') go(diff_scatter_staged<CS, MODE, 8, false, false>, ec);
+              else if (v1 == 'n') go(diff_scatter_staged<CS, MODE, 6, false, false>, ec);
+              else go(diff_scatter_staged<CS, MODE, 6, true, false>, ec);
+            }
           }
         } else if (full) {
           const int grid = resident_grid(P, diff_scatter_ident<CT, MODE, true, kScatterMinBlocks>, sm, tiles);

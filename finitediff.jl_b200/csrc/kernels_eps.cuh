@@ -32,7 +32,7 @@ __device__ __forceinline__ double eps_from_sumsq(double ss, const EpsParams &p) 
 }
 
 // C <= 8: per-thread register accumulators (NC = 4 or 8 of them) over the block's tiles (fixed tile -> block -> lane
-// mapping), shuffle tree, fixed warp order; the LAST block to finish (atomic ticket) reduces the block partials in
+// mapping; colours from a colour source, common.cuh), shuffle tree, fixed warp order; the LAST block to finish (atomic ticket) reduces the block partials in
 // fixed order and applies the step-size formula — one launch, no host involvement, bit-reproducible for a given grid.
 template <int NC>
 __device__ __forceinline__ void sumsq_accumulate(double (&acc)[NC], double v, uint32_t c) {
@@ -44,9 +44,9 @@ __device__ __forceinline__ void sumsq_accumulate(double (&acc)[NC], double v, ui
     if (c == (uint32_t)k) acc[k] += sq;
 }
 
-template <typename CT, int NC, int DEPTH = 1>
+template <typename CS, int NC, int DEPTH = 1>
 __global__ void __launch_bounds__(kThreads)
-color_sumsq_reg(const double *__restrict__ x, const CT *__restrict__ jcolor, int64_t n, int x_aligned, int32_t C,
+color_sumsq_reg(const double *__restrict__ x, const CS colors, int64_t n, int x_aligned, int32_t C,
                 EpsParams prm, double *__restrict__ partial /* [gridDim.x][kEpsRegColors] */,
                 unsigned int *__restrict__ ticket, double *__restrict__ eps, double *__restrict__ sumsq) {
   double acc[NC];
@@ -60,14 +60,11 @@ color_sumsq_reg(const double *__restrict__ x, const CT *__restrict__ jcolor, int
     // two tiles' loads in flight; accumulated in the same order as the one-tile loop (tile, then tile + gridDim.x)
     for (; tile + gridDim.x < nfull; tile += 2 * (int64_t)gridDim.x) {
       const double *__restrict__ xa = x + tile * kTile, *__restrict__ xb = xa + (int64_t)gridDim.x * kTile;
-      const CT *__restrict__ ca = jcolor + tile * kTile, *__restrict__ cb = ca + (int64_t)gridDim.x * kTile;
       const double2 a0 = ld_stream2(xa + tid2), a1 = ld_stream2(xa + kHalf + tid2);
       const double2 b0 = ld_stream2(xb + tid2), b1 = ld_stream2(xb + kHalf + tid2);
       uint32_t p0, p1, p2, p3, q0, q1, q2, q3;
-      ld_color_pair<CT>(ca + tid2, p0, p1);
-      ld_color_pair<CT>(ca + kHalf + tid2, p2, p3);
-      ld_color_pair<CT>(cb + tid2, q0, q1);
-      ld_color_pair<CT>(cb + kHalf + tid2, q2, q3);
+      colors.tile(tile * kTile, tid2, p0, p1, p2, p3);
+      colors.tile((tile + gridDim.x) * kTile, tid2, q0, q1, q2, q3);
       sumsq_accumulate<NC>(acc, a0.x, p0);
       sumsq_accumulate<NC>(acc, a0.y, p1);
       sumsq_accumulate<NC>(acc, a1.x, p2);
@@ -80,12 +77,10 @@ color_sumsq_reg(const double *__restrict__ x, const CT *__restrict__ jcolor, int
   }
   for (; tile < nfull; tile += gridDim.x) {
     const double *__restrict__ xt = x + tile * kTile;
-    const CT *__restrict__ ct = jcolor + tile * kTile;
     const double2 va = ld_stream2(xt + tid2);
     const double2 vb = ld_stream2(xt + kHalf + tid2);
     uint32_t ca0, ca1, cb0, cb1;
-    ld_color_pair<CT>(ct + tid2, ca0, ca1);
-    ld_color_pair<CT>(ct + kHalf + tid2, cb0, cb1);
+    colors.tile(tile * kTile, tid2, ca0, ca1, cb0, cb1);
     sumsq_accumulate<NC>(acc, va.x, ca0);
     sumsq_accumulate<NC>(acc, va.y, ca1);
     sumsq_accumulate<NC>(acc, vb.x, cb0);
@@ -100,8 +95,8 @@ color_sumsq_reg(const double *__restrict__ x, const CT *__restrict__ jcolor, int
 #pragma unroll
       for (int u = 0; u < kPairsPerThread; ++u) {
         const int64_t j = base + u * kHalf + tid2;
-        if (j < n) sumsq_accumulate<NC>(acc, ld_stream(x + j), (uint32_t)jcolor[j]);
-        if (j + 1 < n) sumsq_accumulate<NC>(acc, ld_stream(x + j + 1), (uint32_t)jcolor[j + 1]);
+        if (j < n) sumsq_accumulate<NC>(acc, ld_stream(x + j), colors.at(j));
+        if (j + 1 < n) sumsq_accumulate<NC>(acc, ld_stream(x + j + 1), colors.at(j + 1));
       }
     }
   }

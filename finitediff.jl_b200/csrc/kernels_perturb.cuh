@@ -12,7 +12,8 @@
 // pristine x and the eps table.  The caller's x is never written.
 //
 // Memory shape: one streaming pass, x read once (16-byte loads), every output written once (16-byte stores); the
-// colour ids come as one narrow load per pair; the eps table sits in shared memory.
+// colour ids come as one narrow load per pair, or from the closed form of a cyclic colouring (no colour stream); the eps
+// table sits in shared memory.
 #pragma once
 #include "common.cuh"
 
@@ -23,7 +24,6 @@ constexpr int kPerturbMaxPoints = 4;       // colours (points) built per launch;
 
 struct PerturbArgs {
   const double *x;
-  const void *jcolor;
   const double *eps;
   double *xp, *xm;
   int64_t n, ldx;
@@ -48,16 +48,15 @@ __device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, do
 
 // NP = compile-time bound on the points built per launch (1: the usual one-colour-per-callback case; kPerturbMaxPoints:
 // batched callbacks).  Full tiles take the unchecked 16-byte path; the last partial tile (or unaligned buffers) the scalar one.
-template <typename CT, bool CENTRAL, int NP>
+template <typename CS, bool CENTRAL, int NP>
 __global__ void __launch_bounds__(kThreads)
-perturb_colors(const PerturbArgs a) {
+perturb_colors(const PerturbArgs a, const CS colors) {
   extern __shared__ double s_eps[];
   const bool use_smem = a.C <= kPerturbSmemColors;
   if (use_smem) {
     for (int i = threadIdx.x; i < a.C; i += kThreads) s_eps[i] = a.eps[i];
     __syncthreads();
   }
-  const CT *__restrict__ jcolor = reinterpret_cast<const CT *>(a.jcolor);
   constexpr int kHalf = kTile / 2;
   const int tid2 = 2 * threadIdx.x;
   const int64_t nfull = a.aligned ? a.n / kTile : 0;
@@ -69,8 +68,7 @@ perturb_colors(const PerturbArgs a) {
     const double2 va = ld_stream2(a.x + base + tid2);
     const double2 vb = ld_stream2(a.x + base + kHalf + tid2);
     uint32_t ca0, ca1, cb0, cb1;
-    ld_color_pair<CT>(jcolor + base + tid2, ca0, ca1);
-    ld_color_pair<CT>(jcolor + base + kHalf + tid2, cb0, cb1);
+    colors.tile(base, tid2, ca0, ca1, cb0, cb1);
     const double ea0 = eps_of(ca0), ea1 = eps_of(ca1), eb0 = eps_of(cb0), eb1 = eps_of(cb1);
     const bool ya0 = ca0 < (uint32_t)a.C, ya1 = ca1 < (uint32_t)a.C, yb0 = cb0 < (uint32_t)a.C, yb1 = cb1 < (uint32_t)a.C;
 #pragma unroll
@@ -94,7 +92,7 @@ perturb_colors(const PerturbArgs a) {
   for (int64_t tt = blockIdx.x; tt < ntail; tt += gridDim.x) {
     for (int64_t j = rem0 + tt * kTile + threadIdx.x; j < a.n && j < rem0 + (tt + 1) * kTile; j += kThreads) {
       const double v = ld_stream(a.x + j);
-      const uint32_t c = (uint32_t)jcolor[j];
+      const uint32_t c = colors.at(j);
       const bool y = c < (uint32_t)a.C;
       const double e = eps_of(c);
 #pragma unroll
@@ -113,14 +111,13 @@ perturb_colors(const PerturbArgs a) {
 // The point is complex128 (re, im interleaved): re = x, im = eps on the colour's columns, 0 elsewhere.  No drift: the
 // imaginary part returns to exactly 0 ((0+eps)-eps) and the real part is never touched.  xp is addressed in DOUBLES:
 // point b starts at xp + b*ldx with ldx = 2 * (complex elements per point).
-template <typename CT, int NP>
+template <typename CS, int NP>
 __global__ void __launch_bounds__(kThreads)
-perturb_complex(const PerturbArgs a) {
-  const CT *__restrict__ jcolor = reinterpret_cast<const CT *>(a.jcolor);
+perturb_complex(const PerturbArgs a, const CS colors) {
   const int64_t stride = (int64_t)gridDim.x * kThreads;
   for (int64_t j = blockIdx.x * (int64_t)kThreads + threadIdx.x; j < a.n; j += stride) {
     const double v = ld_stream(a.x + j);
-    const uint32_t c = (uint32_t)jcolor[j];
+    const uint32_t c = colors.at(j);
     const double e = c < (uint32_t)a.C ? __ldg(a.eps + c) : 0.0;
 #pragma unroll
     for (int b = 0; b < NP; ++b) {

@@ -52,6 +52,53 @@ convert_colors(const int64_t *__restrict__ colorvec /* null => 1:n */, int64_t n
   }
 }
 
+// cyclic colouring test: flag = 1 unless jcolor[j] == j mod C for every j (a column without a valid colour never matches)
+template <typename CT>
+__global__ void __launch_bounds__(kThreads)
+check_cyclic(const CT *__restrict__ jcolor, int64_t n, int32_t C, uint32_t *__restrict__ flag) {
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  for (int64_t j = blockIdx.x * (int64_t)kThreads + threadIdx.x; j < n; j += stride)
+    if ((uint32_t)jcolor[j] != (uint32_t)(j % C)) { *flag = 1u; return; }
+}
+
+// exact-band test, pass 1: l = max(c - r), u = max(r - c) over all entries (0-based rows, CSC column pointer)
+__global__ void __launch_bounds__(kThreads)
+band_extent(const int32_t *__restrict__ colptr32, const int32_t *__restrict__ row32, int64_t n, int *__restrict__ lu) {
+  int l = INT_MIN, u = INT_MIN;
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  for (int64_t c = blockIdx.x * (int64_t)kThreads + threadIdx.x; c < n; c += stride) {
+    const int32_t p0 = colptr32[c], p1 = colptr32[c + 1];
+    if (p1 > p0) {                                       // rows may be unsorted here: look at every one
+      for (int32_t p = p0; p < p1; ++p) {
+        const int r = row32[p];
+        l = max(l, (int)c - r);
+        u = max(u, r - (int)c);
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    l = max(l, __shfl_xor_sync(0xffffffffu, l, o));
+    u = max(u, __shfl_xor_sync(0xffffffffu, u, o));
+  }
+  if ((threadIdx.x & 31) == 0) { atomicMax(lu, l); atomicMax(lu + 1, u); }
+}
+
+// pass 2: every column c holds exactly the rows max(0, c-l) .. min(m-1, c+u), in order; flag = 1 on the first mismatch
+__global__ void __launch_bounds__(kThreads)
+band_check(const int32_t *__restrict__ colptr32, const int32_t *__restrict__ row32, int64_t m, int64_t n, int l, int u,
+           uint32_t *__restrict__ flag) {
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  for (int64_t c = blockIdx.x * (int64_t)kThreads + threadIdx.x; c < n; c += stride) {
+    const int64_t lo = c - l > 0 ? c - l : 0, hi = c + u < m - 1 ? c + u : m - 1;
+    const int64_t len = hi >= lo ? hi - lo + 1 : 0;
+    const int32_t p0 = colptr32[c];
+    bool bad = colptr32[c + 1] - p0 != len;
+    for (int64_t i = 0; !bad && i < len; ++i) bad = row32[p0 + i] != lo + i;
+    if (bad) { *flag = 1u; return; }
+  }
+}
+
 __global__ void __launch_bounds__(kThreads)
 validate_colptr(const int64_t *__restrict__ colptr, int64_t n, int64_t nnz, uint32_t *__restrict__ err) {
   const int64_t stride = (int64_t)gridDim.x * kThreads;

@@ -11,6 +11,8 @@
 // The gather form is a latency-limited dependent gather; here the only global loads a warp waits for are its own
 // coalesced index pairs.  cp.async.bulk and mbarrier transaction counts are Hopper (sm_90) instructions.
 // Compulsory bytes per Jacobian: E*(2 + |colour| + 8) + 8*m*(slabs + 1)  (C2 forward: 650 MB; gather form: 710 MB).
+// For an exact clipped band (C2's tridiagonal) the band form reads no per-entry stream at all: E*8 + 8*m*(slabs + 1)
+// (+ n colour bytes unless the colouring is cyclic; C2 forward: 560 MB).
 #pragma once
 #include "common.cuh"
 #include "kernels_scatter.cuh"
@@ -53,10 +55,9 @@ constexpr int kStagesMax = 3;          // tiles in flight per block (2 by defaul
 constexpr int kStageMaxSmem = 46 * 1024;
 
 struct StagedArgs {
-  const uint16_t *row16;     // [E] row - tile_w0[tile]
-  const void *ecolor;        // [E] (CT)
+  const uint16_t *row16;     // [E] row - tile_w0[tile]                        (indexed form)
   const int32_t *tile_w0;    // [E / kTile] even first row of every full tile's window
-  const int32_t *row32;      // [E] (the partial last tile takes the gather path)
+  const int32_t *row32;      // [E] (the partial last tile of the indexed form)
   const double *fx, *Fp, *Fm, *eps;
   double *J;
   int32_t C, W;              // colours (slab == colour), window length in rows (even)
@@ -66,7 +67,31 @@ struct StagedArgs {
   int32_t j_aligned;
   int32_t reverse;           // walk the full tiles from the end of J's storage towards its start: the rows the last f! wrote
                              // most recently (the tail of the last slab) are read while they are still in L2
+  // band form: the pattern is exactly the clipped band, column c holding rows max(0, c-l) .. min(m-1, c+u) in order
+  const int32_t *colptr32;   // [n+1] (only the clipped head / tail columns are searched)
+  int32_t l, n;
+  int32_t col_a, col_b;      // interior columns [col_a, col_b): all w = l+u+1 rows present
+  int32_t e_a, e_b;          // their entries [e_a, e_b) = colptr32[col_a], colptr32[col_b]
+  FastDiv w;
 };
+
+// band form: column and row of entry e.  Interior entries in closed form; the few clipped head / tail columns by a
+// binary search of colptr32 over their own range (head: l columns; tail: the columns after the interior)
+__device__ __forceinline__ void band_locate(const StagedArgs &a, uint32_t e, uint32_t &c, uint32_t &r) {
+  if (e >= (uint32_t)a.e_a && e < (uint32_t)a.e_b) {
+    const uint32_t q = a.w.div(e - a.e_a);
+    c = a.col_a + q;
+    r = c - a.l + (e - a.e_a - q * a.w.d);
+    return;
+  }
+  int32_t lo = e < (uint32_t)a.e_a ? 0 : a.col_b, hi = e < (uint32_t)a.e_a ? a.col_a : a.n;   // colptr32[lo] <= e
+  while (hi - lo > 1) {
+    const int32_t mid = (lo + hi) >> 1;
+    if ((uint32_t)__ldg(a.colptr32 + mid) <= e) lo = mid; else hi = mid;
+  }
+  c = (uint32_t)lo;
+  r = (uint32_t)max(0, lo - a.l) + (e - (uint32_t)__ldg(a.colptr32 + lo));
+}
 
 // plan time: window start (even) of every full tile, 16-bit offsets, largest span
 template <typename CT>
@@ -118,16 +143,21 @@ stage_prepare(const int32_t *__restrict__ row32, int64_t ntiles, int32_t *__rest
   }
 }
 
+// CS: colour source (common.cuh).  Indexed form: TableColors over the per-entry colours (unless PACKED); band form: the
+// colour of the entry's column (the per-column table or the cyclic closed form)
 // MINB: resident blocks per SM the register budget is cut for (8 -> 32 registers, 6 -> 40: no spill of the prefetched
 // index registers; with TMA doing the wide loads the kernel needs fewer resident warps than the gather form)
 // PACKED: few colours and short windows (C <= 14, W <= 4096): the entry's colour rides in the top 4 bits of its 16-bit row
 // offset — the per-entry colour stream is not read at all (2 index bytes per entry instead of 2 + |colour|)
 // EMPTYBAR: a stage is handed back to the producer through a second mbarrier (one arrival per warp) instead of a block-wide
 // __syncthreads(): warps that finished a tile go straight on to the next one (A/B variant, see DESIGN.md §4)
-template <typename CT, int MODE, int MINB, bool PREFETCH, bool PACKED, bool EMPTYBAR = false>
+// BAND: the pattern is an exact clipped band — every entry's row and column follow from its position (band_locate), no
+// per-entry index stream is read: the kernel streams the staged windows in and J out
+template <typename CS, int MODE, int MINB, bool PREFETCH, bool PACKED, bool EMPTYBAR = false, bool BAND = false>
 __global__ void __launch_bounds__(kThreads, MINB)
-diff_scatter_staged(const StagedArgs a) {
+diff_scatter_staged(const StagedArgs a, const CS colors) {
   static_assert(MODE == kForward || MODE == kCentral, "staged scatter: forward / central");
+  static_assert(!(BAND && (PACKED || PREFETCH)), "band form: no index stream to pack or prefetch");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int C = a.C, W = a.W;
   const int nwin = MODE == kCentral ? 2 * C : C + 1;
@@ -137,7 +167,6 @@ diff_scatter_staged(const StagedArgs a) {
   uint64_t *full = reinterpret_cast<uint64_t *>(buf + kStages * stage_elems);
   uint64_t *empty = full + kStagesMax;
   double *s_eps = reinterpret_cast<double *>(full + 2 * kStagesMax);        // [C]
-  const CT *__restrict__ ecolor = reinterpret_cast<const CT *>(a.ecolor);
   const int64_t nfull = a.E / kTile;
   constexpr int kHalf = kTile / 2;
   const int tid2 = 2 * threadIdx.x;
@@ -182,21 +211,45 @@ diff_scatter_staged(const StagedArgs a) {
     return d / (MODE == kCentral ? 2 * e : e);
   };
 
-  // index pairs of a tile: coalesced, independent of the staged data — loaded ONE TILE AHEAD (software pipelining), so
-  // their latency overlaps the previous tile's wait + arithmetic instead of following the block barrier
+  // window offsets and colours of the lane's two entry pairs.  Indexed form: coalesced index pairs, independent of the
+  // staged data (with PREFETCH loaded ONE TILE AHEAD, so their latency overlaps the previous tile's wait + arithmetic).
+  // Band form: derived from the tile's position; an interior tile (all its columns complete) takes one division per pair.
   struct Idx { ushort2 ra, rb; uint32_t ka0, ka1, kb0, kb1; };
   auto load_idx = [&](int64_t tile) {
     Idx x;
-    const uint16_t *__restrict__ rt = a.row16 + tile * kTile;
-    const CT *__restrict__ ct = ecolor + tile * kTile;
-    x.ra = __ldcs(reinterpret_cast<const ushort2 *>(rt + tid2));
-    x.rb = __ldcs(reinterpret_cast<const ushort2 *>(rt + kHalf + tid2));
-    if (PACKED) {
-      x.ka0 = x.ra.x >> 12; x.ka1 = x.ra.y >> 12; x.kb0 = x.rb.x >> 12; x.kb1 = x.rb.y >> 12;
-      x.ra.x &= 0xFFF; x.ra.y &= 0xFFF; x.rb.x &= 0xFFF; x.rb.y &= 0xFFF;
+    if constexpr (BAND) {
+      const uint32_t e0 = (uint32_t)(tile * kTile), w0 = (uint32_t)__ldg(a.tile_w0 + tile);
+      const bool interior = e0 >= (uint32_t)a.e_a && e0 + kTile <= (uint32_t)a.e_b;
+      auto pair = [&](uint32_t e, ushort2 &rr, uint32_t &k0, uint32_t &k1) {
+        uint32_t c, r, c1, r1;
+        if (interior) {
+          const uint32_t v = e - a.e_a, q = a.w.div(v), o = v - q * a.w.d;
+          c = a.col_a + q;
+          r = c - a.l + o;
+          const bool wrap = o + 1 == a.w.d;                  // the pair's second entry starts the next column
+          c1 = wrap ? c + 1 : c;
+          r1 = wrap ? c1 - a.l : r + 1;
+        } else {
+          band_locate(a, e, c, r);
+          band_locate(a, e + 1, c1, r1);
+        }
+        rr.x = (unsigned short)(r - w0);
+        rr.y = (unsigned short)(r1 - w0);
+        k0 = colors.at(c);
+        k1 = c1 == c ? k0 : colors.at(c1);
+      };
+      pair(e0 + tid2, x.ra, x.ka0, x.ka1);
+      pair(e0 + kHalf + tid2, x.rb, x.kb0, x.kb1);
     } else {
-      ld_color_pair<CT>(ct + tid2, x.ka0, x.ka1);
-      ld_color_pair<CT>(ct + kHalf + tid2, x.kb0, x.kb1);
+      const uint16_t *__restrict__ rt = a.row16 + tile * kTile;
+      x.ra = __ldcs(reinterpret_cast<const ushort2 *>(rt + tid2));
+      x.rb = __ldcs(reinterpret_cast<const ushort2 *>(rt + kHalf + tid2));
+      if (PACKED) {
+        x.ka0 = x.ra.x >> 12; x.ka1 = x.ra.y >> 12; x.kb0 = x.rb.x >> 12; x.kb1 = x.rb.y >> 12;
+        x.ra.x &= 0xFFF; x.ra.y &= 0xFFF; x.rb.x &= 0xFFF; x.rb.y &= 0xFFF;
+      } else {
+        colors.tile(tile * kTile, tid2, x.ka0, x.ka1, x.kb0, x.kb1);
+      }
     }
     return x;
   };
@@ -245,10 +298,18 @@ diff_scatter_staged(const StagedArgs a) {
   const int64_t rem0 = nfull * kTile;
   if (rem0 < a.E && blockIdx.x == (unsigned)(nfull % gridDim.x)) {
     for (int64_t e = rem0 + threadIdx.x; e < a.E; e += kThreads) {
-      const uint32_t k = (uint32_t)ecolor[e];
+      uint32_t k, r;
+      if constexpr (BAND) {
+        uint32_t c;
+        band_locate(a, (uint32_t)e, c, r);
+        k = colors.at(c);
+      } else {
+        k = colors.at(e);
+        r = (uint32_t)a.row32[e];
+      }
       double v = 0.0;
       if (k < (uint32_t)C)
-        v = fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, a.row32[e], s_eps[k]);
+        v = fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, r, s_eps[k]);
       a.J[e] = v;
     }
   }
