@@ -735,6 +735,12 @@ static fdb_status new_plan(fdb_plan **out, const fdb_plan_opts *o, int64_t m, in
   cudaError_t e = cudaGetDeviceProperties(&prop, dev);
   if (e != cudaSuccess) { delete P; return fail(FDB_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); }
   P->sm_count = prop.multiProcessorCount;
+  // FDB_SM_COUNT=k (tests): size every grid as if the device had k SMs, so small problems already give each block several
+  // tiles.  Launch geometry only: no plan decision reads sm_count.
+  if (const char *v = getenv("FDB_SM_COUNT")) {
+    const int k = atoi(v);
+    if (k >= 1 && k < P->sm_count) P->sm_count = k;
+  }
   P->l2_bytes = prop.l2CacheSize;
   *out = P;
   return FDB_OK;

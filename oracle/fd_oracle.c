@@ -302,10 +302,12 @@ int fdo_finite_difference_jacobian(const fdo_problem *P, double *J, fdo_fn f, vo
         for (int64_t i = 0; i < m; ++i) fx1[i] = (fx1[i] - fx[i]) / two_eps; /* :607 */
         colorediteration(P, J, fx1, colorvec, color_i, nt);                 /* :608-614 */
         if (o->no_drift) {
-          /* exact restore (not what the reference does; used to compare with drift-free runs) */
+          /* exact restore (not what the reference does; used to compare with drift-free runs).  x2 still holds this
+           * colour's components as they were before :603-604, and with exact restores those are the caller's values:
+           * (x - eps) + eps and (x1 + eps) - eps would replay the drift whenever the rounding does not cancel. */
           PAR_FOR
           for (int64_t j = 0; j < n; ++j)
-            if (color_of(colorvec, j) == color_i) { x[j] = x[j] + eps; x1[j] = x1[j] - eps; }
+            if (color_of(colorvec, j) == color_i) { x[j] = x2[j]; x1[j] = x2[j]; }
         } else {
           PAR_FOR
           for (int64_t j = 0; j < n; ++j) {

@@ -1,7 +1,42 @@
 """Shared helpers for the parity tests: pattern builders in the reference's (Julia) conventions —
 Int64, 1-based CSC exactly as SparseMatrixCSC stores it."""
+import contextlib
+import os
+
 import numpy as np
 import scipy.sparse as sp
+
+
+@contextlib.contextmanager
+def fdb_env(**switches):
+    """Set FDB_* switches (DESIGN.md §4) while plans are created, restoring the previous environment afterwards.
+    fdb_env(NO_BAND=1, SM_COUNT=3) sets FDB_NO_BAND=1 and FDB_SM_COUNT=3; a value of None leaves the variable unset.
+    Plans read the switches once, when they are created (for the Python mirror: on the first call that needs the plan)."""
+    names = {f"FDB_{k}": v for k, v in switches.items()}
+    saved = {k: os.environ.get(k) for k in names}
+    try:
+        for k, v in names.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = str(v)
+        yield
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def band_csc(m, n, l, u):
+    """colptr/rowval (1-based Int64) of the clipped band: column c holds rows max(0, c-l) .. min(m-1, c+u)."""
+    c = np.arange(n)
+    lo, hi = np.maximum(c - l, 0), np.minimum(c + u, m - 1)
+    cnt = np.maximum(hi - lo + 1, 0)
+    colptr = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+    rowval = np.arange(colptr[-1], dtype=np.int64) - np.repeat(colptr[:-1], cnt) + np.repeat(lo, cnt)
+    return colptr + 1, rowval + 1
 
 
 def tridiag_csc(n):

@@ -7,10 +7,11 @@ instead of reading them.  Every case is compared bit for bit with the oracle (fe
 same plan built under FDB_NO_BAND=1 (indexed form); the path a plan took is read from moved_bytes_scatter:
 band form 8*E + 8*m*(windows) (+ n colour bytes unless the colouring is cyclic)."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
+
+from _util import band_csc, fdb_env
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -38,7 +39,8 @@ def cyclic(n, P):
     return (np.arange(n) % P + 1).astype(np.int64)
 
 
-def run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=False, f_in=False, dirv=1.0, no_drift=False):
+def run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=False, f_in=False, dirv=1.0, no_drift=False,
+        sm_count=None):
     L = pkg._lib
     dev = torch.device("cuda:0")
     rng = np.random.default_rng(seed)
@@ -61,18 +63,11 @@ def run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=False, f_in
                                    x.cpu().numpy().ctypes.data_as(C.POINTER(C.c_double)))
         fin_t = torch.from_numpy(fin).to(dev)
         kw["f_in"] = fin
-    old = os.environ.pop("FDB_NO_BAND", None)
-    if no_band:
-        os.environ["FDB_NO_BAND"] = "1"
-    try:
+    with fdb_env(NO_BAND=1 if no_band else None, SM_COUNT=sm_count):
         fx = torch.zeros(m, dtype=torch.float64, device=dev)
         cache = pkg.JacobianCache(x.clone(), fx, fx.clone(), fdtype, colorvec=cv, sparsity=sp, no_drift=no_drift)
         pkg.finite_difference_jacobian_(sp, f, x, cache, fin_t, dir=dirv)
         torch.cuda.synchronize()
-    finally:
-        os.environ.pop("FDB_NO_BAND", None)
-        if old is not None:
-            os.environ["FDB_NO_BAND"] = old
     plan = cache._last_plan
     eps = plan.eps()
     got = sp.nzval.cpu().numpy()
@@ -82,6 +77,10 @@ def run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=False, f_in
                         no_drift=no_drift, dir=dirv, ctx=octx, **kw)
     assert ctx.calls == r["fcalls"]
     assert np.array_equal(got, ref, equal_nan=True)
+    own = oracle.jacobian(oracle.Problem.csc_same(m, n, colptr, rowval), np.zeros(E), oracle.native_fn("synth_ellrows"),
+                          x.cpu().numpy().copy(), fdtype=0 if fdtype == "forward" else 1, colorvec=cv, no_drift=no_drift,
+                          dir=dirv, ctx=octx, **kw)
+    np.testing.assert_allclose(eps, own["eps"], rtol=1e-13)
     return got, eps, plan.info()
 
 
@@ -91,7 +90,7 @@ def band_bytes(info, m, n, E, C_, fdtype, is_cyclic):
 
 
 def check(pkg, oracle, m, n, cols, cv, fdtype, expect_band, is_cyclic=None, seed=1, **kw):
-    colptr, rowval = to_csc(cols)
+    colptr, rowval = cols if isinstance(cols, tuple) else to_csc(cols)
     E = len(rowval)
     C_ = int(cv.max())
     if is_cyclic is None:
@@ -176,3 +175,27 @@ def test_f_in_dir_no_drift(pkg, oracle):
     check(pkg, oracle, m, n, cols, cyclic(n, 3), "forward", expect_band=True, dirv=-1.0)
     for fdtype in FDTYPES:
         check(pkg, oracle, m, n, cols, cyclic(n, 3), fdtype, expect_band=True, no_drift=True)
+
+
+@pytest.mark.parametrize("sm_count", [1, 3])
+@pytest.mark.parametrize("fdtype,m,n,l,u,colouring", [
+    ("forward", 40000, 40000, 2, 1, "cyclic"),     # l != u
+    ("central", 40000, 40000, 2, 1, "cyclic"),
+    ("forward", 20000, 60000, 1, 4, "cyclic"),     # m < n: empty columns after row m
+    ("central", 60000, 30000, 3, 0, "cyclic"),     # m > n
+    ("forward", 50000, 50000, 1, 1, "shifted"),    # non-cyclic colouring: the column colour table is read
+    ("central", 50000, 50000, 1, 1, "colour_0"),
+])
+def test_exact_band_multiwave(pkg, oracle, sm_count, fdtype, m, n, l, u, colouring):
+    # FDB_SM_COUNT=k sizes the grids as if the device had k SMs: the staged scatter walks several tiles per block
+    # (pipeline refill, mbarrier parity flip, reverse walk, the block that takes the partial last tile)
+    colptr, rowval = band_csc(m, n, l, u)
+    P = min(l + u + 1, 3 if fdtype == "central" else 6)
+    cv, is_cyclic = cyclic(n, P), True
+    if colouring == "shifted":
+        cv, is_cyclic = ((np.arange(n) + 1) % P + 1).astype(np.int64), False
+    elif colouring == "colour_0":
+        cv[np.arange(17, n, 997)] = 0
+        is_cyclic = False
+    assert len(rowval) >= 3 * 8 * 3 * 1024      # >= 3 tiles per block at k = 3 with 8 resident blocks per SM
+    check(pkg, oracle, m, n, (colptr, rowval), cv, fdtype, expect_band=True, is_cyclic=is_cyclic, sm_count=sm_count)

@@ -13,7 +13,10 @@ import pytest
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-from _util import (csc_from_dense_pattern, cyc_colors, tridiag_csc)  # noqa: E402
+from _util import (csc_from_dense_pattern, cyc_colors, fdb_env, tridiag_csc)  # noqa: E402
+
+# FDB_SM_COUNT=k: grids sized as if the device had k SMs, so the tile loops take several steps per block at test sizes
+SM_COUNTS = [None, 1, 3]
 
 FD = {"forward": 0, "central": 1}
 
@@ -132,8 +135,18 @@ def test_per_colour_list_strategy_tridiag(pkg, oracle, dev, fdtype):
 @pytest.mark.parametrize("fdtype", ["forward", "central"])
 def test_unaligned_buffers_take_scalar_paths(pkg, oracle, dev, fdtype):
     # x and nzval only 8-byte aligned (views at an odd offset): the 16-byte vector paths must fall back, same bits
+    _unaligned_case(pkg, oracle, dev, fdtype, 5003)
+
+
+@pytest.mark.parametrize("fdtype", ["forward", "central"])
+@pytest.mark.parametrize("N,sm_count", [(5003, 1), (5003, 3), (300_001, 1), (300_001, 3)])
+def test_unaligned_buffers_multiwave(pkg, oracle, dev, fdtype, N, sm_count):
+    # the same scalar paths with several tiles per block
+    _unaligned_case(pkg, oracle, dev, fdtype, N, sm_count)
+
+
+def _unaligned_case(pkg, oracle, dev, fdtype, N, sm_count=None):
     from _util import f_tridiag
-    N = 5003
     colptr, rowval = tridiag_csc(N)
     cv = cyc_colors(N, 3)
     xbuf = torch.zeros(N + 1, dtype=torch.float64, device=dev)
@@ -143,7 +156,8 @@ def test_unaligned_buffers_take_scalar_paths(pkg, oracle, dev, fdtype):
     nzbuf = torch.full((len(rowval) + 1,), float("nan"), dtype=torch.float64, device=dev)
     J = pkg.SparseMatrixCSC(N, N, t64(colptr), t64(rowval), nzbuf[1:])
     cache = pkg.JacobianCache(x, fdtype, colorvec=cv, sparsity=J)
-    pkg.finite_difference_jacobian_(J, f_tridiag_t, x, cache)
+    with fdb_env(SM_COUNT=sm_count):
+        pkg.finite_difference_jacobian_(J, f_tridiag_t, x, cache)
     ref = np.full(len(rowval), np.nan)
     oracle.jacobian(oracle.Problem.csc_same(N, N, colptr, rowval), ref, f_tridiag, oracle.fill_x(N, 41), fdtype=FD[fdtype],
                     colorvec=cv, eps_override=cache._last_plan.eps())
@@ -464,11 +478,25 @@ def test_lap5_csc_and_banded_bitexact(pkg, oracle, dev, fdtype, g):
         assert np.array_equal(Jd.cpu().numpy().reshape(-1, order="F"), refd)
 
 
+NARROW_BANDS = [(30, 30, 1, 1), (50, 40, 3, 0), (40, 50, 0, 2), (17, 17, 16, 16), (300, 200, 70, 10), (200, 300, 5, 90),
+                (130, 130, 129, 129)]
+
+
 def test_narrow_band_and_rectangular_band(pkg, oracle, dev):
     # narrow-band tiling branch (w=3), non-square m != n, unequal l/u
     # (the last three take the warp-per-column wide-band kernel, l+u+1 >= 64)
-    for (m, n, l, u) in [(30, 30, 1, 1), (50, 40, 3, 0), (40, 50, 0, 2), (17, 17, 16, 16), (300, 200, 70, 10),
-                         (200, 300, 5, 90), (130, 130, 129, 129)]:
+    _narrow_bands(pkg, oracle, dev, NARROW_BANDS)
+
+
+@pytest.mark.parametrize("sm_count", SM_COUNTS)
+def test_narrow_band_multiwave(pkg, oracle, dev, sm_count):
+    # the same shapes with several tiles per block, plus two long bands (w = 3, 5) that give every block of the tiled
+    # kernel several tiles at sm_count = 1
+    _narrow_bands(pkg, oracle, dev, NARROW_BANDS + [(60000, 70000, 1, 1), (50000, 40000, 3, 1)], sm_count)
+
+
+def _narrow_bands(pkg, oracle, dev, shapes, sm_count=None):
+    for (m, n, l, u) in shapes:
         cv = cyc_colors(n, l + u + 1)
         x = dev_x(pkg, dev, n, 77)
         xh = oracle.fill_x(n, 77)
@@ -489,17 +517,31 @@ def test_narrow_band_and_rectangular_band(pkg, oracle, dev):
         Jb.data.fill_(float("nan"))
         cache = pkg.JacobianCache(x, torch.zeros(m, dtype=torch.float64, device=dev),
                                   torch.zeros(m, dtype=torch.float64, device=dev), "forward", colorvec=cv, sparsity=Jb)
-        pkg.finite_difference_jacobian_(Jb, f_t, x, cache)
+        with fdb_env(SM_COUNT=sm_count):
+            pkg.finite_difference_jacobian_(Jb, f_t, x, cache)
         ref = np.full((l + u + 1) * n, np.nan)
         oracle.jacobian(oracle.Problem.banded(m, n, l, u), ref, f_n, xh.copy(), colorvec=cv,
                         eps_override=cache._last_plan.eps())
         assert np.array_equal(Jb.data.cpu().numpy(), ref)
 
 
-@pytest.mark.parametrize("m,n,l,u", [(3000, 3000, 64, 64), (2500, 3100, 70, 58), (3100, 2500, 40, 88), (900, 900, 33, 31)])
+WIDE_BANDS = [(3000, 3000, 64, 64), (2500, 3100, 70, 58), (3100, 2500, 40, 88), (900, 900, 33, 31)]
+
+
+@pytest.mark.parametrize("m,n,l,u", WIDE_BANDS)
 def test_wide_band_few_colors_with_colourless_columns(pkg, oracle, dev, m, n, l, u):
     # few colours on a wide band: quotients pre-divided in place + whole-band copy; columns without a valid colour stay 0
     # (fill_matrix!), corner slots outside the matrix 0; square / wide / tall, even and odd l+u+1
+    _wide_band_case(pkg, oracle, dev, m, n, l, u)
+
+
+@pytest.mark.parametrize("sm_count", [1, 3])
+@pytest.mark.parametrize("m,n,l,u", WIDE_BANDS)
+def test_wide_band_multiwave(pkg, oracle, dev, m, n, l, u, sm_count):
+    _wide_band_case(pkg, oracle, dev, m, n, l, u, sm_count)
+
+
+def _wide_band_case(pkg, oracle, dev, m, n, l, u, sm_count=None):
     rng = np.random.default_rng(5)
     cv = cyc_colors(n, 5)
     cv[rng.integers(0, n, 25)] = 0
@@ -523,7 +565,8 @@ def test_wide_band_few_colors_with_colourless_columns(pkg, oracle, dev, m, n, l,
         Jb.data.fill_(float("nan"))
         cache = pkg.JacobianCache(x, torch.zeros(m, dtype=torch.float64, device=dev),
                                   torch.zeros(m, dtype=torch.float64, device=dev), fdtype, colorvec=cv, sparsity=Jb)
-        pkg.finite_difference_jacobian_(Jb, f_t, x, cache)
+        with fdb_env(SM_COUNT=sm_count):
+            pkg.finite_difference_jacobian_(Jb, f_t, x, cache)
         ref = np.full((l + u + 1) * n, np.nan)
         oracle.jacobian(oracle.Problem.banded(m, n, l, u), ref, f_n, xh.copy(), fdtype=FD[fdtype], colorvec=cv,
                         eps_override=cache._last_plan.eps())
@@ -676,6 +719,18 @@ def test_different_pattern_csc_J(pkg, oracle, dev):
 def test_dense_columns_bitexact(pkg, oracle, dev, fdtype, batch, n):
     """sparsity === nothing: dense column branch (jacobians.jl:548-557, :590-598), BASELINE config C5 shape at reduced n
     (even n: 16-byte row pairs; odd n: columns are only 8-byte aligned -> scalar rows)."""
+    _dense_columns_case(pkg, oracle, dev, fdtype, batch, n)
+
+
+@pytest.mark.parametrize("fdtype", ["forward", "central"])
+@pytest.mark.parametrize("batch", [1, 7])
+@pytest.mark.parametrize("n,sm_count", [(300, 1), (301, 3), (2049, 1), (2050, 3)])
+def test_dense_columns_multiwave(pkg, oracle, dev, fdtype, batch, n, sm_count):
+    # the same branch with several grid-stride steps per block (n = 2049: 1024 row pairs per column)
+    _dense_columns_case(pkg, oracle, dev, fdtype, batch, n, sm_count)
+
+
+def _dense_columns_case(pkg, oracle, dev, fdtype, batch, n, sm_count=None):
     w = np.random.default_rng(2).random(n)
     d_w = torch.from_numpy(w).to(dev)
     nblk = (n + 1023) // 1024
@@ -686,7 +741,8 @@ def test_dense_columns_bitexact(pkg, oracle, dev, fdtype, batch, n):
     J = pkg.zeros_colmajor(n, n, dev)
     J.fill_(float("nan"))
     cache = pkg.JacobianCache(x, fdtype, max_batch=batch)
-    pkg.finite_difference_jacobian_(J, native(pkg, "fdbs_rank1", ctx, batch), x, cache)
+    with fdb_env(SM_COUNT=sm_count):
+        pkg.finite_difference_jacobian_(J, native(pkg, "fdbs_rank1", ctx, batch), x, cache)
     eps = cache._last_plan.eps()
     ref = np.zeros(n * n)
     r = oracle.jacobian(oracle.Problem.dense(n, n), ref, oracle.native_fn("synth_rank1"), xh.copy(), fdtype=FD[fdtype],

@@ -9,6 +9,8 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
+from _util import fdb_env
+
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
@@ -21,10 +23,10 @@ def pkg():
     return _bootstrap.load_package()
 
 
-def _case(rng, pkg, oracle, dev):
+def _case(rng, pkg, oracle, dev, sm_count=None, lo=1, hi=400):
     L = pkg._lib
-    m = int(rng.integers(1, 400))
-    n = int(rng.integers(1, 400))
+    m = int(rng.integers(lo, hi))
+    n = int(rng.integers(lo, hi))
     K = int(rng.integers(1, 6))
     cols = rng.integers(0, n, size=(m, K)).astype(np.int32)          # random dependence, duplicates allowed
     coef = rng.uniform(-1, 1, size=(m, K))
@@ -46,7 +48,7 @@ def _case(rng, pkg, oracle, dev):
         # a scratch budget of a few slabs: several scatter groups per Jacobian (colour-major lists: one launch per group,
         # f(x) pre-gathered into list order; storage-order pass: ownership tests per group)
         opts["scratch_bytes"] = int(8 * (m + 2) * (2 if fdtype == "central" else 1) * int(rng.integers(1, 4)) + 64)
-    dense_J = rng.random() < 0.3
+    dense_J = rng.random() < 0.3 and m * n <= 4_000_000
     x = torch.from_numpy(rng.uniform(-2, 2, n)).to(dev)
     colsT, coefT = np.ascontiguousarray(cols.T), np.ascontiguousarray(coef.T)
     d_cols, d_coef = torch.from_numpy(colsT).to(dev), torch.from_numpy(coefT).to(dev)
@@ -76,13 +78,14 @@ def _case(rng, pkg, oracle, dev):
         J = sp
         P = oracle.Problem.csc_same(m, n, colptr, rowval)
         ref = np.full(A.nnz, np.nan)
-    pkg.finite_difference_jacobian_(J, f, x, cache, fin_t, dir=dirv)
-    torch.cuda.synchronize()
+    with fdb_env(SM_COUNT=sm_count):       # grids sized as if the device had sm_count SMs: several tiles per block
+        pkg.finite_difference_jacobian_(J, f, x, cache, fin_t, dir=dirv)
+        torch.cuda.synchronize()
     eps = cache._last_plan.eps()
     r = oracle.jacobian(P, ref, oracle.native_fn("synth_ellrows"), x.cpu().numpy().copy(), fdtype=0 if fdtype == "forward" else 1,
                         colorvec=cv, eps_override=eps, no_drift=opts["no_drift"], dir=dirv, ctx=octx, **kw)
     got = (J.cpu().numpy().reshape(-1, order="F") if dense_J else sp.nzval.cpu().numpy())
-    desc = f"m={m} n={n} K={K} C={cv.max()} {fdtype} {opts} dense={dense_J} f_in={use_fin} dir={dirv}"
+    desc = f"m={m} n={n} K={K} C={cv.max()} {fdtype} {opts} dense={dense_J} f_in={use_fin} dir={dirv} sm_count={sm_count}"
     assert ctx.calls == r["fcalls"], desc
     assert np.array_equal(got, ref, equal_nan=True), desc
     own = oracle.jacobian(P, np.zeros_like(ref), oracle.native_fn("synth_ellrows"), x.cpu().numpy().copy(),
@@ -95,3 +98,22 @@ def test_random_patterns_bitexact(pkg, oracle):
     rng = np.random.default_rng(20260924)
     for _ in range(120):
         _case(rng, pkg, oracle, dev)
+
+
+@pytest.mark.parametrize("sm_count", [1, 3])
+def test_random_patterns_bitexact_multiwave(pkg, oracle, sm_count):
+    # the same generator with the grids sized as if the device had sm_count SMs
+    dev = torch.device("cuda:0")
+    rng = np.random.default_rng(20260924)
+    for _ in range(60):
+        _case(rng, pkg, oracle, dev, sm_count)
+
+
+@pytest.mark.parametrize("sm_count", [1, 3])
+def test_random_patterns_mid_size_multiwave(pkg, oracle, sm_count):
+    # m, n of 10^4 .. 10^5 under FDB_SM_COUNT: every scatter form, the perturbation and step-size passes several tiles
+    # per block
+    dev = torch.device("cuda:0")
+    rng = np.random.default_rng(20261015 + sm_count)
+    for _ in range(8):
+        _case(rng, pkg, oracle, dev, sm_count, lo=10_000, hi=100_000)

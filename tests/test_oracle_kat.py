@@ -372,3 +372,23 @@ def test_nonvector_input_identity(oracle, golden):
             r = oracle.jacobian(oracle.Problem.dense(4, 4), J, ident, x.copy(), fdtype=1)
             assert r["fcalls"] == 8
         assert np.max(np.abs(J.reshape(4, 4, order="F") - np.eye(4))) < g["bound"]
+
+
+@pytest.mark.parametrize("fdtype", [0, 1])
+def test_no_drift_restores_exactly(oracle, fdtype):
+    # no_drift (a test option, not the reference): every perturbed component is restored to its exact value, so each
+    # colour's f! sees the pristine x outside its own colour.  The faithful run keeps the reference's (x1 + eps) - eps
+    # drift, which with |x| up to 2 and a central step of about 1e-4 changes some components (the test has teeth).
+    n = 200_000
+    colptr, rowval = tridiag_csc(n)
+    cv = (np.arange(n) % 3 + 1).astype(np.int64)
+    x0 = np.random.default_rng(3).uniform(-2, 2, n)
+    P = oracle.Problem.csc_same(n, n, colptr, rowval)
+    for no_drift in (True, False):
+        x = x0.copy()
+        r = oracle.jacobian(P, np.zeros(len(rowval)), f_tridiag, x, fdtype=fdtype, colorvec=cv, no_drift=no_drift)
+        x1 = r["cache"]["x1"]
+        if no_drift:
+            assert np.array_equal(x1, x0) and np.array_equal(x, x0)
+        elif fdtype == 1:
+            assert not np.array_equal(x1, x0)
