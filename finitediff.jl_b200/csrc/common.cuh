@@ -97,6 +97,14 @@ struct CyclicColors {
   }
 };
 
+// Julia Base max(a, b) on Float64: NaN when either argument is NaN (it returns a - b then), otherwise the larger one,
+// with +0.0 counted larger than -0.0.  The step-size formula max(relstep*|x|, absstep) uses it, so a NaN in x gives a
+// NaN step (a plain `a > b ? a : b` would return absstep).
+__host__ __device__ __forceinline__ double max_julia(double a, double b) {
+  if (isnan(a) || isnan(b)) return a - b;
+  return signbit(a - b) ? b : a;
+}
+
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

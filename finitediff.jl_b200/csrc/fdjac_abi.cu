@@ -796,7 +796,7 @@ double fdb_default_relstep(int fdtype) {
 // src/epsilons.jl:26-29 / :50-53
 double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep, double dir) {
   const double a = relstep * fabs(x);
-  const double e = a > absstep ? a : absstep;
+  const double e = max_julia(a, absstep);
   return fdtype == FDB_FORWARD ? e * dir : e;
 }
 
@@ -1707,7 +1707,7 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
     const int32_t kc = (int32_t)std::min<int64_t>(B, ncl - c0l);
     const int64_t c0 = P->col_begin + c0l;
     const int sb = (std::max(kc, prevB) + kThreads - 1) / kThreads;
-    if (COMPLEX) set_components_complex<<<sb, kThreads, 0, s>>>(P->eps_cols, c0l, c0, prev_c0, kc, prevB, sX, P->xp);
+    if (COMPLEX) set_components_complex<<<sb, kThreads, 0, s>>>(x, P->eps_cols, c0l, c0, prev_c0, kc, prevB, sX, P->xp);
     else set_components<<<sb, kThreads, 0, s>>>(x, P->eps_cols, c0l, c0, prev_c0, kc, prevB, P->ldx, 1.0, P->xp);
     TRY(call_f(P, f, ctx, P->Fp, P->xp, kc, s));                         // f(fx1, x1)   jacobians.jl:553 / :594 / :629
     if (CENTRAL) {

@@ -26,7 +26,7 @@ struct EpsParams {
 __device__ __forceinline__ double eps_from_sumsq(double ss, const EpsParams &p) {
   const double tmp = sqrt(ss);                        // norm(x2)                     jacobians.jl:560
   const double a = p.relstep * fabs(sqrt(tmp));       // relstep*abs(sqrt(tmp))       :561 + epsilons.jl:28
-  double e = a > p.absstep ? a : p.absstep;           // max(.., absstep)
+  double e = max_julia(a, p.absstep);                 // max(.., absstep)
   if (!p.fdtype_central) e = e * p.dir;               // *dir (forward only)          epsilons.jl:28 vs :52
   return e;
 }
@@ -301,7 +301,7 @@ component_eps(const double *__restrict__ x, int64_t c0, int64_t ncols, int fdtyp
   const int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x;
   if (i >= ncols) return;
   const double a = relstep * fabs(x[c0 + i]);
-  double e = a > absstep ? a : absstep;
+  double e = max_julia(a, absstep);
   if (!fdtype_central) e = e * dir;
   eps[i] = e;
 }

@@ -62,7 +62,7 @@ jvp_dot_eps(const double *__restrict__ x, const double *__restrict__ v, int64_t 
     if (lane == 0) {
       const double tmp = sqrt(fabs(d));                       // sqrt(abs(dot(x, v)))          jvp.jl:252
       const double a = prm.relstep * fabs(tmp);                // compute_epsilon               epsilons.jl:26-29 / :50-53
-      double e = a > prm.absstep ? a : prm.absstep;
+      double e = max_julia(a, prm.absstep);
       if (!prm.fdtype_central) e = e * prm.dir;
       eps[0] = e;
       if (dot_out) dot_out[0] = d;

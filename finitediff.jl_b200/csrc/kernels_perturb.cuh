@@ -11,10 +11,23 @@
 // which needs no sequential dependence between colours — any GPU can build the point of any colour from the
 // pristine x and the eps table.  The caller's x is never written.
 //
+// Signed zeros.  `eps .* (color .== k)` is Julia's Bool product, a strong zero: it adds z_k = copysign(0, eps_k) to every
+// component outside colour k (and the central minus point subtracts it).  That is the identity on every value except a
+// zero, so the table above holds with one amendment for zeros: a whole earlier colour, add then subtract, turns either
+// zero into +0.0, and only a component still holding the caller's value at call k sees the signed add itself.
+//        c(j) == k : y + eps_k                with y = x[j] at the first colour, x[j] + 0.0 after it
+//        c(j) <  k : (x[j]+eps_c)-eps_c       (drift; a zero comes out +0.0 whatever the signs)
+//        otherwise : x[j] + (pristine ? z_k : +0.0)      minus point: x[j] + (pristine ? -z_k : +0.0)
+// "pristine" is k == 0 for components no colour has perturbed yet.  Without drift a perturbed colour is restored to a
+// saved value: forward writes back the caller's x[j] (pristine again at k == c+1), central writes back the value x1 held
+// before colour c, which is the caller's value only for c == 0 (pristine at k == 1).
+//
 // Memory shape: one streaming pass, x read once (16-byte loads), every output written once (16-byte stores); the
 // colour ids come as one narrow load per pair, or from the closed form of a cyclic colouring (no colour stream); the eps
 // table sits in shared memory.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace fdb {
@@ -34,10 +47,28 @@ struct PerturbArgs {
                                   // before left in L2; the heads of the points are what the first f! reads first)
 };
 
+// zk = copysign(0, eps_k), the value the reference adds to the components outside colour k (see the table above)
 template <bool CENTRAL>
-__device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, double e, int drift, uint32_t k,
+__device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, double e, int drift, uint32_t k, double zk,
                                             double &p, double &q) {
-  // plus point
+  const bool mine = valid && c == k, done = valid && c < k;
+  if (done && drift) {
+    p = (v + e) - e;
+    if (CENTRAL) q = (v - e) + e;
+  } else {
+    // the component still holds the caller's value at call k, or (a zero only) +0.0 left by an earlier whole colour
+    const bool pristine = done ? (k == c + 1 && (!CENTRAL || c == 0)) : k == 0;
+    const double y = (v == 0.0 && !pristine) ? 0.0 : v;
+    const double w = mine ? e : zk;
+    p = y + w;
+    if (CENTRAL) q = y - w;
+  }
+}
+
+// The same points for a component that is not a zero: every signed-zero add above is then the identity
+template <bool CENTRAL>
+__device__ __forceinline__ void perturb_nonzero(double v, uint32_t c, bool valid, double e, int drift, uint32_t k,
+                                                double &p, double &q) {
   p = v;
   q = v;
   if (valid) {
@@ -48,6 +79,8 @@ __device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, do
 
 // NP = compile-time bound on the points built per launch (1: the usual one-colour-per-callback case; kPerturbMaxPoints:
 // batched callbacks).  Full tiles take the unchecked 16-byte path; the last partial tile (or unaligned buffers) the scalar one.
+// A one-point full tile in which no lane of the warp holds a zero (a warp vote) takes perturb_nonzero, the instructions the
+// kernel had before the signed-zero rule; the other tiles take the rule.
 template <typename CS, bool CENTRAL, int NP>
 __global__ void __launch_bounds__(kThreads)
 perturb_colors(const PerturbArgs a, const CS colors) {
@@ -71,20 +104,33 @@ perturb_colors(const PerturbArgs a, const CS colors) {
     colors.tile(base, tid2, ca0, ca1, cb0, cb1);
     const double ea0 = eps_of(ca0), ea1 = eps_of(ca1), eb0 = eps_of(cb0), eb1 = eps_of(cb1);
     const bool ya0 = ca0 < (uint32_t)a.C, ya1 = ca1 < (uint32_t)a.C, yb0 = cb0 < (uint32_t)a.C, yb1 = cb1 < (uint32_t)a.C;
+    auto points = [&](auto zero_rule) {
+      constexpr bool Z = decltype(zero_rule)::value;
 #pragma unroll
-    for (int b = 0; b < NP; ++b) {
-      if (NP > 1 && b >= a.kcount) break;
-      const uint32_t k = (uint32_t)a.k[b];
-      double p0, q0, p1, q1;
-      perturb_one<CENTRAL>(va.x, ca0, ya0, ea0, a.drift, k, p0, q0);
-      perturb_one<CENTRAL>(va.y, ca1, ya1, ea1, a.drift, k, p1, q1);
-      st_stream2(a.xp + (int64_t)b * a.ldx + base + tid2, p0, p1);
-      if (CENTRAL) st_stream2(a.xm + (int64_t)b * a.ldx + base + tid2, q0, q1);
-      perturb_one<CENTRAL>(vb.x, cb0, yb0, eb0, a.drift, k, p0, q0);
-      perturb_one<CENTRAL>(vb.y, cb1, yb1, eb1, a.drift, k, p1, q1);
-      st_stream2(a.xp + (int64_t)b * a.ldx + base + kHalf + tid2, p0, p1);
-      if (CENTRAL) st_stream2(a.xm + (int64_t)b * a.ldx + base + kHalf + tid2, q0, q1);
-    }
+      for (int b = 0; b < NP; ++b) {
+        if (NP > 1 && b >= a.kcount) break;
+        const uint32_t k = (uint32_t)a.k[b];
+        const double zk = Z ? copysign(0.0, eps_of(k)) : 0.0;
+        auto one = [&](double v, uint32_t c, bool y, double e, double &p, double &q) {
+          if (Z) perturb_one<CENTRAL>(v, c, y, e, a.drift, k, zk, p, q);
+          else perturb_nonzero<CENTRAL>(v, c, y, e, a.drift, k, p, q);
+        };
+        double p0, q0, p1, q1;
+        one(va.x, ca0, ya0, ea0, p0, q0);
+        one(va.y, ca1, ya1, ea1, p1, q1);
+        st_stream2(a.xp + (int64_t)b * a.ldx + base + tid2, p0, p1);
+        if (CENTRAL) st_stream2(a.xm + (int64_t)b * a.ldx + base + tid2, q0, q1);
+        one(vb.x, cb0, yb0, eb0, p0, q0);
+        one(vb.y, cb1, yb1, eb1, p1, q1);
+        st_stream2(a.xp + (int64_t)b * a.ldx + base + kHalf + tid2, p0, p1);
+        if (CENTRAL) st_stream2(a.xm + (int64_t)b * a.ldx + base + kHalf + tid2, q0, q1);
+      }
+    };
+    // every lane of the block runs the full-tile loop, so the vote is over the whole warp.  Batched launches (NP > 1) always
+    // take the signed-zero rule: a second copy of their larger body would cost them registers.
+    if constexpr (NP > 1) points(std::true_type{});
+    else if (__any_sync(0xffffffffu, va.x == 0.0 || va.y == 0.0 || vb.x == 0.0 || vb.y == 0.0)) points(std::true_type{});
+    else points(std::false_type{});
   }
   // remainder (or everything when a buffer is not 16-byte aligned): scalar, bounds-checked
   const int64_t rem0 = nfull * kTile;
@@ -98,8 +144,9 @@ perturb_colors(const PerturbArgs a, const CS colors) {
 #pragma unroll
       for (int b = 0; b < NP; ++b) {
         if (NP > 1 && b >= a.kcount) break;
+        const uint32_t k = (uint32_t)a.k[b];
         double p, q;
-        perturb_one<CENTRAL>(v, c, y, e, a.drift, (uint32_t)a.k[b], p, q);
+        perturb_one<CENTRAL>(v, c, y, e, a.drift, k, copysign(0.0, eps_of(k)), p, q);
         a.xp[(int64_t)b * a.ldx + j] = p;
         if (CENTRAL) a.xm[(int64_t)b * a.ldx + j] = q;
       }
@@ -108,9 +155,11 @@ perturb_colors(const PerturbArgs a, const CS colors) {
 }
 
 // ---- complex step (jacobians.jl:634,644):  x1 = x + im*eps*(color==k)  ...  x1 = x1 - im*eps*(color==k) ----
-// The point is complex128 (re, im interleaved): re = x, im = eps on the colour's columns, 0 elsewhere.  No drift: the
-// imaginary part returns to exactly 0 ((0+eps)-eps) and the real part is never touched.  xp is addressed in DOUBLES:
-// point b starts at xp + b*ldx with ldx = 2 * (complex elements per point).
+// The point is complex128 (re, im interleaved): re = x + 0.0, im = eps on the colour's columns, 0 elsewhere.  im*eps
+// times a Bool is (+0.0, eps) or the strong zero (+0.0, +0.0), so the reference adds +0.0 to the real part of every
+// component (a -0.0 reads +0.0 from the first colour on) and the restore subtracts +0.0 again (the identity).  No drift:
+// the imaginary part returns to exactly 0 ((0+eps)-eps).  xp is addressed in DOUBLES: point b starts at xp + b*ldx with
+// ldx = 2 * (complex elements per point).
 template <typename CS, int NP>
 __global__ void __launch_bounds__(kThreads)
 perturb_complex(const PerturbArgs a, const CS colors) {
@@ -122,7 +171,7 @@ perturb_complex(const PerturbArgs a, const CS colors) {
 #pragma unroll
     for (int b = 0; b < NP; ++b) {
       if (NP > 1 && b >= a.kcount) break;
-      st_stream2(a.xp + (int64_t)b * a.ldx + 2 * j, v, c == (uint32_t)a.k[b] ? e : 0.0);
+      st_stream2(a.xp + (int64_t)b * a.ldx + 2 * j, v + 0.0, c == (uint32_t)a.k[b] ? e : 0.0);
     }
   }
 }
@@ -137,12 +186,20 @@ replicate_x_complex(const double *__restrict__ x, int64_t n, int64_t ldx /* doub
   }
 }
 
+// x1_save + im*eps with im*eps = (eps*false, eps*true) = (+0.0, eps): the perturbed component's real part is x + 0.0
+// (+0.0 for a -0.0); the restore writes the saved value back, so the other components keep the caller's bits
 __global__ void __launch_bounds__(kThreads)
-set_components_complex(const double *__restrict__ eps_local, int64_t col0_local, int64_t c0, int64_t prev_c0, int32_t B,
-                       int32_t prevB, int64_t ldx /* doubles */, double *__restrict__ X) {
+set_components_complex(const double *__restrict__ x, const double *__restrict__ eps_local, int64_t col0_local, int64_t c0,
+                       int64_t prev_c0, int32_t B, int32_t prevB, int64_t ldx /* doubles */, double *__restrict__ X) {
   const int b = blockIdx.x * kThreads + threadIdx.x;
-  if (b < prevB) X[(int64_t)b * ldx + 2 * (prev_c0 + b) + 1] = 0.0;                      // x1[i] = x1_save   :631
-  if (b < B) X[(int64_t)b * ldx + 2 * (c0 + b) + 1] = eps_local[col0_local + b];          // x1_save + im*eps :628
+  if (b < prevB) {                                                                        // x1[i] = x1_save   :631
+    const int64_t pc = prev_c0 + b;
+    st_stream2(X + (int64_t)b * ldx + 2 * pc, x[pc], 0.0);
+  }
+  if (b < B) {                                                                            // x1_save + im*eps :628
+    const int64_t c = c0 + b;
+    st_stream2(X + (int64_t)b * ldx + 2 * c, x[c] + 0.0, eps_local[col0_local + b]);
+  }
 }
 
 __global__ void __launch_bounds__(kThreads)

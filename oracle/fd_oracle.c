@@ -20,11 +20,18 @@ double fdo_default_relstep(int fdtype) {
   return 1.0;
 }
 
+/* Julia Base max(x::Float64, y::Float64): NaN if either argument is NaN (it returns x - y then), otherwise the larger
+ * one, with +0.0 counted larger than -0.0.  A NaN in x (a diverging Newton or ODE step) therefore gives a NaN step. */
+static inline double max_julia(double a, double b) {
+  if (isnan(a) || isnan(b)) return a - b;
+  return signbit(a - b) ? b : a;
+}
+
 /* src/epsilons.jl:26-29 (forward: max(relstep*abs(x),absstep)*dir)
  * src/epsilons.jl:50-53 (central: max(relstep*abs(x),absstep), dir ignored) */
 double fdo_compute_epsilon(int fdtype, double x, double relstep, double absstep, double dir) {
   double a = relstep * fabs(x);
-  double e = (a > absstep) ? a : absstep; /* Julia max(); NaN not expected here */
+  double e = max_julia(a, absstep);
   if (fdtype == FDO_FORWARD) return e * dir;
   return e;
 }
@@ -256,8 +263,10 @@ int fdo_finite_difference_jacobian(const fdo_problem *P, double *J, fdo_fn f, vo
         for (int64_t i = 0; i < m; ++i) fx1[i] = (fx1[i] - vfx[i]) / eps;                                 /* :565 in place */
         colorediteration(P, J, fx1, colorvec, color_i, nt);                                               /* :566-572 */
         if (o->no_drift) {
+          /* exact restore of the colour's components; the others get :584 as written (x1 - copysign(0, eps), which
+           * only changes the sign of a zero) */
           PAR_FOR
-          for (int64_t j = 0; j < n; ++j) if (color_of(colorvec, j) == color_i) x1[j] = x[j];
+          for (int64_t j = 0; j < n; ++j) x1[j] = color_of(colorvec, j) == color_i ? x[j] : x1[j] - mul_bool(eps, 0);
         } else {
           PAR_FOR
           for (int64_t j = 0; j < n; ++j) x1[j] = x1[j] - mul_bool(eps, color_of(colorvec, j) == color_i); /* :584 */
@@ -306,8 +315,10 @@ int fdo_finite_difference_jacobian(const fdo_problem *P, double *J, fdo_fn f, vo
            * colour's components as they were before :603-604, and with exact restores those are the caller's values:
            * (x - eps) + eps and (x1 + eps) - eps would replay the drift whenever the rounding does not cancel. */
           PAR_FOR
-          for (int64_t j = 0; j < n; ++j)
+          for (int64_t j = 0; j < n; ++j) {
             if (color_of(colorvec, j) == color_i) { x[j] = x2[j]; x1[j] = x2[j]; }
+            else { x1[j] = x1[j] - mul_bool(eps, 0); x[j] = x[j] + mul_bool(eps, 0); }   /* :619-620 as written */
+          }
         } else {
           PAR_FOR
           for (int64_t j = 0; j < n; ++j) {
@@ -384,17 +395,24 @@ int fdo_finite_difference_jacobian_complex(const fdo_problem *P, double *J, fdo_
       for (int64_t i = 0; i < m; ++i) Jc[i] = cimag(fx[i]) / epsilon;   /* :630 */
       x1[color_i - 1] = x1_save;
     } else {
-      /* :632-645 */
+      /* :632-645.  im*epsilon is Complex(epsilon*false, epsilon*true) = (+0.0, eps), and times (color == k) it is
+       * (+0.0, eps) or, by the strong-zero rule of mul_bool applied to each part, (+0.0, +0.0).  So :634 adds +0.0 to
+       * the real part of EVERY component (a -0.0 becomes +0.0 from the first colour on) and :644 subtracts +0.0 (the
+       * identity).  The adds are written out per part: C's complex `+` on these operands is the same two IEEE adds. */
       PAR_FOR
-      for (int64_t j = 0; j < n; ++j)
-        if (color_of(colorvec, j) == color_i) x1[j] = x1[j] + epsilon * _Complex_I;          /* :634 */
+      for (int64_t j = 0; j < n; ++j) {
+        const int b = color_of(colorvec, j) == color_i;
+        x1[j] = CMPLX(creal(x1[j]) + 0.0, cimag(x1[j]) + mul_bool(epsilon, b));              /* :634 */
+      }
       f(ctx, fx, x1); calls++;                                                               /* :635 */
       PAR_FOR
       for (int64_t i = 0; i < m; ++i) { vre[i] = cimag(fx[i]) / epsilon; fx[i] = vre[i]; }     /* :636 vfx = imag(vfx)/eps */
       colorediteration(P, J, vre, colorvec, color_i, nt);                                    /* :637-643 */
       PAR_FOR
-      for (int64_t j = 0; j < n; ++j)
-        if (color_of(colorvec, j) == color_i) x1[j] = x1[j] - epsilon * _Complex_I;          /* :644 */
+      for (int64_t j = 0; j < n; ++j) {
+        const int b = color_of(colorvec, j) == color_i;
+        x1[j] = CMPLX(creal(x1[j]) - 0.0, cimag(x1[j]) - mul_bool(epsilon, b));              /* :644 */
+      }
     }
   }
   if (fcalls) *fcalls = calls;

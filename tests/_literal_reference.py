@@ -45,6 +45,13 @@ def _setindex(J, v, row, col):
         J[row - 1, col - 1] = v
 
 
+def _bool_mul(v, mask):
+    """Julia's Float64 * Bool, elementwise: v * true = v, v * false = copysign(0.0, v) (a "strong zero", never NaN:
+    NaN * false and Inf * false are zeros too, unlike numpy's v * False)."""
+    v = np.broadcast_to(np.asarray(v, dtype=np.float64), np.shape(mask))
+    return np.where(mask, v, np.copysign(0.0, v))
+
+
 def compute_epsilon(fdtype, x, relstep, absstep, dir):
     if fdtype == "forward":
         return max(relstep * abs(x), absstep) * dir            # epsilons.jl:26-29
@@ -59,7 +66,10 @@ def norm(x2):
     if n == 0:
         return 0.0
     if n < 32:
-        maxabs = max(abs(float(v)) for v in x2)
+        maxabs = abs(float(x2[0]))                             # normInf: max propagates NaN (Python's max does not)
+        for v in x2[1:]:
+            a = abs(float(v))
+            maxabs = maxabs if (math.isnan(maxabs) or maxabs > a) else a
         if maxabs == 0.0 or math.isinf(maxabs):
             return maxabs
         if math.isfinite(n * maxabs * maxabs) and maxabs * maxabs != 0.0:
@@ -173,14 +183,14 @@ def finite_difference_jacobian(J, f, x, cache, f_in=None, *, fdtype="forward", r
                 x1[color_i - 1] = x1_save
             else:
                 mask = (_color == color_i)
-                x2[:] = x1 * mask                              # :559
+                x2[:] = _bool_mul(x1, mask)                    # :559
                 tmp = norm(x2)                                 # norm(x2) :560
                 epsilon = compute_epsilon("forward", math.sqrt(tmp), relstep, absstep, dir)   # :561
-                x1[:] = x1 + epsilon * mask                    # :562
+                x1[:] = x1 + _bool_mul(epsilon, mask)          # :562
                 f(fx1, x1); calls += 1                         # :563
                 vfx1[:] = (vfx1 - vfx) / epsilon               # :565
                 _colorediteration(J, sparsity, rows_index, cols_index, vfx1, _color, color_i, n, common)
-                x1[:] = x1 - epsilon * mask                    # :584
+                x1[:] = x1 - _bool_mul(epsilon, mask)          # :584
             eps_list.append(epsilon)
     elif fdtype == "central":
         vfx1 = fx1
@@ -196,17 +206,17 @@ def finite_difference_jacobian(J, f, x, cache, f_in=None, *, fdtype="forward", r
                 x1[color_i - 1] = x_save
             else:
                 mask = (_color == color_i)
-                x2[:] = x1 * mask                              # :600
+                x2[:] = _bool_mul(x1, mask)                    # :600
                 tmp = norm(x2)                                 # :601
                 epsilon = compute_epsilon("central", math.sqrt(tmp), relstep, absstep, dir)
-                x1[:] = x1 + epsilon * mask                    # :603
-                x[:] = x - epsilon * mask                      # :604
+                x1[:] = x1 + _bool_mul(epsilon, mask)          # :603
+                x[:] = x - _bool_mul(epsilon, mask)            # :604
                 f(fx1, x1); calls += 1
                 f(fx, x); calls += 1
                 vfx1[:] = (vfx1 - vfx) / (2 * epsilon)         # :607
                 _colorediteration(J, sparsity, rows_index, cols_index, vfx1, _color, color_i, n, common)
-                x1[:] = x1 - epsilon * mask                    # :619
-                x[:] = x + epsilon * mask                      # :620
+                x1[:] = x1 - _bool_mul(epsilon, mask)          # :619
+                x[:] = x + _bool_mul(epsilon, mask)            # :620
             eps_list.append(epsilon)
     else:
         raise ValueError("fdtype")
@@ -238,12 +248,13 @@ def finite_difference_jacobian_complex(J, f, x, cache, *, colorvec, sparsity):
             x1[color_i - 1] = x1_save
         else:
             mask = (_color == color_i)
-            x1[:] = x1 + 1j * epsilon * mask                   # :634
+            # im*epsilon = Complex(epsilon*false, epsilon*true); times a Bool each part is a strong zero where false
+            x1[:] = x1 + (_bool_mul(0.0, mask) + 1j * _bool_mul(epsilon, mask))   # :634
             f(fx, x1); calls += 1
             q = vfx.imag / epsilon                             # :636  @. vfx = imag(vfx) / epsilon
             vfx[:] = q
             _colorediteration(J, sparsity, rows_index, cols_index, q, _color, color_i, n, common)
-            x1[:] = x1 - 1j * epsilon * mask                   # :644
+            x1[:] = x1 - (_bool_mul(0.0, mask) + 1j * _bool_mul(epsilon, mask))   # :644
     return {"fcalls": calls}
 
 

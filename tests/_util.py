@@ -7,6 +7,35 @@ import numpy as np
 import scipy.sparse as sp
 
 
+def _host_f64(a):
+    if hasattr(a, "detach"):                     # torch tensor, on any device
+        a = a.detach().cpu().numpy()
+    a = np.asarray(a)
+    assert a.dtype == np.float64, f"assert_same_bits compares float64 data, got {a.dtype}"
+    return np.ascontiguousarray(a).reshape(-1)
+
+
+def assert_same_bits(got, ref, what="", *, allow_nan=True):
+    """Bit-for-bit equality of two float64 arrays (numpy arrays or torch tensors, CUDA ones included).
+
+    The values are compared as uint64 bit patterns, so +0.0 and -0.0 differ (`==` and np.array_equal treat them as
+    equal).  Every NaN counts as one class, whatever its sign and payload: the CPU and the GPU encode the NaNs they
+    produce differently.  allow_nan=False also fails on any NaN, as np.array_equal without equal_nan does (for results
+    that must be NaN-free, e.g. a J buffer pre-filled with NaN that every slot has to overwrite).  On a mismatch the
+    message names the first differing index and both hex patterns."""
+    g, r = _host_f64(got), _host_f64(ref)
+    assert g.shape == r.shape, f"{what}: shapes differ, {g.shape} vs {r.shape}"
+    if not allow_nan:
+        assert not (np.isnan(g).any() or np.isnan(r).any()), f"{what}: NaN where none is expected"
+    gb, rb = g.view(np.uint64), r.view(np.uint64)
+    gn, rn = np.isnan(g), np.isnan(r)
+    bad = np.flatnonzero((gb != rb) & ~(gn & rn))
+    if bad.size:
+        i = int(bad[0])
+        raise AssertionError(f"{what}: {bad.size} of {g.size} values differ in their bits; first at index {i}: "
+                             f"got {g[i]!r} (0x{int(gb[i]):016x}), expected {r[i]!r} (0x{int(rb[i]):016x})")
+
+
 @contextlib.contextmanager
 def fdb_env(**switches):
     """Set FDB_* switches (DESIGN.md §4) while plans are created, restoring the previous environment afterwards.

@@ -8,7 +8,7 @@ import pytest
 import scipy.sparse as sps
 import torch
 
-from _util import csc_to_dense
+from _util import assert_same_bits, csc_to_dense
 
 
 def f_lap5(g):
@@ -55,7 +55,7 @@ def test_oracle_bbb_equals_csc_of_same_pattern(pkg, oracle):
     oracle.jacobian(oracle.Problem.csc_same(n, n, colptr, rowval), nz, f_lap5(g), x.copy(), colorvec=colors)
     Jb = np.zeros((n, n))
     Jb[rows - 1, cols - 1] = data[slots - 1]
-    assert np.array_equal(Jb, csc_to_dense(n, n, colptr, rowval, nz))          # Jbbb == Jsparse (coloring_tests.jl:115)
+    assert_same_bits(Jb, csc_to_dense(n, n, colptr, rowval, nz), allow_nan=False)               # Jbbb == Jsparse (coloring_tests.jl:115)
     # and both equal the uncoloured dense Jacobian
     Jd = np.zeros(n * n)
     oracle.jacobian(oracle.Problem.dense(n, n), Jd, f_lap5(g), x.copy())
@@ -90,11 +90,12 @@ def test_gpu_bbb_bitexact(pkg, oracle, fdtype):
     # slots the structure does not address are zero (fill_matrix!), the others bit-identical
     touched = np.zeros(9 * n, bool)
     touched[slots - 1] = True
-    assert np.array_equal(got[touched], ref[touched]) and np.all(got[~touched] == 0)
+    assert_same_bits(got[touched], ref[touched], allow_nan=False)
+    assert np.all(got[~touched] == 0)
     # cache-less entry picks the structured J as its own sparsity (jacobians.jl:455)
     B2 = _bbb(pkg, g, dev)
     pkg.finite_difference_jacobian_(B2, f, x, fdtype, colorvec=colors)
-    assert np.array_equal(B2.data.cpu().numpy()[touched], ref[touched])
+    assert_same_bits(B2.data.cpu().numpy()[touched], ref[touched], allow_nan=False)
 
 
 def test_block_banded_dense_blocks_structure(pkg, oracle):

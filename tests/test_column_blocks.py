@@ -9,7 +9,7 @@ import pytest
 
 torch = pytest.importorskip("torch")
 
-from _util import cyc_colors, tridiag_csc  # noqa: E402
+from _util import assert_same_bits, cyc_colors, tridiag_csc  # noqa: E402
 
 
 def test_column_blocks_balance_entries_cpu():
@@ -110,7 +110,7 @@ def test_tridiagonal_blocks_bit_identical(pkg, fdtype, n, world):
     Jb = pkg.SparseMatrixCSC(n, n, cp, rv, torch.full((nnz,), float("nan"), dtype=torch.float64, device=dev))
     ep = fdist.EpsPlan(n, cv, fdtype, dev)
     eps = ep.compute(x)
-    assert np.array_equal(eps.cpu().numpy()[:3], eps_full)
+    assert_same_bits(eps.cpu().numpy()[:3], eps_full, allow_nan=False)
     bounds = fdist.column_blocks(colptr, world)
     ctxs = []
 
@@ -129,7 +129,7 @@ def test_tridiagonal_blocks_bit_identical(pkg, fdtype, n, world):
             c_loc = int(max(cv[blk.x0:blk.x1]))             # the colour loop runs 1:maximum(colorvec) of the slice
             assert ctxs[-1].calls == (1 + c_loc if fdtype == "forward" else 2 * c_loc)
         calls += ctxs[-1].calls
-    assert torch.equal(Jb.nzval, J.nzval)                 # bit-identical, every slot written exactly once
+    assert_same_bits(Jb.nzval, J.nzval, allow_nan=False)                   # bit-identical, every slot written exactly once
     assert not torch.isnan(Jb.nzval).any()
 
 
@@ -169,7 +169,7 @@ def test_pentadiagonal_python_callable_blocks(pkg):
                                         lambda r0, r1, x0, x1: (lambda fx, xs: rows(fx, xs, r0, r1, x0)))
         blk.run(x, eps)
     torch.cuda.synchronize()
-    assert torch.equal(Jb.nzval, J.nzval)
+    assert_same_bits(Jb.nzval, J.nzval, allow_nan=False)
     # and the values are the analytic derivative 2 w[k] x_j to forward-difference accuracy
     dense = torch.zeros(n, n, dtype=torch.float64)
     col_of = np.repeat(np.arange(n), np.diff(colptr))

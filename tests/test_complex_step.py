@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from _util import band_to_dense, csc_from_dense_pattern, csc_to_dense, cyc_colors, tridiag_csc, tridiagonal_coo, tridiagonal_to_dense
+from _util import assert_same_bits, band_to_dense, csc_from_dense_pattern, csc_to_dense, cyc_colors, tridiag_csc, tridiagonal_coo, tridiagonal_to_dense
 
 EPS = np.finfo(float).eps
 
@@ -105,9 +105,9 @@ def test_oracle_native_complex_tridiag_matches_python(oracle):
     oracle.jacobian_complex(oracle.Problem.csc_same(N, N, colptr, rowval), a, f_tridiag_c, x, colorvec=cv)
     oracle.jacobian_complex(oracle.Problem.csc_same(N, N, colptr, rowval), b, oracle.native_fn("synth_tridiag_c"), x,
                             colorvec=cv, ctx=oracle.SynthTridiagCtx(N, 1))
-    assert np.array_equal(a, b)
+    assert_same_bits(a, b, allow_nan=False)
     col_of = np.repeat(np.arange(1, N + 1), np.diff(colptr))
-    assert np.array_equal(a, np.where(rowval == col_of, -2.0, 1.0))      # (eps*k)/eps is exact
+    assert_same_bits(a, np.where(rowval == col_of, -2.0, 1.0), allow_nan=False)           # (eps*k)/eps is exact
 
 
 # ------------------------------------------------------------------------------------------------ CUDA path (GPU)
@@ -144,14 +144,14 @@ def test_gpu_complex_csc_bitexact(pkg, oracle, strategy):
         x_before = x.clone()
         pkg.finite_difference_jacobian_(J, f, x, cache)
         torch.cuda.synchronize()
-        assert torch.equal(x, x_before)
+        assert_same_bits(x, x_before, allow_nan=False)
         assert ctx.calls == colors                                                  # coloring_tests.jl:48: fcalls == 3
         np.testing.assert_array_equal(cache._last_plan.eps(), np.full(colors, EPS))
         ref = np.full(len(rowval), np.nan)
         r = oracle.jacobian_complex(oracle.Problem.csc_same(N, N, colptr, rowval), ref, oracle.native_fn("synth_tridiag_c"),
                                     oracle.fill_x(N, 0x5EED + 9), colorvec=cv, ctx=oracle.SynthTridiagCtx(N, 1))
         assert r["fcalls"] == colors
-        assert np.array_equal(J.nzval.cpu().numpy(), ref)
+        assert_same_bits(J.nzval.cpu().numpy(), ref, allow_nan=False)
 
 
 @pytest.mark.gpu

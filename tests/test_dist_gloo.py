@@ -34,7 +34,7 @@ def _worker(rank, world, port, mode, out_dir):
         pkg = _bootstrap.load_package()
         from finitediff_jl_b200 import distributed as fdist
         from oracle import fd_oracle as orc
-        from _util import tridiag_csc, cyc_colors, f_tridiag
+        from _util import assert_same_bits, tridiag_csc, cyc_colors, f_tridiag
         N, C_ = 600, 7
         colptr, rowval = tridiag_csc(N)
         cv = cyc_colors(N, C_)
@@ -55,7 +55,7 @@ def _worker(rank, world, port, mode, out_dir):
         mine[sel] = torch.from_numpy(full)[sel]
         fdist.allgather_owned(mine, gp, rank)
         got = mine.numpy()
-        assert np.array_equal(got, full), f"rank {rank}: gathered Jacobian differs"
+        assert_same_bits(got, full, f"rank {rank}: gathered Jacobian differs", allow_nan=False)
         loads = [int(counts[owner == r].sum()) for r in range(world)]
         (Path(out_dir) / f"ok_{rank}").write_text(f"{loads}")
     finally:

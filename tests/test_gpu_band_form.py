@@ -11,7 +11,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from _util import band_csc, fdb_env
+from _util import assert_same_bits, band_csc, fdb_env
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -76,7 +76,7 @@ def run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=False, f_in
                         x.cpu().numpy().copy(), fdtype=0 if fdtype == "forward" else 1, colorvec=cv, eps_override=eps,
                         no_drift=no_drift, dir=dirv, ctx=octx, **kw)
     assert ctx.calls == r["fcalls"]
-    assert np.array_equal(got, ref, equal_nan=True)
+    assert_same_bits(got, ref)
     own = oracle.jacobian(oracle.Problem.csc_same(m, n, colptr, rowval), np.zeros(E), oracle.native_fn("synth_ellrows"),
                           x.cpu().numpy().copy(), fdtype=0 if fdtype == "forward" else 1, colorvec=cv, no_drift=no_drift,
                           dir=dirv, ctx=octx, **kw)
@@ -97,8 +97,8 @@ def check(pkg, oracle, m, n, cols, cv, fdtype, expect_band, is_cyclic=None, seed
         is_cyclic = bool(np.array_equal(cv, cyclic(n, C_)))
     got, eps, info = run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, **kw)
     got0, eps0, info0 = run(pkg, oracle, m, n, colptr, rowval, cv, fdtype, seed, no_band=True, **kw)
-    assert np.array_equal(eps, eps0)
-    assert np.array_equal(got, got0, equal_nan=True)
+    assert_same_bits(eps, eps0, allow_nan=False)
+    assert_same_bits(got, got0)
     want = band_bytes(info, m, n, E, C_, fdtype, is_cyclic)
     if expect_band:
         assert info["staged"] == 1

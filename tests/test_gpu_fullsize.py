@@ -26,7 +26,7 @@ pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 
-from _util import cyc_colors  # noqa: E402
+from _util import assert_same_bits, cyc_colors  # noqa: E402
 
 FD = {"forward": 0, "central": 1}
 
@@ -96,7 +96,7 @@ def test_c3_full_size_sampled_columns_bitexact(pkg, oracle, dev, fdtype):
     rowval = np.concatenate([np.arange(a, b + 1) for a, b in zip(r_lo, r_hi)]).astype(np.int64) + 1
     ref = np.full(len(rowval), np.nan)
     xh = oracle.fill_x(n, 0x5EED + 3)
-    assert np.array_equal(xh, x.cpu().numpy())
+    assert_same_bits(xh, x.cpu().numpy(), allow_nan=False)
     oracle.jacobian(oracle.Problem.csc_same(n, n, colptr, rowval), ref, oracle.native_fn("synth_lap5"), xh, fdtype=FD[fdtype],
                     colorvec=cv, eps_override=eps, ctx=oracle.SynthLap5Ctx(g, 1), nthreads=host_threads())
     p = 0
@@ -104,7 +104,7 @@ def test_c3_full_size_sampled_columns_bitexact(pkg, oracle, dev, fdtype):
         col = J.data[c * w:(c + 1) * w].cpu().numpy()
         k = b - a + 1
         d0 = u + a - c                                    # slot of row a:  u + r - c
-        assert np.array_equal(col[d0:d0 + k], ref[p:p + k]), f"column {c}"
+        assert_same_bits(col[d0:d0 + k], ref[p:p + k], f"column {c}", allow_nan=False)
         assert not col[:d0].any() and not col[d0 + k:].any(), f"corner slots of column {c} must be 0"
         p += k
     # nothing left undefined anywhere in the 16 GB
@@ -144,12 +144,12 @@ def test_c4_full_size_bitexact(pkg, oracle, dev, strategy):
     octx = oracle.SynthEllCtx(n, K, colsT.ctypes.data_as(C.POINTER(C.c_int32)), coefT.ctypes.data_as(C.POINTER(C.c_double)), nt)
     ref = np.full(n * K, np.nan)
     xh = oracle.fill_x(n, 0x5EED + 4, nt)
-    assert np.array_equal(xh, x.cpu().numpy())
+    assert_same_bits(xh, x.cpu().numpy(), allow_nan=False)
     r = oracle.jacobian(oracle.Problem.csc_same(n, n, colptr, rowval), ref, oracle.native_fn("synth_ellrows"), xh,
                         fdtype=FD[fdtype], colorvec=cv, eps_override=eps, ctx=octx, nthreads=nt)
     assert r["fcalls"] == 65 and prob["ctx"].calls == 65
     got = J.nzval.cpu().numpy()
-    assert np.array_equal(got, ref)
+    assert_same_bits(got, ref, allow_nan=False)
     assert np.isfinite(got).all() and np.count_nonzero(got) > 0.99 * got.size
 
 
@@ -182,8 +182,8 @@ def test_c5_column_block_bitexact(pkg, oracle, dev):
     r = oracle.jacobian(oracle.Problem.dense(n, n), ref, oracle.native_fn("synth_rank1"), oracle.fill_x(n, 0x5EED + 5), fdtype=1,
                         colorvec=cv, ctx=oracle.SynthRank1Ctx(n, wh.ctypes.data_as(C.POINTER(C.c_double)), 1))
     assert r["fcalls"] == 2 * (e - b)
-    assert np.array_equal(plan.eps(), r["eps"])
-    assert np.array_equal(Jslab.cpu().numpy(), ref)
+    assert_same_bits(plan.eps(), r["eps"], allow_nan=False)
+    assert_same_bits(Jslab.cpu().numpy(), ref, allow_nan=False)
 
 
 # ---------------------------------------------------------------------------------------------------- large-shape branches
@@ -204,7 +204,7 @@ def test_band_wider_than_2049_bitexact(pkg, oracle, dev, fdtype):
     ref = np.full((l + u + 1) * n, np.nan)
     oracle.jacobian(oracle.Problem.banded(n, n, l, u), ref, oracle.native_fn("synth_lap5"), oracle.fill_x(n, 11), fdtype=FD[fdtype],
                     colorvec=cv, eps_override=cache._last_plan.eps(), ctx=oracle.SynthLap5Ctx(g, 1))
-    assert np.array_equal(J.data.cpu().numpy(), ref)
+    assert_same_bits(J.data.cpu().numpy(), ref, allow_nan=False)
 
 
 @pytest.mark.parametrize("fdtype", ["forward", "central"])
@@ -226,7 +226,7 @@ def test_dense_many_row_blocks_batch_256_bitexact(pkg, oracle, dev, fdtype):
     r = oracle.jacobian(oracle.Problem.dense(n, n), ref, oracle.native_fn("synth_rank1"), oracle.fill_x(n, 13), fdtype=FD[fdtype],
                         ctx=oracle.SynthRank1Ctx(n, w.ctypes.data_as(C.POINTER(C.c_double)), 1), nthreads=host_threads())
     assert ctx.calls == r["fcalls"]
-    assert np.array_equal(J.cpu().numpy().reshape(-1, order="F"), ref)
+    assert_same_bits(J.cpu().numpy().reshape(-1, order="F"), ref, allow_nan=False)
 
 
 def test_windowed_eps_random_pattern_700_colors(pkg, oracle, dev):
@@ -263,7 +263,7 @@ def test_windowed_eps_random_pattern_700_colors(pkg, oracle, dev):
         np.testing.assert_allclose(eps, own["eps"], rtol=1e-14)
         oracle.jacobian(oracle.Problem.csc_same(n, n, colptr, rowval), ref, oracle.native_fn("synth_ellrows"), xh.copy(),
                         colorvec=cv, eps_override=eps, ctx=octx)
-        assert np.array_equal(J.nzval.cpu().numpy(), ref)
+        assert_same_bits(J.nzval.cpu().numpy(), ref, allow_nan=False)
 
 
 # ---------------------------------------------------------------------------------------------------- ADVICE r1 / VERDICT r1 items
@@ -286,7 +286,7 @@ def test_dense_view_with_padding_rows(pkg, oracle, dev):
     oracle.jacobian(oracle.Problem.csc_to_dense(N, N, colptr, rowval), ref, oracle.native_fn("synth_tridiag"), oracle.fill_x(N, 3),
                     colorvec=cv, eps_override=cache._last_plan.eps(), ctx=oracle.SynthTridiagCtx(N, 1))
     got = store.cpu().numpy()
-    assert np.array_equal(got[:, :N].T.reshape(-1, order="F"), ref)
+    assert_same_bits(got[:, :N].T.reshape(-1, order="F"), ref, allow_nan=False)
     assert (got[:, N:] == 7.25).all(), "padding rows between the columns do not belong to J"
     # host-buffer entry point with the same strided layout
     L = pkg._lib
@@ -299,7 +299,8 @@ def test_dense_view_with_padding_rows(pkg, oracle, dev):
     L.check(L.lib().fdb_jacobian_host(plan.handle, C.cast(L.synth().fdbs_tridiag, C.c_void_p), C.cast(C.pointer(ctx), C.c_void_p),
                                       xh.ctypes.data, Jh.ctypes.data, None, None, float("nan"), float("nan"), 1.0))
     hv = np.array(Jh).reshape(N, ld)
-    assert np.array_equal(hv[:, :N].T.reshape(-1, order="F"), ref) and (hv[:, N:] == 7.25).all()
+    assert_same_bits(hv[:, :N].T.reshape(-1, order="F"), ref, allow_nan=False)
+    assert (hv[:, N:] == 7.25).all()
 
 
 @pytest.mark.parametrize("fdtype", ["forward", "central"])

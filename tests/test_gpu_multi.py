@@ -46,6 +46,7 @@ def _worker(rank, world, port, out_dir):
         import scipy.sparse as sps
         import _bootstrap
         pkg = _bootstrap.load_package()
+        from _util import assert_same_bits
         from finitediff_jl_b200 import distributed as fdist
         from oracle import fd_oracle as orc
         L = pkg._lib
@@ -88,7 +89,7 @@ def _worker(rank, world, port, out_dir):
                                  fdtype=0 if fdtype == "forward" else 1, colorvec=cv, eps_override=eps, ctx=octx)
                     got = J.nzval.cpu().numpy()
                     if gather != "root" or rank == 0:
-                        assert np.array_equal(got, ref), f"rank {rank} {fdtype} {mode} partition={partition} {gather}"
+                        assert_same_bits(got, ref, f"rank {rank} {fdtype} {mode} partition={partition} {gather}", allow_nan=False)
                     else:   # gather="root": a non-root rank stores straight into rank 0's nzval; its own buffer is untouched
                         assert np.isnan(got).all()
                     per_call = ctx.calls // 2
@@ -114,7 +115,7 @@ def _worker(rank, world, port, out_dir):
         ref = np.zeros(nd * nd)
         orc.jacobian(orc.Problem.dense(nd, nd), ref, orc.native_fn("synth_rank1"), xd.copy(), fdtype=1,
                      ctx=orc.SynthRank1Ctx(nd, w.ctypes.data_as(C.POINTER(C.c_double)), 1))
-        assert np.array_equal(Jslab.cpu().numpy(), ref[b * nd: e * nd]), f"rank {rank} dense slab"
+        assert_same_bits(Jslab.cpu().numpy(), ref[b * nd: e * nd], f"rank {rank} dense slab", allow_nan=False)
         assert ctx.calls == 2 * (e - b)
         # column-block shards (few-colour problem): every rank owns a block of columns; J sharded, then gathered on rank 0
         from _util import cyc_colors, tridiag_csc
@@ -145,10 +146,10 @@ def _worker(rank, world, port, out_dir):
                              fdtype=0 if fdtype == "forward" else 1, colorvec=cvt, eps_override=eps, ctx=octx_t)
                 got = Jt.nzval.cpu().numpy()
                 if gather == "root" and rank == 0:
-                    assert np.array_equal(got, ref), f"column shards gathered on root, {fdtype}"
+                    assert_same_bits(got, ref, f"column shards gathered on root, {fdtype}", allow_nan=False)
                 elif gather is None:
                     b = cs.block
-                    assert np.array_equal(got[b.p0:b.p1], ref[b.p0:b.p1]), f"rank {rank} column block {fdtype}"
+                    assert_same_bits(got[b.p0:b.p1], ref[b.p0:b.p1], f"rank {rank} column block {fdtype}", allow_nan=False)
                     assert np.isnan(got[:b.p0]).all() and np.isnan(got[b.p1:]).all()
                 cs.close()
         (Path(out_dir) / f"ok_{rank}").write_text("ok")

@@ -20,7 +20,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
-from _util import band_csc, fdb_env, tridiag_csc
+from _util import assert_same_bits, band_csc, fdb_env, tridiag_csc
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -276,7 +276,7 @@ class Problem:
             r = self.oracle.jacobian(P, ref, self.oracle.native_fn("synth_ellrows"), self.xh.copy(), fdtype=FD[self.fdtype],
                                      colorvec=self.cv, eps_override=eps, no_drift=no_drift, dir=dirv, ctx=self.octx(), **kw)
             assert ctx.calls == r["fcalls"]
-            assert np.array_equal(got, ref, equal_nan=True), f"J differs from the oracle at sm_count={sm_count} env={env}"
+            assert_same_bits(got, ref, f"J differs from the oracle at sm_count={sm_count} env={env}")
             np.testing.assert_allclose(eps, self.own_eps(dirv, no_drift), rtol=1e-13)
         return res
 
@@ -382,8 +382,8 @@ def test_staged_switches_bit_identical(pkg, oracle, fdtype, sm_count):
         p = probs[form]
         r = p.run(sm_count, env, profile=True, oracle_check=False)
         ref = base["band" if form == "band" else "packed"]
-        assert np.array_equal(r["eps"], ref["eps"]), (form, env)
-        assert np.array_equal(r["J"], ref["J"], equal_nan=True), (form, env)
+        assert_same_bits(r["eps"], ref["eps"], (form, env), allow_nan=False)
+        assert_same_bits(r["J"], ref["J"], (form, env))
         assert r["calls"] == ref["calls"]
         inst, smem = staged_instance(r["kernels"])
         assert inst == want, (form, env, inst)
@@ -415,7 +415,8 @@ def test_perturb_multiwave(pkg, oracle, fdtype, no_drift, max_batch, sm_count):
     note(r["kernels"], "perturb_colors", -(-n // TILE), need=3 if sm_count == 1 else None)
     if not no_drift and max_batch == 1:
         r0 = p.run(sm_count, {"REVERSE": 0}, oracle_check=False)      # forward walk: same bits
-        assert np.array_equal(r0["eps"], r["eps"]) and np.array_equal(r0["J"], r["J"])
+        assert_same_bits(r0["eps"], r["eps"], allow_nan=False)
+        assert_same_bits(r0["J"], r["J"], allow_nan=False)
 
 
 @pytest.mark.parametrize("C_,kind", [(3, "cyclic"), (7, "random")])
@@ -430,8 +431,8 @@ def test_eps_depth_bit_identical(pkg, oracle, C_, kind, aligned, sm_count):
     off = 0 if aligned else 1
     r2 = p.run(sm_count, x_offset=off, profile=True)
     r1 = p.run(sm_count, {"EPS_DEPTH": 1}, x_offset=off, profile=True)
-    assert np.array_equal(r1["eps"], r2["eps"])
-    assert np.array_equal(r1["J"], r2["J"])
+    assert_same_bits(r1["eps"], r2["eps"], allow_nan=False)
+    assert_same_bits(r1["J"], r2["J"], allow_nan=False)
     d2 = [int(_targs(k[0])[-1]) for k in launches(r2["kernels"], "color_sumsq_reg")]
     d1 = [int(_targs(k[0])[-1]) for k in launches(r1["kernels"], "color_sumsq_reg")]
     assert d2 == [2] and d1 == [1]
@@ -453,8 +454,8 @@ def test_list_eps_independent_of_grid(pkg, oracle, fdtype):
     p = Problem(pkg, oracle, n, n, colptr, rowval, colouring("random", n, 40), fdtype, seed=8)
     runs = {k: p.run(k, profile=True, max_batch=4) for k in (None, 1, 3)}
     for k in (1, 3):
-        assert np.array_equal(runs[k]["eps"], runs[None]["eps"])
-        assert np.array_equal(runs[k]["J"], runs[None]["J"])
+        assert_same_bits(runs[k]["eps"], runs[None]["eps"], allow_nan=False)
+        assert_same_bits(runs[k]["J"], runs[None]["J"], allow_nan=False)
         assert plan_shape(runs[k]["info"]) == plan_shape(runs[None]["info"])
     assert runs[1]["info"]["staged"] == 0
     note(runs[1]["kernels"], "finalize_eps_lists", 40 / 8)
@@ -561,7 +562,7 @@ def banded_run(pkg, oracle, m, n, l, u, C_, fdtype, sm_count, dense=False):
                           ctx=octx)
     got = J.cpu().numpy().reshape(-1, order="F") if dense else Jb.data.cpu().numpy()
     assert ctx.calls == r["fcalls"]
-    assert np.array_equal(got, ref, equal_nan=True)
+    assert_same_bits(got, ref)
     np.testing.assert_allclose(eps, own["eps"], rtol=1e-13)
     return kernels
 
@@ -613,8 +614,8 @@ def test_dense_columns_multiwave(pkg, oracle, fdtype, batch, sm_count):
     r = oracle.jacobian(oracle.Problem.dense(m, n), ref, oracle.native_fn("synth_ellrows"), x.cpu().numpy().copy(),
                         fdtype=FD[fdtype], ctx=octx)
     assert ctx.calls == r["fcalls"] == (n + 1 if fdtype == "forward" else 2 * n)
-    assert np.array_equal(cache._last_plan.eps(), r["eps"])
-    assert np.array_equal(J.cpu().numpy().reshape(-1, order="F"), ref)
+    assert_same_bits(cache._last_plan.eps(), r["eps"], allow_nan=False)
+    assert_same_bits(J.cpu().numpy().reshape(-1, order="F"), ref, allow_nan=False)
     need = 3 if sm_count == 1 else None
     note(ks, "replicate_x", -(-n // THREADS), need=need)
     assert launches(ks, "set_components")

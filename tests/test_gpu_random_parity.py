@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sps
 
-from _util import fdb_env
+from _util import assert_same_bits, fdb_env
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -87,7 +87,7 @@ def _case(rng, pkg, oracle, dev, sm_count=None, lo=1, hi=400):
     got = (J.cpu().numpy().reshape(-1, order="F") if dense_J else sp.nzval.cpu().numpy())
     desc = f"m={m} n={n} K={K} C={cv.max()} {fdtype} {opts} dense={dense_J} f_in={use_fin} dir={dirv} sm_count={sm_count}"
     assert ctx.calls == r["fcalls"], desc
-    assert np.array_equal(got, ref, equal_nan=True), desc
+    assert_same_bits(got, ref, desc)
     own = oracle.jacobian(P, np.zeros_like(ref), oracle.native_fn("synth_ellrows"), x.cpu().numpy().copy(),
                           fdtype=0 if fdtype == "forward" else 1, colorvec=cv, dir=dirv, ctx=octx, **kw)
     np.testing.assert_allclose(eps, own["eps"], rtol=1e-13, err_msg=desc)

@@ -15,7 +15,7 @@ import pytest
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-from _util import cyc_colors, tridiag_csc  # noqa: E402
+from _util import assert_same_bits, cyc_colors, tridiag_csc  # noqa: E402
 
 FD = {"forward": 0, "central": 1}
 
@@ -98,7 +98,7 @@ def test_group_csc_colour_shards(pkg, fdist, oracle, fdtype, partition, strategy
         r = oracle.jacobian(oracle.Problem.csc_same(n, n, colptr, rowval), ref, oracle.native_fn("synth_ellrows"), xh.copy(),
                             fdtype=FD[fdtype], colorvec=cv, eps_override=eps, ctx=octx)
         got = J.nzval.cpu().numpy()
-        assert np.array_equal(got, ref), f"devices={devices} {fdtype} partition={partition} strategy={strategy}"
+        assert_same_bits(got, ref, f"devices={devices} {fdtype} partition={partition} strategy={strategy}", allow_nan=False)
         # ownership is a partition of the colours; every member evaluated exactly its share (+ f(x) in forward mode)
         owner = g.plans[0].color_owner()
         ec = fdist.entry_colors_csc(colptr, cv)
@@ -110,7 +110,7 @@ def test_group_csc_colour_shards(pkg, fdist, oracle, fdtype, partition, strategy
             assert nl == int((owner == i).sum())
             assert c.calls // 2 == (nl + 1 if fdtype == "forward" else 2 * nl)
             total += nl
-            assert np.array_equal(g.plans[i].eps(), eps)          # every member derives the same step sizes
+            assert_same_bits(g.plans[i].eps(), eps, allow_nan=False)               # every member derives the same step sizes
             assert g.plans[i].info()["strategy"] == (1 if strategy == 0 else 0)
         assert total == Cc and r["fcalls"] == (Cc + 1 if fdtype == "forward" else 2 * Cc)
         g.close()
@@ -140,7 +140,7 @@ def test_group_matches_single_plan_and_graph(pkg, fdist, oracle, fdtype):
             J2.nzval.fill_(float("nan"))
             g.run(fs, x)
             g.synchronize()
-        assert torch.equal(J1.nzval, J2.nzval), f"devices={devices}"
+        assert_same_bits(J1.nzval, J2.nzval, f"devices={devices}", allow_nan=False)
         g.close()
 
 
@@ -169,7 +169,7 @@ def test_group_banded(pkg, fdist, oracle, fdtype):
         refb = np.full((2 * gsz + 1) * n, np.nan)
         oracle.jacobian(oracle.Problem.banded(n, n, gsz, gsz), refb, oracle.native_fn("synth_lap5"), xh.copy(),
                         fdtype=FD[fdtype], colorvec=cv, eps_override=g.plans[0].eps(), ctx=oracle.SynthLap5Ctx(gsz, 1))
-        assert np.array_equal(Jb.data.cpu().numpy(), refb), f"band data, devices={devices}"
+        assert_same_bits(Jb.data.cpu().numpy(), refb, f"band data, devices={devices}", allow_nan=False)
         g.close()
         Jd = pkg.zeros_colmajor(n, n, root)
         Jd.fill_(float("nan"))
@@ -179,7 +179,7 @@ def test_group_banded(pkg, fdist, oracle, fdtype):
         refd = np.zeros(n * n)
         oracle.jacobian(oracle.Problem.banded_to_dense(n, n, gsz, gsz), refd, oracle.native_fn("synth_lap5"), xh.copy(),
                         fdtype=FD[fdtype], colorvec=cv, eps_override=g.plans[0].eps(), ctx=oracle.SynthLap5Ctx(gsz, 1))
-        assert np.array_equal(Jd.cpu().numpy().reshape(-1, order="F"), refd), f"dense target, devices={devices}"
+        assert_same_bits(Jd.cpu().numpy().reshape(-1, order="F"), refd, f"dense target, devices={devices}", allow_nan=False)
         g.close()
 
 
@@ -210,7 +210,7 @@ def test_group_dense_column_blocks(pkg, fdist, oracle, fdtype):
         ref = np.zeros(n * n)
         r = oracle.jacobian(oracle.Problem.dense(n, n), ref, oracle.native_fn("synth_rank1"), xh.copy(), fdtype=FD[fdtype],
                             ctx=oracle.SynthRank1Ctx(n, w.ctypes.data_as(C.POINTER(C.c_double)), 1))
-        assert np.array_equal(J.cpu().numpy().reshape(-1, order="F"), ref), f"devices={devices}"
+        assert_same_bits(J.cpu().numpy().reshape(-1, order="F"), ref, f"devices={devices}", allow_nan=False)
         cols = 0
         for i, c in enumerate(ctxs):
             b, e = g.plans[i].dense_range()

@@ -9,6 +9,7 @@ import pytest
 import scipy.sparse as sps
 
 import _literal_reference as lit
+from _util import assert_same_bits
 
 FD = {"forward": 0, "central": 1}
 KINDS = ["csc_same", "csc_to_dense", "proto_to_dense", "banded", "banded_to_dense", "dense_cols"]
@@ -108,15 +109,15 @@ def test_oracle_matches_literal_transcription(oracle, kind, seed):
     ro = oracle.jacobian(P, Jo, f, x.copy(), **okw)
     assert ro["fcalls"] == rl["fcalls"]
     # both restatements evaluate norm as the reference does (generic_norm2 / OpenBLAS dnrm2): same step sizes, same J
-    assert np.array_equal(ro["eps"], rl["eps"]), f"{kind} {fdtype} seed {seed}"
-    assert np.array_equal(Jo, Jl, equal_nan=True), f"{kind} {fdtype} seed {seed}"
+    assert_same_bits(ro["eps"], rl["eps"], f"{kind} {fdtype} seed {seed}", allow_nan=False)
+    assert_same_bits(Jo, Jl, f"{kind} {fdtype} seed {seed}")
     Jo2 = np.full(Jl.size, np.nan)
     cache_o = dict(x1=np.full(n, np.nan), x2=np.full(n, np.nan), fx=np.full(m, np.nan), fx1=np.full(m, np.nan))
     oracle.jacobian(P, Jo2, f, x.copy(), eps_override=None if kind == "dense_cols" else rl["eps"], cache=cache_o, **okw)
-    assert np.array_equal(Jo2, Jl, equal_nan=True), f"{kind} {fdtype} seed {seed}"
+    assert_same_bits(Jo2, Jl, f"{kind} {fdtype} seed {seed}")
     assert np.array_equal(xl, x) or fdtype == "central"       # forward never touches x
     np.testing.assert_allclose(xl, x, rtol=0, atol=1e-12)     # central: restored up to the reference's own drift
-    assert np.array_equal(cache_o["x1"], cache_l["x1"])       # (x1 + eps) - eps drift, same end state
+    assert_same_bits(cache_o["x1"], cache_l["x1"], allow_nan=False)            # (x1 + eps) - eps drift, same end state
 
 
 @pytest.mark.parametrize("seed", range(30))
@@ -159,7 +160,7 @@ def test_oracle_complex_step_matches_literal_transcription(oracle, kind, seed):
     Jo = np.full(Jl.size, np.nan)
     ro = oracle.jacobian_complex(P, Jo, f, x.copy(), colorvec=None if kind == "dense_cols" else cv)
     assert ro["fcalls"] == rl["fcalls"]
-    assert np.array_equal(Jo, Jl, equal_nan=True), f"{kind} seed {seed}"
+    assert_same_bits(Jo, Jl, f"{kind} seed {seed}")
 
 
 @pytest.mark.parametrize("seed", range(60))
@@ -188,8 +189,8 @@ def test_oracle_jvp_matches_literal_transcription(oracle, seed):
     assert ro["fcalls"] == rl["fcalls"]
     np.testing.assert_allclose(ro["eps"], rl["eps"], rtol=1e-14, atol=0)
     ro2 = oracle.jvp(f, x.copy(), v.copy(), m, fdtype=FD[fdtype], f_in=f_in, eps_override=rl["eps"], **kw)
-    assert np.array_equal(ro2["jvp"], out)
-    assert np.array_equal(ro2["x1"][:n], cache["x1"])          # cache.x1 ends as x + eps*v
+    assert_same_bits(ro2["jvp"], out, allow_nan=False)
+    assert_same_bits(ro2["x1"][:n], cache["x1"], allow_nan=False)               # cache.x1 ends as x + eps*v
 
 
 @pytest.mark.parametrize("seed", range(40))
@@ -224,7 +225,7 @@ def test_oracle_cacheless_matches_literal_transcription(oracle, kind, seed):
                          eps_override=None if kind == "dense_cols" else rl["eps"])
     assert ro["fcalls"] == rl["fcalls"] == ((1 if fdtype == "forward" else 0) +
                                             (n if cv is None else int(cv.max())) * (1 if fdtype == "forward" else 2))
-    assert np.array_equal(Jo, Jl, equal_nan=True), f"{kind} {fdtype} seed {seed}"
+    assert_same_bits(Jo, Jl, f"{kind} {fdtype} seed {seed}")
 
 
 @pytest.mark.parametrize("seed", range(12))
@@ -250,5 +251,5 @@ def test_oracle_dense_branch_with_colorvec_matches_literal(oracle, fdtype, seed)
     Jo = np.full(m * n, -7.5)
     ro = oracle.jacobian(oracle.Problem.dense(m, n), Jo, f, x.copy(), fdtype=FD[fdtype], colorvec=cv)
     assert ro["fcalls"] == rl["fcalls"] == (maxc + 1 if fdtype == "forward" else 2 * maxc)
-    assert np.array_equal(Jo.reshape(m, n, order="F"), Jl)
+    assert_same_bits(Jo.reshape(m, n, order="F"), Jl, allow_nan=False)
     assert (Jl[:, maxc:] == -7.5).all() and not (Jl[:, :maxc] == -7.5).any()
