@@ -1340,7 +1340,7 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
       dim3 grid((unsigned)std::min<int64_t>(P->eps_list_max_chunks, 1024), (unsigned)std::min<int32_t>(C, 65535));
       color_sumsq_lists<<<grid, kThreads, 0, s>>>(x, P->cols_by_color, P->bucket_start_d, P->chunk_base_d, C, P->eps_list_partial);
       finalize_eps_lists<<<(int)std::min<int64_t>(((int64_t)C * 32 + kThreads - 1) / kThreads, (int64_t)P->sm_count * 8), kThreads, 0, s>>>(
-          P->eps_list_partial, P->chunk_base_d, C, prm, P->eps, P->sumsq);
+          P->eps_list_partial, P->chunk_base_d, C, prm, P->eps, P->sumsq, x, P->cols_by_color, P->bucket_start_d, P->n);
       P->cnt.kernel_launches += 2;
       CU(cudaGetLastError());
       return FDB_OK;
@@ -1366,8 +1366,8 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
       color_sumsq_win<CT><<<P->eps_blocks, kThreads, (size_t)kEpsWarps * W * sizeof(double), s>>>(
           x, (const CT *)P->jcolor, P->n, P->eps_chunk, k0, W, P->eps_group, P->partial);
       // partial rows are W wide for this pass
-      finalize_eps<<<(W * 32 + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->partial, P->eps_blocks, W, k0, W, prm,
-                                                                        P->eps, P->sumsq);
+      finalize_eps<CT><<<(W * 32 + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->partial, P->eps_blocks, W, k0, W, prm,
+                                                                            P->eps, P->sumsq, x, (const CT *)P->jcolor, P->n);
       P->cnt.kernel_launches += 2;
     }
   }

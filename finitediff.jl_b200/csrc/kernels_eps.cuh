@@ -22,14 +22,74 @@ struct EpsParams {
   double relstep, absstep, dir;
 };
 
-// the step-size formula from a colour's sum of squares
-__device__ __forceinline__ double eps_from_sumsq(double ss, const EpsParams &p) {
-  const double tmp = sqrt(ss);                        // norm(x2)                     jacobians.jl:560
+// the step-size formula from a colour's norm
+__device__ __forceinline__ double eps_from_norm(double tmp, const EpsParams &p) {
   const double a = p.relstep * fabs(sqrt(tmp));       // relstep*abs(sqrt(tmp))       :561 + epsilons.jl:28
   double e = max_julia(a, p.absstep);                 // max(.., absstep)
   if (!p.fdtype_central) e = e * p.dir;               // *dir (forward only)          epsilons.jl:28 vs :52
   return e;
 }
+
+// ... and from its fp64 sum of squares
+__device__ __forceinline__ double eps_from_sumsq(double ss, const EpsParams &p) {
+  return eps_from_norm(sqrt(ss), p);                  // norm(x2)                     jacobians.jl:560
+}
+
+// ---- sums of squares outside the fp64 range ----
+// The reference's norm(x2) is OpenBLAS dnrm2 for n >= 32, an x87 80-bit sum that neither overflows nor underflows for
+// any double, and stdlib generic_norm2 for n < 32.  A plain fp64 sum gives Inf once |x| >~ 1.34e154, and below ~1e-154
+// every square is rounded to a subnormal grid of absolute step 2^-1074: n such roundings put the sum about
+// n*2^-1075 / sum off, even when the sum itself is a normal number.  Below 2^-900 that loss can exceed the parity bar for
+// plausible n; above it, it is under n*2^-175.
+//   n >= 32: the norm is rescued when the sum is +Inf or below 2^-900.
+//   n < 32:  generic_norm2 sums unscaled (as lossily as a plain fp64 sum: subnormal squares add exactly) unless
+//            maxabs^2 == 0 or n*maxabs^2 overflows.  maxabs^2 == 0 is a zero sum; an overflowing n*maxabs^2 with a
+//            finite sum leaves both sums accurate; so the rescue runs when the sum is 0 or +Inf.
+// A NaN sum is never rescued (the step is NaN either way).  Small sums need no rescue when max(relstep*sqrt(tmp),
+// absstep) is absstep for every tmp <= 2^-448 (the default absstep = relstep is such a case).  The check is made per
+// colour where the step size is formed; in-range colours take no other instruction.
+constexpr double kSumsqRescueBelow = 0x1p-900;
+
+// Warp-uniform when ss is (every lane holds the same warp_sum result).
+__device__ __forceinline__ bool sumsq_out_of_range(double ss, int64_t n, const EpsParams &p) {
+  if (ss == INFINITY) return true;
+  if (!(n < 32 ? ss == 0.0 : ss < kSumsqRescueBelow)) return false;
+  return !(fabs(p.relstep) * 0x1p-224 < p.absstep);
+}
+
+// eps of a colour whose fp64 sum of squares `ss` is out of range, from its norm re-read from x (nothing writes the
+// caller's x while the step sizes are computed).  Called by all 32 lanes of a warp; `value(i)` is the colour's i-th component for
+// i in [0, count), or 0.0 for an index outside the colour.  The components are scaled by 2^-600 (sum +Inf) or 2^600
+// (sum small): exact, and the square of every finite scaled double is then a finite normal number.  Lane-strided
+// partial sums and a fixed shuffle tree: the value depends only on the colour's components in the order `value` gives.
+// Not inlined, and it stores eps itself so that little is live across the call: the callers' register counts stay what
+// their in-range code needs.
+template <class Value>
+__device__ __noinline__ void store_rescued_eps(Value value, int64_t count, double ss, EpsParams prm, double *eps_k) {
+  const bool big = ss == INFINITY;
+  const double down = big ? 0x1p-600 : 0x1p600;
+  double acc = 0.0;
+  for (int64_t i = threadIdx.x & 31; i < count; i += 32) {
+    const double v = value(i) * down;
+    acc += v * v;
+  }
+  const double e = eps_from_norm(sqrt(warp_sum(acc)) * (big ? 0x1p600 : 0x1p-600), prm);
+  if ((threadIdx.x & 31) == 0) *eps_k = e;
+}
+
+// colour k's components of x in index order, through a colour source (register path) or a colour table (window path)
+template <typename CS> struct ColourOfSource {
+  const double *x;
+  CS colors;
+  uint32_t k;
+  __device__ __forceinline__ double operator()(int64_t j) const { return colors.at(j) == k ? x[j] : 0.0; }
+};
+// colour k's components through its column list (list path): ascending, as the plan sorted them
+struct ColourOfList {
+  const double *x;
+  const int32_t *cols;
+  __device__ __forceinline__ double operator()(int64_t i) const { return x[cols[i]]; }
+};
 
 // C <= 8: per-thread register accumulators (NC = 4 or 8 of them) over the block's tiles (fixed tile -> block -> lane
 // mapping; colours from a colour source, common.cuh), shuffle tree, fixed warp order; the LAST block to finish (atomic ticket) reduces the block partials in
@@ -133,10 +193,9 @@ color_sumsq_reg(const double *__restrict__ x, const CS colors, int64_t n, int x_
     }
     for (; b < (int)gridDim.x; b += 32) t0 += __ldcg(partial + (int64_t)b * kEpsRegColors + w);
     double t = warp_sum((t0 + t1) + (t2 + t3));
-    if (lane == 0) {
-      eps[w] = eps_from_sumsq(t, prm);
-      if (sumsq) sumsq[w] = t;
-    }
+    if (lane == 0 && sumsq) sumsq[w] = t;
+    if (sumsq_out_of_range(t, n, prm)) store_rescued_eps(ColourOfSource<CS>{x, colors, (uint32_t)w}, n, t, prm, eps + w);
+    else if (lane == 0) eps[w] = eps_from_sumsq(t, prm);
   }
   if (threadIdx.x == 0) *ticket = 0u;   // re-arm for the next call (stream-ordered)
 }
@@ -261,7 +320,8 @@ color_sumsq_lists(const double *__restrict__ x, const int32_t *__restrict__ cols
 // one warp per colour: chunk partials in fixed order, then the step-size formula
 __global__ void __launch_bounds__(kThreads)
 finalize_eps_lists(const double *__restrict__ partial, const int64_t *__restrict__ chunk_base, int32_t C, EpsParams prm,
-                   double *__restrict__ eps, double *__restrict__ sumsq) {
+                   double *__restrict__ eps, double *__restrict__ sumsq, const double *__restrict__ x,
+                   const int32_t *__restrict__ cols_by_color, const int64_t *__restrict__ bucket_start, int64_t n) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = (blockIdx.x * (int64_t)kThreads + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * kThreads) >> 5;
@@ -270,28 +330,34 @@ finalize_eps_lists(const double *__restrict__ partial, const int64_t *__restrict
     double t = 0.0;
     for (int64_t p = p0 + lane; p < p1; p += 32) t += partial[p];
     t = warp_sum(t);
-    if (lane == 0) {
+    if (lane == 0 && sumsq) sumsq[k] = t;
+    if (sumsq_out_of_range(t, n, prm)) {
+      const int64_t b0 = bucket_start[k];
+      store_rescued_eps(ColourOfList{x, cols_by_color + b0}, bucket_start[k + 1] - b0, t, prm, eps + k);
+    } else if (lane == 0) {
       eps[k] = eps_from_sumsq(t, prm);
-      if (sumsq) sumsq[k] = t;
     }
   }
 }
 
 // One warp per colour: fixed-order reduction over the block partials, then the step-size formula.
+template <typename CT>
 __global__ void __launch_bounds__(kThreads)
 finalize_eps(const double *__restrict__ partial, int32_t nblocks, int32_t stride /* colours per partial row */,
              int32_t k0, int32_t ncolors_here, EpsParams prm, double *__restrict__ eps /* [C] */,
-             double *__restrict__ sumsq /* [C] or null */) {
+             double *__restrict__ sumsq /* [C] or null */, const double *__restrict__ x, const CT *__restrict__ jcolor,
+             int64_t n) {
   const int lane = threadIdx.x & 31;
   const int c = (int)((blockIdx.x * (int64_t)kThreads + threadIdx.x) >> 5);
   if (c >= ncolors_here) return;
   double t = 0.0;
   for (int b = lane; b < nblocks; b += 32) t += partial[(int64_t)b * stride + c];
   t = warp_sum(t);
-  if (lane == 0) {
+  if (lane == 0 && sumsq) sumsq[k0 + c] = t;
+  if (sumsq_out_of_range(t, n, prm))
+    store_rescued_eps(ColourOfSource<TableColors<CT>>{x, {jcolor}, (uint32_t)(k0 + c)}, n, t, prm, eps + k0 + c);
+  else if (lane == 0)
     eps[k0 + c] = eps_from_sumsq(t, prm);
-    if (sumsq) sumsq[k0 + c] = t;
-  }
 }
 
 // Dense-column branch: per-COMPONENT step (jacobians.jl:550,592): eps_i = compute_epsilon(fd, x_i, relstep, absstep, dir)

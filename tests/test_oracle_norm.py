@@ -70,6 +70,60 @@ def test_generic_norm2_below_32_elements(oracle):
     assert oracle.norm2(tiny) == 1e-200 * float(np.sqrt(5.0))
 
 
+def _in_order_norm(x):
+    s = 0.0
+    for v in x:
+        s += float(v) * float(v)
+    return float(np.sqrt(s))
+
+
+def _scaled_norm(x):
+    m = float(np.max(np.abs(x)))
+    s = 0.0
+    for v in x:
+        t = abs(float(v)) / m
+        s += t * t
+    return m * float(np.sqrt(s))
+
+
+@pytest.mark.parametrize("n", [13, 31])
+def test_generic_norm2_branches_at_the_ends_of_the_range(oracle, n):
+    # generic_norm2 scales only when maxabs^2 == 0 or n*maxabs^2 overflows; otherwise it keeps the in-order Float64 sum,
+    # however lossy (the device step-size pass follows the same rule for n < 32)
+    rng = np.random.default_rng(n)
+    sub = rng.uniform(0.5, 1.5, n) * 1e-160 * np.where(rng.random(n) < 0.5, -1.0, 1.0)   # squares subnormal, nonzero
+    r = oracle.norm2(sub)
+    assert r == _in_order_norm(sub)
+    assert abs(r / _scaled_norm(sub) - 1) > 1e-9         # the lossy value, not the accurate one
+    zero_sq = rng.uniform(0.5, 1.5, n) * 1e-170              # every square underflows to 0
+    assert oracle.norm2(zero_sq) == _scaled_norm(zero_sq) and oracle.norm2(zero_sq) > 0
+    big = rng.uniform(0.5, 1.5, n) * 1e150                    # n*maxabs^2 overflows, the sum of squares itself does not
+    big[n // 3] = -1.2e154
+    m = float(np.max(np.abs(big)))
+    assert np.isinf(n * m * m) and np.isfinite(float(np.sum(big * big)))
+    assert oracle.norm2(big) == _scaled_norm(big)
+    huge = np.full(n, 1e300)                                  # squares overflow
+    assert oracle.norm2(huge) == _scaled_norm(huge) == 1e300 * float(np.sqrt(float(n)))
+    mixed = np.zeros(n)
+    mixed[[0, n // 2]] = [5e-324, -0.0]                       # the smallest subnormal: its square is 0
+    assert oracle.norm2(mixed) == 5e-324
+
+
+def test_subnormal_square_sums_to_a_normal_number(oracle):
+    # 10^5 equal components whose squares are subnormal and each rounded by nearly half an ulp: the plain Float64 sum is
+    # a normal number but 1.07e-11 off; dnrm2 (x87 extended) is not
+    from fractions import Fraction
+    v = 4.79825341824841e-157
+    sq = v * v
+    err = abs(Fraction(sq) - Fraction(v) ** 2) / Fraction(5e-324)
+    assert 0.45 < err <= 0.5
+    x = np.full(100_000, v)
+    r = oracle.norm2(x)
+    assert r == 1.517340959235351e-154
+    plain = float(np.sqrt(np.sum(x * x)))
+    assert abs(plain / r - 1) > 5e-12
+
+
 @pytest.mark.parametrize("fdtype", [0, 1])
 def test_driver_step_size_uses_this_norm(oracle, fdtype):
     # the eps the oracle's colour loop reports == compute_epsilon(sqrt(norm(x .* (color .== k)))) with fdo_norm2
