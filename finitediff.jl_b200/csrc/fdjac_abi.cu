@@ -437,26 +437,32 @@ static fdb_status finish_colored_plan(fdb_plan *P, const fdb_plan_opts *o, const
   return FDB_OK;
 }
 
-// Per-colour column lists (cols_by_color, ascending inside a colour; P->bucket_start must be set) and, for more colours
-// than the register path takes, the chunk tables of the list-based eps pass.
+// Per-colour column lists: bucket_start ([C+2] offsets into cols_by_color; bucket C = columns without a valid colour),
+// cols_by_color (the column ids stable-sorted by colour: ascending inside a colour) and, for more colours than the
+// register path takes, the chunk tables of the list-based eps pass.
 static fdb_status build_color_lists(fdb_plan *P) {
   const int64_t n = P->n;
   const int32_t C = P->C;
-  if (!P->cols_by_color) TRY(P->alloc_t(&P->cols_by_color, (size_t)std::max<int64_t>(n, 1)));
+  TRY(P->alloc_t(&P->cols_by_color, (size_t)std::max<int64_t>(n, 1)));
+  std::vector<unsigned long long> bc((size_t)C + 1, 0);
   if (n > 0) {
     // a stable radix sort of the column ids by colour (deterministic: the list-based eps pass sums in list order, and
     // sharded and unsharded plans must produce the same bits)
+    unsigned long long *d_bucket = nullptr;
     uint32_t *k_in = nullptr, *k_out = nullptr;
     int32_t *v_in = nullptr;
     void *d_tmp = nullptr;
     size_t tmp_bytes = 0;
-    auto cleanup = [&]() { cudaFree(k_in); cudaFree(k_out); cudaFree(v_in); cudaFree(d_tmp); };
-    cudaError_t e = cudaMalloc((void **)&k_in, (size_t)n * 4);
+    auto cleanup = [&]() { cudaFree(d_bucket); cudaFree(k_in); cudaFree(k_out); cudaFree(v_in); cudaFree(d_tmp); };
+    cudaError_t e = cudaMalloc((void **)&d_bucket, ((size_t)C + 1) * 8);
+    if (e == cudaSuccess) e = cudaMemset(d_bucket, 0, ((size_t)C + 1) * 8);
+    if (e == cudaSuccess) e = cudaMalloc((void **)&k_in, (size_t)n * 4);
     if (e == cudaSuccess) e = cudaMalloc((void **)&k_out, (size_t)n * 4);
     if (e == cudaSuccess) e = cudaMalloc((void **)&v_in, (size_t)n * 4);
     if (e == cudaSuccess) {
       dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
         using CT = decltype(tag);
+        count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, d_bucket);
         color_sort_keys<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, k_in, v_in);
         return FDB_OK;
       });
@@ -465,11 +471,13 @@ static fdb_status build_color_lists(fdb_plan *P) {
       e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in, k_out, v_in, P->cols_by_color, (int)n, 0, end_bit);
       if (e == cudaSuccess) e = cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16);
       if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, k_in, k_out, v_in, P->cols_by_color, (int)n, 0, end_bit);
-      if (e == cudaSuccess) e = cudaDeviceSynchronize();
+      if (e == cudaSuccess) e = cudaMemcpy(bc.data(), d_bucket, ((size_t)C + 1) * 8, cudaMemcpyDeviceToHost);
     }
     cleanup();
     if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "column lists: %s", cudaGetErrorString(e));
   }
+  P->bucket_start.assign((size_t)C + 2, 0);
+  for (int32_t k = 0; k <= C; ++k) P->bucket_start[(size_t)k + 1] = P->bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
   // step sizes from the column lists (more colours than the register path takes)
   if (C > kEpsRegColors && C <= (1 << 22) && n > 0) {
     std::vector<int64_t> cb((size_t)C + 1, 0);
@@ -488,16 +496,6 @@ static fdb_status build_color_lists(fdb_plan *P) {
     P->eps_list_max_chunks = maxc;
     P->eps_lists = true;
   }
-  return FDB_OK;
-}
-
-// host offsets of the per-colour column buckets from their device counts ([C+1]: bucket C = columns without a valid colour)
-static fdb_status bucket_offsets(fdb_plan *P, const unsigned long long *d_bucket_counts) {
-  const int32_t C = P->C;
-  std::vector<unsigned long long> bc((size_t)C + 1, 0);
-  CU(cudaMemcpy(bc.data(), d_bucket_counts, ((size_t)C + 1) * 8, cudaMemcpyDeviceToHost));
-  P->bucket_start.assign((size_t)C + 2, 0);
-  for (int32_t k = 0; k <= C; ++k) P->bucket_start[(size_t)k + 1] = P->bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
   return FDB_OK;
 }
 
@@ -903,26 +901,11 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
   // ---- per-colour column lists + gather-locality metric -> scatter strategy
   {
     const int32_t C = P->C;
-    unsigned long long *d_bucket = nullptr, *d_jump = nullptr;
-    PLAN_TRY(P->alloc_t(&d_bucket, (size_t)C + 2));
+    unsigned long long *d_jump = nullptr;
     PLAN_TRY(P->alloc_t(&d_jump, 1));
-    cudaMemset(d_bucket, 0, ((size_t)C + 2) * 8);
     cudaMemset(d_jump, 0, 8);
     PLAN_TRY(P->alloc_t(&P->colptr32, (size_t)n + 1));
-    PLAN_TRY(P->alloc_t(&P->cols_by_color, (size_t)std::max<int64_t>(n, 1)));
-    PLAN_TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-      using CT = decltype(tag);
-      colptr32_and_count<CT><<<P->grid(n + 1), kThreads>>>(cp.d, n, (const CT *)P->jcolor, C, P->colptr32, d_bucket);
-      CU(cudaGetLastError());
-      return FDB_OK;
-    }));
-    std::vector<unsigned long long> bc((size_t)C + 1, 0);
-    {
-      cudaError_t e = cudaMemcpy(bc.data(), d_bucket, ((size_t)C + 1) * 8, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "column buckets: %s", cudaGetErrorString(e)); }
-    }
-    P->bucket_start.assign((size_t)C + 2, 0);
-    for (int32_t k = 0; k <= C; ++k) P->bucket_start[(size_t)k + 1] = P->bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
+    convert_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, P->colptr32);
     PLAN_TRY(build_color_lists(P));
     if (nnz > 1) {
       row_jump_sum<<<P->grid(nnz), kThreads>>>(P->row32, nnz, d_jump);
@@ -1838,19 +1821,7 @@ fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorv
   PLAN_TRY(alloc_eps_buffers(P));
   // the same list-based eps pass as the Jacobian plans: a column block's external step sizes are then bit-identical to
   // the ones the unsharded plan computes for itself
-  if (P->C > kEpsRegColors && n > 0) {
-    unsigned long long *d_bucket = nullptr;
-    PLAN_TRY(P->alloc_t(&d_bucket, (size_t)P->C + 2));
-    cudaMemset(d_bucket, 0, ((size_t)P->C + 2) * 8);
-    PLAN_TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-      using CT = decltype(tag);
-      count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_bucket);
-      CU(cudaGetLastError());
-      return FDB_OK;
-    }));
-    PLAN_TRY(bucket_offsets(P, d_bucket));
-    PLAN_TRY(build_color_lists(P));
-  }
+  if (P->C > kEpsRegColors && n > 0) PLAN_TRY(build_color_lists(P));
   return FDB_OK;
 }
 

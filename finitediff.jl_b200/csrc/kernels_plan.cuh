@@ -255,27 +255,15 @@ prepare_coo(const int64_t *__restrict__ rows, const int64_t *__restrict__ cols, 
   count_end(s_cnt, C, color_count);
 }
 
-// ---- per-colour column lists (the reference's "for col in 1:ncols; if colorvec[col]==color_i" test, done ONCE) ----
-// colptr32[c] = colptr[c]-1 (0-based int32), column counts per colour bucket (bucket C = columns without a valid colour)
-template <typename CT>
+// colptr32[c] = colptr[c]-1 (0-based int32)
 __global__ void __launch_bounds__(kThreads)
-colptr32_and_count(const int64_t *__restrict__ colptr, int64_t n, const CT *__restrict__ jcolor, int32_t C,
-                   int32_t *__restrict__ colptr32, unsigned long long *__restrict__ bucket_count /* [C+1] */) {
+convert_colptr(const int64_t *__restrict__ colptr, int64_t n, int32_t *__restrict__ colptr32) {
   const int64_t stride = (int64_t)gridDim.x * kThreads;
-  for (int64_t c = blockIdx.x * (int64_t)kThreads + threadIdx.x; c <= n; c += stride) {
-    colptr32[c] = (int32_t)(colptr[c] - 1);
-    if (c < n) {
-      uint32_t k = (uint32_t)jcolor[c];
-      if (k >= (uint32_t)C) k = (uint32_t)C;
-      // warp-aggregated histogram: lanes holding the same colour elect a leader that adds the group's population
-      const unsigned act = __activemask();
-      const unsigned peers = __match_any_sync(act, k);
-      if ((threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(bucket_count + k, (unsigned long long)__popc(peers));
-    }
-  }
+  for (int64_t c = blockIdx.x * (int64_t)kThreads + threadIdx.x; c <= n; c += stride) colptr32[c] = (int32_t)(colptr[c] - 1);
 }
 
-// column counts per colour bucket (bucket C = columns without a valid colour) — plans without a CSC colptr
+// ---- per-colour column lists (the reference's "for col in 1:ncols; if colorvec[col]==color_i" test, done ONCE) ----
+// column counts per colour bucket (bucket C = columns without a valid colour)
 template <typename CT>
 __global__ void __launch_bounds__(kThreads)
 count_color_buckets(const CT *__restrict__ jcolor, int64_t n, int32_t C, unsigned long long *__restrict__ bucket_count /* [C+1] */) {
