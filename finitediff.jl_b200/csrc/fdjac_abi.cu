@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <numeric>
 #include <string>
@@ -58,6 +59,47 @@ static fdb_status fail(fdb_status st, const char *fmt, ...) {
   } while (0)
 
 enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6 };
+
+// Device memory that lives while a plan or a colouring is built: freed when it goes out of scope, unless release()
+// hands it to a plan that keeps it (fdb_plan::adopt).  Declared after the builder's DeviceGuard, it is freed on the
+// device it was allocated on.
+template <typename T> struct DevBuf {
+  T *p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  fdb_status alloc(size_t count) {
+    bytes = count * sizeof(T);
+    if (bytes == 0) bytes = 16;
+    const cudaError_t e = cudaMalloc((void **)&p, bytes);
+    if (e != cudaSuccess) {
+      p = nullptr;
+      return fail(FDB_ERR_NOMEM, "cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
+    }
+    return FDB_OK;
+  }
+  T *get() const { return p; }
+  T *release() { T *q = p; p = nullptr; return q; }
+};
+
+// copy `count` values back from the device; `what` names the value in the error text
+template <typename T> static fdb_status read_back(T *h, const T *d, size_t count, const char *what) {
+  const cudaError_t e = cudaMemcpy(h, d, count * sizeof(T), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e));
+  return FDB_OK;
+}
+
+// a CUB device algorithm, called the two-phase way: `algo(nullptr, bytes)` sizes its scratch, `algo(tmp, bytes)` runs
+template <typename F> static fdb_status cub_run(F &&algo) {
+  size_t bytes = 0;
+  CU(algo(nullptr, bytes));
+  DevBuf<char> tmp;
+  TRY(tmp.alloc(bytes));
+  CU(algo((void *)tmp.get(), bytes));
+  return FDB_OK;
+}
 
 struct DeviceGuard {
   int prev = -1;
@@ -196,15 +238,16 @@ struct fdb_plan {
   bool timing = false;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pending, ev_pool;
 
-  fdb_status alloc(void **p, size_t bytes) {
-    if (bytes == 0) bytes = 16;
-    cudaError_t e = cudaMalloc(p, bytes);
-    if (e != cudaSuccess) {
-      *p = nullptr;
-      return fail(FDB_ERR_NOMEM, "cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
-    }
-    allocs.push_back(*p);
+  // device memory the plan keeps until fdb_plan_destroy (build scratch is a DevBuf instead)
+  void adopt(void *p, size_t bytes) {
+    allocs.push_back(p);
     device_bytes += bytes;
+  }
+  fdb_status alloc(void **p, size_t bytes) {
+    DevBuf<char> b;
+    TRY(b.alloc(bytes));
+    *p = b.get();
+    adopt(b.release(), b.bytes);
     return FDB_OK;
   }
   template <typename T> fdb_status alloc_t(T **p, size_t count) { return alloc((void **)p, count * sizeof(T)); }
@@ -220,8 +263,7 @@ struct fdb_plan {
 // A caller-supplied Int64 array that may live on the host or the device: make it readable by kernels.
 struct I64View {
   const int64_t *d = nullptr;
-  int64_t *owned = nullptr;
-  ~I64View() { if (owned) cudaFree(owned); }
+  DevBuf<int64_t> copy;   // device copy of a host array
 };
 
 static fdb_status view_i64(const int64_t *p, int64_t count, I64View &v) {
@@ -230,9 +272,9 @@ static fdb_status view_i64(const int64_t *p, int64_t count, I64View &v) {
   cudaError_t e = cudaPointerGetAttributes(&at, p);
   if (e != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
   if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) { v.d = p; return FDB_OK; }
-  CU(cudaMalloc((void **)&v.owned, (size_t)count * sizeof(int64_t)));
-  CU(cudaMemcpy(v.owned, p, (size_t)count * sizeof(int64_t), cudaMemcpyHostToDevice));
-  v.d = v.owned;
+  TRY(v.copy.alloc((size_t)count));
+  CU(cudaMemcpy(v.copy.get(), p, (size_t)count * sizeof(int64_t), cudaMemcpyHostToDevice));
+  v.d = v.copy.get();
   return FDB_OK;
 }
 
@@ -273,24 +315,28 @@ static const char *plan_err_text(uint32_t e) {
   return "invalid pattern";
 }
 
+// maximum and minimum of a device colour vector of length n > 0 (order-free: the grid cannot change them)
+static fdb_status color_range(const int64_t *d_colorvec, int64_t n, long long *mx, long long *mn) {
+  DevBuf<long long> d_mm;
+  TRY(d_mm.alloc(2));
+  const long long init[2] = {LLONG_MIN, LLONG_MAX};
+  CU(cudaMemcpy(d_mm.get(), init, sizeof init, cudaMemcpyHostToDevice));
+  const int blocks = (int)std::min<int64_t>((n + kThreads - 1) / kThreads, 132 * 8);
+  color_minmax<<<blocks, kThreads>>>(d_colorvec, n, d_mm.get(), d_mm.get() + 1);
+  long long out[2];
+  TRY(read_back(out, d_mm.get(), 2, "colour min/max failed"));
+  *mx = out[0];
+  *mn = out[1];
+  return FDB_OK;
+}
+
 // colours: max/min, narrow type, per-column colour array
-static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or device or null*/, I64View &cv) {
+static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or device or null*/) {
   const int64_t n = P->n;
+  I64View cv;
   TRY(view_i64(colorvec, n, cv));
   long long mx = n, mn = n > 0 ? 1 : 0;
-  if (cv.d && n > 0) {
-    long long *d_mm = nullptr;
-    CU(cudaMalloc((void **)&d_mm, 2 * sizeof(long long)));
-    long long init[2] = {LLONG_MIN, LLONG_MAX};
-    CU(cudaMemcpy(d_mm, init, sizeof init, cudaMemcpyHostToDevice));
-    color_minmax<<<P->grid(n), kThreads>>>(cv.d, n, d_mm, d_mm + 1);
-    long long out[2];
-    cudaError_t e = cudaMemcpy(out, d_mm, sizeof out, cudaMemcpyDeviceToHost);
-    cudaFree(d_mm);
-    if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "colour min/max failed: %s", cudaGetErrorString(e));
-    mx = out[0];
-    mn = out[1];
-  }
+  if (cv.d && n > 0) TRY(color_range(cv.d, n, &mx, &mn));
   if (n == 0) mx = 0;
   if (mx < 0) mx = 0;                       // maximum(colorvec) < 1: the colour loop 1:max is empty
   if (mx > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "maximum(colorvec) = %lld exceeds 2^31", mx);
@@ -299,30 +345,25 @@ static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or de
   P->color_bits = mx <= 255 ? 8 : (mx <= 65535 ? 16 : 32);
   TRY(P->alloc(&P->jcolor, (size_t)std::max<int64_t>(n, 1) * (P->color_bits / 8)));
   if (n > 0) {
-    uint32_t *d_flags = nullptr;   // [0] lane conflicts (window path), [1] not cyclic
+    DevBuf<uint32_t> d_flags;   // [0] lane conflicts (window path), [1] not cyclic
     const bool window_path = P->C > kEpsRegColors;
-    CU(cudaMalloc((void **)&d_flags, 2 * sizeof(uint32_t)));
-    CU(cudaMemset(d_flags, 0, 2 * sizeof(uint32_t)));
-    fdb_status st = dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(d_flags.alloc(2));
+    CU(cudaMemset(d_flags.get(), 0, 2 * sizeof(uint32_t)));
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
       convert_colors<CT><<<P->grid(n), kThreads>>>(cv.d, n, (CT *)P->jcolor);
-      if (window_path) color_lane_conflicts<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags);
-      if (P->C > 0) check_cyclic<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags + 1);
+      if (window_path) color_lane_conflicts<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags.get());
+      if (P->C > 0) check_cyclic<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags.get() + 1);
       CU(cudaGetLastError());
       return FDB_OK;
-    });
-    if (st == FDB_OK) {
-      uint32_t flags[2] = {0, 0};
-      cudaError_t e = cudaMemcpy(flags, d_flags, sizeof flags, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) st = fail(FDB_ERR_CUDA, "colour flags: %s", cudaGetErrorString(e));
-      P->cyclic = P->C > 0 && flags[1] == 0;
-      if (window_path) {
-        P->eps_group = 1;
-        for (int lg = 1; lg <= 5 && !(flags[0] & (1u << lg)); ++lg) P->eps_group = 1 << lg;
-      }
+    }));
+    uint32_t flags[2] = {0, 0};
+    TRY(read_back(flags, d_flags.get(), 2, "colour flags"));
+    P->cyclic = P->C > 0 && flags[1] == 0;
+    if (window_path) {
+      P->eps_group = 1;
+      for (int lg = 1; lg <= 5 && !(flags[0] & (1u << lg)); ++lg) P->eps_group = 1 << lg;
     }
-    cudaFree(d_flags);
-    if (st != FDB_OK) return st;
   }
   return FDB_OK;
 }
@@ -448,33 +489,26 @@ static fdb_status build_color_lists(fdb_plan *P) {
   if (n > 0) {
     // a stable radix sort of the column ids by colour (deterministic: the list-based eps pass sums in list order, and
     // sharded and unsharded plans must produce the same bits)
-    unsigned long long *d_bucket = nullptr;
-    uint32_t *k_in = nullptr, *k_out = nullptr;
-    int32_t *v_in = nullptr;
-    void *d_tmp = nullptr;
-    size_t tmp_bytes = 0;
-    auto cleanup = [&]() { cudaFree(d_bucket); cudaFree(k_in); cudaFree(k_out); cudaFree(v_in); cudaFree(d_tmp); };
-    cudaError_t e = cudaMalloc((void **)&d_bucket, ((size_t)C + 1) * 8);
-    if (e == cudaSuccess) e = cudaMemset(d_bucket, 0, ((size_t)C + 1) * 8);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&k_in, (size_t)n * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&k_out, (size_t)n * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&v_in, (size_t)n * 4);
-    if (e == cudaSuccess) {
-      dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-        using CT = decltype(tag);
-        count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, d_bucket);
-        color_sort_keys<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, k_in, v_in);
-        return FDB_OK;
-      });
-      int end_bit = 1;
-      while (end_bit < 32 && ((uint64_t)1 << end_bit) <= (uint64_t)C) ++end_bit;
-      e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in, k_out, v_in, P->cols_by_color, (int)n, 0, end_bit);
-      if (e == cudaSuccess) e = cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16);
-      if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, k_in, k_out, v_in, P->cols_by_color, (int)n, 0, end_bit);
-      if (e == cudaSuccess) e = cudaMemcpy(bc.data(), d_bucket, ((size_t)C + 1) * 8, cudaMemcpyDeviceToHost);
-    }
-    cleanup();
-    if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "column lists: %s", cudaGetErrorString(e));
+    DevBuf<unsigned long long> d_bucket;
+    DevBuf<uint32_t> k_in, k_out;
+    DevBuf<int32_t> v_in;
+    TRY(d_bucket.alloc((size_t)C + 1));
+    CU(cudaMemset(d_bucket.get(), 0, ((size_t)C + 1) * 8));
+    TRY(k_in.alloc((size_t)n));
+    TRY(k_out.alloc((size_t)n));
+    TRY(v_in.alloc((size_t)n));
+    dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+      using CT = decltype(tag);
+      count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, d_bucket.get());
+      color_sort_keys<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, k_in.get(), v_in.get());
+      return FDB_OK;
+    });
+    int end_bit = 1;
+    while (end_bit < 32 && ((uint64_t)1 << end_bit) <= (uint64_t)C) ++end_bit;
+    TRY(cub_run([&](void *tmp, size_t &bytes) {
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, k_in.get(), k_out.get(), v_in.get(), P->cols_by_color, (int)n, 0, end_bit);
+    }));
+    TRY(read_back(bc.data(), d_bucket.get(), (size_t)C + 1, "column lists"));
   }
   P->bucket_start.assign((size_t)C + 2, 0);
   for (int32_t k = 0; k <= C; ++k) P->bucket_start[(size_t)k + 1] = P->bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
@@ -547,42 +581,33 @@ static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long lo
   const bool wide = P->dest != nullptr;
   TRY(P->alloc(&P->cm_slot, (size_t)std::max<int64_t>(e_local, 1) * (wide ? 8 : 4)));
   if (ncols == 0 || e_local == 0) return FDB_OK;
-  // temporaries (freed below): column list, counts, offsets, scan scratch
-  int64_t *d_src = nullptr, *d_dst = nullptr;
-  int32_t *list_cols = nullptr, *list_cnt = nullptr, *list_off = nullptr;
-  void *d_tmp = nullptr;
-  size_t tmp_bytes = 0;
-  auto cleanup = [&]() {
-    cudaFree(d_src); cudaFree(d_dst); cudaFree(list_cols); cudaFree(list_cnt); cudaFree(list_off); cudaFree(d_tmp);
-  };
-#define CM_CU(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { cleanup(); \
-    return fail(FDB_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); } } while (0)
-  CM_CU(cudaMalloc((void **)&d_src, (size_t)nseg * 8));
-  CM_CU(cudaMalloc((void **)&d_dst, ((size_t)nseg + 1) * 8));
-  CM_CU(cudaMalloc((void **)&list_cols, (size_t)ncols * 4));
-  CM_CU(cudaMalloc((void **)&list_cnt, (size_t)ncols * 4));
-  CM_CU(cudaMalloc((void **)&list_off, (size_t)ncols * 4));
-  CM_CU(cudaMemcpy(d_src, src.data(), (size_t)nseg * 8, cudaMemcpyHostToDevice));
-  CM_CU(cudaMemcpy(d_dst, dst.data(), ((size_t)nseg + 1) * 8, cudaMemcpyHostToDevice));
-  cm_gather_cols<<<(int)std::min<int64_t>(nseg, (int64_t)P->sm_count * 16), kThreads>>>(P->cols_by_color, d_src, d_dst, nseg, list_cols);
-  cm_column_counts<<<P->grid(ncols), kThreads>>>(list_cols, ncols, P->colptr32, list_cnt);
-  CM_CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, list_cnt, list_off, (int)ncols));
-  CM_CU(cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16));
-  CM_CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, list_cnt, list_off, (int)ncols));
+  // temporaries: segment offsets, column list, counts, offsets
+  DevBuf<int64_t> d_src, d_dst;
+  DevBuf<int32_t> list_cols, list_cnt, list_off;
+  TRY(d_src.alloc((size_t)nseg));
+  TRY(d_dst.alloc((size_t)nseg + 1));
+  TRY(list_cols.alloc((size_t)ncols));
+  TRY(list_cnt.alloc((size_t)ncols));
+  TRY(list_off.alloc((size_t)ncols));
+  CU(cudaMemcpy(d_src.get(), src.data(), (size_t)nseg * 8, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d_dst.get(), dst.data(), ((size_t)nseg + 1) * 8, cudaMemcpyHostToDevice));
+  cm_gather_cols<<<(int)std::min<int64_t>(nseg, (int64_t)P->sm_count * 16), kThreads>>>(P->cols_by_color, d_src.get(), d_dst.get(), nseg, list_cols.get());
+  cm_column_counts<<<P->grid(ncols), kThreads>>>(list_cols.get(), ncols, P->colptr32, list_cnt.get());
+  TRY(cub_run([&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::ExclusiveSum(tmp, bytes, list_cnt.get(), list_off.get(), (int)ncols);
+  }));
   {
     const int lanes = P->lanes;
     const int64_t blocks = (ncols + (kThreads / lanes) - 1) / (kThreads / lanes);
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)P->sm_count * 16));
-    if (wide) cm_expand<int64_t><<<grid, kThreads>>>(list_cols, list_off, ncols, P->colptr32, P->row32, P->dest, lanes, P->cm_row, (int64_t *)P->cm_slot);
-    else cm_expand<int32_t><<<grid, kThreads>>>(list_cols, list_off, ncols, P->colptr32, P->row32, nullptr, lanes, P->cm_row, (int32_t *)P->cm_slot);
+    if (wide) cm_expand<int64_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->colptr32, P->row32, P->dest, lanes, P->cm_row, (int64_t *)P->cm_slot);
+    else cm_expand<int32_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->colptr32, P->row32, nullptr, lanes, P->cm_row, (int32_t *)P->cm_slot);
   }
   // consistency: the last column's end must be the entry total the per-colour counts promised
   int32_t last_off = 0, last_cnt = 0;
-  CM_CU(cudaMemcpy(&last_off, list_off + (ncols - 1), 4, cudaMemcpyDeviceToHost));
-  CM_CU(cudaMemcpy(&last_cnt, list_cnt + (ncols - 1), 4, cudaMemcpyDeviceToHost));
-  CM_CU(cudaDeviceSynchronize());
-#undef CM_CU
-  cleanup();
+  TRY(read_back(&last_off, list_off.get() + (ncols - 1), 1, "colour-major list offsets"));
+  TRY(read_back(&last_cnt, list_cnt.get() + (ncols - 1), 1, "colour-major list counts"));
+  CU(cudaDeviceSynchronize());
   if ((int64_t)last_off + last_cnt != e_local)
     return fail(FDB_ERR_INVALID, "internal: colour-major list holds %lld entries, expected %lld", (long long)last_off + last_cnt,
                 (long long)e_local);
@@ -594,26 +619,26 @@ static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long lo
 static fdb_status try_band_form(fdb_plan *P) {
   P->stage_band = false;
   const int64_t m = P->m, n = P->n;
-  int *d_lu = nullptr;
-  uint32_t *d_flag = nullptr;
-  TRY(P->alloc_t(&d_lu, 2));
-  TRY(P->alloc_t(&d_flag, 1));
+  DevBuf<int> d_lu;
+  DevBuf<uint32_t> d_flag;
+  TRY(d_lu.alloc(2));
+  TRY(d_flag.alloc(1));
   const int init[2] = {INT_MIN, INT_MIN};
-  CU(cudaMemcpy(d_lu, init, sizeof init, cudaMemcpyHostToDevice));
-  CU(cudaMemset(d_flag, 0, 4));
-  band_extent<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, n, d_lu);
+  CU(cudaMemcpy(d_lu.get(), init, sizeof init, cudaMemcpyHostToDevice));
+  CU(cudaMemset(d_flag.get(), 0, 4));
+  band_extent<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, n, d_lu.get());
   int lu[2];
-  CU(cudaMemcpy(lu, d_lu, sizeof lu, cudaMemcpyDeviceToHost));
+  TRY(read_back(lu, d_lu.get(), 2, "band extent"));
   const int l = lu[0], u = lu[1];
-  band_check<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, m, n, l, u, d_flag);
+  band_check<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, m, n, l, u, d_flag.get());
   uint32_t bad = 1;
-  CU(cudaMemcpy(&bad, d_flag, 4, cudaMemcpyDeviceToHost));
+  TRY(read_back(&bad, d_flag.get(), 1, "band check"));
   if (bad) return FDB_OK;
   // interior columns [a, b): c - l >= 0 and c + u <= m - 1 — every one holds all w = l + u + 1 rows
   const int64_t a = std::min<int64_t>(std::max(l, 0), n), b = std::max<int64_t>(a, std::min<int64_t>(n, m - u));
   int32_t ea = 0, eb = 0;
-  CU(cudaMemcpy(&ea, P->colptr32 + a, 4, cudaMemcpyDeviceToHost));
-  CU(cudaMemcpy(&eb, P->colptr32 + b, 4, cudaMemcpyDeviceToHost));
+  TRY(read_back(&ea, P->colptr32 + a, 1, "band column pointer"));
+  TRY(read_back(&eb, P->colptr32 + b, 1, "band column pointer"));
   P->band_l = l;
   P->band_w = l + u + 1;
   P->band_col_a = (int32_t)a;
@@ -634,22 +659,25 @@ static fdb_status try_stage_plan(fdb_plan *P) {
   const int nwin = P->fdtype == FDB_CENTRAL ? 2 * P->C : P->C + 1;
   const int64_t ntiles = P->E / kTile;
   if (nwin > kStageMaxWin || ntiles < 1) return FDB_OK;
-  unsigned int *d_span = nullptr;
-  TRY(P->alloc_t(&d_span, 1));
-  CU(cudaMemset(d_span, 0, 4));
-  TRY(P->alloc_t(&P->tile_w0, (size_t)ntiles));
-  TRY(P->alloc_t(&P->row16, (size_t)ntiles * kTile));
+  // built here, kept by the plan only when the staged form is chosen
+  DevBuf<unsigned int> d_span;
+  DevBuf<int32_t> tile_w0;
+  DevBuf<uint16_t> row16;
+  TRY(d_span.alloc(1));
+  CU(cudaMemset(d_span.get(), 0, 4));
+  TRY(tile_w0.alloc((size_t)ntiles));
+  TRY(row16.alloc((size_t)ntiles * kTile));
   const int pgrid = (int)std::min<int64_t>(ntiles, (int64_t)P->sm_count * 16);
-  stage_prepare<uint8_t><<<pgrid, kThreads>>>(P->row32, ntiles, P->tile_w0, P->row16, d_span, nullptr, P->C);
+  stage_prepare<uint8_t><<<pgrid, kThreads>>>(P->row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), nullptr, P->C);
   unsigned int span = 0;
-  CU(cudaMemcpy(&span, d_span, 4, cudaMemcpyDeviceToHost));
+  TRY(read_back(&span, d_span.get(), 1, "staged row span"));
   const int64_t W = ((int64_t)span + 1) & ~(int64_t)1;
   // few colours, short windows: pack the entry's colour into the top 4 bits of its row offset (no colour stream at all)
   P->stage_packed = P->C <= 14 && W <= 4096 && span > 0 && !P->tune.no_pack;
   if (P->stage_packed) {
     TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      stage_prepare<CT><<<pgrid, kThreads>>>(P->row32, ntiles, P->tile_w0, P->row16, d_span, (const CT *)P->ecolor, P->C);
+      stage_prepare<CT><<<pgrid, kThreads>>>(P->row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), (const CT *)P->ecolor, P->C);
       CU(cudaGetLastError());
       return FDB_OK;
     }));
@@ -657,6 +685,8 @@ static fdb_status try_stage_plan(fdb_plan *P) {
   }
   const size_t smem = (size_t)2 * nwin * W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8;
   if (span == 0 || span > 65535 || smem > (size_t)kStageMaxSmem) return FDB_OK;   // not row-local enough: keep the gather form
+  P->adopt(P->tile_w0 = tile_w0.release(), tile_w0.bytes);
+  P->adopt(P->row16 = row16.release(), row16.bytes);
   P->stage_W = (int32_t)W;
   P->staged = true;
   if (!P->tune.no_band) TRY(try_band_form(P));
@@ -665,7 +695,7 @@ static fdb_status try_stage_plan(fdb_plan *P) {
 
 static fdb_status read_plan_err(uint32_t *d_err, const char *what) {
   uint32_t h = 0;
-  CU(cudaMemcpy(&h, d_err, 4, cudaMemcpyDeviceToHost));
+  TRY(read_back(&h, d_err, 1, what));
   const uint32_t hard = h & ~(uint32_t)(kErrPatternDiff | kErrRowOrder);
   if (hard == kErrMissingInJ) return fail(FDB_ERR_UNSUPPORTED, "%s: %s", what, plan_err_text(hard));
   if (hard) return fail(FDB_ERR_INVALID, "%s: %s", what, plan_err_text(hard));
@@ -703,47 +733,6 @@ static void read_tunables(fdb_plan *P) {
   }
 }
 
-static fdb_status new_plan(fdb_plan **out, const fdb_plan_opts *o, int64_t m, int64_t n) {
-  if (!out) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
-  *out = nullptr;
-  if (m < 0 || n < 0) return fail(FDB_ERR_INVALID, "negative dimensions m=%lld n=%lld", (long long)m, (long long)n);
-  if (m > 0x7FFFFFF0LL || n > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "m, n must be < 2^31");
-  if (o && o->fdtype != FDB_FORWARD && o->fdtype != FDB_CENTRAL && o->fdtype != FDB_COMPLEX)
-    return fail(FDB_ERR_UNSUPPORTED, "Unrecognized fdtype: valid values are forward (0), central (1) and complex (2)");
-  int dev = 0;
-  TRY(check_device(o, &dev));
-  fdb_plan *P = new (std::nothrow) fdb_plan();
-  if (!P) return fail(FDB_ERR_NOMEM, "out of host memory");
-  P->device = dev;
-  P->m = m;
-  P->n = n;
-  P->fdtype = o ? o->fdtype : FDB_FORWARD;
-  P->no_drift = o ? o->no_drift : 0;
-  P->use_graph = o && o->use_graph != 0;
-  P->shared_J = o && o->shared_j != 0;
-  read_tunables(P);
-  P->world = (o && o->world > 1) ? o->world : 1;
-  P->rank = (o && o->world > 1) ? o->rank : 0;
-  if (P->rank < 0 || P->rank >= P->world) {
-    const int bad_rank = P->rank, bad_world = P->world;
-    delete P;
-    return fail(FDB_ERR_INVALID, "rank %d outside world %d", bad_rank, bad_world);
-  }
-  cudaDeviceProp prop;
-  cudaError_t e = cudaGetDeviceProperties(&prop, dev);
-  if (e != cudaSuccess) { delete P; return fail(FDB_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); }
-  P->sm_count = prop.multiProcessorCount;
-  // FDB_SM_COUNT=k (tests): size every grid as if the device had k SMs, so small problems already give each block several
-  // tiles.  Launch geometry only: no plan decision reads sm_count.
-  if (const char *v = getenv("FDB_SM_COUNT")) {
-    const int k = atoi(v);
-    if (k >= 1 && k < P->sm_count) P->sm_count = k;
-  }
-  P->l2_bytes = prop.l2CacheSize;
-  *out = P;
-  return FDB_OK;
-}
-
 static void free_plan(fdb_plan *P) {
   if (!P) return;
   DeviceGuard g(P->device);
@@ -760,11 +749,53 @@ static void free_plan(fdb_plan *P) {
   delete P;
 }
 
-#define PLAN_TRY(expr)                                   \
-  do {                                                   \
-    fdb_status s__ = (expr);                             \
-    if (s__ != FDB_OK) { free_plan(P); *plan = nullptr; return s__; } \
-  } while (0)
+struct PlanFree { void operator()(fdb_plan *P) const { free_plan(P); } };
+// a plan under construction: freed on every failure path, handed to the caller by release() once it is complete
+using PlanPtr = std::unique_ptr<fdb_plan, PlanFree>;
+
+static fdb_status new_plan(fdb_plan **out, PlanPtr &P, const fdb_plan_opts *o, int64_t m, int64_t n) {
+  if (!out) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *out = nullptr;
+  if (m < 0 || n < 0) return fail(FDB_ERR_INVALID, "negative dimensions m=%lld n=%lld", (long long)m, (long long)n);
+  if (m > 0x7FFFFFF0LL || n > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "m, n must be < 2^31");
+  if (o && o->fdtype != FDB_FORWARD && o->fdtype != FDB_CENTRAL && o->fdtype != FDB_COMPLEX)
+    return fail(FDB_ERR_UNSUPPORTED, "Unrecognized fdtype: valid values are forward (0), central (1) and complex (2)");
+  int dev = 0;
+  TRY(check_device(o, &dev));
+  P.reset(new (std::nothrow) fdb_plan());
+  if (!P) return fail(FDB_ERR_NOMEM, "out of host memory");
+  P->device = dev;
+  P->m = m;
+  P->n = n;
+  P->fdtype = o ? o->fdtype : FDB_FORWARD;
+  P->no_drift = o ? o->no_drift : 0;
+  P->use_graph = o && o->use_graph != 0;
+  P->shared_J = o && o->shared_j != 0;
+  read_tunables(P.get());
+  P->world = (o && o->world > 1) ? o->world : 1;
+  P->rank = (o && o->world > 1) ? o->rank : 0;
+  if (P->rank < 0 || P->rank >= P->world) return fail(FDB_ERR_INVALID, "rank %d outside world %d", P->rank, P->world);
+  cudaDeviceProp prop;
+  cudaError_t e = cudaGetDeviceProperties(&prop, dev);
+  if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
+  P->sm_count = prop.multiProcessorCount;
+  // FDB_SM_COUNT=k (tests): size every grid as if the device had k SMs, so small problems already give each block several
+  // tiles.  Launch geometry only: no plan decision reads sm_count.
+  if (const char *v = getenv("FDB_SM_COUNT")) {
+    const int k = atoi(v);
+    if (k >= 1 && k < P->sm_count) P->sm_count = k;
+  }
+  P->l2_bytes = prop.l2CacheSize;
+  return FDB_OK;
+}
+
+// the end of a creator that launched plan-build kernels: wait for them, then hand the plan to the caller
+static fdb_status finish_plan(PlanPtr &P, fdb_plan **plan) {
+  const cudaError_t e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "plan build: %s", cudaGetErrorString(e));
+  *plan = P.release();
+  return FDB_OK;
+}
 
 // relstep / absstep keywords of jacobians.jl:508-510: `relstep = default_relstep(fdtype, eltype(x)), absstep = relstep`.
 // FDB_STEP_DEFAULT (NaN) means "keyword not given"; every other value — 0 and negatives included — is used as passed
@@ -802,115 +833,104 @@ double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep,
 fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval,
                                int jkind, const int64_t *j_colptr, const int64_t *j_rowval, int64_t ldJ,
                                const int64_t *colorvec, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, m, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (!colptr) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "colptr is NULL"); }
-  if (jkind != FDB_J_CSC_NZVAL && jkind != FDB_J_DENSE) {
-    free_plan(P); *plan = nullptr;
+  if (!colptr) return fail(FDB_ERR_INVALID, "colptr is NULL");
+  if (jkind != FDB_J_CSC_NZVAL && jkind != FDB_J_DENSE)
     return fail(FDB_ERR_INVALID, "CSC sparsity supports J kinds CSC_NZVAL and DENSE");
-  }
   P->sp_kind = SP_CSC;
   P->jkind = jkind;
   // nnz = colptr[n]-1 : read the last element wherever it lives
-  I64View cp, rv, cv, jcp, jrv;
-  PLAN_TRY(view_i64(colptr, n + 1, cp));
+  I64View cp, rv, jcp, jrv;
+  TRY(view_i64(colptr, n + 1, cp));
   int64_t last = 1;
-  {
-    cudaError_t e = cudaMemcpy(&last, cp.d + n, 8, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "reading colptr[n]: %s", cudaGetErrorString(e)); }
-  }
+  TRY(read_back(&last, cp.d + n, 1, "reading colptr[n]"));
   const int64_t nnz = last - 1;
-  if (nnz < 0 || nnz > 0x7FFFFFF0LL) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported (must be in [0, 2^31))", (long long)nnz); }
-  if (nnz > 0 && !rowval) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "rowval is NULL"); }
+  if (nnz < 0 || nnz > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported (must be in [0, 2^31))", (long long)nnz);
+  if (nnz > 0 && !rowval) return fail(FDB_ERR_INVALID, "rowval is NULL");
   P->E = nnz;
-  PLAN_TRY(view_i64(rowval, nnz, rv));
-  PLAN_TRY(setup_colors(P, colorvec, cv));
+  TRY(view_i64(rowval, nnz, rv));
+  TRY(setup_colors(P, colorvec));
 
-  uint32_t *d_err = nullptr;
-  unsigned long long *d_cnt = nullptr;
-  PLAN_TRY(P->alloc_t(&d_err, 1));
-  PLAN_TRY(P->alloc_t(&d_cnt, std::max<int32_t>(P->C, 1)));
-  cudaMemset(d_err, 0, 4);
-  cudaMemset(d_cnt, 0, (size_t)std::max<int32_t>(P->C, 1) * 8);
-  PLAN_TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
-  PLAN_TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
+  DevBuf<uint32_t> d_err;
+  DevBuf<unsigned long long> d_cnt;
+  TRY(d_err.alloc(1));
+  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
+  CU(cudaMemset(d_err.get(), 0, 4));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
+  TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
+  TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
 
   bool same_pattern = true;
   bool other_csc = false;
   if (jkind == FDB_J_CSC_NZVAL && j_colptr && j_rowval && (j_colptr != colptr || j_rowval != rowval)) {
     // ext/FiniteDiffSparseArraysExt.jl:51-52
-    PLAN_TRY(view_i64(j_colptr, n + 1, jcp));
+    TRY(view_i64(j_colptr, n + 1, jcp));
     int64_t jlast = 1;
-    {
-      cudaError_t e = cudaMemcpy(&jlast, jcp.d + n, 8, cudaMemcpyDeviceToHost);
-      if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "reading J.colptr[n]: %s", cudaGetErrorString(e)); }
-    }
-    if (jlast < 1 || jlast - 1 > 0x7FFFFFF0LL) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "J.colptr[n+1]=%lld is not a valid CSC end pointer", (long long)jlast); }
+    TRY(read_back(&jlast, jcp.d + n, 1, "reading J.colptr[n]"));
+    if (jlast < 1 || jlast - 1 > 0x7FFFFFF0LL) return fail(FDB_ERR_INVALID, "J.colptr[n+1]=%lld is not a valid CSC end pointer", (long long)jlast);
     const int64_t jnnz = jlast - 1;
-    PLAN_TRY(view_i64(j_rowval, jnnz, jrv));
+    TRY(view_i64(j_rowval, jnnz, jrv));
     if (jnnz != nnz) same_pattern = false;
     else {
-      compare_i64<<<P->grid(n + 1), kThreads>>>(cp.d, jcp.d, n + 1, d_err);
-      if (nnz > 0) compare_i64<<<P->grid(nnz), kThreads>>>(rv.d, jrv.d, nnz, d_err);
+      compare_i64<<<P->grid(n + 1), kThreads>>>(cp.d, jcp.d, n + 1, d_err.get());
+      if (nnz > 0) compare_i64<<<P->grid(nnz), kThreads>>>(rv.d, jrv.d, nnz, d_err.get());
       uint32_t h = 0;
-      cudaMemcpy(&h, d_err, 4, cudaMemcpyDeviceToHost);
+      TRY(read_back(&h, d_err.get(), 1, "comparing J's pattern"));
       same_pattern = !(h & kErrPatternDiff);
-      cudaMemset(d_err, 0, 4);
+      CU(cudaMemset(d_err.get(), 0, 4));
     }
     other_csc = !same_pattern;
     P->j_len = jnnz;
   } else if (jkind == FDB_J_CSC_NZVAL) {
     P->j_len = nnz;
   } else {
-    if (ldJ < m) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "ldJ=%lld < m=%lld", (long long)ldJ, (long long)m); }
+    if (ldJ < m) return fail(FDB_ERR_INVALID, "ldJ=%lld < m=%lld", (long long)ldJ, (long long)m);
     P->ldJ = ldJ;
     P->j_len = ldJ * n;
   }
   const bool need_dest = jkind == FDB_J_DENSE || other_csc;
-  int32_t *col32 = nullptr;
+  DevBuf<int32_t> col32;
   if (need_dest) {
-    PLAN_TRY(P->alloc_t(&col32, std::max<int64_t>(nnz, 1)));
-    PLAN_TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
+    TRY(col32.alloc(std::max<int64_t>(nnz, 1)));
+    TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
   }
-  validate_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, nnz, d_err);
-  PLAN_TRY(read_plan_err(d_err, "CSC sparsity"));
+  validate_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, nnz, d_err.get());
+  TRY(read_plan_err(d_err.get(), "CSC sparsity"));
   if (other_csc) {   // J's own column pointer is searched by dest_other_csc: it must be a valid one too
-    validate_colptr<<<P->grid(n + 1), kThreads>>>(jcp.d, n, P->j_len, d_err);
-    PLAN_TRY(read_plan_err(d_err, "J's CSC pattern"));
+    validate_colptr<<<P->grid(n + 1), kThreads>>>(jcp.d, n, P->j_len, d_err.get());
+    TRY(read_plan_err(d_err.get(), "J's CSC pattern"));
   }
   if (nnz > 0) {
-    PLAN_TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
       const size_t hsm = P->C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->C, 1) * sizeof(unsigned int) : 0;
       expand_csc<CT><<<P->grid(nnz), kThreads, hsm>>>(cp.d, rv.d, m, n, nnz, (const CT *)P->jcolor, P->C, P->row32,
-                                                 (CT *)P->ecolor, col32, d_cnt, d_err);
+                                                 (CT *)P->ecolor, col32.get(), d_cnt.get(), d_err.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
-    if (jkind == FDB_J_DENSE) dest_dense_from_rc<<<P->grid(nnz), kThreads>>>(P->row32, col32, nnz, ldJ, P->dest);
-    else if (other_csc) dest_other_csc<<<P->grid(nnz), kThreads>>>(P->row32, col32, nnz, jcp.d, jrv.d, P->dest, d_err);
+    if (jkind == FDB_J_DENSE) dest_dense_from_rc<<<P->grid(nnz), kThreads>>>(P->row32, col32.get(), nnz, ldJ, P->dest);
+    else if (other_csc) dest_other_csc<<<P->grid(nnz), kThreads>>>(P->row32, col32.get(), nnz, jcp.d, jrv.d, P->dest, d_err.get());
   }
-  PLAN_TRY(read_plan_err(d_err, "CSC sparsity"));
+  TRY(read_plan_err(d_err.get(), "CSC sparsity"));
   std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) {
-    cudaError_t e = cudaMemcpy(cnt.data(), d_cnt, (size_t)P->C * 8, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "colour counts: %s", cudaGetErrorString(e)); }
-  }
+  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
   // ---- per-colour column lists + gather-locality metric -> scatter strategy
   {
     const int32_t C = P->C;
-    unsigned long long *d_jump = nullptr;
-    PLAN_TRY(P->alloc_t(&d_jump, 1));
-    cudaMemset(d_jump, 0, 8);
-    PLAN_TRY(P->alloc_t(&P->colptr32, (size_t)n + 1));
+    DevBuf<unsigned long long> d_jump;
+    TRY(d_jump.alloc(1));
+    CU(cudaMemset(d_jump.get(), 0, 8));
+    TRY(P->alloc_t(&P->colptr32, (size_t)n + 1));
     convert_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, P->colptr32);
-    PLAN_TRY(build_color_lists(P));
+    TRY(build_color_lists(P));
     if (nnz > 1) {
-      row_jump_sum<<<P->grid(nnz), kThreads>>>(P->row32, nnz, d_jump);
+      row_jump_sum<<<P->grid(nnz), kThreads>>>(P->row32, nnz, d_jump.get());
       unsigned long long js = 0;
-      cudaMemcpy(&js, d_jump, 8, cudaMemcpyDeviceToHost);
+      TRY(read_back(&js, d_jump.get(), 1, "row jump sum"));
       P->mean_row_jump = (double)js / (double)(nnz - 1);
     }
     int lanes = 1;
@@ -937,118 +957,109 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
     P->strategy = per_color ? 1 : 0;
     P->strategy_auto = want == 0;
   }
-  PLAN_TRY(finish_colored_plan(P, opts, cnt));
-  if (P->strategy == 1) PLAN_TRY(build_cm_lists(P, cnt));
-  PLAN_TRY(try_stage_plan(P));
+  TRY(finish_colored_plan(P, opts, cnt));
+  if (P->strategy == 1) TRY(build_cm_lists(P, cnt));
+  TRY(try_stage_plan(P));
   // SURVEY.md §8(d): B_alg = 32*nnz + 16*n + 8 (valid colouring; Int64 indices as at the ABI)
   P->alg_bytes = 32 * nnz + 16 * n + 8;
-  {
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "plan build: %s", cudaGetErrorString(e)); }
-  }
-  return FDB_OK;
+  return finish_plan(owner, plan);
 }
 
 fdb_status fdb_plan_create_coo(fdb_plan **plan, int64_t m, int64_t n, int64_t nnz, const int64_t *rows_index,
                                const int64_t *cols_index, int jkind, const int64_t *slots, int64_t ldJ_or_jlen,
                                const int64_t *colorvec, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, m, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (nnz < 0 || nnz > 0x7FFFFFF0LL) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported", (long long)nnz); }
-  if (nnz > 0 && (!rows_index || !cols_index)) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "rows_index/cols_index NULL"); }
-  if (jkind != FDB_J_DENSE && jkind != FDB_J_SLOTS) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "COO sparsity supports J kinds DENSE and SLOTS"); }
-  if (jkind == FDB_J_SLOTS && nnz > 0 && !slots) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "slots is NULL"); }
-  if (jkind == FDB_J_DENSE && ldJ_or_jlen < m) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "ldJ < m"); }
+  if (nnz < 0 || nnz > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported", (long long)nnz);
+  if (nnz > 0 && (!rows_index || !cols_index)) return fail(FDB_ERR_INVALID, "rows_index/cols_index NULL");
+  if (jkind != FDB_J_DENSE && jkind != FDB_J_SLOTS) return fail(FDB_ERR_INVALID, "COO sparsity supports J kinds DENSE and SLOTS");
+  if (jkind == FDB_J_SLOTS && nnz > 0 && !slots) return fail(FDB_ERR_INVALID, "slots is NULL");
+  if (jkind == FDB_J_DENSE && ldJ_or_jlen < m) return fail(FDB_ERR_INVALID, "ldJ < m");
   P->sp_kind = SP_COO;
   P->jkind = jkind;
   P->E = nnz;
   if (jkind == FDB_J_DENSE) { P->ldJ = ldJ_or_jlen; P->j_len = ldJ_or_jlen * n; }
   else P->j_len = ldJ_or_jlen;
-  I64View rv, cvw, sv, cv;
-  PLAN_TRY(view_i64(rows_index, nnz, rv));
-  PLAN_TRY(view_i64(cols_index, nnz, cvw));
-  if (jkind == FDB_J_SLOTS) PLAN_TRY(view_i64(slots, nnz, sv));
-  PLAN_TRY(setup_colors(P, colorvec, cv));
-  uint32_t *d_err = nullptr;
-  unsigned long long *d_cnt = nullptr;
-  PLAN_TRY(P->alloc_t(&d_err, 1));
-  PLAN_TRY(P->alloc_t(&d_cnt, std::max<int32_t>(P->C, 1)));
-  cudaMemset(d_err, 0, 4);
-  cudaMemset(d_cnt, 0, (size_t)std::max<int32_t>(P->C, 1) * 8);
-  PLAN_TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
-  PLAN_TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
-  PLAN_TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
+  I64View rv, cvw, sv;
+  TRY(view_i64(rows_index, nnz, rv));
+  TRY(view_i64(cols_index, nnz, cvw));
+  if (jkind == FDB_J_SLOTS) TRY(view_i64(slots, nnz, sv));
+  TRY(setup_colors(P, colorvec));
+  DevBuf<uint32_t> d_err;
+  DevBuf<unsigned long long> d_cnt;
+  TRY(d_err.alloc(1));
+  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
+  CU(cudaMemset(d_err.get(), 0, 4));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
+  TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
+  TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
+  TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
   if (nnz > 0) {
-    PLAN_TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
       const size_t hsm = P->C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->C, 1) * sizeof(unsigned int) : 0;
       prepare_coo<CT><<<P->grid(nnz), kThreads, hsm>>>(rv.d, cvw.d, jkind == FDB_J_SLOTS ? sv.d : nullptr, nnz, m, n, P->ldJ,
                                                   P->j_len, (const CT *)P->jcolor, P->C, P->row32, (CT *)P->ecolor,
-                                                  P->dest, d_cnt, d_err);
+                                                  P->dest, d_cnt.get(), d_err.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
   }
-  PLAN_TRY(read_plan_err(d_err, "COO sparsity"));
+  TRY(read_plan_err(d_err.get(), "COO sparsity"));
   std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) cudaMemcpy(cnt.data(), d_cnt, (size_t)P->C * 8, cudaMemcpyDeviceToHost);
-  PLAN_TRY(finish_colored_plan(P, opts, cnt));
+  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
+  TRY(finish_colored_plan(P, opts, cnt));
   P->alg_bytes = 32 * nnz + 16 * n + 8;
-  cudaError_t e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "plan build: %s", cudaGetErrorString(e)); }
-  return FDB_OK;
+  return finish_plan(owner, plan);
 }
 
 fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, int jkind, int64_t ldJ,
                                   const int64_t *colorvec, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, m, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (jkind != FDB_J_BAND && jkind != FDB_J_DENSE) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "banded sparsity supports J kinds BAND and DENSE"); }
-  if (l + u + 1 < 1 || l < -n || u < -m) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "invalid bandwidths l=%lld u=%lld", (long long)l, (long long)u); }
-  if (jkind == FDB_J_DENSE && ldJ < m) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "ldJ < m"); }
+  if (jkind != FDB_J_BAND && jkind != FDB_J_DENSE) return fail(FDB_ERR_INVALID, "banded sparsity supports J kinds BAND and DENSE");
+  if (l + u + 1 < 1 || l < -n || u < -m) return fail(FDB_ERR_INVALID, "invalid bandwidths l=%lld u=%lld", (long long)l, (long long)u);
+  if (jkind == FDB_J_DENSE && ldJ < m) return fail(FDB_ERR_INVALID, "ldJ < m");
   P->sp_kind = SP_BANDED;
   P->jkind = jkind;
   P->l = l;
   P->u = u;
   P->ldJ = ldJ;
   P->j_len = jkind == FDB_J_BAND ? (l + u + 1) * n : ldJ * n;
-  I64View cv;
-  PLAN_TRY(setup_colors(P, colorvec, cv));
-  unsigned long long *d_cnt = nullptr;
-  PLAN_TRY(P->alloc_t(&d_cnt, std::max<int32_t>(P->C, 1)));
-  cudaMemset(d_cnt, 0, (size_t)std::max<int32_t>(P->C, 1) * 8);
+  TRY(setup_colors(P, colorvec));
+  DevBuf<unsigned long long> d_cnt;
+  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
   if (n > 0 && P->C > 0) {
-    PLAN_TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      count_band_colors<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, m, n, l, u, P->C, d_cnt);
+      count_band_colors<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, m, n, l, u, P->C, d_cnt.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
   }
   std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) cudaMemcpy(cnt.data(), d_cnt, (size_t)P->C * 8, cudaMemcpyDeviceToHost);
+  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
   unsigned long long total = 0;
   for (auto c : cnt) total += c;
   P->E = (int64_t)total;
-  PLAN_TRY(finish_colored_plan(P, opts, cnt));
+  TRY(finish_colored_plan(P, opts, cnt));
   // SURVEY.md §8(d) banded: 8*sum_c band_len(c) written + 16*m*C read
   P->alg_bytes = 8 * (int64_t)total + 16 * m * (int64_t)P->C;
-  cudaError_t e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_CUDA, "plan build: %s", cudaGetErrorString(e)); }
-  return FDB_OK;
+  return finish_plan(owner, plan);
 }
 
 // dense column branch over the leading `ncols` components (ncols == n for the default colorvec = 1:n)
 static fdb_status create_dense(fdb_plan **plan, int64_t m, int64_t n, int64_t ldJ, int64_t ncols, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, m, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (ldJ < m) { free_plan(P); *plan = nullptr; return fail(FDB_ERR_INVALID, "ldJ < m"); }
+  if (ldJ < m) return fail(FDB_ERR_INVALID, "ldJ < m");
   P->sp_kind = SP_NONE;
   P->jkind = FDB_J_DENSE;
   P->ldJ = ldJ;
@@ -1073,13 +1084,14 @@ static fdb_status create_dense(fdb_plan **plan, int64_t m, int64_t n, int64_t ld
   P->batch = batch;
   P->slabs = batch;
   P->n_groups = ncl == 0 ? 0 : (ncl + batch - 1) / batch;
-  PLAN_TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
-  PLAN_TRY(P->alloc_t(&P->Fp, (size_t)batch * P->ldF * cw));
-  if (central) PLAN_TRY(P->alloc_t(&P->Fm, (size_t)batch * P->ldF));
-  PLAN_TRY(P->alloc_t(&P->xp, (size_t)batch * P->ldx * cw));
-  PLAN_TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(ncl, 1)));
+  TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
+  TRY(P->alloc_t(&P->Fp, (size_t)batch * P->ldF * cw));
+  if (central) TRY(P->alloc_t(&P->Fm, (size_t)batch * P->ldF));
+  TRY(P->alloc_t(&P->xp, (size_t)batch * P->ldx * cw));
+  TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(ncl, 1)));
   // SURVEY.md §8(d) dense: 24*m per column
   P->alg_bytes = 24 * m * ncl;
+  *plan = owner.release();
   return FDB_OK;
 }
 
@@ -1100,21 +1112,11 @@ fdb_status fdb_plan_create_dense_colorvec(fdb_plan **plan, int64_t m, int64_t n,
   int dev = 0;
   TRY(check_device(opts, &dev));
   DeviceGuard g(dev);
-  long long mx = 0;
+  long long mx = 0, mn = 0;
   if (n > 0) {
     I64View cv;
     TRY(view_i64(colorvec, n, cv));
-    long long *d_mm = nullptr;
-    CU(cudaMalloc((void **)&d_mm, 2 * sizeof(long long)));
-    const long long init[2] = {LLONG_MIN, LLONG_MAX};
-    cudaMemcpy(d_mm, init, sizeof init, cudaMemcpyHostToDevice);
-    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, 132 * 8));
-    color_minmax<<<blocks, kThreads>>>(cv.d, n, d_mm, d_mm + 1);
-    long long out[2] = {0, 0};
-    const cudaError_t e = cudaMemcpy(out, d_mm, sizeof out, cudaMemcpyDeviceToHost);
-    cudaFree(d_mm);
-    if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "colour maximum failed: %s", cudaGetErrorString(e));
-    mx = out[0];
+    TRY(color_range(cv.d, n, &mx, &mn));
   }
   if (mx > n) return fail(FDB_ERR_INVALID, "sparsity=nothing: maximum(colorvec)=%lld indexes x beyond length(x)=%lld "
                                            "(BoundsError in the reference, jacobians.jl:549)", mx, (long long)n);
@@ -1811,17 +1813,17 @@ fdb_status fdb_jacobian_complex(fdb_plan *P, fdb_fn_c f, void *ctx, const double
 // (column-block sharded runs: every shard perturbs with the step sizes of the FULL x — jacobians.jl:559-561 takes the
 //  norm over all colour-k components)
 fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorvec, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, 0, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, 0, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
   P->sp_kind = SP_EPS;
-  I64View cv;
-  PLAN_TRY(setup_colors(P, colorvec, cv));
-  PLAN_TRY(alloc_eps_buffers(P));
+  TRY(setup_colors(P, colorvec));
+  TRY(alloc_eps_buffers(P));
   // the same list-based eps pass as the Jacobian plans: a column block's external step sizes are then bit-identical to
   // the ones the unsharded plan computes for itself
-  if (P->C > kEpsRegColors && n > 0) PLAN_TRY(build_color_lists(P));
+  if (P->C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
+  *plan = owner.release();
   return FDB_OK;
 }
 
@@ -1852,28 +1854,27 @@ fdb_status fdb_plan_set_external_eps(fdb_plan *P, const double *d_eps) {
 
 // ------------------------------------------------------------------------------------------------ JVP (src/jvp.jl:238-274)
 fdb_status fdb_jvp_plan_create(fdb_plan **plan, int64_t m, int64_t n, const fdb_plan_opts *opts) {
-  fdb_plan *P = nullptr;
-  TRY(new_plan(plan, opts, m, n));
-  P = *plan;
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (P->fdtype == FDB_COMPLEX) {
-    free_plan(P); *plan = nullptr;
+  if (P->fdtype == FDB_COMPLEX)
     return fail(FDB_ERR_UNSUPPORTED, "finite_difference_jvp doesn't support :complex-mode finite diff");   // jvp.jl:248-250
-  }
   P->sp_kind = SP_JVP;
   P->C = 1;
   P->ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
   P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
   int64_t nb = std::max<int64_t>(1, std::min<int64_t>((n + kTile - 1) / kTile, (int64_t)P->sm_count * 8));
   P->eps_blocks = (int)nb;
-  PLAN_TRY(P->alloc_t(&P->partial, (size_t)nb));
-  PLAN_TRY(P->alloc_t(&P->ticket, 4));
-  cudaMemset(P->ticket, 0, 16);
-  PLAN_TRY(P->alloc_t(&P->eps, 2));
-  PLAN_TRY(P->alloc_t(&P->sumsq, 2));
-  PLAN_TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
-  PLAN_TRY(P->alloc_t(&P->xp, (size_t)P->ldx));
+  TRY(P->alloc_t(&P->partial, (size_t)nb));
+  TRY(P->alloc_t(&P->ticket, 4));
+  CU(cudaMemset(P->ticket, 0, 16));
+  TRY(P->alloc_t(&P->eps, 2));
+  TRY(P->alloc_t(&P->sumsq, 2));
+  TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
+  TRY(P->alloc_t(&P->xp, (size_t)P->ldx));
   P->alg_bytes = 24 * n + 24 * m;   // dot: 16n; point: 16n read + 8n write; quotient: 16m read + 8m write
+  *plan = owner.release();
   return FDB_OK;
 }
 

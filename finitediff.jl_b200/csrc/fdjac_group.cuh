@@ -92,7 +92,7 @@ static fdb_status group_create(fdb_group **out, int n_devices, const int *device
   }
   for (int i = 0; i < n_devices; ++i)
     if (devices[i] < 0 || devices[i] >= count) return fail(FDB_ERR_INVALID, "device %d out of range (%d devices)", devices[i], count);
-  fdb_group *g = new (std::nothrow) fdb_group();
+  std::unique_ptr<fdb_group, void (*)(fdb_group *)> g(new (std::nothrow) fdb_group(), free_group);
   if (!g) return fail(FDB_ERR_NOMEM, "out of host memory");
   g->n = n_devices;
   g->devices.assign(devices, devices + n_devices);
@@ -115,31 +115,28 @@ static fdb_status group_create(fdb_group **out, int n_devices, const int *device
       DeviceGuard dgp(devices[i]);
       int can = 0;
       cudaDeviceCanAccessPeer(&can, devices[i], root);
-      if (!can) { free_group(g); return fail(FDB_ERR_UNSUPPORTED, "device %d cannot access device %d (no peer path)", devices[i], root); }
+      if (!can) return fail(FDB_ERR_UNSUPPORTED, "device %d cannot access device %d (no peer path)", devices[i], root);
       const cudaError_t e = cudaDeviceEnablePeerAccess(root, 0);
-      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) {
-        free_group(g);
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled)
         return fail(FDB_ERR_CUDA, "cudaDeviceEnablePeerAccess(%d -> %d): %s", devices[i], root, cudaGetErrorString(e));
-      }
       cudaGetLastError();
     }
-    fdb_status st = make(i, &o, &g->plans[i]);
-    if (st != FDB_OK) { free_group(g); return st; }
+    TRY(make(i, &o, &g->plans[i]));
     if (i == 0) continue;
     DeviceGuard dg(devices[i]);
     cudaError_t e = cudaStreamCreateWithFlags(&g->streams[i], cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_done[i], cudaEventDisableTiming);
-    if (e != cudaSuccess) { free_group(g); return fail(FDB_ERR_CUDA, "group stream/event: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "group stream/event: %s", cudaGetErrorString(e));
   }
   {
     DeviceGuard dg(root);
     const cudaError_t e = cudaEventCreateWithFlags(&g->ev_start, cudaEventDisableTiming);
-    if (e != cudaSuccess) { free_group(g); return fail(FDB_ERR_CUDA, "group event: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "group event: %s", cudaGetErrorString(e));
   }
   g->nx = g->plans[0]->n;
   g->m = g->plans[0]->m;
   g->kind = g->plans[0]->sp_kind;
-  *out = g;
+  *out = g.release();
   return FDB_OK;
 }
 
@@ -242,18 +239,15 @@ fdb_status fdb_sync_create(fdb_sync **out, int rank, int world, int device) {
   int dev = 0;
   TRY(check_device(&o, &dev));
   DeviceGuard dg(dev);
-  fdb_sync *s = new (std::nothrow) fdb_sync();
+  std::unique_ptr<fdb_sync, fdb_status (*)(fdb_sync *)> s(new (std::nothrow) fdb_sync(), fdb_sync_destroy);
   if (!s) return fail(FDB_ERR_NOMEM, "out of host memory");
   s->rank = rank; s->world = world; s->device = dev;
   cudaError_t e = cudaMalloc((void **)&s->flags, ((size_t)world + 1) * 8);
   if (e == cudaSuccess) e = cudaMemset(s->flags, 0, ((size_t)world + 1) * 8);
   if (e == cudaSuccess) e = cudaMalloc((void **)&s->d_peer_flags, (size_t)world * sizeof(void *));
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    cudaFree(s->flags); cudaFree(s->d_peer_flags); delete s;
-    return fail(FDB_ERR_CUDA, "fdb_sync_create: %s", cudaGetErrorString(e));
-  }
-  *out = s;
+  if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "fdb_sync_create: %s", cudaGetErrorString(e));
+  *out = s.release();
   return FDB_OK;
 }
 
@@ -300,10 +294,9 @@ fdb_status fdb_sync_destroy(fdb_sync *s) {
 // ------------------------------------------------------------------------------------------------ on-device colouring
 // ArrayInterface.matrix_colors analogues (kernels_color.cuh).  Plan-time operations: they synchronise.
 struct CsrPattern {
-  int32_t *rowptr = nullptr, *rcols = nullptr;
+  DevBuf<int32_t> rowptr, rcols;
   I64View cp, rv;
   int64_t nnz = 0;
-  ~CsrPattern() { cudaFree(rowptr); cudaFree(rcols); }
 };
 
 static fdb_status build_csr_pattern(int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval, CsrPattern &P) {
@@ -311,39 +304,32 @@ static fdb_status build_csr_pattern(int64_t m, int64_t n, const int64_t *colptr,
   if (!colptr) return fail(FDB_ERR_INVALID, "colptr is NULL");
   TRY(view_i64(colptr, n + 1, P.cp));
   int64_t last = 1;
-  CU(cudaMemcpy(&last, P.cp.d + n, 8, cudaMemcpyDeviceToHost));
+  TRY(read_back(&last, P.cp.d + n, 1, "reading colptr[n]"));
   P.nnz = last - 1;
   if (P.nnz < 0 || P.nnz > 0x7FFFFFF0LL) return fail(FDB_ERR_INVALID, "nnz=%lld unsupported", (long long)P.nnz);
   if (P.nnz > 0 && !rowval) return fail(FDB_ERR_INVALID, "rowval is NULL");
   TRY(view_i64(rowval, P.nnz, P.rv));
-  uint32_t *d_err = nullptr;
-  int32_t *cnt = nullptr, *cursor = nullptr;
-  void *d_tmp = nullptr;
-  size_t tmp_bytes = 0;
-  auto cleanup = [&]() { cudaFree(d_err); cudaFree(cnt); cudaFree(cursor); cudaFree(d_tmp); };
-#define CSR_CU(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { cleanup(); \
-    return fail(FDB_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); } } while (0)
-  CSR_CU(cudaMalloc((void **)&d_err, 4));
-  CSR_CU(cudaMemset(d_err, 0, 4));
-  CSR_CU(cudaMalloc((void **)&cnt, ((size_t)m + 1) * 4));
-  CSR_CU(cudaMemset(cnt, 0, ((size_t)m + 1) * 4));
-  CSR_CU(cudaMalloc((void **)&cursor, ((size_t)m + 1) * 4));
-  CSR_CU(cudaMemset(cursor, 0, ((size_t)m + 1) * 4));
-  CSR_CU(cudaMalloc((void **)&P.rowptr, ((size_t)m + 1) * 4));
-  CSR_CU(cudaMalloc((void **)&P.rcols, (size_t)std::max<int64_t>(P.nnz, 1) * 4));
+  DevBuf<uint32_t> d_err;
+  DevBuf<int32_t> cnt, cursor;
+  TRY(d_err.alloc(1));
+  CU(cudaMemset(d_err.get(), 0, 4));
+  TRY(cnt.alloc((size_t)m + 1));
+  CU(cudaMemset(cnt.get(), 0, ((size_t)m + 1) * 4));
+  TRY(cursor.alloc((size_t)m + 1));
+  CU(cudaMemset(cursor.get(), 0, ((size_t)m + 1) * 4));
+  TRY(P.rowptr.alloc((size_t)m + 1));
+  TRY(P.rcols.alloc((size_t)std::max<int64_t>(P.nnz, 1)));
   const int gb = (int)std::max<int64_t>(1, std::min<int64_t>((std::max<int64_t>(P.nnz, n + 1) + kThreads - 1) / kThreads, 132 * 16));
-  validate_colptr<<<gb, kThreads>>>(P.cp.d, n, P.nnz, d_err);
-  if (P.nnz > 0) csr_count_rows<<<gb, kThreads>>>(P.rv.d, P.nnz, m, cnt, d_err);
+  validate_colptr<<<gb, kThreads>>>(P.cp.d, n, P.nnz, d_err.get());
+  if (P.nnz > 0) csr_count_rows<<<gb, kThreads>>>(P.rv.d, P.nnz, m, cnt.get(), d_err.get());
   uint32_t herr = 0;
-  CSR_CU(cudaMemcpy(&herr, d_err, 4, cudaMemcpyDeviceToHost));
-  if (herr) { cleanup(); return fail(FDB_ERR_INVALID, "invalid CSC pattern (%s)", (herr & 1u) ? "colptr" : "row index outside 1..m"); }
-  CSR_CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cnt, P.rowptr, (int)(m + 1)));
-  CSR_CU(cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16));
-  CSR_CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, cnt, P.rowptr, (int)(m + 1)));
-  if (n > 0 && P.nnz > 0) csr_fill<<<gb, kThreads>>>(P.cp.d, P.rv.d, n, m, P.rowptr, cursor, P.rcols);
-  CSR_CU(cudaDeviceSynchronize());
-#undef CSR_CU
-  cleanup();
+  TRY(read_back(&herr, d_err.get(), 1, "CSC pattern check"));
+  if (herr) return fail(FDB_ERR_INVALID, "invalid CSC pattern (%s)", (herr & 1u) ? "colptr" : "row index outside 1..m");
+  TRY(cub_run([&](void *tmp, size_t &bytes) {
+    return cub::DeviceScan::ExclusiveSum(tmp, bytes, cnt.get(), P.rowptr.get(), (int)(m + 1));
+  }));
+  if (n > 0 && P.nnz > 0) csr_fill<<<gb, kThreads>>>(P.cp.d, P.rv.d, n, m, P.rowptr.get(), cursor.get(), P.rcols.get());
+  CU(cudaDeviceSynchronize());
   return FDB_OK;
 }
 
@@ -369,33 +355,29 @@ fdb_status fdb_matrix_colors_csc(int64_t m, int64_t n, const int64_t *colptr, co
   if (n == 0) return FDB_OK;
   CsrPattern P;
   TRY(build_csr_pattern(m, n, colptr, rowval, P));
-  int32_t *col_a = nullptr, *col_b = nullptr;
-  unsigned long long *d_pending = nullptr;
-  int *d_max = nullptr;
-  auto cleanup = [&]() { cudaFree(col_a); cudaFree(col_b); cudaFree(d_pending); cudaFree(d_max); };
-#define COL_CU(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) { cleanup(); \
-    return fail(FDB_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); } } while (0)
-  COL_CU(cudaMalloc((void **)&col_a, (size_t)n * 4));
-  COL_CU(cudaMalloc((void **)&col_b, (size_t)n * 4));
-  COL_CU(cudaMalloc((void **)&d_pending, 8));
-  COL_CU(cudaMalloc((void **)&d_max, 4));
-  COL_CU(cudaMemset(col_a, 0, (size_t)n * 4));
-  COL_CU(cudaMemset(d_max, 0, 4));
+  DevBuf<int32_t> buf_a, buf_b;
+  DevBuf<unsigned long long> d_pending;
+  DevBuf<int> d_max;
+  TRY(buf_a.alloc((size_t)n));
+  TRY(buf_b.alloc((size_t)n));
+  TRY(d_pending.alloc(1));
+  TRY(d_max.alloc(1));
+  CU(cudaMemset(buf_a.get(), 0, (size_t)n * 4));
+  CU(cudaMemset(d_max.get(), 0, 4));
+  int32_t *col_a = buf_a.get(), *col_b = buf_b.get();
   const int gb = (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, 132 * 16));
   int64_t rounds = 0;
   unsigned long long pending = (unsigned long long)n;
   while (pending > 0) {
-    COL_CU(cudaMemset(d_pending, 0, 8));
-    jp_color_round<<<gb, kThreads>>>(P.cp.d, P.rv.d, P.rowptr, P.rcols, n, m, col_a, col_b, d_pending);
-    COL_CU(cudaMemcpy(&pending, d_pending, 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemset(d_pending.get(), 0, 8));
+    jp_color_round<<<gb, kThreads>>>(P.cp.d, P.rv.d, P.rowptr.get(), P.rcols.get(), n, m, col_a, col_b, d_pending.get());
+    TRY(read_back(&pending, d_pending.get(), 1, "colouring round"));
     std::swap(col_a, col_b);
-    if (++rounds > 100000) { cleanup(); return fail(FDB_ERR_INVALID, "colouring did not converge"); }
+    if (++rounds > 100000) return fail(FDB_ERR_INVALID, "colouring did not converge");
   }
-  colors_to_i64<<<gb, kThreads>>>(col_a, n, d_colorvec, d_max);
+  colors_to_i64<<<gb, kThreads>>>(col_a, n, d_colorvec, d_max.get());
   int mx = 0;
-  COL_CU(cudaMemcpy(&mx, d_max, 4, cudaMemcpyDeviceToHost));
-#undef COL_CU
-  cleanup();
+  TRY(read_back(&mx, d_max.get(), 1, "colour count"));
   if (n_colors) *n_colors = mx;
   if (n_rounds) *n_rounds = rounds;
   return FDB_OK;
@@ -413,15 +395,13 @@ fdb_status fdb_check_coloring_csc(int64_t m, int64_t n, const int64_t *colptr, c
   TRY(build_csr_pattern(m, n, colptr, rowval, P));
   I64View cv;
   TRY(view_i64(colorvec, n, cv));
-  unsigned long long *d_c = nullptr;
-  CU(cudaMalloc((void **)&d_c, 8));
-  cudaMemset(d_c, 0, 8);
+  DevBuf<unsigned long long> d_c;
+  TRY(d_c.alloc(1));
+  CU(cudaMemset(d_c.get(), 0, 8));
   const int gb = (int)std::max<int64_t>(1, std::min<int64_t>((m + kThreads - 1) / kThreads, 132 * 16));
-  count_color_conflicts<<<gb, kThreads>>>(P.rowptr, P.rcols, m, cv.d, d_c);
+  count_color_conflicts<<<gb, kThreads>>>(P.rowptr.get(), P.rcols.get(), m, cv.d, d_c.get());
   unsigned long long h = 0;
-  const cudaError_t e = cudaMemcpy(&h, d_c, 8, cudaMemcpyDeviceToHost);
-  cudaFree(d_c);
-  if (e != cudaSuccess) return fail(FDB_ERR_CUDA, "conflict count: %s", cudaGetErrorString(e));
+  TRY(read_back(&h, d_c.get(), 1, "conflict count"));
   *n_conflicts = (int64_t)h;
   return FDB_OK;
 }

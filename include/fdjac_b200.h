@@ -109,7 +109,7 @@ typedef struct {
   int64_t n_groups;        /* scatter launches per Jacobian (1 => fully fused single pass) */
   int64_t slabs;           /* colours whose f! outputs are resident at once */
   int64_t fcalls_per_jacobian; /* f! evaluations (points) per call: 1+C fwd, 2C central (local colours only) */
-  int64_t device_bytes;    /* device memory held by the plan */
+  int64_t device_bytes;    /* device memory held by the plan (build scratch is freed when the plan is created) */
   int32_t fdtype, jkind, sp_kind, color_bits;
   int64_t alg_bytes_scatter; /* SURVEY.md §8(d) algorithmic bytes of the diff+scatter per Jacobian */
   int32_t strategy;        /* chosen scatter strategy: 0 fused single pass, 1 per-colour column lists */
