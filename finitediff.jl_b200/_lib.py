@@ -117,6 +117,7 @@ SYNTH_SYMBOLS = {
     "fdbs_tridiag_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_tridiag_rows": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_store_probe": (_int, [_vp, _i64, _int, _int, _vp]),
+    "fdbs_stream_probe": (_int, [_vp, _i64, _int, _vp, _i64, _int, _i64, _int, _vp, _vp]),
     "fdbs_lap5": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_ellrows": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_ellrows_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),

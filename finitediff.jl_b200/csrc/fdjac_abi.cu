@@ -204,6 +204,7 @@ struct fdb_plan {
   // TMA-staged form of the fused pass (row-local patterns; kernels_staged.cuh)
   uint16_t *row16 = nullptr;
   int32_t *tile_w0 = nullptr;
+  unsigned long long *stage_claim = nullptr;   // walk-position counter of the staged pass (re-armed by every launch)
   int32_t stage_W = 0;
   bool staged = false, stage_packed = false;
   bool stage_band = false;             // exact clipped band: the staged pass derives rows and columns, reads no index stream
@@ -683,10 +684,12 @@ static fdb_status try_stage_plan(fdb_plan *P) {
     }));
     CU(cudaDeviceSynchronize());
   }
-  const size_t smem = (size_t)2 * nwin * W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8;
+  const size_t smem = (size_t)2 * nwin * W * 8 + kStageCtlBytes + (size_t)P->C * 8;
   if (span == 0 || span > 65535 || smem > (size_t)kStageMaxSmem) return FDB_OK;   // not row-local enough: keep the gather form
   P->adopt(P->tile_w0 = tile_w0.release(), tile_w0.bytes);
   P->adopt(P->row16 = row16.release(), row16.bytes);
+  TRY(P->alloc_t(&P->stage_claim, 1));
+  CU(cudaMemset(P->stage_claim, 0, sizeof(unsigned long long)));
   P->stage_W = (int32_t)W;
   P->staged = true;
   if (!P->tune.no_band) TRY(try_band_form(P));
@@ -1309,6 +1312,24 @@ static int resident_grid(const fdb_plan *P, K kernel, size_t dyn_smem, int64_t w
   return (int)g;
 }
 
+// Programmatic dependent launch: the kernel may be scheduled while the kernel before it on the stream drains, and runs
+// its set-up (shared memory, barriers) meanwhile; it calls cudaGridDependencySynchronize() before it reads anything
+// that kernel wrote.  A capture keeps the programmatic edge in the graph.
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_pdl(void (*kern)(KArgs...), int grid, size_t smem, cudaStream_t s, Args... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = s;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kern, args...);
+}
+
 template <typename CT>
 static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double absstep, double dir, cudaStream_t s) {
   const int32_t C = P->C;
@@ -1376,10 +1397,49 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   //  here would race with the peers' stores.
   const bool self_defining = (ident || band_data) && n_local > 0;
   if (!self_defining && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
+  // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
+  auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
+      for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
+        PerturbArgs pa{};
+        pa.x = x; pa.eps = P->eps;
+        pa.xp = P->xp + q0 * sX; pa.xm = CENTRAL ? P->xm + q0 * sX : nullptr;
+        pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = P->no_drift ? 0 : 1;
+        pa.reverse = (P->tune.reverse >> 1) & 1;
+        pa.kcount = (int32_t)std::min<int64_t>(kPerturbMaxPoints, kc - q0);
+        for (int32_t q = 0; q < pa.kcount; ++q) pa.k[q] = P->local_colors[(size_t)(li0 + q0 + q)];
+        pa.aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(P->xp) |
+                       reinterpret_cast<uintptr_t>(P->xm)) & 15) == 0 && (P->ldx & 1) == 0;
+        const size_t sm = P->C <= kPerturbSmemColors ? (size_t)P->C * sizeof(double) : 0;
+        const int64_t tiles = (P->n + kTile - 1) / kTile;
+        TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+          using CS = decltype(cs);
+          if (COMPLEX) {
+            if (pa.kcount == 1) perturb_complex<CS, 1><<<P->grid(P->n), kThreads, 0, ps>>>(pa, cs);
+            else perturb_complex<CS, kPerturbMaxPoints><<<P->grid(P->n), kThreads, 0, ps>>>(pa, cs);
+          } else {
+            // store-heavy (NP points written per element read): an oversubscribed grid (16x the resident wave), like the
+            // band and dense-column kernels
+            constexpr int kPerturbGridOver = 16;
+            auto over = [&](int g) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)g * kPerturbGridOver, tiles)); };
+            auto go = [&](auto kern) { return launch_pdl(kern, over(resident_grid(P, kern, sm, tiles)), sm, ps, pa, cs); };
+            if (pa.kcount == 1) CU(go(perturb_colors<CS, CENTRAL, 1>));
+            else CU(go(perturb_colors<CS, CENTRAL, kPerturbMaxPoints>));
+          }
+          return FDB_OK;
+        }));
+        P->cnt.kernel_launches += 1;
+      }
+      return FDB_OK;
+  };
+
   // forward mode without f_in: f(x) (jacobians.jl:541) and the step-size pass are independent — the eps kernels run on the
-  // side stream beside the user's f(x) and are joined before the first perturbation (a parallel branch of the CUDA graph)
+  // side stream beside the user's f(x) (a parallel branch of the CUDA graph)
   bool eps_beside_fx = MODE == kForward && !f_in && !P->ext_eps && P->side && P->ev_fork && P->C > 0;
   if (P->tune.no_eps_overlap) eps_beside_fx = false;
+  // ... and so is the first window of perturbed points, which reads x and the step sizes only: it is built on the side
+  // stream behind the ε pass, and the call's stream waits for both before the first f!(xp).  f! is still called in the
+  // reference's order, f(x) first.
+  const bool perturb_beside_fx = eps_beside_fx && n_local > 0;
   if (P->ext_eps) {
     // sharded runs: the step sizes of the FULL x come from outside (fdb_color_eps on the full vector)
     if (P->C > 0) CU(cudaMemcpyAsync(P->eps, P->ext_eps, (size_t)P->C * 8, cudaMemcpyDeviceToDevice, s));
@@ -1387,6 +1447,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
     CU(cudaEventRecord(P->ev_fork, s));
     CU(cudaStreamWaitEvent(P->side, P->ev_fork, 0));
     TRY(run_eps<CT>(P, x, relstep, absstep, dir, P->side));
+    if (perturb_beside_fx) TRY(perturb_window(0, std::min<int64_t>(P->pbatch, n_local), P->side));
     CU(cudaEventRecord(P->ev_eps, P->side));
   } else {
     TRY(run_eps<CT>(P, x, relstep, absstep, dir, s));
@@ -1407,42 +1468,6 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
       P->cnt.kernel_launches += 1;
     }
   }
-  // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
-  auto perturb_window = [&](int64_t li0, int64_t kc) -> fdb_status {
-      for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
-        PerturbArgs pa{};
-        pa.x = x; pa.eps = P->eps;
-        pa.xp = P->xp + q0 * sX; pa.xm = CENTRAL ? P->xm + q0 * sX : nullptr;
-        pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = P->no_drift ? 0 : 1;
-        pa.reverse = (P->tune.reverse >> 1) & 1;
-        pa.kcount = (int32_t)std::min<int64_t>(kPerturbMaxPoints, kc - q0);
-        for (int32_t q = 0; q < pa.kcount; ++q) pa.k[q] = P->local_colors[(size_t)(li0 + q0 + q)];
-        pa.aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(P->xp) |
-                       reinterpret_cast<uintptr_t>(P->xm)) & 15) == 0 && (P->ldx & 1) == 0;
-        const size_t sm = P->C <= kPerturbSmemColors ? (size_t)P->C * sizeof(double) : 0;
-        const int64_t tiles = (P->n + kTile - 1) / kTile;
-        TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
-          using CS = decltype(cs);
-          if (COMPLEX) {
-            if (pa.kcount == 1) perturb_complex<CS, 1><<<P->grid(P->n), kThreads, 0, s>>>(pa, cs);
-            else perturb_complex<CS, kPerturbMaxPoints><<<P->grid(P->n), kThreads, 0, s>>>(pa, cs);
-          } else {
-            // store-heavy (NP points written per element read): an oversubscribed grid (16x the resident wave), like the
-            // band and dense-column kernels
-            constexpr int kPerturbGridOver = 16;
-            auto over = [&](int g) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)g * kPerturbGridOver, tiles)); };
-            if (pa.kcount == 1)
-              perturb_colors<CS, CENTRAL, 1><<<over(resident_grid(P, perturb_colors<CS, CENTRAL, 1>, sm, tiles)), kThreads, sm, s>>>(pa, cs);
-            else
-              perturb_colors<CS, CENTRAL, kPerturbMaxPoints><<<over(resident_grid(P, perturb_colors<CS, CENTRAL, kPerturbMaxPoints>, sm, tiles)), kThreads, sm, s>>>(pa, cs);
-          }
-          return FDB_OK;
-        }));
-        P->cnt.kernel_launches += 1;
-      }
-      return FDB_OK;
-  };
-
   // per-colour column-list scatter of local colours [l0, l0+G): <= kMaxSegs colours per launch
   // Double-buffered overlap (multi-GPU, column lists): group g's f! outputs live in buffer (g & 1); its scatter — the
   // kernel that also pushes the values to the peers over NVLink — runs on a side stream while the main stream already
@@ -1572,38 +1597,38 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
             StagedArgs sa{};
             sa.row16 = P->row16; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
             sa.fx = vfx; sa.Fp = P->Fp; sa.Fm = P->Fm; sa.eps = P->eps; sa.J = J; sa.C = P->C; sa.W = P->stage_W;
-            sa.ldF = sF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned;
+            sa.ldF = sF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned; sa.claim = P->stage_claim;
             sa.reverse = P->tune.reverse & 1;
             sa.colptr32 = P->colptr32; sa.l = P->band_l; sa.n = (int32_t)P->n;
             sa.col_a = P->band_col_a; sa.col_b = P->band_col_b; sa.e_a = P->band_e_a; sa.e_b = P->band_e_b;
             sa.w = make_fastdiv((uint32_t)P->band_w);
             const int nwin = CENTRAL ? 2 * P->C : P->C + 1;
             int stages = P->tune.stages;
-            if ((size_t)stages * nwin * P->stage_W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8 > (size_t)kStageMaxSmem) stages = 2;
+            if ((size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8 > (size_t)kStageMaxSmem) stages = 2;
             sa.stages = stages;
-            const size_t ssm = (size_t)stages * nwin * P->stage_W * 8 + 2 * kStagesMax * 8 + (size_t)P->C * 8;
+            const size_t ssm = (size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8;
             // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n | 6e): resident blocks per SM x index prefetch / empty mbarrier
             const char v0 = P->tune.staged_variant[0], v1 = P->tune.staged_variant[1];
-            auto go = [&](auto kern, auto cs) {
-              const int grid = resident_grid(P, kern, ssm, tiles);
-              kern<<<grid, kThreads, ssm, s>>>(sa, cs);
+            auto go = [&](auto kern, auto cs) -> fdb_status {
+              CU(launch_pdl(kern, resident_grid(P, kern, ssm, tiles), ssm, s, sa, cs));
+              return FDB_OK;
             };
             if (P->stage_band) {
               TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
                 using CS = decltype(cs);
-                if (v0 == '8') go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs);
-                else if (v1 == 'e') go(diff_scatter_staged<CS, MODE, 6, false, false, true, true>, cs);
-                else go(diff_scatter_staged<CS, MODE, 6, false, false, false, true>, cs);
+                if (v0 == '8') TRY(go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs));
+                else if (v1 == 'e') TRY(go(diff_scatter_staged<CS, MODE, 6, false, false, true, true>, cs));
+                else TRY(go(diff_scatter_staged<CS, MODE, 6, false, false, false, true>, cs));
                 return FDB_OK;
               }));
             } else {
               using CS = TableColors<CT>;          // per-entry colours
               const CS ec{(const CT *)P->ecolor};
-              if (P->stage_packed && v1 == 'e') go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec);
-              else if (P->stage_packed) go(diff_scatter_staged<CS, MODE, 6, false, true>, ec);
-              else if (v0 == '8') go(diff_scatter_staged<CS, MODE, 8, false, false>, ec);
-              else if (v1 == 'n') go(diff_scatter_staged<CS, MODE, 6, false, false>, ec);
-              else go(diff_scatter_staged<CS, MODE, 6, true, false>, ec);
+              if (P->stage_packed && v1 == 'e') TRY(go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec));
+              else if (P->stage_packed) TRY(go(diff_scatter_staged<CS, MODE, 6, false, true>, ec));
+              else if (v0 == '8') TRY(go(diff_scatter_staged<CS, MODE, 8, false, false>, ec));
+              else if (v1 == 'n') TRY(go(diff_scatter_staged<CS, MODE, 6, false, false>, ec));
+              else TRY(go(diff_scatter_staged<CS, MODE, 6, true, false>, ec));
             }
           }
         } else if (full) {
@@ -1629,7 +1654,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   int64_t li = 0;
   while (li < n_local) {
     const int64_t g = li / P->slabs, g0 = g * P->slabs, gend = std::min<int64_t>(g0 + P->slabs, n_local);
-    if (li % P->pbatch == 0) TRY(perturb_window(li, std::min<int64_t>(P->pbatch, n_local - li)));
+    if (li % P->pbatch == 0 && !(li == 0 && perturb_beside_fx)) TRY(perturb_window(li, std::min<int64_t>(P->pbatch, n_local - li), s));
     const int64_t wend = std::min<int64_t>((li / P->pbatch + 1) * P->pbatch, n_local);
     const int64_t fc = std::min<int64_t>(P->batch, std::min<int64_t>(wend - li, gend - li));
     const int64_t gb = overlap ? (g & 1) * P->slabs * sF : 0;           // this group's output buffer

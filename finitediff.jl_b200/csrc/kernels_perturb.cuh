@@ -85,6 +85,7 @@ template <typename CS, bool CENTRAL, int NP>
 __global__ void __launch_bounds__(kThreads)
 perturb_colors(const PerturbArgs a, const CS colors) {
   extern __shared__ double s_eps[];
+  cudaGridDependencySynchronize();   // launched as a programmatic dependent: eps (and x) may come from the kernel before
   const bool use_smem = a.C <= kPerturbSmemColors;
   if (use_smem) {
     for (int i = threadIdx.x; i < a.C; i += kThreads) s_eps[i] = a.eps[i];

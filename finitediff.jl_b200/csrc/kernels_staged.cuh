@@ -53,6 +53,8 @@ __device__ __forceinline__ void fence_mbar_init() {
 constexpr int kStageMaxWin = 8;        // windows per tile: C + 1 (forward: slabs + fx) or 2C (central: plus / minus slabs)
 constexpr int kStagesMax = 3;          // tiles in flight per block (2 by default: 8 blocks/SM; 3 leaves 6)
 constexpr int kStageMaxSmem = 46 * 1024;
+// shared memory behind the staged windows: full / empty mbarriers and two phases of walk positions per stage
+constexpr size_t kStageCtlBytes = 4 * kStagesMax * 8;
 
 struct StagedArgs {
   const uint16_t *row16;     // [E] row - tile_w0[tile]                        (indexed form)
@@ -65,6 +67,7 @@ struct StagedArgs {
   int64_t ldF, src_len;      // slab stride; readable doubles behind fx / every slab (even)
   int64_t E;
   int32_t j_aligned;
+  unsigned long long *claim; // walk positions claimed past each block's first `stages` (0 between launches)
   int32_t reverse;           // walk the full tiles from the end of J's storage towards its start: the rows the last f! wrote
                              // most recently (the tail of the last slab) are read while they are still in L2
   // band form: the pattern is exactly the clipped band, column c holding rows max(0, c-l) .. min(m-1, c+u) in order
@@ -158,6 +161,7 @@ __global__ void __launch_bounds__(kThreads, MINB)
 diff_scatter_staged(const StagedArgs a, const CS colors) {
   static_assert(MODE == kForward || MODE == kCentral, "staged scatter: forward / central");
   static_assert(!(BAND && (PACKED || PREFETCH)), "band form: no index stream to pack or prefetch");
+  static_assert(!(PREFETCH && EMPTYBAR), "index prefetch reads the next walk position behind the block barrier");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int C = a.C, W = a.W;
   const int nwin = MODE == kCentral ? 2 * C : C + 1;
@@ -166,15 +170,19 @@ diff_scatter_staged(const StagedArgs a, const CS colors) {
   double *buf = reinterpret_cast<double *>(smem_raw);                       // [stages][nwin][W]
   uint64_t *full = reinterpret_cast<uint64_t *>(buf + kStages * stage_elems);
   uint64_t *empty = full + kStagesMax;
-  double *s_eps = reinterpret_cast<double *>(full + 2 * kStagesMax);        // [C]
+  int64_t *s_pos = reinterpret_cast<int64_t *>(empty + kStagesMax);         // [2][kStagesMax] walk positions
+  double *s_eps = reinterpret_cast<double *>(s_pos + 2 * kStagesMax);       // [C]
   const int64_t nfull = a.E / kTile;
   constexpr int kHalf = kTile / 2;
   const int tid2 = 2 * threadIdx.x;
   // position in the walk -> tile of J's storage (the walk order is free: every tile is independent)
   auto phys = [&](int64_t t) -> int64_t { return a.reverse ? nfull - 1 - t : t; };
 
-  // one thread feeds the pipeline: nwin bulk copies per tile, all completing on the stage's mbarrier
-  auto issue = [&](int64_t tile, int s) {
+  // one thread feeds the pipeline: nwin bulk copies per tile, all completing on the stage's mbarrier.  A position past
+  // the walk fills nothing: the bare arrival completes the stage's phase and the block reads the end of its walk there.
+  auto issue = [&](int64_t pos, int s) {
+    if (pos >= nfull) { mbar_arrive(full + s); return; }
+    const int64_t tile = phys(pos);
     const int32_t w0 = __ldg(a.tile_w0 + tile);
     int64_t len = a.src_len - w0;
     if (len > W) len = W;
@@ -188,19 +196,31 @@ diff_scatter_staged(const StagedArgs a, const CS colors) {
       bulk_g2s(dst + C * W, a.fx + w0, bytes, full + s);
     }
   };
+  // Walk positions: each block starts on blockIdx.x + s * gridDim.x (s < stages); every later position is claimed from
+  // the counter *a.claim when a stage is refilled, `stages` iterations ahead, so a block that falls behind takes fewer
+  // tiles and the blocks end together.  The position of the iteration on stage s in phase parity p sits in
+  // s_pos[p * kStagesMax + s]: written by the producer before the block barrier (or the empty-stage wait) of the
+  // iteration `stages` earlier, so it is read after that barrier, or after the full-stage wait that the producer's
+  // arrival releases; its previous value was read before that iteration's barrier.
+  // Every iteration that takes a tile claims once, so a launch makes exactly nfull claims: the one that draws nfull - 1
+  // is the last, and re-arms the counter for the next launch (graph replays included) with no host step.
+  auto claim = [&]() -> int64_t {
+    const unsigned long long v = atomicAdd(a.claim, 1ull);
+    if (v == (unsigned long long)nfull - 1) atomicExch(a.claim, 0ull);
+    return (int64_t)kStages * gridDim.x + (int64_t)v;
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, kThreads / 32); }
     fence_mbar_init();
+    for (int s = 0; s < kStages; ++s) s_pos[s] = min((int64_t)blockIdx.x + (int64_t)s * gridDim.x, nfull);
   }
+  // everything above reads nothing the kernel before this one writes (programmatic dependent launch)
+  cudaGridDependencySynchronize();
   for (int i = threadIdx.x; i < C; i += kThreads) s_eps[i] = a.eps[i];
   __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      const int64_t t = (int64_t)blockIdx.x + (int64_t)s * gridDim.x;
-      if (t < nfull) issue(phys(t), s);
-    }
-  }
+  if (threadIdx.x == 0)
+    for (int s = 0; s < kStages; ++s) issue(s_pos[s], s);
 
   auto value = [&](const double *__restrict__ win, uint32_t r, uint32_t k) -> double {
     if (k >= (uint32_t)C) return 0.0;                    // column without a valid colour: stays 0 (fill_matrix!)
@@ -253,19 +273,33 @@ diff_scatter_staged(const StagedArgs a, const CS colors) {
     }
     return x;
   };
-  uint32_t it = 0;
   int s = 0;
   uint32_t parity = 0;
   Idx nx{};
-  if (PREFETCH && (int64_t)blockIdx.x < nfull) nx = load_idx(phys(blockIdx.x));
-  for (int64_t pos = blockIdx.x; pos < nfull; pos += gridDim.x, ++it) {
+  if (PREFETCH && s_pos[0] < nfull) nx = load_idx(phys(s_pos[0]));
+  for (;;) {
+    int64_t pos;
+    if (EMPTYBAR) {                                       // the position is released with the stage
+      while (!mbar_try_wait(full + s, parity)) {}
+      pos = s_pos[parity * kStagesMax + s];
+      if (pos >= nfull) break;
+    } else {                                              // written behind an earlier block barrier
+      pos = s_pos[parity * kStagesMax + s];
+      if (pos >= nfull) break;
+    }
     const int64_t tile = phys(pos);
     double *__restrict__ Jt = a.J + tile * kTile;
     const Idx cur = PREFETCH ? nx : load_idx(tile);
-    if (PREFETCH && pos + gridDim.x < nfull) nx = load_idx(phys(pos + gridDim.x));
+    if (PREFETCH) {                                       // the next iteration's position: stage s + 1, or stage 0 of the next phase
+      const int64_t pn = s + 1 == kStages ? s_pos[(parity ^ 1u) * kStagesMax] : s_pos[parity * kStagesMax + s + 1];
+      if (pn < nfull) nx = load_idx(phys(pn));
+    }
     const ushort2 ra = cur.ra, rb = cur.rb;
     const uint32_t ka0 = cur.ka0, ka1 = cur.ka1, kb0 = cur.kb0, kb1 = cur.kb1;
-    while (!mbar_try_wait(full + s, parity)) {}
+    // the position this stage is refilled with (the iteration `stages` later): claimed while the tile is computed
+    int64_t *refill = s_pos + (parity ^ 1u) * kStagesMax + s;
+    if (threadIdx.x == 0) *refill = claim();
+    if (!EMPTYBAR) while (!mbar_try_wait(full + s, parity)) {}
     const double *__restrict__ win = buf + s * stage_elems;
     const double va0 = value(win, ra.x, ka0), va1 = value(win, ra.y, ka1);
     const double vb0 = value(win, rb.x, kb0), vb1 = value(win, rb.y, kb1);
@@ -279,18 +313,12 @@ diff_scatter_staged(const StagedArgs a, const CS colors) {
       __syncwarp();
       if ((threadIdx.x & 31) == 0) mbar_arrive(empty + s);              // this warp is done with stage s
       if (threadIdx.x == 0) {
-        const int64_t nxt = pos + (int64_t)kStages * gridDim.x;
-        if (nxt < nfull) {
-          while (!mbar_try_wait(empty + s, parity)) {}                   // ... and so are the other seven: refill it
-          issue(phys(nxt), s);
-        }
+        while (!mbar_try_wait(empty + s, parity)) {}                     // ... and so are the other seven: refill it
+        issue(*refill, s);
       }
     } else {
       __syncthreads();                                    // every lane is done with stage s: refill it
-      if (threadIdx.x == 0) {
-        const int64_t nxt = pos + (int64_t)kStages * gridDim.x;
-        if (nxt < nfull) issue(phys(nxt), s);
-      }
+      if (threadIdx.x == 0) issue(*refill, s);
     }
     if (++s == kStages) { s = 0; parity ^= 1u; }
   }

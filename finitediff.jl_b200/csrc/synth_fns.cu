@@ -229,7 +229,40 @@ __global__ void __launch_bounds__(kT) k_store_probe(double *__restrict__ out, in
   }
 }
 
+// Streaming bandwidth probe for a traffic mix: R source vectors read, W destination vectors written, n doubles each,
+// 16-byte streaming loads and stores, grid-stride in address order.  With W = 0 the sum of the loads goes to sink[0]
+// only if it is a NaN (never for finite sources), so the loads are not dead code.
+template <int R, int W>
+__global__ void __launch_bounds__(kT) k_stream_probe(const double *__restrict__ src, int64_t lds, double *__restrict__ dst,
+                                                     int64_t ldd, int64_t n, double *__restrict__ sink) {
+  const int64_t stride = (int64_t)gridDim.x * kT * 2;
+  double acc = 0.0;
+  for (int64_t i = (blockIdx.x * (int64_t)kT + threadIdx.x) * 2; i + 1 < n; i += stride) {
+    double2 v[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) v[r] = __ldcs(reinterpret_cast<const double2 *>(src + r * lds + i));
+    double a = v[0].x, b = v[0].y;
+#pragma unroll
+    for (int r = 1; r < R; ++r) { a += v[r].x; b += v[r].y; }
+#pragma unroll
+    for (int w = 0; w < W; ++w) __stcs(reinterpret_cast<double2 *>(dst + w * ldd + i), make_double2(a + w, b + w));
+    if (W == 0) acc += a + b;
+  }
+  if (W == 0 && acc != acc) sink[0] = acc;
+}
+
 extern "C" {
+
+int fdbs_stream_probe(const double *d_src, int64_t lds, int reads, double *d_dst, int64_t ldd, int writes, int64_t n,
+                      int blocks, double *d_sink, void *stream) {
+  if (n <= 0 || blocks <= 0 || ((uintptr_t)d_src & 15) || ((uintptr_t)d_dst & 15) || (lds & 1) || (ldd & 1)) return 1;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (reads == 1 && writes == 0) k_stream_probe<1, 0><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 1 && writes == 3) k_stream_probe<1, 3><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 4 && writes == 3) k_stream_probe<4, 3><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else return 2;
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
 
 int fdbs_tridiag(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream) {
   fdbs_tridiag_ctx *c = (fdbs_tridiag_ctx *)vctx;

@@ -42,6 +42,10 @@ int fdbs_fill_x(double *d_x, int64_t n, uint64_t seed, void *stream);
 /* write a buffer larger than L2 (flushes L2 between timed iterations) */
 /* store-only bandwidth probe: mode 0 constant data, mode 1 a distinct value per element */
 int fdbs_store_probe(double *d_out, int64_t n, int mode, int blocks, void *stream);
+/* read / write mix probe: `reads` vectors of n doubles from d_src (stride lds) read, `writes` vectors written to d_dst
+ * (stride ldd), 16-byte streaming accesses; mixes (1, 0), (1, 3), (4, 3); d_sink: one double, written only on a NaN sum */
+int fdbs_stream_probe(const double *d_src, int64_t lds, int reads, double *d_dst, int64_t ldd, int writes, int64_t n,
+                      int blocks, double *d_sink, void *stream);
 int fdbs_flush_l2(void *d_buf, int64_t bytes, void *stream);
 
 #ifdef __cplusplus
