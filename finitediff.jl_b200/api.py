@@ -31,7 +31,8 @@ from . import _lib as L
 __all__ = [
     "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "BandedBlockBandedMatrix", "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
     "finite_difference_jacobian_", "finite_difference_jacobian_b", "resize_", "default_relstep", "compute_epsilon",
-    "zeros_colmajor", "pinned_empty",
+    "zeros_colmajor", "pinned_empty", "HessianCache", "finite_difference_hessian_", "finite_difference_hessian",
+    "GradientCache", "finite_difference_gradient_", "finite_difference_gradient",
 ]
 
 _DEFAULT = object()
@@ -373,8 +374,11 @@ class _PyFn:
     """Wraps a Python f!(fx, x) working on CUDA tensors as an fdb_fn.  `batched=True` callables receive 2-D
     (batch, m) / (batch, n) tensors; otherwise they are called once per point with 1-D tensors."""
 
-    def __init__(self, f: Callable, m: int, n: int, device: torch.device, batched: bool, complex_: bool = False):
+    def __init__(self, f: Callable, m: int, n: int, device: torch.device, batched: bool, complex_: bool = False,
+                 scalar: bool = False):
         self.f, self.m, self.n, self.device, self.batched = f, m, n, device, batched
+        # scalar (m = 1) functions are called as f(x) and RETURN their value (a 0-d CUDA tensor needs no host sync)
+        self.scalar = scalar
         self.exc: Optional[BaseException] = None
         self.calls = 0
         # complex-step callbacks (fdb_fn_c) see complex128 tensors; ld* then count complex elements
@@ -392,7 +396,16 @@ class _PyFn:
                 es = self.esize
                 fx2 = torch.as_tensor(_DevArray(p_fx, (batch, self.m), (ldfx * es, es), self.typestr), device=self.device)
                 x2 = torch.as_tensor(_DevArray(p_x, (batch, self.n), (ldx * es, es), self.typestr), device=self.device)
-                if self.batched:
+                if self.scalar and self.batched:
+                    self.calls += int(batch)
+                    # dtype of the slot (float64 / complex128): a Python float or complex must not pass through
+                    # torch's default float32 / complex64
+                    fx2[:, 0].copy_(torch.as_tensor(self.f(x2), dtype=fx2.dtype, device=self.device).reshape(-1))
+                elif self.scalar:
+                    for b in range(int(batch)):
+                        self.calls += 1
+                        fx2[b, 0].copy_(torch.as_tensor(self.f(x2[b]), dtype=fx2.dtype, device=self.device).reshape(()))
+                elif self.batched:
                     self.calls += int(batch)
                     self.f(fx2, x2)
                 else:
@@ -777,10 +790,10 @@ def check_coloring(A: "SparseMatrixCSC", colorvec) -> int:
 
 
 # ------------------------------------------------------------------------------------------------ the public call
-def _as_fn(f, m, n, device, plan_batch, complex_=False):
+def _as_fn(f, m, n, device, plan_batch, complex_=False, scalar=False):
     if isinstance(f, NativeFn):
         return f.address, f.ctx_ptr, None
-    w = _PyFn(f, m, n, device, bool(getattr(f, "batched", False)), complex_)
+    w = _PyFn(f, m, n, device, bool(getattr(f, "batched", False)), complex_, scalar)
     return L.fn_address(w.cfunc), None, w
 
 
@@ -965,3 +978,231 @@ def _shape_of(J):
             return (J.shape[0], 1)
         return tuple(J.shape)
     raise TypeError(f"unsupported J type {type(J)}")
+
+
+# ------------------------------------------------------------------------------------------------ Hessian (src/hessians.jl)
+def _hessian_fdtype_code(fdtype) -> int:
+    """The Hessian's fdtype: "hcentral" (FDB_HCENTRAL); the Jacobian's codes pass through so that the plan rejects them
+    the way the reference's @assert does (hessians.jl:206)."""
+    if isinstance(fdtype, str) and fdtype.lstrip(":") == "hcentral":
+        return L.FDB_HCENTRAL
+    if fdtype == L.FDB_HCENTRAL:
+        return L.FDB_HCENTRAL
+    return _fdtype_code(fdtype)
+
+
+def _scalar_x(x, what="x"):
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise TypeError(f"{what} must be a float64 CUDA tensor: the GPU path has no CPU implementation")
+    if x.dtype != torch.float64:
+        raise TypeError(f"{what} must be float64 (complex-valued x is not supported)")
+    xv = x.reshape(-1)
+    return xv if xv.is_contiguous() else xv.contiguous()
+
+
+class HessianCache:
+    """Mirror of FiniteDiff.HessianCache (hessians.jl:1-9, :60-80):
+
+        HessianCache(x, fdtype="hcentral")                   allocating: xpp, xpm, xmp, xmm = copies of x
+        HessianCache(xpp, xpm, xmp, xmm, fdtype="hcentral")  non-allocating: aliases the arrays passed in
+
+    The cache arrays are scratch (the reference copies x into them before use, :213-216): a cache built from another x
+    changes nothing (issue #185, finitedifftests.jl:608-614).  The GPU path keeps its points in plan-owned memory and
+    does not touch them.  Extra keywords (GPU path only): max_batch, scratch_bytes, use_graph."""
+
+    def __init__(self, *arrays, fdtype="hcentral", **plan_kw):
+        if len(arrays) == 2 and not isinstance(arrays[1], torch.Tensor):     # HessianCache(x, fdtype)
+            arrays, fdtype = arrays[:1], arrays[1]
+        elif len(arrays) == 5:                                                # HessianCache(xpp, xpm, xmp, xmm, fdtype)
+            arrays, fdtype = arrays[:4], arrays[4]
+        if len(arrays) == 1:
+            x = arrays[0]
+            if not _is_cuda(x):
+                raise TypeError("HessianCache needs CUDA float64 tensors (this path has no CPU implementation)")
+            self.xpp, self.xpm, self.xmp, self.xmm = (x.clone() for _ in range(4))
+        elif len(arrays) == 4:
+            self.xpp, self.xpm, self.xmp, self.xmm = arrays
+        else:
+            raise TypeError("HessianCache(x) or HessianCache(xpp, xpm, xmp, xmm)")
+        self.fdtype = fdtype.lstrip(":") if isinstance(fdtype, str) else fdtype
+        self._plan_kw = plan_kw
+        self._plans = {}
+
+    def plan_for(self, n: int, ldH: int, device) -> Plan:
+        key = (n, ldH, str(device))
+        p = self._plans.get(key)
+        if p is None:
+            code = _hessian_fdtype_code(self.fdtype)
+            h = C.c_void_p()
+            o = _opts(code, _device_index(device), **self._plan_kw)
+            L.check(L.lib().fdb_hessian_plan_create(C.byref(h), n, ldH, C.byref(o)))
+            p = self._plans[key] = Plan(h.value)
+        return p
+
+
+def _colmajor_square(H, n):
+    if not isinstance(H, torch.Tensor) or not H.is_cuda or H.dtype != torch.float64:
+        raise TypeError("H must be a float64 CUDA tensor")
+    if H.dim() != 2 or tuple(H.shape) != (n, n):
+        raise ValueError(f"H must be {n} x {n}")
+    if n > 1 and H.stride(0) != 1:
+        raise ValueError("H must be column-major (Julia Matrix layout): use zeros_colmajor(n, n) or X.t()")
+    return max(int(H.stride(1)) if n > 1 else n, n, 1)
+
+
+def finite_difference_hessian_(H, f, x, cache=None, *, relstep=None, absstep=None, fx=None, stream=None):
+    """finite_difference_hessian!(H, f, x, cache::HessianCache; relstep, absstep) (hessians.jl:202-292), or — when
+    `cache` is None or an fdtype string — the cache-less form (:181-189).
+
+    H: column-major float64 CUDA tensor (n, n), e.g. zeros_colmajor(n, n); both triangles are written (copytri!, :291).
+    f: Python callable f(x) -> scalar (a 0-d CUDA tensor needs no host sync; set f.batched=True to receive a (batch, n)
+       tensor and return (batch,) values) or a NativeFn (batched fdb_fn with m = 1).
+    x: float64 CUDA tensor, never modified.  fx: optional 1-element float64 CUDA tensor that receives f(x).
+    Returns None."""
+    if cache is None or isinstance(cache, str):
+        cache = HessianCache(x, fdtype=cache or "hcentral")
+    if not isinstance(cache, HessianCache):
+        raise TypeError("cache must be a HessianCache, an fdtype string, or None")
+    xv = _scalar_x(x)
+    n = xv.numel()
+    ldH = _colmajor_square(H, n)
+    plan = cache.plan_for(n, ldH, xv.device)
+    addr, ctx, pyfn = _as_fn(f, 1, n, xv.device, 1, scalar=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(xv.device).cuda_stream
+    fx_ptr = None
+    if fx is not None:
+        if not _is_cuda(fx) or fx.dtype != torch.float64 or fx.numel() != 1:
+            raise TypeError("fx must be a 1-element float64 CUDA tensor")
+        fx_ptr = fx.data_ptr()
+    with torch.cuda.device(xv.device):
+        st = L.lib().fdb_hessian(plan.handle, addr, ctx, xv.data_ptr(), H.data_ptr() if n > 0 else None, fx_ptr,
+                                 L.STEP_DEFAULT if relstep is None else float(relstep),
+                                 L.STEP_DEFAULT if absstep is None else float(absstep), C.c_void_p(stream))
+    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
+        exc, pyfn.exc = pyfn.exc, None
+        raise exc
+    L.check(st)
+    cache._last_plan = plan
+    return None
+
+
+def finite_difference_hessian(f, x, cache=None, *, relstep=None, absstep=None, stream=None):
+    """finite_difference_hessian(f, x[, cache]; relstep, absstep) (hessians.jl:140-167): a new column-major n x n H with
+    both triangles filled (the reference returns Symmetric(H), whose entries are the same)."""
+    n = x.numel()
+    H = zeros_colmajor(n, n, device=x.device)
+    finite_difference_hessian_(H, f, x, cache, relstep=relstep, absstep=absstep, stream=stream)
+    return H
+
+
+# ------------------------------------------------------------------------------------------------ gradient (src/gradients.jl)
+class GradientCache:
+    """Mirror of FiniteDiff.GradientCache (gradients.jl:1-7) for the vector -> scalar case on real Float64 arrays:
+
+        GradientCache(df, x, fdtype="central", returntype=float64)     allocating, fx = nothing   (:19-62)
+        GradientCache(fx, c1, c2, c3, fdtype="central", returntype)    non-allocating             (:104-123)
+
+    A gradient is the dense column branch of the Jacobian with m = 1 (gradients.jl:408-468 against jacobians.jl:548-557,
+    590-598, 625-631): the same steps, points, quotients and call order.  The GPU path therefore runs a dense Jacobian
+    plan (m = 1, ldJ = 1) with df as J; a non-None fx (a number or a 1-element CUDA tensor) is used as f(x) in forward
+    mode, as :410 does.  c1..c3 are scratch.  Extra keywords (GPU path only): max_batch, scratch_bytes, use_graph."""
+
+    def __init__(self, *arrays, fdtype="central", returntype=torch.float64, **plan_kw):
+        arrays = list(arrays)
+        if arrays and isinstance(arrays[-1], str):
+            fdtype = arrays.pop()
+        if len(arrays) == 2:
+            df, x = arrays
+            for t, name in ((df, "df"), (x, "x")):
+                if not isinstance(t, torch.Tensor):
+                    raise TypeError(f"{name} must be a CUDA tensor (the scalar -> vector form is not supported)")
+                if t.is_complex():
+                    raise TypeError(f"{name} must be real Float64: complex-valued gradients are not supported")
+            self.fx, self.c1, self.c2, self.c3 = None, None, None, torch.zeros_like(x)
+        elif len(arrays) == 4:
+            self.fx, self.c1, self.c2, self.c3 = arrays
+        else:
+            raise TypeError("GradientCache(df, x[, fdtype]) or GradientCache(fx, c1, c2, c3[, fdtype])")
+        if returntype not in (torch.float64, float, np.float64):
+            raise TypeError("only Float64 is supported by the GPU path")
+        self.fdtype = fdtype.lstrip(":") if isinstance(fdtype, str) else fdtype
+        _fdtype_code(self.fdtype)
+        self._plan_kw = plan_kw
+        self._plans = {}
+
+    def plan_for(self, n: int, device) -> Plan:
+        key = (n, str(device))
+        p = self._plans.get(key)
+        if p is None:
+            h = C.c_void_p()
+            o = _opts(_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
+            L.check(L.lib().fdb_plan_create_dense(C.byref(h), 1, n, 1, C.byref(o)))
+            p = self._plans[key] = Plan(h.value)
+        return p
+
+
+def finite_difference_gradient_(df, f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None):
+    """finite_difference_gradient!(df, f, x, cache::GradientCache; relstep, absstep, dir) (gradients.jl:390-473), or —
+    when `cache` is None or an fdtype string — the cache-less form (:220-248).
+
+    df, x: float64 CUDA vectors of length n (complex arrays and a Number x are rejected with TypeError).
+    f: Python callable f(x) -> scalar as for finite_difference_hessian_ (complex step: f receives complex128 x and
+       returns a complex scalar), or a NativeFn (fdb_fn with m = 1; fdb_fn_c for complex).  Returns None."""
+    if cache is None or isinstance(cache, str):
+        cache = GradientCache(df, x, cache or "central")
+    if not isinstance(cache, GradientCache):
+        raise TypeError("cache must be a GradientCache, an fdtype string, or None")
+    if not isinstance(x, torch.Tensor) or not isinstance(df, torch.Tensor):
+        raise TypeError("x and df must be CUDA tensors (the scalar -> vector form is not supported)")
+    xv = _scalar_x(x)
+    dv = _scalar_x(df, "df")
+    n = xv.numel()
+    if dv.numel() != n:
+        raise ValueError(f"length(df)={dv.numel()} != length(x)={n}")
+    if df.reshape(-1).data_ptr() != dv.data_ptr():
+        raise ValueError("df must be contiguous")
+    fd = _fdtype_code(cache.fdtype)
+    plan = cache.plan_for(n, xv.device)
+    addr, ctx, pyfn = _as_fn(f, 1, n, xv.device, 1, fd == L.FDB_COMPLEX, scalar=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(xv.device).cuda_stream
+    with torch.cuda.device(xv.device):
+        if fd == L.FDB_COMPLEX:                                              # :458-469
+            st = L.lib().fdb_jacobian_complex(plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(), C.c_void_p(stream))
+        else:
+            fin = None
+            if fd == L.FDB_FORWARD and cache.fx is not None:                # fx0 = fx !== nothing ? fx : f(x)   :410
+                if isinstance(cache.fx, torch.Tensor):
+                    fin = cache.fx
+                    if not fin.is_cuda or fin.dtype != torch.float64 or fin.numel() != 1:
+                        raise TypeError("cache.fx must be a number or a 1-element float64 CUDA tensor")
+                else:
+                    # a number: staged in ONE device slot kept on the cache, so that the arguments of the call (and a
+                    # captured graph's key under use_graph) stay the same from call to call
+                    fin = getattr(cache, "_fin", None)
+                    if fin is None or fin.device != xv.device:
+                        fin = cache._fin = torch.empty(1, dtype=torch.float64, device=xv.device)
+                    with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=xv.device)):
+                        fin.fill_(float(cache.fx))
+            # d_fx = NULL: f(x) goes to the plan's own buffer (cache.fx is an input here, never written)
+            st = L.lib().fdb_jacobian(plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(), None,
+                                      None if fin is None else fin.data_ptr(),
+                                      L.STEP_DEFAULT if relstep is None else float(relstep),
+                                      L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
+    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
+        exc, pyfn.exc = pyfn.exc, None
+        raise exc
+    L.check(st)
+    cache._last_plan = plan
+    return None
+
+
+def finite_difference_gradient(f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None):
+    """finite_difference_gradient(f, x[, cache | fdtype]; relstep, absstep, dir) (gradients.jl:168-218, :250-300): a new
+    float64 CUDA vector df."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("x must be a CUDA tensor (the scalar -> vector form is not supported)")
+    df = torch.zeros(x.numel(), dtype=torch.float64, device=x.device)
+    finite_difference_gradient_(df, f, x, cache, relstep=relstep, absstep=absstep, dir=dir, stream=stream)
+    return df

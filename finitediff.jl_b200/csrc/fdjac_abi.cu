@@ -29,6 +29,7 @@
 #include "kernels_staged.cuh"
 #include "kernels_jvp.cuh"
 #include "kernels_color.cuh"
+#include "kernels_hessian.cuh"
 
 using namespace fdb;
 
@@ -58,7 +59,7 @@ static fdb_status fail(fdb_status st, const char *fmt, ...) {
     if (s__ != FDB_OK) return s__;   \
   } while (0)
 
-enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6 };
+enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7 };
 
 // Device memory that lives while a plan or a colouring is built: freed when it goes out of scope, unless release()
 // hands it to a plan that keeps it (fdb_plan::adopt).  Declared after the builder's DeviceGuard, it is freed on the
@@ -218,6 +219,10 @@ struct fdb_plan {
   // dense-column plans
   int64_t col_begin = 0, col_end = 0;
   double *eps_cols = nullptr;
+  // Hessian plans (kernels_hessian.cuh): value buffer V (V[0] = f(x), then one chunk of whole i-blocks) and the chunk
+  // boundaries [hess_chunks[c], hess_chunks[c+1]) in i
+  double *hess_V = nullptr;
+  std::vector<int64_t> hess_chunks;
   // host-buffer path
   cudaStream_t hstream = nullptr;
   double *h_dx = nullptr, *h_dJ = nullptr, *h_dfx = nullptr, *h_dfin = nullptr;
@@ -823,6 +828,7 @@ int fdb_device_count(void) {
 double fdb_default_relstep(int fdtype) {
   if (fdtype == FDB_FORWARD) return sqrt(DBL_EPSILON);
   if (fdtype == FDB_CENTRAL) return cbrt(DBL_EPSILON);
+  if (fdtype == FDB_HCENTRAL) return ldexp(1.0, -13);   // eps(Float64)^(1/4) = (2^-52)^(1/4), exact
   return 1.0;
 }
 // src/epsilons.jl:26-29 / :50-53
@@ -1139,11 +1145,13 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   info->n_entries = P->E;
   info->j_len = P->j_len;
   info->n_colors = P->C;
-  const int64_t n_local = P->sp_kind == SP_NONE ? P->col_end - P->col_begin : (int64_t)P->local_colors.size();
+  const int64_t n_local = (P->sp_kind == SP_NONE || P->sp_kind == SP_HESS) ? P->col_end - P->col_begin
+                                                                           : (int64_t)P->local_colors.size();
   info->n_local_colors = n_local;
   info->n_groups = P->n_groups;
   info->slabs = P->slabs;
   info->fcalls_per_jacobian = P->fdtype == FDB_CENTRAL ? 2 * n_local : (P->fdtype == FDB_COMPLEX ? n_local : 1 + n_local);
+  if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = 2 * P->n * P->n + 1;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
   info->jkind = P->jkind;
@@ -1196,7 +1204,7 @@ fdb_status fdb_plan_dense_range(const fdb_plan *P, int64_t *b, int64_t *e) {
 
 fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t cap) {
   if (!P || !owner_out) return fail(FDB_ERR_INVALID, "NULL argument");
-  if (P->sp_kind == SP_NONE) return fail(FDB_ERR_INVALID, "dense plans partition columns by range");
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "dense plans partition columns by range");
   if (cap < (int64_t)P->owner.size()) return fail(FDB_ERR_INVALID, "owner_out too small");
   std::copy(P->owner.begin(), P->owner.end(), owner_out);
   return FDB_OK;
@@ -1205,9 +1213,11 @@ fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t c
 fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *stream) {
   if (!P || !h_eps) return fail(FDB_ERR_INVALID, "NULL argument");
   DeviceGuard g(P->device);
-  const int64_t count = P->sp_kind == SP_NONE ? P->col_end - P->col_begin : P->C;   // JVP plans: C == 1
+  // JVP plans: C == 1; Hessian plans: one step per component (col_begin = 0, col_end = n)
+  const bool per_column = P->sp_kind == SP_NONE || P->sp_kind == SP_HESS;
+  const int64_t count = per_column ? P->col_end - P->col_begin : P->C;
   if (cap < count) return fail(FDB_ERR_INVALID, "h_eps too small (%lld < %lld)", (long long)cap, (long long)count);
-  const double *src = P->sp_kind == SP_NONE ? P->eps_cols : P->eps;
+  const double *src = per_column ? P->eps_cols : P->eps;
   if (count > 0) {
     CU(cudaMemcpyAsync(h_eps, src, (size_t)count * 8, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     CU(cudaStreamSynchronize((cudaStream_t)stream));
@@ -1243,7 +1253,7 @@ fdb_status fdb_plan_read_timing(fdb_plan *P, double *scatter_ms, int64_t *scatte
 fdb_status fdb_plan_set_peers(fdb_plan *P, int n_peers, double *const *peer_J) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
   if (n_peers < 0 || n_peers > 64) return fail(FDB_ERR_INVALID, "n_peers out of range");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_HESS)
     return fail(FDB_ERR_UNSUPPORTED, "peer stores are implemented for the entry-driven (CSC / COO) scatters");
   DeviceGuard g(P->device);
   if (!P->d_peers) TRY(P->alloc_t(&P->d_peers, 64));
@@ -1750,6 +1760,45 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
   return FDB_OK;
 }
 
+// The call as enqueued by `eager(stream)`, or — use_graph — a CUDA-graph replay of it: the launch sequence depends only on
+// the plan and on the arguments in `key` (step sizes are computed on the device inside the graph), so it is captured once
+// and re-launched while the key stays the same.
+template <typename F>
+static fdb_status run_maybe_graph(fdb_plan *P, const GraphKey &key, cudaStream_t s, const char *what, F &&eager) {
+  if (!P->use_graph || P->timing) return eager(s);
+  if (!P->graph_exec || !(key == P->graph_key)) {
+    if (P->graph_exec) { cudaGraphExecDestroy(P->graph_exec); P->graph_exec = nullptr; }
+    if (!P->cstream) CU(cudaStreamCreateWithFlags(&P->cstream, cudaStreamNonBlocking));
+    const fdb_counters_t before = P->cnt;
+    CU(cudaStreamBeginCapture(P->cstream, cudaStreamCaptureModeThreadLocal));
+    const fdb_status st = eager(P->cstream);
+    cudaGraph_t graph = nullptr;
+    cudaError_t e = cudaStreamEndCapture(P->cstream, &graph);
+    if (st != FDB_OK) { if (graph) cudaGraphDestroy(graph); cudaGetLastError(); return st; }
+    if (e != cudaSuccess || !graph) {
+      cudaGetLastError();
+      return fail(FDB_ERR_CUDA, "stream capture of the %s failed (%s): the f! callback must be capture-safe "
+                                "(enqueue-only, no allocation) when use_graph is set", what, cudaGetErrorString(e));
+    }
+    e = cudaGraphInstantiate(&P->graph_exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) { P->graph_exec = nullptr; return fail(FDB_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
+    P->graph_key = key;
+    // what one replay amounts to (the capture pass itself launched nothing)
+    P->graph_delta.f_points = P->cnt.f_points - before.f_points;
+    P->graph_delta.f_invocations = P->cnt.f_invocations - before.f_invocations;
+    P->graph_delta.kernel_launches = P->cnt.kernel_launches - before.kernel_launches;
+    P->graph_delta.scatter_launches = P->cnt.scatter_launches - before.scatter_launches;
+    P->cnt = before;
+  }
+  CU(cudaGraphLaunch(P->graph_exec, s));
+  P->cnt.f_points += P->graph_delta.f_points;
+  P->cnt.f_invocations += P->graph_delta.f_invocations;
+  P->cnt.kernel_launches += P->graph_delta.kernel_launches;
+  P->cnt.scatter_launches += P->graph_delta.scatter_launches;
+  return FDB_OK;
+}
+
 extern "C" {
 
 static fdb_status jacobian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_J, double *fx,
@@ -1773,6 +1822,7 @@ fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, dou
   if ((P->n > 0 && !d_x) || (P->j_len > 0 && !d_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   if (P->sp_kind == SP_JVP) return fail(FDB_ERR_INVALID, "this is a JVP plan: call fdb_jvp");
   if (P->sp_kind == SP_EPS) return fail(FDB_ERR_INVALID, "this is a step-size plan: call fdb_color_eps");
+  if (P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian plan: call fdb_hessian");
   if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
     return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
   DeviceGuard g(P->device);
@@ -1781,45 +1831,10 @@ fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, dou
   // jacobians.jl:508-509 defaults
   resolve_steps(P->fdtype, relstep, absstep);
   double *fx = d_fx ? d_fx : P->fx_own;
-  fdb_status st;
-  if (P->use_graph && !P->timing) {
-    // CUDA-graph replay of the whole call: the launch sequence depends only on the plan and on these arguments
-    // (the step sizes are computed on the device inside the graph), so it is captured once and re-launched.
-    const GraphKey key{(void *)f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, P->n_peers, P->peer_generation, P->ext_eps};
-    if (!P->graph_exec || !(key == P->graph_key)) {
-      if (P->graph_exec) { cudaGraphExecDestroy(P->graph_exec); P->graph_exec = nullptr; }
-      if (!P->cstream) CU(cudaStreamCreateWithFlags(&P->cstream, cudaStreamNonBlocking));
-      const fdb_counters_t before = P->cnt;
-      CU(cudaStreamBeginCapture(P->cstream, cudaStreamCaptureModeThreadLocal));
-      st = jacobian_eager(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, P->cstream);
-      cudaGraph_t graph = nullptr;
-      cudaError_t e = cudaStreamEndCapture(P->cstream, &graph);
-      if (st != FDB_OK) { if (graph) cudaGraphDestroy(graph); cudaGetLastError(); return st; }
-      if (e != cudaSuccess || !graph) {
-        cudaGetLastError();
-        return fail(FDB_ERR_CUDA, "stream capture of the Jacobian failed (%s): the f! callback must be capture-safe "
-                                  "(enqueue-only, no allocation) when use_graph is set", cudaGetErrorString(e));
-      }
-      e = cudaGraphInstantiate(&P->graph_exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (e != cudaSuccess) { P->graph_exec = nullptr; return fail(FDB_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
-      P->graph_key = key;
-      // what one replay amounts to (the capture pass itself launched nothing)
-      P->graph_delta.f_points = P->cnt.f_points - before.f_points;
-      P->graph_delta.f_invocations = P->cnt.f_invocations - before.f_invocations;
-      P->graph_delta.kernel_launches = P->cnt.kernel_launches - before.kernel_launches;
-      P->graph_delta.scatter_launches = P->cnt.scatter_launches - before.scatter_launches;
-      P->cnt = before;
-    }
-    CU(cudaGraphLaunch(P->graph_exec, s));
-    P->cnt.f_points += P->graph_delta.f_points;
-    P->cnt.f_invocations += P->graph_delta.f_invocations;
-    P->cnt.kernel_launches += P->graph_delta.kernel_launches;
-    P->cnt.scatter_launches += P->graph_delta.scatter_launches;
-    st = FDB_OK;
-  } else {
-    st = jacobian_eager(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-  }
+  const GraphKey key{(void *)f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, P->n_peers, P->peer_generation, P->ext_eps};
+  const fdb_status st = run_maybe_graph(P, key, s, "Jacobian", [&](cudaStream_t cs) {
+    return jacobian_eager(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, cs);
+  });
   if (st == FDB_OK) P->cnt.jacobians += 1;
   return st;
 }
@@ -1855,7 +1870,8 @@ fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorv
 fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double absstep, double dir, double *d_eps_out,
                          void *stream) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP) return fail(FDB_ERR_INVALID, "fdb_color_eps needs a coloured plan");
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_HESS)
+    return fail(FDB_ERR_INVALID, "fdb_color_eps needs a coloured plan");
   if (P->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -1871,7 +1887,7 @@ fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double 
 
 fdb_status fdb_plan_set_external_eps(fdb_plan *P, const double *d_eps) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_EPS)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_EPS || P->sp_kind == SP_HESS)
     return fail(FDB_ERR_INVALID, "external step sizes apply to coloured Jacobian plans");
   P->ext_eps = d_eps;
   return FDB_OK;
@@ -1939,6 +1955,133 @@ fdb_status fdb_jvp(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double
   CU(cudaGetLastError());
   P->cnt.jacobians += 1;
   return FDB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Hessian (src/hessians.jl:202-292)
+// n above this would overflow the 64-bit sequence index 2n^2 + 1 long before any device could hold the work
+static constexpr int64_t kHessMaxN = (int64_t)1 << 24;
+// Cap on the points per f call.  scripts/hessian_bench.py's sweep at n = 1000 (fdbs_quartic; H100 80GB HBM3, 700 W; the
+// run's output line is scripts/hessian_bench_h100.json): 64 -> 451 ms, 256 -> 119 ms, 1024 -> 30.4 ms, 4096 -> 10.8 ms per
+// Hessian (requests above the cap are clamped to it).
+static constexpr int64_t kHessBatchCap = 4096;
+
+fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, const fdb_plan_opts *opts) {
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  if (!opts || opts->fdtype != FDB_HCENTRAL)   // @assert fdtype == Val(:hcentral)   hessians.jl:206
+    return fail(FDB_ERR_UNSUPPORTED, "finite_difference_hessian! supports fdtype = hcentral (%d) only", FDB_HCENTRAL);
+  if (n < 0) return fail(FDB_ERR_INVALID, "negative dimension n=%lld", (long long)n);
+  if (ldH < n) return fail(FDB_ERR_INVALID, "ldH < n");
+  if (n > kHessMaxN) return fail(FDB_ERR_UNSUPPORTED, "Hessian plans need n <= %lld", (long long)kHessMaxN);
+  if (opts->world > 1) return fail(FDB_ERR_UNSUPPORTED, "Hessian plans run on one device (world must be <= 1)");
+  fdb_plan_opts o = *opts;
+  o.fdtype = FDB_CENTRAL;   // new_plan validates the Jacobian fdtypes; the Hessian's is set below
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, &o, 1, n));
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  P->fdtype = FDB_HCENTRAL;
+  P->sp_kind = SP_HESS;
+  P->jkind = FDB_J_DENSE;
+  P->ldJ = ldH;
+  P->j_len = ldH * n;
+  P->E = n * n;
+  P->C = (int32_t)std::min<int64_t>(n, INT32_MAX);
+  P->col_begin = 0;
+  P->col_end = n;
+  P->ldF = 1;
+  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  const int64_t total = 2 * n * n + 1;
+  const int64_t budget = opts->scratch_bytes > 0 ? opts->scratch_bytes : (int64_t)8 << 30;
+  // ONE budget for both buffers: the resident point rows X[0..B) take at most half of it, the value buffer V the rest
+  int64_t batch = opts->max_batch > 1 ? opts->max_batch : 1;
+  batch = std::max<int64_t>(1, std::min<int64_t>(batch, budget / 2 / (8 * P->ldx)));
+  batch = std::min<int64_t>(std::min<int64_t>(batch, total), kHessBatchCap);
+  P->batch = batch;
+  P->slabs = batch;
+  // chunks of whole i-blocks whose values fit the budget (at least one i-block each), so that the <= 4 values of an
+  // entry are always in the same chunk
+  const int64_t cap = std::max<int64_t>((budget - batch * P->ldx * 8) / 8 - 1, 0);
+  P->hess_chunks.assign(1, 0);
+  int64_t max_vals = 0;
+  for (int64_t i0 = 0; i0 < n;) {
+    int64_t i1 = i0 + 1;
+    while (i1 < n && hess_block_start(i1 + 1, n) - hess_block_start(i0, n) <= cap) ++i1;
+    max_vals = std::max<int64_t>(max_vals, hess_block_start(i1, n) - hess_block_start(i0, n));
+    P->hess_chunks.push_back(i1);
+    i0 = i1;
+  }
+  if (n == 0) P->hess_chunks.push_back(0);   // one chunk of no i-blocks: f(x) alone
+  P->n_groups = (int64_t)P->hess_chunks.size() - 1;
+  TRY(P->alloc_t(&P->hess_V, (size_t)(1 + max_vals)));
+  TRY(P->alloc_t(&P->xp, (size_t)(batch * P->ldx)));
+  TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(n, 1)));
+  // byte model per Hessian: values read back by the assembly, H written, the one-time replication of x into the B rows,
+  // and the patches (each changed component written once and restored once: 2 per diagonal point, 4 per other point)
+  const int64_t patched = 2 * n + 8 * (n * (n - 1) / 2);
+  P->alg_bytes = 8 * total + 8 * n * n + 8 * n * batch + 16 * patched;
+  *plan = owner.release();
+  return FDB_OK;
+}
+
+static fdb_status hessian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *x, double *H, double *fx_out,
+                                double relstep, double absstep, cudaStream_t s) {
+  const int64_t n = P->n, ldx = P->ldx;
+  const int32_t B = (int32_t)P->batch;
+  if (n > 0) {
+    // eps_i = compute_epsilon(Val(:hcentral) / Val(:central), x_i, relstep, absstep) = max(relstep*|x_i|, absstep)  :223,234,252
+    component_eps<<<(int)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, 0, n, 1, relstep, absstep, 1.0, P->eps_cols);
+    replicate_x<<<P->grid(n), kThreads, 0, s>>>(x, n, ldx, B, P->xp);
+    P->cnt.kernel_launches += 2;
+  }
+  int64_t prev_p0 = 0;
+  int32_t prev_cnt = 0;
+  for (size_t c = 0; c + 1 < P->hess_chunks.size(); ++c) {
+    const int64_t i0 = P->hess_chunks[c], i1 = P->hess_chunks[c + 1];
+    const int64_t cs = hess_block_start(i0, n);
+    const int64_t p_end = hess_block_start(i1, n);
+    for (int64_t p0 = c == 0 ? 0 : cs; p0 < p_end; p0 += B) {
+      const int32_t cnt = (int32_t)std::min<int64_t>(B, p_end - p0);
+      if (n > 0) {
+        hess_patch<<<P->grid(std::max(cnt, prev_cnt)), kThreads, 0, s>>>(x, P->eps_cols, n, ldx, p0, cnt, prev_p0, prev_cnt, P->xp);
+        P->cnt.kernel_launches += 1;
+      }
+      // f(x) (:209), f(_xpp), f(_xmm) (:233), f(_xpp), f(_xpm), f(_xmp), f(_xmm) (:268-269), in this order
+      const int rc = f(ctx, P->hess_V + (p0 - cs + 1), P->xp, cnt, 1, ldx, (void *)s);
+      P->cnt.f_invocations += 1;
+      P->cnt.f_points += cnt;
+      if (rc != 0) return fail(FDB_ERR_CALLBACK, "user f returned %d", rc);
+      prev_p0 = p0;
+      prev_cnt = cnt;
+    }
+    const int64_t tiles = hess_tiles(n, i0, i1);
+    if (tiles > 0) {
+      ScatterTimer tm(P, s);
+      hess_assemble<<<P->grid(tiles, 1), kThreads, 0, s>>>(P->hess_V, P->eps_cols, n, i0, i1, tiles, H, P->ldJ);
+      P->cnt.kernel_launches += 1;
+      P->cnt.scatter_launches += 1;
+    }
+  }
+  if (fx_out) CU(cudaMemcpyAsync(fx_out, P->hess_V, 8, cudaMemcpyDeviceToDevice, s));
+  CU(cudaGetLastError());
+  return FDB_OK;
+}
+
+fdb_status fdb_hessian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_H, double *d_fx, double relstep,
+                       double absstep, void *stream) {
+  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  if (P->sp_kind != SP_HESS) return fail(FDB_ERR_INVALID, "not a Hessian plan (fdb_hessian_plan_create)");
+  if (P->n > 0 && (!d_x || !d_H)) return fail(FDB_ERR_INVALID, "NULL x or H");
+  DeviceGuard g(P->device);
+  if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  resolve_steps(FDB_HCENTRAL, relstep, absstep);                    // hessians.jl:204-205
+  const GraphKey key{(void *)f, ctx, d_x, d_H, d_fx, nullptr, relstep, absstep, 1.0, 0, 0, nullptr};
+  const fdb_status st = run_maybe_graph(P, key, s, "Hessian", [&](cudaStream_t cs) {
+    return hessian_eager(P, f, ctx, d_x, d_H, d_fx, relstep, absstep, cs);
+  });
+  if (st == FDB_OK) P->cnt.jacobians += 1;
+  return st;
 }
 
 fdb_status fdb_jacobian_host(fdb_plan *P, fdb_fn f, void *ctx, const double *h_x, double *h_J, double *h_fx,

@@ -194,6 +194,100 @@ __global__ void __launch_bounds__(kT) k_ellrows_c(double2 *__restrict__ fx, cons
   }
 }
 
+// ---- scalar functions f: R^n -> R (Hessian / gradient harness), one point per block.  Blocked order of k_block_sums:
+// 1024-element blocks, lane l of a warp sums the terms of elements l, l+32, ..., l+992 of its block ascending, an xor
+// butterfly adds the lanes, then thread 0 adds the block sums in block order.  Twins: scalar_oracle/synth_scalar.c.
+//   KIND 0 (quartic): f = sum_i (a_i x_i^4 + x_i x_{i+1}) + (sum_i w_i x_i)^2 / (2n)
+//   KIND 1 (sumsq):   f = sum_i x_i^2  (sum(abs2, x))
+__device__ __forceinline__ double butterfly(double s) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s = add(s, __shfl_xor_sync(0xffffffffu, s, o));
+  return s;
+}
+
+template <int KIND>
+__global__ void k_scalar(double *__restrict__ fx, const double *__restrict__ x, int64_t n, const double *__restrict__ a,
+                         const double *__restrict__ w, int64_t ldfx, int64_t ldx) {
+  extern __shared__ double sh[];   // [2][nblk] block sums
+  const double *xb = x + (int64_t)blockIdx.x * ldx;
+  const int64_t nblk = (n + 1023) / 1024;
+  const int lane = threadIdx.x & 31;
+  for (int64_t b = threadIdx.x >> 5; b < nblk; b += blockDim.x >> 5) {
+    double s1 = 0.0, s2 = 0.0;
+    for (int j = 0; j < 32; ++j) {
+      const int64_t i = b * 1024 + lane + 32 * j;
+      double t1 = 0.0, t2 = 0.0;
+      if (i < n) {
+        const double v = xb[i];
+        if (KIND == 0) {
+          const double q = mul(v, v);
+          t1 = mul(a[i], mul(q, q));
+          if (i + 1 < n) t1 = add(t1, mul(v, xb[i + 1]));
+          t2 = mul(w[i], v);
+        } else {
+          t1 = mul(v, v);
+        }
+      }
+      s1 = add(s1, t1);
+      s2 = add(s2, t2);
+    }
+    s1 = butterfly(s1);
+    s2 = butterfly(s2);
+    if (lane == 0) { sh[b] = s1; sh[nblk + b] = s2; }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double S1 = 0.0, S2 = 0.0;
+    for (int64_t b = 0; b < nblk; ++b) { S1 = add(S1, sh[b]); S2 = add(S2, sh[nblk + b]); }
+    fx[(int64_t)blockIdx.x * ldfx] = (KIND == 0 && n > 0) ? add(S1, __ddiv_rn(mul(S2, S2), (double)(2 * n))) : S1;
+  }
+}
+
+// complex128 twin of the quartic (complex-step gradients): the same sums on (re, im) with Julia's complex product
+// z*w = (zr*wr - zi*wi) + i(zr*wi + zi*wr); a_i, w_i and 2n are real
+__device__ __forceinline__ double2 cmul(double2 z, double2 v) {
+  return make_double2(sub(mul(z.x, v.x), mul(z.y, v.y)), add(mul(z.x, v.y), mul(z.y, v.x)));
+}
+
+__global__ void k_scalar_c(double2 *__restrict__ fx, const double2 *__restrict__ x, int64_t n, const double *__restrict__ a,
+                           const double *__restrict__ w, int64_t ldfx, int64_t ldx) {
+  extern __shared__ double sh[];   // [4][nblk]
+  const double2 *xb = x + (int64_t)blockIdx.x * ldx;
+  const int64_t nblk = (n + 1023) / 1024;
+  const int lane = threadIdx.x & 31;
+  for (int64_t b = threadIdx.x >> 5; b < nblk; b += blockDim.x >> 5) {
+    double s[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int j = 0; j < 32; ++j) {
+      const int64_t i = b * 1024 + lane + 32 * j;
+      double t[4] = {0.0, 0.0, 0.0, 0.0};
+      if (i < n) {
+        const double2 v = xb[i];
+        const double2 q = cmul(v, v), q2 = cmul(q, q);
+        double2 t1 = make_double2(mul(a[i], q2.x), mul(a[i], q2.y));
+        if (i + 1 < n) { const double2 u = cmul(v, xb[i + 1]); t1 = make_double2(add(t1.x, u.x), add(t1.y, u.y)); }
+        t[0] = t1.x; t[1] = t1.y; t[2] = mul(w[i], v.x); t[3] = mul(w[i], v.y);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) s[k] = add(s[k], t[k]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s[k] = butterfly(s[k]);
+    if (lane == 0) for (int k = 0; k < 4; ++k) sh[k * nblk + b] = s[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double S[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int64_t b = 0; b < nblk; ++b) for (int k = 0; k < 4; ++k) S[k] = add(S[k], sh[k * nblk + b]);
+    double2 f = make_double2(S[0], S[1]);
+    if (n > 0) {
+      const double2 sq = cmul(make_double2(S[2], S[3]), make_double2(S[2], S[3]));
+      const double d = (double)(2 * n);
+      f = make_double2(add(f.x, __ddiv_rn(sq.x, d)), add(f.y, __ddiv_rn(sq.y, d)));
+    }
+    fx[(int64_t)blockIdx.x * ldfx] = f;
+  }
+}
+
 __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t i) {
   uint64_t z = seed + (i + 1) * 0x9E3779B97F4A7C15ULL;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
@@ -340,6 +434,46 @@ int fdbs_rank1(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64
   const int vec_ok = (((uintptr_t)d_x | (uintptr_t)d_fx | (uintptr_t)c->d_w) & 15) == 0 && (ldx & 1) == 0 && (ldfx & 1) == 0;
   dim3 g2((unsigned)blocks_for((c->n + 3) / 4, 128), (unsigned)batch);
   k_rank1<<<g2, kT, 0, (cudaStream_t)stream>>>(d_fx, d_x, c->n, c->d_w, c->d_block_sums, nblk, ldfx, ldx, vec_ok);
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+// one block per point: a warp per 1024-block, up to 8 warps; the block sums stay in shared memory
+static int scalar_launch(const fdbs_scalar_ctx *c, int64_t batch, int words, unsigned *threads, size_t *smem) {
+  const int64_t nblk = (c->n + 1023) / 1024;
+  if (nblk * words * 8 > 48 * 1024) return 1;
+  *threads = 32u * (unsigned)(nblk < 1 ? 1 : (nblk > 8 ? 8 : nblk));
+  *smem = (size_t)(nblk * words * 8);
+  return batch < 1 || batch > 2147483647 ? 1 : 0;
+}
+
+int fdbs_quartic(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream) {
+  fdbs_scalar_ctx *c = (fdbs_scalar_ctx *)vctx;
+  unsigned threads;
+  size_t smem;
+  if (!c || c->n < 0 || (c->n > 0 && (!c->d_a || !c->d_w)) || scalar_launch(c, batch, 2, &threads, &smem)) return 1;
+  c->calls += batch;
+  k_scalar<0><<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>(d_fx, d_x, c->n, c->d_a, c->d_w, ldfx, ldx);
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+int fdbs_sumsq(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream) {
+  fdbs_scalar_ctx *c = (fdbs_scalar_ctx *)vctx;
+  unsigned threads;
+  size_t smem;
+  if (!c || c->n < 0 || scalar_launch(c, batch, 2, &threads, &smem)) return 1;
+  c->calls += batch;
+  k_scalar<1><<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>(d_fx, d_x, c->n, nullptr, nullptr, ldfx, ldx);
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+int fdbs_quartic_c(void *vctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream) {
+  fdbs_scalar_ctx *c = (fdbs_scalar_ctx *)vctx;
+  unsigned threads;
+  size_t smem;
+  if (!c || c->n < 0 || (c->n > 0 && (!c->d_a || !c->d_w)) || scalar_launch(c, batch, 4, &threads, &smem)) return 1;
+  c->calls += batch;
+  k_scalar_c<<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>((double2 *)d_fx, (const double2 *)d_x, c->n, c->d_a,
+                                                                       c->d_w, ldfx, ldx);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
 

@@ -17,16 +17,20 @@
 #     DeviceTridiagonal J (structured, COO) src/iteration_utils.jl:25-32 with ArrayInterface.findstructralnz
 #     CuMatrix J + dense 0/1 prototype      src/jacobians.jl:473-488, 526-527
 #     CuMatrix J, sparsity === nothing      src/jacobians.jl:548-557, 590-598 (dense column branch, colorvec quirk included)
-#   for Val(:forward), Val(:central) and Val(:complex) (src/jacobians.jl:623-648), plus the JVP and the multi-GPU group.
-# Everything else of FiniteDiff.jl (CPU arrays, gradients, hessians, out-of-place forms) keeps using the stock package.
+#   for Val(:forward), Val(:central) and Val(:complex) (src/jacobians.jl:623-648), plus the JVP and the multi-GPU group,
+#   and the vector -> scalar entry points on CuVector{Float64} x: finite_difference_hessian! (src/hessians.jl:202-292,
+#   fdb_hessian) and finite_difference_gradient! (src/gradients.jl:390-473, the dense plan with m = 1).
+# Everything else of FiniteDiff.jl (CPU arrays, complex x, scalar -> vector gradients, out-of-place forms) keeps using the
+# stock package.
 module FiniteDiffB200
 
 using FiniteDiff, SparseArrays, CUDA
-import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache
+import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache,
+    finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache
 
 const libfdjac = get(ENV, "FDJAC_B200_LIB", "libfdjac_b200.so")
 
-const FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX = Cint(0), Cint(1), Cint(2)
+const FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = Cint(0), Cint(1), Cint(2), Cint(3)
 const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS = Cint(0), Cint(1), Cint(2), Cint(3)
 const FDB_STEP_DEFAULT = NaN            # relstep / absstep keyword not given (include/fdjac_b200.h)
 
@@ -415,6 +419,61 @@ function finite_difference_jvp!(jvp::CuVector{Float64}, f, x::CuVector{Float64},
     check(rc)
     nothing
 end
+
+# ---- vector -> scalar: Hessian (src/hessians.jl:202-292) and gradient (src/gradients.jl:390-473) -------------------------
+# f(x) returns a scalar; the trampoline stores it at fx[b*ldfx] with a device-side fill (no host synchronisation when the
+# value is already on the device or a plain Number)
+scalar_f(f) = (fx, xv) -> (fx .= f(xv); nothing)
+
+function hessian_plan(H::CuMatrix{Float64}, n::Integer, ldH::Integer; kw...)
+    cached_plan(H, (:hessian, n, ldH, values(kw))) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(FDB_HCENTRAL; kw...))
+        check(ccall((:fdb_hessian_plan_create, libfdjac), Cint, (Ref{Ptr{Cvoid}}, Int64, Int64, Ref{PlanOpts}), h, n, ldH, opts))
+        Plan(h[], nothing)
+    end
+end
+
+function finite_difference_hessian!(H::CuMatrix{Float64}, f, x::CuVector{Float64}, cache::HessianCache{T, fdtype, inplace};
+        relstep = nothing, absstep = relstep) where {T, fdtype, inplace}
+    @assert fdtype == Val(:hcentral)                                   # hessians.jl:206
+    n = length(x)
+    size(H) == (n, n) || throw(DimensionMismatch("H must be $n x $n"))
+    plan = hessian_plan(H, n, ld(H))
+    st = FnState(scalar_f(f), 1, n, nothing)
+    cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+    rc = Cint(0)
+    GC.@preserve st H x begin
+        rc = ccall((:fdb_hessian, libfdjac), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, Float64, Float64, Ptr{Cvoid}),
+            plan.handle, cf, pointer_from_objref(st), pointer(x), pointer(H), CU_NULL, stepval(relstep), stepval(absstep),
+            CUDA.stream().handle)
+    end
+    st.err === nothing || throw(st.err)
+    check(rc)
+    H                                                                  # both triangles written (copytri!, :291)
+end
+
+finite_difference_hessian!(H::CuMatrix{Float64}, f, x::CuVector{Float64}, fdtype = Val(:hcentral), inplace = Val(true);
+        relstep = nothing, absstep = relstep) =
+    finite_difference_hessian!(H, f, x, HessianCache(x, fdtype, inplace); relstep = relstep, absstep = absstep)
+
+# the gradient is the dense column branch with m = 1 (gradients.jl:408-468 vs jacobians.jl:548-557, 590-598, 625-631):
+# df is J (1 x n, ldJ = 1); cache.fx, when given, is f_in (:410)
+function finite_difference_gradient!(df::CuVector{Float64}, f, x::CuVector{Float64},
+        cache::GradientCache{T1, T2, T3, T4, fdtype, returntype, inplace};
+        relstep = nothing, absstep = relstep, dir = true) where {T1, T2, T3, T4, fdtype, returntype, inplace}
+    n = length(x)
+    length(df) == n || throw(DimensionMismatch("length(df) != length(x)"))
+    plan = plan_dense(df, 1, n, 1, 1:n, fdcode(fdtype))
+    f_in = (fdtype == Val(:forward) && cache.fx !== nothing) ? CuArray(Float64[cache.fx]) : nothing
+    run_plan!(plan, df, scalar_f(f), x, nothing, f_in, 1, fdtype, relstep, absstep, dir)
+    df
+end
+
+finite_difference_gradient!(df::CuVector{Float64}, f, x::CuVector{Float64}, fdtype::Union{Type, Val} = Val(:central);
+        relstep = nothing, absstep = relstep, dir = true) =
+    finite_difference_gradient!(df, f, x, GradientCache(df, x, fdtype); relstep = relstep, absstep = absstep, dir = dir)
 
 # ---- several GPUs from ONE call: fdb_group_* (colours / dense column blocks partitioned over `devices`; devices[1] is the
 #      root and owns x, J, cache.fx; every member's scatter kernel stores its entries straight into the root's J).

@@ -48,8 +48,9 @@ typedef enum {
 
 /* fdtype — the Val(:forward)/Val(:central)/Val(:complex) type parameter of JacobianCache (jacobians.jl:1-9).
  * FDB_COMPLEX is the complex-step colour loop (jacobians.jl:623-648): x + im*eps, J = imag(f)/eps, eps = eps(Float64);
- * plans of that type are driven through fdb_jacobian_complex with a complex128 callback. */
-enum { FDB_FORWARD = 0, FDB_CENTRAL = 1, FDB_COMPLEX = 2 };
+ * plans of that type are driven through fdb_jacobian_complex with a complex128 callback.
+ * FDB_HCENTRAL is the Val(:hcentral) of HessianCache (hessians.jl:1-9): Hessian plans only (fdb_hessian_plan_create). */
+enum { FDB_FORWARD = 0, FDB_CENTRAL = 1, FDB_COMPLEX = 2, FDB_HCENTRAL = 3 };
 
 /* Where `J[row, col] = v` lands — what the reference decides by dispatch on typeof(J). */
 typedef enum {
@@ -313,6 +314,25 @@ fdb_status fdb_check_coloring_csc(int64_t m, int64_t n, const int64_t *colptr, c
 fdb_status fdb_jvp_plan_create(fdb_plan **plan, int64_t m, int64_t n, const fdb_plan_opts *opts);
 fdb_status fdb_jvp(fdb_plan *plan, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
                    double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream);
+
+/* ---- Hessian of a scalar f: finite_difference_hessian!(H, f, x, cache::HessianCache; relstep, absstep)
+ *      src/hessians.jl:202-292.  opts->fdtype must be FDB_HCENTRAL (else FDB_ERR_UNSUPPORTED, the reference's
+ *      @assert fdtype == Val(:hcentral), :206); H is dense column-major with leading dimension ldH >= n (else
+ *      FDB_ERR_INVALID).  max_batch: points per f call (at most 4096); scratch_bytes: one budget (0 => 8 GiB) for the point
+ *      rows (at most half of it) and the stacked f values (the rest, filled by whole i-blocks; at least one i-block, 8(4n-1)
+ *      bytes, whatever the budget); use_graph as for fdb_jacobian.  One device (world <= 1).
+ *
+ *      fdb_hessian evaluates f (the batched fdb_fn with m = 1: point b at d_x + b*ldx, its scalar to d_fx[b*ldfx]) at the
+ *      reference's 2n^2 + 1 points in the reference's order — f(x); then per i the pair x +- eps_i e_i and, per j > i,
+ *      (+,+), (+,-), (-,+), (-,-) on (i, j) — with eps_i = max(relstep*|x_i|, absstep) (:223,234,252), and writes
+ *        H[i,i] = ((f++ - 2 f(x)) + f--) / (eps_i*eps_i),  H[i,j] = H[j,i] = (((f++ - f+-) - f-+) + f--) / ((4 eps_i)*eps_j)
+ *      to rows [0, n) of every column (padding rows are not touched).  d_x is never modified; d_fx (nullable, one double)
+ *      receives f(x).  relstep / absstep: FDB_STEP_DEFAULT => eps(Float64)^(1/4) and absstep = relstep.
+ *      Stream-ordered, no host synchronisation.  fdb_plan_info: n_entries = n^2, fcalls_per_jacobian = 2n^2 + 1,
+ *      alg_bytes / moved_bytes the library's bytes per Hessian (values read back, H, point replication, patches). ---- */
+fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, const fdb_plan_opts *opts);
+fdb_status fdb_hessian(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, double *d_H, double *d_fx, double relstep,
+                       double absstep, void *stream);
 
 /* ---- helpers for hosts without their own CUDA bindings ---- */
 fdb_status fdb_host_alloc(void **p, size_t bytes);  /* pinned host memory */

@@ -9,6 +9,13 @@
  *   fdbs_lap5    : test/coloring_tests.jl:99-108  clamped 5-point stencil on a g x g grid (column-major)
  *   fdbs_ellrows : dx[i] = sum_p coef[p,i]*x[cols[p,i]] + 0.1*x[cols[0,i]]^2, ELL layout [K][m]   (SURVEY.md §8d config C4)
  *   fdbs_rank1   : dx[i] = x[i]^2 + w[i]*S, S = blocked-sum(x)/n                (SURVEY.md §8d config C5 variant)
+ *
+ * Scalar functions f: R^n -> R (m = 1: one value per point at d_fx[b*ldfx]) for Hessians and gradients, summed in the
+ * blocked order of fdbs_rank1's block sums; CPU twins in scalar_oracle/synth_scalar.c:
+ *   fdbs_quartic : f = sum_i (a[i] x[i]^4 + x[i] x[i+1]) + (sum_i w[i] x[i])^2 / (2n)
+ *                  Hessian diag(12 a[i] x[i]^2) + (1 on the first sub- and super-diagonal) + w w^T / n
+ *   fdbs_quartic_c : its complex128 twin (an fdb_fn_c), for complex-step gradients
+ *   fdbs_sumsq   : f = sum(abs2, x)
  */
 #ifndef FDJAC_SYNTH_H
 #define FDJAC_SYNTH_H
@@ -23,6 +30,8 @@ typedef struct { int64_t n; int64_t row0; int64_t nrows; int64_t x0; int64_t cal
 typedef struct { int64_t g; int64_t calls; } fdbs_lap5_ctx;
 typedef struct { int64_t m; int64_t K; const int32_t *d_cols; const double *d_coef; int64_t calls; } fdbs_ell_ctx;
 typedef struct { int64_t n; const double *d_w; double *d_block_sums; int64_t max_batch; int64_t calls; } fdbs_rank1_ctx;
+/* scalar functions: d_a / d_w are n doubles (device; unused by fdbs_sumsq); n <= 3 * 2^20 (3 * 2^19 for the complex twin) */
+typedef struct { int64_t n; const double *d_a; const double *d_w; int64_t calls; } fdbs_scalar_ctx;
 
 int fdbs_tridiag(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_tridiag_rows(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
@@ -34,6 +43,9 @@ int fdbs_ellrows(void *ctx, double *d_fx, const double *d_x, int64_t batch, int6
  * complex elements */
 int fdbs_ellrows_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_rank1(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_quartic(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_quartic_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_sumsq(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 /* a callback that always fails (error-path tests) */
 int fdbs_fail(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 
