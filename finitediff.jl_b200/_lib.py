@@ -128,6 +128,7 @@ SYNTH_SYMBOLS = {
     "fdbs_quartic": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_quartic_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_sumsq": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_guarded": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_fill_x": (_int, [_vp, _i64, C.c_uint64, _vp]),
     "fdbs_flush_l2": (_int, [_vp, _i64, _vp]),
 }

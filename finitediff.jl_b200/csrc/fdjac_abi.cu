@@ -117,7 +117,11 @@ struct DeviceGuard {
   }
 };
 
-// identity of a captured call: same function, buffers and scalar arguments => same launch sequence
+// identity of a captured call: same function, buffers and scalar arguments => same launch sequence.  The scalars are
+// compared by bit pattern: relstep = absstep = -0.0 gives the step -0.0, which keeps a -0.0 component of x negative where
+// the step +0.0 does not, so a graph captured with one must not be replayed for the other.
+static inline bool same_bits(double a, double b) { return std::memcmp(&a, &b, sizeof a) == 0; }
+
 struct GraphKey {
   void *f = nullptr, *ctx = nullptr;
   const void *x = nullptr, *J = nullptr, *fx = nullptr, *f_in = nullptr;
@@ -126,9 +130,9 @@ struct GraphKey {
   long long peer_generation = 0;
   const void *ext_eps = nullptr;
   bool operator==(const GraphKey &o) const {
-    return f == o.f && ctx == o.ctx && x == o.x && J == o.J && fx == o.fx && f_in == o.f_in && relstep == o.relstep &&
-           absstep == o.absstep && dir == o.dir && n_peers == o.n_peers && peer_generation == o.peer_generation &&
-           ext_eps == o.ext_eps;
+    return f == o.f && ctx == o.ctx && x == o.x && J == o.J && fx == o.fx && f_in == o.f_in &&
+           same_bits(relstep, o.relstep) && same_bits(absstep, o.absstep) && same_bits(dir, o.dir) &&
+           n_peers == o.n_peers && peer_generation == o.peer_generation && ext_eps == o.ext_eps;
   }
 };
 

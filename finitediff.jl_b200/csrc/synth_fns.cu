@@ -199,11 +199,17 @@ __global__ void __launch_bounds__(kT) k_ellrows_c(double2 *__restrict__ fx, cons
 // butterfly adds the lanes, then thread 0 adds the block sums in block order.  Twins: scalar_oracle/synth_scalar.c.
 //   KIND 0 (quartic): f = sum_i (a_i x_i^4 + x_i x_{i+1}) + (sum_i w_i x_i)^2 / (2n)
 //   KIND 1 (sumsq):   f = sum_i x_i^2  (sum(abs2, x))
+//   KIND 2 (guarded): f = sum_i (g(a_i x_i^4, 1/4) + g(x_i x_{i+1}, -1/2) + z_i) + s^2 / (2n),
+//                     s = g(sum_i g(w_i x_i, 3/4), 3/2),  z_i = (!isnan(x_i) && signbit(x_i)) ? w_i : 0,
+//                     g(t, c) = (isfinite(t) && |t| <= 2^500) ? t : c
+//                     finite for every input; depends on the sign of a zero, never on a NaN's sign or payload
 __device__ __forceinline__ double butterfly(double s) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s = add(s, __shfl_xor_sync(0xffffffffu, s, o));
   return s;
 }
+
+__device__ __forceinline__ double guard(double t, double c) { return (isfinite(t) && fabs(t) <= 0x1p500) ? t : c; }
 
 template <int KIND>
 __global__ void k_scalar(double *__restrict__ fx, const double *__restrict__ x, int64_t n, const double *__restrict__ a,
@@ -224,6 +230,12 @@ __global__ void k_scalar(double *__restrict__ fx, const double *__restrict__ x, 
           t1 = mul(a[i], mul(q, q));
           if (i + 1 < n) t1 = add(t1, mul(v, xb[i + 1]));
           t2 = mul(w[i], v);
+        } else if (KIND == 2) {
+          const double q = mul(v, v);
+          t1 = guard(mul(a[i], mul(q, q)), 0.25);
+          if (i + 1 < n) t1 = add(t1, guard(mul(v, xb[i + 1]), -0.5));
+          t1 = add(t1, (!isnan(v) && signbit(v)) ? w[i] : 0.0);
+          t2 = guard(mul(w[i], v), 0.75);
         } else {
           t1 = mul(v, v);
         }
@@ -239,7 +251,12 @@ __global__ void k_scalar(double *__restrict__ fx, const double *__restrict__ x, 
   if (threadIdx.x == 0) {
     double S1 = 0.0, S2 = 0.0;
     for (int64_t b = 0; b < nblk; ++b) { S1 = add(S1, sh[b]); S2 = add(S2, sh[nblk + b]); }
-    fx[(int64_t)blockIdx.x * ldfx] = (KIND == 0 && n > 0) ? add(S1, __ddiv_rn(mul(S2, S2), (double)(2 * n))) : S1;
+    if (KIND == 2) {
+      const double s = guard(S2, 1.5);
+      fx[(int64_t)blockIdx.x * ldfx] = n > 0 ? add(S1, __ddiv_rn(mul(s, s), (double)(2 * n))) : S1;
+    } else {
+      fx[(int64_t)blockIdx.x * ldfx] = (KIND == 0 && n > 0) ? add(S1, __ddiv_rn(mul(S2, S2), (double)(2 * n))) : S1;
+    }
   }
 }
 
@@ -463,6 +480,16 @@ int fdbs_sumsq(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64
   if (!c || c->n < 0 || scalar_launch(c, batch, 2, &threads, &smem)) return 1;
   c->calls += batch;
   k_scalar<1><<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>(d_fx, d_x, c->n, nullptr, nullptr, ldfx, ldx);
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+int fdbs_guarded(void *vctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream) {
+  fdbs_scalar_ctx *c = (fdbs_scalar_ctx *)vctx;
+  unsigned threads;
+  size_t smem;
+  if (!c || c->n < 0 || (c->n > 0 && (!c->d_a || !c->d_w)) || scalar_launch(c, batch, 2, &threads, &smem)) return 1;
+  c->calls += batch;
+  k_scalar<2><<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>(d_fx, d_x, c->n, c->d_a, c->d_w, ldfx, ldx);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
 

@@ -91,8 +91,9 @@ typedef struct {
                               launch per group of L2-resident f! outputs, overlapped with the next group's f!; 3 colour-major
                               lists with every f! output resident: one launch at the end (see fdb_plan_info_t.strategy) */
   int32_t use_graph;       /* 1: capture the whole call (library kernels + the callback's launches) into a CUDA graph on
-                              first use and replay it while (f, ctx, buffers, scalars) stay the same.  The callback must
-                              be capture-safe: enqueue-only on the given stream, no allocation, no host-side state. */
+                              first use and replay it while (f, ctx, buffers, scalars) stay the same (the scalars bit for
+                              bit: a step of -0.0 is not the step +0.0).  The callback must be capture-safe:
+                              enqueue-only on the given stream, no allocation, no host-side state. */
   int32_t shared_j;        /* 1: the J passed to fdb_jacobian is SHARED with other ranks' plans (a peer-mapped pointer to one
                               buffer, e.g. rank 0's): this plan only stores the entries / columns it owns and never zero-fills
                               J — the owner of the buffer zero-fills it (when the scatter is not self-defining) and orders

@@ -16,6 +16,11 @@
  *                  Hessian diag(12 a[i] x[i]^2) + (1 on the first sub- and super-diagonal) + w w^T / n
  *   fdbs_quartic_c : its complex128 twin (an fdb_fn_c), for complex-step gradients
  *   fdbs_sumsq   : f = sum(abs2, x)
+ *   fdbs_guarded : the quartic with every term guarded, g(t, c) = (isfinite(t) && |t| <= 2^500) ? t : c, plus a
+ *                  signed-zero term: f = sum_i (g(a[i] x[i]^4, 1/4) + g(x[i] x[i+1], -1/2) + z[i]) + s^2 / (2n),
+ *                  s = g(sum_i g(w[i] x[i], 3/4), 3/2), z[i] = (!isnan(x[i]) && signbit(x[i])) ? w[i] : 0.
+ *                  Finite for every double x, so an IEEE edge value in x[k] leaves the entries of H that do not
+ *                  involve k finite; sees the sign of a zero but never the sign or payload of a NaN.
  */
 #ifndef FDJAC_SYNTH_H
 #define FDJAC_SYNTH_H
@@ -46,6 +51,7 @@ int fdbs_rank1(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_
 int fdbs_quartic(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_quartic_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_sumsq(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_guarded(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 /* a callback that always fails (error-path tests) */
 int fdbs_fail(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 

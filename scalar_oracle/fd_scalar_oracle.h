@@ -39,6 +39,7 @@ double fdso_default_relstep(int fdtype);   /* epsilons.jl:134-144; fdtype 3 = hc
 typedef struct { int64_t n; const double *a; const double *w; } synth_scalar_ctx;
 double synth_quartic(void *ctx, const double *x);
 double synth_sumsq(void *ctx, const double *x);
+double synth_guarded(void *ctx, const double *x);
 void synth_quartic_c(void *ctx, const double *x, double *out);
 
 #endif

@@ -61,6 +61,8 @@ def lib():
         L.synth_quartic.argtypes = [C.c_void_p, _f64p]
         L.synth_sumsq.restype = C.c_double
         L.synth_sumsq.argtypes = [C.c_void_p, _f64p]
+        L.synth_guarded.restype = C.c_double
+        L.synth_guarded.argtypes = [C.c_void_p, _f64p]
         L.synth_quartic_c.restype = None
         L.synth_quartic_c.argtypes = [C.c_void_p, _f64p, _f64p]
         _lib = L
@@ -80,21 +82,24 @@ def default_relstep(fdtype: int) -> float:
 
 
 class SynthScalar:
-    """CPU twin of fdbs_quartic / fdbs_sumsq / fdbs_quartic_c: keeps a and w alive with the ctx struct."""
+    """CPU twin of fdbs_quartic / fdbs_sumsq / fdbs_guarded / fdbs_quartic_c: keeps a and w alive with the ctx struct.
+    Calling it evaluates `name` (default: synth_quartic when a is given, else synth_sumsq)."""
 
-    def __init__(self, n, a=None, w=None):
+    def __init__(self, n, a=None, w=None, name=None):
         self.n = int(n)
         self.a = None if a is None else np.ascontiguousarray(a, dtype=np.float64)
         self.w = None if w is None else np.ascontiguousarray(w, dtype=np.float64)
         self.ctx = SynthScalarCtx(self.n, _p(self.a), _p(self.w))
+        self.name = name or ("synth_quartic" if self.a is not None else "synth_sumsq")
 
     def native(self, name: str):
-        """(function address, ctx) for the oracle entry points: name = synth_quartic / synth_sumsq / synth_quartic_c."""
+        """(function address, ctx) for the oracle entry points: name = synth_quartic / synth_sumsq / synth_guarded /
+        synth_quartic_c."""
         return C.cast(getattr(lib(), name), C.c_void_p), C.cast(C.pointer(self.ctx), C.c_void_p)
 
     def __call__(self, x) -> float:
         x = np.ascontiguousarray(x, dtype=np.float64)
-        return lib().synth_quartic(C.byref(self.ctx), _p(x)) if self.a is not None else lib().synth_sumsq(C.byref(self.ctx), _p(x))
+        return getattr(lib(), self.name)(C.byref(self.ctx), _p(x))
 
 
 def _fn(f, n, complex_=False):

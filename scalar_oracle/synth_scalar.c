@@ -4,6 +4,7 @@
  * o = 16, 8, 4, 2, 1; block sums are added in block order.  -ffp-contract=off keeps every operation a single rounding. */
 #include "fd_scalar_oracle.h"
 
+#include <math.h>
 #include <stddef.h>
 
 static void butterfly(double s[32]) {
@@ -45,6 +46,17 @@ static void quartic_terms(const synth_scalar_ctx *c, const double *x, int64_t i,
   t[1] = c->w[i] * v;
 }
 
+/* g(t, c) of fdbs_guarded: a term that is not finite or exceeds 2^500 in magnitude is replaced by c */
+static double guard(double t, double c) { return (isfinite(t) && fabs(t) <= 0x1p500) ? t : c; }
+
+static void guarded_terms(const synth_scalar_ctx *c, const double *x, int64_t i, double *t) {
+  const double v = x[i], q = v * v;
+  t[0] = guard(c->a[i] * (q * q), 0.25);
+  if (i + 1 < c->n) t[0] = t[0] + guard(v * x[i + 1], -0.5);
+  t[0] = t[0] + ((!isnan(v) && signbit(v)) ? c->w[i] : 0.0);
+  t[1] = guard(c->w[i] * v, 0.75);
+}
+
 static void sumsq_terms(const synth_scalar_ctx *c, const double *x, int64_t i, double *t) {
   (void)c;
   t[0] = x[i] * x[i];
@@ -78,6 +90,14 @@ double synth_quartic(void *ctx, const double *x) {
   double S[2];
   blocked(c, x, 2, quartic_terms, S);
   return c->n > 0 ? S[0] + (S[1] * S[1]) / (double)(2 * c->n) : S[0];
+}
+
+double synth_guarded(void *ctx, const double *x) {
+  const synth_scalar_ctx *c = (const synth_scalar_ctx *)ctx;
+  double S[2];
+  blocked(c, x, 2, guarded_terms, S);
+  const double s = guard(S[1], 1.5);
+  return c->n > 0 ? S[0] + (s * s) / (double)(2 * c->n) : S[0];
 }
 
 double synth_sumsq(void *ctx, const double *x) {

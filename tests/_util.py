@@ -126,6 +126,144 @@ def ell_c_numpy(cols, coef, x):
     return re, im
 
 
+def max_julia(a, b):
+    """Julia's max on Float64: NaN propagates (as a - b), otherwise b when a - b is negative (so max(-0.0, 0.0) = 0.0)."""
+    if np.isnan(a) or np.isnan(b):
+        return np.float64(a - b)
+    return b if np.signbit(np.float64(a - b)) else a
+
+
+def hessian_transcribed(f, x, relstep=None, absstep=None):
+    """hessians.jl:202-292, one Python line per Julia line (numpy float64 scalars: IEEE, one rounding per operation).
+    Returns (H, f(x), every point f was called with)."""
+    f64 = np.float64
+    relstep = f64(2.0 ** -13) if relstep is None else f64(relstep)
+    absstep = relstep if absstep is None else f64(absstep)
+    points = []
+
+    def F(v):
+        points.append(v.copy())
+        return f64(f(v.copy()))
+
+    n = len(x)
+    H = np.zeros((n, n))
+    fx = F(x)
+    xpp, xpm, xmp, xmm = x.copy(), x.copy(), x.copy(), x.copy()
+    with np.errstate(all="ignore"):
+        for i in range(n):
+            xi = x[i]
+            epsilon = max_julia(relstep * abs(xi), absstep)
+            xpp[i] = xi + epsilon
+            xmm[i] = xi - epsilon
+            a = F(xpp)
+            b = F(xmm)
+            H[i, i] = (a - f64(2) * fx + b) / (epsilon * epsilon)
+            epsiloni = max_julia(relstep * abs(xi), absstep)
+            xp = xi + epsiloni
+            xm = xi - epsiloni
+            xpp[i], xpm[i], xmp[i], xmm[i] = xp, xp, xm, xm
+            for j in range(i + 1, n):
+                xj = x[j]
+                epsilonj = max_julia(relstep * abs(xj), absstep)
+                xp = xj + epsilonj
+                xm = xj - epsilonj
+                xpp[j], xpm[j], xmp[j], xmm[j] = xp, xm, xp, xm
+                a, b, c, d = F(xpp), F(xpm), F(xmp), F(xmm)
+                H[i, j] = (a - b - c + d) / (f64(4) * epsiloni * epsilonj)
+                xpp[j], xpm[j], xmp[j], xmm[j] = xj, xj, xj, xj
+            xpp[i], xpm[i], xmp[i], xmm[i] = xi, xi, xi, xi
+        for i in range(n):
+            for j in range(i + 1, n):
+                H[j, i] = H[i, j]
+    return H, fx, points
+
+
+def gradient_transcribed(f, x, fdtype, fx=None, relstep=None, absstep=None, dir=1.0):
+    """gradients.jl:390-457 (real x, real df; fdtype 0 forward, 1 central), one Python line per Julia line.
+    Returns (df, every point f was called with)."""
+    f64 = np.float64
+    eps = np.finfo(float).eps
+    if relstep is None:
+        relstep = f64(np.sqrt(eps)) if fdtype == 0 else f64(np.cbrt(eps))
+    absstep = relstep if absstep is None else f64(absstep)
+    relstep = f64(relstep)
+    points = []
+
+    def F(v):
+        points.append(v.copy())
+        return f64(f(v.copy()))
+
+    n = len(x)
+    df = np.zeros(n)
+    c3 = x.copy()
+    with np.errstate(all="ignore"):
+        if fdtype == 0:
+            fx0 = f64(fx) if fx is not None else F(x)
+            for i in range(n):
+                epsilon = max_julia(relstep * abs(x[i]), absstep) * f64(dir)
+                x_old = x[i]
+                c3[i] += epsilon
+                dfi = (F(c3) - fx0) / epsilon
+                c3[i] = x_old
+                df[i] = dfi
+        else:
+            for i in range(n):
+                epsilon = max_julia(relstep * abs(x[i]), absstep)
+                x_old = x[i]
+                c3[i] += epsilon
+                dfi = F(c3)
+                c3[i] = x_old - epsilon
+                dfi -= F(c3)
+                c3[i] = x_old
+                df[i] = dfi / (f64(2) * epsilon)
+    return df, points
+
+
+def blocked_sum(t):
+    """Sum of the float64 vector t in the blocked order of the synthetic scalar functions (fdbs_quartic and its twins):
+    1024-element blocks; lane l (of 32) adds elements l, l+32, ..., l+992 of its block in ascending order, starting from
+    0.0 (0.0 past the end); an xor butterfly s[l] = s[l] + s[l ^ o], o = 16, 8, 4, 2, 1; block sums added in block order."""
+    t = np.asarray(t, dtype=np.float64)
+    nblk = -(-t.size // 1024)
+    T = np.zeros(nblk * 1024)
+    T[:t.size] = t
+    T = T.reshape(nblk, 32, 32)                       # [block, j, lane] = element block*1024 + 32 j + lane
+    s = np.zeros((nblk, 32))
+    for j in range(32):
+        s = s + T[:, j, :]
+    lanes = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        s = s + s[:, lanes ^ o]
+    S = np.float64(0.0)
+    for b in range(nblk):
+        S = S + s[b, 0]
+    return S
+
+
+def _guard(t, c):
+    return np.where(np.isfinite(t) & (np.abs(t) <= 2.0 ** 500), t, np.float64(c))
+
+
+def guarded_numpy(x, a, w):
+    """fdbs_guarded (include/fdjac_synth.h) evaluated with numpy, independently of its C twin synth_guarded:
+    f = sum_i (g(a_i x_i^4, 1/4) + g(x_i x_{i+1}, -1/2) + z_i) + s^2 / (2n), s = g(sum_i g(w_i x_i, 3/4), 3/2),
+    z_i = (!isnan(x_i) && signbit(x_i)) ? w_i : 0, g(t, c) = (isfinite(t) && |t| <= 2^500) ? t : c."""
+    x = np.asarray(x, dtype=np.float64)
+    n = x.size
+    with np.errstate(all="ignore"):
+        q = x * x
+        t1 = _guard(a * (q * q), 0.25)
+        if n > 1:
+            t1[:-1] = t1[:-1] + _guard(x[:-1] * x[1:], -0.5)
+        t1 = t1 + np.where(~np.isnan(x) & np.signbit(x), w, 0.0)
+        t2 = _guard(w * x, 0.75)
+        S1, S2 = blocked_sum(t1), blocked_sum(t2)
+        if n == 0:
+            return S1
+        s = np.float64(_guard(S2, 1.5))
+        return S1 + (s * s) / np.float64(2 * n)
+
+
 def tridiagonal_coo(n):
     """Structural nz of Julia's Tridiagonal(dl,d,du) as (rows, cols, slots) with slots into [dl; d; du]
     (1-based): band order sub-diagonal, diagonal, super-diagonal."""

@@ -54,13 +54,17 @@ def traced(fn):
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        # once the profiler has sat idle for a minute or so in a process, the first few kernel records of the next
-        # session can be missing from its trace: throwaway launches take those places
+        # kernel records at either end of a session can be missing from its trace: the first few once the profiler has
+        # sat idle for a minute or so in a process, the last one when the session stops right after it (seen for the
+        # staged scatter, the last launch of a forward call).  Throwaway launches take those places on both sides.
         pad = torch.empty(1, device="cuda")
         for _ in range(64):
             pad.fill_(0.0)
         torch.cuda.synchronize()
         fn()
+        torch.cuda.synchronize()
+        for _ in range(64):
+            pad.fill_(0.0)
         torch.cuda.synchronize()
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "trace.json")

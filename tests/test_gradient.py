@@ -9,7 +9,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from _util import assert_same_bits
+from _util import assert_same_bits, gradient_transcribed
 from scalar_oracle import fd_scalar_oracle as so
 
 f64 = np.float64
@@ -56,50 +56,6 @@ def test_kat_gradient_of_sum_is_ones(soracle):
     for fd in (so.FORWARD, so.CENTRAL):
         np.testing.assert_allclose(soracle.gradient(lambda v: float(np.sum(v)), np.ones(2), fd)["df"], np.ones(2))
     np.testing.assert_allclose(soracle.gradient(lambda v: complex(np.sum(v)), np.ones(2), so.COMPLEX)["df"], np.ones(2))
-
-
-def _max_julia(a, b):
-    if np.isnan(a) or np.isnan(b):
-        return f64(a - b)
-    return b if np.signbit(f64(a - b)) else a
-
-
-def gradient_transcribed(f, x, fdtype, fx=None, relstep=None, absstep=None, dir=1.0):
-    """gradients.jl:390-457 (real x, real df), one Python line per Julia line."""
-    if relstep is None:
-        relstep = f64(np.sqrt(EPS)) if fdtype == 0 else f64(np.cbrt(EPS))
-    absstep = relstep if absstep is None else f64(absstep)
-    relstep = f64(relstep)
-    points = []
-
-    def F(v):
-        points.append(v.copy())
-        return f64(f(v.copy()))
-
-    n = len(x)
-    df = np.zeros(n)
-    c3 = x.copy()
-    with np.errstate(all="ignore"):
-        if fdtype == 0:
-            fx0 = f64(fx) if fx is not None else F(x)
-            for i in range(n):
-                epsilon = _max_julia(relstep * abs(x[i]), absstep) * f64(dir)
-                x_old = x[i]
-                c3[i] += epsilon
-                dfi = (F(c3) - fx0) / epsilon
-                c3[i] = x_old
-                df[i] = dfi
-        else:
-            for i in range(n):
-                epsilon = _max_julia(relstep * abs(x[i]), absstep)
-                x_old = x[i]
-                c3[i] += epsilon
-                dfi = F(c3)
-                c3[i] = x_old - epsilon
-                dfi -= F(c3)
-                c3[i] = x_old
-                df[i] = dfi / (f64(2) * epsilon)
-    return df, points
 
 
 EDGES = [0.0, -0.0, np.nan, np.inf, -np.inf, 1e-320, 5e-324, 1e300, -1e300, 1.0]

@@ -11,7 +11,7 @@ import os
 import numpy as np
 import pytest
 
-from _util import assert_same_bits
+from _util import assert_same_bits, hessian_transcribed
 from scalar_oracle import fd_scalar_oracle as so
 
 f64 = np.float64
@@ -59,55 +59,6 @@ def test_default_relstep_is_eps_quarter(soracle):
 
 
 # ------------------------------------------------------------------------------------------------ transcription (CPU)
-def _max_julia(a, b):
-    if np.isnan(a) or np.isnan(b):
-        return f64(a - b)
-    return b if np.signbit(f64(a - b)) else a
-
-
-def hessian_transcribed(f, x, relstep=None, absstep=None):
-    """hessians.jl:202-292, one Python line per Julia line (numpy float64 scalars: IEEE, one rounding per operation)."""
-    relstep = f64(2.0 ** -13) if relstep is None else f64(relstep)
-    absstep = relstep if absstep is None else f64(absstep)
-    points = []
-
-    def F(v):
-        points.append(v.copy())
-        return f64(f(v.copy()))
-
-    n = len(x)
-    H = np.zeros((n, n))
-    fx = F(x)
-    xpp, xpm, xmp, xmm = x.copy(), x.copy(), x.copy(), x.copy()
-    with np.errstate(all="ignore"):
-        for i in range(n):
-            xi = x[i]
-            epsilon = _max_julia(relstep * abs(xi), absstep)
-            xpp[i] = xi + epsilon
-            xmm[i] = xi - epsilon
-            a = F(xpp)
-            b = F(xmm)
-            H[i, i] = (a - f64(2) * fx + b) / (epsilon * epsilon)
-            epsiloni = _max_julia(relstep * abs(xi), absstep)
-            xp = xi + epsiloni
-            xm = xi - epsiloni
-            xpp[i], xpm[i], xmp[i], xmm[i] = xp, xp, xm, xm
-            for j in range(i + 1, n):
-                xj = x[j]
-                epsilonj = _max_julia(relstep * abs(xj), absstep)
-                xp = xj + epsilonj
-                xm = xj - epsilonj
-                xpp[j], xpm[j], xmp[j], xmm[j] = xp, xm, xp, xm
-                a, b, c, d = F(xpp), F(xpm), F(xmp), F(xmm)
-                H[i, j] = (a - b - c + d) / (f64(4) * epsiloni * epsilonj)
-                xpp[j], xpm[j], xmp[j], xmm[j] = xj, xj, xj, xj
-            xpp[i], xpm[i], xmp[i], xmm[i] = xi, xi, xi, xi
-        for i in range(n):
-            for j in range(i + 1, n):
-                H[j, i] = H[i, j]
-    return H, fx, points
-
-
 EDGES = [0.0, -0.0, np.nan, np.inf, -np.inf, 1e-320, -1e-320, 5e-324, 1e300, -1e300, 1e-160, 1.0, -2.5]
 
 
@@ -251,6 +202,12 @@ def test_gpu_hessian_reduced_grid(pkg, sm, monkeypatch, tmp_path):
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         H, _, _, _ = _device_H(pkg, q, max_batch=64)
+        # the last kernel record of a session can be missing from its trace when the session stops right after it, and
+        # hess_assemble is the last launch: throwaway launches take that place
+        pad = torch.empty(1, device="cuda")
+        for _ in range(64):
+            pad.fill_(0.0)
+        torch.cuda.synchronize()
     assert_same_bits(H.cpu().numpy(), _oracle_run(q)["H"], f"FDB_SM_COUNT={sm}", allow_nan=False)
     trace = tmp_path / "trace.json"
     prof.export_chrome_trace(str(trace))
