@@ -102,6 +102,10 @@ ABI_SYMBOLS = {
     "fdb_jvp": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
     "fdb_hessian_plan_create": (_int, [_PP, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_hessian": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _vp]),
+    "fdb_derivative_plan_create": (_int, [_PP, _i64, C.POINTER(PlanOpts)]),
+    "fdb_scalar_gradient_plan_create": (_int, [_PP, _i64, C.POINTER(PlanOpts)]),
+    "fdb_derivative": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
+    "fdb_derivative_complex": (_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "fdb_host_alloc": (_int, [_PP, C.c_size_t]),
     "fdb_host_free": (_int, [_vp]),
     "fdb_device_alloc": (_int, [_PP, C.c_size_t]),
@@ -129,6 +133,14 @@ SYNTH_SYMBOLS = {
     "fdbs_quartic_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_sumsq": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_guarded": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_poly": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_poly_guarded": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_poly_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_poly_guarded_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_tpoly": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_tpoly_guarded": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_tpoly_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "fdbs_tpoly_guarded_c": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp]),
     "fdbs_fill_x": (_int, [_vp, _i64, C.c_uint64, _vp]),
     "fdbs_flush_l2": (_int, [_vp, _i64, _vp]),
 }

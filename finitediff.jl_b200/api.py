@@ -19,6 +19,8 @@ All compute happens in libfdjac_b200.so; there is no eager/CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
+import warnings
 import weakref
 import zlib
 from typing import Callable, Optional
@@ -32,7 +34,8 @@ __all__ = [
     "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "BandedBlockBandedMatrix", "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
     "finite_difference_jacobian_", "finite_difference_jacobian_b", "resize_", "default_relstep", "compute_epsilon",
     "zeros_colmajor", "pinned_empty", "HessianCache", "finite_difference_hessian_", "finite_difference_hessian",
-    "GradientCache", "finite_difference_gradient_", "finite_difference_gradient",
+    "GradientCache", "finite_difference_gradient_", "finite_difference_gradient", "DerivativeCache",
+    "finite_difference_derivative_", "finite_difference_derivative",
 ]
 
 _DEFAULT = object()
@@ -375,10 +378,13 @@ class _PyFn:
     (batch, m) / (batch, n) tensors; otherwise they are called once per point with 1-D tensors."""
 
     def __init__(self, f: Callable, m: int, n: int, device: torch.device, batched: bool, complex_: bool = False,
-                 scalar: bool = False):
+                 scalar: bool = False, elementwise: bool = False, tvec: bool = False):
         self.f, self.m, self.n, self.device, self.batched = f, m, n, device, batched
         # scalar (m = 1) functions are called as f(x) and RETURN their value (a 0-d CUDA tensor needs no host sync)
         self.scalar = scalar
+        # elementwise functions (derivatives) are called as f(x) and return a tensor of x's shape; scalar -> vector
+        # functions (tvec, n = 1) are called in place as f(fx, t) with t a 0-d tensor
+        self.elementwise, self.tvec = elementwise, tvec
         self.exc: Optional[BaseException] = None
         self.calls = 0
         # complex-step callbacks (fdb_fn_c) see complex128 tensors; ld* then count complex elements
@@ -396,7 +402,18 @@ class _PyFn:
                 es = self.esize
                 fx2 = torch.as_tensor(_DevArray(p_fx, (batch, self.m), (ldfx * es, es), self.typestr), device=self.device)
                 x2 = torch.as_tensor(_DevArray(p_x, (batch, self.n), (ldx * es, es), self.typestr), device=self.device)
-                if self.scalar and self.batched:
+                if self.elementwise and self.batched:
+                    self.calls += int(batch)
+                    fx2.copy_(torch.as_tensor(self.f(x2), dtype=fx2.dtype, device=self.device))
+                elif self.elementwise:
+                    for b in range(int(batch)):
+                        self.calls += 1
+                        fx2[b].copy_(torch.as_tensor(self.f(x2[b]), dtype=fx2.dtype, device=self.device))
+                elif self.tvec:
+                    for b in range(int(batch)):
+                        self.calls += 1
+                        self.f(fx2[b], x2[b, 0])
+                elif self.scalar and self.batched:
                     self.calls += int(batch)
                     # dtype of the slot (float64 / complex128): a Python float or complex must not pass through
                     # torch's default float32 / complex64
@@ -790,10 +807,10 @@ def check_coloring(A: "SparseMatrixCSC", colorvec) -> int:
 
 
 # ------------------------------------------------------------------------------------------------ the public call
-def _as_fn(f, m, n, device, plan_batch, complex_=False, scalar=False):
+def _as_fn(f, m, n, device, plan_batch, complex_=False, scalar=False, **kind):
     if isinstance(f, NativeFn):
         return f.address, f.ctx_ptr, None
-    w = _PyFn(f, m, n, device, bool(getattr(f, "batched", False)), complex_, scalar)
+    w = _PyFn(f, m, n, device, bool(getattr(f, "batched", False)), complex_, scalar, **kind)
     return L.fn_address(w.cfunc), None, w
 
 
@@ -1097,11 +1114,21 @@ def finite_difference_hessian(f, x, cache=None, *, relstep=None, absstep=None, s
 
 
 # ------------------------------------------------------------------------------------------------ gradient (src/gradients.jl)
+def _is_number(x) -> bool:
+    """x is a scalar input in the reference's sense (x::Number): a Python / numpy number.  (A tensor t is passed to a
+    cache built for the scalar -> vector case.)"""
+    return isinstance(x, numbers.Number)
+
+
 class GradientCache:
-    """Mirror of FiniteDiff.GradientCache (gradients.jl:1-7) for the vector -> scalar case on real Float64 arrays:
+    """Mirror of FiniteDiff.GradientCache (gradients.jl:1-7) on real Float64 arrays:
 
         GradientCache(df, x, fdtype="central", returntype=float64)     allocating, fx = nothing   (:19-62)
         GradientCache(fx, c1, c2, c3, fdtype="central", returntype)    non-allocating             (:104-123)
+
+    x an array: the vector -> scalar gradient.  x a number: the scalar -> vector gradient of an in-place
+    f(fx, t) (:50-59: c1, c2 = zero(df), complex mode c1 = complex zero(df), c3 = x); the non-allocating form is scalar
+    -> vector when c3 is a number.  Its fx, when given, is the m values f(x) and is used in forward mode (:501-502).
 
     A gradient is the dense column branch of the Jacobian with m = 1 (gradients.jl:408-468 against jacobians.jl:548-557,
     590-598, 625-631): the same steps, points, quotients and call order.  The GPU path therefore runs a dense Jacobian
@@ -1112,16 +1139,33 @@ class GradientCache:
         arrays = list(arrays)
         if arrays and isinstance(arrays[-1], str):
             fdtype = arrays.pop()
+        self.scalar_x = False
         if len(arrays) == 2:
             df, x = arrays
-            for t, name in ((df, "df"), (x, "x")):
-                if not isinstance(t, torch.Tensor):
-                    raise TypeError(f"{name} must be a CUDA tensor (the scalar -> vector form is not supported)")
-                if t.is_complex():
-                    raise TypeError(f"{name} must be real Float64: complex-valued gradients are not supported")
-            self.fx, self.c1, self.c2, self.c3 = None, None, None, torch.zeros_like(x)
+            if _is_number(x):
+                # the scalar -> vector case (:50-59)
+                _real_input(x)
+                if not isinstance(df, torch.Tensor) or not df.is_cuda:
+                    raise TypeError("df must be a float64 CUDA tensor: the GPU path has no CPU implementation")
+                if df.is_complex() or df.dtype != torch.float64:
+                    raise TypeError("df must be real Float64: complex-valued gradients are not supported")
+                self.scalar_x = True
+                complex_mode = isinstance(fdtype, str) and fdtype.lstrip(":") == "complex" or fdtype == L.FDB_COMPLEX
+                if complex_mode:
+                    self.fx, self.c1, self.c2 = None, torch.zeros(df.shape, dtype=torch.complex128, device=df.device), None
+                else:
+                    self.fx, self.c1, self.c2 = None, torch.zeros_like(df), torch.zeros_like(df)
+                self.c3 = x
+            else:
+                for t, name in ((df, "df"), (x, "x")):
+                    if not isinstance(t, torch.Tensor):
+                        raise TypeError(f"{name} must be a CUDA tensor or x a number")
+                    if t.is_complex():
+                        raise TypeError(f"{name} must be real Float64: complex-valued gradients are not supported")
+                self.fx, self.c1, self.c2, self.c3 = None, None, None, torch.zeros_like(x)
         elif len(arrays) == 4:
             self.fx, self.c1, self.c2, self.c3 = arrays
+            self.scalar_x = _is_number(self.c3)
         else:
             raise TypeError("GradientCache(df, x[, fdtype]) or GradientCache(fx, c1, c2, c3[, fdtype])")
         if returntype not in (torch.float64, float, np.float64):
@@ -1141,18 +1185,36 @@ class GradientCache:
             p = self._plans[key] = Plan(h.value)
         return p
 
+    def scalar_plan_for(self, m: int, device) -> Plan:
+        key = ("scalar", m, str(device))
+        p = self._plans.get(key)
+        if p is None:
+            h = C.c_void_p()
+            o = _opts(_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
+            L.check(L.lib().fdb_scalar_gradient_plan_create(C.byref(h), m, C.byref(o)))
+            p = self._plans[key] = Plan(h.value)
+        return p
+
 
 def finite_difference_gradient_(df, f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None):
     """finite_difference_gradient!(df, f, x, cache::GradientCache; relstep, absstep, dir) (gradients.jl:390-473), or —
     when `cache` is None or an fdtype string — the cache-less form (:220-248).
 
-    df, x: float64 CUDA vectors of length n (complex arrays and a Number x are rejected with TypeError).
+    df, x: float64 CUDA vectors of length n (complex arrays are rejected with TypeError).
     f: Python callable f(x) -> scalar as for finite_difference_hessian_ (complex step: f receives complex128 x and
-       returns a complex scalar), or a NativeFn (fdb_fn with m = 1; fdb_fn_c for complex).  Returns None."""
+       returns a complex scalar), or a NativeFn (fdb_fn with m = 1; fdb_fn_c for complex).
+
+    Scalar -> vector (gradients.jl:477-533): x a number (or, with a scalar -> vector cache, a 1-element
+    float64 CUDA tensor: the device slot is read by the call, so a captured graph follows t written in place); df the m
+    outputs.  f: in-place f(fx, t) with fx a CUDA row of m values and t a 0-d CUDA tensor (float64, complex128 in complex
+    mode), or a NativeFn (fdb_fn with n = 1 and m outputs; fdb_fn_c for complex).  A number t is staged into one
+    cache-owned device slot on the call's stream.  Returns None."""
     if cache is None or isinstance(cache, str):
         cache = GradientCache(df, x, cache or "central")
     if not isinstance(cache, GradientCache):
         raise TypeError("cache must be a GradientCache, an fdtype string, or None")
+    if cache.scalar_x or _is_number(x):
+        return _scalar_gradient_(df, f, x, cache, relstep, absstep, dir, stream)
     if not isinstance(x, torch.Tensor) or not isinstance(df, torch.Tensor):
         raise TypeError("x and df must be CUDA tensors (the scalar -> vector form is not supported)")
     xv = _scalar_x(x)
@@ -1198,11 +1260,222 @@ def finite_difference_gradient_(df, f, x, cache=None, *, relstep=None, absstep=N
     return None
 
 
-def finite_difference_gradient(f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None):
+def finite_difference_gradient(f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None, fx=None, c1=None,
+                               c2=None):
     """finite_difference_gradient(f, x[, cache | fdtype]; relstep, absstep, dir) (gradients.jl:168-218, :250-300): a new
-    float64 CUDA vector df."""
+    float64 CUDA vector df.
+
+    Scalar x (a number, or a 1-element tensor with a scalar -> vector cache): the scalar -> vector gradient of an in-place f(fx, t).  With a cache, df has
+    the cache's m outputs.  Cache-less, one of fx, c1, c2 (CUDA tensors of m values) must be given to size df (:185-195);
+    as in the reference it only sizes df — the cache is built without it, so forward mode still evaluates f(x)."""
+    if (isinstance(cache, GradientCache) and cache.scalar_x) or _is_number(x):
+        if isinstance(cache, GradientCache):
+            proto = cache.c1 if isinstance(cache.c1, torch.Tensor) else cache.fx
+            if not isinstance(proto, torch.Tensor):
+                raise TypeError("a scalar -> vector GradientCache needs c1 or fx as a CUDA tensor to size df")
+        else:
+            proto = next((a for a in (c1, fx, c2) if a is not None), None)      # :188-194
+            if proto is None:                                                  # :186
+                raise TypeError("In the scalar->vector in-place map case, at least one of fx, c1 or c2 must be provided, "
+                                "otherwise we cannot infer the return size.")
+            if not isinstance(proto, torch.Tensor) or not proto.is_cuda:
+                raise TypeError("fx / c1 / c2 must be CUDA tensors: the GPU path has no CPU implementation")
+        df = torch.zeros(proto.numel(), dtype=torch.float64, device=proto.device)
+        finite_difference_gradient_(df, f, x, cache, relstep=relstep, absstep=absstep, dir=dir, stream=stream)
+        return df
     if not isinstance(x, torch.Tensor):
-        raise TypeError("x must be a CUDA tensor (the scalar -> vector form is not supported)")
+        raise TypeError("x must be a CUDA tensor or a real number")
     df = torch.zeros(x.numel(), dtype=torch.float64, device=x.device)
     finite_difference_gradient_(df, f, x, cache, relstep=relstep, absstep=absstep, dir=dir, stream=stream)
     return df
+
+
+def _real_input(x):
+    if isinstance(x, torch.Tensor):
+        if x.is_complex() or x.dtype != torch.float64:
+            raise TypeError("x must be real Float64: complex-valued x is not supported")
+        if not x.is_cuda:
+            raise TypeError("x must be a CUDA tensor or a number: the GPU path has no CPU implementation")
+    elif isinstance(x, complex) or not isinstance(x, numbers.Real):
+        raise TypeError("x must be a real number: complex-valued x is not supported")
+
+
+def _call_result(st, pyfn):
+    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
+        exc, pyfn.exc = pyfn.exc, None
+        raise exc
+    L.check(st)
+
+
+def _steps(relstep, absstep):
+    return (L.STEP_DEFAULT if relstep is None else float(relstep), L.STEP_DEFAULT if absstep is None else float(absstep))
+
+
+def _flat_f64(t, what):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise TypeError(f"{what} must be a float64 CUDA tensor: the GPU path has no CPU implementation")
+    if t.is_complex() or t.dtype != torch.float64:
+        raise TypeError(f"{what} must be real Float64 (complex-valued arrays are not supported)")
+    if not t.is_contiguous():
+        raise ValueError(f"{what} must be contiguous")
+    return t.reshape(-1)
+
+
+_SLOTS = {}
+
+
+def _fx_ptr(fxv):
+    """Device pointer of a given cache.fx.  An empty one has no storage (data_ptr 0, which the ABI reads as "not given"),
+    so it is passed as a valid one-element slot: nothing is read from it, and f(x) is not evaluated."""
+    if fxv.numel():
+        return fxv.data_ptr()
+    slot = _SLOTS.get(fxv.device)
+    if slot is None:
+        slot = _SLOTS[fxv.device] = torch.zeros(1, dtype=torch.float64, device=fxv.device)
+    return slot.data_ptr()
+
+
+def _scalar_gradient_(df, f, x, cache, relstep, absstep, dir, stream):
+    """finite_difference_gradient!(df, f, x::Number, cache) (gradients.jl:477-533) through fdb_derivative."""
+    _real_input(x)
+    dv = _flat_f64(df, "df")
+    m = dv.numel()
+    if isinstance(cache.c1, torch.Tensor) and cache.c1.numel() != m:
+        raise ValueError(f"length(df)={m} != the cache's {cache.c1.numel()} outputs")
+    dev = dv.device
+    fd = _fdtype_code(cache.fdtype)
+    if isinstance(x, torch.Tensor):
+        if x.numel() != 1 or x.device != dev:
+            raise ValueError("a tensor t must hold one float64 value on df's device")
+        tv = _flat_f64(x, "x")
+    else:
+        tv = None
+    plan = cache.scalar_plan_for(m, dev)
+    addr, ctx, pyfn = _as_fn(f, m, 1, dev, 1, fd == L.FDB_COMPLEX, tvec=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+    if tv is None:
+        # a number: staged in ONE device slot kept on the cache, so the arguments of the call (and a captured graph's key
+        # under use_graph) stay the same from call to call
+        tv = getattr(cache, "_t", None)
+        if tv is None or tv.device != dev:
+            tv = cache._t = torch.empty(1, dtype=torch.float64, device=dev)
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=dev)):
+            tv.fill_(float(x))
+    with torch.cuda.device(dev):
+        if fd == L.FDB_COMPLEX:
+            st = L.lib().fdb_derivative_complex(plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(), C.c_void_p(stream))
+        else:
+            fx_ptr = None
+            if fd == L.FDB_FORWARD and cache.fx is not None:                  # :501-502
+                fxv = _flat_f64(cache.fx, "cache.fx")
+                if fxv.numel() != m or fxv.device != dev:
+                    raise ValueError("cache.fx must hold the m values f(x) on df's device")
+                fx_ptr = _fx_ptr(fxv)
+            st = L.lib().fdb_derivative(plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(), fx_ptr,
+                                        *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
+    _call_result(st, pyfn)
+    cache._last_plan = plan
+    return None
+
+
+# ------------------------------------------------------------------------------------------------ derivative (src/derivatives.jl)
+class DerivativeCache:
+    """Mirror of FiniteDiff.DerivativeCache (derivatives.jl:38-88):
+
+        DerivativeCache(x, fx=None, epsilon=None, fdtype="central", returntype=float64)
+
+    fx (n values f(x)) is kept in forward mode only; otherwise it is dropped with a warning (:67-73).  epsilon is allocated
+    (zeros like x) when not given or of another dtype, and dropped with a warning in complex mode (:78-86); the StridedArray
+    path never reads or writes it.  Complex mode with a non-real returntype is fdtype_error (:63-65).  Extra keywords (GPU
+    path only): max_batch (2: both central points in one f call), use_graph."""
+
+    def __init__(self, x, fx=None, epsilon=None, fdtype="central", returntype=torch.float64, **plan_kw):
+        if isinstance(fx, str):
+            fdtype, fx = fx, None
+        elif isinstance(epsilon, str):
+            fdtype, epsilon = epsilon, None
+        self.fdtype = fdtype.lstrip(":") if isinstance(fdtype, str) else fdtype
+        code = _fdtype_code(self.fdtype)
+        if returntype in (torch.complex128, torch.complex64, complex, np.complex128):
+            if code == L.FDB_COMPLEX:                                          # :63-65
+                raise ValueError(f"Unrecognized fdtype for returntype {returntype}: complex step needs a real return type")
+            raise TypeError("complex-valued derivatives are not supported: only Float64")
+        if returntype not in (torch.float64, float, np.float64):
+            raise TypeError("only Float64 is supported by the GPU path")
+        _flat_f64(x, "x")
+        if code != L.FDB_FORWARD and fx is not None:                            # :67-70
+            warnings.warn("Pre-computed function values are only useful for fdtype==Val(:forward).")
+            fx = None
+        if epsilon is not None and code == L.FDB_COMPLEX:                       # :78-80
+            warnings.warn("Val(:complex) makes the epsilon array redundant.")
+            epsilon = None
+        elif epsilon is None or not isinstance(epsilon, torch.Tensor) or epsilon.dtype != torch.float64:   # :82-84
+            epsilon = torch.zeros_like(x)
+        self.fx, self.epsilon = fx, epsilon
+        self._code = code
+        self._plan_kw = plan_kw
+        self._plans = {}
+
+    def plan_for(self, n: int, device) -> Plan:
+        key = (n, str(device))
+        p = self._plans.get(key)
+        if p is None:
+            h = C.c_void_p()
+            o = _opts(self._code, _device_index(device), **self._plan_kw)
+            L.check(L.lib().fdb_derivative_plan_create(C.byref(h), n, C.byref(o)))
+            p = self._plans[key] = Plan(h.value)
+        return p
+
+
+def finite_difference_derivative_(df, f, x, cache="central", returntype=None, fx=None, epsilon=None, *, relstep=None,
+                                  absstep=None, dir=True, stream=None):
+    """finite_difference_derivative!(df, f, x::StridedArray, cache::DerivativeCache; relstep, absstep, dir)
+    (derivatives.jl:197-233), or — when `cache` is None or an fdtype string — the cache-less form
+    finite_difference_derivative!(df, f, x, fdtype, returntype, fx, epsilon; relstep, absstep) (:133-146).
+
+    df, x: contiguous float64 CUDA tensors of the same size; x is never modified.
+    f: elementwise scalar function as a Python callable applied to a whole CUDA tensor, returning a tensor of its shape
+       (torch.sin works; complex step: complex128 in and out; set f.batched = True to receive a (batch, n) tensor), or a
+       NativeFn (fdb_fn with m = n evaluated elementwise; fdb_fn_c for complex).  Returns df."""
+    if cache is None or isinstance(cache, str):
+        cache = DerivativeCache(x, fx, epsilon, cache or "central", returntype or torch.float64)
+    if not isinstance(cache, DerivativeCache):
+        raise TypeError("cache must be a DerivativeCache, an fdtype string, or None")
+    xv = _flat_f64(x, "x")
+    dv = _flat_f64(df, "df")
+    n = xv.numel()
+    if dv.numel() != n:
+        raise ValueError(f"length(df)={dv.numel()} != length(x)={n}")
+    if dv.device != xv.device:
+        raise ValueError("df and x must be on the same device")
+    plan = cache.plan_for(n, xv.device)
+    addr, ctx, pyfn = _as_fn(f, n, n, xv.device, 1, cache._code == L.FDB_COMPLEX, elementwise=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(xv.device).cuda_stream
+    with torch.cuda.device(xv.device):
+        if cache._code == L.FDB_COMPLEX:
+            st = L.lib().fdb_derivative_complex(plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(), C.c_void_p(stream))
+        else:
+            fx_ptr = None
+            if cache._code == L.FDB_FORWARD and cache.fx is not None:          # :213-214
+                fxv = _flat_f64(cache.fx, "cache.fx")
+                if fxv.numel() != n or fxv.device != xv.device:
+                    raise ValueError("cache.fx must hold the n values f(x) on x's device")
+                fx_ptr = _fx_ptr(fxv)
+            st = L.lib().fdb_derivative(plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(), fx_ptr,
+                                        *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
+    _call_result(st, pyfn)
+    cache._last_plan = plan
+    return df
+
+
+def finite_difference_derivative(f, x, cache="central", returntype=None, fx=None, epsilon=None, *, relstep=None,
+                                 absstep=None, dir=True, stream=None):
+    """finite_difference_derivative(f, x::StridedArray[, fdtype | cache, returntype, fx, epsilon]; relstep, absstep)
+    (derivatives.jl:104-116): a new float64 CUDA tensor of x's shape."""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("x must be a float64 CUDA tensor (the single-point derivative is not provided)")
+    df = torch.zeros(x.shape, dtype=torch.float64, device=x.device)
+    return finite_difference_derivative_(df, f, x, cache, returntype, fx, epsilon, relstep=relstep, absstep=absstep,
+                                         dir=dir, stream=stream)

@@ -30,6 +30,7 @@
 #include "kernels_jvp.cuh"
 #include "kernels_color.cuh"
 #include "kernels_hessian.cuh"
+#include "kernels_derivative.cuh"
 
 using namespace fdb;
 
@@ -59,7 +60,7 @@ static fdb_status fail(fdb_status st, const char *fmt, ...) {
     if (s__ != FDB_OK) return s__;   \
   } while (0)
 
-enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7 };
+enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7, SP_DERIV = 8 };
 
 // Device memory that lives while a plan or a colouring is built: freed when it goes out of scope, unless release()
 // hands it to a plan that keeps it (fdb_plan::adopt).  Declared after the builder's DeviceGuard, it is freed on the
@@ -227,6 +228,9 @@ struct fdb_plan {
   // boundaries [hess_chunks[c], hess_chunks[c+1]) in i
   double *hess_V = nullptr;
   std::vector<int64_t> hess_chunks;
+  // derivative plans (kernels_derivative.cuh): elementwise derivative (m = n) or scalar -> vector gradient (n = 1)
+  bool deriv_elem = false;
+  int64_t deriv_fcalls = 0;   // f evaluations of the most recent call (before any: the count without cache.fx)
   // host-buffer path
   cudaStream_t hstream = nullptr;
   double *h_dx = nullptr, *h_dJ = nullptr, *h_dfx = nullptr, *h_dfin = nullptr;
@@ -1156,6 +1160,7 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   info->slabs = P->slabs;
   info->fcalls_per_jacobian = P->fdtype == FDB_CENTRAL ? 2 * n_local : (P->fdtype == FDB_COMPLEX ? n_local : 1 + n_local);
   if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = 2 * P->n * P->n + 1;
+  if (P->sp_kind == SP_DERIV) info->fcalls_per_jacobian = P->deriv_fcalls;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
   info->jkind = P->jkind;
@@ -1209,6 +1214,7 @@ fdb_status fdb_plan_dense_range(const fdb_plan *P, int64_t *b, int64_t *e) {
 fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t cap) {
   if (!P || !owner_out) return fail(FDB_ERR_INVALID, "NULL argument");
   if (P->sp_kind == SP_NONE || P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "dense plans partition columns by range");
+  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "derivative plans have no colours");
   if (cap < (int64_t)P->owner.size()) return fail(FDB_ERR_INVALID, "owner_out too small");
   std::copy(P->owner.begin(), P->owner.end(), owner_out);
   return FDB_OK;
@@ -1216,6 +1222,7 @@ fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t c
 
 fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *stream) {
   if (!P || !h_eps) return fail(FDB_ERR_INVALID, "NULL argument");
+  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "derivative plans keep no step sizes (the quotient pass recomputes them)");
   DeviceGuard g(P->device);
   // JVP plans: C == 1; Hessian plans: one step per component (col_begin = 0, col_end = n)
   const bool per_column = P->sp_kind == SP_NONE || P->sp_kind == SP_HESS;
@@ -1257,7 +1264,7 @@ fdb_status fdb_plan_read_timing(fdb_plan *P, double *scatter_ms, int64_t *scatte
 fdb_status fdb_plan_set_peers(fdb_plan *P, int n_peers, double *const *peer_J) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
   if (n_peers < 0 || n_peers > 64) return fail(FDB_ERR_INVALID, "n_peers out of range");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_HESS)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_HESS || P->sp_kind == SP_DERIV)
     return fail(FDB_ERR_UNSUPPORTED, "peer stores are implemented for the entry-driven (CSC / COO) scatters");
   DeviceGuard g(P->device);
   if (!P->d_peers) TRY(P->alloc_t(&P->d_peers, 64));
@@ -1827,6 +1834,7 @@ fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, dou
   if (P->sp_kind == SP_JVP) return fail(FDB_ERR_INVALID, "this is a JVP plan: call fdb_jvp");
   if (P->sp_kind == SP_EPS) return fail(FDB_ERR_INVALID, "this is a step-size plan: call fdb_color_eps");
   if (P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian plan: call fdb_hessian");
+  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "this is a derivative plan: call fdb_derivative");
   if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
     return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
   DeviceGuard g(P->device);
@@ -1874,7 +1882,7 @@ fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorv
 fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double absstep, double dir, double *d_eps_out,
                          void *stream) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_HESS)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_HESS || P->sp_kind == SP_DERIV)
     return fail(FDB_ERR_INVALID, "fdb_color_eps needs a coloured plan");
   if (P->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
   DeviceGuard g(P->device);
@@ -1891,7 +1899,8 @@ fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double 
 
 fdb_status fdb_plan_set_external_eps(fdb_plan *P, const double *d_eps) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_EPS || P->sp_kind == SP_HESS)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_EPS || P->sp_kind == SP_HESS ||
+      P->sp_kind == SP_DERIV)
     return fail(FDB_ERR_INVALID, "external step sizes apply to coloured Jacobian plans");
   P->ext_eps = d_eps;
   return FDB_OK;
@@ -2088,9 +2097,141 @@ fdb_status fdb_hessian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, doub
   return st;
 }
 
+// ------------------------------------------------------------------------------------------------ derivatives with a
+// scalar input per step size (src/derivatives.jl:197-233, src/gradients.jl:477-533; kernels_derivative.cuh)
+// Scratch: the point rows xp (two rows of ldx doubles: x+eps and x-eps; complex: one complex128 row) and the f outputs
+// F (two rows of ldF doubles: f(x+eps) and f(x) / f(x-eps); complex: one complex128 row).
+static fdb_status create_derivative(fdb_plan **plan, int64_t m, int64_t n, bool elem, const fdb_plan_opts *opts) {
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  if (opts && opts->fdtype == FDB_HCENTRAL)
+    return fail(FDB_ERR_UNSUPPORTED, "derivative plans take fdtype forward, central or complex (hcentral is for Hessians)");
+  if (opts && opts->world > 1) return fail(FDB_ERR_UNSUPPORTED, "derivative plans run on one device (world must be <= 1)");
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  P->sp_kind = SP_DERIV;
+  P->deriv_elem = elem;
+  P->jkind = FDB_J_DENSE;
+  P->E = m;
+  P->j_len = m;
+  P->ldJ = std::max<int64_t>(m, 1);
+  P->batch = opts && opts->max_batch > 1 ? 2 : 1;
+  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  P->ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
+  TRY(P->alloc_t(&P->xp, (size_t)(2 * P->ldx)));
+  TRY(P->alloc_t(&P->Fp, (size_t)(2 * P->ldF)));
+  P->Fm = P->Fp + P->ldF;
+  P->deriv_fcalls = P->fdtype == FDB_COMPLEX ? 1 : 2;
+  // compulsory bytes per call: points pass (x read; one, two or one complex row written) + quotient pass (f rows and,
+  // elementwise, x read; df written).  Complex reads the whole complex128 f row and no x.
+  const int64_t pts = P->fdtype == FDB_FORWARD ? 16 : 24;
+  const int64_t q = P->fdtype == FDB_COMPLEX || !elem ? 24 : 32;
+  P->alg_bytes = pts * n + q * m;
+  *plan = owner.release();
+  return FDB_OK;
+}
+
+fdb_status fdb_derivative_plan_create(fdb_plan **plan, int64_t n, const fdb_plan_opts *opts) {
+  return create_derivative(plan, n, n, true, opts);
+}
+
+fdb_status fdb_scalar_gradient_plan_create(fdb_plan **plan, int64_t m, const fdb_plan_opts *opts) {
+  return create_derivative(plan, m, 1, false, opts);
+}
+
+}  // extern "C"
+
+template <int MODE>
+static fdb_status derivative_eager(fdb_plan *P, fdb_fn f, void *ctx, double *df, const double *x, const double *fx,
+                                   const DerivSteps &st, cudaStream_t s) {
+  const int64_t n = P->n, m = P->m;
+  const int al_x = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const int64_t tiles_n = (n + kTile - 1) / kTile, tiles_m = (m + kTile - 1) / kTile;
+  if (n > 0) {
+    deriv_points<MODE><<<resident_grid(P, deriv_points<MODE>, 0, tiles_n), kThreads, 0, s>>>(x, n, P->ldx, P->xp, st, al_x);
+    P->cnt.kernel_launches += 1;
+  }
+  // f-call order of the reference: f(x+eps) first, then f(x) (forward without fx) or f(x-eps) (central)
+  //   derivatives.jl:209-215,219-222 (per element) / gradients.jl:495-509,513-515
+  int64_t calls = 1;
+  const double *fb = nullptr;
+  if (MODE == kCentral && P->batch >= 2) {
+    TRY(call_f(P, f, ctx, P->Fp, P->xp, 2, s));                       // both points in one call: rows 0 (+) and 1 (-)
+    calls = 2;
+    fb = P->Fm;
+  } else {
+    TRY(call_f(P, f, ctx, P->Fp, P->xp, 1, s));
+    if (MODE == kCentral) {
+      TRY(call_f(P, f, ctx, P->Fm, P->xp + P->ldx, 1, s));
+      calls = 2;
+      fb = P->Fm;
+    } else if (MODE == kForward) {
+      if (fx) fb = fx;
+      else { TRY(call_f(P, f, ctx, P->Fm, x, 1, s)); calls = 2; fb = P->Fm; }
+    }
+  }
+  P->deriv_fcalls = calls;
+  if (m > 0) {
+    const uintptr_t al = reinterpret_cast<uintptr_t>(df) | (fb ? reinterpret_cast<uintptr_t>(fb) : 0) |
+                         (P->deriv_elem && MODE != kComplex ? reinterpret_cast<uintptr_t>(x) : 0);
+    const int aligned = (al & 15) == 0;
+    ScatterTimer tm(P, s);
+    if (P->deriv_elem)
+      deriv_quotient<MODE, true><<<resident_grid(P, deriv_quotient<MODE, true>, 0, tiles_m), kThreads, 0, s>>>(
+          P->Fp, fb, x, df, m, st, aligned);
+    else
+      deriv_quotient<MODE, false><<<resident_grid(P, deriv_quotient<MODE, false>, 0, tiles_m), kThreads, 0, s>>>(
+          P->Fp, fb, x, df, m, st, aligned);
+    P->cnt.kernel_launches += 1;
+    P->cnt.scatter_launches += 1;
+  }
+  CU(cudaGetLastError());
+  return FDB_OK;
+}
+
+extern "C" {
+
+fdb_status fdb_derivative(fdb_plan *P, fdb_fn f, void *ctx, double *d_df, const double *d_x, const double *d_fx,
+                          double relstep, double absstep, double dir, void *stream) {
+  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  if (P->sp_kind != SP_DERIV)
+    return fail(FDB_ERR_INVALID, "not a derivative plan (fdb_derivative_plan_create / fdb_scalar_gradient_plan_create)");
+  if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
+    return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_derivative_complex with a complex128 callback");
+  if ((P->n > 0 && !d_x) || (P->m > 0 && !d_df)) return fail(FDB_ERR_INVALID, "NULL x or df");
+  DeviceGuard g(P->device);
+  if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  resolve_steps(P->fdtype, relstep, absstep);                       // relstep = default_relstep(fdtype), absstep = relstep
+  const double *fx = P->fdtype == FDB_FORWARD ? d_fx : nullptr;     // cache.fx is read in forward mode only
+  const DerivSteps st{relstep, absstep, dir};
+  const GraphKey key{(void *)f, ctx, d_x, d_df, fx, nullptr, relstep, absstep, dir, 0, 0, nullptr};
+  const fdb_status rc = run_maybe_graph(P, key, s, "derivative", [&](cudaStream_t cs) {
+    if (P->fdtype == FDB_CENTRAL) return derivative_eager<kCentral>(P, f, ctx, d_df, d_x, fx, st, cs);
+    if (P->fdtype == FDB_COMPLEX) return derivative_eager<kComplex>(P, f, ctx, d_df, d_x, fx, st, cs);
+    return derivative_eager<kForward>(P, f, ctx, d_df, d_x, fx, st, cs);
+  });
+  if (rc == FDB_OK) P->cnt.jacobians += 1;
+  return rc;
+}
+
+fdb_status fdb_derivative_complex(fdb_plan *P, fdb_fn_c f, void *ctx, double *d_df, const double *d_x, void *stream) {
+  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  if (P->sp_kind != SP_DERIV || P->fdtype != FDB_COMPLEX)
+    return fail(FDB_ERR_INVALID, "fdb_derivative_complex needs a derivative plan created with fdtype = FDB_COMPLEX");
+  P->complex_entry = true;
+  const fdb_status st = fdb_derivative(P, reinterpret_cast<fdb_fn>(f), ctx, d_df, d_x, nullptr, FDB_STEP_DEFAULT,
+                                       FDB_STEP_DEFAULT, 1.0, stream);
+  P->complex_entry = false;
+  return st;
+}
+
 fdb_status fdb_jacobian_host(fdb_plan *P, fdb_fn f, void *ctx, const double *h_x, double *h_J, double *h_fx,
                              const double *h_f_in, double relstep, double absstep, double dir) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "this is a derivative plan: call fdb_derivative");
   if ((P->n > 0 && !h_x) || (P->j_len > 0 && !h_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);

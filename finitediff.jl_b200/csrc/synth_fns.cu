@@ -305,6 +305,56 @@ __global__ void k_scalar_c(double2 *__restrict__ fx, const double2 *__restrict__
   }
 }
 
+// ---- elementwise and scalar-input functions (derivative / scalar -> vector gradient harness), one output per thread.
+// Output i of point b:  p_i(v) = (a_i (v^2 v) + w_i v^2) + v  with v = x[b*ldx + i] (SCALAR = false: elementwise, for
+// finite_difference_derivative!) or v = x[b*ldx] (SCALAR = true: m outputs of one scalar t, for the scalar -> vector
+// gradient).  GUARD: every term through guard(), plus z = (!isnan(v) && signbit(v)) ? w_i : 0, so p_i is finite for every
+// v and sees the sign of a zero.  Twins: scalar_oracle/synth_scalar.c.
+template <bool GUARD>
+__device__ __forceinline__ double poly_at(double v, double a, double w) {
+  const double q = mul(v, v), c = mul(q, v);
+  if (!GUARD) return add(add(mul(a, c), mul(w, q)), v);
+  const double t = add(add(guard(mul(a, c), 0.25), guard(mul(w, q), -0.5)), guard(v, 0.75));
+  return add(t, (!isnan(v) && signbit(v)) ? w : 0.0);
+}
+
+template <bool GUARD, bool SCALAR>
+__global__ void __launch_bounds__(kT) k_poly(double *__restrict__ fx, const double *__restrict__ x, int64_t n,
+                                             const double *__restrict__ a, const double *__restrict__ w, int64_t ldfx,
+                                             int64_t ldx) {
+  const double *xb = x + (int64_t)blockIdx.y * ldx;
+  double *fb = fx + (int64_t)blockIdx.y * ldfx;
+  for (int64_t i = blockIdx.x * (int64_t)kT + threadIdx.x; i < n; i += (int64_t)gridDim.x * kT)
+    fb[i] = poly_at<GUARD>(SCALAR ? xb[0] : xb[i], a[i], w[i]);
+}
+
+// complex128 twin: the same terms with Julia's complex product; a_i, w_i real.  GUARD: guard() on the real and the
+// imaginary part of each term, and z (from the sign of the real part) added to the IMAGINARY part, the one a complex step
+// reads.
+template <bool GUARD>
+__device__ __forceinline__ double2 poly_at_c(double2 v, double a, double w) {
+  const double2 q = cmul(v, v), c = cmul(q, v);
+  double2 t1 = make_double2(mul(a, c.x), mul(a, c.y)), t2 = make_double2(mul(w, q.x), mul(w, q.y)), t3 = v;
+  if (GUARD) {
+    t1 = make_double2(guard(t1.x, 0.25), guard(t1.y, 0.25));
+    t2 = make_double2(guard(t2.x, -0.5), guard(t2.y, -0.5));
+    t3 = make_double2(guard(t3.x, 0.75), guard(t3.y, 0.75));
+  }
+  double2 r = make_double2(add(add(t1.x, t2.x), t3.x), add(add(t1.y, t2.y), t3.y));
+  if (GUARD) r.y = add(r.y, (!isnan(v.x) && signbit(v.x)) ? w : 0.0);
+  return r;
+}
+
+template <bool GUARD, bool SCALAR>
+__global__ void __launch_bounds__(kT) k_poly_c(double2 *__restrict__ fx, const double2 *__restrict__ x, int64_t n,
+                                               const double *__restrict__ a, const double *__restrict__ w, int64_t ldfx,
+                                               int64_t ldx) {
+  const double2 *xb = x + (int64_t)blockIdx.y * ldx;
+  double2 *fb = fx + (int64_t)blockIdx.y * ldfx;
+  for (int64_t i = blockIdx.x * (int64_t)kT + threadIdx.x; i < n; i += (int64_t)gridDim.x * kT)
+    fb[i] = poly_at_c<GUARD>(SCALAR ? xb[0] : xb[i], a[i], w[i]);
+}
+
 __device__ __forceinline__ uint64_t splitmix64_at(uint64_t seed, uint64_t i) {
   uint64_t z = seed + (i + 1) * 0x9E3779B97F4A7C15ULL;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
@@ -371,6 +421,10 @@ int fdbs_stream_probe(const double *d_src, int64_t lds, int reads, double *d_dst
   if (reads == 1 && writes == 0) k_stream_probe<1, 0><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
   else if (reads == 1 && writes == 3) k_stream_probe<1, 3><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
   else if (reads == 4 && writes == 3) k_stream_probe<4, 3><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 1 && writes == 1) k_stream_probe<1, 1><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 1 && writes == 2) k_stream_probe<1, 2><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 2 && writes == 1) k_stream_probe<2, 1><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
+  else if (reads == 3 && writes == 1) k_stream_probe<3, 1><<<blocks, kT, 0, s>>>(d_src, lds, d_dst, ldd, n, d_sink);
   else return 2;
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
@@ -502,6 +556,52 @@ int fdbs_quartic_c(void *vctx, void *d_fx, const void *d_x, int64_t batch, int64
   k_scalar_c<<<(unsigned)batch, threads, smem, (cudaStream_t)stream>>>((double2 *)d_fx, (const double2 *)d_x, c->n, c->d_a,
                                                                        c->d_w, ldfx, ldx);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+}  // extern "C"
+
+template <bool GUARD, bool SCALAR>
+static int poly_launch(void *vctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream,
+                       bool complex_) {
+  fdbs_scalar_ctx *c = (fdbs_scalar_ctx *)vctx;
+  if (!c || c->n < 0 || (c->n > 0 && (!c->d_a || !c->d_w)) || batch < 1 || batch > 65535) return 1;
+  c->calls += batch;
+  if (c->n == 0) return 0;
+  dim3 grid((unsigned)blocks_for(c->n), (unsigned)batch);
+  if (complex_)
+    k_poly_c<GUARD, SCALAR><<<grid, kT, 0, (cudaStream_t)stream>>>((double2 *)d_fx, (const double2 *)d_x, c->n, c->d_a,
+                                                                    c->d_w, ldfx, ldx);
+  else
+    k_poly<GUARD, SCALAR><<<grid, kT, 0, (cudaStream_t)stream>>>((double *)d_fx, (const double *)d_x, c->n, c->d_a, c->d_w,
+                                                                  ldfx, ldx);
+  return cudaGetLastError() == cudaSuccess ? 0 : 3;
+}
+
+extern "C" {
+
+int fdbs_poly(void *c, double *fx, const double *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<false, false>(c, fx, x, b, lf, lx, s, false);
+}
+int fdbs_poly_guarded(void *c, double *fx, const double *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<true, false>(c, fx, x, b, lf, lx, s, false);
+}
+int fdbs_poly_c(void *c, void *fx, const void *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<false, false>(c, fx, x, b, lf, lx, s, true);
+}
+int fdbs_poly_guarded_c(void *c, void *fx, const void *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<true, false>(c, fx, x, b, lf, lx, s, true);
+}
+int fdbs_tpoly(void *c, double *fx, const double *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<false, true>(c, fx, x, b, lf, lx, s, false);
+}
+int fdbs_tpoly_guarded(void *c, double *fx, const double *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<true, true>(c, fx, x, b, lf, lx, s, false);
+}
+int fdbs_tpoly_c(void *c, void *fx, const void *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<false, true>(c, fx, x, b, lf, lx, s, true);
+}
+int fdbs_tpoly_guarded_c(void *c, void *fx, const void *x, int64_t b, int64_t lf, int64_t lx, void *s) {
+  return poly_launch<true, true>(c, fx, x, b, lf, lx, s, true);
 }
 
 int fdbs_fail(void *, double *, const double *, int64_t, int64_t, int64_t, void *) { return 42; }

@@ -19,14 +19,16 @@
 #     CuMatrix J, sparsity === nothing      src/jacobians.jl:548-557, 590-598 (dense column branch, colorvec quirk included)
 #   for Val(:forward), Val(:central) and Val(:complex) (src/jacobians.jl:623-648), plus the JVP and the multi-GPU group,
 #   and the vector -> scalar entry points on CuVector{Float64} x: finite_difference_hessian! (src/hessians.jl:202-292,
-#   fdb_hessian) and finite_difference_gradient! (src/gradients.jl:390-473, the dense plan with m = 1).
-# Everything else of FiniteDiff.jl (CPU arrays, complex x, scalar -> vector gradients, out-of-place forms) keeps using the
-# stock package.
+#   fdb_hessian) and finite_difference_gradient! (src/gradients.jl:390-473, the dense plan with m = 1), and the scalar-input
+#   entry points through fdb_derivative: finite_difference_derivative! on CuVector{Float64} x (src/derivatives.jl:197-233)
+#   and finite_difference_gradient! at a Real x into a CuVector{Float64} df (src/gradients.jl:477-533).
+# Everything else of FiniteDiff.jl (CPU arrays, complex x, out-of-place forms) keeps using the stock package.
 module FiniteDiffB200
 
 using FiniteDiff, SparseArrays, CUDA
 import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache,
-    finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache
+    finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache, finite_difference_derivative!,
+    DerivativeCache
 
 const libfdjac = get(ENV, "FDJAC_B200_LIB", "libfdjac_b200.so")
 
@@ -472,6 +474,126 @@ function finite_difference_gradient!(df::CuVector{Float64}, f, x::CuVector{Float
 end
 
 finite_difference_gradient!(df::CuVector{Float64}, f, x::CuVector{Float64}, fdtype::Union{Type, Val} = Val(:central);
+        relstep = nothing, absstep = relstep, dir = true) =
+    finite_difference_gradient!(df, f, x, GradientCache(df, x, fdtype); relstep = relstep, absstep = absstep, dir = dir)
+
+# ---- scalar input per step size: finite_difference_derivative! (src/derivatives.jl:197-233) and the scalar -> vector
+#      finite_difference_gradient! (src/gradients.jl:477-533), both through fdb_derivative
+# the derivative's f is a scalar function applied elementwise (the plan's callback has m = n)
+elementwise_f(f) = (fx, xv) -> (fx .= f.(xv); nothing)
+
+# scalar -> vector callback: point b is ONE device double (complex: one ComplexF64), read back for the Number the reference
+# passes to f(fx, t).  The read synchronises the stream, so this callback is not for use_graph plans.
+function tvec_trampoline(ctx::Ptr{Cvoid}, fx::CuPtr{Float64}, x::CuPtr{Float64}, batch::Int64, ldfx::Int64, ldx::Int64,
+        stream::Ptr{Cvoid})::Cint
+    st = unsafe_pointer_to_objref(ctx)::FnState
+    try
+        for b in 0:(batch - 1)
+            fxv = unsafe_wrap(CuArray, fx + b * ldfx * sizeof(Float64), st.m)
+            t = Array(unsafe_wrap(CuArray, x + b * ldx * sizeof(Float64), 1))[1]
+            st.f(fxv, t)
+        end
+        return Cint(0)
+    catch err
+        st.err = err
+        return Cint(1)
+    end
+end
+
+function tvec_trampoline_c(ctx::Ptr{Cvoid}, fx::CuPtr{ComplexF64}, x::CuPtr{ComplexF64}, batch::Int64, ldfx::Int64,
+        ldx::Int64, stream::Ptr{Cvoid})::Cint
+    st = unsafe_pointer_to_objref(ctx)::FnState
+    try
+        for b in 0:(batch - 1)
+            fxv = unsafe_wrap(CuArray, fx + b * ldfx * sizeof(ComplexF64), st.m)
+            t = Array(unsafe_wrap(CuArray, x + b * ldx * sizeof(ComplexF64), 1))[1]
+            st.f(fxv, t)
+        end
+        return Cint(0)
+    catch err
+        st.err = err
+        return Cint(1)
+    end
+end
+
+function derivative_plan(anchor, scalar_input::Bool, len::Integer, fd::Cint; kw...)
+    cached_plan(anchor, (scalar_input ? :scalar_gradient : :derivative, len, fd, values(kw))) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd; kw...))
+        if scalar_input
+            check(ccall((:fdb_scalar_gradient_plan_create, libfdjac), Cint, (Ref{Ptr{Cvoid}}, Int64, Ref{PlanOpts}), h, len, opts))
+        else
+            check(ccall((:fdb_derivative_plan_create, libfdjac), Cint, (Ref{Ptr{Cvoid}}, Int64, Ref{PlanOpts}), h, len, opts))
+        end
+        Plan(h[], nothing)
+    end
+end
+
+function run_derivative!(plan::Plan, df::CuVector{Float64}, st::FnState, x::CuVector{Float64}, fx, fdtype, relstep,
+        absstep, dir, scalar_input::Bool)
+    rc = Cint(0)
+    if fdtype == Val(:complex)
+        cf = scalar_input ?
+            @cfunction(tvec_trampoline_c, Cint, (Ptr{Cvoid}, CuPtr{ComplexF64}, CuPtr{ComplexF64}, Int64, Int64, Int64, Ptr{Cvoid})) :
+            @cfunction(f_trampoline_c, Cint, (Ptr{Cvoid}, CuPtr{ComplexF64}, CuPtr{ComplexF64}, Int64, Int64, Int64, Ptr{Cvoid}))
+        GC.@preserve st x df begin
+            rc = ccall((:fdb_derivative_complex, libfdjac), Cint,
+                (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Ptr{Cvoid}),
+                plan.handle, cf, pointer_from_objref(st), pointer(df), pointer(x), CUDA.stream().handle)
+        end
+    else
+        cf = scalar_input ?
+            @cfunction(tvec_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid})) :
+            @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+        GC.@preserve st x df fx begin
+            rc = ccall((:fdb_derivative, libfdjac), Cint,
+                (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, Float64, Float64,
+                    Float64, Ptr{Cvoid}),
+                plan.handle, cf, pointer_from_objref(st), pointer(df), pointer(x), fx === nothing ? CU_NULL : pointer(fx),
+                stepval(relstep), stepval(absstep), Float64(dir), CUDA.stream().handle)
+        end
+    end
+    st.err === nothing || throw(st.err)
+    check(rc)
+    df
+end
+
+# cache.fx is read in forward mode only (the DerivativeCache constructor already drops it otherwise, :67-73); the
+# epsilon array is neither read nor written on this path
+function finite_difference_derivative!(df::CuVector{Float64}, f, x::CuVector{Float64},
+        cache::DerivativeCache{T1, T2, fdtype, returntype}; relstep = nothing, absstep = relstep,
+        dir = true) where {T1, T2, fdtype, returntype}
+    n = length(x)
+    length(df) == n || throw(DimensionMismatch("length(df) != length(x)"))
+    plan = derivative_plan(df, false, n, fdcode(fdtype))
+    fx = (fdtype == Val(:forward) && cache.fx isa CuVector{Float64}) ? cache.fx : nothing
+    run_derivative!(plan, df, FnState(elementwise_f(f), n, n, nothing), x, fx, fdtype, relstep, absstep, dir, false)
+end
+
+finite_difference_derivative!(df::CuVector{Float64}, f, x::CuVector{Float64}, fdtype::Union{Type, Val} = Val(:central),
+        returntype = eltype(x), fx = nothing, epsilon = nothing; relstep = nothing, absstep = relstep) =
+    finite_difference_derivative!(df, f, x, DerivativeCache(x, fx, epsilon, fdtype, returntype); relstep = relstep,
+        absstep = absstep)
+
+# the scalar t is staged into ONE device slot per cache (anchored on its c1 array, or on df when the cache has none), so
+# repeated calls pass the same device pointer
+const T_SLOTS = WeakKeyDict{Any, CuVector{Float64}}()
+
+function finite_difference_gradient!(df::CuVector{Float64}, f, x::Real,
+        cache::GradientCache{T1, T2, T3, T4, fdtype, returntype, inplace};
+        relstep = nothing, absstep = relstep, dir = true) where {T1, T2, T3, T4, fdtype, returntype, inplace}
+    m = length(df)
+    anchor = cache.c1 isa CuArray ? cache.c1 : df
+    t = lock(PLANS_LOCK) do
+        get!(() -> CuVector{Float64}(undef, 1), T_SLOTS, anchor)
+    end
+    fill!(t, Float64(x))
+    plan = derivative_plan(anchor, true, m, fdcode(fdtype))
+    fx = (fdtype == Val(:forward) && cache.fx isa CuVector{Float64}) ? cache.fx : nothing     # gradients.jl:501-502
+    run_derivative!(plan, df, FnState(f, m, 1, nothing), t, fx, fdtype, relstep, absstep, dir, true)
+end
+
+finite_difference_gradient!(df::CuVector{Float64}, f, x::Real, fdtype::Union{Type, Val} = Val(:central);
         relstep = nothing, absstep = relstep, dir = true) =
     finite_difference_gradient!(df, f, x, GradientCache(df, x, fdtype); relstep = relstep, absstep = absstep, dir = dir)
 

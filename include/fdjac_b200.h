@@ -335,6 +335,36 @@ fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, cons
 fdb_status fdb_hessian(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, double *d_H, double *d_fx, double relstep,
                        double absstep, void *stream);
 
+/* ---- Derivatives with a scalar input per step size ----
+ *   finite_difference_derivative!(df, f, x::StridedArray, cache::DerivativeCache; relstep, absstep, dir)
+ *                                                                        src/derivatives.jl:197-233
+ *   finite_difference_gradient!(df, f, x::Number, cache::GradientCache; relstep, absstep, dir)   src/gradients.jl:477-533
+ * fdb_derivative_plan_create: the elementwise derivative of a scalar function over n components.  f is the batched
+ *   fdb_fn with m = n, applied elementwise: d_fx[b*ldfx + i] = f(d_x[b*ldx + i]).  df, x: n doubles.
+ * fdb_scalar_gradient_plan_create: the scalar -> vector "gradient" of an in-place f(fx, t) with m outputs: the fdb_fn
+ *   with n = 1 (point b is the single double d_x[b*ldx]) and m outputs.  df: m doubles; x: ONE double (device memory,
+ *   so that a solver writing t in place can replay a captured graph).
+ * opts->fdtype: FDB_FORWARD, FDB_CENTRAL or FDB_COMPLEX (FDB_HCENTRAL => FDB_ERR_UNSUPPORTED); one device (world <= 1).
+ * max_batch >= 2: a central call hands both points (rows 0: x+eps, 1: x-eps at the plan's ldx) to ONE f call.
+ *
+ * fdb_derivative evaluates, per component (derivative) or once (gradient), eps = max(relstep*|x|, absstep)*dir (forward;
+ * central without dir) and, in the reference's order, f(x+eps) then f(x) (forward, unless d_fx is given: cache.fx, the
+ * f values at x) or f(x+eps) then f(x-eps) (central), and writes
+ *   forward  df = (f(x+eps) - f(x)) / eps
+ *   central  df = (f(x+eps) - f(x-eps)) * (1 / (2eps))   derivative (the reciprocal is rounded first, derivatives.jl:220-222)
+ *            df = (f(x+eps) - f(x-eps)) / (2eps)         scalar gradient (gradients.jl:520)
+ * d_x is never modified; d_fx is ignored outside forward mode.  relstep / absstep: FDB_STEP_DEFAULT => default_relstep(fdtype)
+ * and absstep = relstep.  fdb_derivative_complex (plans of fdtype FDB_COMPLEX): one complex128 evaluation at
+ * (x + 0.0) + im*eps(Float64), df = imag(f) / eps(Float64).  Stream-ordered, no host synchronisation; use_graph as for
+ * fdb_jacobian.  fdb_plan_info: n_entries = length(df), fcalls_per_jacobian = f evaluations of the last call (before
+ * the first: 2 forward / central, 1 complex), alg_bytes / moved_bytes = the library's compulsory bytes per call.
+ * The Jacobian, Hessian and JVP entry points reject these plans, and fdb_derivative rejects theirs (FDB_ERR_INVALID). ---- */
+fdb_status fdb_derivative_plan_create(fdb_plan **plan, int64_t n, const fdb_plan_opts *opts);
+fdb_status fdb_scalar_gradient_plan_create(fdb_plan **plan, int64_t m, const fdb_plan_opts *opts);
+fdb_status fdb_derivative(fdb_plan *plan, fdb_fn f, void *ctx, double *d_df, const double *d_x, const double *d_fx,
+                          double relstep, double absstep, double dir, void *stream);
+fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double *d_df, const double *d_x, void *stream);
+
 /* ---- helpers for hosts without their own CUDA bindings ---- */
 fdb_status fdb_host_alloc(void **p, size_t bytes);  /* pinned host memory */
 fdb_status fdb_host_free(void *p);

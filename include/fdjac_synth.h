@@ -21,6 +21,16 @@
  *                  s = g(sum_i g(w[i] x[i], 3/4), 3/2), z[i] = (!isnan(x[i]) && signbit(x[i])) ? w[i] : 0.
  *                  Finite for every double x, so an IEEE edge value in x[k] leaves the entries of H that do not
  *                  involve k finite; sees the sign of a zero but never the sign or payload of a NaN.
+ *
+ * Elementwise and scalar-input functions (fdbs_scalar_ctx, n = number of outputs), for derivatives and scalar -> vector
+ * gradients; CPU twins in scalar_oracle/synth_scalar.c.  Output i of a point:
+ *   p_i(v) = (a[i] (v^2 v) + w[i] v^2) + v
+ *   fdbs_poly / fdbs_poly_c       : v = x[i] (elementwise: d_fx[b*ldfx + i] = p_i(d_x[b*ldx + i]))
+ *   fdbs_tpoly / fdbs_tpoly_c     : v = x[0] (m outputs of one scalar t: d_fx[b*ldfx + i] = p_i(d_x[b*ldx]))
+ *   *_guarded                     : every term through g(., c) (c = 1/4, -1/2, 3/4) plus z = (!isnan(v) && signbit(v)) ?
+ *                                   w[i] : 0 — finite for every v, sees the sign of a zero.  The complex twins guard the
+ *                                   real and imaginary part of each term and add z (from the real part) to the imaginary
+ *                                   part, the one a complex step reads.
  */
 #ifndef FDJAC_SYNTH_H
 #define FDJAC_SYNTH_H
@@ -52,6 +62,14 @@ int fdbs_quartic(void *ctx, double *d_fx, const double *d_x, int64_t batch, int6
 int fdbs_quartic_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_sumsq(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 int fdbs_guarded(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_poly(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_poly_guarded(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_poly_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_poly_guarded_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_tpoly(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_tpoly_guarded(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_tpoly_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
+int fdbs_tpoly_guarded_c(void *ctx, void *d_fx, const void *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 /* a callback that always fails (error-path tests) */
 int fdbs_fail(void *ctx, double *d_fx, const double *d_x, int64_t batch, int64_t ldfx, int64_t ldx, void *stream);
 
@@ -61,7 +79,7 @@ int fdbs_fill_x(double *d_x, int64_t n, uint64_t seed, void *stream);
 /* store-only bandwidth probe: mode 0 constant data, mode 1 a distinct value per element */
 int fdbs_store_probe(double *d_out, int64_t n, int mode, int blocks, void *stream);
 /* read / write mix probe: `reads` vectors of n doubles from d_src (stride lds) read, `writes` vectors written to d_dst
- * (stride ldd), 16-byte streaming accesses; mixes (1, 0), (1, 3), (4, 3); d_sink: one double, written only on a NaN sum */
+ * (stride ldd), 16-byte streaming accesses; mixes (1, 0), (1, 1), (1, 2), (1, 3), (2, 1), (3, 1), (4, 3); d_sink: one double, written only on a NaN sum */
 int fdbs_stream_probe(const double *d_src, int64_t lds, int reads, double *d_dst, int64_t ldd, int writes, int64_t n,
                       int blocks, double *d_sink, void *stream);
 int fdbs_flush_l2(void *d_buf, int64_t bytes, void *stream);

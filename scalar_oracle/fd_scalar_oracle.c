@@ -135,3 +135,101 @@ int fdso_gradient_complex(double *df, fdso_fn_c f, void *ctx, const double *x, i
   }
   return 0;
 }
+
+static double epsilon_of(int fdtype, double x, double relstep, double absstep, double dir) {
+  const double e = max_julia(relstep * fabs(x), absstep);                 /* epsilons.jl:28 / :52 */
+  return fdtype == 0 ? e * dir : e;
+}
+
+int fdso_derivative(double *df, fdso_efn f, void *ctx, const double *x, int64_t n, int fdtype, const double *fx,
+                    double relstep, double absstep, double dir, fdso_log_fn log, void *log_ctx, int64_t *fcalls) {
+  if (fdtype != 0 && fdtype != 1) return 1;                                /* :229-230 fdtype_error */
+  steps(fdtype, &relstep, &absstep);                                       /* :202-203 */
+  *fcalls = 0;
+  for (int64_t i = 0; i < n; ++i) {                                        /* :208 / :218 */
+    const double epsilon = epsilon_of(fdtype, x[i], relstep, absstep, dir);   /* :209 / :219 */
+    if (fdtype == 0) {
+      const double x_plus = x[i] + epsilon;                                /* :210 */
+      if (log) log(log_ctx, &x_plus, 1);
+      *fcalls += 1;
+      const double fp = f(ctx, i, x_plus);                                 /* :212 f(x_plus) - f(x[i]), left to right */
+      double fb;
+      if (fx) {
+        fb = fx[i];                                                        /* :214 */
+      } else {
+        if (log) log(log_ctx, &x[i], 1);
+        *fcalls += 1;
+        fb = f(ctx, i, x[i]);
+      }
+      df[i] = (fp - fb) / epsilon;
+    } else {
+      const double epsilon_double_inv = 1.0 / (2 * epsilon);               /* :220 */
+      const double x_plus = x[i] + epsilon, x_minus = x[i] - epsilon;      /* :221 */
+      if (log) log(log_ctx, &x_plus, 1);
+      *fcalls += 1;
+      const double fp = f(ctx, i, x_plus);                                 /* :222 */
+      if (log) log(log_ctx, &x_minus, 1);
+      *fcalls += 1;
+      const double fm = f(ctx, i, x_minus);
+      df[i] = (fp - fm) * epsilon_double_inv;
+    }
+  }
+  return 0;
+}
+
+int fdso_derivative_complex(double *df, fdso_efn_c f, void *ctx, const double *x, int64_t n, fdso_log_fn log,
+                            void *log_ctx, int64_t *fcalls) {
+  *fcalls = 0;
+  const double epsilon_complex = DBL_EPSILON;                              /* :225 eps(eltype(x)) */
+  for (int64_t i = 0; i < n; ++i) {                                        /* :226 */
+    const double z[2] = {x[i] + 0.0, epsilon_complex};                     /* :227 x[i] + im*eps: im*eps = (false*eps, eps) */
+    double out[2];
+    if (log) log(log_ctx, z, 2);
+    *fcalls += 1;
+    f(ctx, i, z, out);
+    df[i] = out[1] / epsilon_complex;                                      /* imag(f(..)) / epsilon_complex */
+  }
+  return 0;
+}
+
+int fdso_scalar_gradient(double *df, fdso_vfn f, void *ctx, double x, int64_t m, int fdtype, const double *fx,
+                         double relstep, double absstep, double dir, double *c1, double *c2, fdso_log_fn log,
+                         void *log_ctx, int64_t *fcalls) {
+  if (fdtype != 0 && fdtype != 1) return 1;                                /* :530 fdtype_error */
+  steps(fdtype, &relstep, &absstep);                                       /* :482-483 */
+  *fcalls = 0;
+  const double epsilon = epsilon_of(fdtype, x, relstep, absstep, dir);     /* :495 / :512 */
+  const double xp = x + epsilon;
+  if (log) log(log_ctx, &xp, 1);
+  *fcalls += 1;
+  f(ctx, c1, xp);                                                          /* :497 / :514 f(c1, x + epsilon) */
+  if (fdtype == 0) {
+    if (fx) {
+      for (int64_t i = 0; i < m; ++i) df[i] = (c1[i] - fx[i]) / epsilon;   /* :502 */
+    } else {
+      if (log) log(log_ctx, &x, 1);
+      *fcalls += 1;
+      f(ctx, c2, x);                                                       /* :505 f(c2, x) */
+      for (int64_t i = 0; i < m; ++i) df[i] = (c1[i] - c2[i]) / epsilon;   /* :509 */
+    }
+  } else {
+    const double xm = x - epsilon;
+    if (log) log(log_ctx, &xm, 1);
+    *fcalls += 1;
+    f(ctx, c2, xm);                                                        /* :515 f(c2, x - epsilon) */
+    for (int64_t i = 0; i < m; ++i) df[i] = (c1[i] - c2[i]) / (2 * epsilon);   /* :520 */
+  }
+  return 0;
+}
+
+int fdso_scalar_gradient_complex(double *df, fdso_vfn_c f, void *ctx, double x, int64_t m, double *c1, fdso_log_fn log,
+                                 void *log_ctx, int64_t *fcalls) {
+  *fcalls = 0;
+  const double epsilon_complex = DBL_EPSILON;                              /* :522 eps(real(eltype(x))) */
+  const double z[2] = {x + 0.0, epsilon_complex};                          /* :524 x + im*epsilon_complex */
+  if (log) log(log_ctx, z, 2);
+  *fcalls += 1;
+  f(ctx, c1, z);                                                           /* :524 f(c1, ..) */
+  for (int64_t i = 0; i < m; ++i) df[i] = c1[2 * i + 1] / epsilon_complex;   /* :528 imag(c1) / epsilon_complex */
+  return 0;
+}

@@ -21,6 +21,10 @@ _f64p = C.POINTER(C.c_double)
 FDSO_FN = C.CFUNCTYPE(C.c_double, C.c_void_p, _f64p)
 FDSO_FN_C = C.CFUNCTYPE(None, C.c_void_p, _f64p, _f64p)
 FDSO_LOG = C.CFUNCTYPE(None, C.c_void_p, _f64p, C.c_int64)
+FDSO_EFN = C.CFUNCTYPE(C.c_double, C.c_void_p, C.c_int64, C.c_double)
+FDSO_EFN_C = C.CFUNCTYPE(None, C.c_void_p, C.c_int64, _f64p, _f64p)
+FDSO_VFN = C.CFUNCTYPE(None, C.c_void_p, _f64p, C.c_double)
+FDSO_VFN_C = C.CFUNCTYPE(None, C.c_void_p, _f64p, _f64p)
 
 
 class SynthScalarCtx(C.Structure):
@@ -65,6 +69,31 @@ def lib():
         L.synth_guarded.argtypes = [C.c_void_p, _f64p]
         L.synth_quartic_c.restype = None
         L.synth_quartic_c.argtypes = [C.c_void_p, _f64p, _f64p]
+        L.fdso_derivative.restype = C.c_int
+        L.fdso_derivative.argtypes = [_f64p, C.c_void_p, C.c_void_p, _f64p, C.c_int64, C.c_int, _f64p, C.c_double,
+                                      C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]
+        L.fdso_derivative_complex.restype = C.c_int
+        L.fdso_derivative_complex.argtypes = [_f64p, C.c_void_p, C.c_void_p, _f64p, C.c_int64, C.c_void_p, C.c_void_p,
+                                              C.POINTER(C.c_int64)]
+        L.fdso_scalar_gradient.restype = C.c_int
+        L.fdso_scalar_gradient.argtypes = [_f64p, C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_int, _f64p,
+                                           C.c_double, C.c_double, C.c_double, _f64p, _f64p, C.c_void_p, C.c_void_p,
+                                           C.POINTER(C.c_int64)]
+        L.fdso_scalar_gradient_complex.restype = C.c_int
+        L.fdso_scalar_gradient_complex.argtypes = [_f64p, C.c_void_p, C.c_void_p, C.c_double, C.c_int64, _f64p,
+                                                   C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]
+        for nm in ("synth_poly", "synth_poly_guarded"):
+            getattr(L, nm).restype = C.c_double
+            getattr(L, nm).argtypes = [C.c_void_p, C.c_int64, C.c_double]
+        for nm in ("synth_poly_c", "synth_poly_guarded_c"):
+            getattr(L, nm).restype = None
+            getattr(L, nm).argtypes = [C.c_void_p, C.c_int64, _f64p, _f64p]
+        for nm in ("synth_tpoly", "synth_tpoly_guarded"):
+            getattr(L, nm).restype = None
+            getattr(L, nm).argtypes = [C.c_void_p, _f64p, C.c_double]
+        for nm in ("synth_tpoly_c", "synth_tpoly_guarded_c"):
+            getattr(L, nm).restype = None
+            getattr(L, nm).argtypes = [C.c_void_p, _f64p, _f64p]
         _lib = L
     return _lib
 
@@ -94,7 +123,7 @@ class SynthScalar:
 
     def native(self, name: str):
         """(function address, ctx) for the oracle entry points: name = synth_quartic / synth_sumsq / synth_guarded /
-        synth_quartic_c."""
+        synth_quartic_c, or synth_poly[_guarded][_c] / synth_tpoly[_guarded][_c] for derivative / scalar_gradient."""
         return C.cast(getattr(lib(), name), C.c_void_p), C.cast(C.pointer(self.ctx), C.c_void_p)
 
     def __call__(self, x) -> float:
@@ -166,3 +195,84 @@ def gradient(f, x, fdtype=FORWARD, *, fx=None, relstep=None, absstep=None, dir=1
     if rc != 0:
         raise ValueError(f"oracle returned {rc}")
     return {"df": df[:n], "fcalls": calls.value, "points": points}
+
+
+def _efn(f, complex_=False):
+    """(address, ctx, keepalive) of a Python scalar f(v) (index-free, as the reference's f) or a native pair."""
+    if isinstance(f, tuple):
+        return f[0], f[1], None
+    if complex_:
+        def tramp_c(_ctx, _i, px, pout):
+            z = complex(f(complex(px[0], px[1])))
+            pout[0], pout[1] = z.real, z.imag
+        cf = FDSO_EFN_C(tramp_c)
+    else:
+        cf = FDSO_EFN(lambda _ctx, _i, v: float(f(v)))
+    return C.cast(cf, C.c_void_p), None, cf
+
+
+def _vfn(f, m, complex_=False):
+    """(address, ctx, keepalive) of a Python in-place f(fx, t) on numpy arrays (fx float64 or complex128 of length m, t a
+    float or complex) or a native pair."""
+    if isinstance(f, tuple):
+        return f[0], f[1], None
+    if complex_:
+        def tramp_c(_ctx, pfx, pt):
+            fx = np.zeros(m, dtype=np.complex128)
+            f(fx, complex(pt[0], pt[1]))
+            np.ctypeslib.as_array(pfx, shape=(2 * m,))[:] = fx.view(np.float64)
+        cf = FDSO_VFN_C(tramp_c)
+    else:
+        def tramp(_ctx, pfx, t):
+            fx = np.zeros(m)
+            f(fx, t)
+            np.ctypeslib.as_array(pfx, shape=(m,))[:] = fx
+        cf = FDSO_VFN(tramp)
+    return C.cast(cf, C.c_void_p), None, cf
+
+
+def derivative(f, x, fdtype=CENTRAL, *, fx=None, relstep=None, absstep=None, dir=1.0, log=False):
+    """finite_difference_derivative!(df, f, x::StridedArray, cache) (derivatives.jl:197-233).  f: Python f(v) -> float
+    (complex for COMPLEX) or a native pair from SynthScalar.native.  Returns dict(df, fcalls, points (each argument: a
+    float, or a (re, im) array for complex))."""
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    n = x.size
+    df = np.zeros(max(n, 1))
+    points = [] if log else None
+    lptr, lkeep = _log(points)
+    calls = C.c_int64(0)
+    fptr, ctx, keep = _efn(f, fdtype == COMPLEX)
+    if fdtype == COMPLEX:
+        rc = lib().fdso_derivative_complex(_p(df), fptr, ctx, _p(x), n, lptr, None, C.byref(calls))
+    else:
+        fxa = None if fx is None else np.ascontiguousarray(fx, dtype=np.float64)
+        rc = lib().fdso_derivative(_p(df), fptr, ctx, _p(x), n, int(fdtype), _p(fxa), _step(relstep), _step(absstep),
+                                   float(dir), lptr, None, C.byref(calls))
+    if rc != 0:
+        raise ValueError(f"oracle returned {rc}")
+    if points is not None and fdtype != COMPLEX:
+        points = [float(p[0]) for p in points]
+    return {"df": df[:n], "fcalls": calls.value, "points": points}
+
+
+def scalar_gradient(f, x, m, fdtype=CENTRAL, *, fx=None, relstep=None, absstep=None, dir=1.0, log=False):
+    """finite_difference_gradient!(df, f, x::Number, cache) (gradients.jl:477-533).  f: Python in-place f(fx, t) or a
+    native pair.  Returns dict(df, fcalls, points)."""
+    df = np.zeros(max(m, 1))
+    points = [] if log else None
+    lptr, lkeep = _log(points)
+    calls = C.c_int64(0)
+    fptr, ctx, keep = _vfn(f, m, fdtype == COMPLEX)
+    if fdtype == COMPLEX:
+        c1 = np.zeros(max(2 * m, 2))
+        rc = lib().fdso_scalar_gradient_complex(_p(df), fptr, ctx, float(x), m, _p(c1), lptr, None, C.byref(calls))
+    else:
+        c1, c2 = np.zeros(max(m, 1)), np.zeros(max(m, 1))
+        fxa = None if fx is None else np.ascontiguousarray(fx, dtype=np.float64)
+        rc = lib().fdso_scalar_gradient(_p(df), fptr, ctx, float(x), m, int(fdtype), _p(fxa), _step(relstep),
+                                        _step(absstep), float(dir), _p(c1), _p(c2), lptr, None, C.byref(calls))
+    if rc != 0:
+        raise ValueError(f"oracle returned {rc}")
+    if points is not None and fdtype != COMPLEX:
+        points = [float(p[0]) for p in points]
+    return {"df": df[:m], "fcalls": calls.value, "points": points}

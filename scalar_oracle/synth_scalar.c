@@ -120,3 +120,49 @@ void synth_quartic_c(void *ctx, const double *x, double *out) {
     out[1] = out[1] + si / d;
   }
 }
+
+/* p_i(v) of fdbs_poly / fdbs_tpoly (synth_fns.cu: poly_at, poly_at_c) */
+static double poly_at(const synth_scalar_ctx *c, int64_t i, double v, int g) {
+  const double q = v * v, cu = q * v;
+  if (!g) return (c->a[i] * cu + c->w[i] * q) + v;
+  const double t = (guard(c->a[i] * cu, 0.25) + guard(c->w[i] * q, -0.5)) + guard(v, 0.75);
+  return t + ((!isnan(v) && signbit(v)) ? c->w[i] : 0.0);
+}
+
+static void poly_at_c(const synth_scalar_ctx *c, int64_t i, const double *v, double *out, int g) {
+  double qr, qi, cr, ci;
+  cmul(v[0], v[1], v[0], v[1], &qr, &qi);
+  cmul(qr, qi, v[0], v[1], &cr, &ci);
+  double t1r = c->a[i] * cr, t1i = c->a[i] * ci, t2r = c->w[i] * qr, t2i = c->w[i] * qi, t3r = v[0], t3i = v[1];
+  if (g) {
+    t1r = guard(t1r, 0.25); t1i = guard(t1i, 0.25);
+    t2r = guard(t2r, -0.5); t2i = guard(t2i, -0.5);
+    t3r = guard(t3r, 0.75); t3i = guard(t3i, 0.75);
+  }
+  out[0] = (t1r + t2r) + t3r;
+  out[1] = (t1i + t2i) + t3i;
+  if (g) out[1] = out[1] + ((!isnan(v[0]) && signbit(v[0])) ? c->w[i] : 0.0);
+}
+
+double synth_poly(void *ctx, int64_t i, double v) { return poly_at((const synth_scalar_ctx *)ctx, i, v, 0); }
+double synth_poly_guarded(void *ctx, int64_t i, double v) { return poly_at((const synth_scalar_ctx *)ctx, i, v, 1); }
+void synth_poly_c(void *ctx, int64_t i, const double *v, double *out) { poly_at_c((const synth_scalar_ctx *)ctx, i, v, out, 0); }
+void synth_poly_guarded_c(void *ctx, int64_t i, const double *v, double *out) {
+  poly_at_c((const synth_scalar_ctx *)ctx, i, v, out, 1);
+}
+void synth_tpoly(void *ctx, double *fx, double t) {
+  const synth_scalar_ctx *c = (const synth_scalar_ctx *)ctx;
+  for (int64_t i = 0; i < c->n; ++i) fx[i] = poly_at(c, i, t, 0);
+}
+void synth_tpoly_guarded(void *ctx, double *fx, double t) {
+  const synth_scalar_ctx *c = (const synth_scalar_ctx *)ctx;
+  for (int64_t i = 0; i < c->n; ++i) fx[i] = poly_at(c, i, t, 1);
+}
+void synth_tpoly_c(void *ctx, double *fx, const double *t) {
+  const synth_scalar_ctx *c = (const synth_scalar_ctx *)ctx;
+  for (int64_t i = 0; i < c->n; ++i) poly_at_c(c, i, t, fx + 2 * i, 0);
+}
+void synth_tpoly_guarded_c(void *ctx, double *fx, const double *t) {
+  const synth_scalar_ctx *c = (const synth_scalar_ctx *)ctx;
+  for (int64_t i = 0; i < c->n; ++i) poly_at_c(c, i, t, fx + 2 * i, 1);
+}
