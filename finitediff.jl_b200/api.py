@@ -391,6 +391,13 @@ class _PyFn:
         self.typestr, self.esize = ("<c16", 16) if complex_ else ("<f8", 8)
         self.cfunc = L.FDB_FN(self._tramp)
 
+    def _view(self, ptr, batch, k, ld):
+        if k == 0:                  # an empty array has no storage: its pointer may be NULL (None through ctypes)
+            dt = torch.complex128 if self.esize == 16 else torch.float64
+            return torch.empty((batch, 0), dtype=dt, device=self.device)
+        es = self.esize
+        return torch.as_tensor(_DevArray(ptr, (batch, k), (ld * es, es), self.typestr), device=self.device)
+
     def _tramp(self, _ctx, p_fx, p_x, batch, ldfx, ldx, stream):
         try:
             cur = torch.cuda.current_stream(self.device)
@@ -399,9 +406,8 @@ class _PyFn:
                 ctx = torch.cuda.stream(torch.cuda.ExternalStream(stream or 0, device=self.device))
                 ctx.__enter__()
             try:
-                es = self.esize
-                fx2 = torch.as_tensor(_DevArray(p_fx, (batch, self.m), (ldfx * es, es), self.typestr), device=self.device)
-                x2 = torch.as_tensor(_DevArray(p_x, (batch, self.n), (ldx * es, es), self.typestr), device=self.device)
+                fx2 = self._view(p_fx, batch, self.m, ldfx)
+                x2 = self._view(p_x, batch, self.n, ldx)
                 if self.elementwise and self.batched:
                     self.calls += int(batch)
                     fx2.copy_(torch.as_tensor(self.f(x2), dtype=fx2.dtype, device=self.device))
@@ -966,18 +972,27 @@ def finite_difference_jvp_(jvp, f, x, v, cache=None, f_in=None, *, relstep=None,
     n, m = xv.numel(), jv.numel()
     if vv.numel() != n:
         raise ValueError("length(v) != length(x)")
-    plan = cache.plan(m, n)
-    if cache.x1.numel() != n or cache.fx1.numel() != m:
+    # The device reads and writes n / m contiguous doubles from each buffer's first element: a strided view, a float32
+    # or short array, or memory on another device would be read past its end or written outside the view.
+    x1v, fx1v = _flat_f64(cache.x1, "cache.x1"), _flat_f64(cache.fx1, "cache.fx1")
+    if x1v.numel() != n or fx1v.numel() != m:
         raise ValueError("JVPCache arrays do not match length(x) / length(jvp)")
+    fin_ptr = None
+    if f_in is not None and cache._code == L.FDB_FORWARD:                              # f_in is only read forward :257-258
+        finv = _flat_f64(f_in, "f_in")
+        if finv.numel() != m:
+            raise ValueError("length(f_in) != length(jvp)")
+        fin_ptr = _fx_ptr(finv)                 # an empty f_in is still given: f(fx1, x) must not run
+    for t in (x1v, fx1v) + (() if fin_ptr is None else (finv,)):
+        if t.device != x.device:
+            raise ValueError("JVPCache arrays and f_in must be on x's device")
+    plan = cache.plan(m, n)
     addr, ctx, pyfn = _as_fn(f, m, n, x.device, 1)
     if stream is None:
         stream = torch.cuda.current_stream(x.device).cuda_stream
-    fin_ptr = None
-    if f_in is not None and cache._code == L.FDB_FORWARD:
-        fin_ptr = f_in.reshape(-1).data_ptr()
     with torch.cuda.device(x.device):
-        st = L.lib().fdb_jvp(plan.handle, addr, ctx, jv.data_ptr(), xv.data_ptr(), vv.data_ptr(), cache.x1.data_ptr(),
-                             cache.fx1.data_ptr(), fin_ptr, L.STEP_DEFAULT if relstep is None else float(relstep),
+        st = L.lib().fdb_jvp(plan.handle, addr, ctx, jv.data_ptr(), xv.data_ptr(), vv.data_ptr(), x1v.data_ptr(),
+                             fx1v.data_ptr(), fin_ptr, L.STEP_DEFAULT if relstep is None else float(relstep),
                              L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
     if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
         exc, pyfn.exc = pyfn.exc, None

@@ -303,8 +303,11 @@ def jacobian_complex(P: Problem, J: np.ndarray, f, x: np.ndarray, *, colorvec=No
 
 
 def jvp(f, x: np.ndarray, v: np.ndarray, m: int, *, fdtype=FORWARD, relstep=None, absstep=None, dir=1.0, f_in=None,
-        eps_override=None, ctx=None):
-    """finite_difference_jvp!(jvp, f, x, v, cache, f_in) (src/jvp.jl:238-274).  Returns dict(jvp, eps, fcalls, x1, fx1)."""
+        eps_override=None, ctx=None, alias_x1=False):
+    """finite_difference_jvp!(jvp, f, x, v, cache, f_in) (src/jvp.jl:238-274).  Returns dict(jvp, eps, fcalls, x1, fx1).
+
+    alias_x1=True passes x's own buffer (a copy of the x given here) as cache.x1, as JVPCache(x, fx1) does
+    (jvp.jl:73-80): central mode then evaluates f at (x - eps*v) + eps*v, and the returned x1 is x's end state."""
     L = lib()
     fn = L.fdo_finite_difference_jvp
     if not hasattr(fn, "_bound"):
@@ -327,7 +330,10 @@ def jvp(f, x: np.ndarray, v: np.ndarray, m: int, *, fdtype=FORWARD, relstep=None
     calls = C.c_int64(0)
     relstep = float("nan") if relstep is None else float(relstep)
     absstep = float("nan") if absstep is None else float(absstep)
-    rc = fn(_p64(out), fptr, cptr, _p64(np.ascontiguousarray(x)), _p64(np.ascontiguousarray(v)), m, n, _p64(x1), _p64(fx1),
+    xa = np.ascontiguousarray(x, dtype=np.float64)
+    if alias_x1:
+        xa = x1 = np.array(xa if n else np.zeros(1), dtype=np.float64, copy=True)    # fd_oracle.c has no restrict
+    rc = fn(_p64(out), fptr, cptr, _p64(xa), _p64(np.ascontiguousarray(v)), m, n, _p64(x1), _p64(fx1),
             _p64(fin), fdtype, relstep, absstep, float(dir), _p64(eo), _p64(eps_out), C.byref(calls))
     if rc != 0:
         raise RuntimeError(f"oracle returned {rc}")

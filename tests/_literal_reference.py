@@ -52,10 +52,20 @@ def _bool_mul(v, mask):
     return np.where(mask, v, np.copysign(0.0, v))
 
 
+def _max(a, b):
+    """Julia's max(::Float64, ::Float64): NaN if either is NaN, and -0.0 < 0.0 (Python's max keeps its first argument on
+    a tie, so max(-0.0, 0.0) would be -0.0, and max(1.0, nan) would be 1.0)."""
+    if math.isnan(a) or math.isnan(b):
+        return a - b
+    if a == b:
+        return b if math.copysign(1.0, a) < 0 else a
+    return a if a > b else b
+
+
 def compute_epsilon(fdtype, x, relstep, absstep, dir):
     if fdtype == "forward":
-        return max(relstep * abs(x), absstep) * dir            # epsilons.jl:26-29
-    return max(relstep * abs(x), absstep)                      # epsilons.jl:50-53
+        return _max(relstep * abs(x), absstep) * dir           # epsilons.jl:26-29
+    return _max(relstep * abs(x), absstep)                     # epsilons.jl:50-53
 
 
 def norm(x2):

@@ -264,6 +264,89 @@ def guarded_numpy(x, a, w):
         return S1 + (s * s) / np.float64(2 * n)
 
 
+def exact_dot_xv(n, seed, kind="unit"):
+    """x, v with x_j = a_j 2^-s and v_j = b_j 2^-t for integers |a_j| < 2^20, |b_j| < 2^12: for n <= 2^20 every product
+    and every partial sum of dot(x, v) is a multiple of 2^-(s+t) below 2^53 * 2^-(s+t), so the dot is exact in any
+    summation order and a device tree, the oracle's in-order loop and np.dot all give the same bits.
+    kind: "unit" (s, t = 20, 12), "big" (x up to 2^500), "tiny" (d ~ 2^-950: the absstep branch of eps), "neg" (a
+    negative dot), "zero" (pairs that cancel: the dot is exactly 0; needs even n for a +0.0 result)."""
+    assert n <= 1 << 20
+    rng = np.random.default_rng(seed)
+    a = rng.integers(-(1 << 20) + 1, 1 << 20, n).astype(np.float64)
+    b = rng.integers(-(1 << 12) + 1, 1 << 12, n).astype(np.float64)
+    s, t = {"unit": (20, 12), "big": (-480, 12), "tiny": (500, 500), "neg": (20, 12), "zero": (20, 12)}[kind]
+    if kind == "neg":
+        b = -np.abs(b) * np.where(a < 0, -1.0, 1.0)
+    if kind == "zero":
+        a[1::2] = a[0:n - n % 2:2]
+        b[1::2] = -b[0:n - n % 2:2]
+        if n % 2:
+            b[-1] = 0.0
+    return np.ldexp(a, -s), np.ldexp(b, -t)
+
+
+class GatherF:
+    """A test f(fx, x) with m outputs of n inputs made only of gathers and separately rounded *, +, -:
+    fx_i = (c_i * x[g0_i] + x[g1_i] * x[g2_i]) - d_i  (fx_i = -d_i when n = 0).  The numpy form (`np_f`) and the torch
+    form (`torch_f`, one elementwise CUDA kernel per operation, so nothing is contracted into an FMA) round identically.
+    Each form records a copy of every x it is called with."""
+
+    def __init__(self, m, n, seed=0):
+        rng = np.random.default_rng(seed + 7919 * m + n)
+        self.m, self.n = m, n
+        self.g = [rng.integers(0, max(n, 1), m) for _ in range(3)]
+        self.c, self.d = rng.uniform(-2, 2, m), rng.uniform(-1, 1, m)
+
+    def np_f(self, log):
+        def f(fx, x):
+            log.append(np.array(x, copy=True))
+            with np.errstate(all="ignore"):
+                if self.n == 0:
+                    fx[:] = -self.d
+                else:
+                    fx[:] = (self.c * x[self.g[0]] + x[self.g[1]] * x[self.g[2]]) - self.d
+        return f
+
+    def torch_f(self, log, device):
+        import torch
+        g = [torch.from_numpy(i).to(device) for i in self.g]
+        c, d = torch.from_numpy(self.c).to(device), torch.from_numpy(self.d).to(device)
+
+        def f(fx, x):
+            log.append(x.detach().cpu().numpy().copy())
+            if self.n == 0:
+                fx.copy_(-d)
+            else:
+                fx.copy_((c * x[g[0]] + x[g[1]] * x[g[2]]) - d)
+        return f
+
+
+def traced(fn):
+    """Run fn() under torch.profiler (CUDA activity); return [(kernel name, grid x)] in launch order."""
+    import json
+    import tempfile
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        pad = torch.empty(1, device="cuda")
+        for _ in range(64):
+            pad.fill_(0.0)
+        torch.cuda.synchronize()
+        fn()
+        torch.cuda.synchronize()
+        for _ in range(64):
+            pad.fill_(0.0)
+        torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as fh:
+            events = json.load(fh)["traceEvents"]
+    return [(e["name"], int(e.get("args", {}).get("grid", [1])[0]))
+            for e in sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e.get("ts", 0))]
+
+
 def tridiagonal_coo(n):
     """Structural nz of Julia's Tridiagonal(dl,d,du) as (rows, cols, slots) with slots into [dl; d; du]
     (1-based): band order sub-diagonal, diagonal, super-diagonal."""

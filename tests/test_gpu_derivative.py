@@ -8,16 +8,13 @@ overrides, sizes around the 1024-element tile, unaligned buffers, batch caps 1 a
 IEEE edges at tile boundaries, every argument f sees, the caller's x left untouched, plan reuse and CUDA-graph replay, and
 the rejections."""
 import ctypes as C
-import json
 import math
-import os
 import re
-import tempfile
 
 import numpy as np
 import pytest
 
-from _util import assert_same_bits, fdb_env
+from _util import assert_same_bits, fdb_env, traced
 from scalar_oracle import fd_scalar_oracle as so
 
 torch = pytest.importorskip("torch")
@@ -297,29 +294,6 @@ def test_gpu_derivative_graph_replay(pkg, mode):
 
 
 # ------------------------------------------------------------------------------------------------ several tiles per block
-def traced(fn):
-    """Run fn() under torch.profiler (CUDA activity); return [(kernel name, grid x)] in launch order."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        pad = torch.empty(1, device="cuda")
-        for _ in range(64):
-            pad.fill_(0.0)
-        torch.cuda.synchronize()
-        fn()
-        torch.cuda.synchronize()
-        for _ in range(64):
-            pad.fill_(0.0)
-        torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "trace.json")
-        prof.export_chrome_trace(path)
-        with open(path) as fh:
-            events = json.load(fh)["traceEvents"]
-    return [(e["name"], int(e.get("args", {}).get("grid", [1])[0]))
-            for e in sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e.get("ts", 0))]
-
-
 @pytest.mark.parametrize("sm", [1, 3])
 @pytest.mark.parametrize("mode", ["forward", "central", "complex"])
 def test_gpu_derivative_multiwave(pkg, mode, sm):
