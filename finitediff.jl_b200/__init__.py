@@ -4,7 +4,7 @@ Layout (only what the path needs):
     csrc/      hand-written CUDA kernels + the C ABI (libfdjac_b200.so; include/fdjac_b200.h)
     api.py     host-side mirror of the reference interface (JacobianCache / finite_difference_jacobian!, HessianCache /
                finite_difference_hessian!, GradientCache / finite_difference_gradient!, DerivativeCache /
-               finite_difference_derivative!)
+               finite_difference_derivative!, and the out-of-place finite_difference_jacobian / finite_difference_jvp)
     distributed.py  multi-GPU plumbing over the C ABI's fdb_group_* / fdb_sync_* (colour shards, column blocks)
     julia/     the `ccall` wrapper a Julia host would load (not executable in this image: no julia)
     _lib.py    ctypes binding of the C ABI (fails loudly if the .so is missing)
@@ -19,10 +19,12 @@ from .api import (BandedBlockBandedMatrix, BandedMatrix, BlockBandedMatrix, Dens
                   check_coloring, make_plan, matrix_colors, pinned_empty, resize_, zeros_colmajor,
                   HessianCache, finite_difference_hessian_, finite_difference_hessian,
                   GradientCache, finite_difference_gradient_, finite_difference_gradient,
-                  DerivativeCache, finite_difference_derivative_, finite_difference_derivative)
+                  DerivativeCache, finite_difference_derivative_, finite_difference_derivative,
+                  finite_difference_jacobian, finite_difference_jvp)
 
 __all__ = ["BandedBlockBandedMatrix", "BandedMatrix", "BlockBandedMatrix", "DenseColumnBlock", "JacobianCache", "JVPCache", "finite_difference_jvp_", "NativeFn", "Plan", "SparseMatrixCSC", "Tridiagonal", "compute_epsilon",
            "default_relstep", "finite_difference_jacobian_", "finite_difference_jacobian_b", "make_plan", "matrix_colors", "check_coloring",
            "pinned_empty", "resize_", "zeros_colmajor", "HessianCache", "finite_difference_hessian_",
            "finite_difference_hessian", "GradientCache", "finite_difference_gradient_", "finite_difference_gradient",
-           "DerivativeCache", "finite_difference_derivative_", "finite_difference_derivative"]
+           "DerivativeCache", "finite_difference_derivative_", "finite_difference_derivative",
+           "finite_difference_jacobian", "finite_difference_jvp"]

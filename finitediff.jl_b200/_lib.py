@@ -16,6 +16,7 @@ SYNTH_PATH = HERE / "libfdjac_synth.so"
 FDB_OK, FDB_ERR_INVALID, FDB_ERR_CUDA, FDB_ERR_CALLBACK, FDB_ERR_NOMEM, FDB_ERR_UNSUPPORTED, FDB_ERR_NO_DEVICE = range(7)
 FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = 0, 1, 2, 3
 FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS = 0, 1, 2, 3
+FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = 0, 1, 2
 # FDB_STEP_DEFAULT: relstep / absstep keyword not given (any other value, 0 included, is used as passed)
 STEP_DEFAULT = float("nan")
 
@@ -52,6 +53,12 @@ class Counters(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class OopOut(C.Structure):
+    """fdb_oop_out: where fdb_jacobian_oop writes its result (device pointers)."""
+    _fields_ = [("J", C.c_void_p), ("colptr", C.c_void_p), ("rowval", C.c_void_p), ("nzval", C.c_void_p),
+                ("cap", C.c_int64), ("nnz", C.c_void_p)]
 
 
 # every symbol include/fdjac_b200.h declares: name -> (restype, argtypes)
@@ -100,6 +107,11 @@ ABI_SYMBOLS = {
     "fdb_check_coloring_csc": (_int, [_i64, _i64, _vp, _vp, _vp, C.POINTER(_i64)]),
     "fdb_jvp_plan_create": (_int, [_PP, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_jvp": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
+    "fdb_oop_plan_create_csc": (_int, [_PP, _i64, _i64, _vp, _vp, _vp, _int, _i64, C.POINTER(PlanOpts)]),
+    "fdb_oop_plan_create_dense": (_int, [_PP, _i64, _i64, _vp, _i64, _int, _i64, C.POINTER(PlanOpts)]),
+    "fdb_jacobian_oop": (_int, [_vp, _vp, _vp, _vp, C.POINTER(OopOut), _vp, _vp, _f64, _f64, _f64, _vp]),
+    "fdb_jacobian_oop_complex": (_int, [_vp, _vp, _vp, _vp, C.POINTER(OopOut), _vp]),
+    "fdb_jvp_oop": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
     "fdb_hessian_plan_create": (_int, [_PP, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_hessian": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _vp]),
     "fdb_derivative_plan_create": (_int, [_PP, _i64, C.POINTER(PlanOpts)]),

@@ -378,13 +378,16 @@ class _PyFn:
     (batch, m) / (batch, n) tensors; otherwise they are called once per point with 1-D tensors."""
 
     def __init__(self, f: Callable, m: int, n: int, device: torch.device, batched: bool, complex_: bool = False,
-                 scalar: bool = False, elementwise: bool = False, tvec: bool = False):
+                 scalar: bool = False, elementwise: bool = False, tvec: bool = False, oop: bool = False):
         self.f, self.m, self.n, self.device, self.batched = f, m, n, device, batched
         # scalar (m = 1) functions are called as f(x) and RETURN their value (a 0-d CUDA tensor needs no host sync)
         self.scalar = scalar
         # elementwise functions (derivatives) are called as f(x) and return a tensor of x's shape; scalar -> vector
         # functions (tvec, n = 1) are called in place as f(fx, t) with t a 0-d tensor
         self.elementwise, self.tvec = elementwise, tvec
+        # out-of-place functions (finite_difference_jacobian / _jvp) are called as f(x) and return a new array of m values
+        # (batched: (batch, m)), which is copied into the slot f! would have written
+        self.oop = oop
         self.exc: Optional[BaseException] = None
         self.calls = 0
         # complex-step callbacks (fdb_fn_c) see complex128 tensors; ld* then count complex elements
@@ -408,7 +411,14 @@ class _PyFn:
             try:
                 fx2 = self._view(p_fx, batch, self.m, ldfx)
                 x2 = self._view(p_x, batch, self.n, ldx)
-                if self.elementwise and self.batched:
+                if self.oop:
+                    self.calls += int(batch)
+                    if self.batched:
+                        fx2.copy_(_oop_result(self.f(x2), fx2.shape, complex_ok=self.esize == 16))
+                    else:
+                        for b in range(int(batch)):
+                            fx2[b].copy_(_oop_result(self.f(x2[b]), fx2[b].shape, complex_ok=self.esize == 16))
+                elif self.elementwise and self.batched:
                     self.calls += int(batch)
                     fx2.copy_(torch.as_tensor(self.f(x2), dtype=fx2.dtype, device=self.device))
                 elif self.elementwise:
@@ -442,6 +452,19 @@ class _PyFn:
         except BaseException as e:  # never let an exception cross the C ABI
             self.exc = e
             return 1
+
+
+def _oop_result(r, shape, complex_ok=False):
+    """The array an out-of-place f returned, checked against the slot it is copied into."""
+    if not isinstance(r, torch.Tensor) or not r.is_cuda:
+        raise TypeError("an out-of-place f must return a CUDA tensor")
+    if r.is_complex() and not complex_ok:
+        raise TypeError("not built: f returns a complex array (complex-valued results of the out-of-place path)")
+    if shape == (-1,):
+        return r.reshape(-1)
+    if r.numel() != int(np.prod(shape)):
+        raise ValueError(f"f returned {r.numel()} values where {int(np.prod(shape))} were expected")
+    return r.reshape(shape)
 
 
 # ------------------------------------------------------------------------------------------------ plans
@@ -1000,6 +1023,252 @@ def finite_difference_jvp_(jvp, f, x, v, cache=None, f_in=None, *, relstep=None,
     L.check(st)
     cache._last_plan = plan
     return None
+
+
+# ------------------------------------------------------------------------------------------------ out-of-place forms
+def _native_call(f: "NativeFn", fx: torch.Tensor, x: torch.Tensor, stream):
+    """Evaluate a native fdb_fn once, f(fx, x), on `stream` (the cache-less out-of-place form's f(x))."""
+    fn = L.FDB_FN(f.address)
+    rc = fn(f.ctx_ptr, fx.data_ptr() if fx.numel() else None, x.data_ptr() if x.numel() else None, 1,
+            max(fx.numel(), 1), max(x.numel(), 1), C.c_void_p(stream))
+    if rc != 0:
+        raise L.FdbError(L.FDB_ERR_CALLBACK, f"user f! returned {rc}")
+
+
+def _oop_kind(sparsity, jac_prototype):
+    """(result kind, m, ncols) the pair (sparsity, jac_prototype) gives; m / ncols None where f and colorvec decide."""
+    if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC):
+        raise TypeError(f"not built: sparsity of type {type(sparsity).__name__} in the out-of-place Jacobian "
+                        "(SparseMatrixCSC or None)")
+    if jac_prototype is not None:
+        if isinstance(jac_prototype, SparseMatrixCSC):
+            pm, pn = jac_prototype.shape
+        elif isinstance(jac_prototype, torch.Tensor) and jac_prototype.dim() == 2 and \
+                (jac_prototype.shape[0] <= 1 or jac_prototype.stride(0) == 1):
+            pm, pn = jac_prototype.shape
+        else:
+            raise TypeError(f"not built: jac_prototype of type {type(jac_prototype).__name__} in the out-of-place "
+                            "Jacobian (a dense column-major tensor, a SparseMatrixCSC or None)")
+        if sparsity is not None and (pm, pn) != sparsity.shape:
+            raise ValueError(f"jac_prototype is {pm}x{pn} but sparsity is {sparsity.shape[0]}x{sparsity.shape[1]}")
+        kind = L.FDB_OOP_SPARSE if isinstance(jac_prototype, SparseMatrixCSC) else L.FDB_OOP_DENSE
+        return kind, int(pm), int(pn)
+    if sparsity is not None:
+        return L.FDB_OOP_DENSE, sparsity.m, sparsity.n
+    return L.FDB_OOP_RAW, None, None
+
+
+def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, fdtype=None, relstep=None, absstep=None,
+                               colorvec=None, sparsity=_DEFAULT, jac_prototype=None, dir=True, stream=None):
+    """J = finite_difference_jacobian(f, x, cache::JacobianCache, f_in=nothing; relstep, absstep, colorvec, sparsity,
+    jac_prototype, dir) (jacobians.jl:277-429), or - when `cache` is None or an fdtype string - the cache-less form
+    (:240-259), which evaluates f(x) once and passes it on as f_in.
+
+    f: an out-of-place Python callable, f(x) -> CUDA tensor of m values (f.batched = True: (batch, n) -> (batch, m);
+       complex step: complex128 in and out), or a NativeFn (the in-place fdb_fn; the trampoline is not needed).
+    x: float64 CUDA tensor, never modified; cache.x1 receives a copy of it (:293-295).
+    The result follows (sparsity, jac_prototype) as the reference's J + Ji does:
+        None / None                 dense m x maximum(colorvec) column-major tensor of the raw quotients
+        None / dense tensor         dense, column i = 0.0 + dx_i, the other columns +0.0
+        None / SparseMatrixCSC      SparseMatrixCSC holding the nonzero entries of each dx_i in column i
+        CSC / None or dense         dense size(sparsity): structural slots 0.0 + dx, +0.0 elsewhere (an invalid colouring
+                                    raises, as _make_Ji throws)
+        CSC / SparseMatrixCSC       SparseMatrixCSC with the structural entries whose value is not +-0.0 (NaN kept)
+    A sparse result is sized to the kept entries: reading that count is the call's one host synchronisation (when most
+    candidates were dropped its rowval / nzval are copied into storage of their own size).  Other sparsity / prototype
+    types and complex-valued results raise TypeError (not built).
+    Rows of the result: size(sparsity, 1) or size(jac_prototype, 1) when given; else those of f(x) — forward mode with a
+    Python f evaluates it first, as the reference does (:299-300), and passes it on as f_in — or of f_in; else length of
+    cache.fx (central and complex mode, and a NativeFn, whose output length the mirror cannot see before the device calls
+    it: build the cache as JacobianCache(x, fx) for m != n).  The cache-less form with a NativeFn sizes f(x) the same way,
+    from sparsity / prototype or length(x)."""
+    if cache is None or isinstance(cache, str):
+        fd = cache if isinstance(cache, str) else (fdtype or "forward")
+        if not _is_cuda(x) or x.dtype != torch.float64:
+            raise TypeError("x must be a float64 CUDA tensor: the GPU path has no CPU implementation")
+        xv = x.reshape(-1)
+        if f_in is None:                                                                  # :250-251
+            if stream is None:
+                stream = torch.cuda.current_stream(x.device).cuda_stream
+            if isinstance(f, NativeFn):
+                sp = None if sparsity is _DEFAULT else sparsity
+                m = sp.m if isinstance(sp, SparseMatrixCSC) else (
+                    jac_prototype.shape[0] if jac_prototype is not None else xv.numel())
+                xin = xv.to(torch.complex128) if _fdtype_code(fd) == L.FDB_COMPLEX else xv
+                fx = torch.empty(m, dtype=xin.dtype, device=x.device)
+                with torch.cuda.device(x.device):
+                    _native_call(f, fx, xin.contiguous(), stream)
+            else:
+                fx = f(x)
+                if not isinstance(fx, torch.Tensor) or not fx.is_cuda:
+                    raise TypeError("an out-of-place f must return a CUDA tensor")
+        else:
+            fx = f_in                                                                     # :252-253
+        if fx.is_complex() and _fdtype_code(fd) != L.FDB_COMPLEX:
+            raise TypeError("not built: f returns a complex array (complex-valued results of the out-of-place path)")
+        c = JacobianCache(xv, fx.reshape(-1).real.to(torch.float64) if fx.is_complex() else fx.reshape(-1), fd)
+        return finite_difference_jacobian(f, x, c, fx.real if fx.is_complex() else fx, relstep=relstep,
+                                          absstep=absstep, colorvec=range(1, xv.numel() + 1) if colorvec is None else colorvec,
+                                          sparsity=None if sparsity is _DEFAULT else sparsity, jac_prototype=jac_prototype,
+                                          dir=dir, stream=stream)                         # :255-258
+    if not isinstance(cache, JacobianCache):
+        raise TypeError("cache must be a JacobianCache, an fdtype string, or None")
+    if not _is_cuda(x) or x.dtype != torch.float64:
+        raise TypeError("x must be a float64 CUDA tensor: the GPU path has no CPU implementation")
+    fd = _fdtype_code(cache.fdtype)
+    colorvec = cache.colorvec if colorvec is None else colorvec                           # :284
+    sparsity = cache.sparsity if sparsity is _DEFAULT else sparsity                       # :285
+    kind, pm, pn = _oop_kind(sparsity, jac_prototype)
+    xv = x.reshape(-1)
+    if not xv.is_contiguous():
+        xv = xv.contiguous()
+    n = xv.numel()
+    if cache.x1 is not x:                                                                 # :293-295
+        cache.x1.reshape(-1).copy_(xv)
+    if f_in is None and fd == L.FDB_FORWARD and not isinstance(f, NativeFn):
+        # vecfx = _vec(f(x)) (:299-300) is evaluated here and handed on as f_in: the same call at the same point, still
+        # before the colours, and the row count is f's own
+        f_in = _oop_result(f(x), (-1,))
+    if f_in is not None:
+        if f_in.is_complex():
+            raise TypeError("not built: complex-valued f_in (complex-valued results of the out-of-place path)")
+        f_in = f_in.reshape(-1)
+    m = f_in.numel() if f_in is not None else cache.fx.numel()
+    if sparsity is not None:
+        m = sparsity.m
+        if sparsity.n != n:
+            raise ValueError(f"size(sparsity, 2) = {sparsity.n} != length(x) = {n}")
+    elif pm is not None and pm != m:
+        raise TypeError(f"not built: a {pm}-row jac_prototype for an f with {m} values")
+    dev = x.device
+    key = ("oop", kind, _sp_key(sparsity) if sparsity is not None else None, _index_key(colorvec), pn, m, n)
+    plan = cache._plans.get(key)
+    if plan is None:
+        h = C.c_void_p()
+        o = _opts(fd, _device_index(dev), **{k: v for k, v in cache._plan_kw.items() if k in ("max_batch", "scratch_bytes")})
+        cv = None if _is_identity_colorvec(colorvec, n) else colorvec
+        cvp, k3 = _index_ptr(cv)
+        with torch.cuda.device(dev):
+            if sparsity is not None:
+                cp, k1 = _index_ptr(sparsity.colptr)
+                rv, k2 = _index_ptr(sparsity.rowval)
+                L.check(L.lib().fdb_oop_plan_create_csc(C.byref(h), m, n, cp, rv, cvp, kind, max(m, 1), C.byref(o)))
+            else:
+                L.check(L.lib().fdb_oop_plan_create_dense(C.byref(h), m, n, cvp, pn or 0, kind, max(m, 1), C.byref(o)))
+        plan = Plan(h.value)
+        cache._plans[key] = plan
+    info = plan.info()
+    ncols = pn if pn is not None else info["n_local_colors"]
+    out = L.OopOut()
+    result = nnz_d = None
+    if kind == L.FDB_OOP_SPARSE:
+        cap = info["m"] * info["n_local_colors"] if sparsity is None else info["n_entries"]
+        colptr = torch.empty(ncols + 1, dtype=torch.int64, device=dev)
+        rowval = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
+        nzval = torch.empty(max(cap, 1), dtype=torch.float64, device=dev)
+        nnz_d = torch.empty(1, dtype=torch.int64, device=dev)
+        out.colptr, out.rowval, out.nzval, out.cap, out.nnz = (colptr.data_ptr(), rowval.data_ptr(), nzval.data_ptr(),
+                                                               cap, nnz_d.data_ptr())
+    else:
+        result = torch.empty((ncols, m), dtype=torch.float64, device=dev).t()            # column-major, ldJ = m
+        out.J = result.data_ptr() if result.numel() else _fx_ptr(result)                 # m = 0: nothing is written
+    addr, ctx, pyfn = _as_fn(f, m, n, dev, 1, fd == L.FDB_COMPLEX, oop=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+    fin_ptr = None
+    if f_in is not None and fd == L.FDB_FORWARD:                                          # :297-298
+        finv = _flat_f64(f_in, "f_in")
+        if finv.numel() != m:
+            raise ValueError("length(f_in) != the rows of the result")
+        fin_ptr = _fx_ptr(finv)
+    with torch.cuda.device(dev):
+        if fd == L.FDB_COMPLEX:
+            st = L.lib().fdb_jacobian_oop_complex(plan.handle, addr, ctx, xv.data_ptr(), C.byref(out), C.c_void_p(stream))
+        else:
+            st = L.lib().fdb_jacobian_oop(plan.handle, addr, ctx, xv.data_ptr(), C.byref(out), None, fin_ptr,
+                                          L.STEP_DEFAULT if relstep is None else float(relstep),
+                                          L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
+                                          C.c_void_p(stream))
+    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
+        exc, pyfn.exc = pyfn.exc, None
+        raise exc
+    L.check(st)
+    cache._last_plan = plan
+    if kind != L.FDB_OOP_SPARSE:
+        return result
+    with torch.cuda.device(dev):
+        L.check(L.lib().fdb_stream_sync(C.c_void_p(stream)))                              # the one host sync
+    nnz = int(nnz_d.item())
+    rowval, nzval = rowval[:nnz], nzval[:nnz]
+    if 2 * nnz < cap:                 # most candidates dropped: give the result storage of its own size
+        rowval, nzval = rowval.clone(), nzval.clone()
+    return SparseMatrixCSC(m, ncols, colptr, rowval, nzval)
+
+
+def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):
+    """jvp = finite_difference_jvp(f, x, v, cache::JVPCache, f_in=nothing; relstep, absstep, dir) (src/jvp.jl:159-189), or -
+    when `cache` is None or an fdtype string - the cache-less form (:133-146), which evaluates f(x) once and passes it on.
+    f is out of place as for finite_difference_jacobian.  Central mode evaluates f(x + eps v) before f(x - eps v).  Returns
+    a new float64 CUDA tensor of m values; the cache arrays are not written (x1 and fx1 are fresh arrays in the reference).
+    m is the length of f(x) in forward mode with a Python f (evaluated first, jvp.jl:175) or of f_in; else length of
+    cache.fx1 (central mode, a NativeFn: build the cache as JVPCache(x, fx1) for m != n)."""
+    if cache is None or isinstance(cache, str):
+        fd = cache if isinstance(cache, str) else "forward"
+        if f_in is None:
+            if isinstance(f, NativeFn):
+                fx = torch.empty(x.numel(), dtype=torch.float64, device=x.device)
+                with torch.cuda.device(x.device):
+                    _native_call(f, fx, x.reshape(-1).contiguous(),
+                                 stream if stream is not None else torch.cuda.current_stream(x.device).cuda_stream)
+            else:
+                fx = f(x)                                                                  # :139-140
+        else:
+            fx = f_in
+        if not isinstance(fx, torch.Tensor) or not fx.is_cuda:
+            raise TypeError("an out-of-place f must return a CUDA tensor")
+        if fx.is_complex():
+            raise TypeError("not built: f returns a complex array (complex-valued results of the out-of-place path)")
+        c = JVPCache(x.reshape(-1), fx.reshape(-1), fd)                                   # :144
+        return finite_difference_jvp(f, x, v, c, fx, relstep=relstep, absstep=absstep, dir=dir, stream=stream)
+    if not isinstance(cache, JVPCache):
+        raise TypeError("cache must be a JVPCache, an fdtype string, or None")
+    for t in (x, v):
+        if not _is_cuda(t) or t.dtype != torch.float64:
+            raise TypeError("x, v must be float64 CUDA tensors: the GPU path has no CPU implementation")
+    xv, vv = x.reshape(-1).contiguous(), v.reshape(-1).contiguous()
+    n = xv.numel()
+    if vv.numel() != n:
+        raise ValueError("length(v) != length(x)")
+    fin_ptr = finv = None
+    if f_in is None and cache._code == L.FDB_FORWARD and not isinstance(f, NativeFn):
+        f_in = _oop_result(f(x), (-1,))                                                   # fx = f(x)  :175
+    if f_in is not None:
+        if f_in.is_complex():
+            raise TypeError("not built: complex-valued f_in (complex-valued results of the out-of-place path)")
+        finv = _flat_f64(f_in, "f_in")
+        m = finv.numel()
+        if cache._code == L.FDB_FORWARD:                                                  # read forward only :175
+            fin_ptr = _fx_ptr(finv)
+    else:
+        m = cache.fx1.numel()
+    plan = cache.plan(m, n)
+    jvp = torch.empty(m, dtype=torch.float64, device=x.device)
+    x1 = torch.empty(n, dtype=torch.float64, device=x.device)
+    fx1 = torch.empty(m, dtype=torch.float64, device=x.device)
+    addr, ctx, pyfn = _as_fn(f, m, n, x.device, 1, oop=True)
+    if stream is None:
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+    with torch.cuda.device(x.device):
+        st = L.lib().fdb_jvp_oop(plan.handle, addr, ctx, _fx_ptr(jvp), xv.data_ptr() if n else None,
+                                 vv.data_ptr() if n else None, _fx_ptr(x1), _fx_ptr(fx1), fin_ptr,
+                                 L.STEP_DEFAULT if relstep is None else float(relstep),
+                                 L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
+    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
+        exc, pyfn.exc = pyfn.exc, None
+        raise exc
+    L.check(st)
+    cache._last_plan = plan
+    return jvp
 
 
 def _shape_of(J):

@@ -241,6 +241,16 @@ struct fdb_plan {
   int64_t alg_bytes = 0;
   int64_t last_eps_count = 0;
   bool complex_entry = false;   // set while fdb_jacobian_complex drives the call
+  // out-of-place Jacobian plans (fdjac_oop.cuh): the colour loop with pristine points and the forward step rule in central
+  // mode, then the result form of the out-of-place finite_difference_jacobian
+  int oop = 0;                  // 1: an out-of-place plan (fdb_jacobian rejects it)
+  int oop_kind = 0;             // FDB_OOP_RAW / FDB_OOP_DENSE / FDB_OOP_SPARSE
+  bool oop_entry = false;       // set while fdb_jacobian_oop drives the call
+  int64_t oop_ncols = 0;        // columns of the result
+  double *oop_vals = nullptr;   // sparse result: the candidate values (nzval of the sparsity, or the m x C dense block)
+  unsigned long long *oop_state = nullptr;   // sparse result: look-back words of the compaction, then its tile counter
+  int32_t *oop_tile_col = nullptr;           // sparse result of a CSC sparsity: first column starting in each tile
+  bool oop_fused = false;                    // sparse result, every colour's f! output resident: quotient + compaction fused
   // optional CUDA-graph replay of the whole call
   bool use_graph = false;
   cudaStream_t cstream = nullptr;
@@ -1361,7 +1371,8 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
     CU(cudaGetLastError());
     return FDB_OK;
   }
-  EpsParams prm{P->fdtype == FDB_CENTRAL ? 1 : 0, relstep, absstep, dir};
+  // out-of-place plans take the forward rule, dir included, in central mode too (jacobians.jl:379-380)
+  EpsParams prm{P->fdtype == FDB_CENTRAL && !P->oop ? 1 : 0, relstep, absstep, dir};
   if (P->eps_lists) {
     if (!P->tune.no_eps_lists) {
       dim3 grid((unsigned)std::min<int64_t>(P->eps_list_max_chunks, 1024), (unsigned)std::min<int32_t>(C, 65535));
@@ -1424,7 +1435,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
         PerturbArgs pa{};
         pa.x = x; pa.eps = P->eps;
         pa.xp = P->xp + q0 * sX; pa.xm = CENTRAL ? P->xm + q0 * sX : nullptr;
-        pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = P->no_drift ? 0 : 1;
+        pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = (P->no_drift || P->oop) ? 0 : 1; pa.oop = P->oop;
         pa.reverse = (P->tune.reverse >> 1) & 1;
         pa.kcount = (int32_t)std::min<int64_t>(kPerturbMaxPoints, kc - q0);
         for (int32_t q = 0; q < pa.kcount; ++q) pa.k[q] = P->local_colors[(size_t)(li0 + q0 + q)];
@@ -1534,6 +1545,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   };
 
   auto scatter_group = [&](int64_t g, int64_t l0, int64_t G) -> fdb_status {
+    if (P->oop_fused) return FDB_OK;   // out-of-place sparse result: the compaction forms the quotients (fdjac_oop.cuh)
     if (P->sp_kind == SP_CSC && P->strategy == 1) return scatter_lists(g, l0, G);
     if (P->sp_kind == SP_BANDED) {
       BandArgs a{};
@@ -1727,8 +1739,9 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
     fill_value<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(P->eps_cols, ncl, DBL_EPSILON);
     replicate_x_complex<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, sX, B, P->xp);
   } else {
-    component_eps<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, P->col_begin, ncl, CENTRAL ? 1 : 0, relstep,
-                                                                            absstep, dir, P->eps_cols);
+    // out-of-place plans: the forward rule, dir included, in central mode too (jacobians.jl:358)
+    component_eps<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, P->col_begin, ncl, CENTRAL && !P->oop ? 1 : 0,
+                                                                            relstep, absstep, dir, P->eps_cols);
     replicate_x<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, P->ldx, B, P->xp);
   }
   P->cnt.kernel_launches += 2;
@@ -1835,6 +1848,7 @@ fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, dou
   if (P->sp_kind == SP_EPS) return fail(FDB_ERR_INVALID, "this is a step-size plan: call fdb_color_eps");
   if (P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian plan: call fdb_hessian");
   if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "this is a derivative plan: call fdb_derivative");
+  if (P->oop && !P->oop_entry) return fail(FDB_ERR_INVALID, "this is an out-of-place plan: call fdb_jacobian_oop");
   if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
     return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
   DeviceGuard g(P->device);
@@ -1932,8 +1946,11 @@ fdb_status fdb_jvp_plan_create(fdb_plan **plan, int64_t m, int64_t n, const fdb_
   return FDB_OK;
 }
 
-fdb_status fdb_jvp(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
-                   double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
+// plus_first: the out-of-place form's central order, f(x + eps v) then f(x - eps v) (jvp.jl:180-183); the in-place form
+// evaluates the minus point first (:265-268)
+static fdb_status jvp_run(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
+                          double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream,
+                          bool plus_first) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
   if (P->sp_kind != SP_JVP) return fail(FDB_ERR_INVALID, "not a JVP plan (fdb_jvp_plan_create)");
   if ((P->n > 0 && (!d_x || !d_v)) || (P->m > 0 && !d_jvp)) return fail(FDB_ERR_INVALID, "NULL jvp, x or v");
@@ -1956,6 +1973,16 @@ fdb_status fdb_jvp(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double
   if (!central) {
     if (d_f_in) base = d_f_in;                                      // fx1 = f_in        :257-258
     else TRY(call_f(P, f, ctx, fx1, d_x, 1, s));                    // f(fx1, x)         :255
+  } else if (plus_first) {
+    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 0, x1, n, al_x1);   // x + eps v :180
+    TRY(call_f(P, f, ctx, d_jvp, x1, 1, s));                        // fx1 = f(x1)       :181
+    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 1, x1, n, al_x1);   // x - eps v :182
+    TRY(call_f(P, f, ctx, fx1, x1, 1, s));                          // fx = f(x1)        :183
+    jvp_quotient<<<P->grid(m), kThreads, 0, s>>>(d_jvp, fx1, P->eps, 1, m);                                   // :184
+    P->cnt.kernel_launches += 3;
+    CU(cudaGetLastError());
+    P->cnt.jacobians += 1;
+    return FDB_OK;
   } else {
     jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 1, x1, n, al_x1);   // x1 = x - eps v :264
     P->cnt.kernel_launches += 1;
@@ -1968,6 +1995,11 @@ fdb_status fdb_jvp(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double
   CU(cudaGetLastError());
   P->cnt.jacobians += 1;
   return FDB_OK;
+}
+
+fdb_status fdb_jvp(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
+                   double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
+  return jvp_run(P, f, ctx, d_jvp, d_x, d_v, d_x1, d_fx1, d_f_in, relstep, absstep, dir, stream, false);
 }
 
 // ------------------------------------------------------------------------------------------------ Hessian (src/hessians.jl:202-292)
@@ -2309,3 +2341,4 @@ fdb_status fdb_ipc_close(void *d_ptr) { CU(cudaIpcCloseMemHandle(d_ptr)); return
 }  // extern "C"
 
 #include "fdjac_group.cuh"
+#include "fdjac_oop.cuh"

@@ -22,6 +22,12 @@
 // saved value: forward writes back the caller's x[j] (pristine again at k == c+1), central writes back the value x1 held
 // before colour c, which is the caller's value only for c == 0 (pristine at k == 1).
 //
+// Out-of-place points (`oop`, jacobians.jl:341,381-382): `vecx ± eps_k*(colorvec .== k)` is built from the caller's x at
+// every colour, so every component is pristine at every call and nothing drifts:
+//        c(j) == k : x[j] ± eps_k            otherwise : x[j] ± z_k      (drift must be 0)
+// This is not the `no_drift` rule above, which restores a perturbed colour to a saved value and so turns a zero into
+// +0.0 from the colour after it on.
+//
 // Memory shape: one streaming pass, x read once (16-byte loads), every output written once (16-byte stores); the
 // colour ids come as one narrow load per pair, or from the closed form of a cyclic colouring (no colour stream); the eps
 // table sits in shared memory.
@@ -41,6 +47,7 @@ struct PerturbArgs {
   double *xp, *xm;
   int64_t n, ldx;
   int32_t C, drift, kcount;
+  int32_t oop;                    // out-of-place points: every component pristine at every colour (drift = 0)
   int32_t k[kPerturbMaxPoints];   // global colour id of each point
   int32_t aligned;                // x, xp, xm 16-byte aligned and ldx even
   int32_t reverse;                // walk the full tiles from the end of x to its start (the tail of x is what the pass
@@ -49,15 +56,15 @@ struct PerturbArgs {
 
 // zk = copysign(0, eps_k), the value the reference adds to the components outside colour k (see the table above)
 template <bool CENTRAL>
-__device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, double e, int drift, uint32_t k, double zk,
-                                            double &p, double &q) {
+__device__ __forceinline__ void perturb_one(double v, uint32_t c, bool valid, double e, int drift, int oop, uint32_t k,
+                                            double zk, double &p, double &q) {
   const bool mine = valid && c == k, done = valid && c < k;
   if (done && drift) {
     p = (v + e) - e;
     if (CENTRAL) q = (v - e) + e;
   } else {
     // the component still holds the caller's value at call k, or (a zero only) +0.0 left by an earlier whole colour
-    const bool pristine = done ? (k == c + 1 && (!CENTRAL || c == 0)) : k == 0;
+    const bool pristine = oop || (done ? (k == c + 1 && (!CENTRAL || c == 0)) : k == 0);
     const double y = (v == 0.0 && !pristine) ? 0.0 : v;
     const double w = mine ? e : zk;
     p = y + w;
@@ -113,7 +120,7 @@ perturb_colors(const PerturbArgs a, const CS colors) {
         const uint32_t k = (uint32_t)a.k[b];
         const double zk = Z ? copysign(0.0, eps_of(k)) : 0.0;
         auto one = [&](double v, uint32_t c, bool y, double e, double &p, double &q) {
-          if (Z) perturb_one<CENTRAL>(v, c, y, e, a.drift, k, zk, p, q);
+          if (Z) perturb_one<CENTRAL>(v, c, y, e, a.drift, a.oop, k, zk, p, q);
           else perturb_nonzero<CENTRAL>(v, c, y, e, a.drift, k, p, q);
         };
         double p0, q0, p1, q1;
@@ -147,7 +154,7 @@ perturb_colors(const PerturbArgs a, const CS colors) {
         if (NP > 1 && b >= a.kcount) break;
         const uint32_t k = (uint32_t)a.k[b];
         double p, q;
-        perturb_one<CENTRAL>(v, c, y, e, a.drift, k, copysign(0.0, eps_of(k)), p, q);
+        perturb_one<CENTRAL>(v, c, y, e, a.drift, a.oop, k, copysign(0.0, eps_of(k)), p, q);
         a.xp[(int64_t)b * a.ldx + j] = p;
         if (CENTRAL) a.xm[(int64_t)b * a.ldx + j] = q;
       }

@@ -22,11 +22,16 @@
 #   fdb_hessian) and finite_difference_gradient! (src/gradients.jl:390-473, the dense plan with m = 1), and the scalar-input
 #   entry points through fdb_derivative: finite_difference_derivative! on CuVector{Float64} x (src/derivatives.jl:197-233)
 #   and finite_difference_gradient! at a Real x into a CuVector{Float64} df (src/gradients.jl:477-533).
-# Everything else of FiniteDiff.jl (CPU arrays, complex x, out-of-place forms) keeps using the stock package.
+#   The out-of-place finite_difference_jacobian (src/jacobians.jl:240-429) and finite_difference_jvp (src/jvp.jl:133-189)
+#   on CuVector{Float64} x go through fdb_jacobian_oop / fdb_jvp_oop: the trampoline copies the array f returns into the
+#   slot f! would have written.
+# Everything else of FiniteDiff.jl (CPU arrays, complex x, other sparsity / prototype types of the out-of-place form)
+# keeps using the stock package.
 module FiniteDiffB200
 
 using FiniteDiff, SparseArrays, CUDA
 import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache,
+    finite_difference_jacobian, finite_difference_jvp,
     finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache, finite_difference_derivative!,
     DerivativeCache
 
@@ -35,6 +40,7 @@ const libfdjac = get(ENV, "FDJAC_B200_LIB", "libfdjac_b200.so")
 const FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = Cint(0), Cint(1), Cint(2), Cint(3)
 const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS = Cint(0), Cint(1), Cint(2), Cint(3)
 const FDB_STEP_DEFAULT = NaN            # relstep / absstep keyword not given (include/fdjac_b200.h)
+const FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = Cint(0), Cint(1), Cint(2)
 
 # mirror of fdb_plan_opts (include/fdjac_b200.h) — field order and widths are checked by tests/test_julia_binding_cpu.py
 struct PlanOpts
@@ -693,5 +699,155 @@ end
 
 set_external_eps!(plan::Plan, eps::CuVector{Float64}) =
     check(ccall((:fdb_plan_set_external_eps, libfdjac), Cint, (Ptr{Cvoid}, CuPtr{Float64}), plan.handle, pointer(eps)))
+
+# ---- out-of-place forms: J = finite_difference_jacobian(f, x, cache, f_in; …)  src/jacobians.jl:240-429, and
+#      jvp = finite_difference_jvp(f, x, v, cache, f_in; …)  src/jvp.jl:133-189.  f(x) returns a new array; the trampoline
+#      copies it into the slot the library hands out.
+oop_f(f) = (fx, xv) -> (copyto!(fx, vec(f(xv))); nothing)
+
+# mirror of fdb_oop_out (include/fdjac_b200.h)
+struct OopOut
+    J::CuPtr{Float64}
+    colptr::CuPtr{Int64}
+    rowval::CuPtr{Int64}
+    nzval::CuPtr{Float64}
+    cap::Int64
+    nnz::CuPtr{Int64}
+end
+
+function oop_plan(anchor, sp, m::Integer, n::Integer, kind::Cint, ncols::Integer, colorvec, fd::Cint)
+    key = (:oop, kind, m, n, ncols, sp === nothing ? 0 : objectid(sp.rowval), color_key(colorvec), fd)
+    cached_plan(anchor, key) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd))
+        cptr, croot = color_arg(colorvec, n)
+        GC.@preserve sp croot begin
+            if sp === nothing
+                check(ccall((:fdb_oop_plan_create_dense, libfdjac), Cint,
+                    (Ref{Ptr{Cvoid}}, Int64, Int64, Ptr{Int64}, Int64, Cint, Int64, Ref{PlanOpts}),
+                    h, m, n, cptr, ncols, kind, max(m, 1), opts))
+            else
+                check(ccall((:fdb_oop_plan_create_csc, libfdjac), Cint,
+                    (Ref{Ptr{Cvoid}}, Int64, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+                    h, m, n, pointer(sp.colptr), pointer(sp.rowval), cptr, kind, max(m, 1), opts))
+            end
+        end
+        Plan(h[], (sp, croot))
+    end
+end
+
+hostcsc(A::DeviceCSC) = A.host
+hostcsc(A::SparseMatrixCSC) = A
+hostcsc(A) = throw(ArgumentError("not built: $(typeof(A)) in the out-of-place Jacobian (SparseMatrixCSC, DeviceCSC or nothing)"))
+
+"""
+    finite_difference_jacobian(f, x::CuVector{Float64}, cache::JacobianCache, f_in = nothing;
+                               relstep, absstep, colorvec, sparsity, jac_prototype, dir)
+
+`src/jacobians.jl:277-429` on the device.  The result follows (sparsity, jac_prototype) as `J + Ji` does in the reference:
+a dense `CuMatrix` (raw quotients without either, `0.0 + dx` with a dense prototype or a CSC sparsity) or, with a sparse
+prototype, a `DeviceCSC` holding the entries whose value is not ±0.0 (its pattern is copied back to the host: reading the
+kept count is the call's one synchronisation).  `cache.x1` receives a copy of x (:293-295).
+"""
+function finite_difference_jacobian(f, x::CuVector{Float64},
+        cache::JacobianCache{T1, T2, T3, T4, cType, sType, fdtype, returntype}, f_in = nothing;
+        relstep = nothing, absstep = relstep, colorvec = cache.colorvec, sparsity = cache.sparsity,
+        jac_prototype = nothing, dir = true) where {T1, T2, T3, T4, cType, sType, fdtype, returntype}
+    cache.x1 === x || copyto!(cache.x1, x)
+    n = length(x)
+    sp = sparsity === nothing ? nothing : hostcsc(sparsity)
+    m = sp !== nothing ? size(sp, 1) : (f_in !== nothing ? length(f_in) : length(cache.fx))
+    if jac_prototype === nothing
+        kind, ncols = sp === nothing ? (FDB_OOP_RAW, 0) : (FDB_OOP_DENSE, n)
+    elseif jac_prototype isa AbstractMatrix && !(jac_prototype isa SparseMatrixCSC)
+        kind, ncols = FDB_OOP_DENSE, size(jac_prototype, 2)
+    else
+        kind, ncols = FDB_OOP_SPARSE, size(hostcsc(jac_prototype), 2)
+    end
+    fd = fdcode(fdtype)
+    plan = oop_plan(sp === nothing ? cache : sp.colptr, sp, m, n, kind, ncols, colorvec, fd)
+    pinfo = info(plan)
+    kind == FDB_OOP_RAW && (ncols = pinfo.n_local_colors)
+    st = FnState(oop_f(f), m, n, nothing)
+    J = nothing
+    colptr = rowval = nzval = nnz = nothing
+    if kind == FDB_OOP_SPARSE
+        cap = sp === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
+        colptr, rowval = CuVector{Int64}(undef, ncols + 1), CuVector{Int64}(undef, max(cap, 1))
+        nzval, nnz = CuVector{Float64}(undef, max(cap, 1)), CuVector{Int64}(undef, 1)
+        out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), cap, pointer(nnz)))
+    else
+        J = CuMatrix{Float64}(undef, max(m, 1), ncols)
+        out = Ref(OopOut(pointer(J), CU_NULL, CU_NULL, CU_NULL, 0, CU_NULL))
+    end
+    rc = Cint(0)
+    GC.@preserve st x J colptr rowval nzval nnz f_in begin
+        if fdtype == Val(:complex)
+            cfc = @cfunction(f_trampoline_c, Cint, (Ptr{Cvoid}, CuPtr{ComplexF64}, CuPtr{ComplexF64}, Int64, Int64, Int64, Ptr{Cvoid}))
+            rc = ccall((:fdb_jacobian_oop_complex, libfdjac), Cint,
+                (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, Ref{OopOut}, Ptr{Cvoid}),
+                plan.handle, cfc, pointer_from_objref(st), pointer(x), out, CUDA.stream().handle)
+        else
+            cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+            rc = ccall((:fdb_jacobian_oop, libfdjac), Cint,
+                (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, Ref{OopOut}, CuPtr{Float64}, CuPtr{Float64},
+                    Float64, Float64, Float64, Ptr{Cvoid}),
+                plan.handle, cf, pointer_from_objref(st), pointer(x), out, CU_NULL,
+                (f_in === nothing || fdtype != Val(:forward)) ? CU_NULL : pointer(f_in),
+                stepval(relstep), stepval(absstep), Float64(dir), CUDA.stream().handle)
+        end
+    end
+    st.err === nothing || throw(st.err)
+    check(rc)
+    kind == FDB_OOP_SPARSE || return m == 0 ? J[1:0, :] : J
+    k = Int(Array(nnz)[1])                                     # the one host synchronisation
+    host = SparseMatrixCSC(m, ncols, Array(colptr), Array(rowval[1:k]), zeros(k))
+    DeviceCSC(host, nzval[1:k])
+end
+
+# cache-less form :240-259: f(x) once, then the cached form with it as f_in
+function finite_difference_jacobian(f, x::CuVector{Float64}, fdtype = Val(:forward), returntype = eltype(x), f_in = nothing;
+        kw...)
+    fdtype isa Type && (fdtype = fdtype())
+    fx = f_in === nothing ? f(x) : f_in
+    cache = JacobianCache(x, fdtype == Val(:complex) ? real(fx) : fx, fdtype, returntype)
+    finite_difference_jacobian(f, x, cache, fdtype == Val(:complex) ? real(fx) : fx; kw...)
+end
+
+"""
+    finite_difference_jvp(f, x::CuVector{Float64}, v::CuVector{Float64}, cache::JVPCache, f_in = nothing; relstep, absstep, dir)
+
+`src/jvp.jl:159-189` on the device (fdb_jvp_oop): central mode evaluates f(x + εv) before f(x − εv).  Returns a new
+`CuVector{Float64}`; the cache arrays are not written.
+"""
+function finite_difference_jvp(f, x::CuVector{Float64}, v::CuVector{Float64}, cache::JVPCache{X1, FX1, fdtype},
+        f_in = nothing; relstep = nothing, absstep = relstep, dir = true) where {X1, FX1, fdtype}
+    fdtype == Val(:complex) && error("finite_difference_jvp doesn't support :complex-mode finite diff")
+    m, n = f_in === nothing ? length(cache.fx1) : length(f_in), length(x)
+    plan = jvp_plan(m, n, fdcode(fdtype))
+    jvp, x1, fx1 = CuVector{Float64}(undef, m), CuVector{Float64}(undef, n), CuVector{Float64}(undef, m)
+    st = FnState(oop_f(f), m, n, nothing)
+    cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+    rc = Cint(0)
+    GC.@preserve st jvp x v x1 fx1 f_in begin
+        rc = ccall((:fdb_jvp_oop, libfdjac), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64},
+                CuPtr{Float64}, Float64, Float64, Float64, Ptr{Cvoid}),
+            plan.handle, cf, pointer_from_objref(st), pointer(jvp), pointer(x), pointer(v), pointer(x1), pointer(fx1),
+            (f_in === nothing || fdtype != Val(:forward)) ? CU_NULL : pointer(f_in), stepval(relstep), stepval(absstep),
+            Float64(dir), CUDA.stream().handle)
+    end
+    st.err === nothing || throw(st.err)
+    check(rc)
+    jvp
+end
+
+# cache-less form :133-146
+function finite_difference_jvp(f, x::CuVector{Float64}, v::CuVector{Float64}, fdtype = Val(:forward), f_in = nothing;
+        kw...)
+    fdtype isa Type && (fdtype = fdtype())
+    fx = f_in === nothing ? f(x) : f_in
+    finite_difference_jvp(f, x, v, JVPCache(x, fx, fdtype), fx; kw...)
+end
 
 end # module

@@ -365,6 +365,57 @@ fdb_status fdb_derivative(fdb_plan *plan, fdb_fn f, void *ctx, double *d_df, con
                           double relstep, double absstep, double dir, void *stream);
 fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double *d_df, const double *d_x, void *stream);
 
+/* ---- Out-of-place Jacobian: J = finite_difference_jacobian(f, x, cache, f_in; relstep, absstep, colorvec, sparsity,
+ *      jac_prototype, dir)  src/jacobians.jl:277-429 (cache-less form :240-259 = f(x) once, then the cached form).
+ * Differences from the in-place colour loop, all reproduced:
+ *   - every point starts from the caller's x: colour k gets x +- eps_k on its columns and x +- copysign(0, eps_k) on every
+ *     other component (sparsity given, :341,381-382); the dense branch changes component i alone (:322,359-360);
+ *   - central mode takes the forward step rule, dir included (:358,379-380);
+ *   - the result is J + Ji summed over the colours, whose form depends on jac_prototype (result_kind):
+ *       FDB_OOP_RAW     sparsity === nothing, no prototype: dense m x maximum(colorvec) holding the raw quotients (:329-331)
+ *       FDB_OOP_DENSE   a dense result (prototype dense, or sparsity given without a sparse prototype): structural slots
+ *                       hold 0.0 + q (-0.0 becomes +0.0), every other element +0.0
+ *       FDB_OOP_SPARSE  a SparseMatrixCSC prototype: the structural entries whose quotient is not +-0.0 (NaN is kept), in
+ *                       storage order (SparseArrays' zero-preserving `+`); sparsity === nothing: the nonzeros of every column
+ *   f! call count and order: forward f(x) (unless d_f_in) then one call per colour; central f(x+) then f(x-) per colour;
+ *   complex one call per colour.  d_x is never modified.
+ * fdb_oop_plan_create_csc: sparsity is a CSC pattern (Int64, 1-based, host or device), result_kind FDB_OOP_DENSE (J dense
+ *   m x n with leading dimension ldJ; a colouring in which two columns of one colour share a row is FDB_ERR_INVALID, as
+ *   _make_Ji throws, :151-162) or FDB_OOP_SPARSE (ldJ ignored; any colouring).
+ * fdb_oop_plan_create_dense: sparsity === nothing.  C = maximum(colorvec) (NULL => n) must be in 1..n.  FDB_OOP_RAW: J is
+ *   m x C (ncols_out ignored); FDB_OOP_DENSE: J is m x ncols_out with ncols_out >= C (a narrower prototype is not built:
+ *   FDB_ERR_UNSUPPORTED); FDB_OOP_SPARSE: ncols_out >= C (else FDB_ERR_INVALID, as sparse() throws).
+ * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans; world <= 1.
+ * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
+ *   dense kinds: out->J (device, ldJ of the plan);
+ *   FDB_OOP_SPARSE: out->colptr [ncols + 1], out->rowval / out->nzval [out->cap >= the candidate count: nnz of the sparsity,
+ *   or m*C], Int64 1-based; the kept count goes to the device scalar *out->nnz (stream-ordered, no host sync).
+ * fdb_plan_info(...).n_entries is the candidate count of a sparse result. */
+enum { FDB_OOP_RAW = 0, FDB_OOP_DENSE = 1, FDB_OOP_SPARSE = 2 };
+
+typedef struct {
+  double *J;                 /* dense kinds */
+  int64_t *colptr, *rowval;  /* FDB_OOP_SPARSE */
+  double *nzval;
+  int64_t cap;
+  int64_t *nnz;              /* device scalar */
+} fdb_oop_out;
+
+fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval,
+                                   const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colorvec, int64_t ncols_out,
+                                     int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_jacobian_oop(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
+                            const double *d_f_in, double relstep, double absstep, double dir, void *stream);
+fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
+                                    void *stream);
+
+/* Out-of-place JVP: jvp = finite_difference_jvp(f, x, v, cache, f_in; relstep, absstep, dir)  src/jvp.jl:159-189.  Same
+ * plan (fdb_jvp_plan_create) and arguments as fdb_jvp; central mode evaluates f(x + eps v) into d_jvp BEFORE f(x - eps v)
+ * into d_fx1 (:180-183; the in-place form calls them the other way round). */
+fdb_status fdb_jvp_oop(fdb_plan *plan, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
+                       double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream);
+
 /* ---- helpers for hosts without their own CUDA bindings ---- */
 fdb_status fdb_host_alloc(void **p, size_t bytes);  /* pinned host memory */
 fdb_status fdb_host_free(void *p);
