@@ -114,6 +114,8 @@ ABI_SYMBOLS = {
     "fdb_jvp_oop": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
     "fdb_hessian_plan_create": (_int, [_PP, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_hessian": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _vp]),
+    "fdb_group_create_hessian": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, C.POINTER(PlanOpts)]),
+    "fdb_group_hessian": (_int, [_vp, _vp, C.POINTER(_vp), _vp, _vp, _vp, _f64, _f64, _vp]),
     "fdb_derivative_plan_create": (_int, [_PP, _i64, C.POINTER(PlanOpts)]),
     "fdb_scalar_gradient_plan_create": (_int, [_PP, _i64, C.POINTER(PlanOpts)]),
     "fdb_derivative": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),

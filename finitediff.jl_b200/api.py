@@ -1309,7 +1309,9 @@ class HessianCache:
 
     The cache arrays are scratch (the reference copies x into them before use, :213-216): a cache built from another x
     changes nothing (issue #185, finitedifftests.jl:608-614).  The GPU path keeps its points in plan-owned memory and
-    does not touch them.  Extra keywords (GPU path only): max_batch, scratch_bytes, use_graph."""
+    does not touch them.  Extra keywords (GPU path only): max_batch, scratch_bytes, use_graph, and rank / world: the
+    plan then evaluates f(x) and the points of rank's share of the i-blocks only and writes only the entries it owns
+    (include/fdjac_b200.h, fdb_hessian_plan_create; distributed.GroupHessian drives all ranks from one process)."""
 
     def __init__(self, *arrays, fdtype="hcentral", **plan_kw):
         if len(arrays) == 2 and not isinstance(arrays[1], torch.Tensor):     # HessianCache(x, fdtype)

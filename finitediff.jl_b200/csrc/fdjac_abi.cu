@@ -228,6 +228,8 @@ struct fdb_plan {
   // boundaries [hess_chunks[c], hess_chunks[c+1]) in i
   double *hess_V = nullptr;
   std::vector<int64_t> hess_chunks;
+  // rank plans: local point q > 0 is global point q + hess_off; hess_points = the rank's f evaluations per call
+  int64_t hess_off = 0, hess_points = 0;
   // derivative plans (kernels_derivative.cuh): elementwise derivative (m = n) or scalar -> vector gradient (n = 1)
   bool deriv_elem = false;
   int64_t deriv_fcalls = 0;   // f evaluations of the most recent call (before any: the count without cache.fx)
@@ -1169,7 +1171,7 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   info->n_groups = P->n_groups;
   info->slabs = P->slabs;
   info->fcalls_per_jacobian = P->fdtype == FDB_CENTRAL ? 2 * n_local : (P->fdtype == FDB_COMPLEX ? n_local : 1 + n_local);
-  if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = 2 * P->n * P->n + 1;
+  if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = P->hess_points;
   if (P->sp_kind == SP_DERIV) info->fcalls_per_jacobian = P->deriv_fcalls;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
@@ -1234,11 +1236,11 @@ fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *strea
   if (!P || !h_eps) return fail(FDB_ERR_INVALID, "NULL argument");
   if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "derivative plans keep no step sizes (the quotient pass recomputes them)");
   DeviceGuard g(P->device);
-  // JVP plans: C == 1; Hessian plans: one step per component (col_begin = 0, col_end = n)
+  // JVP plans: C == 1; Hessian plans: the steps of the rank's components [col_begin, col_end) (eps_cols holds all n)
   const bool per_column = P->sp_kind == SP_NONE || P->sp_kind == SP_HESS;
   const int64_t count = per_column ? P->col_end - P->col_begin : P->C;
   if (cap < count) return fail(FDB_ERR_INVALID, "h_eps too small (%lld < %lld)", (long long)cap, (long long)count);
-  const double *src = per_column ? P->eps_cols : P->eps;
+  const double *src = per_column ? P->eps_cols + (P->sp_kind == SP_HESS ? P->col_begin : 0) : P->eps;
   if (count > 0) {
     CU(cudaMemcpyAsync(h_eps, src, (size_t)count * 8, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     CU(cudaStreamSynchronize((cudaStream_t)stream));
@@ -2010,6 +2012,26 @@ static constexpr int64_t kHessMaxN = (int64_t)1 << 24;
 // Hessian (requests above the cap are clamped to it).
 static constexpr int64_t kHessBatchCap = 4096;
 
+// First i-block of rank r of `world` (see fdb_hessian_plan_create in the header): i_0 = 0, i_world = n, and for
+// 0 < r < world the i in [i_{r-1}, n] whose S(i) - 1 is nearest to r*T/world (T = 2n^2), ties to the smaller i.  The
+// distance is compared exactly as |world*(S(i) - 1) - r*T| (below 2^56 for n <= 2^24, world <= 64).  S is increasing, so
+// the nearest i is the first i whose S(i) - 1 reaches the target or the one before it.
+static int64_t hess_rank_begin(int64_t n, int world, int r) {
+  if (r >= world) return n;
+  int64_t lo = 0;
+  for (int k = 1; k <= r; ++k) {
+    const int64_t target = (int64_t)k * 2 * n * n;
+    int64_t a = lo, b = n;    // first i in [lo, n] with world*(S(i) - 1) >= target (n when none does)
+    while (a < b) {
+      const int64_t mid = (a + b) >> 1;
+      if (world * (hess_block_start(mid, n) - 1) >= target) b = mid; else a = mid + 1;
+    }
+    if (a > lo && target - world * (hess_block_start(a - 1, n) - 1) <= world * (hess_block_start(a, n) - 1) - target) --a;
+    lo = a;
+  }
+  return lo;
+}
+
 fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, const fdb_plan_opts *opts) {
   if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
   *plan = nullptr;
@@ -2018,7 +2040,7 @@ fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, cons
   if (n < 0) return fail(FDB_ERR_INVALID, "negative dimension n=%lld", (long long)n);
   if (ldH < n) return fail(FDB_ERR_INVALID, "ldH < n");
   if (n > kHessMaxN) return fail(FDB_ERR_UNSUPPORTED, "Hessian plans need n <= %lld", (long long)kHessMaxN);
-  if (opts->world > 1) return fail(FDB_ERR_UNSUPPORTED, "Hessian plans run on one device (world must be <= 1)");
+  if (opts->world > 64) return fail(FDB_ERR_INVALID, "Hessian plans take world <= 64");
   fdb_plan_opts o = *opts;
   o.fdtype = FDB_CENTRAL;   // new_plan validates the Jacobian fdtypes; the Hessian's is set below
   PlanPtr owner;
@@ -2030,41 +2052,49 @@ fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, cons
   P->jkind = FDB_J_DENSE;
   P->ldJ = ldH;
   P->j_len = ldH * n;
-  P->E = n * n;
   P->C = (int32_t)std::min<int64_t>(n, INT32_MAX);
-  P->col_begin = 0;
-  P->col_end = n;
+  // this rank's i-blocks [i0, i1) (all of them on one device); it owns column i rows [i, n) and row i columns (i, n)
+  const int64_t ib = hess_rank_begin(n, P->world, P->rank), ie = hess_rank_begin(n, P->world, P->rank + 1);
+  const int64_t nb = ie - ib, own_points = hess_block_start(ie, n) - hess_block_start(ib, n);
+  P->col_begin = ib;
+  P->col_end = ie;
+  P->E = nb * (2 * n - 1) - (ie * (ie - 1) - ib * (ib - 1));
+  P->hess_off = hess_block_start(ib, n) - 1;
+  // f(x) first (the diagonal needs it), then the rank's own points; rank 0 always evaluates f(x) (n = 0 included), a
+  // rank > 0 without i-blocks evaluates nothing
+  const bool idle = nb == 0 && P->rank > 0;
+  P->hess_points = idle ? 0 : 1 + own_points;
   P->ldF = 1;
   P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
-  const int64_t total = 2 * n * n + 1;
   const int64_t budget = opts->scratch_bytes > 0 ? opts->scratch_bytes : (int64_t)8 << 30;
   // ONE budget for both buffers: the resident point rows X[0..B) take at most half of it, the value buffer V the rest
   int64_t batch = opts->max_batch > 1 ? opts->max_batch : 1;
   batch = std::max<int64_t>(1, std::min<int64_t>(batch, budget / 2 / (8 * P->ldx)));
-  batch = std::min<int64_t>(std::min<int64_t>(batch, total), kHessBatchCap);
+  batch = std::min<int64_t>(std::min<int64_t>(batch, std::max<int64_t>(P->hess_points, 1)), kHessBatchCap);
   P->batch = batch;
   P->slabs = batch;
   // chunks of whole i-blocks whose values fit the budget (at least one i-block each), so that the <= 4 values of an
   // entry are always in the same chunk
   const int64_t cap = std::max<int64_t>((budget - batch * P->ldx * 8) / 8 - 1, 0);
-  P->hess_chunks.assign(1, 0);
+  P->hess_chunks.assign(1, ib);
   int64_t max_vals = 0;
-  for (int64_t i0 = 0; i0 < n;) {
+  for (int64_t i0 = ib; i0 < ie;) {
     int64_t i1 = i0 + 1;
-    while (i1 < n && hess_block_start(i1 + 1, n) - hess_block_start(i0, n) <= cap) ++i1;
+    while (i1 < ie && hess_block_start(i1 + 1, n) - hess_block_start(i0, n) <= cap) ++i1;
     max_vals = std::max<int64_t>(max_vals, hess_block_start(i1, n) - hess_block_start(i0, n));
     P->hess_chunks.push_back(i1);
     i0 = i1;
   }
-  if (n == 0) P->hess_chunks.push_back(0);   // one chunk of no i-blocks: f(x) alone
+  if (nb == 0 && !idle) P->hess_chunks.push_back(ib);   // one chunk of no i-blocks: f(x) alone
   P->n_groups = (int64_t)P->hess_chunks.size() - 1;
   TRY(P->alloc_t(&P->hess_V, (size_t)(1 + max_vals)));
   TRY(P->alloc_t(&P->xp, (size_t)(batch * P->ldx)));
   TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(n, 1)));
-  // byte model per Hessian: values read back by the assembly, H written, the one-time replication of x into the B rows,
-  // and the patches (each changed component written once and restored once: 2 per diagonal point, 4 per other point)
-  const int64_t patched = 2 * n + 8 * (n * (n - 1) / 2);
-  P->alg_bytes = 8 * total + 8 * n * n + 8 * n * batch + 16 * patched;
+  // byte model per Hessian (this rank's share): values read back by the assembly, owned entries of H written, the
+  // one-time replication of x into the B rows, and the patches (each changed component written once and restored once:
+  // 2 per diagonal point, 4 per other point)
+  const int64_t patched = 2 * own_points - 2 * nb;
+  P->alg_bytes = idle ? 0 : 8 * P->hess_points + 8 * P->E + 8 * n * batch + 16 * patched;
   *plan = owner.release();
   return FDB_OK;
 }
@@ -2079,16 +2109,20 @@ static fdb_status hessian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *
     replicate_x<<<P->grid(n), kThreads, 0, s>>>(x, n, ldx, B, P->xp);
     P->cnt.kernel_launches += 2;
   }
+  // p0 / p_end run over the rank's local sequence (point q > 0 is global point q + off, kernels_hessian.cuh); a chunk's
+  // points sit at V[1 ..] whatever its rank
+  const int64_t off = P->hess_off;
   int64_t prev_p0 = 0;
   int32_t prev_cnt = 0;
   for (size_t c = 0; c + 1 < P->hess_chunks.size(); ++c) {
     const int64_t i0 = P->hess_chunks[c], i1 = P->hess_chunks[c + 1];
-    const int64_t cs = hess_block_start(i0, n);
-    const int64_t p_end = hess_block_start(i1, n);
+    const int64_t cs = hess_block_start(i0, n) - off;
+    const int64_t p_end = hess_block_start(i1, n) - off;
     for (int64_t p0 = c == 0 ? 0 : cs; p0 < p_end; p0 += B) {
       const int32_t cnt = (int32_t)std::min<int64_t>(B, p_end - p0);
       if (n > 0) {
-        hess_patch<<<P->grid(std::max(cnt, prev_cnt)), kThreads, 0, s>>>(x, P->eps_cols, n, ldx, p0, cnt, prev_p0, prev_cnt, P->xp);
+        hess_patch<<<P->grid(std::max(cnt, prev_cnt)), kThreads, 0, s>>>(x, P->eps_cols, n, ldx, off, p0, cnt, prev_p0,
+                                                                          prev_cnt, P->xp);
         P->cnt.kernel_launches += 1;
       }
       // f(x) (:209), f(_xpp), f(_xmm) (:233), f(_xpp), f(_xpm), f(_xmp), f(_xmm) (:268-269), in this order
@@ -2120,6 +2154,10 @@ fdb_status fdb_hessian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, doub
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
   cudaStream_t s = (cudaStream_t)stream;
+  if (P->hess_points == 0) {                 // a rank > 0 without i-blocks: no f call, no launch, d_fx untouched
+    P->cnt.jacobians += 1;
+    return FDB_OK;
+  }
   resolve_steps(FDB_HCENTRAL, relstep, absstep);                    // hessians.jl:204-205
   const GraphKey key{(void *)f, ctx, d_x, d_H, d_fx, nullptr, relstep, absstep, 1.0, 0, 0, nullptr};
   const fdb_status st = run_maybe_graph(P, key, s, "Hessian", [&](cudaStream_t cs) {

@@ -140,6 +140,50 @@ static fdb_status group_create(fdb_group **out, int n_devices, const int *device
   return FDB_OK;
 }
 
+// member i's view of `count` doubles the root holds at src: src itself when member i runs on the root's device, else a
+// replica on its own device (allocated on first use) refreshed by a peer copy on the member's stream s
+static fdb_status member_replica(fdb_group *g, int i, std::vector<double *> &rep, const double *src, int64_t count,
+                                 cudaStream_t s, const double **out) {
+  *out = src;
+  const int dev = g->devices[i], root = g->devices[0];
+  if (dev == root) return FDB_OK;
+  if (!rep[i]) CU(cudaMalloc((void **)&rep[i], (size_t)std::max<int64_t>(count, 2) * 8));
+  if (count > 0) CU(cudaMemcpyPeerAsync(rep[i], dev, src, root, (size_t)count * 8, s));
+  *out = rep[i];
+  return FDB_OK;
+}
+
+// The ordering every group call follows: members > 0 start after what the caller's stream `s0` holds so far (the start
+// event), each on its own stream with x replicated to its device, then the root runs on s0, and s0 waits for every
+// member.  No host synchronisation.  run(i, x_i, stream) enqueues member i's work; skip(i) leaves out a member that
+// has nothing to do.
+template <typename Run, typename Skip>
+static fdb_status group_run(fdb_group *g, const double *d_x, cudaStream_t s0, Run &&run, Skip &&skip) {
+  const int root = g->devices[0];
+  {
+    DeviceGuard dg(root);
+    if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
+    CU(cudaEventRecord(g->ev_start, s0));
+  }
+  for (int i = 1; i < g->n; ++i) {
+    if (skip(i)) continue;
+    const int dev = g->devices[i];
+    DeviceGuard dg(dev);
+    if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", dev);
+    cudaStream_t s = g->streams[i];
+    CU(cudaStreamWaitEvent(s, g->ev_start, 0));
+    const double *xi = d_x;
+    TRY(member_replica(g, i, g->x_rep, d_x, g->nx, s, &xi));
+    TRY(run(i, xi, s));
+    CU(cudaEventRecord(g->ev_done[i], s));
+  }
+  DeviceGuard dg(root);
+  TRY(run(0, d_x, s0));
+  for (int i = 1; i < g->n; ++i)
+    if (!skip(i)) CU(cudaStreamWaitEvent(s0, g->ev_done[i], 0));
+  return FDB_OK;
+}
+
 extern "C" {
 
 fdb_status fdb_group_create_csc(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
@@ -182,9 +226,17 @@ fdb_status fdb_group_plan(const fdb_group *group, int member, fdb_plan **plan) {
   return FDB_OK;
 }
 
+fdb_status fdb_group_create_hessian(fdb_group **group, int n_devices, const int *devices, int64_t n, int64_t ldH,
+                                    const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_hessian_plan_create(p, n, ldH, o);
+  });
+}
+
 fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const double *d_x, double *d_J, double *d_fx,
                               const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
   if (!g || !f) return fail(FDB_ERR_INVALID, "NULL group or f");
+  if (g->kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian group: call fdb_group_hessian");
   fdb_plan *P0 = g->plans[0];
   if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
   if ((P0->n > 0 && !d_x) || !d_J) return fail(FDB_ERR_INVALID, "NULL x or J");
@@ -195,37 +247,25 @@ fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const do
     if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
     // fill_matrix!(J, false) once, by the owner of the buffer, before any member may store into it
     if (g->n > 1 && P0->sp_kind != SP_NONE && !plan_self_defining(P0) && P0->j_len > 0) TRY(zero_J(P0, d_J, s0));
-    CU(cudaEventRecord(g->ev_start, s0));
   }
-  for (int i = 1; i < g->n; ++i) {
+  return group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {
     fdb_plan *P = g->plans[i];
-    const int dev = g->devices[i];
-    DeviceGuard dg(dev);
-    if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", dev);
-    cudaStream_t s = g->streams[i];
-    CU(cudaStreamWaitEvent(s, g->ev_start, 0));
-    const double *xi = d_x, *fin_i = d_f_in;
-    if (dev != root) {
-      if (!g->x_rep[i]) CU(cudaMalloc((void **)&g->x_rep[i], (size_t)std::max<int64_t>(g->nx, 2) * 8));
-      if (g->nx > 0) CU(cudaMemcpyPeerAsync(g->x_rep[i], dev, d_x, root, (size_t)g->nx * 8, s));
-      xi = g->x_rep[i];
-      if (d_f_in && P->fdtype == FDB_FORWARD) {
-        if (!g->fin_rep[i]) CU(cudaMalloc((void **)&g->fin_rep[i], (size_t)std::max<int64_t>(g->m, 2) * 8));
-        if (g->m > 0) CU(cudaMemcpyPeerAsync(g->fin_rep[i], dev, d_f_in, root, (size_t)g->m * 8, s));
-        fin_i = g->fin_rep[i];
-      }
-    }
+    const double *fin_i = d_f_in;
+    if (i > 0 && d_f_in && P->fdtype == FDB_FORWARD) TRY(member_replica(g, i, g->fin_rep, d_f_in, g->m, s, &fin_i));
     double *Ji = P->sp_kind == SP_NONE ? d_J + P->col_begin * P->ldJ : d_J;
-    TRY(fdb_jacobian(P, f, ctx ? ctx[i] : nullptr, xi, Ji, nullptr, fin_i, relstep, absstep, dir, (void *)s));
-    CU(cudaEventRecord(g->ev_done[i], s));
-  }
-  {
-    DeviceGuard dg(root);
-    double *J0 = P0->sp_kind == SP_NONE ? d_J + P0->col_begin * P0->ldJ : d_J;
-    TRY(fdb_jacobian(P0, f, ctx ? ctx[0] : nullptr, d_x, J0, d_fx, d_f_in, relstep, absstep, dir, (void *)s0));
-    for (int i = 1; i < g->n; ++i) CU(cudaStreamWaitEvent(s0, g->ev_done[i], 0));
-  }
-  return FDB_OK;
+    return fdb_jacobian(P, f, ctx ? ctx[i] : nullptr, xi, Ji, i == 0 ? d_fx : nullptr, fin_i, relstep, absstep, dir, (void *)s);
+  }, [](int) { return false; });
+}
+
+fdb_status fdb_group_hessian(fdb_group *g, fdb_fn f, void *const *ctx, const double *d_x, double *d_H, double *d_fx,
+                             double relstep, double absstep, void *stream) {
+  if (!g || !f) return fail(FDB_ERR_INVALID, "NULL group or f");
+  if (g->kind != SP_HESS) return fail(FDB_ERR_INVALID, "not a Hessian group (fdb_group_create_hessian)");
+  if (g->nx > 0 && (!d_x || !d_H)) return fail(FDB_ERR_INVALID, "NULL x or H");
+  // every member stores the entries of its i-blocks straight into the root's H; only the root reports f(x)
+  return group_run(g, d_x, (cudaStream_t)stream, [&](int i, const double *xi, cudaStream_t s) {
+    return fdb_hessian(g->plans[i], f, ctx ? ctx[i] : nullptr, xi, d_H, i == 0 ? d_fx : nullptr, relstep, absstep, (void *)s);
+  }, [&](int i) { return g->plans[i]->hess_points == 0; });
 }
 
 // ------------------------------------------------------------------------------------------------ fdb_sync (one process per GPU)

@@ -8,6 +8,10 @@
 // at most two components, so the B batch rows stay resident: per batch the patch kernel restores the <= 2 components the
 // previous batch changed on each row and writes the new ones (O(B) bytes).  f writes its scalars (ldfx = 1) into the value
 // buffer V; whole i-blocks fill one chunk of V, and the assembly kernel turns a chunk into H's entries.
+//
+// A rank plan (world > 1) owns the i-blocks [i_r, i_{r+1}) and evaluates f(x) followed by its own points, so its local
+// sequence is {0} u [S(i_r), S(i_{r+1})): local index q is global point q == 0 ? 0 : q + off with off = S(i_r) - 1 (0 on
+// one device, where the map is the identity).
 #pragma once
 #include "common.cuh"
 
@@ -44,22 +48,25 @@ __device__ __forceinline__ double step_from(double xv, double e, int sign) {
   return sign > 0 ? __dadd_rn(xv, e) : __dsub_rn(xv, e);
 }
 
-// Batch of `cnt` points starting at sequence index p0 on rows 0..cnt-1 of X; the previous batch (prev_p0, prev_cnt) left
+// local index q of a rank's sequence -> global point
+__device__ __forceinline__ int64_t hess_global(int64_t q, int64_t off) { return q == 0 ? 0 : q + off; }
+
+// Batch of `cnt` points starting at local index p0 on rows 0..cnt-1 of X; the previous batch (prev_p0, prev_cnt) left
 // its components on rows 0..prev_cnt-1.  Restores exactly (the reference writes the saved x_j / x_i back, :272-289).
 __global__ void __launch_bounds__(kThreads)
-hess_patch(const double *__restrict__ x, const double *__restrict__ eps, int64_t n, int64_t ldx, int64_t p0, int32_t cnt,
-           int64_t prev_p0, int32_t prev_cnt, double *__restrict__ X) {
+hess_patch(const double *__restrict__ x, const double *__restrict__ eps, int64_t n, int64_t ldx, int64_t off, int64_t p0,
+           int32_t cnt, int64_t prev_p0, int32_t prev_cnt, double *__restrict__ X) {
   for (int b = blockIdx.x * kThreads + threadIdx.x; b < max(cnt, prev_cnt); b += gridDim.x * kThreads) {
     double *row = X + (int64_t)b * ldx;
     int64_t i, j;
     int si, sj;
     if (b < prev_cnt) {
-      hess_decode(prev_p0 + b, n, i, j, si, sj);
+      hess_decode(hess_global(prev_p0 + b, off), n, i, j, si, sj);
       if (i >= 0) row[i] = x[i];
       if (j >= 0) row[j] = x[j];
     }
     if (b < cnt) {
-      hess_decode(p0 + b, n, i, j, si, sj);
+      hess_decode(hess_global(p0 + b, off), n, i, j, si, sj);
       if (i >= 0) row[i] = step_from(x[i], eps[i], si);
       if (j >= 0) row[j] = step_from(x[j], eps[j], sj);
     }

@@ -170,7 +170,71 @@ class DeviceBarrier:
         self._h = None
 
 
-class GroupJacobian:
+class _Group:
+    """What GroupJacobian and GroupHessian share: the fdb_group handle, its member plans, one f per member behind one
+    entry point, and the joins."""
+
+    def _set_devices(self, devices):
+        self.devices = [api._device_index(d) if not isinstance(d, int) else int(d) for d in devices]
+        self.root = torch.device("cuda", self.devices[0])
+
+    def _adopt(self, h):
+        lib = L.lib()
+        self._h = h
+        self._fin = api.weakref.finalize(self, lib.fdb_group_destroy, C.c_void_p(h.value))
+        self.plans = []
+        for i in range(len(self.devices)):
+            p = C.c_void_p()
+            L.check(lib.fdb_group_plan(self._h, i, C.byref(p)))
+            self.plans.append(api.Plan(p.value, owned=False))
+        self._fns = None
+
+    def _member_fns(self, fs, m, n, **kind):
+        """(entry address, contexts array, per-member wrappers) for one f per member.  The ABI takes one f and a context
+        per member: NativeFns must share their address; Python callables go through ONE trampoline whose context is the
+        member index + 1, forwarding to that member's wrapper (tensors on that member's device)."""
+        if len(fs) != len(self.devices):
+            raise ValueError("one f! per member")
+        if self._fns is None or self._fns[0] is not fs:
+            keep = None
+            if all(isinstance(f, api.NativeFn) for f in fs):
+                wrapped = [api._as_fn(f, m, n, torch.device("cuda", d), 1) for f, d in zip(fs, self.devices)]
+            else:
+                per = [api._PyFn(f, m, n, torch.device("cuda", d), bool(getattr(f, "batched", False)), **kind)
+                       for f, d in zip(fs, self.devices)]
+
+                def tramp(ctx, p_fx, p_x, batch, ldfx, ldx, stream, _per=per):
+                    return _per[int(ctx or 1) - 1]._tramp(None, p_fx, p_x, batch, ldfx, ldx, stream)
+
+                keep = L.FDB_FN(tramp)
+                wrapped = [(L.fn_address(keep), C.c_void_p(i + 1), per[i]) for i in range(len(per))]
+            self._fns = (fs, wrapped, keep)
+        wrapped = self._fns[1]
+        addr = wrapped[0][0]
+        if any(w[0] != addr for w in wrapped):
+            raise ValueError("all members must share one f! entry point (contexts may differ per device)")
+        ctxs = (C.c_void_p * len(wrapped))(*[C.cast(w[1], C.c_void_p).value if w[1] is not None else None for w in wrapped])
+        return addr, ctxs, wrapped
+
+    @staticmethod
+    def _check(st, wrapped):
+        """A member's Python exception propagates as itself; any other failure as FdbError."""
+        for w in wrapped:
+            if st == L.FDB_ERR_CALLBACK and w[2] is not None and w[2].exc is not None:
+                exc, w[2].exc = w[2].exc, None
+                raise exc
+        L.check(st)
+
+    def synchronize(self):
+        for d in set(self.devices):
+            torch.cuda.synchronize(d)
+
+    def close(self):
+        self.synchronize()
+        self._fin()
+
+
+class GroupJacobian(_Group):
     """ONE process driving several GPUs through fdb_group_* (the C ABI's own multi-GPU entry: no torch.distributed, no
     NCCL): colours (dense: column blocks) are partitioned over `devices`; devices[0] is the root and owns x, J and fx;
     every member's scatter kernel stores the entries it owns straight into the root's J over NVLink.  Device ordinals
@@ -179,8 +243,7 @@ class GroupJacobian:
     fs: one f! per member (NativeFn whose context lives on that member's device, or a Python callable)."""
 
     def __init__(self, J, colorvec, fdtype, devices, *, sparsity=api._DEFAULT, **plan_kw):
-        self.devices = [api._device_index(d) if not isinstance(d, int) else int(d) for d in devices]
-        self.root = torch.device("cuda", self.devices[0])
+        self._set_devices(devices)
         self.J, self.fdtype = J, fdtype
         if sparsity is api._DEFAULT:
             sparsity = J if api._has_sparsestruct(J) else None
@@ -222,39 +285,11 @@ class GroupJacobian:
                                                     cv_ptr, C.byref(o)))
         else:
             raise TypeError(f"GroupJacobian: unsupported sparsity type {type(sparsity)}")
-        self._h = h
-        self._fin = api.weakref.finalize(self, lib.fdb_group_destroy, C.c_void_p(h.value))
-        self.plans = []
-        for i in range(n_dev):
-            p = C.c_void_p()
-            L.check(lib.fdb_group_plan(self._h, i, C.byref(p)))
-            self.plans.append(api.Plan(p.value, owned=False))
-        self._fns = None
+        self._adopt(h)
 
     def run(self, fs, x, fx=None, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):
         m, n = api._shape_of(self.J)
-        if len(fs) != len(self.devices):
-            raise ValueError("one f! per member")
-        if self._fns is None or self._fns[0] is not fs:
-            if all(isinstance(f, api.NativeFn) for f in fs):
-                wrapped = [api._as_fn(f, m, n, torch.device("cuda", d), 1) for f, d in zip(fs, self.devices)]
-            else:
-                # Python callables: ONE trampoline (the ABI takes one f and a context per member); the context is the
-                # member index + 1, the trampoline forwards to that member's wrapper (tensors on that member's device)
-                per = [api._PyFn(f, m, n, torch.device("cuda", d), bool(getattr(f, "batched", False))) for f, d in zip(fs, self.devices)]
-
-                def tramp(ctx, p_fx, p_x, batch, ldfx, ldx, stream, _per=per):
-                    return _per[int(ctx or 1) - 1]._tramp(None, p_fx, p_x, batch, ldfx, ldx, stream)
-
-                cf = L.FDB_FN(tramp)
-                wrapped = [(L.fn_address(cf), C.c_void_p(i + 1), per[i]) for i in range(len(per))]
-                self._tramp_keep = cf
-            self._fns = (fs, wrapped)
-        wrapped = self._fns[1]
-        addr = wrapped[0][0]
-        if any(w[0] != addr for w in wrapped):
-            raise ValueError("all members must share one f! entry point (contexts may differ per device)")
-        ctxs = (C.c_void_p * len(wrapped))(*[C.cast(w[1], C.c_void_p).value if w[1] is not None else None for w in wrapped])
+        addr, ctxs, wrapped = self._member_fns(fs, m, n)
         if stream is None:
             stream = torch.cuda.current_stream(self.root).cuda_stream
         jv = api._j_values(self.J)
@@ -263,19 +298,49 @@ class GroupJacobian:
                                             None if fx is None else fx.data_ptr(), None if f_in is None else f_in.data_ptr(),
                                             L.STEP_DEFAULT if relstep is None else float(relstep),
                                             L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-        for w in wrapped:
-            if st == L.FDB_ERR_CALLBACK and w[2] is not None and w[2].exc is not None:
-                exc, w[2].exc = w[2].exc, None
-                raise exc
-        L.check(st)
+        self._check(st, wrapped)
 
-    def synchronize(self):
-        for d in set(self.devices):
-            torch.cuda.synchronize(d)
 
-    def close(self):
-        self.synchronize()
-        self._fin()
+class GroupHessian(_Group):
+    """finite_difference_hessian! on several GPUs from ONE process (fdb_group_create_hessian / fdb_group_hessian): the
+    i-blocks of the reference's point sequence are split over `devices` in contiguous, point-balanced ranges (member i's
+    is plans[i].dense_range()); devices[0] is the root and owns x, H and fx; every non-empty member evaluates f(x) and
+    its own points and stores the entries it owns straight into the root's H.  H is bit-identical to one device.  Device
+    ordinals may repeat ([0, 0] runs two members on one GPU).
+
+    plan_kw: max_batch, scratch_bytes, use_graph (per member), fdtype (only "hcentral" is built)."""
+
+    def __init__(self, n, devices, *, ldH=None, fdtype="hcentral", **plan_kw):
+        self._set_devices(devices)
+        self.n = int(n)
+        self.ldH = max(self.n, 1) if ldH is None else int(ldH)
+        o = api._opts(api._hessian_fdtype_code(fdtype), self.devices[0], **plan_kw)
+        devs = (C.c_int * len(self.devices))(*self.devices)
+        h = C.c_void_p()
+        L.check(L.lib().fdb_group_create_hessian(C.byref(h), len(self.devices), devs, self.n, self.ldH, C.byref(o)))
+        self._adopt(h)
+
+    def run(self, fs, x, H, fx=None, *, relstep=None, absstep=None, stream=None):
+        """fs: one f per member — a NativeFn (batched fdb_fn with m = 1, context on that member's device) or a Python
+        f(x) -> scalar on that member's device (f.batched = True: (batch, n) in, (batch,) out).  x, H (column-major n x n,
+        leading dimension ldH) and fx (optional 1-element tensor receiving f(x)) live on devices[0]."""
+        xv = api._scalar_x(x)
+        if xv.numel() != self.n or xv.device != self.root:
+            raise ValueError(f"x must hold {self.n} values on {self.root}")
+        ld = api._colmajor_square(H, self.n)
+        if (self.n > 1 and ld != self.ldH) or H.device != self.root:      # n <= 1: one element, any leading dimension
+            raise ValueError(f"H must be column-major with leading dimension {self.ldH} on {self.root}")
+        if fx is not None and (not api._is_cuda(fx) or fx.dtype != torch.float64 or fx.numel() != 1):
+            raise TypeError("fx must be a 1-element float64 CUDA tensor")
+        addr, ctxs, wrapped = self._member_fns(fs, 1, self.n, scalar=True)
+        if stream is None:
+            stream = torch.cuda.current_stream(self.root).cuda_stream
+        with torch.cuda.device(self.root):
+            st = L.lib().fdb_group_hessian(self._h, addr, ctxs, xv.data_ptr(), H.data_ptr() if self.n > 0 else None,
+                                           None if fx is None else fx.data_ptr(),
+                                           L.STEP_DEFAULT if relstep is None else float(relstep),
+                                           L.STEP_DEFAULT if absstep is None else float(absstep), C.c_void_p(stream))
+        self._check(st, wrapped)
 
 
 class ShardedJacobian:

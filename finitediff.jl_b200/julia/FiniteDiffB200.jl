@@ -677,6 +677,42 @@ function group_jacobian!(g::Group, jvals::CuArray{Float64}, fs::Vector, x::CuVec
     nothing
 end
 
+# ---- finite_difference_hessian! on several GPUs from ONE call: the i-blocks are split over `devices` (point-balanced,
+#      contiguous ranges); devices[1] is the root and owns x, H and fx; every member evaluates f(x) and its own points and
+#      stores its entries straight into the root's H, bit-identical to one device.  kw: max_batch, scratch_bytes, use_graph.
+function group_hessian(H::CuMatrix{Float64}, n::Integer, devices::Vector{Cint}; kw...)
+    size(H) == (n, n) || throw(DimensionMismatch("H must be $n x $n"))
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(FDB_HCENTRAL; kw...))
+    GC.@preserve devices begin
+        check(ccall((:fdb_group_create_hessian, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), n, ld(H), opts))
+    end
+    Group(h[], length(devices), nothing)
+end
+
+# fs[i]: the scalar f(x) member i calls (its arrays live on devices[i]); H, x and fx (a 1-element CuVector) live on devices[1]
+function group_hessian!(g::Group, H::CuMatrix{Float64}, fs::Vector, x::CuVector{Float64};
+        relstep = nothing, absstep = relstep, fx = nothing)
+    states = [FnState(scalar_f(f), 1, length(x), nothing) for f in fs]
+    ctxs = Ptr{Cvoid}[pointer_from_objref(s) for s in states]
+    cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+    rc = Cint(0)
+    GC.@preserve states ctxs x H fx begin
+        rc = ccall((:fdb_group_hessian, libfdjac), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Ptr{Cvoid}}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, Float64, Float64,
+                Ptr{Cvoid}),
+            g.handle, cf, pointer(ctxs), pointer(x), pointer(H), fx === nothing ? CU_NULL : pointer(fx), stepval(relstep),
+            stepval(absstep), CUDA.stream().handle)
+    end
+    for s in states
+        s.err === nothing || throw(s.err)
+    end
+    check(rc)
+    H
+end
+
 # ---- column-block shards (few-colour problems on several GPUs): one process per GPU, each owning the columns c0+1:c1.
 # `sub` is the block's pattern (colptr slice rebased to 1, rows rebased to the block's first row), `f_rows!` computes
 # that row range from the x slice the rows depend on, `eps` holds the step sizes of the FULL x (color_eps! below).

@@ -184,7 +184,7 @@ fdb_status fdb_plan_create_dense_colorvec(fdb_plan **plan, int64_t m, int64_t n,
 fdb_status fdb_plan_destroy(fdb_plan *plan);
 fdb_status fdb_plan_info(const fdb_plan *plan, fdb_plan_info_t *info);
 fdb_status fdb_plan_counters(const fdb_plan *plan, fdb_counters_t *out);
-/* dense plans: the [begin,end) 0-based column range this rank owns */
+/* dense plans: the [begin,end) 0-based column range this rank owns; Hessian plans: the rank's i-blocks [i_r, i_{r+1}) */
 fdb_status fdb_plan_dense_range(const fdb_plan *plan, int64_t *col_begin, int64_t *col_end);
 /* colour ownership (0-based colour index -> owning rank), n_colors entries */
 fdb_status fdb_plan_color_owner(const fdb_plan *plan, int32_t *owner_out, int64_t cap);
@@ -321,7 +321,7 @@ fdb_status fdb_jvp(fdb_plan *plan, fdb_fn f, void *ctx, double *d_jvp, const dou
  *      @assert fdtype == Val(:hcentral), :206); H is dense column-major with leading dimension ldH >= n (else
  *      FDB_ERR_INVALID).  max_batch: points per f call (at most 4096); scratch_bytes: one budget (0 => 8 GiB) for the point
  *      rows (at most half of it) and the stacked f values (the rest, filled by whole i-blocks; at least one i-block, 8(4n-1)
- *      bytes, whatever the budget); use_graph as for fdb_jacobian.  One device (world <= 1).
+ *      bytes, whatever the budget); use_graph as for fdb_jacobian; rank / world split the work over devices (below).
  *
  *      fdb_hessian evaluates f (the batched fdb_fn with m = 1: point b at d_x + b*ldx, its scalar to d_fx[b*ldfx]) at the
  *      reference's 2n^2 + 1 points in the reference's order — f(x); then per i the pair x +- eps_i e_i and, per j > i,
@@ -330,10 +330,36 @@ fdb_status fdb_jvp(fdb_plan *plan, fdb_fn f, void *ctx, double *d_jvp, const dou
  *      to rows [0, n) of every column (padding rows are not touched).  d_x is never modified; d_fx (nullable, one double)
  *      receives f(x).  relstep / absstep: FDB_STEP_DEFAULT => eps(Float64)^(1/4) and absstep = relstep.
  *      Stream-ordered, no host synchronisation.  fdb_plan_info: n_entries = n^2, fcalls_per_jacobian = 2n^2 + 1,
- *      alg_bytes / moved_bytes the library's bytes per Hessian (values read back, H, point replication, patches). ---- */
+ *      alg_bytes / moved_bytes the library's bytes per Hessian (values read back, H, point replication, patches).
+ *
+ *      Rank plans (opts.world in 2..64, opts.rank in 0..world-1).  i-block i (the points that change component i and no
+ *      smaller one) starts at S(i) = 1 + 2i + 4(i(n-1) - i(i-1)/2) and holds 2 + 4(n-1-i) points; T = 2n^2.  Rank r owns
+ *      the i-blocks [i_r, i_{r+1}) with i_0 = 0, i_world = n and, for 0 < r < world, i_r = the i in [i_{r-1}, n] whose
+ *      S(i) - 1 is nearest to r*T/world (ties: the smaller i), so each rank's point count is within one block
+ *      (2 + 4(n-1)) of T/world; ranges may be empty (e.g. n < world).  fdb_plan_dense_range reports [i_r, i_{r+1}).
+ *      A rank evaluates f(x) first (its own, the diagonal needs it), then its points in the reference's order; rank 0
+ *      always evaluates f(x) (n = 0 included), a rank > 0 with an empty range calls nothing, launches nothing and leaves
+ *      d_fx untouched.  It writes exactly the entries it owns — column i rows [i, n) and row i columns (i, n) for i in its
+ *      range — into the d_H it is given, so the ranks together write rows [0, n) of every column once, bit-identical to
+ *      one plan; H is never zero-filled and shared_j has no effect.  d_H may be another device's H mapped into this one
+ *      (a group member storing into the root's H, or an fdb_ipc_open mapping with one process per GPU); the ordering is
+ *      then the Jacobian's: fdb_sync_barrier, fdb_hessian, fdb_sync_barrier.  fdb_plan_info per rank: fcalls_per_jacobian
+ *      = 1 + the rank's points (0 for an empty rank > 0), n_entries = sum over its i of 2(n-i) - 1, byte model the
+ *      rank's own; summed over the ranks they give the whole Hessian's figures plus one f(x) per non-empty rank > 0. ---- */
 fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, const fdb_plan_opts *opts);
 fdb_status fdb_hessian(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, double *d_H, double *d_fx, double relstep,
                        double absstep, void *stream);
+/* One process, n devices: the group form of the rank plans above (fdb_group_create_* / fdb_group_plan / fdb_group_destroy
+ * as for Jacobians).  Member i runs rank i of n_devices on its own stream with ctx[i]; d_x, d_H and d_fx live on
+ * devices[0] (the root), x is replicated to members on other devices, every member stores its entries straight into the
+ * root's H, the root writes f(x) to d_fx, and the members are joined on `stream` (a stream of devices[0]) with events —
+ * no host synchronisation.  Device ordinals may repeat.  opts->fdtype must be FDB_HCENTRAL (else FDB_ERR_UNSUPPORTED).
+ * fdb_group_hessian on a Jacobian group and fdb_group_jacobian on a Hessian group return FDB_ERR_INVALID before any
+ * launch.  f is evaluated once per non-empty member at x; H is bit-identical to the one-device result. */
+fdb_status fdb_group_create_hessian(fdb_group **group, int n_devices, const int *devices, int64_t n, int64_t ldH,
+                                    const fdb_plan_opts *opts);
+fdb_status fdb_group_hessian(fdb_group *group, fdb_fn f, void *const *ctx, const double *d_x, double *d_H, double *d_fx,
+                             double relstep, double absstep, void *stream);
 
 /* ---- Derivatives with a scalar input per step size ----
  *   finite_difference_derivative!(df, f, x::StridedArray, cache::DerivativeCache; relstep, absstep, dir)
