@@ -1058,6 +1058,73 @@ def _oop_kind(sparsity, jac_prototype):
     return L.FDB_OOP_RAW, None, None
 
 
+def _oop_rows(f, x, fd, f_in, m_default, sparsity, pm, n):
+    """(f_in, m): the rows of an out-of-place result.  In forward mode a Python f is evaluated at x first — vecfx = _vec(f(x))
+    (:299-300), the same call at the same point, still before the colours — and handed on as f_in, so the row count is f's
+    own; otherwise those of f_in, else m_default.  A sparsity fixes them, and a prototype must agree."""
+    if f_in is None and fd == L.FDB_FORWARD and not isinstance(f, NativeFn):
+        f_in = _oop_result(f(x), (-1,))
+    if f_in is not None:
+        if f_in.is_complex():
+            raise TypeError("not built: complex-valued f_in (complex-valued results of the out-of-place path)")
+        f_in = f_in.reshape(-1)
+    m = f_in.numel() if f_in is not None else m_default
+    if sparsity is not None:
+        m = sparsity.m
+        if sparsity.n != n:
+            raise ValueError(f"size(sparsity, 2) = {sparsity.n} != length(x) = {n}")
+    elif pm is not None and pm != m:
+        raise TypeError(f"not built: a {pm}-row jac_prototype for an f with {m} values")
+    return f_in, m
+
+
+def _oop_fin_ptr(f_in, fd, m):
+    """Device pointer of f_in as the ABI reads it (forward mode only, :297-298), or None."""
+    if f_in is None or fd != L.FDB_FORWARD:
+        return None
+    finv = _flat_f64(f_in, "f_in")
+    if finv.numel() != m:
+        raise ValueError("length(f_in) != the rows of the result")
+    return _fx_ptr(finv)
+
+
+class _OopOutput:
+    """Device storage of an out-of-place result and the fdb_oop_out naming it.  ncols: the prototype's columns, else
+    the quotient columns C = maximum(colorvec) of the whole result (dense branch); a sparse result holds up to m*C
+    candidates without a sparsity and nnz(sparsity) = n_entries with one."""
+
+    def __init__(self, kind, sparsity, pn, m, C, n_entries, dev):
+        self.kind, self.m, self.dev = kind, m, dev
+        self.ncols = pn if pn is not None else C
+        self.out = L.OopOut()
+        self.dense = None
+        if kind == L.FDB_OOP_SPARSE:
+            self.cap = m * C if sparsity is None else n_entries
+            self.colptr = torch.empty(self.ncols + 1, dtype=torch.int64, device=dev)
+            self.rowval = torch.empty(max(self.cap, 1), dtype=torch.int64, device=dev)
+            self.nzval = torch.empty(max(self.cap, 1), dtype=torch.float64, device=dev)
+            self.nnz = torch.empty(1, dtype=torch.int64, device=dev)
+            o = self.out
+            o.colptr, o.rowval, o.nzval, o.cap, o.nnz = (self.colptr.data_ptr(), self.rowval.data_ptr(),
+                                                         self.nzval.data_ptr(), self.cap, self.nnz.data_ptr())
+        else:
+            self.dense = torch.empty((self.ncols, m), dtype=torch.float64, device=dev).t()  # column-major, ldJ = m
+            self.out.J = self.dense.data_ptr() if self.dense.numel() else _fx_ptr(self.dense)  # m = 0: nothing is written
+
+    def result(self, stream):
+        """The dense tensor, or the SparseMatrixCSC sized to the kept entries (reading that count is the one host sync;
+        when most candidates were dropped its rowval / nzval are copied into storage of their own size)."""
+        if self.kind != L.FDB_OOP_SPARSE:
+            return self.dense
+        with torch.cuda.device(self.dev):
+            L.check(L.lib().fdb_stream_sync(C.c_void_p(stream)))
+        nnz = int(self.nnz.item())
+        rowval, nzval = self.rowval[:nnz], self.nzval[:nnz]
+        if 2 * nnz < self.cap:
+            rowval, nzval = rowval.clone(), nzval.clone()
+        return SparseMatrixCSC(self.m, self.ncols, self.colptr, rowval, nzval)
+
+
 def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, fdtype=None, relstep=None, absstep=None,
                                colorvec=None, sparsity=_DEFAULT, jac_prototype=None, dir=True, stream=None):
     """J = finite_difference_jacobian(f, x, cache::JacobianCache, f_in=nothing; relstep, absstep, colorvec, sparsity,
@@ -1125,21 +1192,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
     n = xv.numel()
     if cache.x1 is not x:                                                                 # :293-295
         cache.x1.reshape(-1).copy_(xv)
-    if f_in is None and fd == L.FDB_FORWARD and not isinstance(f, NativeFn):
-        # vecfx = _vec(f(x)) (:299-300) is evaluated here and handed on as f_in: the same call at the same point, still
-        # before the colours, and the row count is f's own
-        f_in = _oop_result(f(x), (-1,))
-    if f_in is not None:
-        if f_in.is_complex():
-            raise TypeError("not built: complex-valued f_in (complex-valued results of the out-of-place path)")
-        f_in = f_in.reshape(-1)
-    m = f_in.numel() if f_in is not None else cache.fx.numel()
-    if sparsity is not None:
-        m = sparsity.m
-        if sparsity.n != n:
-            raise ValueError(f"size(sparsity, 2) = {sparsity.n} != length(x) = {n}")
-    elif pm is not None and pm != m:
-        raise TypeError(f"not built: a {pm}-row jac_prototype for an f with {m} values")
+    f_in, m = _oop_rows(f, x, fd, f_in, cache.fx.numel(), sparsity, pm, n)
     dev = x.device
     key = ("oop", kind, _sp_key(sparsity) if sparsity is not None else None, _index_key(colorvec), pn, m, n)
     plan = cache._plans.get(key)
@@ -1157,35 +1210,17 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
                 L.check(L.lib().fdb_oop_plan_create_dense(C.byref(h), m, n, cvp, pn or 0, kind, max(m, 1), C.byref(o)))
         plan = Plan(h.value)
         cache._plans[key] = plan
-    info = plan.info()
-    ncols = pn if pn is not None else info["n_local_colors"]
-    out = L.OopOut()
-    result = nnz_d = None
-    if kind == L.FDB_OOP_SPARSE:
-        cap = info["m"] * info["n_local_colors"] if sparsity is None else info["n_entries"]
-        colptr = torch.empty(ncols + 1, dtype=torch.int64, device=dev)
-        rowval = torch.empty(max(cap, 1), dtype=torch.int64, device=dev)
-        nzval = torch.empty(max(cap, 1), dtype=torch.float64, device=dev)
-        nnz_d = torch.empty(1, dtype=torch.int64, device=dev)
-        out.colptr, out.rowval, out.nzval, out.cap, out.nnz = (colptr.data_ptr(), rowval.data_ptr(), nzval.data_ptr(),
-                                                               cap, nnz_d.data_ptr())
-    else:
-        result = torch.empty((ncols, m), dtype=torch.float64, device=dev).t()            # column-major, ldJ = m
-        out.J = result.data_ptr() if result.numel() else _fx_ptr(result)                 # m = 0: nothing is written
+    res = _OopOutput(kind, sparsity, pn, m, plan.dense_range()[1], plan.info()["n_entries"], dev)
     addr, ctx, pyfn = _as_fn(f, m, n, dev, 1, fd == L.FDB_COMPLEX, oop=True)
     if stream is None:
         stream = torch.cuda.current_stream(dev).cuda_stream
-    fin_ptr = None
-    if f_in is not None and fd == L.FDB_FORWARD:                                          # :297-298
-        finv = _flat_f64(f_in, "f_in")
-        if finv.numel() != m:
-            raise ValueError("length(f_in) != the rows of the result")
-        fin_ptr = _fx_ptr(finv)
+    fin_ptr = _oop_fin_ptr(f_in, fd, m)
     with torch.cuda.device(dev):
         if fd == L.FDB_COMPLEX:
-            st = L.lib().fdb_jacobian_oop_complex(plan.handle, addr, ctx, xv.data_ptr(), C.byref(out), C.c_void_p(stream))
+            st = L.lib().fdb_jacobian_oop_complex(plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out),
+                                                  C.c_void_p(stream))
         else:
-            st = L.lib().fdb_jacobian_oop(plan.handle, addr, ctx, xv.data_ptr(), C.byref(out), None, fin_ptr,
+            st = L.lib().fdb_jacobian_oop(plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out), None, fin_ptr,
                                           L.STEP_DEFAULT if relstep is None else float(relstep),
                                           L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
                                           C.c_void_p(stream))
@@ -1194,15 +1229,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
         raise exc
     L.check(st)
     cache._last_plan = plan
-    if kind != L.FDB_OOP_SPARSE:
-        return result
-    with torch.cuda.device(dev):
-        L.check(L.lib().fdb_stream_sync(C.c_void_p(stream)))                              # the one host sync
-    nnz = int(nnz_d.item())
-    rowval, nzval = rowval[:nnz], nzval[:nnz]
-    if 2 * nnz < cap:                 # most candidates dropped: give the result storage of its own size
-        rowval, nzval = rowval.clone(), nzval.clone()
-    return SparseMatrixCSC(m, ncols, colptr, rowval, nzval)
+    return res.result(stream)
 
 
 def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):

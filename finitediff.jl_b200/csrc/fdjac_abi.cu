@@ -249,6 +249,9 @@ struct fdb_plan {
   int oop_kind = 0;             // FDB_OOP_RAW / FDB_OOP_DENSE / FDB_OOP_SPARSE
   bool oop_entry = false;       // set while fdb_jacobian_oop drives the call
   int64_t oop_ncols = 0;        // columns of the result
+  int64_t oop_qcols = 0;        // dense branch: columns holding quotients, maximum(colorvec), over every rank
+  const int64_t *oop_dest = nullptr;   // dense result of a CSC sparsity: the slots of this rank's colours (dest when world = 1)
+  int64_t oop_dest_n = 0;
   double *oop_vals = nullptr;   // sparse result: the candidate values (nzval of the sparsity, or the m x C dense block)
   unsigned long long *oop_state = nullptr;   // sparse result: look-back words of the compaction, then its tile counter
   int32_t *oop_tile_col = nullptr;           // sparse result of a CSC sparsity: first column starting in each tile
@@ -1157,6 +1160,11 @@ fdb_status fdb_plan_destroy(fdb_plan *plan) {
   return FDB_OK;
 }
 
+// an out-of-place rank > 0 that owns no colour (dense branch: no column): it calls nothing and launches nothing
+static bool oop_idle(const fdb_plan *P) {
+  return P->oop && P->rank > 0 && (P->sp_kind == SP_NONE ? P->col_end == P->col_begin : P->local_colors.empty());
+}
+
 fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   if (!P || !info) return fail(FDB_ERR_INVALID, "NULL argument");
   memset(info, 0, sizeof *info);
@@ -1173,6 +1181,9 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   info->fcalls_per_jacobian = P->fdtype == FDB_CENTRAL ? 2 * n_local : (P->fdtype == FDB_COMPLEX ? n_local : 1 + n_local);
   if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = P->hess_points;
   if (P->sp_kind == SP_DERIV) info->fcalls_per_jacobian = P->deriv_fcalls;
+  if (oop_idle(P)) info->fcalls_per_jacobian = 0;
+  // out-of-place dense branch: the candidate count of the whole result (a rank's E is its own block)
+  if (P->oop && P->sp_kind == SP_NONE) info->n_entries = P->m * P->oop_qcols;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
   info->jkind = P->jkind;

@@ -47,6 +47,7 @@ sync_barrier_kernel(unsigned long long *const *__restrict__ peer_flags, unsigned
 struct fdb_group {
   int n = 0;
   int kind = SP_CSC;
+  bool oop = false;                      // out-of-place Jacobian members (fdb_group_create_oop_*)
   std::vector<fdb_plan *> plans;
   std::vector<int> devices;
   std::vector<cudaStream_t> streams;     // members > 0 (index 0 unused: the root runs on the caller's stream)
@@ -136,6 +137,7 @@ static fdb_status group_create(fdb_group **out, int n_devices, const int *device
   g->nx = g->plans[0]->n;
   g->m = g->plans[0]->m;
   g->kind = g->plans[0]->sp_kind;
+  g->oop = g->plans[0]->oop != 0;
   *out = g.release();
   return FDB_OK;
 }
@@ -237,6 +239,7 @@ fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const do
                               const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
   if (!g || !f) return fail(FDB_ERR_INVALID, "NULL group or f");
   if (g->kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian group: call fdb_group_hessian");
+  if (g->oop) return fail(FDB_ERR_INVALID, "this is an out-of-place group: call fdb_group_jacobian_oop");
   fdb_plan *P0 = g->plans[0];
   if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
   if ((P0->n > 0 && !d_x) || !d_J) return fail(FDB_ERR_INVALID, "NULL x or J");

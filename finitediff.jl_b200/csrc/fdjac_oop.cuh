@@ -1,8 +1,13 @@
 // fdjac_oop.cuh — the out-of-place Jacobian and JVP (include/fdjac_b200.h, "Out-of-place Jacobian").  Included at the end
 // of fdjac_abi.cu: an out-of-place plan is an in-place colour-loop plan with `oop` set (pristine points, the forward step
 // rule in central mode) whose J target is the result (dense kinds).  A sparse result is formed by oop_compact: from the
-// resident f! outputs directly (the in-place scatter is skipped), or, when they come in several groups, from the
-// candidates the in-place scatter wrote to a plan-owned buffer.
+// resident f! outputs directly (the in-place scatter is skipped), or, when they come in several groups or several ranks,
+// from the candidates the in-place scatter wrote to a plan-owned buffer (the root's, for a group).
+//
+// Rank plans (opts.world > 1) evaluate only their own colours (dense branch: their column block).  Every colour's point
+// starts from the caller's x, so a colour's quotients depend on x and its own step alone and the ranks need no exchange:
+// each writes exactly its own slots (oop_member), and only a sparse result has a root-only step, the compaction over
+// every candidate (oop_root_finish) once every member has finished.
 #include "kernels_oop.cuh"
 
 static fdb_status oop_alloc_sparse(fdb_plan *P, int64_t candidates) {
@@ -19,6 +24,40 @@ static fdb_plan_opts oop_opts(const fdb_plan_opts *opts) {
   return o;
 }
 
+// the slots of a dense result (CSC sparsity) whose `+ 0.0` this rank applies: those of the colours it owns.  One rank
+// owns them all, and `dest` itself is used.
+static fdb_status oop_own_slots(fdb_plan *P) {
+  if (P->world == 1) {
+    P->oop_dest = P->dest;
+    P->oop_dest_n = P->E;
+    return FDB_OK;
+  }
+  const int64_t E = P->E;
+  const size_t cb = (size_t)P->color_bits / 8;
+  std::vector<int64_t> dest((size_t)E), own;
+  std::vector<uint8_t> ec((size_t)E * cb);
+  if (E > 0) {
+    TRY(read_back(dest.data(), P->dest, (size_t)E, "reading the dense result's slots"));
+    TRY(read_back(ec.data(), (const uint8_t *)P->ecolor, (size_t)E * cb, "reading the entry colours"));
+  }
+  for (int64_t e = 0; e < E; ++e) {
+    const uint8_t *p = ec.data() + (size_t)e * cb;
+    const uint32_t k = cb == 1 ? *p : (cb == 2 ? *reinterpret_cast<const uint16_t *>(p) : *reinterpret_cast<const uint32_t *>(p));
+    if (k < (uint32_t)P->C && P->owner[k] == P->rank) own.push_back(dest[(size_t)e]);
+  }
+  int64_t *d = nullptr;
+  TRY(P->alloc_t(&d, std::max<size_t>(own.size(), 1)));
+  if (!own.empty()) CU(cudaMemcpy(d, own.data(), own.size() * 8, cudaMemcpyHostToDevice));
+  P->oop_dest = d;
+  P->oop_dest_n = (int64_t)own.size();
+  return FDB_OK;
+}
+
+// candidates of the whole result: nnz of the sparsity, or m x maximum(colorvec) on the dense branch
+static int64_t oop_candidates(const fdb_plan *P) {
+  return P->sp_kind == SP_NONE ? P->m * P->oop_qcols : P->E;
+}
+
 extern "C" {
 
 fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval,
@@ -28,7 +67,7 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
   if (result_kind != FDB_OOP_DENSE && result_kind != FDB_OOP_SPARSE)
     return fail(FDB_ERR_INVALID, "a CSC sparsity gives a dense (FDB_OOP_DENSE) or a sparse (FDB_OOP_SPARSE) result");
   if (n == 0) return fail(FDB_ERR_INVALID, "maximum(colorvec) of an empty colorvec: the reference throws");
-  if (opts && opts->world > 1) return fail(FDB_ERR_UNSUPPORTED, "out-of-place plans run on one device (world <= 1)");
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
   if (result_kind == FDB_OOP_DENSE && m > 0) {
     int64_t conflicts = 0;   // _make_Ji (jacobians.jl:151-162) throws when two columns of one colour share a row
     TRY(fdb_check_coloring_csc(m, n, colptr, rowval, colorvec, &conflicts));
@@ -47,7 +86,8 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
   P->oop = 1;
   P->oop_kind = result_kind;
   P->oop_ncols = n;
-  if (result_kind == FDB_OOP_SPARSE) {
+  if (result_kind == FDB_OOP_DENSE) TRY(oop_own_slots(P));
+  if (result_kind == FDB_OOP_SPARSE && P->rank == 0) {   // the candidate buffer and the compaction are the root's
     TRY(oop_alloc_sparse(P, P->E));
     // one group of resident f! outputs on one rank: the compaction forms the quotients itself, no candidate is stored
     P->oop_fused = P->n_groups <= 1 && P->world == 1;
@@ -70,7 +110,7 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
   if (result_kind != FDB_OOP_RAW && result_kind != FDB_OOP_DENSE && result_kind != FDB_OOP_SPARSE)
     return fail(FDB_ERR_INVALID, "result_kind must be FDB_OOP_RAW, FDB_OOP_DENSE or FDB_OOP_SPARSE");
   if (n <= 0 || m < 0) return fail(FDB_ERR_INVALID, "n = %lld: maximum(colorvec) of an empty colorvec throws", (long long)n);
-  if (opts && opts->world > 1) return fail(FDB_ERR_UNSUPPORTED, "out-of-place plans run on one device (world <= 1)");
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
   int dev = 0;
   TRY(check_device(opts, &dev));
   long long C = n;
@@ -100,8 +140,96 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
   P->oop = 1;
   P->oop_kind = result_kind;
   P->oop_ncols = ncols_out;
-  if (result_kind == FDB_OOP_SPARSE) TRY(oop_alloc_sparse(P, m * C));
+  P->oop_qcols = C;
+  if (result_kind == FDB_OOP_SPARSE && P->rank == 0) TRY(oop_alloc_sparse(P, m * C));
   *plan = owner.release();
+  return FDB_OK;
+}
+
+}  // extern "C"
+
+// `out` can take the whole result of P's kind
+static fdb_status oop_check_out(const fdb_plan *P, const fdb_oop_out *out) {
+  if (P->oop_kind != FDB_OOP_SPARSE) return FDB_OK;
+  const int64_t candidates = oop_candidates(P);
+  if (!out->colptr || !out->nnz || (candidates > 0 && (!out->rowval || !out->nzval)))
+    return fail(FDB_ERR_INVALID, "NULL colptr, rowval, nzval or nnz");
+  if (out->cap < candidates)
+    return fail(FDB_ERR_INVALID, "rowval / nzval capacity %lld < %lld candidate entries", (long long)out->cap,
+                (long long)candidates);
+  return FDB_OK;
+}
+
+// One rank's share: the colour loop of its colours (dense branch: its column block) and the finish of exactly the slots
+// it owns.  `base` is the whole target: the dense result, or the root's candidate buffer of a sparse result.
+static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *base, double *d_fx,
+                             const double *d_f_in, double relstep, double absstep, double dir, cudaStream_t s) {
+  if (oop_idle(P)) return FDB_OK;
+  const bool full = P->sp_kind == SP_NONE;
+  double *J = full ? base + P->col_begin * P->ldJ : base;
+  DeviceGuard g(P->device);
+  // a sparse result whose colorvec has no valid colour: nobody scatters, and the candidates are the zeros of rank 0
+  if (P->oop_kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->local_colors.empty() && P->E > 0)
+    CU(cudaMemsetAsync(J, 0, (size_t)P->E * 8, s));
+  P->oop_entry = true;
+  const fdb_status st = fdb_jacobian(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, (void *)s);
+  P->oop_entry = false;
+  TRY(st);
+  if (P->oop_kind == FDB_OOP_DENSE) {
+    if (!full && P->oop_dest_n > 0) {
+      oop_plus_zero_slots<<<P->grid(P->oop_dest_n), kThreads, 0, s>>>(J, P->oop_dest, P->oop_dest_n);
+      P->cnt.kernel_launches += 1;
+    } else if (full && P->m > 0) {
+      // column c < C of the block: 0.0 + q; the prototype's columns [C, ncols) are zeros, rank 0's alone
+      auto finish = [&](double *Jc, int64_t qcols, int64_t ncols) {
+        const int64_t work = ((P->m + kTile - 1) / kTile) * ncols;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(work, (int64_t)P->sm_count * 16));
+        oop_dense_finish<<<grid, kThreads, 0, s>>>(Jc, P->ldJ, P->m, qcols, ncols);
+        P->cnt.kernel_launches += 1;
+      };
+      const int64_t ncl = P->col_end - P->col_begin;
+      const int64_t tail = P->rank == 0 ? P->oop_ncols - P->oop_qcols : 0;
+      if (P->col_end == P->oop_qcols) {
+        finish(J, ncl, ncl + tail);
+      } else {
+        finish(J, ncl, ncl);
+        if (tail > 0) finish(base + P->oop_qcols * P->ldJ, 0, tail);
+      }
+    }
+  }
+  CU(cudaGetLastError());
+  return FDB_OK;
+}
+
+// The root-only finish of a sparse result, once every member has written its candidates: the compaction over all of
+// them (the full candidate count and maximum(colorvec)), fused with the quotients when one plan holds every f! output.
+static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const double *d_fx, const double *d_f_in,
+                                  cudaStream_t s) {
+  const bool full = P->sp_kind == SP_NONE;
+  const int64_t candidates = oop_candidates(P);
+  DeviceGuard g(P->device);
+  const int64_t ntiles = (candidates + kTile - 1) / kTile;
+  CU(cudaMemsetAsync(P->oop_state, 0, (size_t)(ntiles + 1) * 8, s));
+  CompactArgs a{};
+  a.vals = P->oop_vals; a.row32 = P->row32; a.colptr32 = P->colptr32;
+  a.ecolor = P->ecolor; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.ncolors = P->C;
+  a.fx = d_f_in ? d_f_in : (d_fx ? d_fx : P->fx_own);
+  a.ldF = P->fdtype == FDB_COMPLEX ? 2 * P->ldF : P->ldF;
+  a.E = candidates; a.m = P->m; a.C = P->oop_qcols; a.ncols = P->oop_ncols;
+  a.colptr = out->colptr; a.rowval = out->rowval; a.nzval = out->nzval; a.nnz = out->nnz;
+  a.state = P->oop_state; a.claim = P->oop_state + ntiles; a.tile_col = P->oop_tile_col;
+  auto go = [&](auto kern) { kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a); };
+  if (full) go(oop_compact<true, kCopy, uint8_t>);
+  else if (!P->oop_fused) go(oop_compact<false, kCopy, uint8_t>);
+  else TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    using CT = decltype(tag);
+    if (P->fdtype == FDB_CENTRAL) go(oop_compact<false, kCentral, CT>);
+    else if (P->fdtype == FDB_COMPLEX) go(oop_compact<false, kComplex, CT>);
+    else go(oop_compact<false, kForward, CT>);
+    return FDB_OK;
+  }));
+  P->cnt.kernel_launches += 1;
+  CU(cudaGetLastError());
   return FDB_OK;
 }
 
@@ -110,59 +238,18 @@ static fdb_status jacobian_oop_run(fdb_plan *P, fdb_fn f, void *ctx, const doubl
   if (!P || !f || !out) return fail(FDB_ERR_INVALID, "NULL plan, f or out");
   if (!P->oop) return fail(FDB_ERR_INVALID, "not an out-of-place plan (fdb_oop_plan_create_csc / _dense)");
   const bool sparse = P->oop_kind == FDB_OOP_SPARSE;
-  const bool full = P->sp_kind == SP_NONE;
-  const int64_t qcols = P->col_end - P->col_begin;   // dense branch: columns holding quotients, maximum(colorvec)
-  const int64_t candidates = full ? P->m * qcols : P->E;
-  if (sparse) {
-    if (!out->colptr || !out->nnz || (candidates > 0 && (!out->rowval || !out->nzval)))
-      return fail(FDB_ERR_INVALID, "NULL colptr, rowval, nzval or nnz");
-    if (out->cap < candidates)
-      return fail(FDB_ERR_INVALID, "rowval / nzval capacity %lld < %lld candidate entries", (long long)out->cap,
-                  (long long)candidates);
-  }
-  double *J = sparse ? P->oop_vals : out->J;
-  P->oop_entry = true;
-  const fdb_status st = fdb_jacobian(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, stream);
-  P->oop_entry = false;
-  TRY(st);
-  DeviceGuard g(P->device);
+  if (sparse && P->world > 1)
+    return fail(FDB_ERR_INVALID, "a sparse result is compacted over every rank's candidates on one device: run sparse rank "
+                                 "plans through fdb_group_create_oop_* / fdb_group_jacobian_oop");
+  if (!sparse && P->j_len > 0 && !out->J) return fail(FDB_ERR_INVALID, "NULL x or J");
+  TRY(oop_check_out(P, out));
   cudaStream_t s = (cudaStream_t)stream;
-  if (P->oop_kind == FDB_OOP_DENSE) {
-    if (!full && P->E > 0) {
-      oop_plus_zero_slots<<<P->grid(P->E), kThreads, 0, s>>>(J, P->dest, P->E);
-      P->cnt.kernel_launches += 1;
-    } else if (full && P->m > 0) {
-      const int64_t work = ((P->m + kTile - 1) / kTile) * P->oop_ncols;
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(work, (int64_t)P->sm_count * 16));
-      oop_dense_finish<<<grid, kThreads, 0, s>>>(J, P->ldJ, P->m, qcols, P->oop_ncols);
-      P->cnt.kernel_launches += 1;
-    }
-  } else if (sparse) {
-    const int64_t ntiles = (candidates + kTile - 1) / kTile;
-    CU(cudaMemsetAsync(P->oop_state, 0, (size_t)(ntiles + 1) * 8, s));
-    CompactArgs a{};
-    a.vals = P->oop_vals; a.row32 = P->row32; a.colptr32 = P->colptr32;
-    a.ecolor = P->ecolor; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.ncolors = P->C;
-    a.fx = d_f_in ? d_f_in : (d_fx ? d_fx : P->fx_own);
-    a.ldF = P->fdtype == FDB_COMPLEX ? 2 * P->ldF : P->ldF;
-    a.E = candidates; a.m = P->m; a.C = qcols; a.ncols = P->oop_ncols;
-    a.colptr = out->colptr; a.rowval = out->rowval; a.nzval = out->nzval; a.nnz = out->nnz;
-    a.state = P->oop_state; a.claim = P->oop_state + ntiles; a.tile_col = P->oop_tile_col;
-    auto go = [&](auto kern) { kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a); };
-    if (full) go(oop_compact<true, kCopy, uint8_t>);
-    else if (!P->oop_fused) go(oop_compact<false, kCopy, uint8_t>);
-    else TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-      using CT = decltype(tag);
-      if (P->fdtype == FDB_CENTRAL) go(oop_compact<false, kCentral, CT>);
-      else if (P->fdtype == FDB_COMPLEX) go(oop_compact<false, kComplex, CT>);
-      else go(oop_compact<false, kForward, CT>);
-      return FDB_OK;
-    }));
-    P->cnt.kernel_launches += 1;
-  }
-  CU(cudaGetLastError());
+  TRY(oop_member(P, f, ctx, d_x, sparse ? P->oop_vals : out->J, d_fx, d_f_in, relstep, absstep, dir, s));
+  if (sparse) TRY(oop_root_finish(P, out, d_fx, d_f_in, s));
   return FDB_OK;
 }
+
+extern "C" {
 
 fdb_status fdb_jacobian_oop(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
@@ -185,6 +272,56 @@ fdb_status fdb_jacobian_oop_complex(fdb_plan *P, fdb_fn_c f, void *ctx, const do
 fdb_status fdb_jvp_oop(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
                        double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
   return jvp_run(P, f, ctx, d_jvp, d_x, d_v, d_x1, d_fx1, d_f_in, relstep, absstep, dir, stream, true);
+}
+
+// ------------------------------------------------------------------------------------------------ single-process group
+fdb_status fdb_group_create_oop_csc(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                    const int64_t *colptr, const int64_t *rowval, const int64_t *colorvec, int result_kind,
+                                    int64_t ldJ, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_csc(p, m, n, colptr, rowval, colorvec, result_kind, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                      const int64_t *colorvec, int64_t ncols_out, int result_kind, int64_t ldJ,
+                                      const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_dense(p, m, n, colorvec, ncols_out, result_kind, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_jacobian_oop(fdb_group *g, fdb_fn f, void *const *ctx, const double *d_x, const fdb_oop_out *out,
+                                  double *d_fx, const double *d_f_in, double relstep, double absstep, double dir,
+                                  void *stream) {
+  if (!g || !f || !out) return fail(FDB_ERR_INVALID, "NULL group, f or out");
+  if (!g->oop) return fail(FDB_ERR_INVALID, "not an out-of-place group (fdb_group_create_oop_csc / _dense)");
+  fdb_plan *P0 = g->plans[0];
+  if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
+  if (P0->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
+  const bool sparse = P0->oop_kind == FDB_OOP_SPARSE;
+  if (!sparse && P0->j_len > 0 && !out->J) return fail(FDB_ERR_INVALID, "NULL x or J");
+  TRY(oop_check_out(P0, out));
+  const int root = g->devices[0];
+  cudaStream_t s0 = (cudaStream_t)stream;
+  {
+    DeviceGuard dg(root);
+    if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
+    // a dense result of a CSC sparsity: zero-filled once, by the owner of the buffer, before any member stores into it
+    if (g->n > 1 && P0->oop_kind == FDB_OOP_DENSE && P0->sp_kind == SP_CSC && P0->j_len > 0) TRY(zero_J(P0, out->J, s0));
+  }
+  double *base = sparse ? P0->oop_vals : out->J;
+  TRY(group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {
+    fdb_plan *P = g->plans[i];
+    const double *fin_i = d_f_in;
+    if (i > 0 && d_f_in && P->fdtype == FDB_FORWARD) TRY(member_replica(g, i, g->fin_rep, d_f_in, g->m, s, &fin_i));
+    return oop_member(P, f, ctx ? ctx[i] : nullptr, xi, base, i == 0 ? d_fx : nullptr, fin_i, relstep, absstep, dir, s);
+  }, [&](int i) { return oop_idle(g->plans[i]); }));
+  if (sparse) {
+    DeviceGuard dg(root);
+    TRY(oop_root_finish(P0, out, d_fx, d_f_in, s0));
+  }
+  return FDB_OK;
 }
 
 }  // extern "C"

@@ -343,6 +343,90 @@ class GroupHessian(_Group):
         self._check(st, wrapped)
 
 
+class GroupJacobianOOP(_Group):
+    """The out-of-place finite_difference_jacobian(f, x, cache, f_in; ...) on several GPUs from ONE process
+    (fdb_group_create_oop_* / fdb_group_jacobian_oop): the colours (dense branch: column blocks of the maximum(colorvec)
+    quotient columns) are split over `devices` as GroupJacobian splits them; devices[0] is the root and owns x and the
+    result.  Every member writes exactly its own slots of the root's result; a sparse result is compacted by the root once
+    every member has finished.  The result is bit-identical to finite_difference_jacobian on one device.  Device ordinals
+    may repeat ([0, 0] runs two members on one GPU).
+
+    fdtype, colorvec, sparsity, jac_prototype: as finite_difference_jacobian takes them (colorvec None: 1:length(x)).
+    The member plans are built on the first run for the (rows, length(x)) it sees, and rebuilt when those change.
+    plan_kw: max_batch, scratch_bytes, partition, use_graph (per member)."""
+
+    def __init__(self, devices, fdtype="forward", colorvec=None, sparsity=None, jac_prototype=None, **plan_kw):
+        self._set_devices(devices)
+        self.fdtype, self.colorvec, self.sparsity, self.jac_prototype = fdtype, colorvec, sparsity, jac_prototype
+        self.kind, self.pm, self.pn = api._oop_kind(sparsity, jac_prototype)
+        self._code = api._fdtype_code(fdtype)
+        self._plan_kw = plan_kw
+        self._key = None
+
+    def _build(self, m, n):
+        if self._key == (m, n):
+            return
+        if self._key is not None:
+            self.close()
+        o = api._opts(self._code, self.devices[0], **self._plan_kw)
+        devs = (C.c_int * len(self.devices))(*self.devices)
+        cv = None if api._is_identity_colorvec(self.colorvec, n) else self.colorvec
+        cvp, k0 = api._index_ptr(cv)
+        self._keep = [k0]
+        h = C.c_void_p()
+        lib = L.lib()
+        with torch.cuda.device(self.root):
+            if self.sparsity is not None:
+                cp, k1 = api._index_ptr(self.sparsity.colptr)
+                rv, k2 = api._index_ptr(self.sparsity.rowval)
+                self._keep += [k1, k2]
+                L.check(lib.fdb_group_create_oop_csc(C.byref(h), len(self.devices), devs, m, n, cp, rv, cvp, self.kind,
+                                                     max(m, 1), C.byref(o)))
+            else:
+                L.check(lib.fdb_group_create_oop_dense(C.byref(h), len(self.devices), devs, m, n, cvp, self.pn or 0,
+                                                       self.kind, max(m, 1), C.byref(o)))
+        self._adopt(h)
+        self._key = (m, n)
+
+    def run(self, fs, x, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):
+        """fs: one f per member — an out-of-place Python f(x) -> CUDA tensor (f.batched = True: (batch, n) -> (batch, m))
+        on that member's device, or a NativeFn (the in-place fdb_fn, context on that member's device).  x (float64, on
+        devices[0]) is never modified.  In forward mode without f_in, f(x) is evaluated once, by fs[0] at the root, and
+        passed on as f_in (jacobians.jl:299-300), so the members evaluate only their colours.  Rows of the result: those
+        of the sparsity or prototype, else of f_in or f(x), else length(x).  Returns what finite_difference_jacobian
+        returns: a dense column-major tensor, or a SparseMatrixCSC sized to the kept entries (one host sync)."""
+        if not api._is_cuda(x) or x.dtype != torch.float64 or x.device != self.root:
+            raise TypeError(f"x must be a float64 CUDA tensor on {self.root}")
+        if len(fs) != len(self.devices):
+            raise ValueError("one f per member")
+        xv = x.reshape(-1).contiguous()
+        n = xv.numel()
+        if stream is None:
+            stream = torch.cuda.current_stream(self.root).cuda_stream
+        f_in, m = api._oop_rows(fs[0], x, self._code, f_in, self.pm if self.pm is not None else n, self.sparsity, self.pm, n)
+        if f_in is None and self._code == L.FDB_FORWARD:       # a NativeFn: f(x) at the root, as the Python f above
+            f_in = torch.empty(m, dtype=torch.float64, device=self.root)
+            with torch.cuda.device(self.root):
+                api._native_call(fs[0], f_in, xv, stream)
+        self._build(m, n)
+        res = api._OopOutput(self.kind, self.sparsity, self.pn, m, self.plans[-1].dense_range()[1],
+                             self.plans[0].info()["n_entries"], self.root)
+        addr, ctxs, wrapped = self._member_fns(fs, m, n, oop=True)
+        fin_ptr = api._oop_fin_ptr(f_in, self._code, m)
+        with torch.cuda.device(self.root):
+            st = L.lib().fdb_group_jacobian_oop(self._h, addr, ctxs, xv.data_ptr(), C.byref(res.out), None, fin_ptr,
+                                                L.STEP_DEFAULT if relstep is None else float(relstep),
+                                                L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
+                                                C.c_void_p(stream))
+        self._check(st, wrapped)
+        return res.result(stream)
+
+    def close(self):
+        if self._key is not None:
+            super().close()
+            self._key = None
+
+
 class ShardedJacobian:
     """finite_difference_jacobian! with the colours of `cache.colorvec` sharded over the ranks of the default process
     group, one process per GPU (the cache must have been built with rank=, world=).

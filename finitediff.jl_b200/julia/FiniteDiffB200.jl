@@ -841,6 +841,111 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     DeviceCSC(host, nzval[1:k])
 end
 
+# ---- the out-of-place Jacobian on several GPUs from ONE call: the colours (dense branch: column blocks of the
+#      maximum(colorvec) quotient columns) are split over `devices`; devices[1] is the root and owns x and the result, every
+#      member writes exactly its own slots of it, and the root compacts a sparse result once every member has finished.
+#      Bit-identical to finite_difference_jacobian on one device.  kw: max_batch, scratch_bytes, partition, use_graph.
+mutable struct OopGroup
+    group::Group
+    kind::Cint
+    m::Int
+    n::Int
+    ncols::Int         # columns of the result (the prototype's, else maximum(colorvec))
+    cap::Int           # candidate entries of a sparse result
+    fdtype::Any
+end
+
+function oop_group_result(h, devices, roots, kind, m, n, ncols, fdtype)
+    g = Group(h[], length(devices), roots)
+    p0, pl = Ref{Ptr{Cvoid}}(C_NULL), Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:fdb_group_plan, libfdjac), Cint, (Ptr{Cvoid}, Cint, Ref{Ptr{Cvoid}}), g.handle, 0, p0))
+    check(ccall((:fdb_group_plan, libfdjac), Cint, (Ptr{Cvoid}, Cint, Ref{Ptr{Cvoid}}), g.handle, length(devices) - 1, pl))
+    i0 = Ref{PlanInfo}()
+    check(ccall((:fdb_plan_info, libfdjac), Cint, (Ptr{Cvoid}, Ref{PlanInfo}), p0[], i0))
+    b, e = Ref{Int64}(0), Ref{Int64}(0)
+    check(ccall((:fdb_plan_dense_range, libfdjac), Cint, (Ptr{Cvoid}, Ref{Int64}, Ref{Int64}), pl[], b, e))
+    kind == FDB_OOP_RAW && (ncols = e[])                       # C of the whole result: where the last block ends
+    OopGroup(g, kind, m, n, ncols, i0[].n_entries, fdtype)
+end
+
+# sparsity: a CSC pattern (SparseMatrixCSC or DeviceCSC); jac_prototype: nothing, a dense matrix or a sparse one
+function group_oop_csc(sparsity, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    sp = hostcsc(sparsity)
+    m, n = size(sp)
+    kind = jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC ? FDB_OOP_SPARSE : FDB_OOP_DENSE
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve sp croot devices begin
+        check(ccall((:fdb_group_create_oop_csc, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Ptr{Int64}, Ptr{Int64}, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), m, n, pointer(sp.colptr), pointer(sp.rowval), cptr, kind, max(m, 1), opts))
+    end
+    oop_group_result(h, devices, (sp, croot), kind, m, n, n, fdtype)
+end
+
+# sparsity === nothing: m rows (length of f(x)), n = length(x)
+function group_oop_dense(m::Integer, n::Integer, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    if jac_prototype === nothing
+        kind, ncols = FDB_OOP_RAW, 0
+    elseif jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC
+        kind, ncols = FDB_OOP_SPARSE, size(hostcsc(jac_prototype), 2)
+    else
+        kind, ncols = FDB_OOP_DENSE, size(jac_prototype, 2)
+    end
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve croot devices begin
+        check(ccall((:fdb_group_create_oop_dense, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Ptr{Int64}, Int64, Cint, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), m, n, cptr, ncols, kind, max(m, 1), opts))
+    end
+    oop_group_result(h, devices, croot, kind, m, n, ncols, fdtype)
+end
+
+# fs[i]: the out-of-place f(x) member i calls (its arrays live on devices[i]); x and f_in live on devices[1].  In forward mode
+# without f_in, f(x) is evaluated once by fs[1] at the root and passed on as f_in (:299-300): 1 + C calls in all.
+function group_jacobian(g::OopGroup, fs::Vector, x::CuVector{Float64}; f_in = nothing, relstep = nothing,
+        absstep = relstep, dir = true)
+    length(x) == g.n || throw(DimensionMismatch("length(x) = $(length(x)), the group was built for $(g.n)"))
+    fd = fdcode(g.fdtype)
+    if f_in === nothing && fd == FDB_FORWARD
+        f_in = vec(fs[1](x))
+    end
+    f_in === nothing || length(f_in) == g.m || throw(DimensionMismatch("length(f_in) != $(g.m)"))
+    states = [FnState(oop_f(f), g.m, g.n, nothing) for f in fs]
+    ctxs = Ptr{Cvoid}[pointer_from_objref(s) for s in states]
+    cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+    J = nothing
+    colptr = rowval = nzval = nnz = nothing
+    if g.kind == FDB_OOP_SPARSE
+        colptr, rowval = CuVector{Int64}(undef, g.ncols + 1), CuVector{Int64}(undef, max(g.cap, 1))
+        nzval, nnz = CuVector{Float64}(undef, max(g.cap, 1)), CuVector{Int64}(undef, 1)
+        out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), g.cap, pointer(nnz)))
+    else
+        J = CuMatrix{Float64}(undef, max(g.m, 1), g.ncols)
+        out = Ref(OopOut(pointer(J), CU_NULL, CU_NULL, CU_NULL, 0, CU_NULL))
+    end
+    rc = Cint(0)
+    GC.@preserve states ctxs x J colptr rowval nzval nnz f_in begin
+        rc = ccall((:fdb_group_jacobian_oop, libfdjac), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Ptr{Cvoid}}, CuPtr{Float64}, Ref{OopOut}, CuPtr{Float64}, CuPtr{Float64},
+                Float64, Float64, Float64, Ptr{Cvoid}),
+            g.group.handle, cf, pointer(ctxs), pointer(x), out, CU_NULL,
+            (f_in === nothing || fd != FDB_FORWARD) ? CU_NULL : pointer(f_in),
+            stepval(relstep), stepval(absstep), Float64(dir), CUDA.stream().handle)
+    end
+    for s in states
+        s.err === nothing || throw(s.err)
+    end
+    check(rc)
+    g.kind == FDB_OOP_SPARSE || return g.m == 0 ? J[1:0, :] : J
+    k = Int(Array(nnz)[1])                                     # the one host synchronisation
+    host = SparseMatrixCSC(g.m, g.ncols, Array(colptr), Array(rowval[1:k]), zeros(k))
+    DeviceCSC(host, nzval[1:k])
+end
+
 # cache-less form :240-259: f(x) once, then the cached form with it as f_in
 function finite_difference_jacobian(f, x::CuVector{Float64}, fdtype = Val(:forward), returntype = eltype(x), f_in = nothing;
         kw...)

@@ -411,12 +411,35 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  * fdb_oop_plan_create_dense: sparsity === nothing.  C = maximum(colorvec) (NULL => n) must be in 1..n.  FDB_OOP_RAW: J is
  *   m x C (ncols_out ignored); FDB_OOP_DENSE: J is m x ncols_out with ncols_out >= C (a narrower prototype is not built:
  *   FDB_ERR_UNSUPPORTED); FDB_OOP_SPARSE: ncols_out >= C (else FDB_ERR_INVALID, as sparse() throws).
- * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans; world <= 1.
+ * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans (rank plans below).
  * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
- *   dense kinds: out->J (device, ldJ of the plan);
+ *   dense kinds: out->J (device, ldJ of the plan; the whole result, rank plans included);
  *   FDB_OOP_SPARSE: out->colptr [ncols + 1], out->rowval / out->nzval [out->cap >= the candidate count: nnz of the sparsity,
  *   or m*C], Int64 1-based; the kept count goes to the device scalar *out->nnz (stream-ordered, no host sync).
- * fdb_plan_info(...).n_entries is the candidate count of a sparse result. */
+ * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a sparsity).
+ *
+ * Rank plans (opts.rank / opts.world, world in 2..64).  A rank evaluates only the colours it owns: the colour partition of
+ * the in-place plans (opts.partition: round-robin or LPT, fdb_plan_color_owner) with a sparsity, the contiguous column
+ * blocks of the dense plans over the C = maximum(colorvec) quotient columns (fdb_plan_dense_range) without one.  It uses
+ * the same pristine points, step rule and dir, and writes exactly the slots it owns:
+ *   FDB_OOP_RAW                 its column block of the m x C quotients;
+ *   FDB_OOP_DENSE, no sparsity  0.0 + q on its own columns; rank 0 also writes +0.0 to the prototype's columns [C, ncols);
+ *   FDB_OOP_DENSE, CSC          q, then + 0.0, on the structural slots of its own colours only; the owner of the buffer
+ *                               zero-fills J before any rank starts (opts.shared_j = 1; without it a rank zero-fills J
+ *                               itself, like an in-place rank plan);
+ *   FDB_OOP_SPARSE, CSC         its colours' candidate quotients, in storage order, into the root's candidate buffer (rank 0
+ *                               also writes the zeros of columns without a valid colour); the root then compacts all nnz
+ *                               candidates into `out`;
+ *   FDB_OOP_SPARSE, no sparsity its column block of the m x C candidates at offset col_begin*m; the root then compacts all
+ *                               m*C of them.
+ * Per rank: forward mode without d_f_in evaluates f(x) first, then its own colours ascending; central f(x+) then f(x-) per
+ * own colour; a rank > 0 that owns no colour (no column) calls nothing and launches nothing.  fdb_plan_info reports the
+ * rank's share (fcalls_per_jacobian, n_local_colors, byte model); n_entries stays the whole result's candidate count.
+ * A dense-kind rank plan may be driven on its own through fdb_jacobian_oop, every rank passing the same whole result: the
+ * ranks are then ordered as in-place shared_j rank plans are (fdb_sync_barrier, fdb_jacobian_oop, fdb_sync_barrier, after
+ * the owner's zero fill).  A sparse result needs every candidate on one device: fdb_jacobian_oop refuses a sparse rank
+ * plan with world > 1 (FDB_ERR_INVALID); fdb_group_jacobian_oop runs it.  Every kind, mode, dir and step override gives
+ * the one-device result bit for bit. */
 enum { FDB_OOP_RAW = 0, FDB_OOP_DENSE = 1, FDB_OOP_SPARSE = 2 };
 
 typedef struct {
@@ -435,6 +458,26 @@ fdb_status fdb_jacobian_oop(fdb_plan *plan, fdb_fn f, void *ctx, const double *d
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream);
 fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
                                     void *stream);
+
+/* One process, n devices: the group form of the out-of-place rank plans (fdb_group_size / fdb_group_plan /
+ * fdb_group_destroy as for Jacobians).  Member i runs rank i of n_devices on its own stream with ctx[i]; d_x, out, d_fx and
+ * d_f_in live on devices[0] (the root), x (and d_f_in, forward mode) is replicated to members on other devices, every
+ * member stores its slots straight into the root's result (sparse: the root's candidate buffer), and the members are
+ * joined on `stream` (a stream of devices[0]) with events.  Before any member starts, the root zero-fills a dense result
+ * of a CSC sparsity; after every member has finished, the root compacts a sparse result.  No host synchronisation: the
+ * kept count lands in *out->nnz.  Only the root writes f(x) to d_fx.  Device ordinals may repeat.  The result is
+ * bit-identical to fdb_jacobian_oop on one device.  Complex-step groups return FDB_ERR_UNSUPPORTED.
+ * fdb_group_jacobian_oop on a Jacobian or Hessian group, and fdb_group_jacobian / fdb_group_hessian on an out-of-place
+ * group, return FDB_ERR_INVALID before any launch. */
+fdb_status fdb_group_create_oop_csc(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                    const int64_t *colptr, const int64_t *rowval, const int64_t *colorvec, int result_kind,
+                                    int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                      const int64_t *colorvec, int64_t ncols_out, int result_kind, int64_t ldJ,
+                                      const fdb_plan_opts *opts);
+fdb_status fdb_group_jacobian_oop(fdb_group *group, fdb_fn f, void *const *ctx, const double *d_x, const fdb_oop_out *out,
+                                  double *d_fx, const double *d_f_in, double relstep, double absstep, double dir,
+                                  void *stream);
 
 /* Out-of-place JVP: jvp = finite_difference_jvp(f, x, v, cache, f_in; relstep, absstep, dir)  src/jvp.jl:159-189.  Same
  * plan (fdb_jvp_plan_create) and arguments as fdb_jvp; central mode evaluates f(x + eps v) into d_jvp BEFORE f(x - eps v)
