@@ -121,7 +121,12 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
     long long mn = 1;
     if (cv.d) TRY(color_range(cv.d, n, &C, &mn));
   }
-  if (C < 1) return fail(FDB_ERR_INVALID, "maximum(colorvec) = %lld: the dense out-of-place branch has no column", C);
+  // maximum(colorvec) < 1: the reference's colour loop 1:maximum(colorvec) is empty and J = zero(jac_prototype) is returned
+  // as it was made (after f(x) in forward mode); without a prototype it sizes J by mapreduce over that empty range, which
+  // throws.  C = 0 quotient columns: the finish zero-fills a dense prototype, the compaction of 0 candidates writes colptr 1
+  if (C < 1 && result_kind == FDB_OOP_RAW)
+    return fail(FDB_ERR_INVALID, "maximum(colorvec) = %lld: the dense out-of-place branch has no column", C);
+  if (C < 1) C = 0;
   if (C > n) return fail(FDB_ERR_INVALID, "maximum(colorvec) = %lld > length(x) = %lld (BoundsError in the reference)", C, (long long)n);
   if (result_kind == FDB_OOP_RAW) ncols_out = C;
   if (result_kind == FDB_OOP_DENSE && ncols_out < C)

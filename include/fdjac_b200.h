@@ -408,9 +408,11 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  * fdb_oop_plan_create_csc: sparsity is a CSC pattern (Int64, 1-based, host or device), result_kind FDB_OOP_DENSE (J dense
  *   m x n with leading dimension ldJ; a colouring in which two columns of one colour share a row is FDB_ERR_INVALID, as
  *   _make_Ji throws, :151-162) or FDB_OOP_SPARSE (ldJ ignored; any colouring).
- * fdb_oop_plan_create_dense: sparsity === nothing.  C = maximum(colorvec) (NULL => n) must be in 1..n.  FDB_OOP_RAW: J is
- *   m x C (ncols_out ignored); FDB_OOP_DENSE: J is m x ncols_out with ncols_out >= C (a narrower prototype is not built:
- *   FDB_ERR_UNSUPPORTED); FDB_OOP_SPARSE: ncols_out >= C (else FDB_ERR_INVALID, as sparse() throws).
+ * fdb_oop_plan_create_dense: sparsity === nothing.  C = maximum(colorvec) (NULL => n) must be at most n.  FDB_OOP_RAW: J is
+ *   m x C (ncols_out ignored; C < 1 is FDB_ERR_INVALID, as mapreduce over the empty colour range throws); FDB_OOP_DENSE: J
+ *   is m x ncols_out with ncols_out >= C (a narrower prototype is not built: FDB_ERR_UNSUPPORTED); FDB_OOP_SPARSE:
+ *   ncols_out >= C (else FDB_ERR_INVALID, as sparse() throws).  With the prototype kinds, C < 1 gives zero(jac_prototype):
+ *   +0.0 everywhere, or colptr all 1 and nnz 0, after f(x) in forward mode without d_f_in and no other call.
  * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans (rank plans below).
  * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
  *   dense kinds: out->J (device, ldJ of the plan; the whole result, rank plans included);

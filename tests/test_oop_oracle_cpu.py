@@ -103,6 +103,42 @@ def test_c_restatement_matches_the_transcription(seed):
             assert bits_equal(p, q), seed
 
 
+@pytest.mark.parametrize("cacheless", [False, True])
+@pytest.mark.parametrize("fd", ["forward", "central", "complex"])
+@pytest.mark.parametrize("proto", ["raw", "dense", "sparse"])
+@pytest.mark.parametrize("colour", [0, -2])
+def test_dense_branch_without_colours(colour, proto, fd, cacheless):
+    """sparsity = nothing with maximum(colorvec) < 1: the colour loop is empty, so both restatements return
+    zero(jac_prototype) (+0.0 everywhere, or colptr all 1 and nnz 0) after f(x) in forward mode; without a prototype the
+    result is sized by mapreduce over the empty range, which throws"""
+    rng = np.random.default_rng(7)
+    m, n = 4, 3
+    p1 = rng.integers(0, n, m)
+    f = lambda x: x[p1] * x[p1]
+    x = np.array([0.5, -0.0, 1.25])
+    kw = {"colorvec": np.full(n, colour, np.int64), "cacheless": cacheless}
+    if proto != "raw":
+        kw["jac_prototype"] = (proto, m, n + 1)
+    rl, ro = Rec(f), Rec(f)
+    outs = []
+    for impl, rec, extra in ((LO, rl, {}), (OO, ro, {"m": m})):
+        try:
+            outs.append(impl.jacobian_oop(rec, x.copy(), fd, None, **kw, **extra))
+        except (LO.MakeJiError, ValueError):
+            outs.append("throws")
+    if proto == "raw":
+        assert outs == ["throws", "throws"]
+        return
+    calls = 1 if (fd == "forward" or cacheless) else 0          # :299-300, or the cache-less form's own f(x) (:250-251)
+    assert len(rl.points) == len(ro.points) == calls
+    for out in outs:
+        if proto == "dense":
+            assert out[0] == "dense" and bits_equal(out[1], np.zeros((m, n + 1)))
+        else:
+            assert out[0] == "sparse" and out[1:3] == (m, n + 1)
+            assert np.array_equal(out[3], np.ones(n + 2, np.int64)) and out[4].size == 0 and out[5].size == 0
+
+
 @pytest.mark.parametrize("seed", range(60))
 def test_c_jvp_matches_the_transcription(seed):
     rng = np.random.default_rng(1000 + seed)
