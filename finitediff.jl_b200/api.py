@@ -620,6 +620,12 @@ def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> P
         else:
             raise TypeError(f"unsupported J type {type(J)} for a Tridiagonal sparsity")
         keep += [rows, cols, slots]
+    elif isinstance(sparsity, BandedBlockBandedMatrix) and _block_banded_plan_args(J, sparsity) is not None:
+        # J and sparsity are one square block-banded structure: the closed-form plan, no entry lists on the host
+        blocks, l, u, lam, mu, ldata = _block_banded_plan_args(J, sparsity)
+        L.check(lib.fdb_plan_create_block_banded(C.byref(h), len(blocks), blocks.ctypes.data if len(blocks) else None,
+                                                 l, u, lam, mu, ldata, cv_ptr, C.byref(o)))
+        keep += [blocks]
     elif isinstance(sparsity, BandedBlockBandedMatrix):
         # ext/FiniteDiffBlockBandedMatricesExt.jl:16-42: the hook's (block-row, sub-band) entry set, written by slot
         rows, cols, slots = sparsity.findstructralnz()
@@ -647,6 +653,21 @@ def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> P
     else:
         raise TypeError(f"unsupported sparsity type {type(sparsity)}")
     return Plan(h.value, tuple(keep))
+
+
+def _block_banded_plan_args(J, sparsity):
+    """(blocks, l, u, lam, mu, ldata) for fdb_plan_create_block_banded when J and `sparsity` are the same block-banded
+    structure with square blocks and non-negative bandwidths (BlockBandedMatrix included, in this mirror's layout);
+    None otherwise: a dense J, rectangular block lists or two different structures keep the slot-addressed route."""
+    if not isinstance(J, BandedBlockBandedMatrix) or not isinstance(sparsity, BandedBlockBandedMatrix):
+        return None
+    key = (J.rb, J.cb, J.l, J.u, J.lam, J.mu)
+    if key != (sparsity.rb, sparsity.cb, sparsity.l, sparsity.u, sparsity.lam, sparsity.mu) or J.rb != J.cb:
+        return None
+    if min(J.l, J.u, J.lam, J.mu) < 0:
+        return None
+    ldata = J.data.numel() if isinstance(J.data, torch.Tensor) else J.w * J.n
+    return np.asarray(J.rb, dtype=np.int64), J.l, J.u, J.lam, J.mu, ldata
 
 
 def _has_sparsestruct(J) -> bool:

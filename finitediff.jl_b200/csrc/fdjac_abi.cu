@@ -31,6 +31,7 @@
 #include "kernels_color.cuh"
 #include "kernels_hessian.cuh"
 #include "kernels_derivative.cuh"
+#include "kernels_blockband.cuh"
 
 using namespace fdb;
 
@@ -60,7 +61,7 @@ static fdb_status fail(fdb_status st, const char *fmt, ...) {
     if (s__ != FDB_OK) return s__;   \
   } while (0)
 
-enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7, SP_DERIV = 8 };
+enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7, SP_DERIV = 8, SP_BLOCKBAND = 9 };
 
 // Device memory that lives while a plan or a colouring is built: freed when it goes out of scope, unless release()
 // hands it to a plan that keeps it (fdb_plan::adopt).  Declared after the builder's DeviceGuard, it is freed on the
@@ -215,6 +216,11 @@ struct fdb_plan {
   bool staged = false, stage_packed = false;
   bool stage_band = false;             // exact clipped band: the staged pass derives rows and columns, reads no index stream
   int32_t band_l = 0, band_col_a = 0, band_col_b = 0, band_e_a = 0, band_e_b = 0, band_w = 1;
+  // block-banded plans (kernels_blockband.cuh): block offsets on the device, sub-block bandwidths, slots per column
+  int32_t *bb_off = nullptr;           // [nblocks + 1]
+  int32_t bb_nblocks = 0, bb_bs = 0;   // bb_bs > 0: every block has bb_bs columns
+  int64_t bb_lam = 0, bb_mu = 0, bb_w = 1;
+  bool bb_cyclic = false;              // colorvec is the block-cyclic closed form of matrix_colors
   std::vector<int64_t> bucket_start;   // [C+2] offsets into cols_by_color; bucket C = columns without a valid colour
   int lanes = 1;
   double mean_row_jump = 0.0;
@@ -1085,6 +1091,87 @@ fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t
   return finish_plan(owner, plan);
 }
 
+// BandedBlockBandedMatrix with square blocks (ext/FiniteDiffBlockBandedMatricesExt.jl:16-42): host work O(nblocks), the
+// structure stays a closed form (kernels_blockband.cuh)
+fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                        int64_t lam, int64_t mu, int64_t ldata, const int64_t *colorvec,
+                                        const fdb_plan_opts *opts) {
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  if (nblocks < 0 || nblocks > 0x7FFFFFF0LL) return fail(FDB_ERR_INVALID, "nblocks=%lld outside [0, 2^31)", (long long)nblocks);
+  if (nblocks > 0 && !blocks) return fail(FDB_ERR_INVALID, "blocks is NULL");
+  if (l < 0 || u < 0 || lam < 0 || mu < 0)
+    return fail(FDB_ERR_INVALID, "negative bandwidths (l, u) = (%lld, %lld), (lam, mu) = (%lld, %lld)", (long long)l,
+                (long long)u, (long long)lam, (long long)mu);
+  // slots per column: the kernels index a column with 32-bit offsets
+  const int64_t kMaxW = 0x7FFFFFF0LL;
+  if (l >= kMaxW || u >= kMaxW || lam >= kMaxW || mu >= kMaxW || (l + u + 1) > kMaxW / (lam + mu + 1))
+    return fail(FDB_ERR_UNSUPPORTED, "(l+u+1)(lam+mu+1) slots per column must be below 2^31");
+  const int64_t w = (l + u + 1) * (lam + mu + 1);
+  std::vector<int64_t> hb((size_t)nblocks);
+  if (nblocks > 0) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, blocks) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+    if (at.type == cudaMemoryTypeDevice) CU(cudaMemcpy(hb.data(), blocks, (size_t)nblocks * 8, cudaMemcpyDeviceToHost));
+    else std::memcpy(hb.data(), blocks, (size_t)nblocks * 8);
+  }
+  std::vector<int32_t> off((size_t)nblocks + 1, 0);
+  int64_t n = 0;
+  for (int64_t K = 0; K < nblocks; ++K) {
+    if (hb[(size_t)K] < 0) return fail(FDB_ERR_INVALID, "block %lld has negative size %lld", (long long)K, (long long)hb[(size_t)K]);
+    n += hb[(size_t)K];
+    if (n > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "the block sizes sum to more than 2^31 columns");
+    off[(size_t)K + 1] = (int32_t)n;
+  }
+  if (ldata < w * n) return fail(FDB_ERR_INVALID, "ldata=%lld < (l+u+1)(lam+mu+1)*n = %lld", (long long)ldata, (long long)(w * n));
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, n, n));
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  P->sp_kind = SP_BLOCKBAND;
+  P->jkind = FDB_J_BLOCK_BAND;
+  P->l = l;
+  P->u = u;
+  P->bb_lam = lam;
+  P->bb_mu = mu;
+  P->bb_w = w;
+  P->bb_nblocks = (int32_t)nblocks;
+  P->j_len = w * n;
+  P->bb_bs = nblocks > 0 && hb[0] > 0 && std::all_of(hb.begin(), hb.end(), [&](int64_t b) { return b == hb[0]; }) ? (int32_t)hb[0] : 0;
+  TRY(P->alloc_t(&P->bb_off, (size_t)nblocks + 1));
+  CU(cudaMemcpy(P->bb_off, off.data(), ((size_t)nblocks + 1) * 4, cudaMemcpyHostToDevice));
+  TRY(setup_colors(P, colorvec));
+  // structural entries per colour (the LPT weights; slot C: columns without a valid colour) and the colouring's form
+  DevBuf<unsigned long long> d_cnt;
+  DevBuf<uint32_t> d_flag;
+  TRY(d_cnt.alloc((size_t)P->C + 1));
+  TRY(d_flag.alloc(1));
+  CU(cudaMemset(d_cnt.get(), 0, ((size_t)P->C + 1) * 8));
+  CU(cudaMemset(d_flag.get(), 0, 4));
+  if (n > 0) {
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+      using CT = decltype(tag);
+      block_band_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, P->bb_off, (int32_t)nblocks, (int32_t)n, l, u,
+                                                        lam, mu, P->C, d_cnt.get(), d_flag.get());
+      CU(cudaGetLastError());
+      return FDB_OK;
+    }));
+  }
+  std::vector<unsigned long long> cnt((size_t)P->C + 1, 0);
+  TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C + 1, "block-banded entry counts"));
+  uint32_t not_cyclic = 1;
+  TRY(read_back(&not_cyclic, d_flag.get(), 1, "block-banded colouring form"));
+  P->bb_cyclic = n > 0 && P->C > 0 && not_cyclic == 0;
+  unsigned long long total = 0;
+  for (auto c : cnt) total += c;
+  P->E = (int64_t)total;
+  cnt.resize((size_t)std::max<int32_t>(P->C, 1));
+  TRY(finish_colored_plan(P, opts, cnt));
+  // every slot written once + the f! outputs read (one slab and f(x) / the minus slab per colour)
+  P->alg_bytes = 8 * w * n + 16 * n * (int64_t)P->C;
+  return finish_plan(owner, plan);
+}
+
 // dense column branch over the leading `ncols` components (ncols == n for the default colorvec = 1:n)
 static fdb_status create_dense(fdb_plan **plan, int64_t m, int64_t n, int64_t ldJ, int64_t ncols, const fdb_plan_opts *opts) {
   PlanPtr owner;
@@ -1287,7 +1374,8 @@ fdb_status fdb_plan_read_timing(fdb_plan *P, double *scatter_ms, int64_t *scatte
 fdb_status fdb_plan_set_peers(fdb_plan *P, int n_peers, double *const *peer_J) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
   if (n_peers < 0 || n_peers > 64) return fail(FDB_ERR_INVALID, "n_peers out of range");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_HESS || P->sp_kind == SP_DERIV)
+  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_BLOCKBAND || P->sp_kind == SP_HESS ||
+      P->sp_kind == SP_DERIV)
     return fail(FDB_ERR_UNSUPPORTED, "peer stores are implemented for the entry-driven (CSC / COO) scatters");
   DeviceGuard g(P->device);
   if (!P->d_peers) TRY(P->alloc_t(&P->d_peers, 64));
@@ -1435,12 +1523,13 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   const int64_t sF = COMPLEX ? 2 * P->ldF : P->ldF, sX = COMPLEX ? 2 * P->ldx : P->ldx;
   const int64_t n_local = (int64_t)P->local_colors.size();
   // fill_matrix!(J, false)  jacobians.jl:530-532 — needed where the scatter does not define every slot itself
-  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
+  const bool block_band = P->sp_kind == SP_BLOCKBAND;
+  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED && !block_band;
   const bool band_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_BAND;
   // (identity / band-data launches define every slot this rank is responsible for, including zeros for columns without
-  //  a valid colour).  With peer buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset
-  //  here would race with the peers' stores.
-  const bool self_defining = (ident || band_data) && n_local > 0;
+  //  a valid colour; block-banded launches do so even when the rank has no colour).  With peer buffers set the caller
+  //  zero-fills J and synchronises the ranks BEFORE the call: a memset here would race with the peers' stores.
+  const bool self_defining = block_band || ((ident || band_data) && n_local > 0);
   if (!self_defining && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
   auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
@@ -1560,6 +1649,34 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   auto scatter_group = [&](int64_t g, int64_t l0, int64_t G) -> fdb_status {
     if (P->oop_fused) return FDB_OK;   // out-of-place sparse result: the compaction forms the quotients (fdjac_oop.cuh)
     if (P->sp_kind == SP_CSC && P->strategy == 1) return scatter_lists(g, l0, G);
+    if (block_band) {
+      // every slot of the columns of this group's colours, and (first group of rank 0) of the columns without a valid
+      // colour: storage order, closed-form structure
+      BlockBandArgs a{};
+      a.jcolor = P->jcolor; a.boff = P->bb_off; a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps;
+      a.local_of = P->local_of; a.J = J; a.total = P->bb_w * P->n; a.ldF = sF;
+      a.C = P->C; a.l0 = (int32_t)l0; a.G = (int32_t)G;
+      a.write_other = (g == 0 && P->rank == 0) ? 1 : 0;
+      a.nblocks = P->bb_nblocks; a.u = (int32_t)P->u; a.mu = (int32_t)P->bb_mu;
+      a.uniform = P->bb_bs > 0 ? 1 : 0;
+      a.block_cyclic = P->bb_cyclic ? 1 : 0;
+      a.w = make_fastdiv((uint32_t)P->bb_w);
+      a.sw = make_fastdiv((uint32_t)(P->bb_lam + P->bb_mu + 1));
+      a.bs = make_fastdiv((uint32_t)std::max<int32_t>(P->bb_bs, 1));
+      a.bw = make_fastdiv((uint32_t)(P->l + P->u + 1));
+      if (a.total == 0) return FDB_OK;
+      const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
+      const int64_t tiles = (a.total + kBbTile - 1) / kBbTile;
+      // a store stream: an oversubscribed grid, as for the other band kernels
+      constexpr int kBbGridOver = 16;
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(
+          (int64_t)resident_grid(P, diff_scatter_block_band<CT, MODE>, sm, tiles) * kBbGridOver, tiles));
+      ScatterTimer tm(P, s);
+      diff_scatter_block_band<CT, MODE><<<grid, kThreads, sm, s>>>(a);
+      P->cnt.kernel_launches += 1;
+      P->cnt.scatter_launches += 1;
+      return FDB_OK;
+    }
     if (P->sp_kind == SP_BANDED) {
       BandArgs a{};
       ScatterTimer tm(P, s);   // one timed region per group: the pre-division pass (when used) + the band kernel
@@ -1729,6 +1846,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   }
   // columns without a valid colour when this rank evaluates no colour at all
   if (n_local == 0 && P->sp_kind == SP_CSC && P->strategy == 1 && (P->n_peers > 0 || P->shared_J)) TRY(scatter_group(0, 0, 0));
+  if (n_local == 0 && block_band && P->rank == 0) TRY(scatter_group(0, 0, 0));
   CU(cudaGetLastError());
   return FDB_OK;
 }

@@ -59,6 +59,8 @@ struct fdb_group {
 
 static bool plan_self_defining(const fdb_plan *P) {
   // the scatter launches of all ranks together define every slot of J (identity CSC: nzval; band data: whole columns)
+  // (block-banded: every column, including those without a valid colour, whatever the colour count)
+  if (P->sp_kind == SP_BLOCKBAND) return true;
   const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
   const bool band_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_BAND;
   return (ident || band_data) && P->C > 0;
@@ -207,6 +209,14 @@ fdb_status fdb_group_create_dense(fdb_group **group, int n_devices, const int *d
                                   const fdb_plan_opts *opts) {
   return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
     return fdb_plan_create_dense(p, m, n, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_create_block_banded(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                         const int64_t *blocks, int64_t l, int64_t u, int64_t lam, int64_t mu, int64_t ldata,
+                                         const int64_t *colorvec, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_plan_create_block_banded(p, nblocks, blocks, l, u, lam, mu, ldata, colorvec, o);
   });
 }
 

@@ -283,6 +283,12 @@ class GroupJacobian(_Group):
                 m, n, ld = api._dense_ld(J)
                 L.check(lib.fdb_group_create_banded(C.byref(h), n_dev, devs, m, n, sparsity.l, sparsity.u, L.FDB_J_DENSE, ld,
                                                     cv_ptr, C.byref(o)))
+        elif api._block_banded_plan_args(J, sparsity) is not None:
+            blocks, l, u, lam, mu, ldata = api._block_banded_plan_args(J, sparsity)
+            self._keep.append(blocks)
+            L.check(lib.fdb_group_create_block_banded(C.byref(h), n_dev, devs, len(blocks),
+                                                      blocks.ctypes.data if len(blocks) else None, l, u, lam, mu, ldata,
+                                                      cv_ptr, C.byref(o)))
         else:
             raise TypeError(f"GroupJacobian: unsupported sparsity type {type(sparsity)}")
         self._adopt(h)

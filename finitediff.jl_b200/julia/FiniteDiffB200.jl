@@ -38,7 +38,7 @@ import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, Jacobian
 const libfdjac = get(ENV, "FDJAC_B200_LIB", "libfdjac_b200.so")
 
 const FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = Cint(0), Cint(1), Cint(2), Cint(3)
-const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS = Cint(0), Cint(1), Cint(2), Cint(3)
+const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND = Cint(0), Cint(1), Cint(2), Cint(3), Cint(4)
 const FDB_STEP_DEFAULT = NaN            # relstep / absstep keyword not given (include/fdjac_b200.h)
 const FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = Cint(0), Cint(1), Cint(2)
 
@@ -117,6 +117,20 @@ struct DeviceBanded                          # BandedMatrices.BandedMatrix: data
 end
 Base.size(J::DeviceBanded) = (J.m, J.n)
 Base.size(J::DeviceBanded, d) = d == 1 ? J.m : J.n
+
+# BlockBandedMatrices.BandedBlockBandedMatrix with square blocks: the block sizes blocklengths(axes(J, 1)), the block
+# bandwidths blockbandwidths(J), the sub-block bandwidths subblockbandwidths(J) and the band data on the device:
+# (l+u+1)(lam+mu+1) slots per column, entry (k, j) of block (K, J) at slot (K-J+u)(lam+mu+1) + (mu+k-j) (0-based k, j)
+struct DeviceBlockBanded
+    blocks::Vector{Int64}
+    l::Int
+    u::Int
+    lam::Int
+    mu::Int
+    data::CuVector{Float64}                  # (l+u+1)(lam+mu+1) * sum(blocks), column-major
+end
+Base.size(J::DeviceBlockBanded) = (sum(J.blocks), sum(J.blocks))
+Base.size(J::DeviceBlockBanded, d) = sum(J.blocks)
 
 struct DeviceTridiagonal                     # LinearAlgebra.Tridiagonal(dl, d, du): one buffer [dl; d; du]
     n::Int
@@ -247,6 +261,24 @@ function plan_banded(anchor, m::Integer, n::Integer, l::Integer, u::Integer, jk:
     end
 end
 
+# sparsity::BandedBlockBandedMatrix, J the same structure: ext/FiniteDiffBlockBandedMatricesExt.jl:16-42 as a closed form
+# (no entry lists on the host)
+function plan_block_banded(J::DeviceBlockBanded, colorvec, fd::Cint; kw...)
+    key = (:block_banded, J.blocks, J.l, J.u, J.lam, J.mu, length(J.data), color_key(colorvec), fd, values(kw))
+    cached_plan(J.data, key) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd; kw...))
+        cptr, croot = color_arg(colorvec, size(J, 2))
+        blocks = J.blocks
+        GC.@preserve blocks croot begin
+            check(ccall((:fdb_plan_create_block_banded, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Ptr{Int64}, Int64, Int64, Int64, Int64, Int64, Ptr{Int64}, Ref{PlanOpts}),
+                h, length(blocks), pointer(blocks), J.l, J.u, J.lam, J.mu, length(J.data), cptr, opts))
+        end
+        Plan(h[], (blocks, croot))
+    end
+end
+
 # sparsity === nothing: dense column branch; a non-default colorvec reproduces jacobians.jl:547-557 as written
 function plan_dense(anchor, m::Integer, n::Integer, ldJ::Integer, colorvec, fd::Cint; kw...)
     key = (:dense, m, n, ldJ, color_key(colorvec), fd, values(kw))
@@ -335,7 +367,7 @@ function run_plan!(plan::Plan, jvals::CuArray{Float64}, f, x::CuVector{Float64},
     nothing                                  # jacobians.jl:652
 end
 
-const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceTridiagonal, CuMatrix{Float64}}
+const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceTridiagonal, CuMatrix{Float64}}
 
 ld(J::CuMatrix) = max(stride(J, 2), size(J, 1), 1)
 
@@ -349,6 +381,11 @@ end
 function plan_for(J::DeviceBanded, sp, colorvec, fd)
     (sp isa DeviceBanded && (sp.l, sp.u) == (J.l, J.u)) || throw(ArgumentError("J and sparsity must have the same bandwidths"))
     (plan_banded(J.data, J.m, J.n, J.l, J.u, FDB_J_BAND, 0, colorvec, fd), J.data)
+end
+function plan_for(J::DeviceBlockBanded, sp, colorvec, fd)
+    (sp isa DeviceBlockBanded && (sp.blocks, sp.l, sp.u, sp.lam, sp.mu) == (J.blocks, J.l, J.u, J.lam, J.mu)) ||
+        throw(ArgumentError("J and sparsity must have the same block structure"))
+    (plan_block_banded(J, colorvec, fd), J.data)
 end
 function plan_for(J::DeviceTridiagonal, sp, colorvec, fd)
     (plan_coo(() -> tridiagonal_structure(J.n), J.buf, J.n, J.n, :tridiagonal, FDB_J_SLOTS, 3 * J.n - 2, colorvec, fd), J.buf)
@@ -382,7 +419,7 @@ end
                                 relstep, absstep, colorvec, sparsity, dir)
 
 Same signature and keyword meaning as `src/jacobians.jl:504-514`.  `J` is a `DeviceCSC`, `DeviceBanded`,
-`DeviceTridiagonal` or a dense `CuMatrix{Float64}`; `x`, `cache.fx`, `f_in` are `CuVector{Float64}`.
+`DeviceBlockBanded`, `DeviceTridiagonal` or a dense `CuMatrix{Float64}`; `x`, `cache.fx`, `f_in` are `CuVector{Float64}`.
 `relstep` / `absstep` left at their defaults are passed as FDB_STEP_DEFAULT; explicit values (0 included) as given.
 """
 function finite_difference_jacobian!(J::DeviceJ, f, x::CuVector{Float64},
@@ -642,6 +679,20 @@ function group_banded(J::DeviceBanded, colorvec, fdtype, devices::Vector{Cint}; 
             h, length(devices), pointer(devices), J.m, J.n, J.l, J.u, FDB_J_BAND, 0, cptr, opts))
     end
     Group(h[], length(devices), croot)
+end
+
+function group_block_banded(J::DeviceBlockBanded, colorvec, fdtype, devices::Vector{Cint}; kw...)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, size(J, 2))
+    blocks = J.blocks
+    GC.@preserve blocks croot devices begin
+        check(ccall((:fdb_group_create_block_banded, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Ptr{Int64}, Int64, Int64, Int64, Int64, Int64, Ptr{Int64}, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), length(blocks), pointer(blocks), J.l, J.u, J.lam, J.mu, length(J.data),
+            cptr, opts))
+    end
+    Group(h[], length(devices), (blocks, croot))
 end
 
 function group_dense(J::CuMatrix{Float64}, fdtype, devices::Vector{Cint}; kw...)

@@ -57,7 +57,8 @@ typedef enum {
   FDB_J_CSC_NZVAL = 0, /* J::SparseMatrixCSC with the sparsity's pattern: nzval[p]   (ext/FiniteDiffSparseArraysExt.jl:38-47) */
   FDB_J_DENSE = 1,     /* J::Matrix column-major, leading dimension ldJ              (ext/..SparseArraysExt.jl:20-28, iteration_utils.jl:25-32) */
   FDB_J_BAND = 2,      /* J::BandedMatrix data[(l+u+1) x n], slot [u+r-c+1, c]        (ext/FiniteDiffBandedMatricesExt.jl:13-27) */
-  FDB_J_SLOTS = 3      /* structured J (e.g. Tridiagonal): explicit 1-based slot per structural entry (iteration_utils.jl:25-32) */
+  FDB_J_SLOTS = 3,     /* structured J (e.g. Tridiagonal): explicit 1-based slot per structural entry (iteration_utils.jl:25-32) */
+  FDB_J_BLOCK_BAND = 4 /* J::BandedBlockBandedMatrix band data, (l+u+1)(lam+mu+1) slots per column (fdb_plan_create_block_banded) */
 } fdb_jkind;
 
 /*
@@ -171,6 +172,25 @@ fdb_status fdb_plan_create_coo(fdb_plan **plan, int64_t m, int64_t n, int64_t nn
 fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, int jkind, int64_t ldJ,
                                   const int64_t *colorvec, const fdb_plan_opts *opts);
 
+/* sparsity::BandedBlockBandedMatrix with square blocks, J the same structure: ext/FiniteDiffBlockBandedMatricesExt.jl:16-42.
+ *   blocks: nblocks block sizes (Int64, host or device; the column sizes are the row sizes, as the hook takes them from
+ *   axes(Jac, 1)); n = m = sum(blocks).  (l, u) block bandwidths, (lam, mu) sub-block bandwidths, all >= 0.
+ *   J is the band data: w = (l+u+1)(lam+mu+1) slots per column, column-major; entry (k, j) of block (K, J) sits at slot
+ *   (K-J+u)(lam+mu+1) + (mu+k-j) of its global column (0-based k, j inside the blocks).  ldata >= w*n doubles.
+ * The structure is a closed form: plan-time host work is O(nblocks), the plan keeps the block offsets on the device and
+ * reads no index stream.  Every call writes every one of the w*n slots exactly once — the quotient on the structural
+ * slots of columns with a valid colour, +0.0 everywhere else — with the values of the fill_matrix!-then-scatter of the
+ * slot-addressed route (fdb_plan_create_coo with FDB_J_SLOTS on the hook's entry set); slots [w*n, ldata) are not touched.
+ * The colouring of ArrayInterface.matrix_colors, (J mod (l+u+1))(lam+mu+1) + (j mod (lam+mu+1)) + 1, is detected and
+ * then read in closed form.  opts as for the other coloured plans (forward / central / complex, max_batch, scratch_bytes,
+ * no_drift, use_graph, rank / world / partition, fdb_plan_set_external_eps); fdb_plan_set_peers is FDB_ERR_UNSUPPORTED.
+ * A rank plan writes the columns of its own colours (rank 0 also those without a valid colour), so the ranks together
+ * write every slot once and nobody zero-fills J.  Negative sizes or bandwidths, ldata < w*n, a NULL blocks with
+ * nblocks > 0: FDB_ERR_INVALID.  fdb_plan_info: jkind FDB_J_BLOCK_BAND, n_entries = structural entries, j_len = w*n. */
+fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                        int64_t lam, int64_t mu, int64_t ldata, const int64_t *colorvec,
+                                        const fdb_plan_opts *opts);
+
 /* sparsity === nothing: dense column branch jacobians.jl:548-557,590-598 (colorvec = 1:n; per-component step).
  * With world>1 the columns are block-partitioned: this rank computes columns [col_begin, col_end) (0-based, see
  * fdb_plan_info) and d_J passed to fdb_jacobian points at THAT column slab (ldJ x ncols_local). */
@@ -269,6 +289,11 @@ fdb_status fdb_group_create_banded(fdb_group **group, int n_devices, const int *
                                    int64_t u, int jkind, int64_t ldJ, const int64_t *colorvec, const fdb_plan_opts *opts);
 fdb_status fdb_group_create_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t ldJ,
                                   const fdb_plan_opts *opts);
+/* block-banded groups: member i writes every slot of the columns of its own colours straight into the root's band data,
+ * member 0 also the columns without a valid colour; the column sets are disjoint, so J is never zero-filled. */
+fdb_status fdb_group_create_block_banded(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                         const int64_t *blocks, int64_t l, int64_t u, int64_t lam, int64_t mu, int64_t ldata,
+                                         const int64_t *colorvec, const fdb_plan_opts *opts);
 fdb_status fdb_group_destroy(fdb_group *group);
 fdb_status fdb_group_size(const fdb_group *group, int *n_members);
 /* member i's plan (owned by the group): fdb_plan_info / fdb_plan_counters / fdb_plan_get_eps / fdb_plan_color_owner */
