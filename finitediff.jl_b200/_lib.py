@@ -15,7 +15,7 @@ SYNTH_PATH = HERE / "libfdjac_synth.so"
 
 FDB_OK, FDB_ERR_INVALID, FDB_ERR_CUDA, FDB_ERR_CALLBACK, FDB_ERR_NOMEM, FDB_ERR_UNSUPPORTED, FDB_ERR_NO_DEVICE = range(7)
 FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = 0, 1, 2, 3
-FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND = 0, 1, 2, 3, 4
+FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND, FDB_J_DIAGONALS = 0, 1, 2, 3, 4, 5
 FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = 0, 1, 2
 # FDB_STEP_DEFAULT: relstep / absstep keyword not given (any other value, 0 included, is used as passed)
 STEP_DEFAULT = float("nan")

@@ -31,7 +31,8 @@ import torch
 from . import _lib as L
 
 __all__ = [
-    "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "BandedBlockBandedMatrix", "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
+    "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "Diagonal", "Bidiagonal", "SymTridiagonal", "BandedBlockBandedMatrix",
+    "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
     "finite_difference_jacobian_", "finite_difference_jacobian_b", "resize_", "default_relstep", "compute_epsilon",
     "zeros_colmajor", "pinned_empty", "HessianCache", "finite_difference_hessian_", "finite_difference_hessian",
     "GradientCache", "finite_difference_gradient_", "finite_difference_gradient", "DerivativeCache",
@@ -258,6 +259,106 @@ class Tridiagonal:
         b = self.buf.cpu().numpy()
         n = self.n
         return np.diag(b[n - 1: 2 * n - 1]) + np.diag(b[: n - 1], -1) + np.diag(b[2 * n - 1:], 1)
+
+
+def _band_entries(n, l, u):
+    """1-based (rows, cols, slots) of the in-matrix band (l, u), l, u in {0, 1}, in the packed diagonal storage:
+    sub-diagonal, main diagonal, super-diagonal, each from the top left (the layout of FDB_J_DIAGONALS)."""
+    rows, cols = [], []
+    if l and n > 1:
+        rows.append(np.arange(2, n + 1))
+        cols.append(np.arange(1, n))
+    rows.append(np.arange(1, n + 1))
+    cols.append(np.arange(1, n + 1))
+    if u and n > 1:
+        rows.append(np.arange(1, n))
+        cols.append(np.arange(2, n + 1))
+    rows = np.concatenate(rows).astype(np.int64)
+    cols = np.concatenate(cols).astype(np.int64)
+    return rows, cols, np.arange(1, len(rows) + 1, dtype=np.int64)
+
+
+class Diagonal:
+    """Mirror of LinearAlgebra.Diagonal(d): one buffer [d] of n values; its structural nonzeros are the main diagonal,
+    the band (0, 0)."""
+
+    l, u = 0, 0
+
+    def __init__(self, n, buf=None, device="cuda"):
+        self.n = int(n)
+        if buf is None:
+            buf = torch.zeros(self.n, dtype=torch.float64, device=device)
+        self.buf = buf
+
+    @property
+    def shape(self):
+        return (self.n, self.n)
+
+    def findstructralnz(self):
+        return _band_entries(self.n, 0, 0)
+
+    def to_dense(self) -> np.ndarray:
+        return np.diag(self.buf.cpu().numpy())
+
+
+class Bidiagonal:
+    """Mirror of LinearAlgebra.Bidiagonal(dv, ev, uplo): one buffer in ascending row-minus-column order, [dv; ev] for
+    uplo = :U (band (0, 1)) and [ev; dv] for :L (band (1, 0)); dv holds n values, ev n-1."""
+
+    def __init__(self, n, uplo, buf=None, device="cuda"):
+        self.n = int(n)
+        self.uplo = str(uplo).lstrip(":").upper()
+        if self.uplo not in ("U", "L"):
+            raise ValueError(f"uplo must be :U or :L, got {uplo!r}")
+        if buf is None:
+            buf = torch.zeros(max(2 * self.n - 1, 0), dtype=torch.float64, device=device)
+        self.buf = buf
+
+    @property
+    def l(self):
+        return 1 if self.uplo == "L" else 0
+
+    @property
+    def u(self):
+        return 1 if self.uplo == "U" else 0
+
+    @property
+    def shape(self):
+        return (self.n, self.n)
+
+    @property
+    def dv(self):
+        return self.buf[: self.n] if self.uplo == "U" else self.buf[self.n - 1: 2 * self.n - 1]
+
+    @property
+    def ev(self):
+        return self.buf[self.n: 2 * self.n - 1] if self.uplo == "U" else self.buf[: max(self.n - 1, 0)]
+
+    def findstructralnz(self):
+        return _band_entries(self.n, self.l, self.u)
+
+    def to_dense(self) -> np.ndarray:
+        dv, ev = self.dv.cpu().numpy(), self.ev.cpu().numpy()
+        return np.diag(dv) + (np.diag(ev, 1) if self.uplo == "U" else np.diag(ev, -1))
+
+
+class SymTridiagonal:
+    """Mirror of LinearAlgebra.SymTridiagonal as a sparsity: the band (1, 1), the same entry lists as Tridiagonal.  It
+    holds no values by default; `buf` = [dv; ev] may be given for n <= 1, where it is a valid Jacobian target.  As a
+    target with n >= 2 it is refused before any f call: LinearAlgebra's setindex! refuses its off-diagonal entries."""
+
+    l, u = 1, 1
+
+    def __init__(self, n, buf=None):
+        self.n = int(n)
+        self.buf = buf
+
+    @property
+    def shape(self):
+        return (self.n, self.n)
+
+    def findstructralnz(self):
+        return _band_entries(self.n, 1, 1)
 
 
 class BandedBlockBandedMatrix:
@@ -559,13 +660,18 @@ def _dense_ld(J: torch.Tensor):
 def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> Plan:
     """Create the fdb_plan for (typeof(J), sparsity, colorvec, fdtype) — the dispatch the reference performs with
     _use_findstructralnz / _use_sparseCSC_common_sparsity / typeof(J) (jacobians.jl:522-535)."""
+    diag_route = _diagonals_route(J, sparsity)     # first: a refused target raises before anything is built
     lib = L.lib()
     fd = _fdtype_code(fdtype)
     o = _opts(fd, _device_index(device), **plan_kw)
     h = C.c_void_p()
     cv_ptr, cv_keep = _index_ptr(colorvec)
     keep = [cv_keep]
-    if sparsity is None:
+    if diag_route is not None:
+        # Diagonal / Bidiagonal / SymTridiagonal sparsity: the banded plan with the band (l, u) of the type, into the packed
+        # diagonal storage of the same type or into a dense J
+        L.check(lib.fdb_plan_create_banded(C.byref(h), *diag_route, cv_ptr, C.byref(o)))
+    elif sparsity is None:
         # dense column branch (jacobians.jl:548-557): column i of J from perturbing component i, colorvec = 1:n.
         # With sparsity === nothing and any OTHER colorvec the reference loops color_i in 1:maximum(colorvec) and
         # perturbs COMPONENT color_i (the colour id used as an index), writing only those leading columns of J (J is
@@ -607,7 +713,7 @@ def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> P
                                                C.byref(o)))
         else:
             raise TypeError(f"unsupported J type {type(J)} for a BandedMatrix sparsity")
-    elif isinstance(sparsity, Tridiagonal):
+    elif isinstance(sparsity, (Tridiagonal, SymTridiagonal)):
         rows, cols, slots = sparsity.findstructralnz()
         n = sparsity.n
         if isinstance(J, Tridiagonal):
@@ -670,9 +776,43 @@ def _block_banded_plan_args(J, sparsity):
     return np.asarray(J.rb, dtype=np.int64), J.l, J.u, J.lam, J.mu, ldata
 
 
+_LA_BANDED = (Diagonal, Bidiagonal, SymTridiagonal)
+
+
+def _diagonals_route(J, sparsity):
+    """(m, n, l, u, jkind, ldJ) for fdb_plan_create_banded when `sparsity` is a Diagonal, Bidiagonal or SymTridiagonal:
+    its band (l, u) written into the packed diagonal storage of a J of the same type and size (FDB_J_DIAGONALS), or into
+    a dense J (FDB_J_DENSE).  None for every other sparsity, which keeps its route (a Tridiagonal sparsity stays on the
+    slot-addressed COO route, and so does a Tridiagonal J with a SymTridiagonal sparsity).
+
+    A SymTridiagonal J with n >= 2 raises ValueError (Julia: ArgumentError) here, before any f call; the reference
+    throws the same from LinearAlgebra's setindex! at the first off-diagonal store, after colour 1's f calls.  A J of
+    another structured type than the sparsity raises TypeError."""
+    if isinstance(J, SymTridiagonal) and J.n >= 2:
+        raise ValueError("ArgumentError: a SymTridiagonal cannot be a Jacobian target: its off-diagonal entries cannot be "
+                         "set one at a time (use Tridiagonal)")
+    if not isinstance(sparsity, _LA_BANDED):
+        return None
+    n, l, u = sparsity.n, sparsity.l, sparsity.u
+    if isinstance(J, torch.Tensor):
+        m, nn, ld = _dense_ld(J)
+        if (m, nn) != (n, n):
+            raise ValueError("size(J) != size(sparsity)")
+        return n, n, l, u, L.FDB_J_DENSE, ld
+    if isinstance(J, Tridiagonal) and isinstance(sparsity, SymTridiagonal):
+        return None
+    if type(J) is not type(sparsity) or (isinstance(J, SymTridiagonal) and J.buf is None):
+        raise TypeError(f"unsupported J type {type(J)} for a {type(sparsity).__name__} sparsity")
+    if J.n != n or (J.l, J.u) != (l, u):
+        raise ValueError("J and sparsity must have the same size and bands")
+    if isinstance(J, SymTridiagonal):
+        l = u = 0                                       # n <= 1: the main diagonal is the whole structure
+    return n, n, l, u, L.FDB_J_DIAGONALS, J.buf.numel()
+
+
 def _has_sparsestruct(J) -> bool:
     """ArrayInterface.has_sparsestruct(J) as used at jacobians.jl:455."""
-    return isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix))
+    return isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix) + _LA_BANDED)
 
 
 def _j_values(J):
@@ -680,7 +820,7 @@ def _j_values(J):
         return J.nzval
     if isinstance(J, BandedMatrix):
         return J.data
-    if isinstance(J, Tridiagonal):
+    if isinstance(J, (Tridiagonal,) + _LA_BANDED):
         return J.buf
     if isinstance(J, BandedBlockBandedMatrix):
         return J.data
@@ -696,6 +836,12 @@ def _j_key(J):
         return ("band", J.m, J.n, J.l, J.u)
     if isinstance(J, Tridiagonal):
         return ("tri", J.n)
+    if isinstance(J, Diagonal):
+        return ("diag", J.n)
+    if isinstance(J, Bidiagonal):
+        return ("bidiag", J.n, J.uplo)
+    if isinstance(J, SymTridiagonal):
+        return ("symtri", J.n)
     if isinstance(J, BandedBlockBandedMatrix):
         return ("bbb", tuple(J.rb), tuple(J.cb), J.l, J.u, J.lam, J.mu)
     if isinstance(J, torch.Tensor):
@@ -710,7 +856,7 @@ def _j_key(J):
 def _sp_key(sp):
     if sp is None:
         return None
-    if isinstance(sp, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix)):
+    if isinstance(sp, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix) + _LA_BANDED):
         return _j_key(sp)
     if isinstance(sp, torch.Tensor):
         return ("proto", sp.data_ptr(), tuple(sp.shape), sp._version)
@@ -808,13 +954,18 @@ def resize_(cache: JacobianCache, i: int):
 # ------------------------------------------------------------------------------------------------ colouring
 def matrix_colors(A, device=None) -> torch.Tensor:
     """ArrayInterface.matrix_colors(A) on the device: an Int64 CUDA tensor of 1-based colours, ready to be passed as
-    `colorvec`.  Tridiagonal -> 1,2,3,...; BandedMatrix(l,u) -> cycle 1:(l+u+1) (ArrayInterface's closed forms);
+    `colorvec`.  Tridiagonal and SymTridiagonal -> 1,2,3,...; Diagonal -> all 1; Bidiagonal -> 1,2,1,2,...;
+    BandedMatrix(l,u) -> cycle 1:(l+u+1) (ArrayInterface's closed forms);
     SparseMatrixCSC -> a valid distance-2 column colouring (deterministic Jones-Plassmann, fdb_matrix_colors_csc);
     dense tensors -> 1:n (ArrayInterface: eachindex of the columns)."""
     lib = L.lib()
     if isinstance(A, Tridiagonal):
         n, l, u = A.n, 1, 1
         dev = A.buf.device if device is None else torch.device(device)
+    elif isinstance(A, _LA_BANDED):
+        n, l, u = A.n, A.l, A.u
+        buf_dev = A.buf.device if isinstance(A.buf, torch.Tensor) and A.buf.is_cuda else torch.device("cuda")
+        dev = buf_dev if device is None else torch.device(device)
     elif isinstance(A, BandedMatrix):
         n, l, u = A.n, A.l, A.u
         dev = (A.data.device if isinstance(A.data, torch.Tensor) and A.data.is_cuda else torch.device("cuda")) if device is None else torch.device(device)
@@ -1320,7 +1471,7 @@ def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absst
 
 
 def _shape_of(J):
-    if isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, DenseColumnBlock)):
+    if isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, DenseColumnBlock) + _LA_BANDED):
         return J.shape
     if isinstance(J, torch.Tensor):
         if J.dim() == 1:

@@ -32,6 +32,7 @@
 #include "kernels_hessian.cuh"
 #include "kernels_derivative.cuh"
 #include "kernels_blockband.cuh"
+#include "kernels_diagonals.cuh"
 
 using namespace fdb;
 
@@ -1059,15 +1060,24 @@ fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t
   TRY(new_plan(plan, owner, opts, m, n));
   fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  if (jkind != FDB_J_BAND && jkind != FDB_J_DENSE) return fail(FDB_ERR_INVALID, "banded sparsity supports J kinds BAND and DENSE");
+  if (jkind != FDB_J_BAND && jkind != FDB_J_DENSE && jkind != FDB_J_DIAGONALS)
+    return fail(FDB_ERR_INVALID, "banded sparsity supports J kinds BAND and DENSE (and DIAGONALS for diagonal storage)");
   if (l + u + 1 < 1 || l < -n || u < -m) return fail(FDB_ERR_INVALID, "invalid bandwidths l=%lld u=%lld", (long long)l, (long long)u);
   if (jkind == FDB_J_DENSE && ldJ < m) return fail(FDB_ERR_INVALID, "ldJ < m");
+  // diagonal storage (kernels_diagonals.cuh): the stored diagonals of a square matrix with l, u in {0, 1}, packed
+  const int64_t diag_len = n > 0 ? (l + u + 1) * n - l - u : 0;
+  if (jkind == FDB_J_DIAGONALS) {
+    if (m != n) return fail(FDB_ERR_INVALID, "diagonal storage needs m == n (m=%lld n=%lld)", (long long)m, (long long)n);
+    if (l < 0 || l > 1 || u < 0 || u > 1)
+      return fail(FDB_ERR_INVALID, "diagonal storage needs l, u in {0, 1} (l=%lld u=%lld)", (long long)l, (long long)u);
+    if (ldJ < diag_len) return fail(FDB_ERR_INVALID, "ldJ=%lld < (l+u+1)*n - l - u = %lld", (long long)ldJ, (long long)diag_len);
+  }
   P->sp_kind = SP_BANDED;
   P->jkind = jkind;
   P->l = l;
   P->u = u;
   P->ldJ = ldJ;
-  P->j_len = jkind == FDB_J_BAND ? (l + u + 1) * n : ldJ * n;
+  P->j_len = jkind == FDB_J_BAND ? (l + u + 1) * n : (jkind == FDB_J_DIAGONALS ? diag_len : ldJ * n);
   TRY(setup_colors(P, colorvec));
   DevBuf<unsigned long long> d_cnt;
   TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
@@ -1086,8 +1096,8 @@ fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t
   for (auto c : cnt) total += c;
   P->E = (int64_t)total;
   TRY(finish_colored_plan(P, opts, cnt));
-  // SURVEY.md §8(d) banded: 8*sum_c band_len(c) written + 16*m*C read
-  P->alg_bytes = 8 * (int64_t)total + 16 * m * (int64_t)P->C;
+  // SURVEY.md §8(d) banded: 8*sum_c band_len(c) written + 16*m*C read (diagonal storage: every slot written once)
+  P->alg_bytes = (jkind == FDB_J_DIAGONALS ? 8 * diag_len : 8 * (int64_t)total) + 16 * m * (int64_t)P->C;
   return finish_plan(owner, plan);
 }
 
@@ -1525,10 +1535,12 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   // fill_matrix!(J, false)  jacobians.jl:530-532 — needed where the scatter does not define every slot itself
   const bool block_band = P->sp_kind == SP_BLOCKBAND;
   const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED && !block_band;
-  const bool band_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_BAND;
-  // (identity / band-data launches define every slot this rank is responsible for, including zeros for columns without
-  //  a valid colour; block-banded launches do so even when the rank has no colour).  With peer buffers set the caller
-  //  zero-fills J and synchronises the ranks BEFORE the call: a memset here would race with the peers' stores.
+  const bool diag_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_DIAGONALS;
+  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || diag_data);
+  // (identity / band-data / diagonal-storage launches define every slot this rank is responsible for, including zeros
+  //  for columns without a valid colour; block-banded launches do so even when the rank has no colour).  With peer
+  //  buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race with the
+  //  peers' stores.
   const bool self_defining = block_band || ((ident || band_data) && n_local > 0);
   if (!self_defining && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
@@ -1673,6 +1685,31 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
           (int64_t)resident_grid(P, diff_scatter_block_band<CT, MODE>, sm, tiles) * kBbGridOver, tiles));
       ScatterTimer tm(P, s);
       diff_scatter_block_band<CT, MODE><<<grid, kThreads, sm, s>>>(a);
+      P->cnt.kernel_launches += 1;
+      P->cnt.scatter_launches += 1;
+      return FDB_OK;
+    }
+    if (diag_data) {
+      // every slot of the columns of this group's colours, and (first group of rank 0) of the columns without a valid
+      // colour: storage order, closed-form diagonal and (row, column)
+      DiagArgs a{};
+      a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.local_of = P->local_of; a.J = J;
+      a.total = P->j_len; a.sub_end = P->l * (P->n - 1); a.main_end = a.sub_end + P->n; a.ldF = sF;
+      a.C = P->C; a.l0 = (int32_t)l0; a.G = (int32_t)G;
+      a.write_other = (g == 0 && P->rank == 0) ? 1 : 0;
+      if (a.total == 0) return FDB_OK;
+      const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
+      const int64_t tiles = (a.total + kDgTile - 1) / kDgTile;
+      ScatterTimer tm(P, s);
+      TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+        using CS = decltype(cs);
+        // a store stream: an oversubscribed grid, as for the other band kernels
+        constexpr int kDgGridOver = 16;
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(
+            (int64_t)resident_grid(P, diff_scatter_diagonals<CS, MODE>, sm, tiles) * kDgGridOver, tiles));
+        diff_scatter_diagonals<CS, MODE><<<grid, kThreads, sm, s>>>(a, cs);
+        return FDB_OK;
+      }));
       P->cnt.kernel_launches += 1;
       P->cnt.scatter_launches += 1;
       return FDB_OK;

@@ -58,11 +58,12 @@ struct fdb_group {
 };
 
 static bool plan_self_defining(const fdb_plan *P) {
-  // the scatter launches of all ranks together define every slot of J (identity CSC: nzval; band data: whole columns)
+  // the scatter launches of all ranks together define every slot of J (identity CSC: nzval; band data: whole columns;
+  // diagonal storage: every stored slot of every column)
   // (block-banded: every column, including those without a valid colour, whatever the colour count)
   if (P->sp_kind == SP_BLOCKBAND) return true;
   const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
-  const bool band_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_BAND;
+  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || P->jkind == FDB_J_DIAGONALS);
   return (ident || band_data) && P->C > 0;
 }
 

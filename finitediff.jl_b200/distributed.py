@@ -252,10 +252,14 @@ class GroupJacobian(_Group):
         n_dev = len(self.devices)
         devs = (C.c_int * n_dev)(*self.devices)
         h = C.c_void_p()
+        diag_route = api._diagonals_route(J, sparsity)
         cv_ptr, k0 = api._index_ptr(colorvec)
         self._keep = [k0]
         lib = L.lib()
-        if sparsity is None:
+        if diag_route is not None:
+            # Diagonal / Bidiagonal / SymTridiagonal sparsity: members write disjoint column sets of the packed diagonals
+            L.check(lib.fdb_group_create_banded(C.byref(h), n_dev, devs, *diag_route, cv_ptr, C.byref(o)))
+        elif sparsity is None:
             m, n, ld = api._dense_ld(J)
             L.check(lib.fdb_group_create_dense(C.byref(h), n_dev, devs, m, n, ld, C.byref(o)))
         elif isinstance(sparsity, api.SparseMatrixCSC):

@@ -15,6 +15,8 @@
 #     CuMatrix J  + CSC sparsity            ext/FiniteDiffSparseArraysExt.jl:20-28
 #     DeviceBanded J or CuMatrix J + Banded ext/FiniteDiffBandedMatricesExt.jl:13-27
 #     DeviceTridiagonal J (structured, COO) src/iteration_utils.jl:25-32 with ArrayInterface.findstructralnz
+#     DeviceDiagonal / DeviceBidiagonal J, or CuMatrix J + Diagonal / Bidiagonal / SymTridiagonal sparsity: the banded
+#                                           plan on the in-matrix band (l, u) of the type (packed diagonal storage)
 #     CuMatrix J + dense 0/1 prototype      src/jacobians.jl:473-488, 526-527
 #     CuMatrix J, sparsity === nothing      src/jacobians.jl:548-557, 590-598 (dense column branch, colorvec quirk included)
 #   for Val(:forward), Val(:central) and Val(:complex) (src/jacobians.jl:623-648), plus the JVP and the multi-GPU group,
@@ -30,6 +32,7 @@
 module FiniteDiffB200
 
 using FiniteDiff, SparseArrays, CUDA
+using LinearAlgebra: Diagonal, Bidiagonal, SymTridiagonal
 import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache,
     finite_difference_jacobian, finite_difference_jvp,
     finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache, finite_difference_derivative!,
@@ -38,7 +41,8 @@ import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, Jacobian
 const libfdjac = get(ENV, "FDJAC_B200_LIB", "libfdjac_b200.so")
 
 const FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = Cint(0), Cint(1), Cint(2), Cint(3)
-const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND = Cint(0), Cint(1), Cint(2), Cint(3), Cint(4)
+const FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND, FDB_J_DIAGONALS =
+    Cint(0), Cint(1), Cint(2), Cint(3), Cint(4), Cint(5)
 const FDB_STEP_DEFAULT = NaN            # relstep / absstep keyword not given (include/fdjac_b200.h)
 const FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = Cint(0), Cint(1), Cint(2)
 
@@ -138,6 +142,39 @@ struct DeviceTridiagonal                     # LinearAlgebra.Tridiagonal(dl, d, 
 end
 Base.size(J::DeviceTridiagonal) = (J.n, J.n)
 Base.size(J::DeviceTridiagonal, d) = J.n
+
+# LinearAlgebra.Diagonal(d) / Bidiagonal(dv, ev, uplo) with the values on the device, in the packed diagonal storage of
+# FDB_J_DIAGONALS (stored diagonals in ascending row-minus-column order): [d], [dv; ev] for :U, [ev; dv] for :L.  The
+# LinearAlgebra types take views of the one buffer: Diagonal(view(buf, 1:n)), Bidiagonal(view(buf, 1:n),
+# view(buf, n+1:2n-1), :U) or Bidiagonal(view(buf, n:2n-1), view(buf, 1:n-1), :L).
+struct DeviceDiagonal
+    n::Int
+    buf::CuVector{Float64}                   # n
+end
+struct DeviceBidiagonal
+    n::Int
+    uplo::Symbol                             # :U or :L
+    buf::CuVector{Float64}                   # 2n - 1
+end
+Base.size(J::Union{DeviceDiagonal, DeviceBidiagonal}) = (J.n, J.n)
+Base.size(J::Union{DeviceDiagonal, DeviceBidiagonal}, d) = J.n
+
+# the in-matrix band (l, u) that is the entry set of each type (ArrayInterface.findstructralnz)
+bands(::Union{DeviceDiagonal, Diagonal}) = (0, 0)
+bands(J::Union{DeviceBidiagonal, Bidiagonal}) = (J.uplo == :U || J.uplo == 'U') ? (0, 1) : (1, 0)
+bands(::SymTridiagonal) = (1, 1)
+
+# ArrayInterface.matrix_colors closed forms: all 1 (Diagonal), cycle 1:2 (Bidiagonal), cycle 1:3 (SymTridiagonal)
+function matrix_colors(J::Union{DeviceDiagonal, DeviceBidiagonal, Diagonal, Bidiagonal, SymTridiagonal})
+    n = size(J, 2)
+    l, u = bands(J)
+    out = CuVector{Int64}(undef, max(n, 1))
+    GC.@preserve out begin
+        check(ccall((:fdb_matrix_colors_banded, libfdjac), Cint, (Int64, Int64, Int64, CuPtr{Int64}, Ptr{Cvoid}),
+            n, l, u, pointer(out), CUDA.stream().handle))
+    end
+    out[1:n]
+end
 
 # ArrayInterface.findstructralnz(::Tridiagonal): band by band (order is irrelevant to the result); slots into [dl; d; du]
 function tridiagonal_structure(n::Int)
@@ -367,7 +404,8 @@ function run_plan!(plan::Plan, jvals::CuArray{Float64}, f, x::CuVector{Float64},
     nothing                                  # jacobians.jl:652
 end
 
-const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceTridiagonal, CuMatrix{Float64}}
+const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceTridiagonal, DeviceDiagonal, DeviceBidiagonal,
+    CuMatrix{Float64}}
 
 ld(J::CuMatrix) = max(stride(J, 2), size(J, 1), 1)
 
@@ -390,6 +428,13 @@ end
 function plan_for(J::DeviceTridiagonal, sp, colorvec, fd)
     (plan_coo(() -> tridiagonal_structure(J.n), J.buf, J.n, J.n, :tridiagonal, FDB_J_SLOTS, 3 * J.n - 2, colorvec, fd), J.buf)
 end
+# Diagonal / Bidiagonal J: the banded plan into the packed diagonal storage; the sparsity is the same type or J itself
+function plan_for(J::Union{DeviceDiagonal, DeviceBidiagonal}, sp, colorvec, fd)
+    (typeof(sp) == typeof(J) && size(sp) == size(J) && bands(sp) == bands(J)) ||
+        throw(ArgumentError("a $(typeof(J)) Jacobian needs a sparsity of the same type, size and bands"))
+    l, u = bands(J)
+    (plan_banded(J.buf, J.n, J.n, l, u, FDB_J_DIAGONALS, length(J.buf), colorvec, fd), J.buf)
+end
 function plan_for(J::CuMatrix{Float64}, sp, colorvec, fd)
     m, n = size(J)
     if sp === nothing                                                   # jacobians.jl:548-557
@@ -404,6 +449,11 @@ function plan_for(J::CuMatrix{Float64}, sp, colorvec, fd)
                 rows, cols, _ = tridiagonal_structure(sp.n)
                 (rows, cols, nothing)
             end, J)
+    elseif sp isa Union{Diagonal, Bidiagonal, SymTridiagonal, DeviceDiagonal, DeviceBidiagonal}
+        # the type's structure only (its band), not its values; LinearAlgebra.Tridiagonal keeps the prototype method below
+        (m, n) == size(sp) || throw(DimensionMismatch("size(J) != size(sparsity)"))
+        l, u = bands(sp)
+        return (plan_banded(J, m, n, l, u, FDB_J_DENSE, ld(J), colorvec, fd), J)
     elseif sp isa AbstractMatrix                                        # dense 0/1 prototype, jacobians.jl:526-527
         # keyed on the prototype's identity: editing it in place needs a new array (as for every cached pattern)
         return (plan_coo(J, m, n, (:prototype, objectid(sp)), FDB_J_DENSE, ld(J), colorvec, fd) do
@@ -419,7 +469,8 @@ end
                                 relstep, absstep, colorvec, sparsity, dir)
 
 Same signature and keyword meaning as `src/jacobians.jl:504-514`.  `J` is a `DeviceCSC`, `DeviceBanded`,
-`DeviceBlockBanded`, `DeviceTridiagonal` or a dense `CuMatrix{Float64}`; `x`, `cache.fx`, `f_in` are `CuVector{Float64}`.
+`DeviceBlockBanded`, `DeviceTridiagonal`, `DeviceDiagonal`, `DeviceBidiagonal` or a dense `CuMatrix{Float64}`; `x`,
+`cache.fx`, `f_in` are `CuVector{Float64}`.
 `relstep` / `absstep` left at their defaults are passed as FDB_STEP_DEFAULT; explicit values (0 included) as given.
 """
 function finite_difference_jacobian!(J::DeviceJ, f, x::CuVector{Float64},
@@ -677,6 +728,20 @@ function group_banded(J::DeviceBanded, colorvec, fdtype, devices::Vector{Cint}; 
         check(ccall((:fdb_group_create_banded, libfdjac), Cint,
             (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Int64, Int64, Cint, Int64, Ptr{Int64}, Ref{PlanOpts}),
             h, length(devices), pointer(devices), J.m, J.n, J.l, J.u, FDB_J_BAND, 0, cptr, opts))
+    end
+    Group(h[], length(devices), croot)
+end
+
+# Diagonal / Bidiagonal J: members write disjoint column sets of the packed diagonals, with no zero fill
+function group_banded(J::Union{DeviceDiagonal, DeviceBidiagonal}, colorvec, fdtype, devices::Vector{Cint}; kw...)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, J.n)
+    l, u = bands(J)
+    GC.@preserve croot devices begin
+        check(ccall((:fdb_group_create_banded, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Int64, Int64, Cint, Int64, Ptr{Int64}, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), J.n, J.n, l, u, FDB_J_DIAGONALS, length(J.buf), cptr, opts))
     end
     Group(h[], length(devices), croot)
 end

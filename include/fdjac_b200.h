@@ -58,7 +58,8 @@ typedef enum {
   FDB_J_DENSE = 1,     /* J::Matrix column-major, leading dimension ldJ              (ext/..SparseArraysExt.jl:20-28, iteration_utils.jl:25-32) */
   FDB_J_BAND = 2,      /* J::BandedMatrix data[(l+u+1) x n], slot [u+r-c+1, c]        (ext/FiniteDiffBandedMatricesExt.jl:13-27) */
   FDB_J_SLOTS = 3,     /* structured J (e.g. Tridiagonal): explicit 1-based slot per structural entry (iteration_utils.jl:25-32) */
-  FDB_J_BLOCK_BAND = 4 /* J::BandedBlockBandedMatrix band data, (l+u+1)(lam+mu+1) slots per column (fdb_plan_create_block_banded) */
+  FDB_J_BLOCK_BAND = 4, /* J::BandedBlockBandedMatrix band data, (l+u+1)(lam+mu+1) slots per column (fdb_plan_create_block_banded) */
+  FDB_J_DIAGONALS = 5  /* J::Diagonal / Bidiagonal / Tridiagonal storage: the stored diagonals packed in one buffer (fdb_plan_create_banded) */
 } fdb_jkind;
 
 /*
@@ -168,7 +169,21 @@ fdb_status fdb_plan_create_coo(fdb_plan **plan, int64_t m, int64_t n, int64_t nn
                                const int64_t *colorvec, const fdb_plan_opts *opts);
 
 /* sparsity::BandedMatrix with bandwidths (l,u): ext/FiniteDiffBandedMatricesExt.jl:13-27 (writes the WHOLE band).
- *   jkind = FDB_J_BAND (J is the (l+u+1) x n band data) or FDB_J_DENSE (ldJ). */
+ *   jkind = FDB_J_BAND (J is the (l+u+1) x n band data) or FDB_J_DENSE (ldJ).
+ *   jkind = FDB_J_DIAGONALS: LinearAlgebra's Diagonal (l, u) = (0, 0), Bidiagonal :U (0, 1) / :L (1, 0) and Tridiagonal
+ *           (1, 1) storage, whose entry set is the in-matrix band (l, u).  Needs m == n and l, u in {0, 1}.  J is one
+ *           packed buffer holding the stored diagonals in ascending row-minus-column order: the sub-diagonal (r = c+1,
+ *           n-1 values, when l = 1), the main diagonal (n values), the super-diagonal (c = r+1, n-1 values, when u = 1);
+ *           entry t of each diagonal is its t-th element from the top left.  So the buffer is [dl; d; du] for
+ *           Tridiagonal, [dv; ev] for Bidiagonal :U, [ev; dv] for :L and [d] for Diagonal.  ldJ is the buffer's length in
+ *           doubles, at least (l+u+1)*n - l - u (0 for n = 0); slots beyond that are not touched.  Every call writes every
+ *           slot exactly once — the quotient for columns with a valid colour, +0.0 for the others — so J is never
+ *           zero-filled; a rank plan writes the slots of its own colours' columns (rank 0 also those without a valid
+ *           colour), and a rank without colours, or a plan with no colour at all, zero-fills J like FDB_J_BAND.  The column
+ *           colours come from the table, or from the closed form when colorvec[j] == j mod C + 1 (matrix_colors).
+ *           Any other (m, n, l, u, ldJ): FDB_ERR_INVALID.  fdb_plan_info: jkind FDB_J_DIAGONALS, j_len = that length,
+ *           n_entries = the structural entries of columns with a valid colour (j_len when every column has one),
+ *           alg_bytes_scatter = 8*j_len + 16*n*C. */
 fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, int jkind, int64_t ldJ,
                                   const int64_t *colorvec, const fdb_plan_opts *opts);
 
@@ -285,6 +300,8 @@ typedef struct fdb_group fdb_group;
 fdb_status fdb_group_create_csc(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
                                 const int64_t *colptr, const int64_t *rowval, int jkind, const int64_t *j_colptr,
                                 const int64_t *j_rowval, int64_t ldJ, const int64_t *colorvec, const fdb_plan_opts *opts);
+/* banded groups: with FDB_J_BAND or FDB_J_DIAGONALS member i writes every slot of the columns of its own colours straight
+ * into the root's buffer, member 0 also the columns without a valid colour; J is zero-filled only when there is no colour. */
 fdb_status fdb_group_create_banded(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t l,
                                    int64_t u, int jkind, int64_t ldJ, const int64_t *colorvec, const fdb_plan_opts *opts);
 fdb_status fdb_group_create_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t ldJ,
