@@ -253,7 +253,10 @@ fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const do
   if (g->oop) return fail(FDB_ERR_INVALID, "this is an out-of-place group: call fdb_group_jacobian_oop");
   fdb_plan *P0 = g->plans[0];
   if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
-  if ((P0->n > 0 && !d_x) || !d_J) return fail(FDB_ERR_INVALID, "NULL x or J");
+  // J may be NULL only when no member has a slot to write (as fdb_jacobian allows; e.g. an empty gradient, n = 0)
+  bool writes_J = false;
+  for (const fdb_plan *P : g->plans) writes_J = writes_J || P->j_len > 0;
+  if ((P0->n > 0 && !d_x) || (writes_J && !d_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   const int root = g->devices[0];
   cudaStream_t s0 = (cudaStream_t)stream;
   {

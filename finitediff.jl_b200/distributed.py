@@ -353,6 +353,100 @@ class GroupHessian(_Group):
         self._check(st, wrapped)
 
 
+def dense_column_blocks(n: int, world: int) -> List[tuple]:
+    """[(col_begin, col_end)] of every member of a dense group (csrc/fdjac_abi.cu create_dense): member r owns the
+    contiguous columns [min(n, r*p), min(n, (r+1)*p)) with p = ceil(n / world).  Every column costs the same f calls, so
+    the largest block, ceil(n / world) columns, is as small as any split makes it; trailing members may be empty."""
+    if n < 0 or world < 1:
+        raise ValueError("n must be >= 0 and world >= 1")
+    p = -(-n // world)
+    return [(min(n, r * p), min(n, (r + 1) * p)) for r in range(world)]
+
+
+class GroupGradient(_Group):
+    """finite_difference_gradient!(df, f, x, cache) for a vector x on several GPUs from ONE process: the dense group with
+    m = 1 and ldJ = 1 (fdb_group_create_dense / fdb_group_jacobian), df as J.  Member i owns the contiguous components
+    plans[i].dense_range() (dense_column_blocks) and writes exactly those entries of the root's df; devices[0] is the
+    root and owns x and df.  df is bit-identical to finite_difference_gradient_ on one device.  Device ordinals may repeat
+    ([0, 0] runs two members on one GPU).
+
+    fdtype: "forward" or "central" ("complex" builds, and its run raises FdbError(FDB_ERR_UNSUPPORTED) before any f
+    call).  plan_kw: max_batch, scratch_bytes, use_graph (per member)."""
+
+    def __init__(self, n, devices, fdtype="central", **plan_kw):
+        if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 0:
+            raise ValueError("n must be a non-negative integer")
+        if len(devices) < 1:
+            raise ValueError("a group needs at least one device")
+        self.n = int(n)
+        self.fdtype = fdtype.lstrip(":") if isinstance(fdtype, str) else fdtype
+        self._code = api._fdtype_code(self.fdtype)
+        self._set_devices(devices)
+        o = api._opts(self._code, self.devices[0], **plan_kw)
+        devs = (C.c_int * len(self.devices))(*self.devices)
+        h = C.c_void_p()
+        L.check(L.lib().fdb_group_create_dense(C.byref(h), len(self.devices), devs, 1, self.n, 1, C.byref(o)))
+        self._adopt(h)
+        self.columns = dense_column_blocks(self.n, len(self.devices))      # member i: plans[i].dense_range()
+        self._fx_slot = None        # the root's one device slot for f(x) in forward mode (a stable pointer for graphs)
+
+    def run(self, fs, x, df, fx=None, *, relstep=None, absstep=None, dir=True, stream=None):
+        """fs: one f per member — a NativeFn (batched fdb_fn with m = 1, context on that member's device) or a Python
+        f(x) -> scalar on that member's device (f.batched = True: (batch, n) in, (batch,) out).  x and df: float64 CUDA
+        vectors of length n on devices[0]; x is never modified.  Forward mode: f(x) is evaluated once, by fs[0] at the
+        root, unless fx (a number, or a 1-element float64 CUDA tensor on devices[0]) is given (gradients.jl:409-410); it
+        is passed to every member as f_in, so a call makes 1 + n evaluations (n with fx).  fx is not read otherwise."""
+        if len(fs) != len(self.devices):
+            raise ValueError("one f per member")
+        xv = api._scalar_x(x)
+        dv = api._scalar_x(df, "df")
+        if xv.numel() != self.n or xv.device != self.root:
+            raise ValueError(f"x must hold {self.n} values on {self.root}")
+        if dv.numel() != self.n or dv.device != self.root:
+            raise ValueError(f"df must hold {self.n} values on {self.root}")
+        if df.reshape(-1).data_ptr() != dv.data_ptr():
+            raise ValueError("df must be contiguous")
+        if isinstance(fx, torch.Tensor):
+            if not api._is_cuda(fx) or fx.dtype != torch.float64 or fx.numel() != 1 or fx.device != self.root:
+                raise TypeError(f"fx must be a number or a 1-element float64 CUDA tensor on {self.root}")
+        elif fx is not None and not api._is_number(fx):
+            raise TypeError("fx must be a number or a 1-element float64 CUDA tensor")
+        addr, ctxs, wrapped = self._member_fns(fs, 1, self.n, scalar=True)
+        if stream is None:
+            stream = torch.cuda.current_stream(self.root).cuda_stream
+        with torch.cuda.device(self.root):
+            fin = None
+            if self._code == L.FDB_FORWARD:
+                fin = fx if isinstance(fx, torch.Tensor) else self._root_slot()
+                if fx is None:
+                    self._root_fx(fs, wrapped, xv, fin, stream)
+                elif not isinstance(fx, torch.Tensor):
+                    with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=self.root)):
+                        fin.fill_(float(fx))
+            st = L.lib().fdb_group_jacobian(self._h, addr, ctxs, xv.data_ptr() or None, dv.data_ptr() or None, None,
+                                            None if fin is None else fin.data_ptr(),
+                                            L.STEP_DEFAULT if relstep is None else float(relstep),
+                                            L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
+                                            C.c_void_p(stream))
+        self._check(st, wrapped)
+
+    def _root_slot(self):
+        if self._fx_slot is None:
+            self._fx_slot = torch.empty(1, dtype=torch.float64, device=self.root)
+        return self._fx_slot
+
+    @staticmethod
+    def _root_fx(fs, wrapped, xv, fin, stream):
+        """f(x) by member 0's f, into fin on the root's stream (fx0 = f(x), gradients.jl:410)"""
+        py = wrapped[0][2]
+        if py is None:
+            api._native_call(fs[0], fin, xv, stream)
+            return
+        if py._tramp(None, fin.data_ptr(), xv.data_ptr() or None, 1, 1, max(xv.numel(), 1), stream) != 0:
+            exc, py.exc = py.exc, None
+            raise exc
+
+
 class GroupJacobianOOP(_Group):
     """The out-of-place finite_difference_jacobian(f, x, cache, f_in; ...) on several GPUs from ONE process
     (fdb_group_create_oop_* / fdb_group_jacobian_oop): the colours (dense branch: column blocks of the maximum(colorvec)

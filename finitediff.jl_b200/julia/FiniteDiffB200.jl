@@ -829,6 +829,65 @@ function group_hessian!(g::Group, H::CuMatrix{Float64}, fs::Vector, x::CuVector{
     H
 end
 
+# ---- finite_difference_gradient! on several GPUs from ONE call: the dense group with m = 1 (df is J, 1 x n, ldJ = 1).
+#      Member i owns a contiguous block of the n components (every component costs the same f calls) and writes its
+#      entries of df straight into the root's df; devices[1] is the root and owns x and df.  Bit-identical to one device.
+#      kw: max_batch, scratch_bytes, use_graph.  :complex groups are refused by fdb_group_jacobian (FDB_ERR_UNSUPPORTED).
+mutable struct GradientGroup
+    group::Group
+    n::Int
+    fdtype::Any
+end
+
+function group_gradient(n::Integer, devices::Vector{Cint}; fdtype = Val(:central), kw...)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    GC.@preserve devices begin
+        check(ccall((:fdb_group_create_dense, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), 1, n, 1, opts))
+    end
+    GradientGroup(Group(h[], length(devices), nothing), n, fdtype)
+end
+
+# fs[i]: the scalar f(x) member i calls (its arrays live on devices[i]); df and x live on devices[1].  Forward mode: f(x)
+# is evaluated once, by fs[1] at the root, unless fx (a Number or a 1-element CuVector, gradients.jl:409-410) is given,
+# and passed to every member as f_in, so a call makes 1 + n evaluations (n with fx), as the reference does.
+function group_gradient!(g::GradientGroup, df::CuVector{Float64}, fs::Vector, x::CuVector{Float64};
+        fx = nothing, relstep = nothing, absstep = relstep, dir = true)
+    length(x) == g.n || throw(DimensionMismatch("length(x) = $(length(x)), the group was built for $(g.n)"))
+    length(df) == g.n || throw(DimensionMismatch("length(df) != length(x)"))
+    length(fs) == g.group.n || throw(ArgumentError("one f per member"))
+    f_in = nothing
+    if fdcode(g.fdtype) == FDB_FORWARD
+        if fx isa CuVector{Float64}
+            length(fx) == 1 || throw(DimensionMismatch("fx must hold one value"))
+            f_in = fx
+        elseif fx !== nothing
+            f_in = CuArray(Float64[fx])
+        else
+            f_in = CuVector{Float64}(undef, 1)
+            scalar_f(fs[1])(f_in, x)
+        end
+    end
+    states = [FnState(scalar_f(f), 1, g.n, nothing) for f in fs]
+    ctxs = Ptr{Cvoid}[pointer_from_objref(s) for s in states]
+    cf = @cfunction(f_trampoline, Cint, (Ptr{Cvoid}, CuPtr{Float64}, CuPtr{Float64}, Int64, Int64, Int64, Ptr{Cvoid}))
+    rc = Cint(0)
+    GC.@preserve states ctxs x df f_in begin
+        rc = ccall((:fdb_group_jacobian, libfdjac), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Ptr{Cvoid}}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64}, CuPtr{Float64},
+                Float64, Float64, Float64, Ptr{Cvoid}),
+            g.group.handle, cf, pointer(ctxs), pointer(x), pointer(df), CU_NULL,
+            f_in === nothing ? CU_NULL : pointer(f_in), stepval(relstep), stepval(absstep), Float64(dir), CUDA.stream().handle)
+    end
+    for s in states
+        s.err === nothing || throw(s.err)
+    end
+    check(rc)
+    df
+end
+
 # ---- column-block shards (few-colour problems on several GPUs): one process per GPU, each owning the columns c0+1:c1.
 # `sub` is the block's pattern (colptr slice rebased to 1, rows rebased to the block's first row), `f_rows!` computes
 # that row range from the x slice the rows depend on, `eps` holds the step sizes of the FULL x (color_eps! below).

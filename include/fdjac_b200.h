@@ -304,6 +304,10 @@ fdb_status fdb_group_create_csc(fdb_group **group, int n_devices, const int *dev
  * into the root's buffer, member 0 also the columns without a valid colour; J is zero-filled only when there is no colour. */
 fdb_status fdb_group_create_banded(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t l,
                                    int64_t u, int jkind, int64_t ldJ, const int64_t *colorvec, const fdb_plan_opts *opts);
+/* dense groups: member i owns the contiguous columns [min(n, i*p), min(n, (i+1)*p)), p = ceil(n / n_devices)
+ * (fdb_plan_dense_range of its plan); a member left with no column calls f only for f(x) in forward mode without d_f_in,
+ * and writes nothing.  With m = 1 and ldJ = 1 this is the gradient of a scalar f (finite_difference_gradient!, df as J):
+ * pass f(x), evaluated once at the root, as d_f_in in forward mode, and a call makes 1 + n evaluations as on one device. */
 fdb_status fdb_group_create_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t ldJ,
                                   const fdb_plan_opts *opts);
 /* block-banded groups: member i writes every slot of the columns of its own colours straight into the root's band data,
@@ -315,7 +319,8 @@ fdb_status fdb_group_destroy(fdb_group *group);
 fdb_status fdb_group_size(const fdb_group *group, int *n_members);
 /* member i's plan (owned by the group): fdb_plan_info / fdb_plan_counters / fdb_plan_get_eps / fdb_plan_color_owner */
 fdb_status fdb_group_plan(const fdb_group *group, int member, fdb_plan **plan);
-/* arguments as fdb_jacobian; d_x, d_J, d_fx, d_f_in live on devices[0], `stream` is a stream of devices[0] */
+/* arguments as fdb_jacobian; d_x, d_J, d_fx, d_f_in live on devices[0], `stream` is a stream of devices[0].  As for
+ * fdb_jacobian, d_J may be NULL when no member has a slot of J to write (n = 0). */
 fdb_status fdb_group_jacobian(fdb_group *group, fdb_fn f, void *const *ctx, const double *d_x, double *d_J, double *d_fx,
                               const double *d_f_in, double relstep, double absstep, double dir, void *stream);
 
