@@ -657,31 +657,78 @@ def _dense_ld(J: torch.Tensor):
     return m, n, max(int(ld), m, 1)
 
 
-def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> Plan:
-    """Create the fdb_plan for (typeof(J), sparsity, colorvec, fdtype) — the dispatch the reference performs with
-    _use_findstructralnz / _use_sparseCSC_common_sparsity / typeof(J) (jacobians.jl:522-535)."""
-    diag_route = _diagonals_route(J, sparsity)     # first: a refused target raises before anything is built
-    lib = L.lib()
-    fd = _fdtype_code(fdtype)
-    o = _opts(fd, _device_index(device), **plan_kw)
+def _new_handle(creator: str, *args):
+    """The handle fdb_<creator>(&h, *args) creates."""
     h = C.c_void_p()
+    L.check(getattr(L.lib(), creator)(C.byref(h), *args))
+    return h
+
+
+def _cached_plan(cache, key, create) -> Plan:
+    """cache._plans[key], created by create() on first use."""
+    p = cache._plans.get(key)
+    if p is None:
+        p = cache._plans[key] = create()
+    return p
+
+
+def _stream(stream, device) -> int:
+    """The call's stream: the one given, else the current stream of `device`."""
+    return torch.cuda.current_stream(device).cuda_stream if stream is None else stream
+
+
+def _steps(relstep, absstep):
+    return (L.STEP_DEFAULT if relstep is None else float(relstep), L.STEP_DEFAULT if absstep is None else float(absstep))
+
+
+def _call(device, pyfns, fn, *args):
+    """fn(*args) on `device`.  When a Python f failed (FDB_ERR_CALLBACK), the first exception pending on the call's
+    wrappers `pyfns` propagates as itself, as Julia propagates it; any other failure raises FdbError."""
+    with torch.cuda.device(device):
+        st = fn(*args)
+    if st == L.FDB_ERR_CALLBACK:
+        for w in pyfns:
+            if w is not None and w.exc is not None:
+                exc, w.exc = w.exc, None
+                raise exc
+    L.check(st)
+
+
+def _device_slot(owner, attr: str, device, stream, value=None) -> torch.Tensor:
+    """owner.<attr>: a one-element float64 tensor on `device` that keeps its pointer from call to call (the arguments of
+    a call, and a captured graph's key under use_graph, stay the same), with `value` written on `stream` when given."""
+    slot = getattr(owner, attr, None)
+    if slot is None or slot.device != device:
+        slot = torch.empty(1, dtype=torch.float64, device=device)
+        setattr(owner, attr, slot)
+    if value is not None:
+        with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=device)):
+            slot.fill_(float(value))
+    return slot
+
+
+def _plan_route(J, sparsity, colorvec):
+    """(kind, args, keep) for (typeof(J), sparsity, colorvec) — the dispatch the reference performs with
+    _use_findstructralnz / _use_sparseCSC_common_sparsity / typeof(J) (jacobians.jl:522-535): the plan is made by
+    fdb_plan_create_<kind>(&h, *args, &opts) (or fdb_group_create_<kind>(&h, n_devices, devices, *args, &opts)), and
+    `keep` holds the host arrays the pointers in args point into."""
+    diag_route = _diagonals_route(J, sparsity)     # first: a refused target raises before anything is built
     cv_ptr, cv_keep = _index_ptr(colorvec)
     keep = [cv_keep]
     if diag_route is not None:
         # Diagonal / Bidiagonal / SymTridiagonal sparsity: the banded plan with the band (l, u) of the type, into the packed
         # diagonal storage of the same type or into a dense J
-        L.check(lib.fdb_plan_create_banded(C.byref(h), *diag_route, cv_ptr, C.byref(o)))
-    elif sparsity is None:
+        return "banded", (*diag_route, cv_ptr), keep
+    if sparsity is None:
         # dense column branch (jacobians.jl:548-557): column i of J from perturbing component i, colorvec = 1:n.
         # With sparsity === nothing and any OTHER colorvec the reference loops color_i in 1:maximum(colorvec) and
         # perturbs COMPONENT color_i (the colour id used as an index), writing only those leading columns of J (J is
         # not zero-filled on this branch) — reproduced as written by fdb_plan_create_dense_colorvec.
         m, n, ld = _dense_ld(J)
         if colorvec is not None and not _is_identity_colorvec(colorvec, n):
-            L.check(lib.fdb_plan_create_dense_colorvec(C.byref(h), m, n, ld, cv_ptr, C.byref(o)))
-        else:
-            L.check(lib.fdb_plan_create_dense(C.byref(h), m, n, ld, C.byref(o)))
-    elif isinstance(sparsity, SparseMatrixCSC):
+            return "dense_colorvec", (m, n, ld, cv_ptr), keep
+        return "dense", (m, n, ld), keep
+    if isinstance(sparsity, SparseMatrixCSC):
         cp, k1 = _index_ptr(sparsity.colptr)
         rv, k2 = _index_ptr(sparsity.rowval)
         keep += [k1, k2]
@@ -692,73 +739,69 @@ def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> P
                 jcp, k3 = _index_ptr(J.colptr)
                 jrv, k4 = _index_ptr(J.rowval)
                 keep += [k3, k4]
-            L.check(lib.fdb_plan_create_csc(C.byref(h), sparsity.m, sparsity.n, cp, rv, L.FDB_J_CSC_NZVAL, jcp, jrv, 0,
-                                            cv_ptr, C.byref(o)))
-        elif isinstance(J, torch.Tensor):
+            return "csc", (sparsity.m, sparsity.n, cp, rv, L.FDB_J_CSC_NZVAL, jcp, jrv, 0, cv_ptr), keep
+        if isinstance(J, torch.Tensor):
             m, n, ld = _dense_ld(J)
             if (m, n) != (sparsity.m, sparsity.n):
                 raise ValueError("size(J) != size(sparsity)")
-            L.check(lib.fdb_plan_create_csc(C.byref(h), m, n, cp, rv, L.FDB_J_DENSE, None, None, ld, cv_ptr, C.byref(o)))
-        else:
-            raise TypeError(f"unsupported J type {type(J)} for a SparseMatrixCSC sparsity")
-    elif isinstance(sparsity, BandedMatrix):
+            return "csc", (m, n, cp, rv, L.FDB_J_DENSE, None, None, ld, cv_ptr), keep
+        raise TypeError(f"unsupported J type {type(J)} for a SparseMatrixCSC sparsity")
+    if isinstance(sparsity, BandedMatrix):
         if isinstance(J, BandedMatrix):
             if (J.l, J.u) != (sparsity.l, sparsity.u):
                 raise ValueError("J and sparsity must have the same bandwidths")
-            L.check(lib.fdb_plan_create_banded(C.byref(h), sparsity.m, sparsity.n, sparsity.l, sparsity.u, L.FDB_J_BAND,
-                                               0, cv_ptr, C.byref(o)))
-        elif isinstance(J, torch.Tensor):
+            return "banded", (sparsity.m, sparsity.n, sparsity.l, sparsity.u, L.FDB_J_BAND, 0, cv_ptr), keep
+        if isinstance(J, torch.Tensor):
             m, n, ld = _dense_ld(J)
-            L.check(lib.fdb_plan_create_banded(C.byref(h), m, n, sparsity.l, sparsity.u, L.FDB_J_DENSE, ld, cv_ptr,
-                                               C.byref(o)))
-        else:
-            raise TypeError(f"unsupported J type {type(J)} for a BandedMatrix sparsity")
-    elif isinstance(sparsity, (Tridiagonal, SymTridiagonal)):
+            return "banded", (m, n, sparsity.l, sparsity.u, L.FDB_J_DENSE, ld, cv_ptr), keep
+        raise TypeError(f"unsupported J type {type(J)} for a BandedMatrix sparsity")
+    if isinstance(sparsity, BandedBlockBandedMatrix) and (bb := _block_banded_plan_args(J, sparsity)) is not None:
+        # J and sparsity are one square block-banded structure: the closed-form plan, no entry lists on the host
+        blocks, l, u, lam, mu, ldata = bb
+        return "block_banded", (len(blocks), blocks.ctypes.data if len(blocks) else None, l, u, lam, mu, ldata,
+                                cv_ptr), keep + [blocks]
+    if isinstance(sparsity, (Tridiagonal, SymTridiagonal)):
         rows, cols, slots = sparsity.findstructralnz()
         n = sparsity.n
         if isinstance(J, Tridiagonal):
-            L.check(lib.fdb_plan_create_coo(C.byref(h), n, n, len(rows), rows.ctypes.data, cols.ctypes.data,
-                                            L.FDB_J_SLOTS, slots.ctypes.data, 3 * n - 2, cv_ptr, C.byref(o)))
+            jargs = (n, n, L.FDB_J_SLOTS, slots.ctypes.data, 3 * n - 2)
         elif isinstance(J, torch.Tensor):
             m, nn, ld = _dense_ld(J)
-            L.check(lib.fdb_plan_create_coo(C.byref(h), m, nn, len(rows), rows.ctypes.data, cols.ctypes.data,
-                                            L.FDB_J_DENSE, None, ld, cv_ptr, C.byref(o)))
+            jargs = (m, nn, L.FDB_J_DENSE, None, ld)
         else:
             raise TypeError(f"unsupported J type {type(J)} for a Tridiagonal sparsity")
-        keep += [rows, cols, slots]
-    elif isinstance(sparsity, BandedBlockBandedMatrix) and _block_banded_plan_args(J, sparsity) is not None:
-        # J and sparsity are one square block-banded structure: the closed-form plan, no entry lists on the host
-        blocks, l, u, lam, mu, ldata = _block_banded_plan_args(J, sparsity)
-        L.check(lib.fdb_plan_create_block_banded(C.byref(h), len(blocks), blocks.ctypes.data if len(blocks) else None,
-                                                 l, u, lam, mu, ldata, cv_ptr, C.byref(o)))
-        keep += [blocks]
     elif isinstance(sparsity, BandedBlockBandedMatrix):
         # ext/FiniteDiffBlockBandedMatricesExt.jl:16-42: the hook's (block-row, sub-band) entry set, written by slot
         rows, cols, slots = sparsity.findstructralnz()
         if isinstance(J, BandedBlockBandedMatrix):
             if (J.rb, J.cb, J.l, J.u, J.lam, J.mu) != (sparsity.rb, sparsity.cb, sparsity.l, sparsity.u, sparsity.lam, sparsity.mu):
                 raise ValueError("J and sparsity must have the same block structure")
-            L.check(lib.fdb_plan_create_coo(C.byref(h), sparsity.m, sparsity.n, len(rows), rows.ctypes.data, cols.ctypes.data,
-                                            L.FDB_J_SLOTS, slots.ctypes.data, sparsity.w * sparsity.n, cv_ptr, C.byref(o)))
+            jargs = (sparsity.m, sparsity.n, L.FDB_J_SLOTS, slots.ctypes.data, sparsity.w * sparsity.n)
         elif isinstance(J, torch.Tensor):
             m, nn, ld = _dense_ld(J)
-            L.check(lib.fdb_plan_create_coo(C.byref(h), m, nn, len(rows), rows.ctypes.data, cols.ctypes.data,
-                                            L.FDB_J_DENSE, None, ld, cv_ptr, C.byref(o)))
+            jargs = (m, nn, L.FDB_J_DENSE, None, ld)
         else:
             raise TypeError(f"unsupported J type {type(J)} for a BandedBlockBandedMatrix sparsity")
-        keep += [rows, cols, slots]
     elif isinstance(sparsity, (torch.Tensor, np.ndarray, list)):
         # dense 0/1 prototype: rows/cols from _findstructralnz (jacobians.jl:526-527), J must be dense
         rows, cols = _findstructralnz_dense(sparsity)
+        slots = None
         if not isinstance(J, torch.Tensor):
             raise TypeError("a dense prototype sparsity needs a dense J")
         m, n, ld = _dense_ld(J)
-        L.check(lib.fdb_plan_create_coo(C.byref(h), m, n, len(rows), rows.ctypes.data, cols.ctypes.data, L.FDB_J_DENSE,
-                                        None, ld, cv_ptr, C.byref(o)))
-        keep += [rows, cols]
+        jargs = (m, n, L.FDB_J_DENSE, None, ld)
     else:
         raise TypeError(f"unsupported sparsity type {type(sparsity)}")
-    return Plan(h.value, tuple(keep))
+    m, n, jkind, slot_ptr, ld = jargs          # the entry lists (rows, cols) go into J's slots or into a dense J
+    return "coo", (m, n, len(rows), rows.ctypes.data, cols.ctypes.data, jkind, slot_ptr, ld, cv_ptr), \
+        keep + [rows, cols, slots]
+
+
+def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> Plan:
+    """Create the fdb_plan for (typeof(J), sparsity, colorvec, fdtype) by the creator _plan_route chooses."""
+    kind, args, keep = _plan_route(J, sparsity, colorvec)
+    o = _opts(_fdtype_code(fdtype), _device_index(device), **plan_kw)
+    return Plan(_new_handle(f"fdb_plan_create_{kind}", *args, C.byref(o)).value, tuple(keep))
 
 
 def _block_banded_plan_args(J, sparsity):
@@ -918,12 +961,20 @@ class JacobianCache:
     def plan_for(self, J, sparsity, colorvec, x_len) -> Plan:
         default_cv = isinstance(colorvec, range) and colorvec == range(1, x_len + 1)
         key = (_j_key(J), _sp_key(sparsity), None if default_cv else _index_key(colorvec), self.fdtype)
-        p = self._plans.get(key)
-        if p is None:
-            p = make_plan(J, sparsity, None if default_cv else colorvec, self.fdtype, x_len, self.x1.device,
-                          **self._plan_kw)
-            self._plans[key] = p
-        return p
+        return _cached_plan(self, key, lambda: make_plan(J, sparsity, None if default_cv else colorvec, self.fdtype, x_len,
+                                                         self.x1.device, **self._plan_kw))
+
+    def _oop_plan_for(self, kind, sparsity, colorvec, pn, m, n, device) -> Plan:
+        """The out-of-place plan (finite_difference_jacobian) for a result of `kind` with m rows and n = length(x); of
+        the plan keywords it takes max_batch and scratch_bytes."""
+        def create():
+            suffix, args, keep = _oop_plan_route(kind, sparsity, colorvec, pn, m, n)
+            o = _opts(_fdtype_code(self.fdtype), _device_index(device),
+                      **{k: v for k, v in self._plan_kw.items() if k in ("max_batch", "scratch_bytes")})
+            with torch.cuda.device(device):
+                return Plan(_new_handle(f"fdb_oop_plan_create_{suffix}", *args, C.byref(o)).value)
+        key = ("oop", kind, _sp_key(sparsity) if sparsity is not None else None, _index_key(colorvec), pn, m, n)
+        return _cached_plan(self, key, create)
 
     def invalidate(self):
         for p in self._plans.values():
@@ -977,8 +1028,7 @@ def matrix_colors(A, device=None) -> torch.Tensor:
         cp, k1 = _index_ptr(A.colptr)
         rv, k2 = _index_ptr(A.rowval)
         nc, nr = C.c_int64(), C.c_int64()
-        with torch.cuda.device(dev):
-            L.check(lib.fdb_matrix_colors_csc(A.m, A.n, cp, rv, out.data_ptr(), C.byref(nc), C.byref(nr)))
+        _call(dev, (), lib.fdb_matrix_colors_csc, A.m, A.n, cp, rv, out.data_ptr(), C.byref(nc), C.byref(nr))
         out = out[: A.n]
         out.n_colors, out.n_rounds = nc.value, nr.value
         return out
@@ -992,8 +1042,7 @@ def matrix_colors(A, device=None) -> torch.Tensor:
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     out = torch.zeros(max(n, 1), dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        L.check(lib.fdb_matrix_colors_banded(n, l, u, out.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    _call(dev, (), lib.fdb_matrix_colors_banded, n, l, u, out.data_ptr(), C.c_void_p(_stream(None, dev)))
     return out[:n]
 
 
@@ -1075,16 +1124,11 @@ def finite_difference_jacobian_(J, f, x, cache=None, f_in=None, returntype=None,
     if cache.fx.numel() != m:
         raise ValueError(f"length(cache.fx)={cache.fx.numel()} != size(J,1)={m} (use the 3-array constructor)")
     addr, ctx, pyfn = _as_fn(f, m, n, x.device, 1, fd == L.FDB_COMPLEX)
-    if stream is None:
-        stream = torch.cuda.current_stream(x.device).cuda_stream
+    stream = _stream(stream, x.device)
     if fd == L.FDB_COMPLEX:
         # jacobians.jl:623-648: one complex evaluation per colour, J = imag(f(x + im*eps*e_k))/eps, eps = eps(Float64)
-        with torch.cuda.device(x.device):
-            st = L.lib().fdb_jacobian_complex(plan.handle, addr, ctx, xv.data_ptr(), jv.data_ptr(), C.c_void_p(stream))
-        if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-            exc, pyfn.exc = pyfn.exc, None
-            raise exc
-        L.check(st)
+        _call(x.device, [pyfn], L.lib().fdb_jacobian_complex, plan.handle, addr, ctx, xv.data_ptr(), jv.data_ptr(),
+              C.c_void_p(stream))
         cache._last_plan = plan
         return None
     fin_ptr = None
@@ -1093,14 +1137,8 @@ def finite_difference_jacobian_(J, f, x, cache=None, f_in=None, returntype=None,
         if not _is_cuda(f_in) or f_in.dtype != torch.float64 or f_in.numel() != m:
             raise TypeError("f_in must be a float64 CUDA tensor of length size(J,1)")
         fin_ptr = f_in.data_ptr()
-    with torch.cuda.device(x.device):
-        st = L.lib().fdb_jacobian(plan.handle, addr, ctx, xv.data_ptr(), jv.data_ptr(), cache.fx.data_ptr(), fin_ptr,
-                                  L.STEP_DEFAULT if relstep is None else float(relstep),
-                                  L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc                                          # user f threw: propagate like Julia does
-    L.check(st)
+    _call(x.device, [pyfn], L.lib().fdb_jacobian, plan.handle, addr, ctx, xv.data_ptr(), jv.data_ptr(), cache.fx.data_ptr(),
+          fin_ptr, *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
     cache._last_plan = plan
     return None
 
@@ -1135,10 +1173,8 @@ class JVPCache:
             if self._code == L.FDB_COMPLEX:
                 # jvp.jl:248-250
                 raise ValueError("finite_difference_jvp doesn't support :complex-mode finite diff")
-            h = C.c_void_p()
             o = _opts(self._code, _device_index(self.x1.device))
-            L.check(L.lib().fdb_jvp_plan_create(C.byref(h), m, n, C.byref(o)))
-            self._plan, self._plan_key = Plan(h.value), (m, n)
+            self._plan, self._plan_key = Plan(_new_handle("fdb_jvp_plan_create", m, n, C.byref(o)).value), (m, n)
         return self._plan
 
 
@@ -1183,16 +1219,9 @@ def finite_difference_jvp_(jvp, f, x, v, cache=None, f_in=None, *, relstep=None,
             raise ValueError("JVPCache arrays and f_in must be on x's device")
     plan = cache.plan(m, n)
     addr, ctx, pyfn = _as_fn(f, m, n, x.device, 1)
-    if stream is None:
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-    with torch.cuda.device(x.device):
-        st = L.lib().fdb_jvp(plan.handle, addr, ctx, jv.data_ptr(), xv.data_ptr(), vv.data_ptr(), x1v.data_ptr(),
-                             fx1v.data_ptr(), fin_ptr, L.STEP_DEFAULT if relstep is None else float(relstep),
-                             L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
+    _call(x.device, [pyfn], L.lib().fdb_jvp, plan.handle, addr, ctx, jv.data_ptr(), xv.data_ptr(), vv.data_ptr(),
+          x1v.data_ptr(), fx1v.data_ptr(), fin_ptr, *_steps(relstep, absstep), float(dir),
+          C.c_void_p(_stream(stream, x.device)))
     cache._last_plan = plan
     return None
 
@@ -1228,6 +1257,18 @@ def _oop_kind(sparsity, jac_prototype):
     if sparsity is not None:
         return L.FDB_OOP_DENSE, sparsity.m, sparsity.n
     return L.FDB_OOP_RAW, None, None
+
+
+def _oop_plan_route(kind, sparsity, colorvec, pn, m, n):
+    """(suffix, args, keep) of the out-of-place plan for a result of `kind` with m rows and n = length(x): it is made by
+    fdb_oop_plan_create_<suffix>(&h, *args, &opts) (or fdb_group_create_oop_<suffix>(&h, n_devices, devices, *args,
+    &opts)), and `keep` holds the host arrays the pointers in args point into."""
+    cvp, k0 = _index_ptr(None if _is_identity_colorvec(colorvec, n) else colorvec)
+    if sparsity is not None:
+        cp, k1 = _index_ptr(sparsity.colptr)
+        rv, k2 = _index_ptr(sparsity.rowval)
+        return "csc", (m, n, cp, rv, cvp, kind, max(m, 1)), [k0, k1, k2]
+    return "dense", (m, n, cvp, pn or 0, kind, max(m, 1)), [k0]
 
 
 def _oop_rows(f, x, fd, f_in, m_default, sparsity, pm, n):
@@ -1288,8 +1329,7 @@ class _OopOutput:
         when most candidates were dropped its rowval / nzval are copied into storage of their own size)."""
         if self.kind != L.FDB_OOP_SPARSE:
             return self.dense
-        with torch.cuda.device(self.dev):
-            L.check(L.lib().fdb_stream_sync(C.c_void_p(stream)))
+        _call(self.dev, (), L.lib().fdb_stream_sync, C.c_void_p(stream))
         nnz = int(self.nnz.item())
         rowval, nzval = self.rowval[:nnz], self.nzval[:nnz]
         if 2 * nnz < self.cap:
@@ -1327,8 +1367,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
             raise TypeError("x must be a float64 CUDA tensor: the GPU path has no CPU implementation")
         xv = x.reshape(-1)
         if f_in is None:                                                                  # :250-251
-            if stream is None:
-                stream = torch.cuda.current_stream(x.device).cuda_stream
+            stream = _stream(stream, x.device)
             if isinstance(f, NativeFn):
                 sp = None if sparsity is _DEFAULT else sparsity
                 m = sp.m if isinstance(sp, SparseMatrixCSC) else (
@@ -1366,40 +1405,17 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
         cache.x1.reshape(-1).copy_(xv)
     f_in, m = _oop_rows(f, x, fd, f_in, cache.fx.numel(), sparsity, pm, n)
     dev = x.device
-    key = ("oop", kind, _sp_key(sparsity) if sparsity is not None else None, _index_key(colorvec), pn, m, n)
-    plan = cache._plans.get(key)
-    if plan is None:
-        h = C.c_void_p()
-        o = _opts(fd, _device_index(dev), **{k: v for k, v in cache._plan_kw.items() if k in ("max_batch", "scratch_bytes")})
-        cv = None if _is_identity_colorvec(colorvec, n) else colorvec
-        cvp, k3 = _index_ptr(cv)
-        with torch.cuda.device(dev):
-            if sparsity is not None:
-                cp, k1 = _index_ptr(sparsity.colptr)
-                rv, k2 = _index_ptr(sparsity.rowval)
-                L.check(L.lib().fdb_oop_plan_create_csc(C.byref(h), m, n, cp, rv, cvp, kind, max(m, 1), C.byref(o)))
-            else:
-                L.check(L.lib().fdb_oop_plan_create_dense(C.byref(h), m, n, cvp, pn or 0, kind, max(m, 1), C.byref(o)))
-        plan = Plan(h.value)
-        cache._plans[key] = plan
+    plan = cache._oop_plan_for(kind, sparsity, colorvec, pn, m, n, dev)
     res = _OopOutput(kind, sparsity, pn, m, plan.dense_range()[1], plan.info()["n_entries"], dev)
     addr, ctx, pyfn = _as_fn(f, m, n, dev, 1, fd == L.FDB_COMPLEX, oop=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(dev).cuda_stream
+    stream = _stream(stream, dev)
     fin_ptr = _oop_fin_ptr(f_in, fd, m)
-    with torch.cuda.device(dev):
-        if fd == L.FDB_COMPLEX:
-            st = L.lib().fdb_jacobian_oop_complex(plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out),
-                                                  C.c_void_p(stream))
-        else:
-            st = L.lib().fdb_jacobian_oop(plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out), None, fin_ptr,
-                                          L.STEP_DEFAULT if relstep is None else float(relstep),
-                                          L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
-                                          C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
+    if fd == L.FDB_COMPLEX:
+        _call(dev, [pyfn], L.lib().fdb_jacobian_oop_complex, plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out),
+              C.c_void_p(stream))
+    else:
+        _call(dev, [pyfn], L.lib().fdb_jacobian_oop, plan.handle, addr, ctx, xv.data_ptr(), C.byref(res.out), None, fin_ptr,
+              *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
     cache._last_plan = plan
     return res.result(stream)
 
@@ -1417,8 +1433,7 @@ def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absst
             if isinstance(f, NativeFn):
                 fx = torch.empty(x.numel(), dtype=torch.float64, device=x.device)
                 with torch.cuda.device(x.device):
-                    _native_call(f, fx, x.reshape(-1).contiguous(),
-                                 stream if stream is not None else torch.cuda.current_stream(x.device).cuda_stream)
+                    _native_call(f, fx, x.reshape(-1).contiguous(), _stream(stream, x.device))
             else:
                 fx = f(x)                                                                  # :139-140
         else:
@@ -1455,17 +1470,9 @@ def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absst
     x1 = torch.empty(n, dtype=torch.float64, device=x.device)
     fx1 = torch.empty(m, dtype=torch.float64, device=x.device)
     addr, ctx, pyfn = _as_fn(f, m, n, x.device, 1, oop=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(x.device).cuda_stream
-    with torch.cuda.device(x.device):
-        st = L.lib().fdb_jvp_oop(plan.handle, addr, ctx, _fx_ptr(jvp), xv.data_ptr() if n else None,
-                                 vv.data_ptr() if n else None, _fx_ptr(x1), _fx_ptr(fx1), fin_ptr,
-                                 L.STEP_DEFAULT if relstep is None else float(relstep),
-                                 L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
+    _call(x.device, [pyfn], L.lib().fdb_jvp_oop, plan.handle, addr, ctx, _fx_ptr(jvp), xv.data_ptr() if n else None,
+          vv.data_ptr() if n else None, _fx_ptr(x1), _fx_ptr(fx1), fin_ptr, *_steps(relstep, absstep), float(dir),
+          C.c_void_p(_stream(stream, x.device)))
     cache._last_plan = plan
     return jvp
 
@@ -1531,15 +1538,10 @@ class HessianCache:
         self._plans = {}
 
     def plan_for(self, n: int, ldH: int, device) -> Plan:
-        key = (n, ldH, str(device))
-        p = self._plans.get(key)
-        if p is None:
-            code = _hessian_fdtype_code(self.fdtype)
-            h = C.c_void_p()
-            o = _opts(code, _device_index(device), **self._plan_kw)
-            L.check(L.lib().fdb_hessian_plan_create(C.byref(h), n, ldH, C.byref(o)))
-            p = self._plans[key] = Plan(h.value)
-        return p
+        def create():
+            o = _opts(_hessian_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
+            return Plan(_new_handle("fdb_hessian_plan_create", n, ldH, C.byref(o)).value)
+        return _cached_plan(self, (n, ldH, str(device)), create)
 
 
 def _colmajor_square(H, n):
@@ -1570,21 +1572,13 @@ def finite_difference_hessian_(H, f, x, cache=None, *, relstep=None, absstep=Non
     ldH = _colmajor_square(H, n)
     plan = cache.plan_for(n, ldH, xv.device)
     addr, ctx, pyfn = _as_fn(f, 1, n, xv.device, 1, scalar=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(xv.device).cuda_stream
     fx_ptr = None
     if fx is not None:
         if not _is_cuda(fx) or fx.dtype != torch.float64 or fx.numel() != 1:
             raise TypeError("fx must be a 1-element float64 CUDA tensor")
         fx_ptr = fx.data_ptr()
-    with torch.cuda.device(xv.device):
-        st = L.lib().fdb_hessian(plan.handle, addr, ctx, xv.data_ptr(), H.data_ptr() if n > 0 else None, fx_ptr,
-                                 L.STEP_DEFAULT if relstep is None else float(relstep),
-                                 L.STEP_DEFAULT if absstep is None else float(absstep), C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
+    _call(xv.device, [pyfn], L.lib().fdb_hessian, plan.handle, addr, ctx, xv.data_ptr(), H.data_ptr() if n > 0 else None,
+          fx_ptr, *_steps(relstep, absstep), C.c_void_p(_stream(stream, xv.device)))
     cache._last_plan = plan
     return None
 
@@ -1660,25 +1654,16 @@ class GradientCache:
         self._plan_kw = plan_kw
         self._plans = {}
 
+    def _plan(self, creator, device, *args) -> Plan:
+        o = _opts(_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
+        return Plan(_new_handle(creator, *args, C.byref(o)).value)
+
     def plan_for(self, n: int, device) -> Plan:
-        key = (n, str(device))
-        p = self._plans.get(key)
-        if p is None:
-            h = C.c_void_p()
-            o = _opts(_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
-            L.check(L.lib().fdb_plan_create_dense(C.byref(h), 1, n, 1, C.byref(o)))
-            p = self._plans[key] = Plan(h.value)
-        return p
+        return _cached_plan(self, (n, str(device)), lambda: self._plan("fdb_plan_create_dense", device, 1, n, 1))
 
     def scalar_plan_for(self, m: int, device) -> Plan:
-        key = ("scalar", m, str(device))
-        p = self._plans.get(key)
-        if p is None:
-            h = C.c_void_p()
-            o = _opts(_fdtype_code(self.fdtype), _device_index(device), **self._plan_kw)
-            L.check(L.lib().fdb_scalar_gradient_plan_create(C.byref(h), m, C.byref(o)))
-            p = self._plans[key] = Plan(h.value)
-        return p
+        return _cached_plan(self, ("scalar", m, str(device)),
+                            lambda: self._plan("fdb_scalar_gradient_plan_create", device, m))
 
 
 def finite_difference_gradient_(df, f, x, cache=None, *, relstep=None, absstep=None, dir=True, stream=None):
@@ -1712,35 +1697,22 @@ def finite_difference_gradient_(df, f, x, cache=None, *, relstep=None, absstep=N
     fd = _fdtype_code(cache.fdtype)
     plan = cache.plan_for(n, xv.device)
     addr, ctx, pyfn = _as_fn(f, 1, n, xv.device, 1, fd == L.FDB_COMPLEX, scalar=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(xv.device).cuda_stream
-    with torch.cuda.device(xv.device):
-        if fd == L.FDB_COMPLEX:                                              # :458-469
-            st = L.lib().fdb_jacobian_complex(plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(), C.c_void_p(stream))
-        else:
-            fin = None
-            if fd == L.FDB_FORWARD and cache.fx is not None:                # fx0 = fx !== nothing ? fx : f(x)   :410
-                if isinstance(cache.fx, torch.Tensor):
-                    fin = cache.fx
-                    if not fin.is_cuda or fin.dtype != torch.float64 or fin.numel() != 1:
-                        raise TypeError("cache.fx must be a number or a 1-element float64 CUDA tensor")
-                else:
-                    # a number: staged in ONE device slot kept on the cache, so that the arguments of the call (and a
-                    # captured graph's key under use_graph) stay the same from call to call
-                    fin = getattr(cache, "_fin", None)
-                    if fin is None or fin.device != xv.device:
-                        fin = cache._fin = torch.empty(1, dtype=torch.float64, device=xv.device)
-                    with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=xv.device)):
-                        fin.fill_(float(cache.fx))
-            # d_fx = NULL: f(x) goes to the plan's own buffer (cache.fx is an input here, never written)
-            st = L.lib().fdb_jacobian(plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(), None,
-                                      None if fin is None else fin.data_ptr(),
-                                      L.STEP_DEFAULT if relstep is None else float(relstep),
-                                      L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
+    stream = _stream(stream, xv.device)
+    if fd == L.FDB_COMPLEX:                                                  # :458-469
+        _call(xv.device, [pyfn], L.lib().fdb_jacobian_complex, plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(),
+              C.c_void_p(stream))
+    else:
+        fin = None
+        if fd == L.FDB_FORWARD and cache.fx is not None:                    # fx0 = fx !== nothing ? fx : f(x)   :410
+            if isinstance(cache.fx, torch.Tensor):
+                fin = cache.fx
+                if not fin.is_cuda or fin.dtype != torch.float64 or fin.numel() != 1:
+                    raise TypeError("cache.fx must be a number or a 1-element float64 CUDA tensor")
+            else:
+                fin = _device_slot(cache, "_fin", xv.device, stream, cache.fx)
+        # d_fx = NULL: f(x) goes to the plan's own buffer (cache.fx is an input here, never written)
+        _call(xv.device, [pyfn], L.lib().fdb_jacobian, plan.handle, addr, ctx, xv.data_ptr(), dv.data_ptr(), None,
+              None if fin is None else fin.data_ptr(), *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
     cache._last_plan = plan
     return None
 
@@ -1785,17 +1757,6 @@ def _real_input(x):
         raise TypeError("x must be a real number: complex-valued x is not supported")
 
 
-def _call_result(st, pyfn):
-    if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-        exc, pyfn.exc = pyfn.exc, None
-        raise exc
-    L.check(st)
-
-
-def _steps(relstep, absstep):
-    return (L.STEP_DEFAULT if relstep is None else float(relstep), L.STEP_DEFAULT if absstep is None else float(absstep))
-
-
 def _flat_f64(t, what):
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
         raise TypeError(f"{what} must be a float64 CUDA tensor: the GPU path has no CPU implementation")
@@ -1837,29 +1798,21 @@ def _scalar_gradient_(df, f, x, cache, relstep, absstep, dir, stream):
         tv = None
     plan = cache.scalar_plan_for(m, dev)
     addr, ctx, pyfn = _as_fn(f, m, 1, dev, 1, fd == L.FDB_COMPLEX, tvec=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(dev).cuda_stream
+    stream = _stream(stream, dev)
     if tv is None:
-        # a number: staged in ONE device slot kept on the cache, so the arguments of the call (and a captured graph's key
-        # under use_graph) stay the same from call to call
-        tv = getattr(cache, "_t", None)
-        if tv is None or tv.device != dev:
-            tv = cache._t = torch.empty(1, dtype=torch.float64, device=dev)
-        with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=dev)):
-            tv.fill_(float(x))
-    with torch.cuda.device(dev):
-        if fd == L.FDB_COMPLEX:
-            st = L.lib().fdb_derivative_complex(plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(), C.c_void_p(stream))
-        else:
-            fx_ptr = None
-            if fd == L.FDB_FORWARD and cache.fx is not None:                  # :501-502
-                fxv = _flat_f64(cache.fx, "cache.fx")
-                if fxv.numel() != m or fxv.device != dev:
-                    raise ValueError("cache.fx must hold the m values f(x) on df's device")
-                fx_ptr = _fx_ptr(fxv)
-            st = L.lib().fdb_derivative(plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(), fx_ptr,
-                                        *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
-    _call_result(st, pyfn)
+        tv = _device_slot(cache, "_t", dev, stream, x)
+    if fd == L.FDB_COMPLEX:
+        _call(dev, [pyfn], L.lib().fdb_derivative_complex, plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(),
+              C.c_void_p(stream))
+    else:
+        fx_ptr = None
+        if fd == L.FDB_FORWARD and cache.fx is not None:                      # :501-502
+            fxv = _flat_f64(cache.fx, "cache.fx")
+            if fxv.numel() != m or fxv.device != dev:
+                raise ValueError("cache.fx must hold the m values f(x) on df's device")
+            fx_ptr = _fx_ptr(fxv)
+        _call(dev, [pyfn], L.lib().fdb_derivative, plan.handle, addr, ctx, dv.data_ptr(), tv.data_ptr(), fx_ptr,
+              *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
     cache._last_plan = plan
     return None
 
@@ -1903,14 +1856,10 @@ class DerivativeCache:
         self._plans = {}
 
     def plan_for(self, n: int, device) -> Plan:
-        key = (n, str(device))
-        p = self._plans.get(key)
-        if p is None:
-            h = C.c_void_p()
+        def create():
             o = _opts(self._code, _device_index(device), **self._plan_kw)
-            L.check(L.lib().fdb_derivative_plan_create(C.byref(h), n, C.byref(o)))
-            p = self._plans[key] = Plan(h.value)
-        return p
+            return Plan(_new_handle("fdb_derivative_plan_create", n, C.byref(o)).value)
+        return _cached_plan(self, (n, str(device)), create)
 
 
 def finite_difference_derivative_(df, f, x, cache="central", returntype=None, fx=None, epsilon=None, *, relstep=None,
@@ -1936,21 +1885,19 @@ def finite_difference_derivative_(df, f, x, cache="central", returntype=None, fx
         raise ValueError("df and x must be on the same device")
     plan = cache.plan_for(n, xv.device)
     addr, ctx, pyfn = _as_fn(f, n, n, xv.device, 1, cache._code == L.FDB_COMPLEX, elementwise=True)
-    if stream is None:
-        stream = torch.cuda.current_stream(xv.device).cuda_stream
-    with torch.cuda.device(xv.device):
-        if cache._code == L.FDB_COMPLEX:
-            st = L.lib().fdb_derivative_complex(plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(), C.c_void_p(stream))
-        else:
-            fx_ptr = None
-            if cache._code == L.FDB_FORWARD and cache.fx is not None:          # :213-214
-                fxv = _flat_f64(cache.fx, "cache.fx")
-                if fxv.numel() != n or fxv.device != xv.device:
-                    raise ValueError("cache.fx must hold the n values f(x) on x's device")
-                fx_ptr = _fx_ptr(fxv)
-            st = L.lib().fdb_derivative(plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(), fx_ptr,
-                                        *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
-    _call_result(st, pyfn)
+    stream = _stream(stream, xv.device)
+    if cache._code == L.FDB_COMPLEX:
+        _call(xv.device, [pyfn], L.lib().fdb_derivative_complex, plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(),
+              C.c_void_p(stream))
+    else:
+        fx_ptr = None
+        if cache._code == L.FDB_FORWARD and cache.fx is not None:              # :213-214
+            fxv = _flat_f64(cache.fx, "cache.fx")
+            if fxv.numel() != n or fxv.device != xv.device:
+                raise ValueError("cache.fx must hold the n values f(x) on x's device")
+            fx_ptr = _fx_ptr(fxv)
+        _call(xv.device, [pyfn], L.lib().fdb_derivative, plan.handle, addr, ctx, dv.data_ptr(), xv.data_ptr(), fx_ptr,
+              *_steps(relstep, absstep), float(dir), C.c_void_p(stream))
     cache._last_plan = plan
     return df
 

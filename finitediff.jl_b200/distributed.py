@@ -96,8 +96,7 @@ class IpcBuffer:
     def __init__(self, count: int, device: torch.device):
         self.count = int(count)
         p = C.c_void_p()
-        with torch.cuda.device(device):
-            L.check(L.lib().fdb_device_alloc(C.byref(p), max(self.count, 2) * 8))
+        api._call(device, (), L.lib().fdb_device_alloc, C.byref(p), max(self.count, 2) * 8)
         self.ptr = p.value
         self.device = device
         self.tensor = torch.as_tensor(api._DevArray(self.ptr, (self.count,)), device=device)
@@ -125,8 +124,7 @@ class DeviceBarrier:
         self.group = group
         self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
         h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            L.check(L.lib().fdb_sync_create(C.byref(h), self.rank, self.world, api._device_index(self.device)))
+        api._call(self.device, (), L.lib().fdb_sync_create, C.byref(h), self.rank, self.world, api._device_index(self.device))
         self._h = h
         flags = C.c_void_p()
         L.check(L.lib().fdb_sync_flags(self._h, C.byref(flags)))
@@ -150,9 +148,7 @@ class DeviceBarrier:
 
     def wait(self, stream=None):
         """Enqueue one barrier on `stream` (default: the current stream of the device)."""
-        if stream is None:
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-        L.check(L.lib().fdb_sync_barrier(self._h, C.c_void_p(stream)))
+        L.check(L.lib().fdb_sync_barrier(self._h, C.c_void_p(api._stream(stream, self.device))))
 
     def close(self):
         if self._h is None:
@@ -162,21 +158,65 @@ class DeviceBarrier:
             for p in self._mapped:
                 L.lib().fdb_ipc_close(C.c_void_p(p))
             self._mapped = []
-        try:
-            dist.barrier(group=self.group)       # nobody frees a flag block a peer may still signal
-        except Exception:
-            pass
+        _barrier(self.group)                     # nobody frees a flag block a peer may still signal
         L.lib().fdb_sync_destroy(self._h)
         self._h = None
 
 
+def _barrier(group):
+    """dist.barrier on `group` at teardown, where the process group may already be gone."""
+    try:
+        dist.barrier(group=group)
+    except Exception:
+        pass
+
+
+class _RootValues:
+    """Rank 0's J.nzval mapped into every rank over CUDA IPC.  Rank 0 moves its values into an IpcBuffer (so that the
+    handle maps exactly them, and J.nzval is that buffer from then on); every other rank opens rank 0's handle and finds
+    the mapping at `ptr` (None on rank 0)."""
+
+    def __init__(self, J: api.SparseMatrixCSC, device, rank: int, world: int, group):
+        self.device, self.group = device, group
+        self._ipc: Optional[IpcBuffer] = None
+        self.ptr = None
+        mine = None
+        if rank == 0:
+            self._ipc = IpcBuffer(J.nzval.numel(), device)
+            self._ipc.tensor.copy_(J.nzval)
+            J.nzval = self._ipc.tensor
+            mine = self._ipc.handle()
+        handles = [None] * world
+        dist.all_gather_object(handles, mine, group=group)
+        if rank != 0:
+            p = C.c_void_p()
+            api._call(device, (), L.lib().fdb_ipc_open, handles[0], C.byref(p))
+            self.ptr = p.value
+
+    def close(self):
+        """Unmap, then a barrier, then free: rank 0 frees its buffer only once no rank maps it."""
+        if self.ptr:
+            with torch.cuda.device(self.device):
+                L.lib().fdb_ipc_close(C.c_void_p(self.ptr))
+            self.ptr = None
+        _barrier(self.group)
+        if self._ipc is not None:
+            self._ipc.free()
+            self._ipc = None
+
+
 class _Group:
-    """What GroupJacobian and GroupHessian share: the fdb_group handle, its member plans, one f per member behind one
-    entry point, and the joins."""
+    """What the group classes share: the fdb_group handle, its member plans, one f per member behind one entry point,
+    and the joins."""
 
     def _set_devices(self, devices):
         self.devices = [api._device_index(d) if not isinstance(d, int) else int(d) for d in devices]
         self.root = torch.device("cuda", self.devices[0])
+
+    def _create(self, creator, opts, *args):
+        """Adopt the group fdb_group_create_<creator>(&h, n_devices, devices, *args, &opts) creates."""
+        devs = (C.c_int * len(self.devices))(*self.devices)
+        self._adopt(api._new_handle(f"fdb_group_create_{creator}", len(self.devices), devs, *args, C.byref(opts)))
 
     def _adopt(self, h):
         lib = L.lib()
@@ -190,9 +230,9 @@ class _Group:
         self._fns = None
 
     def _member_fns(self, fs, m, n, **kind):
-        """(entry address, contexts array, per-member wrappers) for one f per member.  The ABI takes one f and a context
-        per member: NativeFns must share their address; Python callables go through ONE trampoline whose context is the
-        member index + 1, forwarding to that member's wrapper (tensors on that member's device)."""
+        """(entry address, contexts array, per-member Python wrappers or None) for one f per member.  The ABI takes one f
+        and a context per member: NativeFns must share their address; Python callables go through ONE trampoline whose
+        context is the member index + 1, forwarding to that member's wrapper (tensors on that member's device)."""
         if len(fs) != len(self.devices):
             raise ValueError("one f! per member")
         if self._fns is None or self._fns[0] is not fs:
@@ -214,16 +254,7 @@ class _Group:
         if any(w[0] != addr for w in wrapped):
             raise ValueError("all members must share one f! entry point (contexts may differ per device)")
         ctxs = (C.c_void_p * len(wrapped))(*[C.cast(w[1], C.c_void_p).value if w[1] is not None else None for w in wrapped])
-        return addr, ctxs, wrapped
-
-    @staticmethod
-    def _check(st, wrapped):
-        """A member's Python exception propagates as itself; any other failure as FdbError."""
-        for w in wrapped:
-            if st == L.FDB_ERR_CALLBACK and w[2] is not None and w[2].exc is not None:
-                exc, w[2].exc = w[2].exc, None
-                raise exc
-        L.check(st)
+        return addr, ctxs, [w[2] for w in wrapped]
 
     def synchronize(self):
         for d in set(self.devices):
@@ -247,68 +278,20 @@ class GroupJacobian(_Group):
         self.J, self.fdtype = J, fdtype
         if sparsity is api._DEFAULT:
             sparsity = J if api._has_sparsestruct(J) else None
-        fd = api._fdtype_code(fdtype)
-        o = api._opts(fd, self.devices[0], **plan_kw)
-        n_dev = len(self.devices)
-        devs = (C.c_int * n_dev)(*self.devices)
-        h = C.c_void_p()
-        diag_route = api._diagonals_route(J, sparsity)
-        cv_ptr, k0 = api._index_ptr(colorvec)
-        self._keep = [k0]
-        lib = L.lib()
-        if diag_route is not None:
-            # Diagonal / Bidiagonal / SymTridiagonal sparsity: members write disjoint column sets of the packed diagonals
-            L.check(lib.fdb_group_create_banded(C.byref(h), n_dev, devs, *diag_route, cv_ptr, C.byref(o)))
-        elif sparsity is None:
-            m, n, ld = api._dense_ld(J)
-            L.check(lib.fdb_group_create_dense(C.byref(h), n_dev, devs, m, n, ld, C.byref(o)))
-        elif isinstance(sparsity, api.SparseMatrixCSC):
-            cp, k1 = api._index_ptr(sparsity.colptr)
-            rv, k2 = api._index_ptr(sparsity.rowval)
-            self._keep += [k1, k2]
-            if isinstance(J, api.SparseMatrixCSC):
-                same = J is sparsity or (J.colptr is sparsity.colptr and J.rowval is sparsity.rowval)
-                jcp = jrv = None
-                if not same:
-                    jcp, k3 = api._index_ptr(J.colptr)
-                    jrv, k4 = api._index_ptr(J.rowval)
-                    self._keep += [k3, k4]
-                L.check(lib.fdb_group_create_csc(C.byref(h), n_dev, devs, sparsity.m, sparsity.n, cp, rv, L.FDB_J_CSC_NZVAL,
-                                                 jcp, jrv, 0, cv_ptr, C.byref(o)))
-            else:
-                m, n, ld = api._dense_ld(J)
-                L.check(lib.fdb_group_create_csc(C.byref(h), n_dev, devs, m, n, cp, rv, L.FDB_J_DENSE, None, None, ld,
-                                                 cv_ptr, C.byref(o)))
-        elif isinstance(sparsity, api.BandedMatrix):
-            if isinstance(J, api.BandedMatrix):
-                L.check(lib.fdb_group_create_banded(C.byref(h), n_dev, devs, sparsity.m, sparsity.n, sparsity.l, sparsity.u,
-                                                    L.FDB_J_BAND, 0, cv_ptr, C.byref(o)))
-            else:
-                m, n, ld = api._dense_ld(J)
-                L.check(lib.fdb_group_create_banded(C.byref(h), n_dev, devs, m, n, sparsity.l, sparsity.u, L.FDB_J_DENSE, ld,
-                                                    cv_ptr, C.byref(o)))
-        elif api._block_banded_plan_args(J, sparsity) is not None:
-            blocks, l, u, lam, mu, ldata = api._block_banded_plan_args(J, sparsity)
-            self._keep.append(blocks)
-            L.check(lib.fdb_group_create_block_banded(C.byref(h), n_dev, devs, len(blocks),
-                                                      blocks.ctypes.data if len(blocks) else None, l, u, lam, mu, ldata,
-                                                      cv_ptr, C.byref(o)))
-        else:
+        kind, args, self._keep = api._plan_route(J, sparsity, colorvec)
+        if kind == "coo":
             raise TypeError(f"GroupJacobian: unsupported sparsity type {type(sparsity)}")
-        self._adopt(h)
+        if kind == "dense_colorvec":
+            kind, args = "dense", args[:3]          # a dense group splits the columns 1:n; colorvec is not read
+        self._create(kind, api._opts(api._fdtype_code(fdtype), self.devices[0], **plan_kw), *args)
 
     def run(self, fs, x, fx=None, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):
         m, n = api._shape_of(self.J)
-        addr, ctxs, wrapped = self._member_fns(fs, m, n)
-        if stream is None:
-            stream = torch.cuda.current_stream(self.root).cuda_stream
-        jv = api._j_values(self.J)
-        with torch.cuda.device(self.root):
-            st = L.lib().fdb_group_jacobian(self._h, addr, ctxs, x.data_ptr(), jv.data_ptr(),
-                                            None if fx is None else fx.data_ptr(), None if f_in is None else f_in.data_ptr(),
-                                            L.STEP_DEFAULT if relstep is None else float(relstep),
-                                            L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), C.c_void_p(stream))
-        self._check(st, wrapped)
+        addr, ctxs, pyfns = self._member_fns(fs, m, n)
+        api._call(self.root, pyfns, L.lib().fdb_group_jacobian, self._h, addr, ctxs, x.data_ptr(),
+                  api._j_values(self.J).data_ptr(), None if fx is None else fx.data_ptr(),
+                  None if f_in is None else f_in.data_ptr(), *api._steps(relstep, absstep), float(dir),
+                  C.c_void_p(api._stream(stream, self.root)))
 
 
 class GroupHessian(_Group):
@@ -324,11 +307,7 @@ class GroupHessian(_Group):
         self._set_devices(devices)
         self.n = int(n)
         self.ldH = max(self.n, 1) if ldH is None else int(ldH)
-        o = api._opts(api._hessian_fdtype_code(fdtype), self.devices[0], **plan_kw)
-        devs = (C.c_int * len(self.devices))(*self.devices)
-        h = C.c_void_p()
-        L.check(L.lib().fdb_group_create_hessian(C.byref(h), len(self.devices), devs, self.n, self.ldH, C.byref(o)))
-        self._adopt(h)
+        self._create("hessian", api._opts(api._hessian_fdtype_code(fdtype), self.devices[0], **plan_kw), self.n, self.ldH)
 
     def run(self, fs, x, H, fx=None, *, relstep=None, absstep=None, stream=None):
         """fs: one f per member — a NativeFn (batched fdb_fn with m = 1, context on that member's device) or a Python
@@ -342,15 +321,10 @@ class GroupHessian(_Group):
             raise ValueError(f"H must be column-major with leading dimension {self.ldH} on {self.root}")
         if fx is not None and (not api._is_cuda(fx) or fx.dtype != torch.float64 or fx.numel() != 1):
             raise TypeError("fx must be a 1-element float64 CUDA tensor")
-        addr, ctxs, wrapped = self._member_fns(fs, 1, self.n, scalar=True)
-        if stream is None:
-            stream = torch.cuda.current_stream(self.root).cuda_stream
-        with torch.cuda.device(self.root):
-            st = L.lib().fdb_group_hessian(self._h, addr, ctxs, xv.data_ptr(), H.data_ptr() if self.n > 0 else None,
-                                           None if fx is None else fx.data_ptr(),
-                                           L.STEP_DEFAULT if relstep is None else float(relstep),
-                                           L.STEP_DEFAULT if absstep is None else float(absstep), C.c_void_p(stream))
-        self._check(st, wrapped)
+        addr, ctxs, pyfns = self._member_fns(fs, 1, self.n, scalar=True)
+        api._call(self.root, pyfns, L.lib().fdb_group_hessian, self._h, addr, ctxs, xv.data_ptr(),
+                  H.data_ptr() if self.n > 0 else None, None if fx is None else fx.data_ptr(),
+                  *api._steps(relstep, absstep), C.c_void_p(api._stream(stream, self.root)))
 
 
 def dense_column_blocks(n: int, world: int) -> List[tuple]:
@@ -382,13 +356,8 @@ class GroupGradient(_Group):
         self.fdtype = fdtype.lstrip(":") if isinstance(fdtype, str) else fdtype
         self._code = api._fdtype_code(self.fdtype)
         self._set_devices(devices)
-        o = api._opts(self._code, self.devices[0], **plan_kw)
-        devs = (C.c_int * len(self.devices))(*self.devices)
-        h = C.c_void_p()
-        L.check(L.lib().fdb_group_create_dense(C.byref(h), len(self.devices), devs, 1, self.n, 1, C.byref(o)))
-        self._adopt(h)
+        self._create("dense", api._opts(self._code, self.devices[0], **plan_kw), 1, self.n, 1)
         self.columns = dense_column_blocks(self.n, len(self.devices))      # member i: plans[i].dense_range()
-        self._fx_slot = None        # the root's one device slot for f(x) in forward mode (a stable pointer for graphs)
 
     def run(self, fs, x, df, fx=None, *, relstep=None, absstep=None, dir=True, stream=None):
         """fs: one f per member — a NativeFn (batched fdb_fn with m = 1, context on that member's device) or a Python
@@ -411,36 +380,24 @@ class GroupGradient(_Group):
                 raise TypeError(f"fx must be a number or a 1-element float64 CUDA tensor on {self.root}")
         elif fx is not None and not api._is_number(fx):
             raise TypeError("fx must be a number or a 1-element float64 CUDA tensor")
-        addr, ctxs, wrapped = self._member_fns(fs, 1, self.n, scalar=True)
-        if stream is None:
-            stream = torch.cuda.current_stream(self.root).cuda_stream
-        with torch.cuda.device(self.root):
-            fin = None
-            if self._code == L.FDB_FORWARD:
-                fin = fx if isinstance(fx, torch.Tensor) else self._root_slot()
-                if fx is None:
-                    self._root_fx(fs, wrapped, xv, fin, stream)
-                elif not isinstance(fx, torch.Tensor):
-                    with torch.cuda.stream(torch.cuda.ExternalStream(stream, device=self.root)):
-                        fin.fill_(float(fx))
-            st = L.lib().fdb_group_jacobian(self._h, addr, ctxs, xv.data_ptr() or None, dv.data_ptr() or None, None,
-                                            None if fin is None else fin.data_ptr(),
-                                            L.STEP_DEFAULT if relstep is None else float(relstep),
-                                            L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
-                                            C.c_void_p(stream))
-        self._check(st, wrapped)
-
-    def _root_slot(self):
-        if self._fx_slot is None:
-            self._fx_slot = torch.empty(1, dtype=torch.float64, device=self.root)
-        return self._fx_slot
+        addr, ctxs, pyfns = self._member_fns(fs, 1, self.n, scalar=True)
+        stream = api._stream(stream, self.root)
+        fin = None
+        if self._code == L.FDB_FORWARD:
+            # a number (or nothing: f(x) below) goes into the root's one device slot, a stable pointer for graphs
+            fin = fx if isinstance(fx, torch.Tensor) else api._device_slot(self, "_fx_slot", self.root, stream, fx)
+            if fx is None:
+                with torch.cuda.device(self.root):
+                    self._root_fx(fs[0], pyfns[0], xv, fin, stream)
+        api._call(self.root, pyfns, L.lib().fdb_group_jacobian, self._h, addr, ctxs, xv.data_ptr() or None,
+                  dv.data_ptr() or None, None, None if fin is None else fin.data_ptr(), *api._steps(relstep, absstep),
+                  float(dir), C.c_void_p(stream))
 
     @staticmethod
-    def _root_fx(fs, wrapped, xv, fin, stream):
+    def _root_fx(f0, py, xv, fin, stream):
         """f(x) by member 0's f, into fin on the root's stream (fx0 = f(x), gradients.jl:410)"""
-        py = wrapped[0][2]
         if py is None:
-            api._native_call(fs[0], fin, xv, stream)
+            api._native_call(f0, fin, xv, stream)
             return
         if py._tramp(None, fin.data_ptr(), xv.data_ptr() or None, 1, 1, max(xv.numel(), 1), stream) != 0:
             exc, py.exc = py.exc, None
@@ -473,23 +430,9 @@ class GroupJacobianOOP(_Group):
         if self._key is not None:
             self.close()
         o = api._opts(self._code, self.devices[0], **self._plan_kw)
-        devs = (C.c_int * len(self.devices))(*self.devices)
-        cv = None if api._is_identity_colorvec(self.colorvec, n) else self.colorvec
-        cvp, k0 = api._index_ptr(cv)
-        self._keep = [k0]
-        h = C.c_void_p()
-        lib = L.lib()
+        suffix, args, self._keep = api._oop_plan_route(self.kind, self.sparsity, self.colorvec, self.pn, m, n)
         with torch.cuda.device(self.root):
-            if self.sparsity is not None:
-                cp, k1 = api._index_ptr(self.sparsity.colptr)
-                rv, k2 = api._index_ptr(self.sparsity.rowval)
-                self._keep += [k1, k2]
-                L.check(lib.fdb_group_create_oop_csc(C.byref(h), len(self.devices), devs, m, n, cp, rv, cvp, self.kind,
-                                                     max(m, 1), C.byref(o)))
-            else:
-                L.check(lib.fdb_group_create_oop_dense(C.byref(h), len(self.devices), devs, m, n, cvp, self.pn or 0,
-                                                       self.kind, max(m, 1), C.byref(o)))
-        self._adopt(h)
+            self._create(f"oop_{suffix}", o, *args)
         self._key = (m, n)
 
     def run(self, fs, x, f_in=None, *, relstep=None, absstep=None, dir=True, stream=None):
@@ -505,8 +448,7 @@ class GroupJacobianOOP(_Group):
             raise ValueError("one f per member")
         xv = x.reshape(-1).contiguous()
         n = xv.numel()
-        if stream is None:
-            stream = torch.cuda.current_stream(self.root).cuda_stream
+        stream = api._stream(stream, self.root)
         f_in, m = api._oop_rows(fs[0], x, self._code, f_in, self.pm if self.pm is not None else n, self.sparsity, self.pm, n)
         if f_in is None and self._code == L.FDB_FORWARD:       # a NativeFn: f(x) at the root, as the Python f above
             f_in = torch.empty(m, dtype=torch.float64, device=self.root)
@@ -515,14 +457,10 @@ class GroupJacobianOOP(_Group):
         self._build(m, n)
         res = api._OopOutput(self.kind, self.sparsity, self.pn, m, self.plans[-1].dense_range()[1],
                              self.plans[0].info()["n_entries"], self.root)
-        addr, ctxs, wrapped = self._member_fns(fs, m, n, oop=True)
-        fin_ptr = api._oop_fin_ptr(f_in, self._code, m)
-        with torch.cuda.device(self.root):
-            st = L.lib().fdb_group_jacobian_oop(self._h, addr, ctxs, xv.data_ptr(), C.byref(res.out), None, fin_ptr,
-                                                L.STEP_DEFAULT if relstep is None else float(relstep),
-                                                L.STEP_DEFAULT if absstep is None else float(absstep), float(dir),
-                                                C.c_void_p(stream))
-        self._check(st, wrapped)
+        addr, ctxs, pyfns = self._member_fns(fs, m, n, oop=True)
+        api._call(self.root, pyfns, L.lib().fdb_group_jacobian_oop, self._h, addr, ctxs, xv.data_ptr(), C.byref(res.out),
+                  None, api._oop_fin_ptr(f_in, self._code, m), *api._steps(relstep, absstep), float(dir),
+                  C.c_void_p(stream))
         return res.result(stream)
 
     def close(self):
@@ -565,7 +503,7 @@ class ShardedJacobian:
         self.flag = torch.zeros(1, dtype=torch.float32, device=self.device)
         self.mode = mode
         self._peers = []
-        self._root_ptr = None
+        self._root: Optional[_RootValues] = None
         self._J_run = J
         self._ipc: Optional[IpcBuffer] = None
         self.barrier: Optional[DeviceBarrier] = None
@@ -584,27 +522,17 @@ class ShardedJacobian:
 
     def _setup_p2p(self):
         nnz = self.J.nzval.numel()
-        handles = [None] * self.world
         if self.shared:
-            mine = None
-            if self.rank == 0:
-                self._ipc = IpcBuffer(nnz, self.device)
-                self._ipc.tensor.copy_(self.J.nzval)
-                self.J.nzval = self._ipc.tensor             # rank 0's values now live in the IPC-exportable buffer
-                mine = self._ipc.handle()
-            dist.all_gather_object(handles, mine, group=self.group)
-            if self.rank != 0:
-                p = C.c_void_p()
-                with torch.cuda.device(self.device):
-                    L.check(L.lib().fdb_ipc_open(handles[0], C.byref(p)))
-                self._root_ptr = p.value
+            self._root = _RootValues(self.J, self.device, self.rank, self.world, self.group)
+            if self._root.ptr is not None:
                 # rank 0's nzval as mapped into this process: a raw pointer (api.PeerValues), never a torch tensor
                 self._J_run = api.SparseMatrixCSC(self.J.m, self.J.n, self.J.colptr, self.J.rowval,
-                                                  api.PeerValues(self._root_ptr, nnz))
+                                                  api.PeerValues(self._root.ptr, nnz))
         else:
             self._ipc = IpcBuffer(nnz, self.device)
             self._ipc.tensor.copy_(self.J.nzval)
             self.J.nzval = self._ipc.tensor
+            handles = [None] * self.world
             dist.all_gather_object(handles, self._ipc.handle(), group=self.group)
             ptrs = []
             with torch.cuda.device(self.device):
@@ -647,19 +575,15 @@ class ShardedJacobian:
                 for p in self._peers:
                     L.lib().fdb_ipc_close(C.c_void_p(p))
             self._peers = []
-        if self._root_ptr:
-            with torch.cuda.device(self.device):
-                L.lib().fdb_ipc_close(C.c_void_p(self._root_ptr))
-            self._root_ptr = None
-            self._J_run = self.J
         if self.barrier is not None:
             self.barrier.close()
             self.barrier = None
-        if self.group is None or dist.is_initialized():
-            try:
-                dist.barrier(group=self.group)
-            except Exception:
-                pass
+        if self._root is not None:
+            self._root.close()
+            self._root = None
+            self._J_run = self.J
+            return
+        _barrier(self.group)
         if self._ipc is not None:
             self._ipc.free()
             self._ipc = None
@@ -718,22 +642,17 @@ class EpsPlan:
 
     def __init__(self, n: int, colorvec, fdtype, device):
         self.device = torch.device(device)
-        h = C.c_void_p()
         o = api._opts(api._fdtype_code(fdtype), api._device_index(device))
         cv_ptr, keep = api._index_ptr(colorvec)
         with torch.cuda.device(self.device):
-            L.check(L.lib().fdb_eps_plan_create(C.byref(h), int(n), cv_ptr, C.byref(o)))
+            h = api._new_handle("fdb_eps_plan_create", int(n), cv_ptr, C.byref(o))
         self.plan = api.Plan(h.value, keep=(keep,))
         self.n_colors = self.plan.info()["n_colors"]
         self.eps = torch.zeros(max(self.n_colors, 1), dtype=torch.float64, device=self.device)
 
     def compute(self, x: torch.Tensor, relstep=None, absstep=None, dir=True, stream=None) -> torch.Tensor:
-        if stream is None:
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-        with torch.cuda.device(self.device):
-            L.check(L.lib().fdb_color_eps(self.plan.handle, x.data_ptr(), L.STEP_DEFAULT if relstep is None else float(relstep),
-                                          L.STEP_DEFAULT if absstep is None else float(absstep), float(dir), self.eps.data_ptr(),
-                                          C.c_void_p(stream)))
+        api._call(self.device, (), L.lib().fdb_color_eps, self.plan.handle, x.data_ptr(), *api._steps(relstep, absstep),
+                  float(dir), self.eps.data_ptr(), C.c_void_p(api._stream(stream, self.device)))
         return self.eps
 
 
@@ -773,16 +692,10 @@ class ColumnBlockJacobian:
         if self._eps_set != eps.data_ptr():
             L.check(L.lib().fdb_plan_set_external_eps(self.plan.handle, eps.data_ptr()))
             self._eps_set = eps.data_ptr()
-        if stream is None:
-            stream = torch.cuda.current_stream(self.device).cuda_stream
         base = self.values_default.data_ptr() if values_ptr is None else int(values_ptr)
-        with torch.cuda.device(self.device):
-            st = L.lib().fdb_jacobian(self.plan.handle, addr, ctx, x.data_ptr() + 8 * self.x0, base + 8 * self.p0, None,
-                                      None, L.STEP_DEFAULT, L.STEP_DEFAULT, float(dir), C.c_void_p(stream))
-        if st == L.FDB_ERR_CALLBACK and pyfn is not None and pyfn.exc is not None:
-            exc, pyfn.exc = pyfn.exc, None
-            raise exc
-        L.check(st)
+        api._call(self.device, [pyfn], L.lib().fdb_jacobian, self.plan.handle, addr, ctx, x.data_ptr() + 8 * self.x0,
+                  base + 8 * self.p0, None, None, L.STEP_DEFAULT, L.STEP_DEFAULT, float(dir),
+                  C.c_void_p(api._stream(stream, self.device)))
 
 
 class ColumnShardedJacobian:
@@ -801,46 +714,28 @@ class ColumnShardedJacobian:
         self.block = ColumnBlockJacobian(J, colorvec, fdtype, self.bounds[self.rank], self.bounds[self.rank + 1], device,
                                          f_factory, max_batch=max_batch, use_graph=use_graph)
         self.flag = torch.zeros(1, dtype=torch.float32, device=self.device)
-        self._ipc: Optional[IpcBuffer] = None
-        self._root_ptr = None
+        self._root: Optional[_RootValues] = None
         self.barrier: Optional[DeviceBarrier] = None
         if gather == "root":
             self.barrier = DeviceBarrier(self.device, group)
-            handles = [None] * self.world
-            mine = None
-            if self.rank == 0:
-                self._ipc = IpcBuffer(J.nzval.numel(), self.device)
-                self._ipc.tensor.copy_(J.nzval)
-                J.nzval = self._ipc.tensor
-                self.block.values_default = J.nzval
-                mine = self._ipc.handle()
-            dist.all_gather_object(handles, mine, group=group)
-            if self.rank != 0:
-                p = C.c_void_p()
-                with torch.cuda.device(self.device):
-                    L.check(L.lib().fdb_ipc_open(handles[0], C.byref(p)))
-                self._root_ptr = p.value
+            self._root = _RootValues(J, self.device, self.rank, self.world, group)
+            self.block.values_default = J.nzval
 
     def run(self, x: torch.Tensor, dir=True):
         eps = self.eps_plan.compute(x, dir=dir)
         if self.gather == "root":
             self.barrier.wait()                               # rank 0 is done reading the previous J
-        self.block.run(x, eps, values_ptr=self._root_ptr, dir=dir)
+        self.block.run(x, eps, values_ptr=None if self._root is None else self._root.ptr, dir=dir)
         if self.gather == "root":
             self.barrier.wait()                               # every block (incl. its NVLink stores) has completed
 
     def close(self):
         torch.cuda.synchronize(self.device)
-        if self._root_ptr:
-            with torch.cuda.device(self.device):
-                L.lib().fdb_ipc_close(C.c_void_p(self._root_ptr))
-            self._root_ptr = None
         if self.barrier is not None:
             self.barrier.close()
             self.barrier = None
-        try:
-            dist.barrier(group=self.group)
-        except Exception:
-            pass
-        if self._ipc is not None:
-            self._ipc.free()
+        if self._root is not None:
+            self._root.close()
+            self._root = None
+        else:
+            _barrier(self.group)
