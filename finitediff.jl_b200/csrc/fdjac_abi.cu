@@ -249,12 +249,10 @@ struct fdb_plan {
   fdb_counters_t cnt{};
   int64_t alg_bytes = 0;
   int64_t last_eps_count = 0;
-  bool complex_entry = false;   // set while fdb_jacobian_complex drives the call
   // out-of-place Jacobian plans (fdjac_oop.cuh): the colour loop with pristine points and the forward step rule in central
   // mode, then the result form of the out-of-place finite_difference_jacobian
   int oop = 0;                  // 1: an out-of-place plan (fdb_jacobian rejects it)
   int oop_kind = 0;             // FDB_OOP_RAW / FDB_OOP_DENSE / FDB_OOP_SPARSE
-  bool oop_entry = false;       // set while fdb_jacobian_oop drives the call
   int64_t oop_ncols = 0;        // columns of the result
   int64_t oop_qcols = 0;        // dense branch: columns holding quotients, maximum(colorvec), over every rank
   const int64_t *oop_dest = nullptr;   // dense result of a CSC sparsity: the slots of this rank's colours (dest when world = 1)
@@ -340,6 +338,69 @@ template <typename F> static fdb_status dispatch_ct(int bits, F &&fn) {
 template <typename CT, typename F> static fdb_status dispatch_colors(const fdb_plan *P, F &&fn) {
   if (P->cyclic) return fn(CyclicColors{make_fastdiv((uint32_t)P->C)});
   return fn(TableColors<CT>{(const CT *)P->jcolor});
+}
+
+// fn(tag) with the compile-time difference mode (kForward / kCentral / kComplex) of a plan's fdtype as decltype(tag)::value
+template <typename F> static fdb_status dispatch_mode(int fdtype, F &&fn) {
+  if (fdtype == FDB_CENTRAL) return fn(std::integral_constant<int, kCentral>{});
+  if (fdtype == FDB_COMPLEX) return fn(std::integral_constant<int, kComplex>{});
+  return fn(std::integral_constant<int, kForward>{});
+}
+
+// ------------------------------------------------------------------------------------------------ which calls a plan takes
+// The compute and query calls whose acceptance depends on the plan.  fdb_jacobian_host is checked as fdb_jacobian,
+// fdb_jvp_oop as fdb_jvp; a group call checks the group's member 0.
+enum class Call {
+  jacobian, jacobian_complex, jacobian_oop, jacobian_oop_complex, color_eps, set_external_eps, set_peers, color_owner,
+  get_eps, jvp, hessian, derivative, derivative_complex, group_jacobian, group_jacobian_oop, group_hessian
+};
+
+// FDB_OK when plan P takes call c, else the refusal (its status and fdb_last_error() text): the one statement of the
+// rule, listed per call in include/fdjac_b200.h.  The first refusal that applies is returned.  Every entry point checks
+// before it allocates, launches or calls f.
+static fdb_status check_call(const fdb_plan *P, Call c) {
+  using K = Call;
+  const int k = P->sp_kind;
+  const bool cplx = P->fdtype == FDB_COMPLEX;
+  const bool colored = k == SP_CSC || k == SP_COO || k == SP_BANDED || k == SP_BLOCKBAND;   // coloured Jacobian plans
+  const bool jac = c == K::jacobian || c == K::jacobian_complex, oop = c == K::jacobian_oop || c == K::jacobian_oop_complex;
+  const bool group = c == K::group_jacobian || c == K::group_jacobian_oop;
+  const fdb_status INV = FDB_ERR_INVALID;
+  if (c == K::jacobian_complex && !cplx) return fail(INV, "fdb_jacobian_complex needs a plan created with fdtype = FDB_COMPLEX");
+  if (jac && k == SP_JVP) return fail(INV, "this is a JVP plan: call fdb_jvp");
+  if (jac && k == SP_EPS) return fail(INV, "this is a step-size plan: call fdb_color_eps");
+  if (jac && k == SP_HESS) return fail(INV, "this is a Hessian plan: call fdb_hessian");
+  if (jac && k == SP_DERIV) return fail(INV, "this is a derivative plan: call fdb_derivative");
+  if (jac && P->oop) return fail(INV, "this is an out-of-place plan: call fdb_jacobian_oop");
+  if (c == K::jacobian && cplx)
+    return fail(INV, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
+  if (c == K::jacobian_oop && cplx)
+    return fail(INV, "this plan is a complex-step plan: call fdb_jacobian_oop_complex with a complex128 callback");
+  if (c == K::jacobian_oop_complex && !cplx)
+    return fail(INV, "fdb_jacobian_oop_complex needs a plan created with fdtype = FDB_COMPLEX");
+  if (oop && !P->oop) return fail(INV, "not an out-of-place plan (fdb_oop_plan_create_csc / _dense)");
+  if (c == K::color_eps && !colored && k != SP_EPS) return fail(INV, "fdb_color_eps needs a coloured plan");
+  if (c == K::set_external_eps && !colored) return fail(INV, "external step sizes apply to coloured Jacobian plans");
+  if (c == K::set_peers && k != SP_CSC && k != SP_COO && k != SP_JVP && k != SP_EPS)
+    return fail(FDB_ERR_UNSUPPORTED, "peer stores are implemented for the entry-driven (CSC / COO) scatters");
+  if (c == K::color_owner && (k == SP_NONE || k == SP_HESS)) return fail(INV, "dense plans partition columns by range");
+  if (c == K::color_owner && k == SP_DERIV) return fail(INV, "derivative plans have no colours");
+  if (c == K::get_eps && k == SP_DERIV)
+    return fail(INV, "derivative plans keep no step sizes (the quotient pass recomputes them)");
+  if (c == K::jvp && k != SP_JVP) return fail(INV, "not a JVP plan (fdb_jvp_plan_create)");
+  if (c == K::hessian && k != SP_HESS) return fail(INV, "not a Hessian plan (fdb_hessian_plan_create)");
+  if (c == K::derivative && k != SP_DERIV)
+    return fail(INV, "not a derivative plan (fdb_derivative_plan_create / fdb_scalar_gradient_plan_create)");
+  if (c == K::derivative && cplx)
+    return fail(INV, "this plan is a complex-step plan: call fdb_derivative_complex with a complex128 callback");
+  if (c == K::derivative_complex && (k != SP_DERIV || !cplx))
+    return fail(INV, "fdb_derivative_complex needs a derivative plan created with fdtype = FDB_COMPLEX");
+  if (c == K::group_jacobian && k == SP_HESS) return fail(INV, "this is a Hessian group: call fdb_group_hessian");
+  if (c == K::group_jacobian && P->oop) return fail(INV, "this is an out-of-place group: call fdb_group_jacobian_oop");
+  if (c == K::group_jacobian_oop && !P->oop) return fail(INV, "not an out-of-place group (fdb_group_create_oop_csc / _dense)");
+  if (group && cplx) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
+  if (c == K::group_hessian && k != SP_HESS) return fail(INV, "not a Hessian group (fdb_group_create_hessian)");
+  return FDB_OK;
 }
 
 static const char *plan_err_text(uint32_t e) {
@@ -1333,8 +1394,7 @@ fdb_status fdb_plan_dense_range(const fdb_plan *P, int64_t *b, int64_t *e) {
 
 fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t cap) {
   if (!P || !owner_out) return fail(FDB_ERR_INVALID, "NULL argument");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "dense plans partition columns by range");
-  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "derivative plans have no colours");
+  TRY(check_call(P, Call::color_owner));
   if (cap < (int64_t)P->owner.size()) return fail(FDB_ERR_INVALID, "owner_out too small");
   std::copy(P->owner.begin(), P->owner.end(), owner_out);
   return FDB_OK;
@@ -1342,7 +1402,7 @@ fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t c
 
 fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *stream) {
   if (!P || !h_eps) return fail(FDB_ERR_INVALID, "NULL argument");
-  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "derivative plans keep no step sizes (the quotient pass recomputes them)");
+  TRY(check_call(P, Call::get_eps));
   DeviceGuard g(P->device);
   // JVP plans: C == 1; Hessian plans: the steps of the rank's components [col_begin, col_end) (eps_cols holds all n)
   const bool per_column = P->sp_kind == SP_NONE || P->sp_kind == SP_HESS;
@@ -1384,9 +1444,7 @@ fdb_status fdb_plan_read_timing(fdb_plan *P, double *scatter_ms, int64_t *scatte
 fdb_status fdb_plan_set_peers(fdb_plan *P, int n_peers, double *const *peer_J) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
   if (n_peers < 0 || n_peers > 64) return fail(FDB_ERR_INVALID, "n_peers out of range");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_BANDED || P->sp_kind == SP_BLOCKBAND || P->sp_kind == SP_HESS ||
-      P->sp_kind == SP_DERIV)
-    return fail(FDB_ERR_UNSUPPORTED, "peer stores are implemented for the entry-driven (CSC / COO) scatters");
+  TRY(check_call(P, Call::set_peers));
   DeviceGuard g(P->device);
   if (!P->d_peers) TRY(P->alloc_t(&P->d_peers, 64));
   if (n_peers > 0) CU(cudaMemcpy(P->d_peers, peer_J, (size_t)n_peers * sizeof(double *), cudaMemcpyHostToDevice));
@@ -1429,6 +1487,17 @@ static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
   }
   CU(cudaMemsetAsync(J, 0, (size_t)P->j_len * 8, s));
   return FDB_OK;
+}
+
+// fill_matrix!(J, false) (jacobians.jl:530-532) is needed unless the scatter launches over `colours` colours (one rank's
+// or a whole group's) define every slot of J themselves, zeros for the columns without a valid colour included:
+// block-banded launches always do; identity CSC (nzval), band-data and diagonal-storage launches do once there is a
+// colour to launch for.
+static bool scatter_defines_J(const fdb_plan *P, int64_t colours) {
+  if (P->sp_kind == SP_BLOCKBAND) return true;
+  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
+  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || P->jkind == FDB_J_DIAGONALS);
+  return (ident || band_data) && colours > 0;
 }
 
 static fdb_status call_f(fdb_plan *P, fdb_fn f, void *ctx, double *fx, const double *x, int64_t batch, cudaStream_t s) {
@@ -1532,17 +1601,12 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   // strides, in doubles, of one f! output slab / one perturbed point (complex128 in complex-step mode)
   const int64_t sF = COMPLEX ? 2 * P->ldF : P->ldF, sX = COMPLEX ? 2 * P->ldx : P->ldx;
   const int64_t n_local = (int64_t)P->local_colors.size();
-  // fill_matrix!(J, false)  jacobians.jl:530-532 — needed where the scatter does not define every slot itself
   const bool block_band = P->sp_kind == SP_BLOCKBAND;
   const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED && !block_band;
   const bool diag_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_DIAGONALS;
-  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || diag_data);
-  // (identity / band-data / diagonal-storage launches define every slot this rank is responsible for, including zeros
-  //  for columns without a valid colour; block-banded launches do so even when the rank has no colour).  With peer
-  //  buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race with the
-  //  peers' stores.
-  const bool self_defining = block_band || ((ident || band_data) && n_local > 0);
-  if (!self_defining && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
+  // With peer buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race
+  // with the peers' stores.
+  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
   auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
       for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
@@ -1995,30 +2059,18 @@ extern "C" {
 
 static fdb_status jacobian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_J, double *fx,
                                  const double *d_f_in, double relstep, double absstep, double dir, cudaStream_t s) {
-  if (P->sp_kind == SP_NONE) {
-    if (P->fdtype == FDB_CENTRAL) return run_dense<kCentral>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-    if (P->fdtype == FDB_COMPLEX) return run_dense<kComplex>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-    return run_dense<kForward>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-  }
-  return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-    using CT = decltype(tag);
-    if (P->fdtype == FDB_CENTRAL) return run_colored<CT, kCentral>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-    if (P->fdtype == FDB_COMPLEX) return run_colored<CT, kComplex>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-    return run_colored<CT, kForward>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
+  return dispatch_mode(P->fdtype, [&](auto mode) -> fdb_status {
+    constexpr int MODE = decltype(mode)::value;
+    if (P->sp_kind == SP_NONE) return run_dense<MODE>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
+    return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+      return run_colored<decltype(tag), MODE>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
+    });
   });
 }
 
-fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_J, double *d_fx,
-                        const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
-  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if ((P->n > 0 && !d_x) || (P->j_len > 0 && !d_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
-  if (P->sp_kind == SP_JVP) return fail(FDB_ERR_INVALID, "this is a JVP plan: call fdb_jvp");
-  if (P->sp_kind == SP_EPS) return fail(FDB_ERR_INVALID, "this is a step-size plan: call fdb_color_eps");
-  if (P->sp_kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian plan: call fdb_hessian");
-  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "this is a derivative plan: call fdb_derivative");
-  if (P->oop && !P->oop_entry) return fail(FDB_ERR_INVALID, "this is an out-of-place plan: call fdb_jacobian_oop");
-  if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
-    return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
+// A Jacobian call once check_call has accepted it (the complex, host-buffer, out-of-place and group entries included)
+static fdb_status jacobian_run(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_J, double *d_fx,
+                               const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
   cudaStream_t s = (cudaStream_t)stream;
@@ -2033,14 +2085,21 @@ fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, dou
   return st;
 }
 
+fdb_status fdb_jacobian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_J, double *d_fx,
+                        const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
+  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  if ((P->n > 0 && !d_x) || (P->j_len > 0 && !d_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
+  TRY(check_call(P, Call::jacobian));
+  return jacobian_run(P, f, ctx, d_x, d_J, d_fx, d_f_in, relstep, absstep, dir, stream);
+}
+
 fdb_status fdb_jacobian_complex(fdb_plan *P, fdb_fn_c f, void *ctx, const double *d_x, double *d_J, void *stream) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->fdtype != FDB_COMPLEX) return fail(FDB_ERR_INVALID, "fdb_jacobian_complex needs a plan created with fdtype = FDB_COMPLEX");
+  TRY(check_call(P, Call::jacobian_complex));
+  if ((P->n > 0 && !d_x) || (P->j_len > 0 && !d_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   // same C signature up to the element type of the buffers: the complex128 slabs are handed over as raw pointers
-  P->complex_entry = true;
-  const fdb_status st = fdb_jacobian(P, reinterpret_cast<fdb_fn>(f), ctx, d_x, d_J, nullptr, nullptr, FDB_STEP_DEFAULT, FDB_STEP_DEFAULT, 1.0, stream);
-  P->complex_entry = false;
-  return st;
+  return jacobian_run(P, reinterpret_cast<fdb_fn>(f), ctx, d_x, d_J, nullptr, nullptr, FDB_STEP_DEFAULT, FDB_STEP_DEFAULT,
+                      1.0, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ step sizes on their own
@@ -2064,8 +2123,7 @@ fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorv
 fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double absstep, double dir, double *d_eps_out,
                          void *stream) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_HESS || P->sp_kind == SP_DERIV)
-    return fail(FDB_ERR_INVALID, "fdb_color_eps needs a coloured plan");
+  TRY(check_call(P, Call::color_eps));
   if (P->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -2081,9 +2139,7 @@ fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double 
 
 fdb_status fdb_plan_set_external_eps(fdb_plan *P, const double *d_eps) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  if (P->sp_kind == SP_NONE || P->sp_kind == SP_JVP || P->sp_kind == SP_EPS || P->sp_kind == SP_HESS ||
-      P->sp_kind == SP_DERIV)
-    return fail(FDB_ERR_INVALID, "external step sizes apply to coloured Jacobian plans");
+  TRY(check_call(P, Call::set_external_eps));
   P->ext_eps = d_eps;
   return FDB_OK;
 }
@@ -2120,7 +2176,7 @@ static fdb_status jvp_run(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const
                           double *d_fx1, const double *d_f_in, double relstep, double absstep, double dir, void *stream,
                           bool plus_first) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->sp_kind != SP_JVP) return fail(FDB_ERR_INVALID, "not a JVP plan (fdb_jvp_plan_create)");
+  TRY(check_call(P, Call::jvp));
   if ((P->n > 0 && (!d_x || !d_v)) || (P->m > 0 && !d_jvp)) return fail(FDB_ERR_INVALID, "NULL jvp, x or v");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -2315,7 +2371,7 @@ static fdb_status hessian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *
 fdb_status fdb_hessian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, double *d_H, double *d_fx, double relstep,
                        double absstep, void *stream) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->sp_kind != SP_HESS) return fail(FDB_ERR_INVALID, "not a Hessian plan (fdb_hessian_plan_create)");
+  TRY(check_call(P, Call::hessian));
   if (P->n > 0 && (!d_x || !d_H)) return fail(FDB_ERR_INVALID, "NULL x or H");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -2429,13 +2485,9 @@ static fdb_status derivative_eager(fdb_plan *P, fdb_fn f, void *ctx, double *df,
 
 extern "C" {
 
-fdb_status fdb_derivative(fdb_plan *P, fdb_fn f, void *ctx, double *d_df, const double *d_x, const double *d_fx,
-                          double relstep, double absstep, double dir, void *stream) {
-  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->sp_kind != SP_DERIV)
-    return fail(FDB_ERR_INVALID, "not a derivative plan (fdb_derivative_plan_create / fdb_scalar_gradient_plan_create)");
-  if (P->fdtype == FDB_COMPLEX && !P->complex_entry)
-    return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_derivative_complex with a complex128 callback");
+// A derivative call once check_call has accepted it
+static fdb_status derivative_run(fdb_plan *P, fdb_fn f, void *ctx, double *d_df, const double *d_x, const double *d_fx,
+                                 double relstep, double absstep, double dir, void *stream) {
   if ((P->n > 0 && !d_x) || (P->m > 0 && !d_df)) return fail(FDB_ERR_INVALID, "NULL x or df");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -2445,29 +2497,32 @@ fdb_status fdb_derivative(fdb_plan *P, fdb_fn f, void *ctx, double *d_df, const 
   const DerivSteps st{relstep, absstep, dir};
   const GraphKey key{(void *)f, ctx, d_x, d_df, fx, nullptr, relstep, absstep, dir, 0, 0, nullptr};
   const fdb_status rc = run_maybe_graph(P, key, s, "derivative", [&](cudaStream_t cs) {
-    if (P->fdtype == FDB_CENTRAL) return derivative_eager<kCentral>(P, f, ctx, d_df, d_x, fx, st, cs);
-    if (P->fdtype == FDB_COMPLEX) return derivative_eager<kComplex>(P, f, ctx, d_df, d_x, fx, st, cs);
-    return derivative_eager<kForward>(P, f, ctx, d_df, d_x, fx, st, cs);
+    return dispatch_mode(P->fdtype, [&](auto mode) {
+      return derivative_eager<decltype(mode)::value>(P, f, ctx, d_df, d_x, fx, st, cs);
+    });
   });
   if (rc == FDB_OK) P->cnt.jacobians += 1;
   return rc;
 }
 
+fdb_status fdb_derivative(fdb_plan *P, fdb_fn f, void *ctx, double *d_df, const double *d_x, const double *d_fx,
+                          double relstep, double absstep, double dir, void *stream) {
+  if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
+  TRY(check_call(P, Call::derivative));
+  return derivative_run(P, f, ctx, d_df, d_x, d_fx, relstep, absstep, dir, stream);
+}
+
 fdb_status fdb_derivative_complex(fdb_plan *P, fdb_fn_c f, void *ctx, double *d_df, const double *d_x, void *stream) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->sp_kind != SP_DERIV || P->fdtype != FDB_COMPLEX)
-    return fail(FDB_ERR_INVALID, "fdb_derivative_complex needs a derivative plan created with fdtype = FDB_COMPLEX");
-  P->complex_entry = true;
-  const fdb_status st = fdb_derivative(P, reinterpret_cast<fdb_fn>(f), ctx, d_df, d_x, nullptr, FDB_STEP_DEFAULT,
-                                       FDB_STEP_DEFAULT, 1.0, stream);
-  P->complex_entry = false;
-  return st;
+  TRY(check_call(P, Call::derivative_complex));
+  return derivative_run(P, reinterpret_cast<fdb_fn>(f), ctx, d_df, d_x, nullptr, FDB_STEP_DEFAULT, FDB_STEP_DEFAULT, 1.0,
+                        stream);
 }
 
 fdb_status fdb_jacobian_host(fdb_plan *P, fdb_fn f, void *ctx, const double *h_x, double *h_J, double *h_fx,
                              const double *h_f_in, double relstep, double absstep, double dir) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->sp_kind == SP_DERIV) return fail(FDB_ERR_INVALID, "this is a derivative plan: call fdb_derivative");
+  TRY(check_call(P, Call::jacobian));
   if ((P->n > 0 && !h_x) || (P->j_len > 0 && !h_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
@@ -2485,7 +2540,7 @@ fdb_status fdb_jacobian_host(fdb_plan *P, fdb_fn f, void *ctx, const double *h_x
     CU(cudaMemcpyAsync(P->h_dfin, h_f_in, (size_t)P->m * 8, cudaMemcpyHostToDevice, s));
     fin = P->h_dfin;
   }
-  fdb_status st = fdb_jacobian(P, f, ctx, P->h_dx, P->h_dJ, P->h_dfx, fin, relstep, absstep, dir, (void *)s);
+  fdb_status st = jacobian_run(P, f, ctx, P->h_dx, P->h_dJ, P->h_dfx, fin, relstep, absstep, dir, (void *)s);
   if (st != FDB_OK) { cudaStreamSynchronize(s); return st; }
   if (P->j_len > 0) {
     if (P->jkind == FDB_J_DENSE && P->ldJ > P->m) {

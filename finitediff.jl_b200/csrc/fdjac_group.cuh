@@ -46,9 +46,7 @@ sync_barrier_kernel(unsigned long long *const *__restrict__ peer_flags, unsigned
 // ------------------------------------------------------------------------------------------------ single-process group
 struct fdb_group {
   int n = 0;
-  int kind = SP_CSC;
-  bool oop = false;                      // out-of-place Jacobian members (fdb_group_create_oop_*)
-  std::vector<fdb_plan *> plans;
+  std::vector<fdb_plan *> plans;         // the calls a group accepts are those check_call accepts for member 0
   std::vector<int> devices;
   std::vector<cudaStream_t> streams;     // members > 0 (index 0 unused: the root runs on the caller's stream)
   std::vector<cudaEvent_t> ev_done;
@@ -56,16 +54,6 @@ struct fdb_group {
   std::vector<double *> x_rep, fin_rep;  // x / f_in replicas on members living on another device than the root
   int64_t nx = 0, m = 0;
 };
-
-static bool plan_self_defining(const fdb_plan *P) {
-  // the scatter launches of all ranks together define every slot of J (identity CSC: nzval; band data: whole columns;
-  // diagonal storage: every stored slot of every column)
-  // (block-banded: every column, including those without a valid colour, whatever the colour count)
-  if (P->sp_kind == SP_BLOCKBAND) return true;
-  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
-  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || P->jkind == FDB_J_DIAGONALS);
-  return (ident || band_data) && P->C > 0;
-}
 
 static void free_group(fdb_group *g) {
   if (!g) return;
@@ -139,8 +127,6 @@ static fdb_status group_create(fdb_group **out, int n_devices, const int *device
   }
   g->nx = g->plans[0]->n;
   g->m = g->plans[0]->m;
-  g->kind = g->plans[0]->sp_kind;
-  g->oop = g->plans[0]->oop != 0;
   *out = g.release();
   return FDB_OK;
 }
@@ -249,10 +235,8 @@ fdb_status fdb_group_create_hessian(fdb_group **group, int n_devices, const int 
 fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const double *d_x, double *d_J, double *d_fx,
                               const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
   if (!g || !f) return fail(FDB_ERR_INVALID, "NULL group or f");
-  if (g->kind == SP_HESS) return fail(FDB_ERR_INVALID, "this is a Hessian group: call fdb_group_hessian");
-  if (g->oop) return fail(FDB_ERR_INVALID, "this is an out-of-place group: call fdb_group_jacobian_oop");
   fdb_plan *P0 = g->plans[0];
-  if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
+  TRY(check_call(P0, Call::group_jacobian));
   // J may be NULL only when no member has a slot to write (as fdb_jacobian allows; e.g. an empty gradient, n = 0)
   bool writes_J = false;
   for (const fdb_plan *P : g->plans) writes_J = writes_J || P->j_len > 0;
@@ -262,22 +246,23 @@ fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const do
   {
     DeviceGuard dg(root);
     if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
-    // fill_matrix!(J, false) once, by the owner of the buffer, before any member may store into it
-    if (g->n > 1 && P0->sp_kind != SP_NONE && !plan_self_defining(P0) && P0->j_len > 0) TRY(zero_J(P0, d_J, s0));
+    // fill_matrix!(J, false) once, by the owner of the buffer, before any member may store into it (the members of a
+    // dense group write whole column blocks)
+    if (g->n > 1 && P0->sp_kind != SP_NONE && !scatter_defines_J(P0, P0->C) && P0->j_len > 0) TRY(zero_J(P0, d_J, s0));
   }
   return group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {
     fdb_plan *P = g->plans[i];
     const double *fin_i = d_f_in;
     if (i > 0 && d_f_in && P->fdtype == FDB_FORWARD) TRY(member_replica(g, i, g->fin_rep, d_f_in, g->m, s, &fin_i));
     double *Ji = P->sp_kind == SP_NONE ? d_J + P->col_begin * P->ldJ : d_J;
-    return fdb_jacobian(P, f, ctx ? ctx[i] : nullptr, xi, Ji, i == 0 ? d_fx : nullptr, fin_i, relstep, absstep, dir, (void *)s);
+    return jacobian_run(P, f, ctx ? ctx[i] : nullptr, xi, Ji, i == 0 ? d_fx : nullptr, fin_i, relstep, absstep, dir, (void *)s);
   }, [](int) { return false; });
 }
 
 fdb_status fdb_group_hessian(fdb_group *g, fdb_fn f, void *const *ctx, const double *d_x, double *d_H, double *d_fx,
                              double relstep, double absstep, void *stream) {
   if (!g || !f) return fail(FDB_ERR_INVALID, "NULL group or f");
-  if (g->kind != SP_HESS) return fail(FDB_ERR_INVALID, "not a Hessian group (fdb_group_create_hessian)");
+  TRY(check_call(g->plans[0], Call::group_hessian));
   if (g->nx > 0 && (!d_x || !d_H)) return fail(FDB_ERR_INVALID, "NULL x or H");
   // every member stores the entries of its i-blocks straight into the root's H; only the root reports f(x)
   return group_run(g, d_x, (cudaStream_t)stream, [&](int i, const double *xi, cudaStream_t s) {

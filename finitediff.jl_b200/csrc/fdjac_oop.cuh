@@ -176,10 +176,8 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
   // a sparse result whose colorvec has no valid colour: nobody scatters, and the candidates are the zeros of rank 0
   if (P->oop_kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->local_colors.empty() && P->E > 0)
     CU(cudaMemsetAsync(J, 0, (size_t)P->E * 8, s));
-  P->oop_entry = true;
-  const fdb_status st = fdb_jacobian(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, (void *)s);
-  P->oop_entry = false;
-  TRY(st);
+  if ((P->n > 0 && !d_x) || (P->j_len > 0 && !J)) return fail(FDB_ERR_INVALID, "NULL x or J");
+  TRY(jacobian_run(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, (void *)s));
   if (P->oop_kind == FDB_OOP_DENSE) {
     if (!full && P->oop_dest_n > 0) {
       oop_plus_zero_slots<<<P->grid(P->oop_dest_n), kThreads, 0, s>>>(J, P->oop_dest, P->oop_dest_n);
@@ -226,22 +224,20 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
   auto go = [&](auto kern) { kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a); };
   if (full) go(oop_compact<true, kCopy, uint8_t>);
   else if (!P->oop_fused) go(oop_compact<false, kCopy, uint8_t>);
-  else TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
-    using CT = decltype(tag);
-    if (P->fdtype == FDB_CENTRAL) go(oop_compact<false, kCentral, CT>);
-    else if (P->fdtype == FDB_COMPLEX) go(oop_compact<false, kComplex, CT>);
-    else go(oop_compact<false, kForward, CT>);
-    return FDB_OK;
+  else TRY(dispatch_mode(P->fdtype, [&](auto mode) {
+    return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+      go(oop_compact<false, decltype(mode)::value, decltype(tag)>);
+      return FDB_OK;
+    });
   }));
   P->cnt.kernel_launches += 1;
   CU(cudaGetLastError());
   return FDB_OK;
 }
 
+// An out-of-place call once check_call has accepted it
 static fdb_status jacobian_oop_run(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                                    const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
-  if (!P || !f || !out) return fail(FDB_ERR_INVALID, "NULL plan, f or out");
-  if (!P->oop) return fail(FDB_ERR_INVALID, "not an out-of-place plan (fdb_oop_plan_create_csc / _dense)");
   const bool sparse = P->oop_kind == FDB_OOP_SPARSE;
   if (sparse && P->world > 1)
     return fail(FDB_ERR_INVALID, "a sparse result is compacted over every rank's candidates on one device: run sparse rank "
@@ -258,20 +254,18 @@ extern "C" {
 
 fdb_status fdb_jacobian_oop(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
-  if (P && P->fdtype == FDB_COMPLEX)
-    return fail(FDB_ERR_INVALID, "this plan is a complex-step plan: call fdb_jacobian_oop_complex with a complex128 callback");
+  if (!P || !f || !out) return fail(FDB_ERR_INVALID, "NULL plan, f or out");
+  TRY(check_call(P, Call::jacobian_oop));
   return jacobian_oop_run(P, f, ctx, d_x, out, d_fx, d_f_in, relstep, absstep, dir, stream);
 }
 
 fdb_status fdb_jacobian_oop_complex(fdb_plan *P, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
                                     void *stream) {
   if (!P || !f) return fail(FDB_ERR_INVALID, "NULL plan or f");
-  if (P->fdtype != FDB_COMPLEX) return fail(FDB_ERR_INVALID, "fdb_jacobian_oop_complex needs a plan created with fdtype = FDB_COMPLEX");
-  P->complex_entry = true;
-  const fdb_status st = jacobian_oop_run(P, reinterpret_cast<fdb_fn>(f), ctx, d_x, out, nullptr, nullptr, FDB_STEP_DEFAULT,
-                                         FDB_STEP_DEFAULT, 1.0, stream);
-  P->complex_entry = false;
-  return st;
+  TRY(check_call(P, Call::jacobian_oop_complex));
+  if (!out) return fail(FDB_ERR_INVALID, "NULL plan, f or out");
+  return jacobian_oop_run(P, reinterpret_cast<fdb_fn>(f), ctx, d_x, out, nullptr, nullptr, FDB_STEP_DEFAULT, FDB_STEP_DEFAULT,
+                          1.0, stream);
 }
 
 fdb_status fdb_jvp_oop(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const double *d_x, const double *d_v, double *d_x1,
@@ -300,9 +294,8 @@ fdb_status fdb_group_jacobian_oop(fdb_group *g, fdb_fn f, void *const *ctx, cons
                                   double *d_fx, const double *d_f_in, double relstep, double absstep, double dir,
                                   void *stream) {
   if (!g || !f || !out) return fail(FDB_ERR_INVALID, "NULL group, f or out");
-  if (!g->oop) return fail(FDB_ERR_INVALID, "not an out-of-place group (fdb_group_create_oop_csc / _dense)");
   fdb_plan *P0 = g->plans[0];
-  if (P0->fdtype == FDB_COMPLEX) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
+  TRY(check_call(P0, Call::group_jacobian_oop));
   if (P0->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
   const bool sparse = P0->oop_kind == FDB_OOP_SPARSE;
   if (!sparse && P0->j_len > 0 && !out->J) return fail(FDB_ERR_INVALID, "NULL x or J");

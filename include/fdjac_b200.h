@@ -151,6 +151,27 @@ double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep,
 /* ---- plans: the per-(pattern, colorvec, fdtype) state the reference rebuilds on every call
  *      (jacobians.jl:515-535: colour reshape, findstructralnz, same-pattern test) ---- */
 
+/* Which plans each call takes.  Coloured plans: fdb_plan_create_csc / _coo / _banded / _block_banded; dense plans:
+ * fdb_plan_create_dense / _dense_colorvec; out-of-place plans: fdb_oop_plan_create_*.  Any other plan is refused with
+ * FDB_ERR_INVALID (FDB_ERR_UNSUPPORTED where noted) before the call allocates, launches or calls f.
+ *   fdb_jacobian, fdb_jacobian_host   coloured and dense plans, fdtype forward / central
+ *   fdb_jacobian_complex              coloured and dense plans, fdtype complex
+ *   fdb_jacobian_oop                  out-of-place plans, fdtype forward / central
+ *   fdb_jacobian_oop_complex          out-of-place plans, fdtype complex
+ *   fdb_color_eps                     coloured plans (out-of-place CSC included) and step-size plans
+ *   fdb_plan_set_external_eps         coloured plans (out-of-place CSC included)
+ *   fdb_plan_set_peers                CSC, COO, JVP and step-size plans (else FDB_ERR_UNSUPPORTED)
+ *   fdb_plan_color_owner              every plan but dense, Hessian and derivative plans
+ *   fdb_plan_get_eps                  every plan but derivative plans
+ *   fdb_jvp, fdb_jvp_oop              JVP plans
+ *   fdb_hessian                       Hessian plans
+ *   fdb_derivative                    derivative and scalar-gradient plans, fdtype forward / central
+ *   fdb_derivative_complex            derivative and scalar-gradient plans, fdtype complex
+ *   fdb_group_jacobian                groups of coloured or dense plans, fdtype forward / central (complex:
+ *                                     FDB_ERR_UNSUPPORTED)
+ *   fdb_group_jacobian_oop            groups of out-of-place plans, fdtype forward / central (complex: FDB_ERR_UNSUPPORTED)
+ *   fdb_group_hessian                 groups of Hessian plans */
+
 /* sparsity::SparseMatrixCSC (m x n, colptr[n+1], rowval[nnz]).
  *   jkind = FDB_J_CSC_NZVAL: J is a CSC with pattern (j_colptr, j_rowval); NULL,NULL => same arrays as the sparsity.
  *           Same pattern (ext/..SparseArraysExt.jl:51-52) => fast path nzval[p]; a different pattern is accepted when every
