@@ -1236,11 +1236,19 @@ def _native_call(f: "NativeFn", fx: torch.Tensor, x: torch.Tensor, stream):
         raise L.FdbError(L.FDB_ERR_CALLBACK, f"user f! returned {rc}")
 
 
+def _oop_band(sparsity):
+    """(l, u) of a band sparsity the out-of-place Jacobian takes in closed form (BandedMatrix with l, u >= 0, Diagonal,
+    Bidiagonal, SymTridiagonal), else None."""
+    if isinstance(sparsity, (BandedMatrix,) + _LA_BANDED) and sparsity.l >= 0 and sparsity.u >= 0:
+        return int(sparsity.l), int(sparsity.u)
+    return None
+
+
 def _oop_kind(sparsity, jac_prototype):
     """(result kind, m, ncols) the pair (sparsity, jac_prototype) gives; m / ncols None where f and colorvec decide."""
-    if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC):
+    if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC) and _oop_band(sparsity) is None:
         raise TypeError(f"not built: sparsity of type {type(sparsity).__name__} in the out-of-place Jacobian "
-                        "(SparseMatrixCSC or None)")
+                        "(SparseMatrixCSC, BandedMatrix with l, u >= 0, Diagonal, Bidiagonal, SymTridiagonal or None)")
     if jac_prototype is not None:
         if isinstance(jac_prototype, SparseMatrixCSC):
             pm, pn = jac_prototype.shape
@@ -1255,7 +1263,7 @@ def _oop_kind(sparsity, jac_prototype):
         kind = L.FDB_OOP_SPARSE if isinstance(jac_prototype, SparseMatrixCSC) else L.FDB_OOP_DENSE
         return kind, int(pm), int(pn)
     if sparsity is not None:
-        return L.FDB_OOP_DENSE, sparsity.m, sparsity.n
+        return L.FDB_OOP_DENSE, sparsity.shape[0], sparsity.shape[1]
     return L.FDB_OOP_RAW, None, None
 
 
@@ -1264,6 +1272,9 @@ def _oop_plan_route(kind, sparsity, colorvec, pn, m, n):
     fdb_oop_plan_create_<suffix>(&h, *args, &opts) (or fdb_group_create_oop_<suffix>(&h, n_devices, devices, *args,
     &opts)), and `keep` holds the host arrays the pointers in args point into."""
     cvp, k0 = _index_ptr(None if _is_identity_colorvec(colorvec, n) else colorvec)
+    band = _oop_band(sparsity)
+    if band is not None:
+        return "banded", (m, n, band[0], band[1], cvp, kind, max(m, 1)), [k0]
     if sparsity is not None:
         cp, k1 = _index_ptr(sparsity.colptr)
         rv, k2 = _index_ptr(sparsity.rowval)
@@ -1283,9 +1294,9 @@ def _oop_rows(f, x, fd, f_in, m_default, sparsity, pm, n):
         f_in = f_in.reshape(-1)
     m = f_in.numel() if f_in is not None else m_default
     if sparsity is not None:
-        m = sparsity.m
-        if sparsity.n != n:
-            raise ValueError(f"size(sparsity, 2) = {sparsity.n} != length(x) = {n}")
+        m, sn = sparsity.shape
+        if sn != n:
+            raise ValueError(f"size(sparsity, 2) = {sn} != length(x) = {n}")
     elif pm is not None and pm != m:
         raise TypeError(f"not built: a {pm}-row jac_prototype for an f with {m} values")
     return f_in, m
@@ -1353,6 +1364,9 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
         CSC / None or dense         dense size(sparsity): structural slots 0.0 + dx, +0.0 elsewhere (an invalid colouring
                                     raises, as _make_Ji throws)
         CSC / SparseMatrixCSC       SparseMatrixCSC with the structural entries whose value is not +-0.0 (NaN kept)
+        band / as for CSC           the same results for a BandedMatrix (l, u >= 0), Diagonal, Bidiagonal or SymTridiagonal
+                                    sparsity, whose structural entries are the in-matrix band (l, u): a closed-form plan
+                                    (fdb_oop_plan_create_banded) builds no entry list
     A sparse result is sized to the kept entries: reading that count is the call's one host synchronisation (when most
     candidates were dropped its rowval / nzval are copied into storage of their own size).  Other sparsity / prototype
     types and complex-valued results raise TypeError (not built).
@@ -1370,7 +1384,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
             stream = _stream(stream, x.device)
             if isinstance(f, NativeFn):
                 sp = None if sparsity is _DEFAULT else sparsity
-                m = sp.m if isinstance(sp, SparseMatrixCSC) else (
+                m = sp.shape[0] if isinstance(sp, SparseMatrixCSC) or _oop_band(sp) is not None else (
                     jac_prototype.shape[0] if jac_prototype is not None else xv.numel())
                 xin = xv.to(torch.complex128) if _fdtype_code(fd) == L.FDB_COMPLEX else xv
                 fx = torch.empty(m, dtype=xin.dtype, device=x.device)

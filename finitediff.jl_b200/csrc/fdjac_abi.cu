@@ -261,6 +261,7 @@ struct fdb_plan {
   unsigned long long *oop_state = nullptr;   // sparse result: look-back words of the compaction, then its tile counter
   int32_t *oop_tile_col = nullptr;           // sparse result of a CSC sparsity: first column starting in each tile
   bool oop_fused = false;                    // sparse result, every colour's f! output resident: quotient + compaction fused
+  int64_t oop_band_nnz = 0;                  // result of a band sparsity: |E|, every in-matrix band entry (E counts coloured ones)
   // optional CUDA-graph replay of the whole call
   bool use_graph = false;
   cudaStream_t cstream = nullptr;
@@ -1342,6 +1343,7 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   if (oop_idle(P)) info->fcalls_per_jacobian = 0;
   // out-of-place dense branch: the candidate count of the whole result (a rank's E is its own block)
   if (P->oop && P->sp_kind == SP_NONE) info->n_entries = P->m * P->oop_qcols;
+  if (P->oop && P->sp_kind == SP_BANDED) info->n_entries = P->oop_band_nnz;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
   info->jkind = P->jkind;
@@ -1606,7 +1608,9 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   const bool diag_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_DIAGONALS;
   // With peer buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race
   // with the peers' stores.
-  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
+  // (an out-of-place plan with a fused compaction stores no candidate: its candidate buffer is not J-sized)
+  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && !P->oop_fused && P->j_len > 0)
+    TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
   auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
       for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {

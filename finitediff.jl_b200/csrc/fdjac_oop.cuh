@@ -10,8 +10,9 @@
 // every candidate (oop_root_finish) once every member has finished.
 #include "kernels_oop.cuh"
 
-static fdb_status oop_alloc_sparse(fdb_plan *P, int64_t candidates) {
-  TRY(P->alloc_t(&P->oop_vals, (size_t)std::max<int64_t>(candidates, 2)));
+// `vals`: doubles of the candidate buffer the colour loop writes (the band data of a band sparsity)
+static fdb_status oop_alloc_sparse(fdb_plan *P, int64_t candidates, int64_t vals) {
+  TRY(P->alloc_t(&P->oop_vals, (size_t)std::max<int64_t>(vals, 2)));
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
   TRY(P->alloc_t(&P->oop_state, (size_t)ntiles + 1));
   return FDB_OK;
@@ -55,8 +56,12 @@ static fdb_status oop_own_slots(fdb_plan *P) {
 
 // candidates of the whole result: nnz of the sparsity, or m x maximum(colorvec) on the dense branch
 static int64_t oop_candidates(const fdb_plan *P) {
+  if (P->sp_kind == SP_BANDED) return P->oop_band_nnz;
   return P->sp_kind == SP_NONE ? P->m * P->oop_qcols : P->E;
 }
+
+// the entry set of a band plan (its bandwidths are clamped to the matrix at creation)
+static BandShape oop_band_shape(const fdb_plan *P) { return make_band_shape(P->m, P->n, P->l, P->u); }
 
 extern "C" {
 
@@ -88,7 +93,7 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
   P->oop_ncols = n;
   if (result_kind == FDB_OOP_DENSE) TRY(oop_own_slots(P));
   if (result_kind == FDB_OOP_SPARSE && P->rank == 0) {   // the candidate buffer and the compaction are the root's
-    TRY(oop_alloc_sparse(P, P->E));
+    TRY(oop_alloc_sparse(P, P->E, P->E));
     // one group of resident f! outputs on one rank: the compaction forms the quotients itself, no candidate is stored
     P->oop_fused = P->n_groups <= 1 && P->world == 1;
     const int64_t ntiles = (P->E + kTile - 1) / kTile;
@@ -98,6 +103,64 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
       CU(cudaGetLastError());
       CU(cudaDeviceSynchronize());
     }
+  }
+  *plan = owner.release();
+  return FDB_OK;
+}
+
+fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, const int64_t *colorvec,
+                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  if (result_kind != FDB_OOP_DENSE && result_kind != FDB_OOP_SPARSE)
+    return fail(FDB_ERR_INVALID, "a banded sparsity gives a dense (FDB_OOP_DENSE) or a sparse (FDB_OOP_SPARSE) result");
+  if (n == 0) return fail(FDB_ERR_INVALID, "maximum(colorvec) of an empty colorvec: the reference throws");
+  if (m < 0 || n < 0) return fail(FDB_ERR_INVALID, "negative dimensions m=%lld n=%lld", (long long)m, (long long)n);
+  if (l < 0 || u < 0)
+    return fail(FDB_ERR_UNSUPPORTED, "not built: negative bandwidths (l, u) = (%lld, %lld) in the out-of-place Jacobian",
+                (long long)l, (long long)u);
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
+  // bandwidths beyond the matrix give the same entry set as the matrix's own: the candidates and band data use those
+  const int64_t lc = std::min<int64_t>(l, std::max<int64_t>(m - 1, 0)), uc = std::min<int64_t>(u, n - 1);
+  if (m > 0x7FFFFFF0LL || n > 0x7FFFFFF0LL || lc + uc + 1 > 0x7FFFFFF0LL)
+    return fail(FDB_ERR_UNSUPPORTED, "banded out-of-place plans take m, n and l + u + 1 below 2^31");
+  fdb_plan_opts o = oop_opts(opts);
+  fdb_plan *raw = nullptr;
+  TRY(fdb_plan_create_banded(&raw, m, n, lc, uc, result_kind == FDB_OOP_DENSE ? FDB_J_DENSE : FDB_J_BAND, ldJ, colorvec, &o));
+  PlanPtr owner(raw);
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  P->oop = 1;
+  P->oop_kind = result_kind;
+  P->oop_ncols = n;
+  const BandShape b = oop_band_shape(P);
+  P->oop_band_nnz = b.E;
+  // many colours: the step sizes from the per-colour column lists, in the CSC plan's summation order
+  if (P->C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
+  // _make_Ji (jacobians.jl:151-162) throws when two columns of one colour share a row.  A cyclic colouring with more
+  // colours than l + u gives distinct colours to every pair of columns that can share one.
+  if (result_kind == FDB_OOP_DENSE && m > 0 && P->C > 0 && !(P->cyclic && P->C > lc + uc)) {
+    DevBuf<unsigned long long> d_c;
+    TRY(d_c.alloc(1));
+    CU(cudaMemset(d_c.get(), 0, 8));
+    TRY(dispatch_ct(P->color_bits, [&](auto tag) {
+      return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
+        count_band_conflicts<<<P->grid(n), kThreads>>>(b, cs, P->C, d_c.get());
+        CU(cudaGetLastError());
+        return FDB_OK;
+      });
+    }));
+    unsigned long long conflicts = 0;
+    TRY(read_back(&conflicts, d_c.get(), 1, "conflict count"));
+    if (conflicts > 0)
+      return fail(FDB_ERR_INVALID, "invalid colouring: %lld (row, colour) collisions; the dense out-of-place result is "
+                                   "undefined for it (the reference throws in _make_Ji)", (long long)conflicts);
+  }
+  if (result_kind == FDB_OOP_SPARSE && P->rank == 0) {
+    // one group of resident f! outputs on one rank: the compaction forms the quotients itself; otherwise the colour loop's
+    // band scatter writes the candidates in band-data layout (every rank into the root's buffer)
+    P->oop_fused = P->n_groups <= 1 && P->world == 1;
+    TRY(oop_alloc_sparse(P, b.E, P->oop_fused ? 0 : P->j_len));
   }
   *plan = owner.release();
   return FDB_OK;
@@ -146,7 +209,7 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
   P->oop_kind = result_kind;
   P->oop_ncols = ncols_out;
   P->oop_qcols = C;
-  if (result_kind == FDB_OOP_SPARSE && P->rank == 0) TRY(oop_alloc_sparse(P, m * C));
+  if (result_kind == FDB_OOP_SPARSE && P->rank == 0) TRY(oop_alloc_sparse(P, m * C, m * C));
   *plan = owner.release();
   return FDB_OK;
 }
@@ -174,12 +237,25 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
   double *J = full ? base + P->col_begin * P->ldJ : base;
   DeviceGuard g(P->device);
   // a sparse result whose colorvec has no valid colour: nobody scatters, and the candidates are the zeros of rank 0
-  if (P->oop_kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->local_colors.empty() && P->E > 0)
-    CU(cudaMemsetAsync(J, 0, (size_t)P->E * 8, s));
+  const int64_t cand_len = P->sp_kind == SP_BANDED ? P->j_len : P->E;   // band data: every column's slots
+  if (P->oop_kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->local_colors.empty() && cand_len > 0)
+    CU(cudaMemsetAsync(J, 0, (size_t)cand_len * 8, s));
   if ((P->n > 0 && !d_x) || (P->j_len > 0 && !J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   TRY(jacobian_run(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, (void *)s));
   if (P->oop_kind == FDB_OOP_DENSE) {
-    if (!full && P->oop_dest_n > 0) {
+    if (P->sp_kind == SP_BANDED) {
+      // + 0.0 over the band entries of this rank's colours, in closed form
+      const BandShape b = oop_band_shape(P);
+      if (b.E > 0 && !P->local_colors.empty()) {
+        TRY(dispatch_ct(P->color_bits, [&](auto tag) {
+          return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
+            oop_band_plus_zero<<<P->grid(b.E), kThreads, 0, s>>>(J, P->ldJ, b, cs, P->local_of, P->C);
+            return FDB_OK;
+          });
+        }));
+        P->cnt.kernel_launches += 1;
+      }
+    } else if (!full && P->oop_dest_n > 0) {
       oop_plus_zero_slots<<<P->grid(P->oop_dest_n), kThreads, 0, s>>>(J, P->oop_dest, P->oop_dest_n);
       P->cnt.kernel_launches += 1;
     } else if (full && P->m > 0) {
@@ -208,7 +284,7 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
 // them (the full candidate count and maximum(colorvec)), fused with the quotients when one plan holds every f! output.
 static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const double *d_fx, const double *d_f_in,
                                   cudaStream_t s) {
-  const bool full = P->sp_kind == SP_NONE;
+  const bool full = P->sp_kind == SP_NONE, band = P->sp_kind == SP_BANDED;
   const int64_t candidates = oop_candidates(P);
   DeviceGuard g(P->device);
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
@@ -221,8 +297,20 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
   a.E = candidates; a.m = P->m; a.C = P->oop_qcols; a.ncols = P->oop_ncols;
   a.colptr = out->colptr; a.rowval = out->rowval; a.nzval = out->nzval; a.nnz = out->nnz;
   a.state = P->oop_state; a.claim = P->oop_state + ntiles; a.tile_col = P->oop_tile_col;
-  auto go = [&](auto kern) { kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a); };
+  if (band) a.band = oop_band_shape(P);
+  auto go = [&](auto kern, auto... cs) {
+    kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a, cs...);
+  };
   if (full) go(oop_compact<true, kCopy, uint8_t>);
+  else if (band && !P->oop_fused) go(oop_compact_band<kCopy, TableColors<uint8_t>>, TableColors<uint8_t>{nullptr});
+  else if (band) TRY(dispatch_mode(P->fdtype, [&](auto mode) {
+    return dispatch_ct(P->color_bits, [&](auto tag) {
+      return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
+        go(oop_compact_band<decltype(mode)::value, decltype(cs)>, cs);
+        return FDB_OK;
+      });
+    });
+  }));
   else if (!P->oop_fused) go(oop_compact<false, kCopy, uint8_t>);
   else TRY(dispatch_mode(P->fdtype, [&](auto mode) {
     return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
@@ -282,6 +370,14 @@ fdb_status fdb_group_create_oop_csc(fdb_group **group, int n_devices, const int 
   });
 }
 
+fdb_status fdb_group_create_oop_banded(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t l,
+                                       int64_t u, const int64_t *colorvec, int result_kind, int64_t ldJ,
+                                       const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_banded(p, m, n, l, u, colorvec, result_kind, ldJ, o);
+  });
+}
+
 fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
                                       const int64_t *colorvec, int64_t ncols_out, int result_kind, int64_t ldJ,
                                       const fdb_plan_opts *opts) {
@@ -305,8 +401,10 @@ fdb_status fdb_group_jacobian_oop(fdb_group *g, fdb_fn f, void *const *ctx, cons
   {
     DeviceGuard dg(root);
     if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
-    // a dense result of a CSC sparsity: zero-filled once, by the owner of the buffer, before any member stores into it
-    if (g->n > 1 && P0->oop_kind == FDB_OOP_DENSE && P0->sp_kind == SP_CSC && P0->j_len > 0) TRY(zero_J(P0, out->J, s0));
+    // a dense result of a CSC or band sparsity: zero-filled once, by the owner of the buffer, before any member stores
+    // into it
+    if (g->n > 1 && P0->oop_kind == FDB_OOP_DENSE && (P0->sp_kind == SP_CSC || P0->sp_kind == SP_BANDED) && P0->j_len > 0)
+      TRY(zero_J(P0, out->J, s0));
   }
   double *base = sparse ? P0->oop_vals : out->J;
   TRY(group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {

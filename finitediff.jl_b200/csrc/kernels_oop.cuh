@@ -53,9 +53,79 @@ oop_dense_finish(double *__restrict__ J, int64_t ldJ, int64_t m, int64_t C, int6
 // "Single-pass Parallel Prefix Scan with Decoupled Look-back", NVIDIA 2016).  Tiles are claimed in order from a counter,
 // so every tile a block waits for is held by a block that is running.  The kernel writes 1-based Int64 rowval, nzval,
 // colptr for every column that starts in the tile, and the kept count to *nnz.
-//   FULL = false: candidates are a CSC pattern's entries (row32[e], colptr32 0-based, ncols columns);
-//   FULL = true:  candidates are every element of an m x C column-major block (sparsity === nothing), ncols >= C.
+// FORM is the structure of the candidates:
+//   kFormCsc:  a CSC pattern's entries (row32[e], colptr32 0-based, ncols columns);
+//   kFormFull: every element of an m x C column-major block (sparsity === nothing), ncols >= C;
+//   kFormBand: the in-matrix band (l, u) of an m x n matrix, column-major and row-sorted, in closed form (BandShape): no
+//              row, colour-per-entry or column-start stream.  kCopy reads the candidates in band-data layout (slot u + r - c
+//              of column c, stride l + u + 1), as the in-place band scatter writes them.
 constexpr uint64_t kLbAggregate = 1ull << 62, kLbPrefix = 2ull << 62, kLbValue = (1ull << 62) - 1;
+enum { kFormCsc = 0, kFormFull = 1, kFormBand = 2 };
+
+// The in-matrix band E(m, n, l, u) = {(r, c) : -u <= r - c <= l, 0 <= r < m, 0 <= c < n} (0-based), l, u >= 0, clamped to
+// l <= m - 1, u <= n - 1 (the same set).  Column c holds rows max(0, c - u) .. min(m - 1, c + l); columns c >= m + u are
+// empty.  The interior columns [ca, cb) hold w = l + u + 1 rows each and start at sa + (c - ca) w.
+struct BandShape {
+  int64_t m, n, l, u, w;
+  int64_t ca, cb, sa, sb, E;
+  FastDiv wdiv;
+};
+
+// entries in the columns before c, 0 <= c <= n: sum over j < c of min(m-1, j+l) - max(0, j-u) + 1
+__host__ __device__ __forceinline__ int64_t band_col_start(int64_t m, int64_t l, int64_t u, int64_t c) {
+  if (m <= 0) return 0;
+  const int64_t k = c < m + u ? c : m + u;                         // non-empty columns before c
+  const int64_t K = m - 1;
+  int64_t t = K - l + 1;                                           // columns j < k with j + l <= K
+  t = t < 0 ? 0 : (t > k ? k : t);
+  const int64_t A = t * l + t * (t - 1) / 2 + (k - t) * K;         // sum of min(K, j + l)
+  const int64_t s = k - u - 1 > 0 ? k - u - 1 : 0;                 // columns j < k with j > u
+  return k + A - s * (s + 1) / 2;                                  // - sum of max(0, j - u)
+}
+
+inline BandShape make_band_shape(int64_t m, int64_t n, int64_t l, int64_t u) {
+  BandShape b{};
+  b.m = m; b.n = n; b.l = l; b.u = u; b.w = l + u + 1;
+  b.ca = u < n ? u : n;
+  b.cb = m - l < n ? m - l : n;
+  if (b.cb < b.ca) b.cb = b.ca;
+  b.sa = band_col_start(m, l, u, b.ca);
+  b.sb = band_col_start(m, l, u, b.cb);
+  b.E = band_col_start(m, l, u, n);
+  b.wdiv = make_fastdiv((uint32_t)b.w);
+  return b;
+}
+
+__device__ __forceinline__ int64_t band_start(const BandShape &b, int64_t c) {
+  if (c >= b.ca && c <= b.cb) return b.sa + (c - b.ca) * b.w;
+  return band_col_start(b.m, b.l, b.u, c);
+}
+
+// the column c and row r of candidate e, 0 <= e < E: division in the interior, a search over the closed-form column
+// starts in the head and tail columns
+__device__ __forceinline__ void band_locate(const BandShape &b, int64_t e, int64_t &c, int64_t &r) {
+  if (e >= b.sa && e < b.sb) {
+    const int64_t q = e - b.sa;
+    const int64_t d = q < (int64_t)0xFFFFFFFFll ? (int64_t)b.wdiv.div((uint32_t)q) : q / b.w;
+    c = b.ca + d;
+    r = c - b.u + (q - d * b.w);
+    return;
+  }
+  int64_t lo = 0, hi = b.n - 1;                                    // the last column starting at or before e
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (band_col_start(b.m, b.l, b.u, mid) <= e) lo = mid; else hi = mid - 1;
+  }
+  c = lo;
+  r = (c - b.u > 0 ? c - b.u : 0) + (e - band_col_start(b.m, b.l, b.u, c));
+}
+
+// the first column that starts at or after candidate t0 < E (columns between the interior and E are never empty)
+__device__ __forceinline__ int64_t band_first_col(const BandShape &b, int64_t t0) {
+  int64_t c, r;
+  band_locate(b, t0, c, r);
+  return band_start(b, c) < t0 ? c + 1 : c;
+}
 
 struct CompactArgs {
   const double *vals;        // [E] candidate values in storage order (kCopy)
@@ -63,20 +133,22 @@ struct CompactArgs {
   const double *Fp, *Fm, *fx, *eps;   // resident f! outputs [C][ldF], central minus outputs, f(x), step sizes [C]
   int64_t ldF;               // doubles between two colours' outputs
   int32_t ncolors;
-  const int32_t *row32;      // [E] 0-based rows (FULL = false)
-  const int32_t *colptr32;   // [ncols + 1] 0-based column starts (FULL = false)
+  const int32_t *row32;      // [E] 0-based rows (kFormCsc)
+  const int32_t *colptr32;   // [ncols + 1] 0-based column starts (kFormCsc)
   int64_t E, m, C, ncols;
   int64_t *colptr, *rowval;  // outputs: [ncols + 1], [<= E]  (1-based)
   double *nzval;             // [<= E]
   int64_t *nnz;              // kept count
   unsigned long long *state; // [ntiles] look-back words, zeroed before the launch
   unsigned long long *claim; // tile counter, zeroed before the launch
-  const int32_t *tile_col;   // [ntiles] first column starting at or after the tile's first entry (FULL = false)
+  const int32_t *tile_col;   // [ntiles] first column starting at or after the tile's first entry (kFormCsc)
+  BandShape band;            // kFormBand
 };
 
-template <bool FULL>
+template <int FORM>
 __device__ __forceinline__ int64_t compact_col_start(const CompactArgs &a, int64_t c) {
-  if (FULL) return (c < a.C ? c : a.C) * a.m;
+  if (FORM == kFormFull) return (c < a.C ? c : a.C) * a.m;
+  if (FORM == kFormBand) return c < a.ncols ? band_start(a.band, c) : a.E;
   return c < a.ncols ? (int64_t)__ldg(a.colptr32 + c) : a.E;
 }
 
@@ -96,9 +168,10 @@ oop_tile_first_col(const int32_t *__restrict__ colptr32, int64_t ncols, int64_t 
   }
 }
 
-template <bool FULL, int MODE, typename CT>
-__global__ void __launch_bounds__(kThreads)
-oop_compact(const CompactArgs a) {
+// The compaction over candidates of structure FORM.  CS: the colour source, of the entry (kFormCsc: TableColors over
+// ecolor) or of the column (kFormBand); unused by kCopy.
+template <int FORM, int MODE, typename CS>
+__device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs) {
   constexpr int kWarps = kThreads / 32, kRounds = kTile / kThreads;
   __shared__ uint32_t s_mask[kRounds * kWarps];
   __shared__ uint32_t s_pre[kRounds * kWarps + 1];
@@ -125,12 +198,22 @@ oop_compact(const CompactArgs a) {
     for (int u = 0; u < kRounds; ++u) {
       const int64_t e = t0 + u * kThreads + threadIdx.x;
       const bool in = e < a.E;
-      if (FULL) r[u] = in ? (int32_t)(e % a.m) : 0;
-      else r[u] = in ? __ldcs(a.row32 + e) : 0;
-      if (MODE == kCopy) {
-        v[u] = in ? __ldcs(a.vals + e) : 0.0;
+      int64_t bc = 0, br = 0;                      // kFormBand: the candidate's column and row
+      if (FORM == kFormBand) {
+        if (in) band_locate(a.band, e, bc, br);
+        r[u] = (int32_t)br;
+      } else if (FORM == kFormFull) {
+        r[u] = in ? (int32_t)(e % a.m) : 0;
       } else {
-        const uint32_t k = in ? (uint32_t)reinterpret_cast<const CT *>(a.ecolor)[e] : 0xFFFFFFFFu;
+        r[u] = in ? __ldcs(a.row32 + e) : 0;
+      }
+      if (MODE == kCopy) {
+        const int64_t src = FORM == kFormBand ? bc * a.band.w + a.band.u + br - bc : e;
+        v[u] = in ? __ldcs(a.vals + src) : 0.0;
+      } else {
+        uint32_t k = 0xFFFFFFFFu;
+        if constexpr (FORM == kFormBand) { if (in) k = cs.at(bc); }
+        else if (in) k = (uint32_t)cs.p[e];
         // a column without a valid colour is never perturbed: its entries are 0 and dropped
         v[u] = k < (uint32_t)a.ncolors
                    ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, r[u],
@@ -196,10 +279,12 @@ oop_compact(const CompactArgs a) {
     // colptr of the columns that start inside this tile (the last tile also takes the columns that start at E)
     const bool last = tile == ntiles - 1;
     const int64_t t1 = last ? a.E + 1 : t0 + kTile;
-    // first column that starts at or after t0 (FULL: ceil(t0 / m), at most C since t0 < E = C*m)
-    const int64_t clo = FULL ? (t0 + a.m - 1) / a.m : (int64_t)__ldg(a.tile_col + tile);
+    // first column that starts at or after t0 (kFormFull: ceil(t0 / m), at most C since t0 < E = C*m)
+    const int64_t clo = FORM == kFormFull   ? (t0 + a.m - 1) / a.m
+                        : FORM == kFormBand ? band_first_col(a.band, t0)
+                                            : (int64_t)__ldg(a.tile_col + tile);
     for (int64_t c = clo + threadIdx.x; c <= a.ncols; c += kThreads) {
-      const int64_t p = compact_col_start<FULL>(a, c);
+      const int64_t p = compact_col_start<FORM>(a, c);
       if (p >= t1) break;
       const int64_t q = p - t0;                      // position inside the tile, 0..1024
       int64_t before;
@@ -213,6 +298,61 @@ oop_compact(const CompactArgs a) {
     if (last && threadIdx.x == 0) *a.nnz = base + (int64_t)s_pre[32];
     __syncthreads();
   }
+}
+
+// FULL = false: a CSC pattern's entries (kFormCsc, per-entry colours of type CT); FULL = true: the m x C block
+template <bool FULL, int MODE, typename CT>
+__global__ void __launch_bounds__(kThreads)
+oop_compact(const CompactArgs a) {
+  compact_tiles<FULL ? kFormFull : kFormCsc, MODE>(a, TableColors<CT>{reinterpret_cast<const CT *>(a.ecolor)});
+}
+
+// the in-matrix band (kFormBand), per-column colours from CS
+template <int MODE, typename CS>
+__global__ void __launch_bounds__(kThreads)
+oop_compact_band(const CompactArgs a, const CS cs) {
+  compact_tiles<kFormBand, MODE>(a, cs);
+}
+
+// J[r + c ldJ] += 0.0 over the band entries of the columns whose colour this rank owns, for a zero-filled dense J that
+// holds their quotients: the closed-form counterpart of oop_plus_zero_slots (no destination list)
+template <typename CS>
+__global__ void __launch_bounds__(kThreads)
+oop_band_plus_zero(double *__restrict__ J, int64_t ldJ, const BandShape b, const CS cs, const int32_t *__restrict__ local_of,
+                   int32_t C) {
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  for (int64_t e = blockIdx.x * (int64_t)kThreads + threadIdx.x; e < b.E; e += stride) {
+    int64_t c, r;
+    band_locate(b, e, c, r);
+    const uint32_t k = cs.at(c);
+    if (k >= (uint32_t)C || __ldg(local_of + k) < 0) continue;
+    double *p = J + c * ldJ + r;
+    *p = *p + 0.0;
+  }
+}
+
+// Plan time, dense result: the (row, colour) collisions of count_color_conflicts in closed form.  Columns c1 < c2 share
+// rows only when c2 - c1 <= l + u, and then exactly min(m-1, c1+l) - max(0, c2-u) + 1 of them when that is positive; each
+// shared row of two columns of one valid colour is one collision.
+template <typename CS>
+__global__ void __launch_bounds__(kThreads)
+count_band_conflicts(const BandShape b, const CS cs, int32_t C, unsigned long long *__restrict__ conflicts) {
+  const int64_t stride = (int64_t)gridDim.x * kThreads;
+  unsigned long long bad = 0;
+  for (int64_t c1 = blockIdx.x * (int64_t)kThreads + threadIdx.x; c1 < b.n; c1 += stride) {
+    const uint32_t k = cs.at(c1);
+    if (k >= (uint32_t)C) continue;
+    const int64_t hi1 = c1 + b.l < b.m - 1 ? c1 + b.l : b.m - 1;
+    const int64_t last = c1 + b.l + b.u < b.n - 1 ? c1 + b.l + b.u : b.n - 1;
+    for (int64_t c2 = c1 + 1; c2 <= last; ++c2) {
+      const int64_t lo2 = c2 - b.u > 0 ? c2 - b.u : 0;
+      if (lo2 > hi1) break;
+      if (cs.at(c2) == k) bad += (unsigned long long)(hi1 - lo2 + 1);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, o);
+  if ((threadIdx.x & 31) == 0 && bad) atomicAdd(conflicts, bad);
 }
 
 }  // namespace fdb

@@ -32,7 +32,7 @@
 module FiniteDiffB200
 
 using FiniteDiff, SparseArrays, CUDA
-using LinearAlgebra: Diagonal, Bidiagonal, SymTridiagonal
+using LinearAlgebra: Diagonal, Bidiagonal, SymTridiagonal, Tridiagonal
 import FiniteDiff: finite_difference_jacobian!, finite_difference_jvp!, JacobianCache, JVPCache,
     finite_difference_jacobian, finite_difference_jvp,
     finite_difference_hessian!, HessianCache, finite_difference_gradient!, GradientCache, finite_difference_derivative!,
@@ -949,7 +949,30 @@ end
 
 hostcsc(A::DeviceCSC) = A.host
 hostcsc(A::SparseMatrixCSC) = A
-hostcsc(A) = throw(ArgumentError("not built: $(typeof(A)) in the out-of-place Jacobian (SparseMatrixCSC, DeviceCSC or nothing)"))
+hostcsc(A) = throw(ArgumentError("not built: $(typeof(A)) in the out-of-place Jacobian (SparseMatrixCSC, DeviceCSC, a band " *
+                                 "type or nothing)"))
+
+# band sparsities the out-of-place Jacobian takes in closed form (fdb_oop_plan_create_banded): (m, n, l, u), else nothing.
+# Their structural entries are the in-matrix band; Tridiagonal is the band (1, 1).
+oopband(A::DeviceBanded) = A.l >= 0 && A.u >= 0 ? (A.m, A.n, A.l, A.u) : nothing
+oopband(A::Union{DeviceDiagonal, DeviceBidiagonal, Diagonal, Bidiagonal, SymTridiagonal}) = (size(A, 1), size(A, 2), bands(A)...)
+oopband(A::Union{Tridiagonal, DeviceTridiagonal}) = (size(A, 1), size(A, 2), 1, 1)
+oopband(A) = nothing
+
+function oop_band_plan(anchor, band, kind::Cint, colorvec, fd::Cint)
+    m, n, l, u = band
+    cached_plan(anchor, (:oop_band, kind, band, color_key(colorvec), fd)) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd))
+        cptr, croot = color_arg(colorvec, n)
+        GC.@preserve croot begin
+            check(ccall((:fdb_oop_plan_create_banded, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Int64, Int64, Int64, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+                h, m, n, l, u, cptr, kind, max(m, 1), opts))
+        end
+        Plan(h[], croot)
+    end
+end
 
 """
     finite_difference_jacobian(f, x::CuVector{Float64}, cache::JacobianCache, f_in = nothing;
@@ -966,24 +989,26 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
         jac_prototype = nothing, dir = true) where {T1, T2, T3, T4, cType, sType, fdtype, returntype}
     cache.x1 === x || copyto!(cache.x1, x)
     n = length(x)
-    sp = sparsity === nothing ? nothing : hostcsc(sparsity)
-    m = sp !== nothing ? size(sp, 1) : (f_in !== nothing ? length(f_in) : length(cache.fx))
+    band = sparsity === nothing ? nothing : oopband(sparsity)
+    sp = sparsity === nothing || band !== nothing ? nothing : hostcsc(sparsity)
+    m = band !== nothing ? band[1] : sp !== nothing ? size(sp, 1) : (f_in !== nothing ? length(f_in) : length(cache.fx))
     if jac_prototype === nothing
-        kind, ncols = sp === nothing ? (FDB_OOP_RAW, 0) : (FDB_OOP_DENSE, n)
+        kind, ncols = sp === nothing && band === nothing ? (FDB_OOP_RAW, 0) : (FDB_OOP_DENSE, n)
     elseif jac_prototype isa AbstractMatrix && !(jac_prototype isa SparseMatrixCSC)
         kind, ncols = FDB_OOP_DENSE, size(jac_prototype, 2)
     else
         kind, ncols = FDB_OOP_SPARSE, size(hostcsc(jac_prototype), 2)
     end
     fd = fdcode(fdtype)
-    plan = oop_plan(sp === nothing ? cache : sp.colptr, sp, m, n, kind, ncols, colorvec, fd)
+    plan = band !== nothing ? oop_band_plan(cache, band, kind, colorvec, fd) :
+           oop_plan(sp === nothing ? cache : sp.colptr, sp, m, n, kind, ncols, colorvec, fd)
     pinfo = info(plan)
     kind == FDB_OOP_RAW && (ncols = pinfo.n_local_colors)
     st = FnState(oop_f(f), m, n, nothing)
     J = nothing
     colptr = rowval = nzval = nnz = nothing
     if kind == FDB_OOP_SPARSE
-        cap = sp === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
+        cap = sp === nothing && band === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
         colptr, rowval = CuVector{Int64}(undef, ncols + 1), CuVector{Int64}(undef, max(cap, 1))
         nzval, nnz = CuVector{Float64}(undef, max(cap, 1)), CuVector{Int64}(undef, 1)
         out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), cap, pointer(nnz)))
@@ -1057,6 +1082,23 @@ function group_oop_csc(sparsity, colorvec, fdtype, devices::Vector{Cint}; jac_pr
             h, length(devices), pointer(devices), m, n, pointer(sp.colptr), pointer(sp.rowval), cptr, kind, max(m, 1), opts))
     end
     oop_group_result(h, devices, (sp, croot), kind, m, n, n, fdtype)
+end
+
+# sparsity: a band type oopband takes (DeviceBanded with l, u >= 0, Diagonal, Bidiagonal, SymTridiagonal, Tridiagonal)
+function group_oop_banded(sparsity, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    band = oopband(sparsity)
+    band === nothing && throw(ArgumentError("not built: $(typeof(sparsity)) as a band sparsity"))
+    m, n, l, u = band
+    kind = jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC ? FDB_OOP_SPARSE : FDB_OOP_DENSE
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve croot devices begin
+        check(ccall((:fdb_group_create_oop_banded, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, Int64, Int64, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), m, n, l, u, cptr, kind, max(m, 1), opts))
+    end
+    oop_group_result(h, devices, croot, kind, m, n, n, fdtype)
 end
 
 # sparsity === nothing: m rows (length of f(x)), n = length(x)

@@ -481,12 +481,21 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   is m x ncols_out with ncols_out >= C (a narrower prototype is not built: FDB_ERR_UNSUPPORTED); FDB_OOP_SPARSE:
  *   ncols_out >= C (else FDB_ERR_INVALID, as sparse() throws).  With the prototype kinds, C < 1 gives zero(jac_prototype):
  *   +0.0 everywhere, or colptr all 1 and nnz 0, after f(x) in forward mode without d_f_in and no other call.
+ * fdb_oop_plan_create_banded: the sparsity is the in-matrix band (l, u) of an m x n matrix, E = {(r, c) : -u <= r - c <= l}
+ *   (BandedMatrix(m, n, l, u); Diagonal (0, 0), Bidiagonal :U (0, 1) and :L (1, 0), SymTridiagonal and Tridiagonal (1, 1)),
+ *   result_kind FDB_OOP_DENSE or FDB_OOP_SPARSE exactly as fdb_oop_plan_create_csc given the CSC of E: the same result,
+ *   status and f! calls.  No entry list is built on the host or the device: the structure stays a closed form.  l < 0 or
+ *   u < 0 is FDB_ERR_UNSUPPORTED; bandwidths beyond the matrix give the matrix's own band.  A dense result counts the
+ *   colouring's conflicts on the device at plan time (skipped for a cyclic colouring with more than l + u colours, which has
+ *   none).  A sparse result is compacted from the resident f! outputs in closed form, or, when they come in several groups
+ *   or ranks, from candidates the band scatter wrote in band-data layout.
  * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans (rank plans below).
  * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
  *   dense kinds: out->J (device, ldJ of the plan; the whole result, rank plans included);
  *   FDB_OOP_SPARSE: out->colptr [ncols + 1], out->rowval / out->nzval [out->cap >= the candidate count: nnz of the sparsity,
  *   or m*C], Int64 1-based; the kept count goes to the device scalar *out->nnz (stream-ordered, no host sync).
- * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a sparsity).
+ * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a sparsity,
+ * |E| with a band).
  *
  * Rank plans (opts.rank / opts.world, world in 2..64).  A rank evaluates only the colours it owns: the colour partition of
  * the in-place plans (opts.partition: round-robin or LPT, fdb_plan_color_owner) with a sparsity, the contiguous column
@@ -500,6 +509,9 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   FDB_OOP_SPARSE, CSC         its colours' candidate quotients, in storage order, into the root's candidate buffer (rank 0
  *                               also writes the zeros of columns without a valid colour); the root then compacts all nnz
  *                               candidates into `out`;
+ *   FDB_OOP_DENSE, band         as for a CSC sparsity, the + 0.0 in closed form over its own colours' band entries;
+ *   FDB_OOP_SPARSE, band        its colours' columns of the band data into the root's buffer (rank 0 also writes the zeros
+ *                               of columns without a valid colour); the root then compacts every band entry into `out`;
  *   FDB_OOP_SPARSE, no sparsity its column block of the m x C candidates at offset col_begin*m; the root then compacts all
  *                               m*C of them.
  * Per rank: forward mode without d_f_in evaluates f(x) first, then its own colours ascending; central f(x+) then f(x-) per
@@ -524,6 +536,8 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
                                    const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colorvec, int64_t ncols_out,
                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, const int64_t *colorvec,
+                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_jacobian_oop(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream);
 fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
@@ -534,7 +548,7 @@ fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const
  * d_f_in live on devices[0] (the root), x (and d_f_in, forward mode) is replicated to members on other devices, every
  * member stores its slots straight into the root's result (sparse: the root's candidate buffer), and the members are
  * joined on `stream` (a stream of devices[0]) with events.  Before any member starts, the root zero-fills a dense result
- * of a CSC sparsity; after every member has finished, the root compacts a sparse result.  No host synchronisation: the
+ * of a CSC or band sparsity; after every member has finished, the root compacts a sparse result.  No host synchronisation: the
  * kept count lands in *out->nnz.  Only the root writes f(x) to d_fx.  Device ordinals may repeat.  The result is
  * bit-identical to fdb_jacobian_oop on one device.  Complex-step groups return FDB_ERR_UNSUPPORTED.
  * fdb_group_jacobian_oop on a Jacobian or Hessian group, and fdb_group_jacobian / fdb_group_hessian on an out-of-place
@@ -545,6 +559,9 @@ fdb_status fdb_group_create_oop_csc(fdb_group **group, int n_devices, const int 
 fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
                                       const int64_t *colorvec, int64_t ncols_out, int result_kind, int64_t ldJ,
                                       const fdb_plan_opts *opts);
+fdb_status fdb_group_create_oop_banded(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t l,
+                                       int64_t u, const int64_t *colorvec, int result_kind, int64_t ldJ,
+                                       const fdb_plan_opts *opts);
 fdb_status fdb_group_jacobian_oop(fdb_group *group, fdb_fn f, void *const *ctx, const double *d_x, const fdb_oop_out *out,
                                   double *d_fx, const double *d_f_in, double relstep, double absstep, double dir,
                                   void *stream);
