@@ -1491,15 +1491,28 @@ static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
   return FDB_OK;
 }
 
+// How a coloured plan turns a group's f! outputs into J: one launcher per family (scatter_lists ... scatter_entries), and
+// none for an out-of-place sparse result whose compaction forms the quotients itself (fdjac_oop.cuh).  Fixed once the
+// plan is built, but derived rather than stored: the out-of-place creators set oop_fused after the in-place creator.
+enum class Scatter { none, lists, block_band, diagonals, band, entries };
+
+static Scatter scatter_family(const fdb_plan *P) {
+  if (P->oop_fused) return Scatter::none;
+  if (P->sp_kind == SP_CSC && P->strategy == 1) return Scatter::lists;
+  if (P->sp_kind == SP_BLOCKBAND) return Scatter::block_band;
+  if (P->sp_kind == SP_BANDED) return P->jkind == FDB_J_DIAGONALS ? Scatter::diagonals : Scatter::band;
+  return Scatter::entries;
+}
+
 // fill_matrix!(J, false) (jacobians.jl:530-532) is needed unless the scatter launches over `colours` colours (one rank's
-// or a whole group's) define every slot of J themselves, zeros for the columns without a valid colour included:
-// block-banded launches always do; identity CSC (nzval), band-data and diagonal-storage launches do once there is a
-// colour to launch for.
+// or a whole group's) define every slot of J themselves, zeros for the columns without a valid colour included.  A fused
+// out-of-place plan stores no candidate, and its candidate buffer is not J-sized: nothing to fill.
 static bool scatter_defines_J(const fdb_plan *P, int64_t colours) {
-  if (P->sp_kind == SP_BLOCKBAND) return true;
-  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED;
-  const bool band_data = P->sp_kind == SP_BANDED && (P->jkind == FDB_J_BAND || P->jkind == FDB_J_DIAGONALS);
-  return (ident || band_data) && colours > 0;
+  const Scatter f = scatter_family(P);
+  if (f == Scatter::none || f == Scatter::block_band) return true;
+  if (f == Scatter::band && P->jkind != FDB_J_BAND) return false;   // a dense J
+  if ((f == Scatter::lists || f == Scatter::entries) && P->dest != nullptr) return false;   // explicit destinations
+  return colours > 0;
 }
 
 static fdb_status call_f(fdb_plan *P, fdb_fn f, void *ctx, double *fx, const double *x, int64_t batch, cudaStream_t s) {
@@ -1523,6 +1536,24 @@ static int resident_grid(const fdb_plan *P, K kernel, size_t dyn_smem, int64_t w
   if (g > work_blocks) g = work_blocks;
   if (g < 1) g = 1;
   return (int)g;
+}
+
+// Store-heavy streams gain from an oversubscribed grid: `over` times the resident wave, capped by the work.
+template <typename K>
+static int oversubscribed_grid(const fdb_plan *P, K kernel, size_t dyn_smem, int64_t work_blocks, int over) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)resident_grid(P, kernel, dyn_smem, work_blocks) * over, work_blocks));
+}
+
+// launch `kern` on the resident grid that its occupancy gives for `work_blocks` blocks
+template <typename... KArgs, typename... Args>
+static void launch_resident(const fdb_plan *P, void (*kern)(KArgs...), int64_t work_blocks, size_t smem, cudaStream_t s,
+                            Args... args) {
+  kern<<<resident_grid(P, kern, smem, work_blocks), kThreads, smem, s>>>(args...);
+}
+
+// dynamic shared memory of a scatter that stages its per-colour (step size, slab) tables: none past kSmemTable colours
+static size_t color_table_smem(const fdb_plan *P) {
+  return P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
 }
 
 // Programmatic dependent launch: the kernel may be scheduled while the kernel before it on the stream drains, and runs
@@ -1595,6 +1626,239 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
   return FDB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ the colour scatter
+// What one colour group's scatter reads.  Every family takes its f! outputs and its stream from here, so the
+// double-buffered overlap hands its buffer and side stream to whichever family it runs.
+struct ScatterGroup {
+  fdb_plan *P;
+  double *J;
+  const double *fx;        // f(x), forward mode
+  double *Fp, *Fm;         // the group's f! outputs, one slab of ldF doubles per colour (Fm: central mode)
+  int64_t ldF;
+  cudaStream_t s;
+  int64_t l0, G;           // local colours [l0, l0 + G); G = 0: a rank that owns no colour
+  bool first;              // the first group of rank 0: it also writes the columns without a valid colour
+};
+
+// colour-major lists: the entries of the columns without a valid colour are 0
+static void zero_uncoloured_slots(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  const int64_t z0 = P->cm_start_h[P->local_colors.size()], z1 = P->cm_invalid_end;
+  if (z1 <= z0) return;
+  const int grid = P->grid(z1 - z0);
+  if (P->dest != nullptr) zero_slots<int64_t><<<grid, kThreads, 0, g.s>>>(P->cm_slot, z0, z1, g.J, P->d_peers, P->n_peers);
+  else zero_slots<int32_t><<<grid, kThreads, 0, g.s>>>(P->cm_slot, z0, z1, g.J, P->d_peers, P->n_peers);
+  P->cnt.kernel_launches += 1;
+}
+
+// colour-major lists: the entry lists of the group's colours, <= kMaxSegs colours per launch
+template <int MODE>
+static fdb_status scatter_lists(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  const int64_t total = P->cm_start_h[(size_t)(g.l0 + g.G)] - P->cm_start_h[(size_t)g.l0];
+  CmArgs a{};
+  a.row = P->cm_row; a.slot = P->cm_slot; a.seg_start = P->cm_start; a.local_colors = P->d_local_colors;
+  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.J = g.J; a.peers = P->d_peers; a.n_peers = P->n_peers;
+  a.fx_cm = MODE == kForward ? P->fx_cm : nullptr;
+  a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G; a.ldF = g.ldF;
+  a.m = MODE == kComplex ? 2 * P->m : P->m;
+  // (software L2 prefetch of the next colour's slab: off unless FDB_CM_PREFETCH=1 — on C4 the 40 MB slab, the next one
+  //  and f(x) do not fit the L2 together)
+  a.prefetch_next = (g.G > 1 && P->tune.cm_prefetch) ? 1 : 0;
+  a.slab_stream = P->tune.cm_slab_stream;
+  const int64_t tiles = (total + kCmTile - 1) / kCmTile;
+  ScatterTimer tm(P, g.s);
+  if (P->dest != nullptr) launch_resident(P, diff_scatter_cm<MODE, int64_t>, tiles, 0, g.s, a);
+  else launch_resident(P, diff_scatter_cm<MODE, int32_t>, tiles, 0, g.s, a);
+  return FDB_OK;
+}
+
+// block-banded: every slot of the columns of the group's colours, and (first group of rank 0) of the columns without a
+// valid colour: storage order, closed-form structure
+template <typename CT, int MODE>
+static fdb_status scatter_block_band(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  BlockBandArgs a{};
+  a.jcolor = P->jcolor; a.boff = P->bb_off; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps;
+  a.local_of = P->local_of; a.J = g.J; a.total = P->bb_w * P->n; a.ldF = g.ldF;
+  a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.write_other = g.first ? 1 : 0;
+  a.nblocks = P->bb_nblocks; a.u = (int32_t)P->u; a.mu = (int32_t)P->bb_mu;
+  a.uniform = P->bb_bs > 0 ? 1 : 0;
+  a.block_cyclic = P->bb_cyclic ? 1 : 0;
+  a.w = make_fastdiv((uint32_t)P->bb_w);
+  a.sw = make_fastdiv((uint32_t)(P->bb_lam + P->bb_mu + 1));
+  a.bs = make_fastdiv((uint32_t)std::max<int32_t>(P->bb_bs, 1));
+  a.bw = make_fastdiv((uint32_t)(P->l + P->u + 1));
+  const size_t sm = color_table_smem(P);
+  const int64_t tiles = (a.total + kBbTile - 1) / kBbTile;
+  // a store stream: an oversubscribed grid, as for the other band kernels
+  const int grid = oversubscribed_grid(P, diff_scatter_block_band<CT, MODE>, sm, tiles, 16);
+  ScatterTimer tm(P, g.s);
+  diff_scatter_block_band<CT, MODE><<<grid, kThreads, sm, g.s>>>(a);
+  return FDB_OK;
+}
+
+// diagonal storage: every slot of the columns of the group's colours, and (first group of rank 0) of the columns without
+// a valid colour: storage order, closed-form diagonal and (row, column)
+template <typename CT, int MODE>
+static fdb_status scatter_diagonals(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  DiagArgs a{};
+  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.local_of = P->local_of; a.J = g.J;
+  a.total = P->j_len; a.sub_end = P->l * (P->n - 1); a.main_end = a.sub_end + P->n; a.ldF = g.ldF;
+  a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.write_other = g.first ? 1 : 0;
+  const size_t sm = color_table_smem(P);
+  const int64_t tiles = (a.total + kDgTile - 1) / kDgTile;
+  ScatterTimer tm(P, g.s);
+  return dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+    using CS = decltype(cs);
+    // a store stream: an oversubscribed grid, as for the other band kernels
+    const int grid = oversubscribed_grid(P, diff_scatter_diagonals<CS, MODE>, sm, tiles, 16);
+    diff_scatter_diagonals<CS, MODE><<<grid, kThreads, sm, g.s>>>(a, cs);
+    return FDB_OK;
+  });
+}
+
+// band data or a dense J of a banded sparsity: one timed region per group, the pre-division pass (when used) and the
+// band kernel
+template <typename CT, int MODE>
+static fdb_status scatter_band(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  BandArgs a{};
+  ScatterTimer tm(P, g.s);
+  a.jcolor = P->jcolor; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.local_of = P->local_of;
+  a.J = g.J; a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.write_other = g.first ? 1 : 0;
+  a.to_dense = P->jkind == FDB_J_DENSE ? 1 : 0;
+  a.ldF = g.ldF; a.ldJ = P->ldJ; a.m = P->m; a.n = P->n; a.l = P->l; a.u = P->u;
+  const int64_t w = P->l + P->u + 1;
+  a.cols_per_tile = std::max<int64_t>(1, 4096 / w);
+  // every (colour, row) quotient lands in about (l+u+1)/C columns of the whole-band fill: when that reuse is >= 2,
+  // divide once per (colour, row) in place (the reference's own `vfx1 = (vfx1 - vfx)/eps` pass) and let the band
+  // kernel copy; otherwise divide at gather time.
+  // On C3 (16 GB band, 5 colours) the flat stream over pre-divided slabs with 4-deep batched loads was kept over
+  // warp-per-column, dividing at gather time, row-stationary, colour-grouped columns and block-per-column forms.
+  const bool prediv = MODE != kComplex && w >= 64 && w >= 2 * (int64_t)P->C;
+  if (prediv) {
+    dim3 grid((unsigned)std::max(1, std::min(P->grid(P->m), std::max(1, P->sm_count * 8 / (int)g.G))), (unsigned)g.G);
+    diff_slabs<MODE><<<grid, kThreads, 0, g.s>>>(g.Fp, MODE == kCentral ? g.Fm : g.fx, P->eps, P->d_local_colors + g.l0, P->m, g.ldF);
+    P->cnt.kernel_launches += 1;
+  }
+  if (w >= 64) {
+    // wide band: one warp per column
+    const size_t sm = color_table_smem(P);
+    if (!a.to_dense && (reinterpret_cast<uintptr_t>(g.J) & 15) == 0) {
+      // band-data target: aligned flat stream, 16-byte stores
+      const int32_t CH = (int32_t)std::min<int64_t>(2048, w & ~(int64_t)1);
+      const int64_t nchunks = (w * P->n + CH - 1) / CH;
+      if (prediv) {
+        // unlike the read-modify kernels (C2: no gain), this store-dominated stream gains from an oversubscribed grid
+        // (64x the resident wave); a bare store-only stream (fdbs_store_probe) shows the same trend
+        const int grid = oversubscribed_grid(P, diff_scatter_band_flat<CT, kCopy>, sm, (nchunks + 7) / 8, 64);
+        diff_scatter_band_flat<CT, kCopy><<<grid, kThreads, sm, g.s>>>(a, CH);
+      } else {
+        launch_resident(P, diff_scatter_band_flat<CT, MODE>, (nchunks + 7) / 8, sm, g.s, a, CH);
+      }
+    } else if (prediv) launch_resident(P, diff_scatter_band_wide<CT, kCopy>, (P->n + 7) / 8, sm, g.s, a);
+    else launch_resident(P, diff_scatter_band_wide<CT, MODE>, (P->n + 7) / 8, sm, g.s, a);
+  } else {
+    diff_scatter_band<CT, MODE><<<P->grid(P->n, (int)a.cols_per_tile, 16), kThreads, 0, g.s>>>(a);
+  }
+  return FDB_OK;
+}
+
+// CSC in storage order and COO: one pass over the entries.  Which kernel runs also depends on the call's pointers.
+template <typename CT, int MODE>
+static fdb_status scatter_entries(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  ScatterArgs a{};
+  a.row = P->row32; a.ecolor = P->ecolor; a.dest = P->dest; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps;
+  a.local_of = P->local_of; a.J = g.J; a.peers = P->d_peers; a.n_peers = P->n_peers; a.C = P->C;
+  a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.write_invalid_zero = (g.first && P->has_invalid) ? 1 : 0;
+  a.ldF = g.ldF; a.E = P->E;
+  a.j_aligned = (reinterpret_cast<uintptr_t>(g.J) & 15) == 0 && P->peers_aligned;
+  // random patterns (mean row jump beyond a few cache lines): slab gathers are read-once
+  a.hi_stream = P->tune.hi_stream >= 0 ? P->tune.hi_stream : (P->mean_row_jump > 4096.0 ? 1 : 0);
+  const size_t sm = color_table_smem(P);
+  ScatterTimer tm(P, g.s);
+  const int64_t tiles = (P->E + kTile - 1) / kTile;
+  // single group on a single rank: every valid colour is resident -> the FULL variant (no ownership tests)
+  const bool full = P->n_groups == 1 && P->world == 1 && P->n_peers == 0;
+  // staged form (identity destination): needs 16-byte aligned sources and (forward) ldF readable doubles behind f(x)
+  bool staged = P->dest == nullptr && full && P->staged && MODE != kComplex;
+  if (staged && MODE == kForward)
+    staged = (reinterpret_cast<uintptr_t>(g.fx) & 15) == 0 && ((P->m & 1) == 0 || g.fx == P->fx_own);
+  if (staged) {
+    if constexpr (MODE != kComplex) {
+      StagedArgs sa{};
+      sa.row16 = P->row16; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
+      sa.fx = g.fx; sa.Fp = g.Fp; sa.Fm = g.Fm; sa.eps = P->eps; sa.J = g.J; sa.C = P->C; sa.W = P->stage_W;
+      sa.ldF = g.ldF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned; sa.claim = P->stage_claim;
+      sa.reverse = P->tune.reverse & 1;
+      sa.colptr32 = P->colptr32; sa.l = P->band_l; sa.n = (int32_t)P->n;
+      sa.col_a = P->band_col_a; sa.col_b = P->band_col_b; sa.e_a = P->band_e_a; sa.e_b = P->band_e_b;
+      sa.w = make_fastdiv((uint32_t)P->band_w);
+      const int nwin = MODE == kCentral ? 2 * P->C : P->C + 1;
+      auto smem = [&](int stages) { return (size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8; };
+      sa.stages = smem(P->tune.stages) > (size_t)kStageMaxSmem ? 2 : P->tune.stages;
+      const size_t ssm = smem(sa.stages);
+      // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n | 6e): resident blocks per SM x index prefetch / empty mbarrier
+      const char v0 = P->tune.staged_variant[0], v1 = P->tune.staged_variant[1];
+      auto go = [&](auto kern, auto cs) -> fdb_status {
+        CU(launch_pdl(kern, resident_grid(P, kern, ssm, tiles), ssm, g.s, sa, cs));
+        return FDB_OK;
+      };
+      if (P->stage_band) {
+        return dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+          using CS = decltype(cs);
+          if (v0 == '8') return go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs);
+          if (v1 == 'e') return go(diff_scatter_staged<CS, MODE, 6, false, false, true, true>, cs);
+          return go(diff_scatter_staged<CS, MODE, 6, false, false, false, true>, cs);
+        });
+      }
+      using CS = TableColors<CT>;          // per-entry colours
+      const CS ec{(const CT *)P->ecolor};
+      if (P->stage_packed && v1 == 'e') return go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec);
+      if (P->stage_packed) return go(diff_scatter_staged<CS, MODE, 6, false, true>, ec);
+      if (v0 == '8') return go(diff_scatter_staged<CS, MODE, 8, false, false>, ec);
+      if (v1 == 'n') return go(diff_scatter_staged<CS, MODE, 6, false, false>, ec);
+      return go(diff_scatter_staged<CS, MODE, 6, true, false>, ec);
+    }
+  }
+  if (P->dest != nullptr) launch_resident(P, diff_scatter_dest<CT, MODE>, (P->E + kThreads - 1) / kThreads, sm, g.s, a);
+  else if (full) launch_resident(P, diff_scatter_ident<CT, MODE, true, kScatterMinBlocks>, tiles, sm, g.s, a);
+  else launch_resident(P, diff_scatter_ident<CT, MODE, false, kScatterMinBlocks>, tiles, sm, g.s, a);
+  return FDB_OK;
+}
+
+// The scatter of one colour group (G = 0: once, on a rank that owns no colour).  Whether a family launches is decided
+// here and counted here; what it launches, and which part of it is timed, is its launcher's.
+template <typename CT, int MODE>
+static fdb_status scatter(Scatter family, const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  // colour-major lists: rank 0 zeroes the entries of the columns without a valid colour with its first group; owning no
+  // colour, it does so only where this call does not zero-fill J (peer stores, a shared J)
+  if (family == Scatter::lists && g.first && (g.G > 0 || P->n_peers > 0 || P->shared_J)) zero_uncoloured_slots(g);
+  // a rank that owns no colour launches the block-banded scatter of rank 0 alone: the columns without a valid colour
+  if (g.G == 0 && !(family == Scatter::block_band && g.first)) return FDB_OK;
+  switch (family) {   // (a group has a colour: C > 0 and n > 0, so band and diagonal storage have slots)
+    case Scatter::none: return FDB_OK;
+    case Scatter::lists:
+      if (P->cm_start_h[(size_t)(g.l0 + g.G)] == P->cm_start_h[(size_t)g.l0]) return FDB_OK;   // empty lists
+      TRY(scatter_lists<MODE>(g)); break;
+    case Scatter::block_band: if (P->bb_w * P->n == 0) return FDB_OK; TRY((scatter_block_band<CT, MODE>(g))); break;
+    case Scatter::diagonals: TRY((scatter_diagonals<CT, MODE>(g))); break;
+    case Scatter::band: TRY((scatter_band<CT, MODE>(g))); break;
+    case Scatter::entries: if (P->E == 0) return FDB_OK; TRY((scatter_entries<CT, MODE>(g))); break;
+  }
+  P->cnt.kernel_launches += 1;
+  P->cnt.scatter_launches += 1;
+  return FDB_OK;
+}
+
 template <typename CT, int MODE>
 static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x, double *J, double *fx,
                               const double *f_in, double relstep, double absstep, double dir, cudaStream_t s) {
@@ -1603,14 +1867,10 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   // strides, in doubles, of one f! output slab / one perturbed point (complex128 in complex-step mode)
   const int64_t sF = COMPLEX ? 2 * P->ldF : P->ldF, sX = COMPLEX ? 2 * P->ldx : P->ldx;
   const int64_t n_local = (int64_t)P->local_colors.size();
-  const bool block_band = P->sp_kind == SP_BLOCKBAND;
-  const bool ident = P->dest == nullptr && P->sp_kind != SP_BANDED && !block_band;
-  const bool diag_data = P->sp_kind == SP_BANDED && P->jkind == FDB_J_DIAGONALS;
+  const Scatter family = scatter_family(P);
   // With peer buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race
   // with the peers' stores.
-  // (an out-of-place plan with a fused compaction stores no candidate: its candidate buffer is not J-sized)
-  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && !P->oop_fused && P->j_len > 0)
-    TRY(zero_J(P, J, s));
+  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
   auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
       for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
@@ -1633,9 +1893,7 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
           } else {
             // store-heavy (NP points written per element read): an oversubscribed grid (16x the resident wave), like the
             // band and dense-column kernels
-            constexpr int kPerturbGridOver = 16;
-            auto over = [&](int g) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)g * kPerturbGridOver, tiles)); };
-            auto go = [&](auto kern) { return launch_pdl(kern, over(resident_grid(P, kern, sm, tiles)), sm, ps, pa, cs); };
+            auto go = [&](auto kern) { return launch_pdl(kern, oversubscribed_grid(P, kern, sm, tiles, 16), sm, ps, pa, cs); };
             if (pa.kcount == 1) CU(go(perturb_colors<CS, CENTRAL, 1>));
             else CU(go(perturb_colors<CS, CENTRAL, kPerturbMaxPoints>));
           }
@@ -1673,248 +1931,18 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   }
   if (eps_beside_fx) CU(cudaStreamWaitEvent(s, P->ev_eps, 0));
   // colour-major lists, forward: f(x) once into list order (read as a coalesced stream by every colour's launch)
-  if (MODE == kForward && P->sp_kind == SP_CSC && P->strategy == 1 && P->fx_cm && n_local > 0) {
+  if (MODE == kForward && family == Scatter::lists && P->fx_cm && n_local > 0) {
     const int64_t cnt = P->cm_start_h[(size_t)n_local];
     if (cnt > 0) {
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((cnt + kThreads * 4 - 1) / (kThreads * 4), (int64_t)P->sm_count * 16));
       ScatterTimer tm(P, s);            // part of the diff+scatter formulation: timed with it
-      gather_fx_cm<<<grid, kThreads, 0, s>>>(P->cm_row, vfx, cnt, P->fx_cm);
+      gather_fx_cm<<<P->grid(cnt, kThreads * 4, 16), kThreads, 0, s>>>(P->cm_row, vfx, cnt, P->fx_cm);
       P->cnt.kernel_launches += 1;
     }
   }
-  // per-colour column-list scatter of local colours [l0, l0+G): <= kMaxSegs colours per launch
   // Double-buffered overlap (multi-GPU, column lists): group g's f! outputs live in buffer (g & 1); its scatter — the
   // kernel that also pushes the values to the peers over NVLink — runs on a side stream while the main stream already
   // evaluates group g+1 into the other buffer.  Events order buffer reuse; everything joins the caller's stream at the end.
   const bool overlap = P->double_buffer && P->side != nullptr;
-  const double *Fp_g = P->Fp, *Fm_g = P->Fm;
-  cudaStream_t ss = s;
-  auto scatter_lists = [&](int64_t g, int64_t l0, int64_t G) -> fdb_status {
-    const bool wide = P->dest != nullptr;
-    // columns without a valid colour (rank 0, with the first group): their entries are 0
-    if (g == 0 && P->rank == 0 && P->cm_invalid_end > P->cm_start_h[(size_t)n_local]) {
-      const int64_t z0 = P->cm_start_h[(size_t)n_local], z1 = P->cm_invalid_end;
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((z1 - z0 + kThreads - 1) / kThreads, (int64_t)P->sm_count * 8));
-      if (wide) zero_slots<int64_t><<<grid, kThreads, 0, ss>>>(P->cm_slot, z0, z1, J, P->d_peers, P->n_peers);
-      else zero_slots<int32_t><<<grid, kThreads, 0, ss>>>(P->cm_slot, z0, z1, J, P->d_peers, P->n_peers);
-      P->cnt.kernel_launches += 1;
-    }
-    if (G <= 0) return FDB_OK;
-    const int64_t total = P->cm_start_h[(size_t)(l0 + G)] - P->cm_start_h[(size_t)l0];
-    if (total == 0) return FDB_OK;
-    CmArgs a{};
-    a.row = P->cm_row; a.slot = P->cm_slot; a.seg_start = P->cm_start; a.local_colors = P->d_local_colors;
-    a.fx = vfx; a.Fp = Fp_g; a.Fm = Fm_g; a.eps = P->eps; a.J = J; a.peers = P->d_peers; a.n_peers = P->n_peers;
-    a.fx_cm = MODE == kForward ? P->fx_cm : nullptr;
-    a.l0 = (int32_t)l0; a.G = (int32_t)G; a.ldF = sF;
-    a.m = COMPLEX ? 2 * P->m : P->m;
-    // (software L2 prefetch of the next colour's slab: off unless FDB_CM_PREFETCH=1 — on C4 the 40 MB slab, the next one
-    //  and f(x) do not fit the L2 together)
-    a.prefetch_next = (G > 1 && P->tune.cm_prefetch) ? 1 : 0;
-    a.slab_stream = P->tune.cm_slab_stream;
-    const int64_t tiles = (total + kCmTile - 1) / kCmTile;
-    ScatterTimer tm(P, ss);
-    if (wide) {
-      const int grid = resident_grid(P, diff_scatter_cm<MODE, int64_t>, 0, tiles);
-      diff_scatter_cm<MODE, int64_t><<<grid, kThreads, 0, ss>>>(a);
-    } else {
-      const int grid = resident_grid(P, diff_scatter_cm<MODE, int32_t>, 0, tiles);
-      diff_scatter_cm<MODE, int32_t><<<grid, kThreads, 0, ss>>>(a);
-    }
-    P->cnt.kernel_launches += 1;
-    P->cnt.scatter_launches += 1;
-    return FDB_OK;
-  };
-
-  auto scatter_group = [&](int64_t g, int64_t l0, int64_t G) -> fdb_status {
-    if (P->oop_fused) return FDB_OK;   // out-of-place sparse result: the compaction forms the quotients (fdjac_oop.cuh)
-    if (P->sp_kind == SP_CSC && P->strategy == 1) return scatter_lists(g, l0, G);
-    if (block_band) {
-      // every slot of the columns of this group's colours, and (first group of rank 0) of the columns without a valid
-      // colour: storage order, closed-form structure
-      BlockBandArgs a{};
-      a.jcolor = P->jcolor; a.boff = P->bb_off; a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps;
-      a.local_of = P->local_of; a.J = J; a.total = P->bb_w * P->n; a.ldF = sF;
-      a.C = P->C; a.l0 = (int32_t)l0; a.G = (int32_t)G;
-      a.write_other = (g == 0 && P->rank == 0) ? 1 : 0;
-      a.nblocks = P->bb_nblocks; a.u = (int32_t)P->u; a.mu = (int32_t)P->bb_mu;
-      a.uniform = P->bb_bs > 0 ? 1 : 0;
-      a.block_cyclic = P->bb_cyclic ? 1 : 0;
-      a.w = make_fastdiv((uint32_t)P->bb_w);
-      a.sw = make_fastdiv((uint32_t)(P->bb_lam + P->bb_mu + 1));
-      a.bs = make_fastdiv((uint32_t)std::max<int32_t>(P->bb_bs, 1));
-      a.bw = make_fastdiv((uint32_t)(P->l + P->u + 1));
-      if (a.total == 0) return FDB_OK;
-      const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
-      const int64_t tiles = (a.total + kBbTile - 1) / kBbTile;
-      // a store stream: an oversubscribed grid, as for the other band kernels
-      constexpr int kBbGridOver = 16;
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(
-          (int64_t)resident_grid(P, diff_scatter_block_band<CT, MODE>, sm, tiles) * kBbGridOver, tiles));
-      ScatterTimer tm(P, s);
-      diff_scatter_block_band<CT, MODE><<<grid, kThreads, sm, s>>>(a);
-      P->cnt.kernel_launches += 1;
-      P->cnt.scatter_launches += 1;
-      return FDB_OK;
-    }
-    if (diag_data) {
-      // every slot of the columns of this group's colours, and (first group of rank 0) of the columns without a valid
-      // colour: storage order, closed-form diagonal and (row, column)
-      DiagArgs a{};
-      a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.local_of = P->local_of; a.J = J;
-      a.total = P->j_len; a.sub_end = P->l * (P->n - 1); a.main_end = a.sub_end + P->n; a.ldF = sF;
-      a.C = P->C; a.l0 = (int32_t)l0; a.G = (int32_t)G;
-      a.write_other = (g == 0 && P->rank == 0) ? 1 : 0;
-      if (a.total == 0) return FDB_OK;
-      const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
-      const int64_t tiles = (a.total + kDgTile - 1) / kDgTile;
-      ScatterTimer tm(P, s);
-      TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
-        using CS = decltype(cs);
-        // a store stream: an oversubscribed grid, as for the other band kernels
-        constexpr int kDgGridOver = 16;
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(
-            (int64_t)resident_grid(P, diff_scatter_diagonals<CS, MODE>, sm, tiles) * kDgGridOver, tiles));
-        diff_scatter_diagonals<CS, MODE><<<grid, kThreads, sm, s>>>(a, cs);
-        return FDB_OK;
-      }));
-      P->cnt.kernel_launches += 1;
-      P->cnt.scatter_launches += 1;
-      return FDB_OK;
-    }
-    if (P->sp_kind == SP_BANDED) {
-      BandArgs a{};
-      ScatterTimer tm(P, s);   // one timed region per group: the pre-division pass (when used) + the band kernel
-      a.jcolor = P->jcolor; a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.local_of = P->local_of;
-      a.J = J; a.C = P->C; a.l0 = (int32_t)l0; a.G = (int32_t)G;
-      a.write_other = (g == 0 && P->rank == 0) ? 1 : 0;
-      a.to_dense = P->jkind == FDB_J_DENSE ? 1 : 0;
-      a.ldF = sF; a.ldJ = P->ldJ; a.m = P->m; a.n = P->n; a.l = P->l; a.u = P->u;
-      const int64_t w = P->l + P->u + 1;
-      int64_t ntiles;
-      a.cols_per_tile = std::max<int64_t>(1, 4096 / w);
-      ntiles = (P->n + a.cols_per_tile - 1) / a.cols_per_tile;
-      // every (colour, row) quotient lands in about (l+u+1)/C columns of the whole-band fill: when that reuse is >= 2,
-      // divide once per (colour, row) in place (the reference's own `vfx1 = (vfx1 - vfx)/eps` pass) and let the band
-      // kernel copy; otherwise divide at gather time.
-      // On C3 (16 GB band, 5 colours) the flat stream over pre-divided slabs with 4-deep batched loads was kept over
-      // warp-per-column, dividing at gather time, row-stationary, colour-grouped columns and block-per-column forms.
-      const bool prediv = !COMPLEX && w >= 64 && P->n > 0 && P->C > 0 && G > 0 && w >= 2 * (int64_t)P->C;
-      if (prediv) {
-        dim3 grid((unsigned)std::max(1, std::min(P->grid(P->m), std::max(1, P->sm_count * 8 / (int)G))), (unsigned)G);
-        diff_slabs<MODE><<<grid, kThreads, 0, s>>>(P->Fp, CENTRAL ? P->Fm : vfx, P->eps, P->d_local_colors + l0, P->m, sF);
-        P->cnt.kernel_launches += 1;
-      }
-      if (w >= 64 && P->n > 0) {
-        // wide band: one warp per column
-        const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
-        if (!a.to_dense && (reinterpret_cast<uintptr_t>(J) & 15) == 0) {
-          // band-data target: aligned flat stream, 16-byte stores
-          const int32_t CH = (int32_t)std::min<int64_t>(2048, w & ~(int64_t)1);
-          const int64_t nchunks = (w * P->n + CH - 1) / CH;
-          if (prediv) {
-            // unlike the read-modify kernels (C2: no gain), this store-dominated stream gains from an oversubscribed grid
-            // (64x the resident wave); a bare store-only stream (fdbs_store_probe) shows the same trend
-            constexpr int kBandGridOver = 64;
-            int grid = resident_grid(P, diff_scatter_band_flat<CT, kCopy>, sm, (nchunks + 7) / 8);
-            grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)grid * kBandGridOver, (nchunks + 7) / 8));
-            diff_scatter_band_flat<CT, kCopy><<<grid, kThreads, sm, s>>>(a, CH);
-          } else {
-            const int grid = resident_grid(P, diff_scatter_band_flat<CT, MODE>, sm, (nchunks + 7) / 8);
-            diff_scatter_band_flat<CT, MODE><<<grid, kThreads, sm, s>>>(a, CH);
-          }
-        } else if (prediv) {
-          const int grid = resident_grid(P, diff_scatter_band_wide<CT, kCopy>, sm, (P->n + 7) / 8);
-          diff_scatter_band_wide<CT, kCopy><<<grid, kThreads, sm, s>>>(a);
-        } else {
-          const int grid = resident_grid(P, diff_scatter_band_wide<CT, MODE>, sm, (P->n + 7) / 8);
-          diff_scatter_band_wide<CT, MODE><<<grid, kThreads, sm, s>>>(a);
-        }
-        P->cnt.kernel_launches += 1;
-        P->cnt.scatter_launches += 1;
-      } else if (ntiles > 0) {
-        const int blocks = (int)std::min<int64_t>(ntiles, (int64_t)P->sm_count * 16);
-        diff_scatter_band<CT, MODE><<<blocks, kThreads, 0, s>>>(a);
-        P->cnt.kernel_launches += 1;
-        P->cnt.scatter_launches += 1;
-      }
-    } else if (P->E > 0) {
-      ScatterArgs a{};
-      a.row = P->row32; a.ecolor = P->ecolor; a.dest = P->dest; a.fx = vfx; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps;
-      a.local_of = P->local_of; a.J = J; a.peers = P->d_peers; a.n_peers = P->n_peers; a.C = P->C;
-      a.l0 = (int32_t)l0; a.G = (int32_t)G;
-      a.write_invalid_zero = (g == 0 && P->rank == 0 && P->has_invalid) ? 1 : 0;
-      a.ldF = sF; a.E = P->E;
-      a.j_aligned = (reinterpret_cast<uintptr_t>(J) & 15) == 0 && P->peers_aligned;
-      {
-        // random patterns (mean row jump beyond a few cache lines): slab gathers are read-once
-        a.hi_stream = P->tune.hi_stream >= 0 ? P->tune.hi_stream : (P->mean_row_jump > 4096.0 ? 1 : 0);
-      }
-      const size_t sm = P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
-      ScatterTimer tm(P, s);
-      if (ident) {
-        const int64_t tiles = (P->E + kTile - 1) / kTile;
-        // single group on a single rank: every valid colour is resident -> the FULL variant (no ownership tests)
-        const bool full = P->n_groups == 1 && P->world == 1 && P->n_peers == 0;
-        // staged form: needs 16-byte aligned sources and (forward) ldF readable doubles behind f(x)
-        bool staged = full && P->staged && MODE != kComplex;
-        if (staged && MODE == kForward)
-          staged = (reinterpret_cast<uintptr_t>(vfx) & 15) == 0 && ((P->m & 1) == 0 || vfx == P->fx_own);
-        if (staged) {
-          if constexpr (MODE != kComplex) {
-            StagedArgs sa{};
-            sa.row16 = P->row16; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
-            sa.fx = vfx; sa.Fp = P->Fp; sa.Fm = P->Fm; sa.eps = P->eps; sa.J = J; sa.C = P->C; sa.W = P->stage_W;
-            sa.ldF = sF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned; sa.claim = P->stage_claim;
-            sa.reverse = P->tune.reverse & 1;
-            sa.colptr32 = P->colptr32; sa.l = P->band_l; sa.n = (int32_t)P->n;
-            sa.col_a = P->band_col_a; sa.col_b = P->band_col_b; sa.e_a = P->band_e_a; sa.e_b = P->band_e_b;
-            sa.w = make_fastdiv((uint32_t)P->band_w);
-            const int nwin = CENTRAL ? 2 * P->C : P->C + 1;
-            int stages = P->tune.stages;
-            if ((size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8 > (size_t)kStageMaxSmem) stages = 2;
-            sa.stages = stages;
-            const size_t ssm = (size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8;
-            // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n | 6e): resident blocks per SM x index prefetch / empty mbarrier
-            const char v0 = P->tune.staged_variant[0], v1 = P->tune.staged_variant[1];
-            auto go = [&](auto kern, auto cs) -> fdb_status {
-              CU(launch_pdl(kern, resident_grid(P, kern, ssm, tiles), ssm, s, sa, cs));
-              return FDB_OK;
-            };
-            if (P->stage_band) {
-              TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
-                using CS = decltype(cs);
-                if (v0 == '8') TRY(go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs));
-                else if (v1 == 'e') TRY(go(diff_scatter_staged<CS, MODE, 6, false, false, true, true>, cs));
-                else TRY(go(diff_scatter_staged<CS, MODE, 6, false, false, false, true>, cs));
-                return FDB_OK;
-              }));
-            } else {
-              using CS = TableColors<CT>;          // per-entry colours
-              const CS ec{(const CT *)P->ecolor};
-              if (P->stage_packed && v1 == 'e') TRY(go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec));
-              else if (P->stage_packed) TRY(go(diff_scatter_staged<CS, MODE, 6, false, true>, ec));
-              else if (v0 == '8') TRY(go(diff_scatter_staged<CS, MODE, 8, false, false>, ec));
-              else if (v1 == 'n') TRY(go(diff_scatter_staged<CS, MODE, 6, false, false>, ec));
-              else TRY(go(diff_scatter_staged<CS, MODE, 6, true, false>, ec));
-            }
-          }
-        } else if (full) {
-          const int grid = resident_grid(P, diff_scatter_ident<CT, MODE, true, kScatterMinBlocks>, sm, tiles);
-          diff_scatter_ident<CT, MODE, true, kScatterMinBlocks><<<grid, kThreads, sm, s>>>(a);
-        } else {
-          const int grid = resident_grid(P, diff_scatter_ident<CT, MODE, false, kScatterMinBlocks>, sm, tiles);
-          diff_scatter_ident<CT, MODE, false, kScatterMinBlocks><<<grid, kThreads, sm, s>>>(a);
-        }
-      } else {
-        const int grid = resident_grid(P, diff_scatter_dest<CT, MODE>, sm, (P->E + kThreads - 1) / kThreads);
-        diff_scatter_dest<CT, MODE><<<grid, kThreads, sm, s>>>(a);
-      }
-      P->cnt.kernel_launches += 1;
-      P->cnt.scatter_launches += 1;
-    }
-    return FDB_OK;
-  };
 
   // colours ascending (jacobians.jl:547).  Points are built in windows of `pbatch` colours, f! is called once per point
   // (reference order f(fx1,x1) then f(fx,x) per colour, :563 / :605-606) or once per `batch` points for batch-capable
@@ -1931,27 +1959,21 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
     if (CENTRAL) TRY(call_f(P, f, ctx, P->Fm + gb + (li - g0) * sF, P->xm + (li % P->pbatch) * sX, fc, s));
     li += fc;
     if (li == gend) {
-      Fp_g = P->Fp + gb;
-      Fm_g = CENTRAL ? P->Fm + gb : nullptr;
+      const ScatterGroup grp{P, J, vfx, P->Fp + gb, CENTRAL ? P->Fm + gb : nullptr, sF, overlap ? P->side : s,
+                             g0, gend - g0, g == 0 && P->rank == 0};
       if (overlap) {
         CU(cudaEventRecord(P->ev_f[g & 1], s));
         CU(cudaStreamWaitEvent(P->side, P->ev_f[g & 1], 0));
-        ss = P->side;
-        TRY(scatter_group(g, g0, gend - g0));
-        CU(cudaEventRecord(P->ev_scat[g & 1], P->side));
-        ss = s;
-      } else {
-        TRY(scatter_group(g, g0, gend - g0));
       }
+      TRY((scatter<CT, MODE>(family, grp)));
+      if (overlap) CU(cudaEventRecord(P->ev_scat[g & 1], P->side));
     }
   }
   if (overlap) {   // join the side stream back into the caller's stream
     const int64_t ng = (n_local + P->slabs - 1) / P->slabs;
     for (int64_t b = 0; b < std::min<int64_t>(ng, 2); ++b) CU(cudaStreamWaitEvent(s, P->ev_scat[b], 0));
   }
-  // columns without a valid colour when this rank evaluates no colour at all
-  if (n_local == 0 && P->sp_kind == SP_CSC && P->strategy == 1 && (P->n_peers > 0 || P->shared_J)) TRY(scatter_group(0, 0, 0));
-  if (n_local == 0 && block_band && P->rank == 0) TRY(scatter_group(0, 0, 0));
+  if (n_local == 0) TRY((scatter<CT, MODE>(family, {P, J, vfx, P->Fp, P->Fm, sF, s, 0, 0, P->rank == 0})));
   CU(cudaGetLastError());
   return FDB_OK;
 }
