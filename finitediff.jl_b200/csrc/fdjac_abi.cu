@@ -140,48 +140,16 @@ struct GraphKey {
 };
 
 // ------------------------------------------------------------------------------------------------ plan
+// A plan's state: the fields every plan has, then one part per piece of work, each filled only by the plan kinds named
+// on it (the other kinds leave it at its defaults).  SP_NONE is the dense-column plan.
 struct fdb_plan {
   int device = 0, sm_count = 132;
   int64_t l2_bytes = 50 << 20;
   int fdtype = FDB_FORWARD, sp_kind = SP_CSC, jkind = FDB_J_CSC_NZVAL;
-  int no_drift = 0;
   int rank = 0, world = 1;
-  int64_t m = 0, n = 0, E = 0, j_len = 0, ldJ = 0, l = 0, u = 0;
-  int32_t C = 0;
-  int color_bits = 8;
-  bool has_invalid = false;
-  bool cyclic = false;        // colorvec[j] == j mod C + 1 for every j: kernels use the closed form, jcolor is not read
-  // compressed index streams (device)
-  void *jcolor = nullptr;     // [n] CT
-  int32_t *row32 = nullptr;   // [E]
-  void *ecolor = nullptr;     // [E] CT
-  int64_t *dest = nullptr;    // [E] or null (identity)
-  int32_t *local_of = nullptr;      // [C] device
-  int32_t *d_local_colors = nullptr;// [n_local] device (global colour ids, ascending)
-  std::vector<int32_t> local_colors, owner;
-  // step sizes
-  double *eps = nullptr, *sumsq = nullptr, *partial = nullptr;
-  int eps_blocks = 0;
-  int64_t eps_chunk = 0;
-  int32_t eps_group = 1;   // largest aligned lane group without a repeated colour (color_lane_conflicts)
-  const double *ext_eps = nullptr;   // step sizes supplied by the caller (fdb_plan_set_external_eps), device, >= C entries
-  unsigned int *ticket = nullptr;   // last-block-done counter of color_sumsq_reg
-  // eps from the per-colour column lists (CSC plans with more than kEpsRegColors colours)
-  bool eps_lists = false;
-  int64_t *bucket_start_d = nullptr, *chunk_base_d = nullptr;
-  double *eps_list_partial = nullptr;
-  int64_t eps_list_max_chunks = 0;
-  bool peers_aligned = true;
+  int64_t m = 0, n = 0, j_len = 0, ldJ = 0;
   bool shared_J = false;            // member of an fdb_group: J is shared with the other members (root zero-fills it)
-  // scratch
-  double *fx_own = nullptr, *Fp = nullptr, *Fm = nullptr, *xp = nullptr, *xm = nullptr;
-  int64_t slabs = 0, ldF = 0, ldx = 0, batch = 1, n_groups = 0;
-  int64_t pbatch = 1;   // perturbed points built per perturb pass (>= batch): x is read once for all of them
-  // scatter form of a CSC plan (internal; opts->strategy 0..3 is mapped onto it in fdb_plan_create_csc):
-  // 0 = one fused pass over J's storage order, 1 = colour-major entry lists (per group of resident colours)
-  int strategy = 0;
-  bool strategy_auto = true;
-  bool lists_resident = false;         // lists with every local colour's f! output resident: ONE launch over them
+  int no_drift = 0;
   // A/B switches (environment, read ONCE when the plan is created — never on the hot path; DESIGN.md §4)
   struct Tunables {
     bool no_staged = false, no_eps_lists = false, no_eps_overlap = false, cm_prefetch = false, force_overlap = false;
@@ -197,81 +165,169 @@ struct fdb_plan {
     int stages = 2;
     char staged_variant[3] = {'6', 'n', 0};
   } tune;
-  bool double_buffer = false;          // two output buffers so a group's scatter overlaps the next group's f!
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_f[2] = {nullptr, nullptr}, ev_scat[2] = {nullptr, nullptr};
-  cudaEvent_t ev_fork = nullptr, ev_eps = nullptr;   // forward mode: the eps pass runs beside f(x) on the side stream
-  int32_t *colptr32 = nullptr, *cols_by_color = nullptr;
-  // colour-major entry lists of this rank's colours (strategy 1; built by build_cm_lists)
-  int32_t *cm_row = nullptr;
-  void *cm_slot = nullptr;            // int32 (nzval slot) or int64 (explicit destination: dest != nullptr)
-  int64_t *cm_start = nullptr;        // device [n_local + 1]
-  double *fx_cm = nullptr;            // forward: f(x) in colour-major order (rebuilt by every Jacobian)
-  std::vector<int64_t> cm_start_h;    // host copy; [n_local] .. cm_invalid_end = entries of columns without a valid colour
-  int64_t cm_invalid_end = 0;
-  // TMA-staged form of the fused pass (row-local patterns; kernels_staged.cuh)
-  uint16_t *row16 = nullptr;
-  int32_t *tile_w0 = nullptr;
-  unsigned long long *stage_claim = nullptr;   // walk-position counter of the staged pass (re-armed by every launch)
-  int32_t stage_W = 0;
-  bool staged = false, stage_packed = false;
-  bool stage_band = false;             // exact clipped band: the staged pass derives rows and columns, reads no index stream
-  int32_t band_l = 0, band_col_a = 0, band_col_b = 0, band_e_a = 0, band_e_b = 0, band_w = 1;
-  // block-banded plans (kernels_blockband.cuh): block offsets on the device, sub-block bandwidths, slots per column
-  int32_t *bb_off = nullptr;           // [nblocks + 1]
-  int32_t bb_nblocks = 0, bb_bs = 0;   // bb_bs > 0: every block has bb_bs columns
-  int64_t bb_lam = 0, bb_mu = 0, bb_w = 1;
-  bool bb_cyclic = false;              // colorvec is the block-cyclic closed form of matrix_colors
-  std::vector<int64_t> bucket_start;   // [C+2] offsets into cols_by_color; bucket C = columns without a valid colour
-  int lanes = 1;
-  double mean_row_jump = 0.0;
-  // peers (multi-GPU fused gather)
-  double **d_peers = nullptr;
-  int n_peers = 0;
-  // dense-column plans
-  int64_t col_begin = 0, col_end = 0;
-  double *eps_cols = nullptr;
-  // Hessian plans (kernels_hessian.cuh): value buffer V (V[0] = f(x), then one chunk of whole i-blocks) and the chunk
-  // boundaries [hess_chunks[c], hess_chunks[c+1]) in i
-  double *hess_V = nullptr;
-  std::vector<int64_t> hess_chunks;
-  // rank plans: local point q > 0 is global point q + hess_off; hess_points = the rank's f evaluations per call
-  int64_t hess_off = 0, hess_points = 0;
-  // derivative plans (kernels_derivative.cuh): elementwise derivative (m = n) or scalar -> vector gradient (n = 1)
-  bool deriv_elem = false;
-  int64_t deriv_fcalls = 0;   // f evaluations of the most recent call (before any: the count without cache.fx)
-  // host-buffer path
-  cudaStream_t hstream = nullptr;
-  double *h_dx = nullptr, *h_dJ = nullptr, *h_dfx = nullptr, *h_dfin = nullptr;
-  // bookkeeping
-  std::vector<void *> allocs;
-  size_t device_bytes = 0;
   fdb_counters_t cnt{};
   int64_t alg_bytes = 0;
-  int64_t last_eps_count = 0;
-  // out-of-place Jacobian plans (fdjac_oop.cuh): the colour loop with pristine points and the forward step rule in central
-  // mode, then the result form of the out-of-place finite_difference_jacobian
-  int oop = 0;                  // 1: an out-of-place plan (fdb_jacobian rejects it)
-  int oop_kind = 0;             // FDB_OOP_RAW / FDB_OOP_DENSE / FDB_OOP_SPARSE
-  int64_t oop_ncols = 0;        // columns of the result
-  int64_t oop_qcols = 0;        // dense branch: columns holding quotients, maximum(colorvec), over every rank
-  const int64_t *oop_dest = nullptr;   // dense result of a CSC sparsity: the slots of this rank's colours (dest when world = 1)
-  int64_t oop_dest_n = 0;
-  double *oop_vals = nullptr;   // sparse result: the candidate values (nzval of the sparsity, or the m x C dense block)
-  unsigned long long *oop_state = nullptr;   // sparse result: look-back words of the compaction, then its tile counter
-  int32_t *oop_tile_col = nullptr;           // sparse result of a CSC sparsity: first column starting in each tile
-  bool oop_fused = false;                    // sparse result, every colour's f! output resident: quotient + compaction fused
-  int64_t oop_band_nnz = 0;                  // result of a band sparsity: |E|, every in-matrix band entry (E counts coloured ones)
+  std::vector<void *> allocs;
+  size_t device_bytes = 0;
+
+  // f! outputs and perturbed points: every kind but the step-size plan.  What batch, slabs and n_groups count:
+  //   coloured (CSC, COO, banded, block-banded): points per f! call; colours whose f! outputs are resident at once;
+  //     scatter groups per call
+  //   dense: columns per f! call = slabs; column batches per call
+  //   Hessian: points per f call = slabs; chunks of whole i-blocks
+  //   derivative: 2 when the two central points go to f in one call, else 1 (no slabs, no groups)
+  //   JVP: 1 (no slabs, no groups)
+  struct Scratch {
+    double *fx_own = nullptr, *Fp = nullptr, *Fm = nullptr, *xp = nullptr, *xm = nullptr;
+    int64_t ldF = 0, ldx = 0;
+    int64_t batch = 1, slabs = 0, n_groups = 0;
+    int64_t pbatch = 1;   // coloured: perturbed points built per perturb pass (>= batch): x is read once for all of them
+  } scratch;
+  // colours: coloured plans and the step-size plan (C, the colour table and the column lists); coloured plans also fill
+  // the ownership and local colours, and E
+  struct Colors {
+    int32_t C = 0;                    // maximum(colorvec)
+    int bits = 8;                     // width of a colour in the tables: 8, 16 or 32
+    bool has_invalid = false;
+    bool cyclic = false;              // colorvec[j] == j mod C + 1 for every j: kernels use the closed form, jcolor is not read
+    void *jcolor = nullptr;           // [n] CT
+    int64_t E = 0;                    // structural entries of the coloured pattern (banded: in-band slots of valid colours)
+    std::vector<int32_t> owner;       // [C] rank evaluating each colour
+    std::vector<int32_t> local;       // this rank's colours, ascending
+    int32_t *d_local = nullptr;       // [n_local] device copy of `local`
+    int32_t *local_of = nullptr;      // [C] device: local index of each colour, -1 when another rank owns it
+    // per-colour column lists (CSC plans, and plans with more than kEpsRegColors colours): bucket_start [C+2] offsets
+    // into cols_by_color; bucket C = columns without a valid colour
+    std::vector<int64_t> bucket_start;
+    int32_t *cols_by_color = nullptr;
+  } colors;
+  // step sizes: coloured plans, the step-size plan (per colour) and the JVP plan (one)
+  struct Steps {
+    double *eps = nullptr, *sumsq = nullptr, *partial = nullptr;
+    unsigned int *ticket = nullptr;   // last-block-done counter of color_sumsq_reg
+    int blocks = 0;
+    int64_t chunk = 0;
+    int32_t group = 1;   // largest aligned lane group without a repeated colour (color_lane_conflicts)
+    const double *ext = nullptr;   // step sizes supplied by the caller (fdb_plan_set_external_eps), device, >= C entries
+    // eps from the per-colour column lists (more than kEpsRegColors colours)
+    bool lists = false;
+    int64_t *bucket_start_d = nullptr, *chunk_base_d = nullptr;
+    double *list_partial = nullptr;
+    int64_t list_max_chunks = 0;
+  } steps;
+  // compressed entry streams: CSC and COO plans.  strategy (CSC; internal, opts->strategy 0..3 is mapped onto it in
+  // fdb_plan_create_csc): 0 = one fused pass over J's storage order, 1 = colour-major entry lists (per group of
+  // resident colours)
+  struct Entries {
+    int32_t *row32 = nullptr;         // [E]
+    void *ecolor = nullptr;           // [E] CT
+    int64_t *dest = nullptr;          // [E] or null (identity)
+    int32_t *colptr32 = nullptr;      // [n + 1] (CSC)
+    int lanes = 1;
+    double mean_row_jump = 0.0;
+    int strategy = 0;
+    bool strategy_auto = true;
+    bool lists_resident = false;      // lists with every local colour's f! output resident: ONE launch over them
+  } entries;
+  // colour-major entry lists of this rank's colours: CSC plans with strategy 1 (built by build_cm_lists)
+  struct ColorMajor {
+    int32_t *row = nullptr;
+    void *slot = nullptr;             // int32 (nzval slot) or int64 (explicit destination: entries.dest != nullptr)
+    int64_t *start = nullptr;         // device [n_local + 1]
+    double *fx = nullptr;             // forward: f(x) in colour-major order (rebuilt by every Jacobian)
+    std::vector<int64_t> start_h;     // host copy; [n_local] .. invalid_end = entries of columns without a valid colour
+    int64_t invalid_end = 0;
+  } cm;
+  // TMA-staged form of the fused pass: CSC plans with a row-local pattern (kernels_staged.cuh)
+  struct Staged {
+    bool on = false, packed = false;
+    uint16_t *row16 = nullptr;
+    int32_t *tile_w0 = nullptr;
+    unsigned long long *claim = nullptr;   // walk-position counter of the staged pass (re-armed by every launch)
+    int32_t W = 0;
+    bool band = false;                // exact clipped band: the staged pass derives rows and columns, reads no index stream
+    int32_t band_l = 0, band_col_a = 0, band_col_b = 0, band_e_a = 0, band_e_b = 0, band_w = 1;
+  } staged;
+  // bandwidths: banded and block-banded plans
+  struct Band {
+    int64_t l = 0, u = 0;
+  } band;
+  // block-banded plans (kernels_blockband.cuh): block offsets on the device, sub-block bandwidths, slots per column
+  struct BlockBand {
+    int32_t *off = nullptr;           // [nblocks + 1]
+    int32_t nblocks = 0, bs = 0;      // bs > 0: every block has bs columns
+    int64_t lam = 0, mu = 0, w = 1;
+    bool cyclic = false;              // colorvec is the block-cyclic closed form of matrix_colors
+  } block_band;
+  // dense plans: this rank's column block [begin, end) and its steps
+  struct Columns {
+    int64_t begin = 0, end = 0;
+    double *eps = nullptr;            // [end - begin]
+  } columns;
+  // Hessian plans (kernels_hessian.cuh): value buffer V (V[0] = f(x), then one chunk of whole i-blocks) and the chunk
+  // boundaries [chunks[c], chunks[c+1]) in i
+  struct Hessian {
+    double *V = nullptr;
+    std::vector<int64_t> chunks;
+    // rank plans: local point q > 0 is global point q + off; points = the rank's f evaluations per call
+    int64_t off = 0, points = 0;
+    int64_t i_begin = 0, i_end = 0;   // this rank's i-blocks
+    int64_t entries = 0;              // entries of H the rank's i-blocks write
+    double *eps = nullptr;            // [n] per-component steps of all n components
+  } hess;
+  // derivative plans (kernels_derivative.cuh): elementwise derivative (m = n) or scalar -> vector gradient (n = 1)
+  struct Derivative {
+    bool elem = false;
+    int64_t fcalls = 0;   // f evaluations of the most recent call (before any: the count without cache.fx)
+  } deriv;
+  // out-of-place Jacobian plans (fdjac_oop.cuh): the colour loop with pristine points and the forward step rule in
+  // central mode, then the result form of the out-of-place finite_difference_jacobian
+  struct OutOfPlace {
+    bool on = false;                  // an out-of-place plan (fdb_jacobian rejects it)
+    int kind = 0;                     // FDB_OOP_RAW / FDB_OOP_DENSE / FDB_OOP_SPARSE
+    int64_t ncols = 0;                // columns of the result
+    int64_t qcols = 0;                // dense branch: columns holding quotients, maximum(colorvec), over every rank
+    const int64_t *dest = nullptr;    // dense result of a CSC sparsity: the slots of this rank's colours (entries.dest when world = 1)
+    int64_t dest_n = 0;
+    double *vals = nullptr;           // sparse result: the candidate values (nzval of the sparsity, or the m x C dense block)
+    unsigned long long *state = nullptr;   // sparse result: look-back words of the compaction, then its tile counter
+    int32_t *tile_col = nullptr;      // sparse result of a CSC sparsity: first column starting in each tile
+    bool fused = false;               // sparse result, every colour's f! output resident: quotient + compaction fused
+    int64_t band_nnz = 0;             // result of a band sparsity: |E|, every in-matrix band entry (colors.E counts coloured ones)
+  } oop;
+  // side stream and events: coloured plans.  Forward mode runs the eps pass beside f(x) on the side stream; with
+  // double_buffer, two output buffers let a group's scatter overlap the next group's f!
+  struct Overlap {
+    bool double_buffer = false;
+    cudaStream_t side = nullptr;
+    cudaEvent_t ev_f[2] = {nullptr, nullptr}, ev_scat[2] = {nullptr, nullptr};
+    cudaEvent_t ev_fork = nullptr, ev_eps = nullptr;
+  } overlap;
+  // peer J buffers (multi-GPU fused gather): CSC, COO, JVP and step-size plans (fdb_plan_set_peers)
+  struct Peers {
+    double **d = nullptr;
+    int n = 0;
+    long long generation = 0;
+    bool aligned = true;
+  } peers;
   // optional CUDA-graph replay of the whole call
-  bool use_graph = false;
-  cudaStream_t cstream = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
-  GraphKey graph_key;
-  fdb_counters_t graph_delta{};
-  long long peer_generation = 0;
+  struct Graph {
+    bool use = false;
+    cudaStream_t stream = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    GraphKey key;
+    fdb_counters_t delta{};
+  } graph;
   // optional device-side timing of the scatter launches
-  bool timing = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pending, ev_pool;
+  struct Timing {
+    bool on = false;
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending, pool;
+  } timing;
+  // host-buffer path (fdb_jacobian_host): its stream and device staging buffers, made by the first call
+  struct Host {
+    cudaStream_t stream = nullptr;
+    double *dx = nullptr, *dJ = nullptr, *dfx = nullptr, *dfin = nullptr;
+  } host;
 
   // device memory the plan keeps until fdb_plan_destroy (build scratch is a DevBuf instead)
   void adopt(void *p, size_t bytes) {
@@ -337,8 +393,8 @@ template <typename F> static fdb_status dispatch_ct(int bits, F &&fn) {
 
 // the per-column colour source of a plan whose table has type CT: the cyclic closed form when it holds, else the table
 template <typename CT, typename F> static fdb_status dispatch_colors(const fdb_plan *P, F &&fn) {
-  if (P->cyclic) return fn(CyclicColors{make_fastdiv((uint32_t)P->C)});
-  return fn(TableColors<CT>{(const CT *)P->jcolor});
+  if (P->colors.cyclic) return fn(CyclicColors{make_fastdiv((uint32_t)P->colors.C)});
+  return fn(TableColors<CT>{(const CT *)P->colors.jcolor});
 }
 
 // fn(tag) with the compile-time difference mode (kForward / kCentral / kComplex) of a plan's fdtype as decltype(tag)::value
@@ -372,14 +428,14 @@ static fdb_status check_call(const fdb_plan *P, Call c) {
   if (jac && k == SP_EPS) return fail(INV, "this is a step-size plan: call fdb_color_eps");
   if (jac && k == SP_HESS) return fail(INV, "this is a Hessian plan: call fdb_hessian");
   if (jac && k == SP_DERIV) return fail(INV, "this is a derivative plan: call fdb_derivative");
-  if (jac && P->oop) return fail(INV, "this is an out-of-place plan: call fdb_jacobian_oop");
+  if (jac && P->oop.on) return fail(INV, "this is an out-of-place plan: call fdb_jacobian_oop");
   if (c == K::jacobian && cplx)
     return fail(INV, "this plan is a complex-step plan: call fdb_jacobian_complex with a complex128 callback");
   if (c == K::jacobian_oop && cplx)
     return fail(INV, "this plan is a complex-step plan: call fdb_jacobian_oop_complex with a complex128 callback");
   if (c == K::jacobian_oop_complex && !cplx)
     return fail(INV, "fdb_jacobian_oop_complex needs a plan created with fdtype = FDB_COMPLEX");
-  if (oop && !P->oop) return fail(INV, "not an out-of-place plan (fdb_oop_plan_create_csc / _dense)");
+  if (oop && !P->oop.on) return fail(INV, "not an out-of-place plan (fdb_oop_plan_create_csc / _dense)");
   if (c == K::color_eps && !colored && k != SP_EPS) return fail(INV, "fdb_color_eps needs a coloured plan");
   if (c == K::set_external_eps && !colored) return fail(INV, "external step sizes apply to coloured Jacobian plans");
   if (c == K::set_peers && k != SP_CSC && k != SP_COO && k != SP_JVP && k != SP_EPS)
@@ -397,8 +453,8 @@ static fdb_status check_call(const fdb_plan *P, Call c) {
   if (c == K::derivative_complex && (k != SP_DERIV || !cplx))
     return fail(INV, "fdb_derivative_complex needs a derivative plan created with fdtype = FDB_COMPLEX");
   if (c == K::group_jacobian && k == SP_HESS) return fail(INV, "this is a Hessian group: call fdb_group_hessian");
-  if (c == K::group_jacobian && P->oop) return fail(INV, "this is an out-of-place group: call fdb_group_jacobian_oop");
-  if (c == K::group_jacobian_oop && !P->oop) return fail(INV, "not an out-of-place group (fdb_group_create_oop_csc / _dense)");
+  if (c == K::group_jacobian && P->oop.on) return fail(INV, "this is an out-of-place group: call fdb_group_jacobian_oop");
+  if (c == K::group_jacobian_oop && !P->oop.on) return fail(INV, "not an out-of-place group (fdb_group_create_oop_csc / _dense)");
   if (group && cplx) return fail(FDB_ERR_UNSUPPORTED, "groups run forward / central plans");
   if (c == K::group_hessian && k != SP_HESS) return fail(INV, "not a Hessian group (fdb_group_create_hessian)");
   return FDB_OK;
@@ -438,29 +494,29 @@ static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or de
   if (n == 0) mx = 0;
   if (mx < 0) mx = 0;                       // maximum(colorvec) < 1: the colour loop 1:max is empty
   if (mx > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "maximum(colorvec) = %lld exceeds 2^31", mx);
-  P->C = (int32_t)mx;
-  P->has_invalid = n > 0 && mn < 1;
-  P->color_bits = mx <= 255 ? 8 : (mx <= 65535 ? 16 : 32);
-  TRY(P->alloc(&P->jcolor, (size_t)std::max<int64_t>(n, 1) * (P->color_bits / 8)));
+  P->colors.C = (int32_t)mx;
+  P->colors.has_invalid = n > 0 && mn < 1;
+  P->colors.bits = mx <= 255 ? 8 : (mx <= 65535 ? 16 : 32);
+  TRY(P->alloc(&P->colors.jcolor, (size_t)std::max<int64_t>(n, 1) * (P->colors.bits / 8)));
   if (n > 0) {
     DevBuf<uint32_t> d_flags;   // [0] lane conflicts (window path), [1] not cyclic
-    const bool window_path = P->C > kEpsRegColors;
+    const bool window_path = P->colors.C > kEpsRegColors;
     TRY(d_flags.alloc(2));
     CU(cudaMemset(d_flags.get(), 0, 2 * sizeof(uint32_t)));
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      convert_colors<CT><<<P->grid(n), kThreads>>>(cv.d, n, (CT *)P->jcolor);
-      if (window_path) color_lane_conflicts<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags.get());
-      if (P->C > 0) check_cyclic<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, P->C, d_flags.get() + 1);
+      convert_colors<CT><<<P->grid(n), kThreads>>>(cv.d, n, (CT *)P->colors.jcolor);
+      if (window_path) color_lane_conflicts<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, n, P->colors.C, d_flags.get());
+      if (P->colors.C > 0) check_cyclic<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, n, P->colors.C, d_flags.get() + 1);
       CU(cudaGetLastError());
       return FDB_OK;
     }));
     uint32_t flags[2] = {0, 0};
     TRY(read_back(flags, d_flags.get(), 2, "colour flags"));
-    P->cyclic = P->C > 0 && flags[1] == 0;
+    P->colors.cyclic = P->colors.C > 0 && flags[1] == 0;
     if (window_path) {
-      P->eps_group = 1;
-      for (int lg = 1; lg <= 5 && !(flags[0] & (1u << lg)); ++lg) P->eps_group = 1 << lg;
+      P->steps.group = 1;
+      for (int lg = 1; lg <= 5 && !(flags[0] & (1u << lg)); ++lg) P->steps.group = 1 << lg;
     }
   }
   return FDB_OK;
@@ -468,20 +524,20 @@ static fdb_status setup_colors(fdb_plan *P, const int64_t *colorvec /*host or de
 
 // step-size buffers of a coloured plan: eps / sumsq per colour, block partials of the one-pass reduction
 static fdb_status alloc_eps_buffers(fdb_plan *P) {
-  const int32_t C = P->C;
-  TRY(P->alloc_t(&P->eps, std::max<int32_t>(C, 1)));
-  TRY(P->alloc_t(&P->sumsq, std::max<int32_t>(C, 1)));
+  const int32_t C = P->colors.C;
+  TRY(P->alloc_t(&P->steps.eps, std::max<int32_t>(C, 1)));
+  TRY(P->alloc_t(&P->steps.sumsq, std::max<int32_t>(C, 1)));
   {
     int64_t nb = (P->n + 2047) / 2048;
     // window path: 64 bytes of shared memory per window colour and block (<= 32 KB) -> one resident wave
     nb = std::max<int64_t>(1, std::min<int64_t>(nb, (int64_t)P->sm_count * (C <= 256 ? 8 : 6)));
-    P->eps_blocks = (int)nb;
+    P->steps.blocks = (int)nb;
     int64_t chunk = (P->n + nb - 1) / nb;
-    P->eps_chunk = (std::max<int64_t>(chunk, 1) + 31) & ~(int64_t)31;   // aligned 32-column steps on the window path
+    P->steps.chunk = (std::max<int64_t>(chunk, 1) + 31) & ~(int64_t)31;   // aligned 32-column steps on the window path
     const int64_t stride = C <= kEpsRegColors ? kEpsRegColors : std::min<int64_t>(C, kEpsWindow);
-    TRY(P->alloc_t(&P->partial, (size_t)nb * stride));
-    TRY(P->alloc_t(&P->ticket, 4));
-    CU(cudaMemset(P->ticket, 0, 16));
+    TRY(P->alloc_t(&P->steps.partial, (size_t)nb * stride));
+    TRY(P->alloc_t(&P->steps.ticket, 4));
+    CU(cudaMemset(P->steps.ticket, 0, 16));
   }
 
   return FDB_OK;
@@ -489,8 +545,8 @@ static fdb_status alloc_eps_buffers(fdb_plan *P) {
 
 // colour ownership (multi-GPU), local colour list, scratch sizing
 static fdb_status finish_colored_plan(fdb_plan *P, const fdb_plan_opts *o, const std::vector<unsigned long long> &count) {
-  const int32_t C = P->C;
-  P->owner.assign(C, 0);
+  const int32_t C = P->colors.C;
+  P->colors.owner.assign(C, 0);
   const int world = P->world;
   if (world > 1) {
     if (o && o->partition == 1) {
@@ -502,76 +558,76 @@ static fdb_status finish_colored_plan(fdb_plan *P, const fdb_plan_opts *o, const
       for (int32_t k : order) {
         int best = 0;
         for (int r = 1; r < world; ++r) if (load[r] < load[best]) best = r;
-        P->owner[k] = best;
+        P->colors.owner[k] = best;
         load[best] += count[k] + 1;
       }
     } else {
-      for (int32_t k = 0; k < C; ++k) P->owner[k] = k % world;
+      for (int32_t k = 0; k < C; ++k) P->colors.owner[k] = k % world;
     }
   }
   std::vector<int32_t> local_of(C, -1);
-  P->local_colors.clear();
+  P->colors.local.clear();
   for (int32_t k = 0; k < C; ++k)
-    if (P->owner[k] == P->rank) { local_of[k] = (int32_t)P->local_colors.size(); P->local_colors.push_back(k); }
-  const int64_t n_local = (int64_t)P->local_colors.size();
-  TRY(P->alloc_t(&P->local_of, std::max<int32_t>(C, 1)));
-  TRY(P->alloc_t(&P->d_local_colors, std::max<int64_t>(n_local, 1)));
-  if (C > 0) CU(cudaMemcpy(P->local_of, local_of.data(), (size_t)C * 4, cudaMemcpyHostToDevice));
-  if (n_local > 0) CU(cudaMemcpy(P->d_local_colors, P->local_colors.data(), (size_t)n_local * 4, cudaMemcpyHostToDevice));
+    if (P->colors.owner[k] == P->rank) { local_of[k] = (int32_t)P->colors.local.size(); P->colors.local.push_back(k); }
+  const int64_t n_local = (int64_t)P->colors.local.size();
+  TRY(P->alloc_t(&P->colors.local_of, std::max<int32_t>(C, 1)));
+  TRY(P->alloc_t(&P->colors.d_local, std::max<int64_t>(n_local, 1)));
+  if (C > 0) CU(cudaMemcpy(P->colors.local_of, local_of.data(), (size_t)C * 4, cudaMemcpyHostToDevice));
+  if (n_local > 0) CU(cudaMemcpy(P->colors.d_local, P->colors.local.data(), (size_t)n_local * 4, cudaMemcpyHostToDevice));
 
   TRY(alloc_eps_buffers(P));
 
   // scratch: stacked f! outputs (slabs) + perturbed points
   const bool central = P->fdtype == FDB_CENTRAL;
   const int64_t cw = P->fdtype == FDB_COMPLEX ? 2 : 1;     // doubles per element of the f! in/outputs
-  P->ldF = (P->m + 1) & ~(int64_t)1;
-  P->ldx = (P->n + 1) & ~(int64_t)1;
-  if (P->ldF < 2) P->ldF = 2;
-  if (P->ldx < 2) P->ldx = 2;
+  P->scratch.ldF = (P->m + 1) & ~(int64_t)1;
+  P->scratch.ldx = (P->n + 1) & ~(int64_t)1;
+  if (P->scratch.ldF < 2) P->scratch.ldF = 2;
+  if (P->scratch.ldx < 2) P->scratch.ldx = 2;
   int64_t budget = (o && o->scratch_bytes > 0) ? o->scratch_bytes : (int64_t)8 << 30;
-  const int64_t per_slab = 8 * cw * P->ldF * (central ? 2 : 1);
+  const int64_t per_slab = 8 * cw * P->scratch.ldF * (central ? 2 : 1);
   int64_t slabs = std::max<int64_t>(1, budget / per_slab);
   slabs = std::min<int64_t>(slabs, std::max<int64_t>(n_local, 1));
-  if (P->sp_kind == SP_CSC && P->strategy == 0 && P->strategy_auto && slabs < n_local) P->strategy = 1;
-  if (P->strategy == 1 && !P->lists_resident) {
+  if (P->sp_kind == SP_CSC && P->entries.strategy == 0 && P->entries.strategy_auto && slabs < n_local) P->entries.strategy = 1;
+  if (P->entries.strategy == 1 && !P->entries.lists_resident) {
     // per-colour lists: keep only as many f! outputs in flight as stay L2-resident until their scatter (~40 % of the L2:
     // 20 MB of an H100's 50 MB, the rest is left to f(x) and the index streams)
     const int64_t l2_slabs = std::max<int64_t>(1, P->l2_bytes * 2 / 5 / per_slab);
     slabs = std::min<int64_t>(slabs, l2_slabs);
   }
-  if (P->strategy == 1) slabs = std::min<int64_t>(slabs, kCmMaxGroup);
-  P->slabs = slabs;
-  P->n_groups = n_local == 0 ? 0 : (n_local + slabs - 1) / slabs;
+  if (P->entries.strategy == 1) slabs = std::min<int64_t>(slabs, kCmMaxGroup);
+  P->scratch.slabs = slabs;
+  P->scratch.n_groups = n_local == 0 ? 0 : (n_local + slabs - 1) / slabs;
   int64_t batch = (o && o->max_batch > 1) ? o->max_batch : 1;
   batch = std::min<int64_t>(batch, slabs);
-  P->batch = batch;
+  P->scratch.batch = batch;
   // even when f! takes one point per call, build up to kPerturbMaxPoints points per pass over x (one read of x and
   // the colour stream instead of one per colour) when the point buffers fit in an eighth of the scratch budget
   int64_t pbatch = std::max<int64_t>(batch, std::min<int64_t>(kPerturbMaxPoints, std::max<int64_t>(n_local, 1)));
-  while (pbatch > batch && pbatch * 8 * cw * P->ldx * (central ? 2 : 1) > budget / 8) --pbatch;
-  P->pbatch = pbatch;
+  while (pbatch > batch && pbatch * 8 * cw * P->scratch.ldx * (central ? 2 : 1) > budget / 8) --pbatch;
+  P->scratch.pbatch = pbatch;
   // two output buffers + a side stream: a group's scatter (and its NVLink stores, when peers are set) overlaps the next
   // group's f! evaluations
   // Off by default: the scatter and the next f! compete for the same L2 / DRAM, and the NVLink stores of a 5 MB colour
   // need no hiding.  FDB_FORCE_OVERLAP=1 switches the double-buffered side-stream form back on.
-  P->double_buffer = false;
-  if (P->tune.force_overlap && P->sp_kind == SP_CSC && P->strategy == 1 && (int64_t)P->local_colors.size() > slabs) P->double_buffer = true;
-  const size_t nbuf = P->double_buffer ? 2 : 1;
-  CU(cudaStreamCreateWithFlags(&P->side, cudaStreamNonBlocking));
-  CU(cudaEventCreateWithFlags(&P->ev_fork, cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(&P->ev_eps, cudaEventDisableTiming));
-  if (P->double_buffer) {
+  P->overlap.double_buffer = false;
+  if (P->tune.force_overlap && P->sp_kind == SP_CSC && P->entries.strategy == 1 && (int64_t)P->colors.local.size() > slabs) P->overlap.double_buffer = true;
+  const size_t nbuf = P->overlap.double_buffer ? 2 : 1;
+  CU(cudaStreamCreateWithFlags(&P->overlap.side, cudaStreamNonBlocking));
+  CU(cudaEventCreateWithFlags(&P->overlap.ev_fork, cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(&P->overlap.ev_eps, cudaEventDisableTiming));
+  if (P->overlap.double_buffer) {
     for (int b = 0; b < 2; ++b) {
-      CU(cudaEventCreateWithFlags(&P->ev_f[b], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&P->ev_scat[b], cudaEventDisableTiming));
+      CU(cudaEventCreateWithFlags(&P->overlap.ev_f[b], cudaEventDisableTiming));
+      CU(cudaEventCreateWithFlags(&P->overlap.ev_scat[b], cudaEventDisableTiming));
     }
   }
-  TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
-  TRY(P->alloc_t(&P->Fp, nbuf * (size_t)slabs * P->ldF * cw));
-  TRY(P->alloc_t(&P->xp, (size_t)pbatch * P->ldx * cw));
+  TRY(P->alloc_t(&P->scratch.fx_own, (size_t)P->scratch.ldF));
+  TRY(P->alloc_t(&P->scratch.Fp, nbuf * (size_t)slabs * P->scratch.ldF * cw));
+  TRY(P->alloc_t(&P->scratch.xp, (size_t)pbatch * P->scratch.ldx * cw));
   if (central) {
-    TRY(P->alloc_t(&P->Fm, nbuf * (size_t)slabs * P->ldF));
-    TRY(P->alloc_t(&P->xm, (size_t)pbatch * P->ldx));
+    TRY(P->alloc_t(&P->scratch.Fm, nbuf * (size_t)slabs * P->scratch.ldF));
+    TRY(P->alloc_t(&P->scratch.xm, (size_t)pbatch * P->scratch.ldx));
   }
   return FDB_OK;
 }
@@ -581,8 +637,8 @@ static fdb_status finish_colored_plan(fdb_plan *P, const fdb_plan_opts *o, const
 // register path takes, the chunk tables of the list-based eps pass.
 static fdb_status build_color_lists(fdb_plan *P) {
   const int64_t n = P->n;
-  const int32_t C = P->C;
-  TRY(P->alloc_t(&P->cols_by_color, (size_t)std::max<int64_t>(n, 1)));
+  const int32_t C = P->colors.C;
+  TRY(P->alloc_t(&P->colors.cols_by_color, (size_t)std::max<int64_t>(n, 1)));
   std::vector<unsigned long long> bc((size_t)C + 1, 0);
   if (n > 0) {
     // a stable radix sort of the column ids by colour (deterministic: the list-based eps pass sums in list order, and
@@ -595,38 +651,38 @@ static fdb_status build_color_lists(fdb_plan *P) {
     TRY(k_in.alloc((size_t)n));
     TRY(k_out.alloc((size_t)n));
     TRY(v_in.alloc((size_t)n));
-    dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, d_bucket.get());
-      color_sort_keys<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, n, C, k_in.get(), v_in.get());
+      count_color_buckets<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, n, C, d_bucket.get());
+      color_sort_keys<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, n, C, k_in.get(), v_in.get());
       return FDB_OK;
     });
     int end_bit = 1;
     while (end_bit < 32 && ((uint64_t)1 << end_bit) <= (uint64_t)C) ++end_bit;
     TRY(cub_run([&](void *tmp, size_t &bytes) {
-      return cub::DeviceRadixSort::SortPairs(tmp, bytes, k_in.get(), k_out.get(), v_in.get(), P->cols_by_color, (int)n, 0, end_bit);
+      return cub::DeviceRadixSort::SortPairs(tmp, bytes, k_in.get(), k_out.get(), v_in.get(), P->colors.cols_by_color, (int)n, 0, end_bit);
     }));
     TRY(read_back(bc.data(), d_bucket.get(), (size_t)C + 1, "column lists"));
   }
-  P->bucket_start.assign((size_t)C + 2, 0);
-  for (int32_t k = 0; k <= C; ++k) P->bucket_start[(size_t)k + 1] = P->bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
+  P->colors.bucket_start.assign((size_t)C + 2, 0);
+  for (int32_t k = 0; k <= C; ++k) P->colors.bucket_start[(size_t)k + 1] = P->colors.bucket_start[(size_t)k] + (int64_t)bc[(size_t)k];
   // step sizes from the column lists (more colours than the register path takes)
   if (C > kEpsRegColors && C <= (1 << 22) && n > 0) {
     std::vector<int64_t> cb((size_t)C + 1, 0);
     int64_t maxc = 1;
     for (int32_t k = 0; k < C; ++k) {
-      const int64_t len = P->bucket_start[(size_t)k + 1] - P->bucket_start[(size_t)k];
+      const int64_t len = P->colors.bucket_start[(size_t)k + 1] - P->colors.bucket_start[(size_t)k];
       const int64_t nc = (len + kEpsListChunk - 1) / kEpsListChunk;
       cb[(size_t)k + 1] = cb[(size_t)k] + nc;
       maxc = std::max(maxc, nc);
     }
-    TRY(P->alloc_t(&P->bucket_start_d, (size_t)C + 2));
-    TRY(P->alloc_t(&P->chunk_base_d, (size_t)C + 1));
-    TRY(P->alloc_t(&P->eps_list_partial, (size_t)std::max<int64_t>(cb[(size_t)C], 1)));
-    CU(cudaMemcpy(P->bucket_start_d, P->bucket_start.data(), ((size_t)C + 2) * 8, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(P->chunk_base_d, cb.data(), ((size_t)C + 1) * 8, cudaMemcpyHostToDevice));
-    P->eps_list_max_chunks = maxc;
-    P->eps_lists = true;
+    TRY(P->alloc_t(&P->steps.bucket_start_d, (size_t)C + 2));
+    TRY(P->alloc_t(&P->steps.chunk_base_d, (size_t)C + 1));
+    TRY(P->alloc_t(&P->steps.list_partial, (size_t)std::max<int64_t>(cb[(size_t)C], 1)));
+    CU(cudaMemcpy(P->steps.bucket_start_d, P->colors.bucket_start.data(), ((size_t)C + 2) * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(P->steps.chunk_base_d, cb.data(), ((size_t)C + 1) * 8, cudaMemcpyHostToDevice));
+    P->steps.list_max_chunks = maxc;
+    P->steps.lists = true;
   }
   return FDB_OK;
 }
@@ -643,41 +699,41 @@ cm_gather_cols(const int32_t *__restrict__ cols_by_color, const int64_t *__restr
 
 // Colour-major entry lists of the colours this rank evaluates (CSC plans, strategy 1): see kernels_scatter.cuh.
 static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long long> &count /* entries per colour */) {
-  const int64_t n_local = (int64_t)P->local_colors.size();
-  const int32_t C = P->C;
-  const bool zero_bucket = P->rank == 0 && P->bucket_start[(size_t)C + 1] > P->bucket_start[(size_t)C];
+  const int64_t n_local = (int64_t)P->colors.local.size();
+  const int32_t C = P->colors.C;
+  const bool zero_bucket = P->rank == 0 && P->colors.bucket_start[(size_t)C + 1] > P->colors.bucket_start[(size_t)C];
   const int64_t nseg = n_local + (zero_bucket ? 1 : 0);
   std::vector<int64_t> src(std::max<int64_t>(nseg, 1), 0), dst((size_t)nseg + 1, 0);
-  P->cm_start_h.assign((size_t)n_local + 1, 0);
+  P->cm.start_h.assign((size_t)n_local + 1, 0);
   unsigned long long valid_total = 0;
   for (int32_t k = 0; k < C; ++k) valid_total += count[(size_t)k];
   for (int64_t li = 0; li < n_local; ++li) {
-    const int32_t k = P->local_colors[(size_t)li];
-    src[(size_t)li] = P->bucket_start[(size_t)k];
-    dst[(size_t)li + 1] = dst[(size_t)li] + (P->bucket_start[(size_t)k + 1] - P->bucket_start[(size_t)k]);
-    P->cm_start_h[(size_t)li + 1] = P->cm_start_h[(size_t)li] + (int64_t)count[(size_t)k];
+    const int32_t k = P->colors.local[(size_t)li];
+    src[(size_t)li] = P->colors.bucket_start[(size_t)k];
+    dst[(size_t)li + 1] = dst[(size_t)li] + (P->colors.bucket_start[(size_t)k + 1] - P->colors.bucket_start[(size_t)k]);
+    P->cm.start_h[(size_t)li + 1] = P->cm.start_h[(size_t)li] + (int64_t)count[(size_t)k];
   }
-  int64_t e_local = P->cm_start_h[(size_t)n_local];
-  P->cm_invalid_end = e_local;
+  int64_t e_local = P->cm.start_h[(size_t)n_local];
+  P->cm.invalid_end = e_local;
   if (zero_bucket) {
-    src[(size_t)n_local] = P->bucket_start[(size_t)C];
-    dst[(size_t)n_local + 1] = dst[(size_t)n_local] + (P->bucket_start[(size_t)C + 1] - P->bucket_start[(size_t)C]);
-    e_local += P->E - (int64_t)valid_total;
-    P->cm_invalid_end = e_local;
+    src[(size_t)n_local] = P->colors.bucket_start[(size_t)C];
+    dst[(size_t)n_local + 1] = dst[(size_t)n_local] + (P->colors.bucket_start[(size_t)C + 1] - P->colors.bucket_start[(size_t)C]);
+    e_local += P->colors.E - (int64_t)valid_total;
+    P->cm.invalid_end = e_local;
   }
   const int64_t ncols = dst[(size_t)nseg];
-  TRY(P->alloc_t(&P->cm_start, (size_t)n_local + 1));
-  CU(cudaMemcpy(P->cm_start, P->cm_start_h.data(), ((size_t)n_local + 1) * 8, cudaMemcpyHostToDevice));
-  TRY(P->alloc_t(&P->cm_row, (size_t)std::max<int64_t>(e_local, 1)));
+  TRY(P->alloc_t(&P->cm.start, (size_t)n_local + 1));
+  CU(cudaMemcpy(P->cm.start, P->cm.start_h.data(), ((size_t)n_local + 1) * 8, cudaMemcpyHostToDevice));
+  TRY(P->alloc_t(&P->cm.row, (size_t)std::max<int64_t>(e_local, 1)));
   {
     // only where f(x) would otherwise be dragged through DRAM once per launch: several launches per Jacobian (colours
     // sharded over GPUs, or more colours than resident slabs).  One launch over all colours reads f(x) once anyway: not
     // used there (it would cost E_local * 8 bytes more for no gain).
-    const bool want = P->n_groups > 1 || P->tune.force_fx_cm;
-    if (P->fdtype == FDB_FORWARD && e_local > 0 && want && !P->tune.no_fx_cm) TRY(P->alloc_t(&P->fx_cm, (size_t)e_local));
+    const bool want = P->scratch.n_groups > 1 || P->tune.force_fx_cm;
+    if (P->fdtype == FDB_FORWARD && e_local > 0 && want && !P->tune.no_fx_cm) TRY(P->alloc_t(&P->cm.fx, (size_t)e_local));
   }
-  const bool wide = P->dest != nullptr;
-  TRY(P->alloc(&P->cm_slot, (size_t)std::max<int64_t>(e_local, 1) * (wide ? 8 : 4)));
+  const bool wide = P->entries.dest != nullptr;
+  TRY(P->alloc(&P->cm.slot, (size_t)std::max<int64_t>(e_local, 1) * (wide ? 8 : 4)));
   if (ncols == 0 || e_local == 0) return FDB_OK;
   // temporaries: segment offsets, column list, counts, offsets
   DevBuf<int64_t> d_src, d_dst;
@@ -689,17 +745,17 @@ static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long lo
   TRY(list_off.alloc((size_t)ncols));
   CU(cudaMemcpy(d_src.get(), src.data(), (size_t)nseg * 8, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(d_dst.get(), dst.data(), ((size_t)nseg + 1) * 8, cudaMemcpyHostToDevice));
-  cm_gather_cols<<<(int)std::min<int64_t>(nseg, (int64_t)P->sm_count * 16), kThreads>>>(P->cols_by_color, d_src.get(), d_dst.get(), nseg, list_cols.get());
-  cm_column_counts<<<P->grid(ncols), kThreads>>>(list_cols.get(), ncols, P->colptr32, list_cnt.get());
+  cm_gather_cols<<<(int)std::min<int64_t>(nseg, (int64_t)P->sm_count * 16), kThreads>>>(P->colors.cols_by_color, d_src.get(), d_dst.get(), nseg, list_cols.get());
+  cm_column_counts<<<P->grid(ncols), kThreads>>>(list_cols.get(), ncols, P->entries.colptr32, list_cnt.get());
   TRY(cub_run([&](void *tmp, size_t &bytes) {
     return cub::DeviceScan::ExclusiveSum(tmp, bytes, list_cnt.get(), list_off.get(), (int)ncols);
   }));
   {
-    const int lanes = P->lanes;
+    const int lanes = P->entries.lanes;
     const int64_t blocks = (ncols + (kThreads / lanes) - 1) / (kThreads / lanes);
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)P->sm_count * 16));
-    if (wide) cm_expand<int64_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->colptr32, P->row32, P->dest, lanes, P->cm_row, (int64_t *)P->cm_slot);
-    else cm_expand<int32_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->colptr32, P->row32, nullptr, lanes, P->cm_row, (int32_t *)P->cm_slot);
+    if (wide) cm_expand<int64_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->entries.colptr32, P->entries.row32, P->entries.dest, lanes, P->cm.row, (int64_t *)P->cm.slot);
+    else cm_expand<int32_t><<<grid, kThreads>>>(list_cols.get(), list_off.get(), ncols, P->entries.colptr32, P->entries.row32, nullptr, lanes, P->cm.row, (int32_t *)P->cm.slot);
   }
   // consistency: the last column's end must be the entry total the per-colour counts promised
   int32_t last_off = 0, last_cnt = 0;
@@ -715,7 +771,7 @@ static fdb_status build_cm_lists(fdb_plan *P, const std::vector<unsigned long lo
 // Band form of the staged pass: the pattern is exactly the clipped band of some (l, u) — column c holds the rows
 // max(0, c-l) .. min(m-1, c+u), in order — so every entry's row and column follow from its position.
 static fdb_status try_band_form(fdb_plan *P) {
-  P->stage_band = false;
+  P->staged.band = false;
   const int64_t m = P->m, n = P->n;
   DevBuf<int> d_lu;
   DevBuf<uint32_t> d_flag;
@@ -724,38 +780,38 @@ static fdb_status try_band_form(fdb_plan *P) {
   const int init[2] = {INT_MIN, INT_MIN};
   CU(cudaMemcpy(d_lu.get(), init, sizeof init, cudaMemcpyHostToDevice));
   CU(cudaMemset(d_flag.get(), 0, 4));
-  band_extent<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, n, d_lu.get());
+  band_extent<<<P->grid(n), kThreads>>>(P->entries.colptr32, P->entries.row32, n, d_lu.get());
   int lu[2];
   TRY(read_back(lu, d_lu.get(), 2, "band extent"));
   const int l = lu[0], u = lu[1];
-  band_check<<<P->grid(n), kThreads>>>(P->colptr32, P->row32, m, n, l, u, d_flag.get());
+  band_check<<<P->grid(n), kThreads>>>(P->entries.colptr32, P->entries.row32, m, n, l, u, d_flag.get());
   uint32_t bad = 1;
   TRY(read_back(&bad, d_flag.get(), 1, "band check"));
   if (bad) return FDB_OK;
   // interior columns [a, b): c - l >= 0 and c + u <= m - 1 — every one holds all w = l + u + 1 rows
   const int64_t a = std::min<int64_t>(std::max(l, 0), n), b = std::max<int64_t>(a, std::min<int64_t>(n, m - u));
   int32_t ea = 0, eb = 0;
-  TRY(read_back(&ea, P->colptr32 + a, 1, "band column pointer"));
-  TRY(read_back(&eb, P->colptr32 + b, 1, "band column pointer"));
-  P->band_l = l;
-  P->band_w = l + u + 1;
-  P->band_col_a = (int32_t)a;
-  P->band_col_b = (int32_t)b;
-  P->band_e_a = ea;
-  P->band_e_b = eb;
-  P->stage_band = true;
+  TRY(read_back(&ea, P->entries.colptr32 + a, 1, "band column pointer"));
+  TRY(read_back(&eb, P->entries.colptr32 + b, 1, "band column pointer"));
+  P->staged.band_l = l;
+  P->staged.band_w = l + u + 1;
+  P->staged.band_col_a = (int32_t)a;
+  P->staged.band_col_b = (int32_t)b;
+  P->staged.band_e_a = ea;
+  P->staged.band_e_b = eb;
+  P->staged.band = true;
   return FDB_OK;
 }
 
 // TMA-staged fused pass: eligible when the whole Jacobian is one resident group on one rank, the destination is the
 // identity (CSC nzval) and every 1024-entry tile touches a short row window (row-local pattern).
 static fdb_status try_stage_plan(fdb_plan *P) {
-  P->staged = false;
+  P->staged.on = false;
   if (P->tune.no_staged) return FDB_OK;
-  if (P->sp_kind != SP_CSC || P->dest != nullptr || P->strategy != 0 || P->world != 1 || P->n_groups != 1) return FDB_OK;
-  if (P->fdtype == FDB_COMPLEX || P->C < 1) return FDB_OK;
-  const int nwin = P->fdtype == FDB_CENTRAL ? 2 * P->C : P->C + 1;
-  const int64_t ntiles = P->E / kTile;
+  if (P->sp_kind != SP_CSC || P->entries.dest != nullptr || P->entries.strategy != 0 || P->world != 1 || P->scratch.n_groups != 1) return FDB_OK;
+  if (P->fdtype == FDB_COMPLEX || P->colors.C < 1) return FDB_OK;
+  const int nwin = P->fdtype == FDB_CENTRAL ? 2 * P->colors.C : P->colors.C + 1;
+  const int64_t ntiles = P->colors.E / kTile;
   if (nwin > kStageMaxWin || ntiles < 1) return FDB_OK;
   // built here, kept by the plan only when the staged form is chosen
   DevBuf<unsigned int> d_span;
@@ -766,29 +822,29 @@ static fdb_status try_stage_plan(fdb_plan *P) {
   TRY(tile_w0.alloc((size_t)ntiles));
   TRY(row16.alloc((size_t)ntiles * kTile));
   const int pgrid = (int)std::min<int64_t>(ntiles, (int64_t)P->sm_count * 16);
-  stage_prepare<uint8_t><<<pgrid, kThreads>>>(P->row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), nullptr, P->C);
+  stage_prepare<uint8_t><<<pgrid, kThreads>>>(P->entries.row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), nullptr, P->colors.C);
   unsigned int span = 0;
   TRY(read_back(&span, d_span.get(), 1, "staged row span"));
   const int64_t W = ((int64_t)span + 1) & ~(int64_t)1;
   // few colours, short windows: pack the entry's colour into the top 4 bits of its row offset (no colour stream at all)
-  P->stage_packed = P->C <= 14 && W <= 4096 && span > 0 && !P->tune.no_pack;
-  if (P->stage_packed) {
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+  P->staged.packed = P->colors.C <= 14 && W <= 4096 && span > 0 && !P->tune.no_pack;
+  if (P->staged.packed) {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      stage_prepare<CT><<<pgrid, kThreads>>>(P->row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), (const CT *)P->ecolor, P->C);
+      stage_prepare<CT><<<pgrid, kThreads>>>(P->entries.row32, ntiles, tile_w0.get(), row16.get(), d_span.get(), (const CT *)P->entries.ecolor, P->colors.C);
       CU(cudaGetLastError());
       return FDB_OK;
     }));
     CU(cudaDeviceSynchronize());
   }
-  const size_t smem = (size_t)2 * nwin * W * 8 + kStageCtlBytes + (size_t)P->C * 8;
+  const size_t smem = (size_t)2 * nwin * W * 8 + kStageCtlBytes + (size_t)P->colors.C * 8;
   if (span == 0 || span > 65535 || smem > (size_t)kStageMaxSmem) return FDB_OK;   // not row-local enough: keep the gather form
-  P->adopt(P->tile_w0 = tile_w0.release(), tile_w0.bytes);
-  P->adopt(P->row16 = row16.release(), row16.bytes);
-  TRY(P->alloc_t(&P->stage_claim, 1));
-  CU(cudaMemset(P->stage_claim, 0, sizeof(unsigned long long)));
-  P->stage_W = (int32_t)W;
-  P->staged = true;
+  P->adopt(P->staged.tile_w0 = tile_w0.release(), tile_w0.bytes);
+  P->adopt(P->staged.row16 = row16.release(), row16.bytes);
+  TRY(P->alloc_t(&P->staged.claim, 1));
+  CU(cudaMemset(P->staged.claim, 0, sizeof(unsigned long long)));
+  P->staged.W = (int32_t)W;
+  P->staged.on = true;
   if (!P->tune.no_band) TRY(try_band_form(P));
   return FDB_OK;
 }
@@ -836,16 +892,17 @@ static void read_tunables(fdb_plan *P) {
 static void free_plan(fdb_plan *P) {
   if (!P) return;
   DeviceGuard g(P->device);
-  for (void *p : P->allocs) cudaFree(p);
-  for (auto &ev : P->ev_pending) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-  for (auto &ev : P->ev_pool) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-  if (P->hstream) cudaStreamDestroy(P->hstream);
-  if (P->side) cudaStreamDestroy(P->side);
-  for (int b = 0; b < 2; ++b) { if (P->ev_f[b]) cudaEventDestroy(P->ev_f[b]); if (P->ev_scat[b]) cudaEventDestroy(P->ev_scat[b]); }
-  if (P->ev_fork) cudaEventDestroy(P->ev_fork);
-  if (P->ev_eps) cudaEventDestroy(P->ev_eps);
-  if (P->graph_exec) cudaGraphExecDestroy(P->graph_exec);
-  if (P->cstream) cudaStreamDestroy(P->cstream);
+  for (void *p : P->allocs) cudaFree(p);   // the device buffers of every part
+  for (auto &ev : P->timing.pending) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
+  for (auto &ev : P->timing.pool) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
+  if (P->host.stream) cudaStreamDestroy(P->host.stream);
+  const auto &o = P->overlap;
+  if (o.side) cudaStreamDestroy(o.side);
+  for (int b = 0; b < 2; ++b) { if (o.ev_f[b]) cudaEventDestroy(o.ev_f[b]); if (o.ev_scat[b]) cudaEventDestroy(o.ev_scat[b]); }
+  if (o.ev_fork) cudaEventDestroy(o.ev_fork);
+  if (o.ev_eps) cudaEventDestroy(o.ev_eps);
+  if (P->graph.exec) cudaGraphExecDestroy(P->graph.exec);
+  if (P->graph.stream) cudaStreamDestroy(P->graph.stream);
   delete P;
 }
 
@@ -869,7 +926,7 @@ static fdb_status new_plan(fdb_plan **out, PlanPtr &P, const fdb_plan_opts *o, i
   P->n = n;
   P->fdtype = o ? o->fdtype : FDB_FORWARD;
   P->no_drift = o ? o->no_drift : 0;
-  P->use_graph = o && o->use_graph != 0;
+  P->graph.use = o && o->use_graph != 0;
   P->shared_J = o && o->shared_j != 0;
   read_tunables(P.get());
   P->world = (o && o->world > 1) ? o->world : 1;
@@ -951,18 +1008,18 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
   const int64_t nnz = last - 1;
   if (nnz < 0 || nnz > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported (must be in [0, 2^31))", (long long)nnz);
   if (nnz > 0 && !rowval) return fail(FDB_ERR_INVALID, "rowval is NULL");
-  P->E = nnz;
+  P->colors.E = nnz;
   TRY(view_i64(rowval, nnz, rv));
   TRY(setup_colors(P, colorvec));
 
   DevBuf<uint32_t> d_err;
   DevBuf<unsigned long long> d_cnt;
   TRY(d_err.alloc(1));
-  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
+  TRY(d_cnt.alloc(std::max<int32_t>(P->colors.C, 1)));
   CU(cudaMemset(d_err.get(), 0, 4));
-  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
-  TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
-  TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->colors.C, 1) * 8));
+  TRY(P->alloc_t(&P->entries.row32, std::max<int64_t>(nnz, 4)));
+  TRY(P->alloc(&P->entries.ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->colors.bits / 8) + 16));
 
   bool same_pattern = true;
   bool other_csc = false;
@@ -996,7 +1053,7 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
   DevBuf<int32_t> col32;
   if (need_dest) {
     TRY(col32.alloc(std::max<int64_t>(nnz, 1)));
-    TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
+    TRY(P->alloc_t(&P->entries.dest, std::max<int64_t>(nnz, 1)));
   }
   validate_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, nnz, d_err.get());
   TRY(read_plan_err(d_err.get(), "CSC sparsity"));
@@ -1005,39 +1062,39 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
     TRY(read_plan_err(d_err.get(), "J's CSC pattern"));
   }
   if (nnz > 0) {
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      const size_t hsm = P->C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->C, 1) * sizeof(unsigned int) : 0;
-      expand_csc<CT><<<P->grid(nnz), kThreads, hsm>>>(cp.d, rv.d, m, n, nnz, (const CT *)P->jcolor, P->C, P->row32,
-                                                 (CT *)P->ecolor, col32.get(), d_cnt.get(), d_err.get());
+      const size_t hsm = P->colors.C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->colors.C, 1) * sizeof(unsigned int) : 0;
+      expand_csc<CT><<<P->grid(nnz), kThreads, hsm>>>(cp.d, rv.d, m, n, nnz, (const CT *)P->colors.jcolor, P->colors.C, P->entries.row32,
+                                                 (CT *)P->entries.ecolor, col32.get(), d_cnt.get(), d_err.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
-    if (jkind == FDB_J_DENSE) dest_dense_from_rc<<<P->grid(nnz), kThreads>>>(P->row32, col32.get(), nnz, ldJ, P->dest);
-    else if (other_csc) dest_other_csc<<<P->grid(nnz), kThreads>>>(P->row32, col32.get(), nnz, jcp.d, jrv.d, P->dest, d_err.get());
+    if (jkind == FDB_J_DENSE) dest_dense_from_rc<<<P->grid(nnz), kThreads>>>(P->entries.row32, col32.get(), nnz, ldJ, P->entries.dest);
+    else if (other_csc) dest_other_csc<<<P->grid(nnz), kThreads>>>(P->entries.row32, col32.get(), nnz, jcp.d, jrv.d, P->entries.dest, d_err.get());
   }
   TRY(read_plan_err(d_err.get(), "CSC sparsity"));
-  std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
+  std::vector<unsigned long long> cnt(std::max<int32_t>(P->colors.C, 1), 0);
+  if (P->colors.C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C, "colour counts"));
   // ---- per-colour column lists + gather-locality metric -> scatter strategy
   {
-    const int32_t C = P->C;
+    const int32_t C = P->colors.C;
     DevBuf<unsigned long long> d_jump;
     TRY(d_jump.alloc(1));
     CU(cudaMemset(d_jump.get(), 0, 8));
-    TRY(P->alloc_t(&P->colptr32, (size_t)n + 1));
-    convert_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, P->colptr32);
+    TRY(P->alloc_t(&P->entries.colptr32, (size_t)n + 1));
+    convert_colptr<<<P->grid(n + 1), kThreads>>>(cp.d, n, P->entries.colptr32);
     TRY(build_color_lists(P));
     if (nnz > 1) {
-      row_jump_sum<<<P->grid(nnz), kThreads>>>(P->row32, nnz, d_jump.get());
+      row_jump_sum<<<P->grid(nnz), kThreads>>>(P->entries.row32, nnz, d_jump.get());
       unsigned long long js = 0;
       TRY(read_back(&js, d_jump.get(), 1, "row jump sum"));
-      P->mean_row_jump = (double)js / (double)(nnz - 1);
+      P->entries.mean_row_jump = (double)js / (double)(nnz - 1);
     }
     int lanes = 1;
     const double avg = n > 0 ? (double)nnz / (double)n : 1.0;
     while (lanes < 32 && lanes < avg) lanes *= 2;
-    P->lanes = lanes;
+    P->entries.lanes = lanes;
     // opts->strategy: 0 auto, 1 fused storage-order pass, 2 colour-major lists launched per group of resident colours,
     // 3 colour-major lists with every slab resident (one launch).  The lists are what a launch needs whenever it would
     // otherwise stream entries it does not own: several ranks sharing the colours, or more colours than resident slabs
@@ -1046,20 +1103,20 @@ fdb_status fdb_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int6
     bool per_color = P->world > 1;
     if (want == 1) per_color = false;
     if (want == 2 || want == 3) per_color = true;
-    P->lists_resident = want == 3;       // colour-major lists, all slabs resident, one launch at the end
+    P->entries.lists_resident = want == 3;       // colour-major lists, all slabs resident, one launch at the end
     // auto, one GPU, random pattern with many colours: colour-major lists with every slab resident (one launch) — the
     // colour-by-colour order keeps the gathers of a launch phase inside one 8m-byte slab + f(x) instead of spreading them
     // over C slabs at once.  That only pays while slab + f(x) stay in L2: on an H100 (50 MB) C4's 40 + 40 MB do not, and
     // the storage-order pass is the faster scatter there.  Row-local patterns stay fused / staged.
-    if (want == 0 && P->world == 1 && P->mean_row_jump > 4096.0 && C >= 16 && 16 * P->m <= P->l2_bytes) {
+    if (want == 0 && P->world == 1 && P->entries.mean_row_jump > 4096.0 && C >= 16 && 16 * P->m <= P->l2_bytes) {
       per_color = true;
-      P->lists_resident = true;
+      P->entries.lists_resident = true;
     }
-    P->strategy = per_color ? 1 : 0;
-    P->strategy_auto = want == 0;
+    P->entries.strategy = per_color ? 1 : 0;
+    P->entries.strategy_auto = want == 0;
   }
   TRY(finish_colored_plan(P, opts, cnt));
-  if (P->strategy == 1) TRY(build_cm_lists(P, cnt));
+  if (P->entries.strategy == 1) TRY(build_cm_lists(P, cnt));
   TRY(try_stage_plan(P));
   // SURVEY.md §8(d): B_alg = 32*nnz + 16*n + 8 (valid colouring; Int64 indices as at the ABI)
   P->alg_bytes = 32 * nnz + 16 * n + 8;
@@ -1080,7 +1137,7 @@ fdb_status fdb_plan_create_coo(fdb_plan **plan, int64_t m, int64_t n, int64_t nn
   if (jkind == FDB_J_DENSE && ldJ_or_jlen < m) return fail(FDB_ERR_INVALID, "ldJ < m");
   P->sp_kind = SP_COO;
   P->jkind = jkind;
-  P->E = nnz;
+  P->colors.E = nnz;
   if (jkind == FDB_J_DENSE) { P->ldJ = ldJ_or_jlen; P->j_len = ldJ_or_jlen * n; }
   else P->j_len = ldJ_or_jlen;
   I64View rv, cvw, sv;
@@ -1091,26 +1148,26 @@ fdb_status fdb_plan_create_coo(fdb_plan **plan, int64_t m, int64_t n, int64_t nn
   DevBuf<uint32_t> d_err;
   DevBuf<unsigned long long> d_cnt;
   TRY(d_err.alloc(1));
-  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
+  TRY(d_cnt.alloc(std::max<int32_t>(P->colors.C, 1)));
   CU(cudaMemset(d_err.get(), 0, 4));
-  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
-  TRY(P->alloc_t(&P->row32, std::max<int64_t>(nnz, 4)));
-  TRY(P->alloc(&P->ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->color_bits / 8) + 16));
-  TRY(P->alloc_t(&P->dest, std::max<int64_t>(nnz, 1)));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->colors.C, 1) * 8));
+  TRY(P->alloc_t(&P->entries.row32, std::max<int64_t>(nnz, 4)));
+  TRY(P->alloc(&P->entries.ecolor, (size_t)std::max<int64_t>(nnz, 4) * (P->colors.bits / 8) + 16));
+  TRY(P->alloc_t(&P->entries.dest, std::max<int64_t>(nnz, 1)));
   if (nnz > 0) {
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      const size_t hsm = P->C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->C, 1) * sizeof(unsigned int) : 0;
+      const size_t hsm = P->colors.C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->colors.C, 1) * sizeof(unsigned int) : 0;
       prepare_coo<CT><<<P->grid(nnz), kThreads, hsm>>>(rv.d, cvw.d, jkind == FDB_J_SLOTS ? sv.d : nullptr, nnz, m, n, P->ldJ,
-                                                  P->j_len, (const CT *)P->jcolor, P->C, P->row32, (CT *)P->ecolor,
-                                                  P->dest, d_cnt.get(), d_err.get());
+                                                  P->j_len, (const CT *)P->colors.jcolor, P->colors.C, P->entries.row32, (CT *)P->entries.ecolor,
+                                                  P->entries.dest, d_cnt.get(), d_err.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
   }
   TRY(read_plan_err(d_err.get(), "COO sparsity"));
-  std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
+  std::vector<unsigned long long> cnt(std::max<int32_t>(P->colors.C, 1), 0);
+  if (P->colors.C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C, "colour counts"));
   TRY(finish_colored_plan(P, opts, cnt));
   P->alg_bytes = 32 * nnz + 16 * n + 8;
   return finish_plan(owner, plan);
@@ -1136,30 +1193,30 @@ fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t
   }
   P->sp_kind = SP_BANDED;
   P->jkind = jkind;
-  P->l = l;
-  P->u = u;
+  P->band.l = l;
+  P->band.u = u;
   P->ldJ = ldJ;
   P->j_len = jkind == FDB_J_BAND ? (l + u + 1) * n : (jkind == FDB_J_DIAGONALS ? diag_len : ldJ * n);
   TRY(setup_colors(P, colorvec));
   DevBuf<unsigned long long> d_cnt;
-  TRY(d_cnt.alloc(std::max<int32_t>(P->C, 1)));
-  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->C, 1) * 8));
-  if (n > 0 && P->C > 0) {
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+  TRY(d_cnt.alloc(std::max<int32_t>(P->colors.C, 1)));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->colors.C, 1) * 8));
+  if (n > 0 && P->colors.C > 0) {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      count_band_colors<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, m, n, l, u, P->C, d_cnt.get());
+      count_band_colors<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, m, n, l, u, P->colors.C, d_cnt.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
   }
-  std::vector<unsigned long long> cnt(std::max<int32_t>(P->C, 1), 0);
-  if (P->C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C, "colour counts"));
+  std::vector<unsigned long long> cnt(std::max<int32_t>(P->colors.C, 1), 0);
+  if (P->colors.C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C, "colour counts"));
   unsigned long long total = 0;
   for (auto c : cnt) total += c;
-  P->E = (int64_t)total;
+  P->colors.E = (int64_t)total;
   TRY(finish_colored_plan(P, opts, cnt));
   // SURVEY.md §8(d) banded: 8*sum_c band_len(c) written + 16*m*C read (diagonal storage: every slot written once)
-  P->alg_bytes = (jkind == FDB_J_DIAGONALS ? 8 * diag_len : 8 * (int64_t)total) + 16 * m * (int64_t)P->C;
+  P->alg_bytes = (jkind == FDB_J_DIAGONALS ? 8 * diag_len : 8 * (int64_t)total) + 16 * m * (int64_t)P->colors.C;
   return finish_plan(owner, plan);
 }
 
@@ -1202,45 +1259,45 @@ fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const 
   DeviceGuard g(P->device);
   P->sp_kind = SP_BLOCKBAND;
   P->jkind = FDB_J_BLOCK_BAND;
-  P->l = l;
-  P->u = u;
-  P->bb_lam = lam;
-  P->bb_mu = mu;
-  P->bb_w = w;
-  P->bb_nblocks = (int32_t)nblocks;
+  P->band.l = l;
+  P->band.u = u;
+  P->block_band.lam = lam;
+  P->block_band.mu = mu;
+  P->block_band.w = w;
+  P->block_band.nblocks = (int32_t)nblocks;
   P->j_len = w * n;
-  P->bb_bs = nblocks > 0 && hb[0] > 0 && std::all_of(hb.begin(), hb.end(), [&](int64_t b) { return b == hb[0]; }) ? (int32_t)hb[0] : 0;
-  TRY(P->alloc_t(&P->bb_off, (size_t)nblocks + 1));
-  CU(cudaMemcpy(P->bb_off, off.data(), ((size_t)nblocks + 1) * 4, cudaMemcpyHostToDevice));
+  P->block_band.bs = nblocks > 0 && hb[0] > 0 && std::all_of(hb.begin(), hb.end(), [&](int64_t b) { return b == hb[0]; }) ? (int32_t)hb[0] : 0;
+  TRY(P->alloc_t(&P->block_band.off, (size_t)nblocks + 1));
+  CU(cudaMemcpy(P->block_band.off, off.data(), ((size_t)nblocks + 1) * 4, cudaMemcpyHostToDevice));
   TRY(setup_colors(P, colorvec));
   // structural entries per colour (the LPT weights; slot C: columns without a valid colour) and the colouring's form
   DevBuf<unsigned long long> d_cnt;
   DevBuf<uint32_t> d_flag;
-  TRY(d_cnt.alloc((size_t)P->C + 1));
+  TRY(d_cnt.alloc((size_t)P->colors.C + 1));
   TRY(d_flag.alloc(1));
-  CU(cudaMemset(d_cnt.get(), 0, ((size_t)P->C + 1) * 8));
+  CU(cudaMemset(d_cnt.get(), 0, ((size_t)P->colors.C + 1) * 8));
   CU(cudaMemset(d_flag.get(), 0, 4));
   if (n > 0) {
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       using CT = decltype(tag);
-      block_band_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->jcolor, P->bb_off, (int32_t)nblocks, (int32_t)n, l, u,
-                                                        lam, mu, P->C, d_cnt.get(), d_flag.get());
+      block_band_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, P->block_band.off, (int32_t)nblocks, (int32_t)n, l, u,
+                                                        lam, mu, P->colors.C, d_cnt.get(), d_flag.get());
       CU(cudaGetLastError());
       return FDB_OK;
     }));
   }
-  std::vector<unsigned long long> cnt((size_t)P->C + 1, 0);
-  TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->C + 1, "block-banded entry counts"));
+  std::vector<unsigned long long> cnt((size_t)P->colors.C + 1, 0);
+  TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C + 1, "block-banded entry counts"));
   uint32_t not_cyclic = 1;
   TRY(read_back(&not_cyclic, d_flag.get(), 1, "block-banded colouring form"));
-  P->bb_cyclic = n > 0 && P->C > 0 && not_cyclic == 0;
+  P->block_band.cyclic = n > 0 && P->colors.C > 0 && not_cyclic == 0;
   unsigned long long total = 0;
   for (auto c : cnt) total += c;
-  P->E = (int64_t)total;
-  cnt.resize((size_t)std::max<int32_t>(P->C, 1));
+  P->colors.E = (int64_t)total;
+  cnt.resize((size_t)std::max<int32_t>(P->colors.C, 1));
   TRY(finish_colored_plan(P, opts, cnt));
   // every slot written once + the f! outputs read (one slab and f(x) / the minus slab per colour)
-  P->alg_bytes = 8 * w * n + 16 * n * (int64_t)P->C;
+  P->alg_bytes = 8 * w * n + 16 * n * (int64_t)P->colors.C;
   return finish_plan(owner, plan);
 }
 
@@ -1256,30 +1313,28 @@ static fdb_status create_dense(fdb_plan **plan, int64_t m, int64_t n, int64_t ld
   P->ldJ = ldJ;
   // contiguous column blocks per rank (SURVEY.md §8e)
   const int64_t per = (ncols + P->world - 1) / P->world;
-  P->col_begin = std::min<int64_t>(ncols, per * P->rank);
-  P->col_end = std::min<int64_t>(ncols, P->col_begin + per);
-  const int64_t ncl = P->col_end - P->col_begin;
+  P->columns.begin = std::min<int64_t>(ncols, per * P->rank);
+  P->columns.end = std::min<int64_t>(ncols, P->columns.begin + per);
+  const int64_t ncl = P->columns.end - P->columns.begin;
   P->j_len = ldJ * ncl;
-  P->E = m * ncl;
-  P->C = (int32_t)n;
   const bool central = P->fdtype == FDB_CENTRAL;
-  P->ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
-  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  P->scratch.ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
+  P->scratch.ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
   int64_t batch = (opts && opts->max_batch > 1) ? opts->max_batch : 1;
   int64_t budget = (opts && opts->scratch_bytes > 0) ? opts->scratch_bytes : (int64_t)8 << 30;
   const int64_t cw = P->fdtype == FDB_COMPLEX ? 2 : 1;
-  const int64_t per_point = 8 * cw * (P->ldx + P->ldF * (central ? 2 : 1));
+  const int64_t per_point = 8 * cw * (P->scratch.ldx + P->scratch.ldF * (central ? 2 : 1));
   batch = std::max<int64_t>(1, std::min<int64_t>(batch, budget / per_point));
   batch = std::min<int64_t>(batch, std::max<int64_t>(ncl, 1));
   batch = std::min<int64_t>(batch, 65535);   // gridDim.y of diff_columns
-  P->batch = batch;
-  P->slabs = batch;
-  P->n_groups = ncl == 0 ? 0 : (ncl + batch - 1) / batch;
-  TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
-  TRY(P->alloc_t(&P->Fp, (size_t)batch * P->ldF * cw));
-  if (central) TRY(P->alloc_t(&P->Fm, (size_t)batch * P->ldF));
-  TRY(P->alloc_t(&P->xp, (size_t)batch * P->ldx * cw));
-  TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(ncl, 1)));
+  P->scratch.batch = batch;
+  P->scratch.slabs = batch;
+  P->scratch.n_groups = ncl == 0 ? 0 : (ncl + batch - 1) / batch;
+  TRY(P->alloc_t(&P->scratch.fx_own, (size_t)P->scratch.ldF));
+  TRY(P->alloc_t(&P->scratch.Fp, (size_t)batch * P->scratch.ldF * cw));
+  if (central) TRY(P->alloc_t(&P->scratch.Fm, (size_t)batch * P->scratch.ldF));
+  TRY(P->alloc_t(&P->scratch.xp, (size_t)batch * P->scratch.ldx * cw));
+  TRY(P->alloc_t(&P->columns.eps, (size_t)std::max<int64_t>(ncl, 1)));
   // SURVEY.md §8(d) dense: 24*m per column
   P->alg_bytes = 24 * m * ncl;
   *plan = owner.release();
@@ -1319,9 +1374,24 @@ fdb_status fdb_plan_destroy(fdb_plan *plan) {
   return FDB_OK;
 }
 
+// the part of the whole problem this rank evaluates, as the ABI reports it (fdb_plan_info, fdb_plan_dense_range): a dense
+// plan's columns, a Hessian plan's i-blocks, and nothing for the other kinds
+static std::pair<int64_t, int64_t> own_range(const fdb_plan *P) {
+  if (P->sp_kind == SP_NONE) return {P->columns.begin, P->columns.end};
+  if (P->sp_kind == SP_HESS) return {P->hess.i_begin, P->hess.i_end};
+  return {0, 0};
+}
+
+// colours this rank evaluates (dense and Hessian plans: columns / i-blocks, counted as colours)
+static int64_t local_units(const fdb_plan *P) {
+  if (P->sp_kind != SP_NONE && P->sp_kind != SP_HESS) return (int64_t)P->colors.local.size();
+  const auto r = own_range(P);
+  return r.second - r.first;
+}
+
 // an out-of-place rank > 0 that owns no colour (dense branch: no column): it calls nothing and launches nothing
 static bool oop_idle(const fdb_plan *P) {
-  return P->oop && P->rank > 0 && (P->sp_kind == SP_NONE ? P->col_end == P->col_begin : P->local_colors.empty());
+  return P->oop.on && P->rank > 0 && local_units(P) == 0;
 }
 
 fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
@@ -1329,50 +1399,56 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
   memset(info, 0, sizeof *info);
   info->m = P->m;
   info->n = P->n;
-  info->n_entries = P->E;
   info->j_len = P->j_len;
-  info->n_colors = P->C;
-  const int64_t n_local = (P->sp_kind == SP_NONE || P->sp_kind == SP_HESS) ? P->col_end - P->col_begin
-                                                                           : (int64_t)P->local_colors.size();
+  const int64_t n_local = local_units(P);
   info->n_local_colors = n_local;
-  info->n_groups = P->n_groups;
-  info->slabs = P->slabs;
+  switch (P->sp_kind) {   // maximum(colorvec) and the entries the scatter writes, by kind
+    case SP_NONE:   // every column its own colour; out-of-place: the candidates of the whole result
+      info->n_colors = P->n;
+      info->n_entries = P->oop.on ? P->m * P->oop.qcols : P->m * n_local;
+      break;
+    case SP_HESS: info->n_colors = P->n; info->n_entries = P->hess.entries; break;
+    case SP_JVP: info->n_colors = 1; break;
+    case SP_DERIV: info->n_entries = P->m; break;
+    default:   // coloured and step-size plans; out-of-place band: every in-matrix band entry
+      info->n_colors = P->colors.C;
+      info->n_entries = P->oop.on && P->sp_kind == SP_BANDED ? P->oop.band_nnz : P->colors.E;
+  }
+  info->n_groups = P->scratch.n_groups;
+  info->slabs = P->scratch.slabs;
   info->fcalls_per_jacobian = P->fdtype == FDB_CENTRAL ? 2 * n_local : (P->fdtype == FDB_COMPLEX ? n_local : 1 + n_local);
-  if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = P->hess_points;
-  if (P->sp_kind == SP_DERIV) info->fcalls_per_jacobian = P->deriv_fcalls;
+  if (P->sp_kind == SP_HESS) info->fcalls_per_jacobian = P->hess.points;
+  if (P->sp_kind == SP_DERIV) info->fcalls_per_jacobian = P->deriv.fcalls;
   if (oop_idle(P)) info->fcalls_per_jacobian = 0;
-  // out-of-place dense branch: the candidate count of the whole result (a rank's E is its own block)
-  if (P->oop && P->sp_kind == SP_NONE) info->n_entries = P->m * P->oop_qcols;
-  if (P->oop && P->sp_kind == SP_BANDED) info->n_entries = P->oop_band_nnz;
   info->device_bytes = (int64_t)P->device_bytes;
   info->fdtype = P->fdtype;
   info->jkind = P->jkind;
   info->sp_kind = P->sp_kind;
-  info->color_bits = P->color_bits;
+  info->color_bits = P->colors.bits;
   info->alg_bytes_scatter = P->alg_bytes;
-  info->strategy = P->strategy;
-  info->lanes = P->lanes;
-  info->mean_row_jump = P->mean_row_jump;
-  info->staged = P->staged ? 1 : 0;
-  info->lists_resident = P->lists_resident ? 1 : 0;
+  info->strategy = P->entries.strategy;
+  info->lanes = P->entries.lanes;
+  info->mean_row_jump = P->entries.mean_row_jump;
+  info->staged = P->staged.on ? 1 : 0;
+  info->lists_resident = P->entries.lists_resident ? 1 : 0;
   {
     // compulsory bytes of the formulation that runs (see the header); slabs read per entry: 1 (forward / complex), 2 (central)
-    const int64_t ct = P->color_bits / 8;
+    const int64_t ct = P->colors.bits / 8;
     const int64_t slabs_read = P->fdtype == FDB_CENTRAL ? 2 : 1;
     const int64_t fx_once = P->fdtype == FDB_FORWARD ? 8 * P->m : 0;
     if (P->sp_kind == SP_CSC || P->sp_kind == SP_COO) {
-      if (P->sp_kind == SP_CSC && P->strategy == 1) {
-        const int64_t e_local = P->cm_start_h.empty() ? 0 : P->cm_start_h.back();
-        info->moved_bytes_scatter = e_local * (4 + (P->dest ? 8 : 4) + 8 * slabs_read + 8) + fx_once + (P->fx_cm ? e_local * (4 + 8 + 8) : 0);
+      if (P->sp_kind == SP_CSC && P->entries.strategy == 1) {
+        const int64_t e_local = P->cm.start_h.empty() ? 0 : P->cm.start_h.back();
+        info->moved_bytes_scatter = e_local * (4 + (P->entries.dest ? 8 : 4) + 8 * slabs_read + 8) + fx_once + (P->cm.fx ? e_local * (4 + 8 + 8) : 0);
       } else {
-        const int64_t C = std::max<int32_t>(P->C, 1);
-        const int64_t owned = P->world > 1 ? P->E * (int64_t)P->local_colors.size() / C : P->E;   // approx. share
-        info->moved_bytes_scatter = P->E * (4 + ct) * std::max<int64_t>(P->n_groups, 1) + owned * (8 * slabs_read + 8 + (P->dest ? 8 : 0)) + fx_once;
-        const int64_t staged_rows = 8 * P->m * (int64_t)(P->fdtype == FDB_CENTRAL ? 2 * P->C : P->C + 1);
-        if (P->staged && P->stage_band)   // no index stream; the column colour table unless the colouring is cyclic
-          info->moved_bytes_scatter = 8 * P->E + staged_rows + (P->cyclic ? 0 : P->n * ct);
-        else if (P->staged)   // 16-bit row offsets; every slab row and f(x) row staged once
-          info->moved_bytes_scatter = P->E * (2 + (P->stage_packed ? 0 : ct) + 8) + staged_rows;
+        const int64_t C = std::max<int32_t>(P->colors.C, 1);
+        const int64_t owned = P->world > 1 ? P->colors.E * (int64_t)P->colors.local.size() / C : P->colors.E;   // approx. share
+        info->moved_bytes_scatter = P->colors.E * (4 + ct) * std::max<int64_t>(P->scratch.n_groups, 1) + owned * (8 * slabs_read + 8 + (P->entries.dest ? 8 : 0)) + fx_once;
+        const int64_t staged_rows = 8 * P->m * (int64_t)(P->fdtype == FDB_CENTRAL ? 2 * P->colors.C : P->colors.C + 1);
+        if (P->staged.on && P->staged.band)   // no index stream; the column colour table unless the colouring is cyclic
+          info->moved_bytes_scatter = 8 * P->colors.E + staged_rows + (P->colors.cyclic ? 0 : P->n * ct);
+        else if (P->staged.on)   // 16-bit row offsets; every slab row and f(x) row staged once
+          info->moved_bytes_scatter = P->colors.E * (2 + (P->staged.packed ? 0 : ct) + 8) + staged_rows;
       }
     } else {
       info->moved_bytes_scatter = P->alg_bytes;
@@ -1389,16 +1465,17 @@ fdb_status fdb_plan_counters(const fdb_plan *P, fdb_counters_t *out) {
 
 fdb_status fdb_plan_dense_range(const fdb_plan *P, int64_t *b, int64_t *e) {
   if (!P || !b || !e) return fail(FDB_ERR_INVALID, "NULL argument");
-  *b = P->col_begin;
-  *e = P->col_end;
+  const auto r = own_range(P);
+  *b = r.first;
+  *e = r.second;
   return FDB_OK;
 }
 
 fdb_status fdb_plan_color_owner(const fdb_plan *P, int32_t *owner_out, int64_t cap) {
   if (!P || !owner_out) return fail(FDB_ERR_INVALID, "NULL argument");
   TRY(check_call(P, Call::color_owner));
-  if (cap < (int64_t)P->owner.size()) return fail(FDB_ERR_INVALID, "owner_out too small");
-  std::copy(P->owner.begin(), P->owner.end(), owner_out);
+  if (cap < (int64_t)P->colors.owner.size()) return fail(FDB_ERR_INVALID, "owner_out too small");
+  std::copy(P->colors.owner.begin(), P->colors.owner.end(), owner_out);
   return FDB_OK;
 }
 
@@ -1406,11 +1483,13 @@ fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *strea
   if (!P || !h_eps) return fail(FDB_ERR_INVALID, "NULL argument");
   TRY(check_call(P, Call::get_eps));
   DeviceGuard g(P->device);
-  // JVP plans: C == 1; Hessian plans: the steps of the rank's components [col_begin, col_end) (eps_cols holds all n)
-  const bool per_column = P->sp_kind == SP_NONE || P->sp_kind == SP_HESS;
-  const int64_t count = per_column ? P->col_end - P->col_begin : P->C;
+  // dense plans: the steps of the rank's columns; Hessian plans: those of the rank's components (hess.eps holds all n);
+  // JVP plans: the one step; coloured and step-size plans: one per colour
+  const double *src = P->steps.eps;
+  int64_t count = P->sp_kind == SP_JVP ? 1 : P->colors.C;
+  if (P->sp_kind == SP_NONE) { src = P->columns.eps; count = local_units(P); }
+  if (P->sp_kind == SP_HESS) { src = P->hess.eps + P->hess.i_begin; count = local_units(P); }
   if (cap < count) return fail(FDB_ERR_INVALID, "h_eps too small (%lld < %lld)", (long long)cap, (long long)count);
-  const double *src = per_column ? P->eps_cols + (P->sp_kind == SP_HESS ? P->col_begin : 0) : P->eps;
   if (count > 0) {
     CU(cudaMemcpyAsync(h_eps, src, (size_t)count * 8, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     CU(cudaStreamSynchronize((cudaStream_t)stream));
@@ -1420,7 +1499,7 @@ fdb_status fdb_plan_get_eps(fdb_plan *P, double *h_eps, int64_t cap, void *strea
 
 fdb_status fdb_plan_enable_timing(fdb_plan *P, int enable) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
-  P->timing = enable != 0;
+  P->timing.on = enable != 0;
   return FDB_OK;
 }
 
@@ -1429,15 +1508,15 @@ fdb_status fdb_plan_read_timing(fdb_plan *P, double *scatter_ms, int64_t *scatte
   DeviceGuard g(P->device);
   double total = 0.0;
   int64_t count = 0;
-  for (auto &ev : P->ev_pending) {
+  for (auto &ev : P->timing.pending) {
     CU(cudaEventSynchronize(ev.second));
     float ms = 0.f;
     CU(cudaEventElapsedTime(&ms, ev.first, ev.second));
     total += ms;
     count += 1;
-    P->ev_pool.push_back(ev);
+    P->timing.pool.push_back(ev);
   }
-  P->ev_pending.clear();
+  P->timing.pending.clear();
   *scatter_ms = total;
   *scatter_launches = count;
   return FDB_OK;
@@ -1448,13 +1527,13 @@ fdb_status fdb_plan_set_peers(fdb_plan *P, int n_peers, double *const *peer_J) {
   if (n_peers < 0 || n_peers > 64) return fail(FDB_ERR_INVALID, "n_peers out of range");
   TRY(check_call(P, Call::set_peers));
   DeviceGuard g(P->device);
-  if (!P->d_peers) TRY(P->alloc_t(&P->d_peers, 64));
-  if (n_peers > 0) CU(cudaMemcpy(P->d_peers, peer_J, (size_t)n_peers * sizeof(double *), cudaMemcpyHostToDevice));
-  P->n_peers = n_peers;
-  P->peer_generation += 1;
-  P->peers_aligned = true;
+  if (!P->peers.d) TRY(P->alloc_t(&P->peers.d, 64));
+  if (n_peers > 0) CU(cudaMemcpy(P->peers.d, peer_J, (size_t)n_peers * sizeof(double *), cudaMemcpyHostToDevice));
+  P->peers.n = n_peers;
+  P->peers.generation += 1;
+  P->peers.aligned = true;
   for (int i = 0; i < n_peers; ++i)
-    if (reinterpret_cast<uintptr_t>(peer_J[i]) & 15) P->peers_aligned = false;
+    if (reinterpret_cast<uintptr_t>(peer_J[i]) & 15) P->peers.aligned = false;
   return FDB_OK;
 }
 
@@ -1466,15 +1545,15 @@ struct ScatterTimer {
   cudaStream_t s;
   std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
   ScatterTimer(fdb_plan *p, cudaStream_t st) : P(p), s(st) {
-    if (!P->timing) return;
-    if (!P->ev_pool.empty()) { ev = P->ev_pool.back(); P->ev_pool.pop_back(); }
+    if (!P->timing.on) return;
+    if (!P->timing.pool.empty()) { ev = P->timing.pool.back(); P->timing.pool.pop_back(); }
     else { cudaEventCreate(&ev.first); cudaEventCreate(&ev.second); }
     cudaEventRecord(ev.first, s);
   }
   ~ScatterTimer() {
-    if (!P->timing || !ev.first) return;
+    if (!P->timing.on || !ev.first) return;
     cudaEventRecord(ev.second, s);
-    P->ev_pending.push_back(ev);
+    P->timing.pending.push_back(ev);
   }
 };
 
@@ -1482,7 +1561,7 @@ struct ScatterTimer {
 // rows [0, m) of every column belong to J — the padding rows between the columns are not touched.
 static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
   if (P->jkind == FDB_J_DENSE && P->ldJ > P->m) {
-    const int64_t ncols = P->sp_kind == SP_NONE ? P->col_end - P->col_begin : P->n;
+    const int64_t ncols = P->sp_kind == SP_NONE ? P->columns.end - P->columns.begin : P->n;
     if (P->m > 0 && ncols > 0)
       CU(cudaMemset2DAsync(J, (size_t)P->ldJ * 8, 0, (size_t)P->m * 8, (size_t)ncols, s));
     return FDB_OK;
@@ -1493,12 +1572,12 @@ static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
 
 // How a coloured plan turns a group's f! outputs into J: one launcher per family (scatter_lists ... scatter_entries), and
 // none for an out-of-place sparse result whose compaction forms the quotients itself (fdjac_oop.cuh).  Fixed once the
-// plan is built, but derived rather than stored: the out-of-place creators set oop_fused after the in-place creator.
+// plan is built, but derived rather than stored: the out-of-place creators set oop.fused after the in-place creator.
 enum class Scatter { none, lists, block_band, diagonals, band, entries };
 
 static Scatter scatter_family(const fdb_plan *P) {
-  if (P->oop_fused) return Scatter::none;
-  if (P->sp_kind == SP_CSC && P->strategy == 1) return Scatter::lists;
+  if (P->oop.fused) return Scatter::none;
+  if (P->sp_kind == SP_CSC && P->entries.strategy == 1) return Scatter::lists;
   if (P->sp_kind == SP_BLOCKBAND) return Scatter::block_band;
   if (P->sp_kind == SP_BANDED) return P->jkind == FDB_J_DIAGONALS ? Scatter::diagonals : Scatter::band;
   return Scatter::entries;
@@ -1511,12 +1590,12 @@ static bool scatter_defines_J(const fdb_plan *P, int64_t colours) {
   const Scatter f = scatter_family(P);
   if (f == Scatter::none || f == Scatter::block_band) return true;
   if (f == Scatter::band && P->jkind != FDB_J_BAND) return false;   // a dense J
-  if ((f == Scatter::lists || f == Scatter::entries) && P->dest != nullptr) return false;   // explicit destinations
+  if ((f == Scatter::lists || f == Scatter::entries) && P->entries.dest != nullptr) return false;   // explicit destinations
   return colours > 0;
 }
 
 static fdb_status call_f(fdb_plan *P, fdb_fn f, void *ctx, double *fx, const double *x, int64_t batch, cudaStream_t s) {
-  const int rc = f(ctx, fx, x, batch, P->ldF, P->ldx, (void *)s);
+  const int rc = f(ctx, fx, x, batch, P->scratch.ldF, P->scratch.ldx, (void *)s);
   P->cnt.f_invocations += 1;
   P->cnt.f_points += batch;
   if (rc != 0) return fail(FDB_ERR_CALLBACK, "user f! returned %d", rc);
@@ -1553,7 +1632,7 @@ static void launch_resident(const fdb_plan *P, void (*kern)(KArgs...), int64_t w
 
 // dynamic shared memory of a scatter that stages its per-colour (step size, slab) tables: none past kSmemTable colours
 static size_t color_table_smem(const fdb_plan *P) {
-  return P->C <= kSmemTable ? (size_t)P->C * (sizeof(double) + sizeof(int32_t)) : 0;
+  return P->colors.C <= kSmemTable ? (size_t)P->colors.C * (sizeof(double) + sizeof(int32_t)) : 0;
 }
 
 // Programmatic dependent launch: the kernel may be scheduled while the kernel before it on the stream drains, and runs
@@ -1576,22 +1655,22 @@ static cudaError_t launch_pdl(void (*kern)(KArgs...), int grid, size_t smem, cud
 
 template <typename CT>
 static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double absstep, double dir, cudaStream_t s) {
-  const int32_t C = P->C;
+  const int32_t C = P->colors.C;
   if (C <= 0) return FDB_OK;
   if (P->fdtype == FDB_COMPLEX) {   // epsilon = eps(eltype(x))  jacobians.jl:624 — the same for every colour
-    fill_value<<<(C + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->eps, C, DBL_EPSILON);
+    fill_value<<<(C + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->steps.eps, C, DBL_EPSILON);
     P->cnt.kernel_launches += 1;
     CU(cudaGetLastError());
     return FDB_OK;
   }
   // out-of-place plans take the forward rule, dir included, in central mode too (jacobians.jl:379-380)
-  EpsParams prm{P->fdtype == FDB_CENTRAL && !P->oop ? 1 : 0, relstep, absstep, dir};
-  if (P->eps_lists) {
+  EpsParams prm{P->fdtype == FDB_CENTRAL && !P->oop.on ? 1 : 0, relstep, absstep, dir};
+  if (P->steps.lists) {
     if (!P->tune.no_eps_lists) {
-      dim3 grid((unsigned)std::min<int64_t>(P->eps_list_max_chunks, 1024), (unsigned)std::min<int32_t>(C, 65535));
-      color_sumsq_lists<<<grid, kThreads, 0, s>>>(x, P->cols_by_color, P->bucket_start_d, P->chunk_base_d, C, P->eps_list_partial);
+      dim3 grid((unsigned)std::min<int64_t>(P->steps.list_max_chunks, 1024), (unsigned)std::min<int32_t>(C, 65535));
+      color_sumsq_lists<<<grid, kThreads, 0, s>>>(x, P->colors.cols_by_color, P->steps.bucket_start_d, P->steps.chunk_base_d, C, P->steps.list_partial);
       finalize_eps_lists<<<(int)std::min<int64_t>(((int64_t)C * 32 + kThreads - 1) / kThreads, (int64_t)P->sm_count * 8), kThreads, 0, s>>>(
-          P->eps_list_partial, P->chunk_base_d, C, prm, P->eps, P->sumsq, x, P->cols_by_color, P->bucket_start_d, P->n);
+          P->steps.list_partial, P->steps.chunk_base_d, C, prm, P->steps.eps, P->steps.sumsq, x, P->colors.cols_by_color, P->steps.bucket_start_d, P->n);
       P->cnt.kernel_launches += 2;
       CU(cudaGetLastError());
       return FDB_OK;
@@ -1603,8 +1682,8 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
     TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
       using CS = decltype(cs);
       auto go = [&](auto kern) {
-        const int grid = std::min(resident_grid(P, kern, 0, ntiles), P->eps_blocks);  // partial capacity
-        kern<<<grid, kThreads, 0, s>>>(x, cs, P->n, aligned, C, prm, P->partial, P->ticket, P->eps, P->sumsq);
+        const int grid = std::min(resident_grid(P, kern, 0, ntiles), P->steps.blocks);  // partial capacity
+        kern<<<grid, kThreads, 0, s>>>(x, cs, P->n, aligned, C, prm, P->steps.partial, P->steps.ticket, P->steps.eps, P->steps.sumsq);
       };
       if (C <= 4) { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CS, 4, 2>); else go(color_sumsq_reg<CS, 4, 1>); }
       else { if (P->tune.eps_depth == 2) go(color_sumsq_reg<CS, 8, 2>); else go(color_sumsq_reg<CS, 8, 1>); }
@@ -1614,11 +1693,11 @@ static fdb_status run_eps(fdb_plan *P, const double *x, double relstep, double a
   } else {
     for (int32_t k0 = 0; k0 < C; k0 += kEpsWindow) {
       const int32_t W = std::min<int32_t>(kEpsWindow, C - k0);
-      color_sumsq_win<CT><<<P->eps_blocks, kThreads, (size_t)kEpsWarps * W * sizeof(double), s>>>(
-          x, (const CT *)P->jcolor, P->n, P->eps_chunk, k0, W, P->eps_group, P->partial);
+      color_sumsq_win<CT><<<P->steps.blocks, kThreads, (size_t)kEpsWarps * W * sizeof(double), s>>>(
+          x, (const CT *)P->colors.jcolor, P->n, P->steps.chunk, k0, W, P->steps.group, P->steps.partial);
       // partial rows are W wide for this pass
-      finalize_eps<CT><<<(W * 32 + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->partial, P->eps_blocks, W, k0, W, prm,
-                                                                            P->eps, P->sumsq, x, (const CT *)P->jcolor, P->n);
+      finalize_eps<CT><<<(W * 32 + kThreads - 1) / kThreads, kThreads, 0, s>>>(P->steps.partial, P->steps.blocks, W, k0, W, prm,
+                                                                            P->steps.eps, P->steps.sumsq, x, (const CT *)P->colors.jcolor, P->n);
       P->cnt.kernel_launches += 2;
     }
   }
@@ -1643,11 +1722,11 @@ struct ScatterGroup {
 // colour-major lists: the entries of the columns without a valid colour are 0
 static void zero_uncoloured_slots(const ScatterGroup &g) {
   fdb_plan *P = g.P;
-  const int64_t z0 = P->cm_start_h[P->local_colors.size()], z1 = P->cm_invalid_end;
+  const int64_t z0 = P->cm.start_h[P->colors.local.size()], z1 = P->cm.invalid_end;
   if (z1 <= z0) return;
   const int grid = P->grid(z1 - z0);
-  if (P->dest != nullptr) zero_slots<int64_t><<<grid, kThreads, 0, g.s>>>(P->cm_slot, z0, z1, g.J, P->d_peers, P->n_peers);
-  else zero_slots<int32_t><<<grid, kThreads, 0, g.s>>>(P->cm_slot, z0, z1, g.J, P->d_peers, P->n_peers);
+  if (P->entries.dest != nullptr) zero_slots<int64_t><<<grid, kThreads, 0, g.s>>>(P->cm.slot, z0, z1, g.J, P->peers.d, P->peers.n);
+  else zero_slots<int32_t><<<grid, kThreads, 0, g.s>>>(P->cm.slot, z0, z1, g.J, P->peers.d, P->peers.n);
   P->cnt.kernel_launches += 1;
 }
 
@@ -1655,11 +1734,11 @@ static void zero_uncoloured_slots(const ScatterGroup &g) {
 template <int MODE>
 static fdb_status scatter_lists(const ScatterGroup &g) {
   fdb_plan *P = g.P;
-  const int64_t total = P->cm_start_h[(size_t)(g.l0 + g.G)] - P->cm_start_h[(size_t)g.l0];
+  const int64_t total = P->cm.start_h[(size_t)(g.l0 + g.G)] - P->cm.start_h[(size_t)g.l0];
   CmArgs a{};
-  a.row = P->cm_row; a.slot = P->cm_slot; a.seg_start = P->cm_start; a.local_colors = P->d_local_colors;
-  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.J = g.J; a.peers = P->d_peers; a.n_peers = P->n_peers;
-  a.fx_cm = MODE == kForward ? P->fx_cm : nullptr;
+  a.row = P->cm.row; a.slot = P->cm.slot; a.seg_start = P->cm.start; a.local_colors = P->colors.d_local;
+  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps; a.J = g.J; a.peers = P->peers.d; a.n_peers = P->peers.n;
+  a.fx_cm = MODE == kForward ? P->cm.fx : nullptr;
   a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G; a.ldF = g.ldF;
   a.m = MODE == kComplex ? 2 * P->m : P->m;
   // (software L2 prefetch of the next colour's slab: off unless FDB_CM_PREFETCH=1 — on C4 the 40 MB slab, the next one
@@ -1668,7 +1747,7 @@ static fdb_status scatter_lists(const ScatterGroup &g) {
   a.slab_stream = P->tune.cm_slab_stream;
   const int64_t tiles = (total + kCmTile - 1) / kCmTile;
   ScatterTimer tm(P, g.s);
-  if (P->dest != nullptr) launch_resident(P, diff_scatter_cm<MODE, int64_t>, tiles, 0, g.s, a);
+  if (P->entries.dest != nullptr) launch_resident(P, diff_scatter_cm<MODE, int64_t>, tiles, 0, g.s, a);
   else launch_resident(P, diff_scatter_cm<MODE, int32_t>, tiles, 0, g.s, a);
   return FDB_OK;
 }
@@ -1679,17 +1758,17 @@ template <typename CT, int MODE>
 static fdb_status scatter_block_band(const ScatterGroup &g) {
   fdb_plan *P = g.P;
   BlockBandArgs a{};
-  a.jcolor = P->jcolor; a.boff = P->bb_off; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps;
-  a.local_of = P->local_of; a.J = g.J; a.total = P->bb_w * P->n; a.ldF = g.ldF;
-  a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.jcolor = P->colors.jcolor; a.boff = P->block_band.off; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps;
+  a.local_of = P->colors.local_of; a.J = g.J; a.total = P->block_band.w * P->n; a.ldF = g.ldF;
+  a.C = P->colors.C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
   a.write_other = g.first ? 1 : 0;
-  a.nblocks = P->bb_nblocks; a.u = (int32_t)P->u; a.mu = (int32_t)P->bb_mu;
-  a.uniform = P->bb_bs > 0 ? 1 : 0;
-  a.block_cyclic = P->bb_cyclic ? 1 : 0;
-  a.w = make_fastdiv((uint32_t)P->bb_w);
-  a.sw = make_fastdiv((uint32_t)(P->bb_lam + P->bb_mu + 1));
-  a.bs = make_fastdiv((uint32_t)std::max<int32_t>(P->bb_bs, 1));
-  a.bw = make_fastdiv((uint32_t)(P->l + P->u + 1));
+  a.nblocks = P->block_band.nblocks; a.u = (int32_t)P->band.u; a.mu = (int32_t)P->block_band.mu;
+  a.uniform = P->block_band.bs > 0 ? 1 : 0;
+  a.block_cyclic = P->block_band.cyclic ? 1 : 0;
+  a.w = make_fastdiv((uint32_t)P->block_band.w);
+  a.sw = make_fastdiv((uint32_t)(P->block_band.lam + P->block_band.mu + 1));
+  a.bs = make_fastdiv((uint32_t)std::max<int32_t>(P->block_band.bs, 1));
+  a.bw = make_fastdiv((uint32_t)(P->band.l + P->band.u + 1));
   const size_t sm = color_table_smem(P);
   const int64_t tiles = (a.total + kBbTile - 1) / kBbTile;
   // a store stream: an oversubscribed grid, as for the other band kernels
@@ -1705,9 +1784,9 @@ template <typename CT, int MODE>
 static fdb_status scatter_diagonals(const ScatterGroup &g) {
   fdb_plan *P = g.P;
   DiagArgs a{};
-  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.local_of = P->local_of; a.J = g.J;
-  a.total = P->j_len; a.sub_end = P->l * (P->n - 1); a.main_end = a.sub_end + P->n; a.ldF = g.ldF;
-  a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps; a.local_of = P->colors.local_of; a.J = g.J;
+  a.total = P->j_len; a.sub_end = P->band.l * (P->n - 1); a.main_end = a.sub_end + P->n; a.ldF = g.ldF;
+  a.C = P->colors.C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
   a.write_other = g.first ? 1 : 0;
   const size_t sm = color_table_smem(P);
   const int64_t tiles = (a.total + kDgTile - 1) / kDgTile;
@@ -1728,22 +1807,22 @@ static fdb_status scatter_band(const ScatterGroup &g) {
   fdb_plan *P = g.P;
   BandArgs a{};
   ScatterTimer tm(P, g.s);
-  a.jcolor = P->jcolor; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps; a.local_of = P->local_of;
-  a.J = g.J; a.C = P->C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.jcolor = P->colors.jcolor; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps; a.local_of = P->colors.local_of;
+  a.J = g.J; a.C = P->colors.C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
   a.write_other = g.first ? 1 : 0;
   a.to_dense = P->jkind == FDB_J_DENSE ? 1 : 0;
-  a.ldF = g.ldF; a.ldJ = P->ldJ; a.m = P->m; a.n = P->n; a.l = P->l; a.u = P->u;
-  const int64_t w = P->l + P->u + 1;
+  a.ldF = g.ldF; a.ldJ = P->ldJ; a.m = P->m; a.n = P->n; a.l = P->band.l; a.u = P->band.u;
+  const int64_t w = P->band.l + P->band.u + 1;
   a.cols_per_tile = std::max<int64_t>(1, 4096 / w);
   // every (colour, row) quotient lands in about (l+u+1)/C columns of the whole-band fill: when that reuse is >= 2,
   // divide once per (colour, row) in place (the reference's own `vfx1 = (vfx1 - vfx)/eps` pass) and let the band
   // kernel copy; otherwise divide at gather time.
   // On C3 (16 GB band, 5 colours) the flat stream over pre-divided slabs with 4-deep batched loads was kept over
   // warp-per-column, dividing at gather time, row-stationary, colour-grouped columns and block-per-column forms.
-  const bool prediv = MODE != kComplex && w >= 64 && w >= 2 * (int64_t)P->C;
+  const bool prediv = MODE != kComplex && w >= 64 && w >= 2 * (int64_t)P->colors.C;
   if (prediv) {
     dim3 grid((unsigned)std::max(1, std::min(P->grid(P->m), std::max(1, P->sm_count * 8 / (int)g.G))), (unsigned)g.G);
-    diff_slabs<MODE><<<grid, kThreads, 0, g.s>>>(g.Fp, MODE == kCentral ? g.Fm : g.fx, P->eps, P->d_local_colors + g.l0, P->m, g.ldF);
+    diff_slabs<MODE><<<grid, kThreads, 0, g.s>>>(g.Fp, MODE == kCentral ? g.Fm : g.fx, P->steps.eps, P->colors.d_local + g.l0, P->m, g.ldF);
     P->cnt.kernel_launches += 1;
   }
   if (w >= 64) {
@@ -1774,35 +1853,35 @@ template <typename CT, int MODE>
 static fdb_status scatter_entries(const ScatterGroup &g) {
   fdb_plan *P = g.P;
   ScatterArgs a{};
-  a.row = P->row32; a.ecolor = P->ecolor; a.dest = P->dest; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->eps;
-  a.local_of = P->local_of; a.J = g.J; a.peers = P->d_peers; a.n_peers = P->n_peers; a.C = P->C;
+  a.row = P->entries.row32; a.ecolor = P->entries.ecolor; a.dest = P->entries.dest; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps;
+  a.local_of = P->colors.local_of; a.J = g.J; a.peers = P->peers.d; a.n_peers = P->peers.n; a.C = P->colors.C;
   a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
-  a.write_invalid_zero = (g.first && P->has_invalid) ? 1 : 0;
-  a.ldF = g.ldF; a.E = P->E;
-  a.j_aligned = (reinterpret_cast<uintptr_t>(g.J) & 15) == 0 && P->peers_aligned;
+  a.write_invalid_zero = (g.first && P->colors.has_invalid) ? 1 : 0;
+  a.ldF = g.ldF; a.E = P->colors.E;
+  a.j_aligned = (reinterpret_cast<uintptr_t>(g.J) & 15) == 0 && P->peers.aligned;
   // random patterns (mean row jump beyond a few cache lines): slab gathers are read-once
-  a.hi_stream = P->tune.hi_stream >= 0 ? P->tune.hi_stream : (P->mean_row_jump > 4096.0 ? 1 : 0);
+  a.hi_stream = P->tune.hi_stream >= 0 ? P->tune.hi_stream : (P->entries.mean_row_jump > 4096.0 ? 1 : 0);
   const size_t sm = color_table_smem(P);
   ScatterTimer tm(P, g.s);
-  const int64_t tiles = (P->E + kTile - 1) / kTile;
+  const int64_t tiles = (P->colors.E + kTile - 1) / kTile;
   // single group on a single rank: every valid colour is resident -> the FULL variant (no ownership tests)
-  const bool full = P->n_groups == 1 && P->world == 1 && P->n_peers == 0;
+  const bool full = P->scratch.n_groups == 1 && P->world == 1 && P->peers.n == 0;
   // staged form (identity destination): needs 16-byte aligned sources and (forward) ldF readable doubles behind f(x)
-  bool staged = P->dest == nullptr && full && P->staged && MODE != kComplex;
+  bool staged = P->entries.dest == nullptr && full && P->staged.on && MODE != kComplex;
   if (staged && MODE == kForward)
-    staged = (reinterpret_cast<uintptr_t>(g.fx) & 15) == 0 && ((P->m & 1) == 0 || g.fx == P->fx_own);
+    staged = (reinterpret_cast<uintptr_t>(g.fx) & 15) == 0 && ((P->m & 1) == 0 || g.fx == P->scratch.fx_own);
   if (staged) {
     if constexpr (MODE != kComplex) {
       StagedArgs sa{};
-      sa.row16 = P->row16; sa.tile_w0 = P->tile_w0; sa.row32 = P->row32;
-      sa.fx = g.fx; sa.Fp = g.Fp; sa.Fm = g.Fm; sa.eps = P->eps; sa.J = g.J; sa.C = P->C; sa.W = P->stage_W;
-      sa.ldF = g.ldF; sa.src_len = P->ldF; sa.E = P->E; sa.j_aligned = a.j_aligned; sa.claim = P->stage_claim;
+      sa.row16 = P->staged.row16; sa.tile_w0 = P->staged.tile_w0; sa.row32 = P->entries.row32;
+      sa.fx = g.fx; sa.Fp = g.Fp; sa.Fm = g.Fm; sa.eps = P->steps.eps; sa.J = g.J; sa.C = P->colors.C; sa.W = P->staged.W;
+      sa.ldF = g.ldF; sa.src_len = P->scratch.ldF; sa.E = P->colors.E; sa.j_aligned = a.j_aligned; sa.claim = P->staged.claim;
       sa.reverse = P->tune.reverse & 1;
-      sa.colptr32 = P->colptr32; sa.l = P->band_l; sa.n = (int32_t)P->n;
-      sa.col_a = P->band_col_a; sa.col_b = P->band_col_b; sa.e_a = P->band_e_a; sa.e_b = P->band_e_b;
-      sa.w = make_fastdiv((uint32_t)P->band_w);
-      const int nwin = MODE == kCentral ? 2 * P->C : P->C + 1;
-      auto smem = [&](int stages) { return (size_t)stages * nwin * P->stage_W * 8 + kStageCtlBytes + (size_t)P->C * 8; };
+      sa.colptr32 = P->entries.colptr32; sa.l = P->staged.band_l; sa.n = (int32_t)P->n;
+      sa.col_a = P->staged.band_col_a; sa.col_b = P->staged.band_col_b; sa.e_a = P->staged.band_e_a; sa.e_b = P->staged.band_e_b;
+      sa.w = make_fastdiv((uint32_t)P->staged.band_w);
+      const int nwin = MODE == kCentral ? 2 * P->colors.C : P->colors.C + 1;
+      auto smem = [&](int stages) { return (size_t)stages * nwin * P->staged.W * 8 + kStageCtlBytes + (size_t)P->colors.C * 8; };
       sa.stages = smem(P->tune.stages) > (size_t)kStageMaxSmem ? 2 : P->tune.stages;
       const size_t ssm = smem(sa.stages);
       // variants (FDB_STAGED_VARIANT = 8n | 6p | 6n | 6e): resident blocks per SM x index prefetch / empty mbarrier
@@ -1811,7 +1890,7 @@ static fdb_status scatter_entries(const ScatterGroup &g) {
         CU(launch_pdl(kern, resident_grid(P, kern, ssm, tiles), ssm, g.s, sa, cs));
         return FDB_OK;
       };
-      if (P->stage_band) {
+      if (P->staged.band) {
         return dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
           using CS = decltype(cs);
           if (v0 == '8') return go(diff_scatter_staged<CS, MODE, 8, false, false, false, true>, cs);
@@ -1820,15 +1899,15 @@ static fdb_status scatter_entries(const ScatterGroup &g) {
         });
       }
       using CS = TableColors<CT>;          // per-entry colours
-      const CS ec{(const CT *)P->ecolor};
-      if (P->stage_packed && v1 == 'e') return go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec);
-      if (P->stage_packed) return go(diff_scatter_staged<CS, MODE, 6, false, true>, ec);
+      const CS ec{(const CT *)P->entries.ecolor};
+      if (P->staged.packed && v1 == 'e') return go(diff_scatter_staged<CS, MODE, 6, false, true, true>, ec);
+      if (P->staged.packed) return go(diff_scatter_staged<CS, MODE, 6, false, true>, ec);
       if (v0 == '8') return go(diff_scatter_staged<CS, MODE, 8, false, false>, ec);
       if (v1 == 'n') return go(diff_scatter_staged<CS, MODE, 6, false, false>, ec);
       return go(diff_scatter_staged<CS, MODE, 6, true, false>, ec);
     }
   }
-  if (P->dest != nullptr) launch_resident(P, diff_scatter_dest<CT, MODE>, (P->E + kThreads - 1) / kThreads, sm, g.s, a);
+  if (P->entries.dest != nullptr) launch_resident(P, diff_scatter_dest<CT, MODE>, (P->colors.E + kThreads - 1) / kThreads, sm, g.s, a);
   else if (full) launch_resident(P, diff_scatter_ident<CT, MODE, true, kScatterMinBlocks>, tiles, sm, g.s, a);
   else launch_resident(P, diff_scatter_ident<CT, MODE, false, kScatterMinBlocks>, tiles, sm, g.s, a);
   return FDB_OK;
@@ -1841,18 +1920,18 @@ static fdb_status scatter(Scatter family, const ScatterGroup &g) {
   fdb_plan *P = g.P;
   // colour-major lists: rank 0 zeroes the entries of the columns without a valid colour with its first group; owning no
   // colour, it does so only where this call does not zero-fill J (peer stores, a shared J)
-  if (family == Scatter::lists && g.first && (g.G > 0 || P->n_peers > 0 || P->shared_J)) zero_uncoloured_slots(g);
+  if (family == Scatter::lists && g.first && (g.G > 0 || P->peers.n > 0 || P->shared_J)) zero_uncoloured_slots(g);
   // a rank that owns no colour launches the block-banded scatter of rank 0 alone: the columns without a valid colour
   if (g.G == 0 && !(family == Scatter::block_band && g.first)) return FDB_OK;
   switch (family) {   // (a group has a colour: C > 0 and n > 0, so band and diagonal storage have slots)
     case Scatter::none: return FDB_OK;
     case Scatter::lists:
-      if (P->cm_start_h[(size_t)(g.l0 + g.G)] == P->cm_start_h[(size_t)g.l0]) return FDB_OK;   // empty lists
+      if (P->cm.start_h[(size_t)(g.l0 + g.G)] == P->cm.start_h[(size_t)g.l0]) return FDB_OK;   // empty lists
       TRY(scatter_lists<MODE>(g)); break;
-    case Scatter::block_band: if (P->bb_w * P->n == 0) return FDB_OK; TRY((scatter_block_band<CT, MODE>(g))); break;
+    case Scatter::block_band: if (P->block_band.w * P->n == 0) return FDB_OK; TRY((scatter_block_band<CT, MODE>(g))); break;
     case Scatter::diagonals: TRY((scatter_diagonals<CT, MODE>(g))); break;
     case Scatter::band: TRY((scatter_band<CT, MODE>(g))); break;
-    case Scatter::entries: if (P->E == 0) return FDB_OK; TRY((scatter_entries<CT, MODE>(g))); break;
+    case Scatter::entries: if (P->colors.E == 0) return FDB_OK; TRY((scatter_entries<CT, MODE>(g))); break;
   }
   P->cnt.kernel_launches += 1;
   P->cnt.scatter_launches += 1;
@@ -1865,25 +1944,25 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
   constexpr bool CENTRAL = MODE == kCentral;
   constexpr bool COMPLEX = MODE == kComplex;
   // strides, in doubles, of one f! output slab / one perturbed point (complex128 in complex-step mode)
-  const int64_t sF = COMPLEX ? 2 * P->ldF : P->ldF, sX = COMPLEX ? 2 * P->ldx : P->ldx;
-  const int64_t n_local = (int64_t)P->local_colors.size();
+  const int64_t sF = COMPLEX ? 2 * P->scratch.ldF : P->scratch.ldF, sX = COMPLEX ? 2 * P->scratch.ldx : P->scratch.ldx;
+  const int64_t n_local = (int64_t)P->colors.local.size();
   const Scatter family = scatter_family(P);
   // With peer buffers set the caller zero-fills J and synchronises the ranks BEFORE the call: a memset here would race
   // with the peers' stores.
-  if (!scatter_defines_J(P, n_local) && P->n_peers == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
+  if (!scatter_defines_J(P, n_local) && P->peers.n == 0 && !P->shared_J && P->j_len > 0) TRY(zero_J(P, J, s));
   // build the perturbed points of local colours [li0, li0+kc) into the point buffers (one pass over x per 4 colours)
   auto perturb_window = [&](int64_t li0, int64_t kc, cudaStream_t ps) -> fdb_status {
       for (int64_t q0 = 0; q0 < kc; q0 += kPerturbMaxPoints) {
         PerturbArgs pa{};
-        pa.x = x; pa.eps = P->eps;
-        pa.xp = P->xp + q0 * sX; pa.xm = CENTRAL ? P->xm + q0 * sX : nullptr;
-        pa.n = P->n; pa.ldx = sX; pa.C = P->C; pa.drift = (P->no_drift || P->oop) ? 0 : 1; pa.oop = P->oop;
+        pa.x = x; pa.eps = P->steps.eps;
+        pa.xp = P->scratch.xp + q0 * sX; pa.xm = CENTRAL ? P->scratch.xm + q0 * sX : nullptr;
+        pa.n = P->n; pa.ldx = sX; pa.C = P->colors.C; pa.drift = (P->no_drift || P->oop.on) ? 0 : 1; pa.oop = P->oop.on;
         pa.reverse = (P->tune.reverse >> 1) & 1;
         pa.kcount = (int32_t)std::min<int64_t>(kPerturbMaxPoints, kc - q0);
-        for (int32_t q = 0; q < pa.kcount; ++q) pa.k[q] = P->local_colors[(size_t)(li0 + q0 + q)];
-        pa.aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(P->xp) |
-                       reinterpret_cast<uintptr_t>(P->xm)) & 15) == 0 && (P->ldx & 1) == 0;
-        const size_t sm = P->C <= kPerturbSmemColors ? (size_t)P->C * sizeof(double) : 0;
+        for (int32_t q = 0; q < pa.kcount; ++q) pa.k[q] = P->colors.local[(size_t)(li0 + q0 + q)];
+        pa.aligned = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(P->scratch.xp) |
+                       reinterpret_cast<uintptr_t>(P->scratch.xm)) & 15) == 0 && (P->scratch.ldx & 1) == 0;
+        const size_t sm = P->colors.C <= kPerturbSmemColors ? (size_t)P->colors.C * sizeof(double) : 0;
         const int64_t tiles = (P->n + kTile - 1) / kTile;
         TRY(dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
           using CS = decltype(cs);
@@ -1906,21 +1985,21 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
 
   // forward mode without f_in: f(x) (jacobians.jl:541) and the step-size pass are independent — the eps kernels run on the
   // side stream beside the user's f(x) (a parallel branch of the CUDA graph)
-  bool eps_beside_fx = MODE == kForward && !f_in && !P->ext_eps && P->side && P->ev_fork && P->C > 0;
+  bool eps_beside_fx = MODE == kForward && !f_in && !P->steps.ext && P->overlap.side && P->overlap.ev_fork && P->colors.C > 0;
   if (P->tune.no_eps_overlap) eps_beside_fx = false;
   // ... and so is the first window of perturbed points, which reads x and the step sizes only: it is built on the side
   // stream behind the ε pass, and the call's stream waits for both before the first f!(xp).  f! is still called in the
   // reference's order, f(x) first.
   const bool perturb_beside_fx = eps_beside_fx && n_local > 0;
-  if (P->ext_eps) {
+  if (P->steps.ext) {
     // sharded runs: the step sizes of the FULL x come from outside (fdb_color_eps on the full vector)
-    if (P->C > 0) CU(cudaMemcpyAsync(P->eps, P->ext_eps, (size_t)P->C * 8, cudaMemcpyDeviceToDevice, s));
+    if (P->colors.C > 0) CU(cudaMemcpyAsync(P->steps.eps, P->steps.ext, (size_t)P->colors.C * 8, cudaMemcpyDeviceToDevice, s));
   } else if (eps_beside_fx) {
-    CU(cudaEventRecord(P->ev_fork, s));
-    CU(cudaStreamWaitEvent(P->side, P->ev_fork, 0));
-    TRY(run_eps<CT>(P, x, relstep, absstep, dir, P->side));
-    if (perturb_beside_fx) TRY(perturb_window(0, std::min<int64_t>(P->pbatch, n_local), P->side));
-    CU(cudaEventRecord(P->ev_eps, P->side));
+    CU(cudaEventRecord(P->overlap.ev_fork, s));
+    CU(cudaStreamWaitEvent(P->overlap.side, P->overlap.ev_fork, 0));
+    TRY(run_eps<CT>(P, x, relstep, absstep, dir, P->overlap.side));
+    if (perturb_beside_fx) TRY(perturb_window(0, std::min<int64_t>(P->scratch.pbatch, n_local), P->overlap.side));
+    CU(cudaEventRecord(P->overlap.ev_eps, P->overlap.side));
   } else {
     TRY(run_eps<CT>(P, x, relstep, absstep, dir, s));
   }
@@ -1929,51 +2008,51 @@ static fdb_status run_colored(fdb_plan *P, fdb_fn f, void *ctx, const double *x,
     if (f_in) vfx = f_in;                                  // jacobians.jl:543-544
     else { TRY(call_f(P, f, ctx, fx, x, 1, s)); vfx = fx; } // :541-542
   }
-  if (eps_beside_fx) CU(cudaStreamWaitEvent(s, P->ev_eps, 0));
+  if (eps_beside_fx) CU(cudaStreamWaitEvent(s, P->overlap.ev_eps, 0));
   // colour-major lists, forward: f(x) once into list order (read as a coalesced stream by every colour's launch)
-  if (MODE == kForward && family == Scatter::lists && P->fx_cm && n_local > 0) {
-    const int64_t cnt = P->cm_start_h[(size_t)n_local];
+  if (MODE == kForward && family == Scatter::lists && P->cm.fx && n_local > 0) {
+    const int64_t cnt = P->cm.start_h[(size_t)n_local];
     if (cnt > 0) {
       ScatterTimer tm(P, s);            // part of the diff+scatter formulation: timed with it
-      gather_fx_cm<<<P->grid(cnt, kThreads * 4, 16), kThreads, 0, s>>>(P->cm_row, vfx, cnt, P->fx_cm);
+      gather_fx_cm<<<P->grid(cnt, kThreads * 4, 16), kThreads, 0, s>>>(P->cm.row, vfx, cnt, P->cm.fx);
       P->cnt.kernel_launches += 1;
     }
   }
   // Double-buffered overlap (multi-GPU, column lists): group g's f! outputs live in buffer (g & 1); its scatter — the
   // kernel that also pushes the values to the peers over NVLink — runs on a side stream while the main stream already
   // evaluates group g+1 into the other buffer.  Events order buffer reuse; everything joins the caller's stream at the end.
-  const bool overlap = P->double_buffer && P->side != nullptr;
+  const bool overlap = P->overlap.double_buffer && P->overlap.side != nullptr;
 
   // colours ascending (jacobians.jl:547).  Points are built in windows of `pbatch` colours, f! is called once per point
   // (reference order f(fx1,x1) then f(fx,x) per colour, :563 / :605-606) or once per `batch` points for batch-capable
   // callbacks; a group's scatter is launched as soon as its `slabs` outputs are complete.
   int64_t li = 0;
   while (li < n_local) {
-    const int64_t g = li / P->slabs, g0 = g * P->slabs, gend = std::min<int64_t>(g0 + P->slabs, n_local);
-    if (li % P->pbatch == 0 && !(li == 0 && perturb_beside_fx)) TRY(perturb_window(li, std::min<int64_t>(P->pbatch, n_local - li), s));
-    const int64_t wend = std::min<int64_t>((li / P->pbatch + 1) * P->pbatch, n_local);
-    const int64_t fc = std::min<int64_t>(P->batch, std::min<int64_t>(wend - li, gend - li));
-    const int64_t gb = overlap ? (g & 1) * P->slabs * sF : 0;           // this group's output buffer
-    if (overlap && li == g0 && g >= 2) CU(cudaStreamWaitEvent(s, P->ev_scat[g & 1], 0));   // buffer free again?
-    TRY(call_f(P, f, ctx, P->Fp + gb + (li - g0) * sF, P->xp + (li % P->pbatch) * sX, fc, s));
-    if (CENTRAL) TRY(call_f(P, f, ctx, P->Fm + gb + (li - g0) * sF, P->xm + (li % P->pbatch) * sX, fc, s));
+    const int64_t g = li / P->scratch.slabs, g0 = g * P->scratch.slabs, gend = std::min<int64_t>(g0 + P->scratch.slabs, n_local);
+    if (li % P->scratch.pbatch == 0 && !(li == 0 && perturb_beside_fx)) TRY(perturb_window(li, std::min<int64_t>(P->scratch.pbatch, n_local - li), s));
+    const int64_t wend = std::min<int64_t>((li / P->scratch.pbatch + 1) * P->scratch.pbatch, n_local);
+    const int64_t fc = std::min<int64_t>(P->scratch.batch, std::min<int64_t>(wend - li, gend - li));
+    const int64_t gb = overlap ? (g & 1) * P->scratch.slabs * sF : 0;           // this group's output buffer
+    if (overlap && li == g0 && g >= 2) CU(cudaStreamWaitEvent(s, P->overlap.ev_scat[g & 1], 0));   // buffer free again?
+    TRY(call_f(P, f, ctx, P->scratch.Fp + gb + (li - g0) * sF, P->scratch.xp + (li % P->scratch.pbatch) * sX, fc, s));
+    if (CENTRAL) TRY(call_f(P, f, ctx, P->scratch.Fm + gb + (li - g0) * sF, P->scratch.xm + (li % P->scratch.pbatch) * sX, fc, s));
     li += fc;
     if (li == gend) {
-      const ScatterGroup grp{P, J, vfx, P->Fp + gb, CENTRAL ? P->Fm + gb : nullptr, sF, overlap ? P->side : s,
+      const ScatterGroup grp{P, J, vfx, P->scratch.Fp + gb, CENTRAL ? P->scratch.Fm + gb : nullptr, sF, overlap ? P->overlap.side : s,
                              g0, gend - g0, g == 0 && P->rank == 0};
       if (overlap) {
-        CU(cudaEventRecord(P->ev_f[g & 1], s));
-        CU(cudaStreamWaitEvent(P->side, P->ev_f[g & 1], 0));
+        CU(cudaEventRecord(P->overlap.ev_f[g & 1], s));
+        CU(cudaStreamWaitEvent(P->overlap.side, P->overlap.ev_f[g & 1], 0));
       }
       TRY((scatter<CT, MODE>(family, grp)));
-      if (overlap) CU(cudaEventRecord(P->ev_scat[g & 1], P->side));
+      if (overlap) CU(cudaEventRecord(P->overlap.ev_scat[g & 1], P->overlap.side));
     }
   }
   if (overlap) {   // join the side stream back into the caller's stream
-    const int64_t ng = (n_local + P->slabs - 1) / P->slabs;
-    for (int64_t b = 0; b < std::min<int64_t>(ng, 2); ++b) CU(cudaStreamWaitEvent(s, P->ev_scat[b], 0));
+    const int64_t ng = (n_local + P->scratch.slabs - 1) / P->scratch.slabs;
+    for (int64_t b = 0; b < std::min<int64_t>(ng, 2); ++b) CU(cudaStreamWaitEvent(s, P->overlap.ev_scat[b], 0));
   }
-  if (n_local == 0) TRY((scatter<CT, MODE>(family, {P, J, vfx, P->Fp, P->Fm, sF, s, 0, 0, P->rank == 0})));
+  if (n_local == 0) TRY((scatter<CT, MODE>(family, {P, J, vfx, P->scratch.Fp, P->scratch.Fm, sF, s, 0, 0, P->rank == 0})));
   CU(cudaGetLastError());
   return FDB_OK;
 }
@@ -1983,38 +2062,38 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
                             double relstep, double absstep, double dir, cudaStream_t s) {
   constexpr bool CENTRAL = MODE == kCentral;
   constexpr bool COMPLEX = MODE == kComplex;
-  const int64_t sF = COMPLEX ? 2 * P->ldF : P->ldF, sX = COMPLEX ? 2 * P->ldx : P->ldx;
-  const int64_t ncl = P->col_end - P->col_begin;
+  const int64_t sF = COMPLEX ? 2 * P->scratch.ldF : P->scratch.ldF, sX = COMPLEX ? 2 * P->scratch.ldx : P->scratch.ldx;
+  const int64_t ncl = P->columns.end - P->columns.begin;
   const double *vfx = nullptr;
   if (MODE == kForward) {
     if (f_in) vfx = f_in;
     else { TRY(call_f(P, f, ctx, fx, x, 1, s)); vfx = fx; }
   }
   if (ncl == 0) return FDB_OK;
-  const int32_t B = (int32_t)P->batch;
+  const int32_t B = (int32_t)P->scratch.batch;
   if (COMPLEX) {
     // epsilon = eps(eltype(x)) for every column (jacobians.jl:624); X[b] = complex(x)
-    fill_value<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(P->eps_cols, ncl, DBL_EPSILON);
-    replicate_x_complex<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, sX, B, P->xp);
+    fill_value<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(P->columns.eps, ncl, DBL_EPSILON);
+    replicate_x_complex<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, sX, B, P->scratch.xp);
   } else {
     // out-of-place plans: the forward rule, dir included, in central mode too (jacobians.jl:358)
-    component_eps<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, P->col_begin, ncl, CENTRAL && !P->oop ? 1 : 0,
-                                                                            relstep, absstep, dir, P->eps_cols);
-    replicate_x<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, P->ldx, B, P->xp);
+    component_eps<<<(int)((ncl + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, P->columns.begin, ncl, CENTRAL && !P->oop.on ? 1 : 0,
+                                                                            relstep, absstep, dir, P->columns.eps);
+    replicate_x<<<P->grid(P->n), kThreads, 0, s>>>(x, P->n, P->scratch.ldx, B, P->scratch.xp);
   }
   P->cnt.kernel_launches += 2;
   int64_t prev_c0 = 0;
   int32_t prevB = 0;
   for (int64_t c0l = 0; c0l < ncl; c0l += B) {
     const int32_t kc = (int32_t)std::min<int64_t>(B, ncl - c0l);
-    const int64_t c0 = P->col_begin + c0l;
+    const int64_t c0 = P->columns.begin + c0l;
     const int sb = (std::max(kc, prevB) + kThreads - 1) / kThreads;
-    if (COMPLEX) set_components_complex<<<sb, kThreads, 0, s>>>(x, P->eps_cols, c0l, c0, prev_c0, kc, prevB, sX, P->xp);
-    else set_components<<<sb, kThreads, 0, s>>>(x, P->eps_cols, c0l, c0, prev_c0, kc, prevB, P->ldx, 1.0, P->xp);
-    TRY(call_f(P, f, ctx, P->Fp, P->xp, kc, s));                         // f(fx1, x1)   jacobians.jl:553 / :594 / :629
+    if (COMPLEX) set_components_complex<<<sb, kThreads, 0, s>>>(x, P->columns.eps, c0l, c0, prev_c0, kc, prevB, sX, P->scratch.xp);
+    else set_components<<<sb, kThreads, 0, s>>>(x, P->columns.eps, c0l, c0, prev_c0, kc, prevB, P->scratch.ldx, 1.0, P->scratch.xp);
+    TRY(call_f(P, f, ctx, P->scratch.Fp, P->scratch.xp, kc, s));                         // f(fx1, x1)   jacobians.jl:553 / :594 / :629
     if (CENTRAL) {
-      set_components<<<sb, kThreads, 0, s>>>(x, P->eps_cols, c0l, c0, 0, kc, 0, P->ldx, -1.0, P->xp);
-      TRY(call_f(P, f, ctx, P->Fm, P->xp, kc, s));                       // f(fx, x1)    :596
+      set_components<<<sb, kThreads, 0, s>>>(x, P->columns.eps, c0l, c0, 0, kc, 0, P->scratch.ldx, -1.0, P->scratch.xp);
+      TRY(call_f(P, f, ctx, P->scratch.Fm, P->scratch.xp, kc, s));                       // f(fx, x1)    :596
       P->cnt.kernel_launches += 1;
     }
     // a store-heavy stream (24 bytes moved per 8 written): many small blocks rather than one resident wave — each thread
@@ -2022,11 +2101,11 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
     const int gx = (int)std::max<int64_t>(1, std::min<int64_t>((P->m / 2 + kThreads * 4 - 1) / (kThreads * 4), P->tune.cols_gx));
     dim3 grid((unsigned)gx, (unsigned)kc);
     {
-      const double *lo_ptr = CENTRAL ? P->Fm : vfx;
+      const double *lo_ptr = CENTRAL ? P->scratch.Fm : vfx;
       const int pairs_ok = ((reinterpret_cast<uintptr_t>(J + c0l * P->ldJ) | reinterpret_cast<uintptr_t>(lo_ptr) |
-                             reinterpret_cast<uintptr_t>(P->Fp)) & 15) == 0 && (P->ldJ & 1) == 0 && (sF & 1) == 0;
+                             reinterpret_cast<uintptr_t>(P->scratch.Fp)) & 15) == 0 && (P->ldJ & 1) == 0 && (sF & 1) == 0;
       ScatterTimer tm(P, s);
-      auto go = [&](auto kern) { kern<<<grid, kThreads, 0, s>>>(P->Fp, lo_ptr, P->eps_cols, c0l, kc, P->m, sF, P->ldJ, J + c0l * P->ldJ, pairs_ok); };
+      auto go = [&](auto kern) { kern<<<grid, kThreads, 0, s>>>(P->scratch.Fp, lo_ptr, P->columns.eps, c0l, kc, P->m, sF, P->ldJ, J + c0l * P->ldJ, pairs_ok); };
       // independent 16-byte loads in flight per thread before the first quotient (C5 shape: 4 central, 2 forward)
       const int depth = P->tune.cols_depth ? P->tune.cols_depth : (CENTRAL ? 4 : 2);
       if (depth == 4) go(diff_columns<MODE, 4>);
@@ -2047,37 +2126,37 @@ static fdb_status run_dense(fdb_plan *P, fdb_fn f, void *ctx, const double *x, d
 // and re-launched while the key stays the same.
 template <typename F>
 static fdb_status run_maybe_graph(fdb_plan *P, const GraphKey &key, cudaStream_t s, const char *what, F &&eager) {
-  if (!P->use_graph || P->timing) return eager(s);
-  if (!P->graph_exec || !(key == P->graph_key)) {
-    if (P->graph_exec) { cudaGraphExecDestroy(P->graph_exec); P->graph_exec = nullptr; }
-    if (!P->cstream) CU(cudaStreamCreateWithFlags(&P->cstream, cudaStreamNonBlocking));
+  if (!P->graph.use || P->timing.on) return eager(s);
+  if (!P->graph.exec || !(key == P->graph.key)) {
+    if (P->graph.exec) { cudaGraphExecDestroy(P->graph.exec); P->graph.exec = nullptr; }
+    if (!P->graph.stream) CU(cudaStreamCreateWithFlags(&P->graph.stream, cudaStreamNonBlocking));
     const fdb_counters_t before = P->cnt;
-    CU(cudaStreamBeginCapture(P->cstream, cudaStreamCaptureModeThreadLocal));
-    const fdb_status st = eager(P->cstream);
+    CU(cudaStreamBeginCapture(P->graph.stream, cudaStreamCaptureModeThreadLocal));
+    const fdb_status st = eager(P->graph.stream);
     cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(P->cstream, &graph);
+    cudaError_t e = cudaStreamEndCapture(P->graph.stream, &graph);
     if (st != FDB_OK) { if (graph) cudaGraphDestroy(graph); cudaGetLastError(); return st; }
     if (e != cudaSuccess || !graph) {
       cudaGetLastError();
       return fail(FDB_ERR_CUDA, "stream capture of the %s failed (%s): the f! callback must be capture-safe "
                                 "(enqueue-only, no allocation) when use_graph is set", what, cudaGetErrorString(e));
     }
-    e = cudaGraphInstantiate(&P->graph_exec, graph, 0);
+    e = cudaGraphInstantiate(&P->graph.exec, graph, 0);
     cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { P->graph_exec = nullptr; return fail(FDB_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
-    P->graph_key = key;
+    if (e != cudaSuccess) { P->graph.exec = nullptr; return fail(FDB_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e)); }
+    P->graph.key = key;
     // what one replay amounts to (the capture pass itself launched nothing)
-    P->graph_delta.f_points = P->cnt.f_points - before.f_points;
-    P->graph_delta.f_invocations = P->cnt.f_invocations - before.f_invocations;
-    P->graph_delta.kernel_launches = P->cnt.kernel_launches - before.kernel_launches;
-    P->graph_delta.scatter_launches = P->cnt.scatter_launches - before.scatter_launches;
+    P->graph.delta.f_points = P->cnt.f_points - before.f_points;
+    P->graph.delta.f_invocations = P->cnt.f_invocations - before.f_invocations;
+    P->graph.delta.kernel_launches = P->cnt.kernel_launches - before.kernel_launches;
+    P->graph.delta.scatter_launches = P->cnt.scatter_launches - before.scatter_launches;
     P->cnt = before;
   }
-  CU(cudaGraphLaunch(P->graph_exec, s));
-  P->cnt.f_points += P->graph_delta.f_points;
-  P->cnt.f_invocations += P->graph_delta.f_invocations;
-  P->cnt.kernel_launches += P->graph_delta.kernel_launches;
-  P->cnt.scatter_launches += P->graph_delta.scatter_launches;
+  CU(cudaGraphLaunch(P->graph.exec, s));
+  P->cnt.f_points += P->graph.delta.f_points;
+  P->cnt.f_invocations += P->graph.delta.f_invocations;
+  P->cnt.kernel_launches += P->graph.delta.kernel_launches;
+  P->cnt.scatter_launches += P->graph.delta.scatter_launches;
   return FDB_OK;
 }
 
@@ -2088,7 +2167,7 @@ static fdb_status jacobian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double 
   return dispatch_mode(P->fdtype, [&](auto mode) -> fdb_status {
     constexpr int MODE = decltype(mode)::value;
     if (P->sp_kind == SP_NONE) return run_dense<MODE>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
-    return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    return dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       return run_colored<decltype(tag), MODE>(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, s);
     });
   });
@@ -2102,8 +2181,8 @@ static fdb_status jacobian_run(fdb_plan *P, fdb_fn f, void *ctx, const double *d
   cudaStream_t s = (cudaStream_t)stream;
   // jacobians.jl:508-509 defaults
   resolve_steps(P->fdtype, relstep, absstep);
-  double *fx = d_fx ? d_fx : P->fx_own;
-  const GraphKey key{(void *)f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, P->n_peers, P->peer_generation, P->ext_eps};
+  double *fx = d_fx ? d_fx : P->scratch.fx_own;
+  const GraphKey key{(void *)f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, P->peers.n, P->peers.generation, P->steps.ext};
   const fdb_status st = run_maybe_graph(P, key, s, "Jacobian", [&](cudaStream_t cs) {
     return jacobian_eager(P, f, ctx, d_x, d_J, fx, d_f_in, relstep, absstep, dir, cs);
   });
@@ -2141,7 +2220,7 @@ fdb_status fdb_eps_plan_create(fdb_plan **plan, int64_t n, const int64_t *colorv
   TRY(alloc_eps_buffers(P));
   // the same list-based eps pass as the Jacobian plans: a column block's external step sizes are then bit-identical to
   // the ones the unsharded plan computes for itself
-  if (P->C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
+  if (P->colors.C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
   *plan = owner.release();
   return FDB_OK;
 }
@@ -2155,18 +2234,18 @@ fdb_status fdb_color_eps(fdb_plan *P, const double *d_x, double relstep, double 
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
   cudaStream_t s = (cudaStream_t)stream;
   resolve_steps(P->fdtype, relstep, absstep);
-  TRY(dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+  TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
     using CT = decltype(tag);
     return run_eps<CT>(P, d_x, relstep, absstep, dir, s);
   }));
-  if (d_eps_out && P->C > 0) CU(cudaMemcpyAsync(d_eps_out, P->eps, (size_t)P->C * 8, cudaMemcpyDeviceToDevice, s));
+  if (d_eps_out && P->colors.C > 0) CU(cudaMemcpyAsync(d_eps_out, P->steps.eps, (size_t)P->colors.C * 8, cudaMemcpyDeviceToDevice, s));
   return FDB_OK;
 }
 
 fdb_status fdb_plan_set_external_eps(fdb_plan *P, const double *d_eps) {
   if (!P) return fail(FDB_ERR_INVALID, "NULL plan");
   TRY(check_call(P, Call::set_external_eps));
-  P->ext_eps = d_eps;
+  P->steps.ext = d_eps;
   return FDB_OK;
 }
 
@@ -2179,18 +2258,17 @@ fdb_status fdb_jvp_plan_create(fdb_plan **plan, int64_t m, int64_t n, const fdb_
   if (P->fdtype == FDB_COMPLEX)
     return fail(FDB_ERR_UNSUPPORTED, "finite_difference_jvp doesn't support :complex-mode finite diff");   // jvp.jl:248-250
   P->sp_kind = SP_JVP;
-  P->C = 1;
-  P->ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
-  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  P->scratch.ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
+  P->scratch.ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
   int64_t nb = std::max<int64_t>(1, std::min<int64_t>((n + kTile - 1) / kTile, (int64_t)P->sm_count * 8));
-  P->eps_blocks = (int)nb;
-  TRY(P->alloc_t(&P->partial, (size_t)nb));
-  TRY(P->alloc_t(&P->ticket, 4));
-  CU(cudaMemset(P->ticket, 0, 16));
-  TRY(P->alloc_t(&P->eps, 2));
-  TRY(P->alloc_t(&P->sumsq, 2));
-  TRY(P->alloc_t(&P->fx_own, (size_t)P->ldF));
-  TRY(P->alloc_t(&P->xp, (size_t)P->ldx));
+  P->steps.blocks = (int)nb;
+  TRY(P->alloc_t(&P->steps.partial, (size_t)nb));
+  TRY(P->alloc_t(&P->steps.ticket, 4));
+  CU(cudaMemset(P->steps.ticket, 0, 16));
+  TRY(P->alloc_t(&P->steps.eps, 2));
+  TRY(P->alloc_t(&P->steps.sumsq, 2));
+  TRY(P->alloc_t(&P->scratch.fx_own, (size_t)P->scratch.ldF));
+  TRY(P->alloc_t(&P->scratch.xp, (size_t)P->scratch.ldx));
   P->alg_bytes = 24 * n + 24 * m;   // dot: 16n; point: 16n read + 8n write; quotient: 16m read + 8m write
   *plan = owner.release();
   return FDB_OK;
@@ -2208,39 +2286,39 @@ static fdb_status jvp_run(fdb_plan *P, fdb_fn f, void *ctx, double *d_jvp, const
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
   cudaStream_t s = (cudaStream_t)stream;
   resolve_steps(P->fdtype, relstep, absstep);                       // jvp.jl:245-246
-  double *x1 = d_x1 ? d_x1 : P->xp;
-  double *fx1 = d_fx1 ? d_fx1 : P->fx_own;
+  double *x1 = d_x1 ? d_x1 : P->scratch.xp;
+  double *fx1 = d_fx1 ? d_fx1 : P->scratch.fx_own;
   const bool central = P->fdtype == FDB_CENTRAL;
   const int64_t n = P->n, m = P->m;
   const int al_xv = ((reinterpret_cast<uintptr_t>(d_x) | reinterpret_cast<uintptr_t>(d_v)) & 15) == 0;
   const int al_x1 = al_xv && (reinterpret_cast<uintptr_t>(x1) & 15) == 0;
   EpsParams prm{central ? 1 : 0, relstep, absstep, dir};
   const int64_t tiles = (n + kTile - 1) / kTile;
-  const int grid_n = std::min(resident_grid(P, jvp_dot_eps, 0, tiles), P->eps_blocks);
-  jvp_dot_eps<<<grid_n, kThreads, 0, s>>>(d_x, d_v, n, al_xv, prm, P->partial, P->ticket, P->eps, P->sumsq);   // :252-253
+  const int grid_n = std::min(resident_grid(P, jvp_dot_eps, 0, tiles), P->steps.blocks);
+  jvp_dot_eps<<<grid_n, kThreads, 0, s>>>(d_x, d_v, n, al_xv, prm, P->steps.partial, P->steps.ticket, P->steps.eps, P->steps.sumsq);   // :252-253
   P->cnt.kernel_launches += 1;
   const double *base = fx1;
   if (!central) {
     if (d_f_in) base = d_f_in;                                      // fx1 = f_in        :257-258
     else TRY(call_f(P, f, ctx, fx1, d_x, 1, s));                    // f(fx1, x)         :255
   } else if (plus_first) {
-    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 0, x1, n, al_x1);   // x + eps v :180
+    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->steps.eps, 0, x1, n, al_x1);   // x + eps v :180
     TRY(call_f(P, f, ctx, d_jvp, x1, 1, s));                        // fx1 = f(x1)       :181
-    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 1, x1, n, al_x1);   // x - eps v :182
+    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->steps.eps, 1, x1, n, al_x1);   // x - eps v :182
     TRY(call_f(P, f, ctx, fx1, x1, 1, s));                          // fx = f(x1)        :183
-    jvp_quotient<<<P->grid(m), kThreads, 0, s>>>(d_jvp, fx1, P->eps, 1, m);                                   // :184
+    jvp_quotient<<<P->grid(m), kThreads, 0, s>>>(d_jvp, fx1, P->steps.eps, 1, m);                                   // :184
     P->cnt.kernel_launches += 3;
     CU(cudaGetLastError());
     P->cnt.jacobians += 1;
     return FDB_OK;
   } else {
-    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 1, x1, n, al_x1);   // x1 = x - eps v :264
+    jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->steps.eps, 1, x1, n, al_x1);   // x1 = x - eps v :264
     P->cnt.kernel_launches += 1;
     TRY(call_f(P, f, ctx, fx1, x1, 1, s));                          // f(fx1, x1)        :265
   }
-  jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->eps, 0, x1, n, al_x1);     // x1 = x + eps v :260/:266
+  jvp_point<<<resident_grid(P, jvp_point, 0, tiles), kThreads, 0, s>>>(d_x, d_v, P->steps.eps, 0, x1, n, al_x1);     // x1 = x + eps v :260/:266
   TRY(call_f(P, f, ctx, d_jvp, x1, 1, s));                          // f(jvp, x1)        :261/:267
-  jvp_quotient<<<P->grid(m), kThreads, 0, s>>>(d_jvp, base, P->eps, central ? 1 : 0, m);                        // :262/:268
+  jvp_quotient<<<P->grid(m), kThreads, 0, s>>>(d_jvp, base, P->steps.eps, central ? 1 : 0, m);                        // :262/:268
   P->cnt.kernel_launches += 2;
   CU(cudaGetLastError());
   P->cnt.jacobians += 1;
@@ -2300,81 +2378,80 @@ fdb_status fdb_hessian_plan_create(fdb_plan **plan, int64_t n, int64_t ldH, cons
   P->jkind = FDB_J_DENSE;
   P->ldJ = ldH;
   P->j_len = ldH * n;
-  P->C = (int32_t)std::min<int64_t>(n, INT32_MAX);
   // this rank's i-blocks [i0, i1) (all of them on one device); it owns column i rows [i, n) and row i columns (i, n)
   const int64_t ib = hess_rank_begin(n, P->world, P->rank), ie = hess_rank_begin(n, P->world, P->rank + 1);
   const int64_t nb = ie - ib, own_points = hess_block_start(ie, n) - hess_block_start(ib, n);
-  P->col_begin = ib;
-  P->col_end = ie;
-  P->E = nb * (2 * n - 1) - (ie * (ie - 1) - ib * (ib - 1));
-  P->hess_off = hess_block_start(ib, n) - 1;
+  P->hess.i_begin = ib;
+  P->hess.i_end = ie;
+  P->hess.entries = nb * (2 * n - 1) - (ie * (ie - 1) - ib * (ib - 1));
+  P->hess.off = hess_block_start(ib, n) - 1;
   // f(x) first (the diagonal needs it), then the rank's own points; rank 0 always evaluates f(x) (n = 0 included), a
   // rank > 0 without i-blocks evaluates nothing
   const bool idle = nb == 0 && P->rank > 0;
-  P->hess_points = idle ? 0 : 1 + own_points;
-  P->ldF = 1;
-  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  P->hess.points = idle ? 0 : 1 + own_points;
+  P->scratch.ldF = 1;
+  P->scratch.ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
   const int64_t budget = opts->scratch_bytes > 0 ? opts->scratch_bytes : (int64_t)8 << 30;
   // ONE budget for both buffers: the resident point rows X[0..B) take at most half of it, the value buffer V the rest
   int64_t batch = opts->max_batch > 1 ? opts->max_batch : 1;
-  batch = std::max<int64_t>(1, std::min<int64_t>(batch, budget / 2 / (8 * P->ldx)));
-  batch = std::min<int64_t>(std::min<int64_t>(batch, std::max<int64_t>(P->hess_points, 1)), kHessBatchCap);
-  P->batch = batch;
-  P->slabs = batch;
+  batch = std::max<int64_t>(1, std::min<int64_t>(batch, budget / 2 / (8 * P->scratch.ldx)));
+  batch = std::min<int64_t>(std::min<int64_t>(batch, std::max<int64_t>(P->hess.points, 1)), kHessBatchCap);
+  P->scratch.batch = batch;
+  P->scratch.slabs = batch;
   // chunks of whole i-blocks whose values fit the budget (at least one i-block each), so that the <= 4 values of an
   // entry are always in the same chunk
-  const int64_t cap = std::max<int64_t>((budget - batch * P->ldx * 8) / 8 - 1, 0);
-  P->hess_chunks.assign(1, ib);
+  const int64_t cap = std::max<int64_t>((budget - batch * P->scratch.ldx * 8) / 8 - 1, 0);
+  P->hess.chunks.assign(1, ib);
   int64_t max_vals = 0;
   for (int64_t i0 = ib; i0 < ie;) {
     int64_t i1 = i0 + 1;
     while (i1 < ie && hess_block_start(i1 + 1, n) - hess_block_start(i0, n) <= cap) ++i1;
     max_vals = std::max<int64_t>(max_vals, hess_block_start(i1, n) - hess_block_start(i0, n));
-    P->hess_chunks.push_back(i1);
+    P->hess.chunks.push_back(i1);
     i0 = i1;
   }
-  if (nb == 0 && !idle) P->hess_chunks.push_back(ib);   // one chunk of no i-blocks: f(x) alone
-  P->n_groups = (int64_t)P->hess_chunks.size() - 1;
-  TRY(P->alloc_t(&P->hess_V, (size_t)(1 + max_vals)));
-  TRY(P->alloc_t(&P->xp, (size_t)(batch * P->ldx)));
-  TRY(P->alloc_t(&P->eps_cols, (size_t)std::max<int64_t>(n, 1)));
+  if (nb == 0 && !idle) P->hess.chunks.push_back(ib);   // one chunk of no i-blocks: f(x) alone
+  P->scratch.n_groups = (int64_t)P->hess.chunks.size() - 1;
+  TRY(P->alloc_t(&P->hess.V, (size_t)(1 + max_vals)));
+  TRY(P->alloc_t(&P->scratch.xp, (size_t)(batch * P->scratch.ldx)));
+  TRY(P->alloc_t(&P->hess.eps, (size_t)std::max<int64_t>(n, 1)));
   // byte model per Hessian (this rank's share): values read back by the assembly, owned entries of H written, the
   // one-time replication of x into the B rows, and the patches (each changed component written once and restored once:
   // 2 per diagonal point, 4 per other point)
   const int64_t patched = 2 * own_points - 2 * nb;
-  P->alg_bytes = idle ? 0 : 8 * P->hess_points + 8 * P->E + 8 * n * batch + 16 * patched;
+  P->alg_bytes = idle ? 0 : 8 * P->hess.points + 8 * P->hess.entries + 8 * n * batch + 16 * patched;
   *plan = owner.release();
   return FDB_OK;
 }
 
 static fdb_status hessian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *x, double *H, double *fx_out,
                                 double relstep, double absstep, cudaStream_t s) {
-  const int64_t n = P->n, ldx = P->ldx;
-  const int32_t B = (int32_t)P->batch;
+  const int64_t n = P->n, ldx = P->scratch.ldx;
+  const int32_t B = (int32_t)P->scratch.batch;
   if (n > 0) {
     // eps_i = compute_epsilon(Val(:hcentral) / Val(:central), x_i, relstep, absstep) = max(relstep*|x_i|, absstep)  :223,234,252
-    component_eps<<<(int)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, 0, n, 1, relstep, absstep, 1.0, P->eps_cols);
-    replicate_x<<<P->grid(n), kThreads, 0, s>>>(x, n, ldx, B, P->xp);
+    component_eps<<<(int)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, 0, n, 1, relstep, absstep, 1.0, P->hess.eps);
+    replicate_x<<<P->grid(n), kThreads, 0, s>>>(x, n, ldx, B, P->scratch.xp);
     P->cnt.kernel_launches += 2;
   }
   // p0 / p_end run over the rank's local sequence (point q > 0 is global point q + off, kernels_hessian.cuh); a chunk's
   // points sit at V[1 ..] whatever its rank
-  const int64_t off = P->hess_off;
+  const int64_t off = P->hess.off;
   int64_t prev_p0 = 0;
   int32_t prev_cnt = 0;
-  for (size_t c = 0; c + 1 < P->hess_chunks.size(); ++c) {
-    const int64_t i0 = P->hess_chunks[c], i1 = P->hess_chunks[c + 1];
+  for (size_t c = 0; c + 1 < P->hess.chunks.size(); ++c) {
+    const int64_t i0 = P->hess.chunks[c], i1 = P->hess.chunks[c + 1];
     const int64_t cs = hess_block_start(i0, n) - off;
     const int64_t p_end = hess_block_start(i1, n) - off;
     for (int64_t p0 = c == 0 ? 0 : cs; p0 < p_end; p0 += B) {
       const int32_t cnt = (int32_t)std::min<int64_t>(B, p_end - p0);
       if (n > 0) {
-        hess_patch<<<P->grid(std::max(cnt, prev_cnt)), kThreads, 0, s>>>(x, P->eps_cols, n, ldx, off, p0, cnt, prev_p0,
-                                                                          prev_cnt, P->xp);
+        hess_patch<<<P->grid(std::max(cnt, prev_cnt)), kThreads, 0, s>>>(x, P->hess.eps, n, ldx, off, p0, cnt, prev_p0,
+                                                                          prev_cnt, P->scratch.xp);
         P->cnt.kernel_launches += 1;
       }
       // f(x) (:209), f(_xpp), f(_xmm) (:233), f(_xpp), f(_xpm), f(_xmp), f(_xmm) (:268-269), in this order
-      const int rc = f(ctx, P->hess_V + (p0 - cs + 1), P->xp, cnt, 1, ldx, (void *)s);
+      const int rc = f(ctx, P->hess.V + (p0 - cs + 1), P->scratch.xp, cnt, 1, ldx, (void *)s);
       P->cnt.f_invocations += 1;
       P->cnt.f_points += cnt;
       if (rc != 0) return fail(FDB_ERR_CALLBACK, "user f returned %d", rc);
@@ -2384,12 +2461,12 @@ static fdb_status hessian_eager(fdb_plan *P, fdb_fn f, void *ctx, const double *
     const int64_t tiles = hess_tiles(n, i0, i1);
     if (tiles > 0) {
       ScatterTimer tm(P, s);
-      hess_assemble<<<P->grid(tiles, 1), kThreads, 0, s>>>(P->hess_V, P->eps_cols, n, i0, i1, tiles, H, P->ldJ);
+      hess_assemble<<<P->grid(tiles, 1), kThreads, 0, s>>>(P->hess.V, P->hess.eps, n, i0, i1, tiles, H, P->ldJ);
       P->cnt.kernel_launches += 1;
       P->cnt.scatter_launches += 1;
     }
   }
-  if (fx_out) CU(cudaMemcpyAsync(fx_out, P->hess_V, 8, cudaMemcpyDeviceToDevice, s));
+  if (fx_out) CU(cudaMemcpyAsync(fx_out, P->hess.V, 8, cudaMemcpyDeviceToDevice, s));
   CU(cudaGetLastError());
   return FDB_OK;
 }
@@ -2402,7 +2479,7 @@ fdb_status fdb_hessian(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, doub
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
   cudaStream_t s = (cudaStream_t)stream;
-  if (P->hess_points == 0) {                 // a rank > 0 without i-blocks: no f call, no launch, d_fx untouched
+  if (P->hess.points == 0) {                 // a rank > 0 without i-blocks: no f call, no launch, d_fx untouched
     P->cnt.jacobians += 1;
     return FDB_OK;
   }
@@ -2430,18 +2507,16 @@ static fdb_status create_derivative(fdb_plan **plan, int64_t m, int64_t n, bool 
   fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
   P->sp_kind = SP_DERIV;
-  P->deriv_elem = elem;
+  P->deriv.elem = elem;
   P->jkind = FDB_J_DENSE;
-  P->E = m;
   P->j_len = m;
   P->ldJ = std::max<int64_t>(m, 1);
-  P->batch = opts && opts->max_batch > 1 ? 2 : 1;
-  P->ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
-  P->ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
-  TRY(P->alloc_t(&P->xp, (size_t)(2 * P->ldx)));
-  TRY(P->alloc_t(&P->Fp, (size_t)(2 * P->ldF)));
-  P->Fm = P->Fp + P->ldF;
-  P->deriv_fcalls = P->fdtype == FDB_COMPLEX ? 1 : 2;
+  P->scratch.batch = opts && opts->max_batch > 1 ? 2 : 1;
+  P->scratch.ldx = std::max<int64_t>(2, (n + 1) & ~(int64_t)1);
+  P->scratch.ldF = std::max<int64_t>(2, (m + 1) & ~(int64_t)1);
+  TRY(P->alloc_t(&P->scratch.xp, (size_t)(2 * P->scratch.ldx)));
+  TRY(P->alloc_t(&P->scratch.Fp, (size_t)(2 * P->scratch.ldF)));
+  P->deriv.fcalls = P->fdtype == FDB_COMPLEX ? 1 : 2;
   // compulsory bytes per call: points pass (x read; one, two or one complex row written) + quotient pass (f rows and,
   // elementwise, x read; df written).  Complex reads the whole complex128 f row and no x.
   const int64_t pts = P->fdtype == FDB_FORWARD ? 16 : 24;
@@ -2468,40 +2543,42 @@ static fdb_status derivative_eager(fdb_plan *P, fdb_fn f, void *ctx, double *df,
   const int al_x = (reinterpret_cast<uintptr_t>(x) & 15) == 0;
   const int64_t tiles_n = (n + kTile - 1) / kTile, tiles_m = (m + kTile - 1) / kTile;
   if (n > 0) {
-    deriv_points<MODE><<<resident_grid(P, deriv_points<MODE>, 0, tiles_n), kThreads, 0, s>>>(x, n, P->ldx, P->xp, st, al_x);
+    deriv_points<MODE><<<resident_grid(P, deriv_points<MODE>, 0, tiles_n), kThreads, 0, s>>>(x, n, P->scratch.ldx, P->scratch.xp, st, al_x);
     P->cnt.kernel_launches += 1;
   }
   // f-call order of the reference: f(x+eps) first, then f(x) (forward without fx) or f(x-eps) (central)
   //   derivatives.jl:209-215,219-222 (per element) / gradients.jl:495-509,513-515
+  // the two f rows of ldF doubles: f(x+eps), then f(x) / f(x-eps)
+  double *const f_hi = P->scratch.Fp, *const f_lo = P->scratch.Fp + P->scratch.ldF;
   int64_t calls = 1;
   const double *fb = nullptr;
-  if (MODE == kCentral && P->batch >= 2) {
-    TRY(call_f(P, f, ctx, P->Fp, P->xp, 2, s));                       // both points in one call: rows 0 (+) and 1 (-)
+  if (MODE == kCentral && P->scratch.batch >= 2) {
+    TRY(call_f(P, f, ctx, f_hi, P->scratch.xp, 2, s));                // both points in one call: rows 0 (+) and 1 (-)
     calls = 2;
-    fb = P->Fm;
+    fb = f_lo;
   } else {
-    TRY(call_f(P, f, ctx, P->Fp, P->xp, 1, s));
+    TRY(call_f(P, f, ctx, f_hi, P->scratch.xp, 1, s));
     if (MODE == kCentral) {
-      TRY(call_f(P, f, ctx, P->Fm, P->xp + P->ldx, 1, s));
+      TRY(call_f(P, f, ctx, f_lo, P->scratch.xp + P->scratch.ldx, 1, s));
       calls = 2;
-      fb = P->Fm;
+      fb = f_lo;
     } else if (MODE == kForward) {
       if (fx) fb = fx;
-      else { TRY(call_f(P, f, ctx, P->Fm, x, 1, s)); calls = 2; fb = P->Fm; }
+      else { TRY(call_f(P, f, ctx, f_lo, x, 1, s)); calls = 2; fb = f_lo; }
     }
   }
-  P->deriv_fcalls = calls;
+  P->deriv.fcalls = calls;
   if (m > 0) {
     const uintptr_t al = reinterpret_cast<uintptr_t>(df) | (fb ? reinterpret_cast<uintptr_t>(fb) : 0) |
-                         (P->deriv_elem && MODE != kComplex ? reinterpret_cast<uintptr_t>(x) : 0);
+                         (P->deriv.elem && MODE != kComplex ? reinterpret_cast<uintptr_t>(x) : 0);
     const int aligned = (al & 15) == 0;
     ScatterTimer tm(P, s);
-    if (P->deriv_elem)
+    if (P->deriv.elem)
       deriv_quotient<MODE, true><<<resident_grid(P, deriv_quotient<MODE, true>, 0, tiles_m), kThreads, 0, s>>>(
-          P->Fp, fb, x, df, m, st, aligned);
+          f_hi, fb, x, df, m, st, aligned);
     else
       deriv_quotient<MODE, false><<<resident_grid(P, deriv_quotient<MODE, false>, 0, tiles_m), kThreads, 0, s>>>(
-          P->Fp, fb, x, df, m, st, aligned);
+          f_hi, fb, x, df, m, st, aligned);
     P->cnt.kernel_launches += 1;
     P->cnt.scatter_launches += 1;
   }
@@ -2552,35 +2629,35 @@ fdb_status fdb_jacobian_host(fdb_plan *P, fdb_fn f, void *ctx, const double *h_x
   if ((P->n > 0 && !h_x) || (P->j_len > 0 && !h_J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   DeviceGuard g(P->device);
   if (!g.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", P->device);
-  if (!P->hstream) {
-    CU(cudaStreamCreateWithFlags(&P->hstream, cudaStreamNonBlocking));
-    TRY(P->alloc_t(&P->h_dx, (size_t)std::max<int64_t>(P->n, 1)));
-    TRY(P->alloc_t(&P->h_dJ, (size_t)std::max<int64_t>(P->j_len, 1)));
-    TRY(P->alloc_t(&P->h_dfx, (size_t)P->ldF));
-    TRY(P->alloc_t(&P->h_dfin, (size_t)P->ldF));
+  if (!P->host.stream) {
+    CU(cudaStreamCreateWithFlags(&P->host.stream, cudaStreamNonBlocking));
+    TRY(P->alloc_t(&P->host.dx, (size_t)std::max<int64_t>(P->n, 1)));
+    TRY(P->alloc_t(&P->host.dJ, (size_t)std::max<int64_t>(P->j_len, 1)));
+    TRY(P->alloc_t(&P->host.dfx, (size_t)P->scratch.ldF));
+    TRY(P->alloc_t(&P->host.dfin, (size_t)P->scratch.ldF));
   }
-  cudaStream_t s = P->hstream;
-  if (P->n > 0) CU(cudaMemcpyAsync(P->h_dx, h_x, (size_t)P->n * 8, cudaMemcpyHostToDevice, s));
+  cudaStream_t s = P->host.stream;
+  if (P->n > 0) CU(cudaMemcpyAsync(P->host.dx, h_x, (size_t)P->n * 8, cudaMemcpyHostToDevice, s));
   const double *fin = nullptr;
   if (h_f_in && P->fdtype == FDB_FORWARD) {
-    CU(cudaMemcpyAsync(P->h_dfin, h_f_in, (size_t)P->m * 8, cudaMemcpyHostToDevice, s));
-    fin = P->h_dfin;
+    CU(cudaMemcpyAsync(P->host.dfin, h_f_in, (size_t)P->m * 8, cudaMemcpyHostToDevice, s));
+    fin = P->host.dfin;
   }
-  fdb_status st = jacobian_run(P, f, ctx, P->h_dx, P->h_dJ, P->h_dfx, fin, relstep, absstep, dir, (void *)s);
+  fdb_status st = jacobian_run(P, f, ctx, P->host.dx, P->host.dJ, P->host.dfx, fin, relstep, absstep, dir, (void *)s);
   if (st != FDB_OK) { cudaStreamSynchronize(s); return st; }
   if (P->j_len > 0) {
     if (P->jkind == FDB_J_DENSE && P->ldJ > P->m) {
       // strided dense view: only rows [0, m) of each column are J's (the host padding rows stay untouched)
-      const int64_t ncols = P->sp_kind == SP_NONE ? P->col_end - P->col_begin : P->n;
+      const int64_t ncols = P->sp_kind == SP_NONE ? P->columns.end - P->columns.begin : P->n;
       if (P->m > 0 && ncols > 0)
-        CU(cudaMemcpy2DAsync(h_J, (size_t)P->ldJ * 8, P->h_dJ, (size_t)P->ldJ * 8, (size_t)P->m * 8, (size_t)ncols,
+        CU(cudaMemcpy2DAsync(h_J, (size_t)P->ldJ * 8, P->host.dJ, (size_t)P->ldJ * 8, (size_t)P->m * 8, (size_t)ncols,
                              cudaMemcpyDeviceToHost, s));
     } else {
-      CU(cudaMemcpyAsync(h_J, P->h_dJ, (size_t)P->j_len * 8, cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(h_J, P->host.dJ, (size_t)P->j_len * 8, cudaMemcpyDeviceToHost, s));
     }
   }
   if (h_fx && P->fdtype == FDB_FORWARD && !fin && P->m > 0)
-    CU(cudaMemcpyAsync(h_fx, P->h_dfx, (size_t)P->m * 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(h_fx, P->host.dfx, (size_t)P->m * 8, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   return FDB_OK;
 }

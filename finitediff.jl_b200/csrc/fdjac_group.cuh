@@ -248,13 +248,13 @@ fdb_status fdb_group_jacobian(fdb_group *g, fdb_fn f, void *const *ctx, const do
     if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
     // fill_matrix!(J, false) once, by the owner of the buffer, before any member may store into it (the members of a
     // dense group write whole column blocks)
-    if (g->n > 1 && P0->sp_kind != SP_NONE && !scatter_defines_J(P0, P0->C) && P0->j_len > 0) TRY(zero_J(P0, d_J, s0));
+    if (g->n > 1 && P0->sp_kind != SP_NONE && !scatter_defines_J(P0, P0->colors.C) && P0->j_len > 0) TRY(zero_J(P0, d_J, s0));
   }
   return group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {
     fdb_plan *P = g->plans[i];
     const double *fin_i = d_f_in;
     if (i > 0 && d_f_in && P->fdtype == FDB_FORWARD) TRY(member_replica(g, i, g->fin_rep, d_f_in, g->m, s, &fin_i));
-    double *Ji = P->sp_kind == SP_NONE ? d_J + P->col_begin * P->ldJ : d_J;
+    double *Ji = d_J + P->columns.begin * P->ldJ;   // a dense member's column block
     return jacobian_run(P, f, ctx ? ctx[i] : nullptr, xi, Ji, i == 0 ? d_fx : nullptr, fin_i, relstep, absstep, dir, (void *)s);
   }, [](int) { return false; });
 }
@@ -267,7 +267,7 @@ fdb_status fdb_group_hessian(fdb_group *g, fdb_fn f, void *const *ctx, const dou
   // every member stores the entries of its i-blocks straight into the root's H; only the root reports f(x)
   return group_run(g, d_x, (cudaStream_t)stream, [&](int i, const double *xi, cudaStream_t s) {
     return fdb_hessian(g->plans[i], f, ctx ? ctx[i] : nullptr, xi, d_H, i == 0 ? d_fx : nullptr, relstep, absstep, (void *)s);
-  }, [&](int i) { return g->plans[i]->hess_points == 0; });
+  }, [&](int i) { return g->plans[i]->hess.points == 0; });
 }
 
 // ------------------------------------------------------------------------------------------------ fdb_sync (one process per GPU)

@@ -1,5 +1,5 @@
 // fdjac_oop.cuh — the out-of-place Jacobian and JVP (include/fdjac_b200.h, "Out-of-place Jacobian").  Included at the end
-// of fdjac_abi.cu: an out-of-place plan is an in-place colour-loop plan with `oop` set (pristine points, the forward step
+// of fdjac_abi.cu: an out-of-place plan is an in-place colour-loop plan with `oop.on` set (pristine points, the forward step
 // rule in central mode) whose J target is the result (dense kinds).  A sparse result is formed by oop_compact: from the
 // resident f! outputs directly (the in-place scatter is skipped), or, when they come in several groups or several ranks,
 // from the candidates the in-place scatter wrote to a plan-owned buffer (the root's, for a group).
@@ -12,9 +12,9 @@
 
 // `vals`: doubles of the candidate buffer the colour loop writes (the band data of a band sparsity)
 static fdb_status oop_alloc_sparse(fdb_plan *P, int64_t candidates, int64_t vals) {
-  TRY(P->alloc_t(&P->oop_vals, (size_t)std::max<int64_t>(vals, 2)));
+  TRY(P->alloc_t(&P->oop.vals, (size_t)std::max<int64_t>(vals, 2)));
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
-  TRY(P->alloc_t(&P->oop_state, (size_t)ntiles + 1));
+  TRY(P->alloc_t(&P->oop.state, (size_t)ntiles + 1));
   return FDB_OK;
 }
 
@@ -29,39 +29,39 @@ static fdb_plan_opts oop_opts(const fdb_plan_opts *opts) {
 // owns them all, and `dest` itself is used.
 static fdb_status oop_own_slots(fdb_plan *P) {
   if (P->world == 1) {
-    P->oop_dest = P->dest;
-    P->oop_dest_n = P->E;
+    P->oop.dest = P->entries.dest;
+    P->oop.dest_n = P->colors.E;
     return FDB_OK;
   }
-  const int64_t E = P->E;
-  const size_t cb = (size_t)P->color_bits / 8;
+  const int64_t E = P->colors.E;
+  const size_t cb = (size_t)P->colors.bits / 8;
   std::vector<int64_t> dest((size_t)E), own;
   std::vector<uint8_t> ec((size_t)E * cb);
   if (E > 0) {
-    TRY(read_back(dest.data(), P->dest, (size_t)E, "reading the dense result's slots"));
-    TRY(read_back(ec.data(), (const uint8_t *)P->ecolor, (size_t)E * cb, "reading the entry colours"));
+    TRY(read_back(dest.data(), P->entries.dest, (size_t)E, "reading the dense result's slots"));
+    TRY(read_back(ec.data(), (const uint8_t *)P->entries.ecolor, (size_t)E * cb, "reading the entry colours"));
   }
   for (int64_t e = 0; e < E; ++e) {
     const uint8_t *p = ec.data() + (size_t)e * cb;
     const uint32_t k = cb == 1 ? *p : (cb == 2 ? *reinterpret_cast<const uint16_t *>(p) : *reinterpret_cast<const uint32_t *>(p));
-    if (k < (uint32_t)P->C && P->owner[k] == P->rank) own.push_back(dest[(size_t)e]);
+    if (k < (uint32_t)P->colors.C && P->colors.owner[k] == P->rank) own.push_back(dest[(size_t)e]);
   }
   int64_t *d = nullptr;
   TRY(P->alloc_t(&d, std::max<size_t>(own.size(), 1)));
   if (!own.empty()) CU(cudaMemcpy(d, own.data(), own.size() * 8, cudaMemcpyHostToDevice));
-  P->oop_dest = d;
-  P->oop_dest_n = (int64_t)own.size();
+  P->oop.dest = d;
+  P->oop.dest_n = (int64_t)own.size();
   return FDB_OK;
 }
 
 // candidates of the whole result: nnz of the sparsity, or m x maximum(colorvec) on the dense branch
 static int64_t oop_candidates(const fdb_plan *P) {
-  if (P->sp_kind == SP_BANDED) return P->oop_band_nnz;
-  return P->sp_kind == SP_NONE ? P->m * P->oop_qcols : P->E;
+  if (P->sp_kind == SP_BANDED) return P->oop.band_nnz;
+  return P->sp_kind == SP_NONE ? P->m * P->oop.qcols : P->colors.E;
 }
 
 // the entry set of a band plan (its bandwidths are clamped to the matrix at creation)
-static BandShape oop_band_shape(const fdb_plan *P) { return make_band_shape(P->m, P->n, P->l, P->u); }
+static BandShape oop_band_shape(const fdb_plan *P) { return make_band_shape(P->m, P->n, P->band.l, P->band.u); }
 
 extern "C" {
 
@@ -88,18 +88,18 @@ fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const 
   PlanPtr owner(raw);
   fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  P->oop = 1;
-  P->oop_kind = result_kind;
-  P->oop_ncols = n;
+  P->oop.on = 1;
+  P->oop.kind = result_kind;
+  P->oop.ncols = n;
   if (result_kind == FDB_OOP_DENSE) TRY(oop_own_slots(P));
   if (result_kind == FDB_OOP_SPARSE && P->rank == 0) {   // the candidate buffer and the compaction are the root's
-    TRY(oop_alloc_sparse(P, P->E, P->E));
+    TRY(oop_alloc_sparse(P, P->colors.E, P->colors.E));
     // one group of resident f! outputs on one rank: the compaction forms the quotients itself, no candidate is stored
-    P->oop_fused = P->n_groups <= 1 && P->world == 1;
-    const int64_t ntiles = (P->E + kTile - 1) / kTile;
-    TRY(P->alloc_t(&P->oop_tile_col, (size_t)std::max<int64_t>(ntiles, 1)));
+    P->oop.fused = P->scratch.n_groups <= 1 && P->world == 1;
+    const int64_t ntiles = (P->colors.E + kTile - 1) / kTile;
+    TRY(P->alloc_t(&P->oop.tile_col, (size_t)std::max<int64_t>(ntiles, 1)));
     if (ntiles > 0) {
-      oop_tile_first_col<<<P->grid(ntiles), kThreads>>>(P->colptr32, n, ntiles, P->oop_tile_col);
+      oop_tile_first_col<<<P->grid(ntiles), kThreads>>>(P->entries.colptr32, n, ntiles, P->oop.tile_col);
       CU(cudaGetLastError());
       CU(cudaDeviceSynchronize());
     }
@@ -130,22 +130,22 @@ fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int
   PlanPtr owner(raw);
   fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  P->oop = 1;
-  P->oop_kind = result_kind;
-  P->oop_ncols = n;
+  P->oop.on = 1;
+  P->oop.kind = result_kind;
+  P->oop.ncols = n;
   const BandShape b = oop_band_shape(P);
-  P->oop_band_nnz = b.E;
+  P->oop.band_nnz = b.E;
   // many colours: the step sizes from the per-colour column lists, in the CSC plan's summation order
-  if (P->C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
+  if (P->colors.C > kEpsRegColors && n > 0) TRY(build_color_lists(P));
   // _make_Ji (jacobians.jl:151-162) throws when two columns of one colour share a row.  A cyclic colouring with more
   // colours than l + u gives distinct colours to every pair of columns that can share one.
-  if (result_kind == FDB_OOP_DENSE && m > 0 && P->C > 0 && !(P->cyclic && P->C > lc + uc)) {
+  if (result_kind == FDB_OOP_DENSE && m > 0 && P->colors.C > 0 && !(P->colors.cyclic && P->colors.C > lc + uc)) {
     DevBuf<unsigned long long> d_c;
     TRY(d_c.alloc(1));
     CU(cudaMemset(d_c.get(), 0, 8));
-    TRY(dispatch_ct(P->color_bits, [&](auto tag) {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) {
       return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
-        count_band_conflicts<<<P->grid(n), kThreads>>>(b, cs, P->C, d_c.get());
+        count_band_conflicts<<<P->grid(n), kThreads>>>(b, cs, P->colors.C, d_c.get());
         CU(cudaGetLastError());
         return FDB_OK;
       });
@@ -159,8 +159,8 @@ fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int
   if (result_kind == FDB_OOP_SPARSE && P->rank == 0) {
     // one group of resident f! outputs on one rank: the compaction forms the quotients itself; otherwise the colour loop's
     // band scatter writes the candidates in band-data layout (every rank into the root's buffer)
-    P->oop_fused = P->n_groups <= 1 && P->world == 1;
-    TRY(oop_alloc_sparse(P, b.E, P->oop_fused ? 0 : P->j_len));
+    P->oop.fused = P->scratch.n_groups <= 1 && P->world == 1;
+    TRY(oop_alloc_sparse(P, b.E, P->oop.fused ? 0 : P->j_len));
   }
   *plan = owner.release();
   return FDB_OK;
@@ -205,10 +205,10 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
   PlanPtr owner(raw);
   fdb_plan *P = owner.get();
   DeviceGuard g(P->device);
-  P->oop = 1;
-  P->oop_kind = result_kind;
-  P->oop_ncols = ncols_out;
-  P->oop_qcols = C;
+  P->oop.on = 1;
+  P->oop.kind = result_kind;
+  P->oop.ncols = ncols_out;
+  P->oop.qcols = C;
   if (result_kind == FDB_OOP_SPARSE && P->rank == 0) TRY(oop_alloc_sparse(P, m * C, m * C));
   *plan = owner.release();
   return FDB_OK;
@@ -218,7 +218,7 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
 
 // `out` can take the whole result of P's kind
 static fdb_status oop_check_out(const fdb_plan *P, const fdb_oop_out *out) {
-  if (P->oop_kind != FDB_OOP_SPARSE) return FDB_OK;
+  if (P->oop.kind != FDB_OOP_SPARSE) return FDB_OK;
   const int64_t candidates = oop_candidates(P);
   if (!out->colptr || !out->nnz || (candidates > 0 && (!out->rowval || !out->nzval)))
     return fail(FDB_ERR_INVALID, "NULL colptr, rowval, nzval or nnz");
@@ -234,29 +234,29 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
                              const double *d_f_in, double relstep, double absstep, double dir, cudaStream_t s) {
   if (oop_idle(P)) return FDB_OK;
   const bool full = P->sp_kind == SP_NONE;
-  double *J = full ? base + P->col_begin * P->ldJ : base;
+  double *J = base + P->columns.begin * P->ldJ;   // dense branch: this rank's column block
   DeviceGuard g(P->device);
   // a sparse result whose colorvec has no valid colour: nobody scatters, and the candidates are the zeros of rank 0
-  const int64_t cand_len = P->sp_kind == SP_BANDED ? P->j_len : P->E;   // band data: every column's slots
-  if (P->oop_kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->local_colors.empty() && cand_len > 0)
+  const int64_t cand_len = P->sp_kind == SP_BANDED ? P->j_len : P->colors.E;   // band data: every column's slots
+  if (P->oop.kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->colors.local.empty() && cand_len > 0)
     CU(cudaMemsetAsync(J, 0, (size_t)cand_len * 8, s));
   if ((P->n > 0 && !d_x) || (P->j_len > 0 && !J)) return fail(FDB_ERR_INVALID, "NULL x or J");
   TRY(jacobian_run(P, f, ctx, d_x, J, d_fx, d_f_in, relstep, absstep, dir, (void *)s));
-  if (P->oop_kind == FDB_OOP_DENSE) {
+  if (P->oop.kind == FDB_OOP_DENSE) {
     if (P->sp_kind == SP_BANDED) {
       // + 0.0 over the band entries of this rank's colours, in closed form
       const BandShape b = oop_band_shape(P);
-      if (b.E > 0 && !P->local_colors.empty()) {
-        TRY(dispatch_ct(P->color_bits, [&](auto tag) {
+      if (b.E > 0 && !P->colors.local.empty()) {
+        TRY(dispatch_ct(P->colors.bits, [&](auto tag) {
           return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
-            oop_band_plus_zero<<<P->grid(b.E), kThreads, 0, s>>>(J, P->ldJ, b, cs, P->local_of, P->C);
+            oop_band_plus_zero<<<P->grid(b.E), kThreads, 0, s>>>(J, P->ldJ, b, cs, P->colors.local_of, P->colors.C);
             return FDB_OK;
           });
         }));
         P->cnt.kernel_launches += 1;
       }
-    } else if (!full && P->oop_dest_n > 0) {
-      oop_plus_zero_slots<<<P->grid(P->oop_dest_n), kThreads, 0, s>>>(J, P->oop_dest, P->oop_dest_n);
+    } else if (!full && P->oop.dest_n > 0) {
+      oop_plus_zero_slots<<<P->grid(P->oop.dest_n), kThreads, 0, s>>>(J, P->oop.dest, P->oop.dest_n);
       P->cnt.kernel_launches += 1;
     } else if (full && P->m > 0) {
       // column c < C of the block: 0.0 + q; the prototype's columns [C, ncols) are zeros, rank 0's alone
@@ -266,13 +266,13 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
         oop_dense_finish<<<grid, kThreads, 0, s>>>(Jc, P->ldJ, P->m, qcols, ncols);
         P->cnt.kernel_launches += 1;
       };
-      const int64_t ncl = P->col_end - P->col_begin;
-      const int64_t tail = P->rank == 0 ? P->oop_ncols - P->oop_qcols : 0;
-      if (P->col_end == P->oop_qcols) {
+      const int64_t ncl = P->columns.end - P->columns.begin;
+      const int64_t tail = P->rank == 0 ? P->oop.ncols - P->oop.qcols : 0;
+      if (P->columns.end == P->oop.qcols) {
         finish(J, ncl, ncl + tail);
       } else {
         finish(J, ncl, ncl);
-        if (tail > 0) finish(base + P->oop_qcols * P->ldJ, 0, tail);
+        if (tail > 0) finish(base + P->oop.qcols * P->ldJ, 0, tail);
       }
     }
   }
@@ -288,32 +288,32 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
   const int64_t candidates = oop_candidates(P);
   DeviceGuard g(P->device);
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
-  CU(cudaMemsetAsync(P->oop_state, 0, (size_t)(ntiles + 1) * 8, s));
+  CU(cudaMemsetAsync(P->oop.state, 0, (size_t)(ntiles + 1) * 8, s));
   CompactArgs a{};
-  a.vals = P->oop_vals; a.row32 = P->row32; a.colptr32 = P->colptr32;
-  a.ecolor = P->ecolor; a.Fp = P->Fp; a.Fm = P->Fm; a.eps = P->eps; a.ncolors = P->C;
-  a.fx = d_f_in ? d_f_in : (d_fx ? d_fx : P->fx_own);
-  a.ldF = P->fdtype == FDB_COMPLEX ? 2 * P->ldF : P->ldF;
-  a.E = candidates; a.m = P->m; a.C = P->oop_qcols; a.ncols = P->oop_ncols;
+  a.vals = P->oop.vals; a.row32 = P->entries.row32; a.colptr32 = P->entries.colptr32;
+  a.ecolor = P->entries.ecolor; a.Fp = P->scratch.Fp; a.Fm = P->scratch.Fm; a.eps = P->steps.eps; a.ncolors = P->colors.C;
+  a.fx = d_f_in ? d_f_in : (d_fx ? d_fx : P->scratch.fx_own);
+  a.ldF = P->fdtype == FDB_COMPLEX ? 2 * P->scratch.ldF : P->scratch.ldF;
+  a.E = candidates; a.m = P->m; a.C = P->oop.qcols; a.ncols = P->oop.ncols;
   a.colptr = out->colptr; a.rowval = out->rowval; a.nzval = out->nzval; a.nnz = out->nnz;
-  a.state = P->oop_state; a.claim = P->oop_state + ntiles; a.tile_col = P->oop_tile_col;
+  a.state = P->oop.state; a.claim = P->oop.state + ntiles; a.tile_col = P->oop.tile_col;
   if (band) a.band = oop_band_shape(P);
   auto go = [&](auto kern, auto... cs) {
     kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a, cs...);
   };
   if (full) go(oop_compact<true, kCopy, uint8_t>);
-  else if (band && !P->oop_fused) go(oop_compact_band<kCopy, TableColors<uint8_t>>, TableColors<uint8_t>{nullptr});
+  else if (band && !P->oop.fused) go(oop_compact_band<kCopy, TableColors<uint8_t>>, TableColors<uint8_t>{nullptr});
   else if (band) TRY(dispatch_mode(P->fdtype, [&](auto mode) {
-    return dispatch_ct(P->color_bits, [&](auto tag) {
+    return dispatch_ct(P->colors.bits, [&](auto tag) {
       return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
         go(oop_compact_band<decltype(mode)::value, decltype(cs)>, cs);
         return FDB_OK;
       });
     });
   }));
-  else if (!P->oop_fused) go(oop_compact<false, kCopy, uint8_t>);
+  else if (!P->oop.fused) go(oop_compact<false, kCopy, uint8_t>);
   else TRY(dispatch_mode(P->fdtype, [&](auto mode) {
-    return dispatch_ct(P->color_bits, [&](auto tag) -> fdb_status {
+    return dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
       go(oop_compact<false, decltype(mode)::value, decltype(tag)>);
       return FDB_OK;
     });
@@ -326,14 +326,14 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
 // An out-of-place call once check_call has accepted it
 static fdb_status jacobian_oop_run(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                                    const double *d_f_in, double relstep, double absstep, double dir, void *stream) {
-  const bool sparse = P->oop_kind == FDB_OOP_SPARSE;
+  const bool sparse = P->oop.kind == FDB_OOP_SPARSE;
   if (sparse && P->world > 1)
     return fail(FDB_ERR_INVALID, "a sparse result is compacted over every rank's candidates on one device: run sparse rank "
                                  "plans through fdb_group_create_oop_* / fdb_group_jacobian_oop");
   if (!sparse && P->j_len > 0 && !out->J) return fail(FDB_ERR_INVALID, "NULL x or J");
   TRY(oop_check_out(P, out));
   cudaStream_t s = (cudaStream_t)stream;
-  TRY(oop_member(P, f, ctx, d_x, sparse ? P->oop_vals : out->J, d_fx, d_f_in, relstep, absstep, dir, s));
+  TRY(oop_member(P, f, ctx, d_x, sparse ? P->oop.vals : out->J, d_fx, d_f_in, relstep, absstep, dir, s));
   if (sparse) TRY(oop_root_finish(P, out, d_fx, d_f_in, s));
   return FDB_OK;
 }
@@ -393,7 +393,7 @@ fdb_status fdb_group_jacobian_oop(fdb_group *g, fdb_fn f, void *const *ctx, cons
   fdb_plan *P0 = g->plans[0];
   TRY(check_call(P0, Call::group_jacobian_oop));
   if (P0->n > 0 && !d_x) return fail(FDB_ERR_INVALID, "NULL x");
-  const bool sparse = P0->oop_kind == FDB_OOP_SPARSE;
+  const bool sparse = P0->oop.kind == FDB_OOP_SPARSE;
   if (!sparse && P0->j_len > 0 && !out->J) return fail(FDB_ERR_INVALID, "NULL x or J");
   TRY(oop_check_out(P0, out));
   const int root = g->devices[0];
@@ -403,10 +403,10 @@ fdb_status fdb_group_jacobian_oop(fdb_group *g, fdb_fn f, void *const *ctx, cons
     if (!dg.ok) return fail(FDB_ERR_CUDA, "cannot select device %d", root);
     // a dense result of a CSC or band sparsity: zero-filled once, by the owner of the buffer, before any member stores
     // into it
-    if (g->n > 1 && P0->oop_kind == FDB_OOP_DENSE && (P0->sp_kind == SP_CSC || P0->sp_kind == SP_BANDED) && P0->j_len > 0)
+    if (g->n > 1 && P0->oop.kind == FDB_OOP_DENSE && (P0->sp_kind == SP_CSC || P0->sp_kind == SP_BANDED) && P0->j_len > 0)
       TRY(zero_J(P0, out->J, s0));
   }
-  double *base = sparse ? P0->oop_vals : out->J;
+  double *base = sparse ? P0->oop.vals : out->J;
   TRY(group_run(g, d_x, s0, [&](int i, const double *xi, cudaStream_t s) {
     fdb_plan *P = g->plans[i];
     const double *fin_i = d_f_in;
