@@ -16,6 +16,7 @@ SYNTH_PATH = HERE / "libfdjac_synth.so"
 FDB_OK, FDB_ERR_INVALID, FDB_ERR_CUDA, FDB_ERR_CALLBACK, FDB_ERR_NOMEM, FDB_ERR_UNSUPPORTED, FDB_ERR_NO_DEVICE = range(7)
 FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = 0, 1, 2, 3
 FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND, FDB_J_DIAGONALS = 0, 1, 2, 3, 4, 5
+FDB_J_BLOCK_DENSE = 6
 FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = 0, 1, 2
 # FDB_STEP_DEFAULT: relstep / absstep keyword not given (any other value, 0 included, is used as passed)
 STEP_DEFAULT = float("nan")
@@ -74,6 +75,7 @@ ABI_SYMBOLS = {
     "fdb_plan_create_coo": (_int, [_PP, _i64, _i64, _i64, _vp, _vp, _int, _vp, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_banded": (_int, [_PP, _i64, _i64, _i64, _i64, _int, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_block_banded": (_int, [_PP, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
+    "fdb_plan_create_block_dense": (_int, [_PP, _i64, _vp, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_dense": (_int, [_PP, _i64, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_plan_create_dense_colorvec": (_int, [_PP, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_destroy": (_int, [_vp]),
@@ -96,6 +98,8 @@ ABI_SYMBOLS = {
     "fdb_group_create_dense": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_group_create_block_banded": (_int, [_PP, _int, C.POINTER(_int), _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp,
                                               C.POINTER(PlanOpts)]),
+    "fdb_group_create_block_dense": (_int, [_PP, _int, C.POINTER(_int), _i64, _vp, _i64, _i64, _i64, _vp,
+                                             C.POINTER(PlanOpts)]),
     "fdb_group_destroy": (_int, [_vp]),
     "fdb_group_size": (_int, [_vp, C.POINTER(_int)]),
     "fdb_group_plan": (_int, [_vp, _int, _PP]),

@@ -32,7 +32,7 @@ from . import _lib as L
 
 __all__ = [
     "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "Diagonal", "Bidiagonal", "SymTridiagonal", "BandedBlockBandedMatrix",
-    "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
+    "BlockSkylineMatrix", "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
     "finite_difference_jacobian_", "finite_difference_jacobian_b", "resize_", "default_relstep", "compute_epsilon",
     "zeros_colmajor", "pinned_empty", "HessianCache", "finite_difference_hessian_", "finite_difference_hessian",
     "GradientCache", "finite_difference_gradient_", "finite_difference_gradient", "DerivativeCache",
@@ -435,6 +435,64 @@ class BlockBandedMatrix(BandedBlockBandedMatrix):
         super().__init__(rowblocks, colblocks, blockbandwidths, (full, full), data=data, device=device)
 
 
+class BlockSkylineMatrix:
+    """Mirror of BlockBandedMatrices.BlockBandedMatrix as that package stores it (a BlockSkylineMatrix with constant
+    block bandwidths (l, u)): dense blocks inside the block band, hook ext/FiniteDiffBlockBandedMatricesExt.jl:44-68.
+    Block column J (0-based here) covers block rows max(0, J-u) .. min(N-1, J+l); its data is one column-major slab of
+    height h_J (the rows of those blocks) and cb[J] columns, starting at slot start_J = sum_{J'<J} h_J' cb[J'].  Entry
+    (r, c) of block (K, J) sits at start_J + c h_J + rowoff_J(K) + r.  Every slot is a structural entry, so `data` holds
+    j_len = start_N values and nothing else.  (BlockBandedMatrix above is this structure in the padded band layout.)"""
+
+    def __init__(self, rowblocks, colblocks, blockbandwidths, data=None, device="cuda"):
+        self.rb, self.cb = [int(b) for b in rowblocks], [int(b) for b in colblocks]
+        self.l, self.u = (int(b) for b in blockbandwidths)
+        self.m, self.n = sum(self.rb), sum(self.cb)
+        ro = np.concatenate([[0], np.cumsum(self.rb, dtype=np.int64)]).astype(np.int64)
+        Nr = len(self.rb)
+        J = np.arange(len(self.cb), dtype=np.int64)
+        k0 = np.clip(J - self.u, 0, Nr)                                 # block rows [k0, k1) of block column J
+        k1 = np.clip(J + self.l + 1, k0, Nr)
+        self.row0 = ro[k0]                                              # first row of each slab, 0-based
+        self.heights = ro[k1] - ro[k0]
+        self.col0 = np.concatenate([[0], np.cumsum(self.cb, dtype=np.int64)])[:-1].astype(np.int64)
+        self.starts = np.concatenate([[0], np.cumsum(self.heights * np.asarray(self.cb, np.int64))]).astype(np.int64)
+        self.j_len = int(self.starts[-1])
+        if data is None:
+            data = torch.zeros(self.j_len, dtype=torch.float64, device=device)
+        self.data = data
+        self._nz = None
+
+    @property
+    def shape(self):
+        return (self.m, self.n)
+
+    def findstructralnz(self):
+        """(rows, cols, slots), 1-based, in the order the reference's hook visits them: block column J, its column j,
+        then every row of every block row in blockcolrange(J) — which is storage order, so slots = 1:j_len."""
+        if self._nz is None:
+            s = np.arange(self.j_len, dtype=np.int64)
+            J = np.searchsorted(self.starts, s, side="right") - 1     # an empty slab shares its start with the next
+            rel = s - self.starts[J]
+            h = self.heights[J]
+            self._nz = (self.row0[J] + rel % h + 1, self.col0[J] + rel // h + 1, s + 1)
+        return self._nz
+
+    def to_dense(self) -> np.ndarray:
+        rows, cols, slots = self.findstructralnz()
+        d = self.data.cpu().numpy() if isinstance(self.data, torch.Tensor) else np.asarray(self.data)
+        J = np.zeros((self.m, self.n))
+        J[rows - 1, cols - 1] = d[slots - 1]
+        return J
+
+    def matrix_colors(self) -> np.ndarray:
+        """A valid colouring for the full structure: block colour (cycle l+u+1) x column within the block, b colours
+        per block colour — ArrayInterface.matrix_colors(::BlockBandedMatrix) for uniform blocks of size b, so
+        (l+u+1)*b colours.  Non-uniform blocks take b = the largest block."""
+        bw, b = max(self.l + self.u + 1, 1), max(self.cb, default=0)
+        out = [(J % bw) * b + np.arange(nb) + 1 for J, nb in enumerate(self.cb)]
+        return np.concatenate(out).astype(np.int64) if out else np.zeros(0, np.int64)
+
+
 class DenseColumnBlock:
     """Columns [col0, col0+ncols) of a dense m x n Jacobian held by ONE rank (north_star config 5: the dense Jacobian is
     column-partitioned over the GPUs and may stay that way): `slab` is the rank's own column-major (m, ncols) storage.
@@ -760,6 +818,17 @@ def _plan_route(J, sparsity, colorvec):
         blocks, l, u, lam, mu, ldata = bb
         return "block_banded", (len(blocks), blocks.ctypes.data if len(blocks) else None, l, u, lam, mu, ldata,
                                 cv_ptr), keep + [blocks]
+    if isinstance(sparsity, BlockSkylineMatrix):
+        # ext/FiniteDiffBlockBandedMatricesExt.jl:44-68 takes the row and the colour blocks from axes(Jac, 1)
+        if sparsity.rb != sparsity.cb:
+            raise L.FdbError(L.FDB_ERR_INVALID, "a BlockBandedMatrix Jacobian needs square blocks (rowblocks == colblocks)")
+        if isinstance(J, BlockSkylineMatrix):
+            if (J.rb, J.cb, J.l, J.u) != (sparsity.rb, sparsity.cb, sparsity.l, sparsity.u):
+                raise ValueError("J and sparsity must have the same block structure")
+            blocks = np.asarray(J.rb, dtype=np.int64)
+            ldata = J.data.numel() if isinstance(J.data, torch.Tensor) else J.j_len
+            return "block_dense", (len(blocks), blocks.ctypes.data if len(blocks) else None, J.l, J.u, ldata, cv_ptr), \
+                keep + [blocks]
     if isinstance(sparsity, (Tridiagonal, SymTridiagonal)):
         rows, cols, slots = sparsity.findstructralnz()
         n = sparsity.n
@@ -782,6 +851,14 @@ def _plan_route(J, sparsity, colorvec):
             jargs = (m, nn, L.FDB_J_DENSE, None, ld)
         else:
             raise TypeError(f"unsupported J type {type(J)} for a BandedBlockBandedMatrix sparsity")
+    elif isinstance(sparsity, BlockSkylineMatrix):
+        # a dense J: the hook's entry set, written by (row, column)
+        rows, cols, slots = sparsity.findstructralnz()
+        slots = None
+        if not isinstance(J, torch.Tensor):
+            raise TypeError(f"unsupported J type {type(J)} for a BlockSkylineMatrix sparsity")
+        m, nn, ld = _dense_ld(J)
+        jargs = (m, nn, L.FDB_J_DENSE, None, ld)
     elif isinstance(sparsity, (torch.Tensor, np.ndarray, list)):
         # dense 0/1 prototype: rows/cols from _findstructralnz (jacobians.jl:526-527), J must be dense
         rows, cols = _findstructralnz_dense(sparsity)
@@ -855,7 +932,8 @@ def _diagonals_route(J, sparsity):
 
 def _has_sparsestruct(J) -> bool:
     """ArrayInterface.has_sparsestruct(J) as used at jacobians.jl:455."""
-    return isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix) + _LA_BANDED)
+    return isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix)
+                      + _LA_BANDED)
 
 
 def _j_values(J):
@@ -865,7 +943,7 @@ def _j_values(J):
         return J.data
     if isinstance(J, (Tridiagonal,) + _LA_BANDED):
         return J.buf
-    if isinstance(J, BandedBlockBandedMatrix):
+    if isinstance(J, (BandedBlockBandedMatrix, BlockSkylineMatrix)):
         return J.data
     if isinstance(J, DenseColumnBlock):
         return J.slab
@@ -887,6 +965,8 @@ def _j_key(J):
         return ("symtri", J.n)
     if isinstance(J, BandedBlockBandedMatrix):
         return ("bbb", tuple(J.rb), tuple(J.cb), J.l, J.u, J.lam, J.mu)
+    if isinstance(J, BlockSkylineMatrix):
+        return ("bsky", tuple(J.rb), tuple(J.cb), J.l, J.u)
     if isinstance(J, torch.Tensor):
         return ("dense", tuple(J.shape), tuple(J.stride()))
     if isinstance(J, DenseColumnBlock):
@@ -899,7 +979,7 @@ def _j_key(J):
 def _sp_key(sp):
     if sp is None:
         return None
-    if isinstance(sp, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix) + _LA_BANDED):
+    if isinstance(sp, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix) + _LA_BANDED):
         return _j_key(sp)
     if isinstance(sp, torch.Tensor):
         return ("proto", sp.data_ptr(), tuple(sp.shape), sp._version)
@@ -1032,7 +1112,7 @@ def matrix_colors(A, device=None) -> torch.Tensor:
         out = out[: A.n]
         out.n_colors, out.n_rounds = nc.value, nr.value
         return out
-    elif isinstance(A, BandedBlockBandedMatrix):
+    elif isinstance(A, (BandedBlockBandedMatrix, BlockSkylineMatrix)):
         return torch.from_numpy(A.matrix_colors()).to(torch.device("cuda") if device is None else torch.device(device))
     elif isinstance(A, torch.Tensor):
         n = A.shape[1] if A.dim() == 2 else 1
@@ -1492,7 +1572,8 @@ def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absst
 
 
 def _shape_of(J):
-    if isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, DenseColumnBlock) + _LA_BANDED):
+    if isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix, DenseColumnBlock)
+                  + _LA_BANDED):
         return J.shape
     if isinstance(J, torch.Tensor):
         if J.dim() == 1:

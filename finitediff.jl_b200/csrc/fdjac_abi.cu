@@ -252,12 +252,14 @@ struct fdb_plan {
   struct Band {
     int64_t l = 0, u = 0;
   } band;
-  // block-banded plans (kernels_blockband.cuh): block offsets on the device, sub-block bandwidths, slots per column
+  // block-banded and block-dense plans (kernels_blockband.cuh): block offsets on the device, sub-block bandwidths, slots
+  // per column (block-banded), the slab starts (block-dense, jkind FDB_J_BLOCK_DENSE)
   struct BlockBand {
     int32_t *off = nullptr;           // [nblocks + 1]
     int32_t nblocks = 0, bs = 0;      // bs > 0: every block has bs columns
     int64_t lam = 0, mu = 0, w = 1;
     bool cyclic = false;              // colorvec is the block-cyclic closed form of matrix_colors
+    int64_t *start = nullptr;         // block-dense: [nblocks + 1] first slot of every block column's slab
   } block_band;
   // dense plans: this rank's column block [begin, end) and its steps
   struct Columns {
@@ -962,6 +964,60 @@ static inline void resolve_steps(int fdtype, double &relstep, double &absstep) {
   if (std::isnan(absstep)) absstep = relstep;
 }
 
+// The block sizes of a block-structured plan (host or device Int64), their 0-based offsets off[nblocks + 1] and their
+// sum n: a negative size is FDB_ERR_INVALID, more than 2^31 columns FDB_ERR_UNSUPPORTED
+static fdb_status read_block_sizes(int64_t nblocks, const int64_t *blocks, std::vector<int64_t> &hb,
+                                   std::vector<int32_t> &off, int64_t &n) {
+  hb.assign((size_t)nblocks, 0);
+  if (nblocks > 0) {
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, blocks) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+    if (at.type == cudaMemoryTypeDevice) CU(cudaMemcpy(hb.data(), blocks, (size_t)nblocks * 8, cudaMemcpyDeviceToHost));
+    else std::memcpy(hb.data(), blocks, (size_t)nblocks * 8);
+  }
+  off.assign((size_t)nblocks + 1, 0);
+  n = 0;
+  for (int64_t K = 0; K < nblocks; ++K) {
+    if (hb[(size_t)K] < 0) return fail(FDB_ERR_INVALID, "block %lld has negative size %lld", (long long)K, (long long)hb[(size_t)K]);
+    n += hb[(size_t)K];
+    if (n > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "the block sizes sum to more than 2^31 columns");
+    off[(size_t)K + 1] = (int32_t)n;
+  }
+  return FDB_OK;
+}
+
+// The rest of a block-structured plan once its colours are set up: pass(CT{}, cnt, not_cyclic) launches the kind's plan
+// pass, which sums the structural entries per colour (the LPT weights; cnt[C]: columns without a valid colour) and
+// clears nothing in *not_cyclic when the colouring is the kind's block-cyclic closed form.  Fills colors.E and
+// block_band.cyclic, then the coloured plan's ownership and scratch.
+template <typename Pass>
+static fdb_status finish_block_plan(fdb_plan *P, const fdb_plan_opts *opts, Pass &&pass) {
+  const int64_t n = P->n;
+  DevBuf<unsigned long long> d_cnt;
+  DevBuf<uint32_t> d_flag;
+  TRY(d_cnt.alloc((size_t)P->colors.C + 1));
+  TRY(d_flag.alloc(1));
+  CU(cudaMemset(d_cnt.get(), 0, ((size_t)P->colors.C + 1) * 8));
+  CU(cudaMemset(d_flag.get(), 0, 4));
+  if (n > 0) {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
+      pass(tag, d_cnt.get(), d_flag.get());
+      CU(cudaGetLastError());
+      return FDB_OK;
+    }));
+  }
+  std::vector<unsigned long long> cnt((size_t)P->colors.C + 1, 0);
+  TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C + 1, "block-banded entry counts"));
+  uint32_t not_cyclic = 1;
+  TRY(read_back(&not_cyclic, d_flag.get(), 1, "block-banded colouring form"));
+  P->block_band.cyclic = n > 0 && P->colors.C > 0 && not_cyclic == 0;
+  unsigned long long total = 0;
+  for (auto c : cnt) total += c;
+  P->colors.E = (int64_t)total;
+  cnt.resize((size_t)std::max<int32_t>(P->colors.C, 1));
+  return finish_colored_plan(P, opts, cnt);
+}
+
 // ------------------------------------------------------------------------------------------------ exported: misc
 extern "C" {
 
@@ -1237,21 +1293,10 @@ fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const 
   if (l >= kMaxW || u >= kMaxW || lam >= kMaxW || mu >= kMaxW || (l + u + 1) > kMaxW / (lam + mu + 1))
     return fail(FDB_ERR_UNSUPPORTED, "(l+u+1)(lam+mu+1) slots per column must be below 2^31");
   const int64_t w = (l + u + 1) * (lam + mu + 1);
-  std::vector<int64_t> hb((size_t)nblocks);
-  if (nblocks > 0) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, blocks) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
-    if (at.type == cudaMemoryTypeDevice) CU(cudaMemcpy(hb.data(), blocks, (size_t)nblocks * 8, cudaMemcpyDeviceToHost));
-    else std::memcpy(hb.data(), blocks, (size_t)nblocks * 8);
-  }
-  std::vector<int32_t> off((size_t)nblocks + 1, 0);
+  std::vector<int64_t> hb;
+  std::vector<int32_t> off;
   int64_t n = 0;
-  for (int64_t K = 0; K < nblocks; ++K) {
-    if (hb[(size_t)K] < 0) return fail(FDB_ERR_INVALID, "block %lld has negative size %lld", (long long)K, (long long)hb[(size_t)K]);
-    n += hb[(size_t)K];
-    if (n > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "the block sizes sum to more than 2^31 columns");
-    off[(size_t)K + 1] = (int32_t)n;
-  }
+  TRY(read_block_sizes(nblocks, blocks, hb, off, n));
   if (ldata < w * n) return fail(FDB_ERR_INVALID, "ldata=%lld < (l+u+1)(lam+mu+1)*n = %lld", (long long)ldata, (long long)(w * n));
   PlanPtr owner;
   TRY(new_plan(plan, owner, opts, n, n));
@@ -1270,34 +1315,68 @@ fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const 
   TRY(P->alloc_t(&P->block_band.off, (size_t)nblocks + 1));
   CU(cudaMemcpy(P->block_band.off, off.data(), ((size_t)nblocks + 1) * 4, cudaMemcpyHostToDevice));
   TRY(setup_colors(P, colorvec));
-  // structural entries per colour (the LPT weights; slot C: columns without a valid colour) and the colouring's form
-  DevBuf<unsigned long long> d_cnt;
-  DevBuf<uint32_t> d_flag;
-  TRY(d_cnt.alloc((size_t)P->colors.C + 1));
-  TRY(d_flag.alloc(1));
-  CU(cudaMemset(d_cnt.get(), 0, ((size_t)P->colors.C + 1) * 8));
-  CU(cudaMemset(d_flag.get(), 0, 4));
-  if (n > 0) {
-    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
-      using CT = decltype(tag);
-      block_band_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, P->block_band.off, (int32_t)nblocks, (int32_t)n, l, u,
-                                                        lam, mu, P->colors.C, d_cnt.get(), d_flag.get());
-      CU(cudaGetLastError());
-      return FDB_OK;
-    }));
-  }
-  std::vector<unsigned long long> cnt((size_t)P->colors.C + 1, 0);
-  TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C + 1, "block-banded entry counts"));
-  uint32_t not_cyclic = 1;
-  TRY(read_back(&not_cyclic, d_flag.get(), 1, "block-banded colouring form"));
-  P->block_band.cyclic = n > 0 && P->colors.C > 0 && not_cyclic == 0;
-  unsigned long long total = 0;
-  for (auto c : cnt) total += c;
-  P->colors.E = (int64_t)total;
-  cnt.resize((size_t)std::max<int32_t>(P->colors.C, 1));
-  TRY(finish_colored_plan(P, opts, cnt));
+  TRY(finish_block_plan(P, opts, [&](auto tag, unsigned long long *cnt, uint32_t *not_cyclic) {
+    using CT = decltype(tag);
+    block_band_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, P->block_band.off, (int32_t)nblocks, (int32_t)n, l, u,
+                                                      lam, mu, P->colors.C, cnt, not_cyclic);
+  }));
   // every slot written once + the f! outputs read (one slab and f(x) / the minus slab per colour)
   P->alg_bytes = 8 * w * n + 16 * n * (int64_t)P->colors.C;
+  return finish_plan(owner, plan);
+}
+
+// BlockBandedMatrix with square blocks (ext/FiniteDiffBlockBandedMatricesExt.jl:44-68) in BlockBandedMatrices' own
+// storage: one column-major slab per block column (kernels_blockband.cuh).  Host work O(nblocks); the plan keeps the
+// block offsets and the slab starts on the device.
+fdb_status fdb_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                       int64_t ldata, const int64_t *colorvec, const fdb_plan_opts *opts) {
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  if (nblocks < 0 || nblocks > 0x7FFFFFF0LL) return fail(FDB_ERR_INVALID, "nblocks=%lld outside [0, 2^31)", (long long)nblocks);
+  if (nblocks > 0 && !blocks) return fail(FDB_ERR_INVALID, "blocks is NULL");
+  if (l < 0 || u < 0) return fail(FDB_ERR_INVALID, "negative block bandwidths (l, u) = (%lld, %lld)", (long long)l, (long long)u);
+  std::vector<int64_t> hb;
+  std::vector<int32_t> off;
+  int64_t n = 0;
+  TRY(read_block_sizes(nblocks, blocks, hb, off, n));
+  // bandwidths of nblocks or more describe the same structure (and the same closed-form colouring) as nblocks
+  l = std::min(l, nblocks);
+  u = std::min(u, nblocks);
+  // slab J: the rows of block rows max(0, J-u) .. min(N-1, J+l), cb[J] columns; the kernel indexes a slab with 32 bits
+  std::vector<int64_t> start((size_t)nblocks + 1, 0);
+  for (int64_t J = 0; J < nblocks; ++J) {
+    const int64_t K0 = std::max<int64_t>(0, J - u), K1 = std::min<int64_t>(nblocks - 1, J + l);
+    const int64_t slab = (int64_t)(off[(size_t)K1 + 1] - off[(size_t)K0]) * hb[(size_t)J];
+    if (slab > 0xFFFFFFFFLL)
+      return fail(FDB_ERR_UNSUPPORTED, "block column %lld holds %lld slots; a block column is limited to 2^32", (long long)J,
+                  (long long)slab);
+    start[(size_t)J + 1] = start[(size_t)J] + slab;
+  }
+  const int64_t jlen = start[(size_t)nblocks];
+  if (ldata < jlen) return fail(FDB_ERR_INVALID, "ldata=%lld < the %lld slots of the block columns", (long long)ldata, (long long)jlen);
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, n, n));
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  P->sp_kind = SP_BLOCKBAND;
+  P->jkind = FDB_J_BLOCK_DENSE;
+  P->band.l = l;
+  P->band.u = u;
+  P->block_band.nblocks = (int32_t)nblocks;
+  P->j_len = jlen;
+  P->block_band.bs = nblocks > 0 && hb[0] > 0 && std::all_of(hb.begin(), hb.end(), [&](int64_t b) { return b == hb[0]; }) ? (int32_t)hb[0] : 0;
+  TRY(P->alloc_t(&P->block_band.off, (size_t)nblocks + 1));
+  CU(cudaMemcpy(P->block_band.off, off.data(), ((size_t)nblocks + 1) * 4, cudaMemcpyHostToDevice));
+  TRY(P->alloc_t(&P->block_band.start, (size_t)nblocks + 1));
+  CU(cudaMemcpy(P->block_band.start, start.data(), ((size_t)nblocks + 1) * 8, cudaMemcpyHostToDevice));
+  TRY(setup_colors(P, colorvec));
+  TRY(finish_block_plan(P, opts, [&](auto tag, unsigned long long *cnt, uint32_t *not_cyclic) {
+    using CT = decltype(tag);
+    block_dense_plan_pass<CT><<<P->grid(n), kThreads>>>((const CT *)P->colors.jcolor, P->block_band.off, (int32_t)nblocks, (int32_t)n, l, u,
+                                                       P->block_band.bs, P->colors.C, cnt, not_cyclic);
+  }));
+  // the block-banded byte model: every slot written once + the f! outputs read
+  P->alg_bytes = 8 * jlen + 16 * n * (int64_t)P->colors.C;
   return finish_plan(owner, plan);
 }
 
@@ -1573,12 +1652,12 @@ static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
 // How a coloured plan turns a group's f! outputs into J: one launcher per family (scatter_lists ... scatter_entries), and
 // none for an out-of-place sparse result whose compaction forms the quotients itself (fdjac_oop.cuh).  Fixed once the
 // plan is built, but derived rather than stored: the out-of-place creators set oop.fused after the in-place creator.
-enum class Scatter { none, lists, block_band, diagonals, band, entries };
+enum class Scatter { none, lists, block_band, block_dense, diagonals, band, entries };
 
 static Scatter scatter_family(const fdb_plan *P) {
   if (P->oop.fused) return Scatter::none;
   if (P->sp_kind == SP_CSC && P->entries.strategy == 1) return Scatter::lists;
-  if (P->sp_kind == SP_BLOCKBAND) return Scatter::block_band;
+  if (P->sp_kind == SP_BLOCKBAND) return P->jkind == FDB_J_BLOCK_DENSE ? Scatter::block_dense : Scatter::block_band;
   if (P->sp_kind == SP_BANDED) return P->jkind == FDB_J_DIAGONALS ? Scatter::diagonals : Scatter::band;
   return Scatter::entries;
 }
@@ -1588,7 +1667,7 @@ static Scatter scatter_family(const fdb_plan *P) {
 // out-of-place plan stores no candidate, and its candidate buffer is not J-sized: nothing to fill.
 static bool scatter_defines_J(const fdb_plan *P, int64_t colours) {
   const Scatter f = scatter_family(P);
-  if (f == Scatter::none || f == Scatter::block_band) return true;
+  if (f == Scatter::none || f == Scatter::block_band || f == Scatter::block_dense) return true;
   if (f == Scatter::band && P->jkind != FDB_J_BAND) return false;   // a dense J
   if ((f == Scatter::lists || f == Scatter::entries) && P->entries.dest != nullptr) return false;   // explicit destinations
   return colours > 0;
@@ -1778,6 +1857,28 @@ static fdb_status scatter_block_band(const ScatterGroup &g) {
   return FDB_OK;
 }
 
+// block-dense: every slot of the columns of the group's colours, and (first group of rank 0) of the columns without a
+// valid colour: storage order, block column from the slab starts
+template <typename CT, int MODE>
+static fdb_status scatter_block_dense(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  BlockDenseArgs a{};
+  a.jcolor = P->colors.jcolor; a.boff = P->block_band.off; a.start = P->block_band.start; a.fx = g.fx; a.Fp = g.Fp;
+  a.Fm = g.Fm; a.eps = P->steps.eps; a.local_of = P->colors.local_of; a.J = g.J; a.total = P->j_len; a.ldF = g.ldF;
+  a.C = P->colors.C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  a.write_other = g.first ? 1 : 0;
+  a.nblocks = P->block_band.nblocks; a.l = (int32_t)P->band.l; a.u = (int32_t)P->band.u;
+  a.bs = P->block_band.bs;
+  a.block_cyclic = P->block_band.cyclic ? 1 : 0;
+  a.bw = make_fastdiv((uint32_t)(P->band.l + P->band.u + 1));
+  const size_t sm = color_table_smem(P);
+  const int64_t tiles = (a.total + kBbTile - 1) / kBbTile;
+  const int grid = oversubscribed_grid(P, diff_scatter_block_dense<CT, MODE>, sm, tiles, 16);
+  ScatterTimer tm(P, g.s);
+  diff_scatter_block_dense<CT, MODE><<<grid, kThreads, sm, g.s>>>(a);
+  return FDB_OK;
+}
+
 // diagonal storage: every slot of the columns of the group's colours, and (first group of rank 0) of the columns without
 // a valid colour: storage order, closed-form diagonal and (row, column)
 template <typename CT, int MODE>
@@ -1921,14 +2022,16 @@ static fdb_status scatter(Scatter family, const ScatterGroup &g) {
   // colour-major lists: rank 0 zeroes the entries of the columns without a valid colour with its first group; owning no
   // colour, it does so only where this call does not zero-fill J (peer stores, a shared J)
   if (family == Scatter::lists && g.first && (g.G > 0 || P->peers.n > 0 || P->shared_J)) zero_uncoloured_slots(g);
-  // a rank that owns no colour launches the block-banded scatter of rank 0 alone: the columns without a valid colour
-  if (g.G == 0 && !(family == Scatter::block_band && g.first)) return FDB_OK;
+  // a rank that owns no colour launches the block-banded or block-dense scatter of rank 0 alone: the columns without a
+  // valid colour
+  if (g.G == 0 && !((family == Scatter::block_band || family == Scatter::block_dense) && g.first)) return FDB_OK;
   switch (family) {   // (a group has a colour: C > 0 and n > 0, so band and diagonal storage have slots)
     case Scatter::none: return FDB_OK;
     case Scatter::lists:
       if (P->cm.start_h[(size_t)(g.l0 + g.G)] == P->cm.start_h[(size_t)g.l0]) return FDB_OK;   // empty lists
       TRY(scatter_lists<MODE>(g)); break;
     case Scatter::block_band: if (P->block_band.w * P->n == 0) return FDB_OK; TRY((scatter_block_band<CT, MODE>(g))); break;
+    case Scatter::block_dense: if (P->j_len == 0) return FDB_OK; TRY((scatter_block_dense<CT, MODE>(g))); break;
     case Scatter::diagonals: TRY((scatter_diagonals<CT, MODE>(g))); break;
     case Scatter::band: TRY((scatter_band<CT, MODE>(g))); break;
     case Scatter::entries: if (P->colors.E == 0) return FDB_OK; TRY((scatter_entries<CT, MODE>(g))); break;

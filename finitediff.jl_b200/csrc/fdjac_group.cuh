@@ -207,6 +207,14 @@ fdb_status fdb_group_create_block_banded(fdb_group **group, int n_devices, const
   });
 }
 
+fdb_status fdb_group_create_block_dense(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                        const int64_t *blocks, int64_t l, int64_t u, int64_t ldata, const int64_t *colorvec,
+                                        const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_plan_create_block_dense(p, nblocks, blocks, l, u, ldata, colorvec, o);
+  });
+}
+
 fdb_status fdb_group_destroy(fdb_group *group) {
   free_group(group);
   return FDB_OK;

@@ -136,6 +136,19 @@ end
 Base.size(J::DeviceBlockBanded) = (sum(J.blocks), sum(J.blocks))
 Base.size(J::DeviceBlockBanded, d) = sum(J.blocks)
 
+# BlockBandedMatrices.BlockBandedMatrix with square blocks, in that package's own storage: the block sizes
+# blocklengths(axes(J, 1)), the block bandwidths blockbandwidths(J) and the data vector on the device (a
+# BlockBandedMatrix{Float64} whose data is a CuVector{Float64}: the plan writes pointer(data)).  Block column J
+# is one column-major slab holding every row of the block rows in blockcolrange(J) (FDB_J_BLOCK_DENSE in the header).
+struct DeviceBlockDense
+    blocks::Vector{Int64}
+    l::Int
+    u::Int
+    data::CuVector{Float64}                  # sum over block columns of (slab height) * (block width)
+end
+Base.size(J::DeviceBlockDense) = (sum(J.blocks), sum(J.blocks))
+Base.size(J::DeviceBlockDense, d) = sum(J.blocks)
+
 struct DeviceTridiagonal                     # LinearAlgebra.Tridiagonal(dl, d, du): one buffer [dl; d; du]
     n::Int
     buf::CuVector{Float64}                   # 3n - 2
@@ -316,6 +329,24 @@ function plan_block_banded(J::DeviceBlockBanded, colorvec, fd::Cint; kw...)
     end
 end
 
+# sparsity::BlockBandedMatrix, J the same structure: ext/FiniteDiffBlockBandedMatricesExt.jl:44-68 as a closed form
+# over BlockBandedMatrices' storage (no entry lists on the host)
+function plan_block_dense(J::DeviceBlockDense, colorvec, fd::Cint; kw...)
+    key = (:block_dense, J.blocks, J.l, J.u, length(J.data), color_key(colorvec), fd, values(kw))
+    cached_plan(J.data, key) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd; kw...))
+        cptr, croot = color_arg(colorvec, size(J, 2))
+        blocks = J.blocks
+        GC.@preserve blocks croot begin
+            check(ccall((:fdb_plan_create_block_dense, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Ptr{Int64}, Int64, Int64, Int64, Ptr{Int64}, Ref{PlanOpts}),
+                h, length(blocks), pointer(blocks), J.l, J.u, length(J.data), cptr, opts))
+        end
+        Plan(h[], (blocks, croot))
+    end
+end
+
 # sparsity === nothing: dense column branch; a non-default colorvec reproduces jacobians.jl:547-557 as written
 function plan_dense(anchor, m::Integer, n::Integer, ldJ::Integer, colorvec, fd::Cint; kw...)
     key = (:dense, m, n, ldJ, color_key(colorvec), fd, values(kw))
@@ -404,7 +435,7 @@ function run_plan!(plan::Plan, jvals::CuArray{Float64}, f, x::CuVector{Float64},
     nothing                                  # jacobians.jl:652
 end
 
-const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceTridiagonal, DeviceDiagonal, DeviceBidiagonal,
+const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceBlockDense, DeviceTridiagonal, DeviceDiagonal, DeviceBidiagonal,
     CuMatrix{Float64}}
 
 ld(J::CuMatrix) = max(stride(J, 2), size(J, 1), 1)
@@ -424,6 +455,11 @@ function plan_for(J::DeviceBlockBanded, sp, colorvec, fd)
     (sp isa DeviceBlockBanded && (sp.blocks, sp.l, sp.u, sp.lam, sp.mu) == (J.blocks, J.l, J.u, J.lam, J.mu)) ||
         throw(ArgumentError("J and sparsity must have the same block structure"))
     (plan_block_banded(J, colorvec, fd), J.data)
+end
+function plan_for(J::DeviceBlockDense, sp, colorvec, fd)
+    (sp isa DeviceBlockDense && (sp.blocks, sp.l, sp.u) == (J.blocks, J.l, J.u)) ||
+        throw(ArgumentError("J and sparsity must have the same block structure"))
+    (plan_block_dense(J, colorvec, fd), J.data)
 end
 function plan_for(J::DeviceTridiagonal, sp, colorvec, fd)
     (plan_coo(() -> tridiagonal_structure(J.n), J.buf, J.n, J.n, :tridiagonal, FDB_J_SLOTS, 3 * J.n - 2, colorvec, fd), J.buf)
@@ -469,7 +505,7 @@ end
                                 relstep, absstep, colorvec, sparsity, dir)
 
 Same signature and keyword meaning as `src/jacobians.jl:504-514`.  `J` is a `DeviceCSC`, `DeviceBanded`,
-`DeviceBlockBanded`, `DeviceTridiagonal`, `DeviceDiagonal`, `DeviceBidiagonal` or a dense `CuMatrix{Float64}`; `x`,
+`DeviceBlockBanded`, `DeviceBlockDense`, `DeviceTridiagonal`, `DeviceDiagonal`, `DeviceBidiagonal` or a dense `CuMatrix{Float64}`; `x`,
 `cache.fx`, `f_in` are `CuVector{Float64}`.
 `relstep` / `absstep` left at their defaults are passed as FDB_STEP_DEFAULT; explicit values (0 included) as given.
 """
@@ -756,6 +792,19 @@ function group_block_banded(J::DeviceBlockBanded, colorvec, fdtype, devices::Vec
             (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Ptr{Int64}, Int64, Int64, Int64, Int64, Int64, Ptr{Int64}, Ref{PlanOpts}),
             h, length(devices), pointer(devices), length(blocks), pointer(blocks), J.l, J.u, J.lam, J.mu, length(J.data),
             cptr, opts))
+    end
+    Group(h[], length(devices), (blocks, croot))
+end
+
+function group_block_dense(J::DeviceBlockDense, colorvec, fdtype, devices::Vector{Cint}; kw...)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, size(J, 2))
+    blocks = J.blocks
+    GC.@preserve blocks croot devices begin
+        check(ccall((:fdb_group_create_block_dense, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Ptr{Int64}, Int64, Int64, Int64, Ptr{Int64}, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), length(blocks), pointer(blocks), J.l, J.u, length(J.data), cptr, opts))
     end
     Group(h[], length(devices), (blocks, croot))
 end

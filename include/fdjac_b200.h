@@ -59,7 +59,11 @@ typedef enum {
   FDB_J_BAND = 2,      /* J::BandedMatrix data[(l+u+1) x n], slot [u+r-c+1, c]        (ext/FiniteDiffBandedMatricesExt.jl:13-27) */
   FDB_J_SLOTS = 3,     /* structured J (e.g. Tridiagonal): explicit 1-based slot per structural entry (iteration_utils.jl:25-32) */
   FDB_J_BLOCK_BAND = 4, /* J::BandedBlockBandedMatrix band data, (l+u+1)(lam+mu+1) slots per column (fdb_plan_create_block_banded) */
-  FDB_J_DIAGONALS = 5  /* J::Diagonal / Bidiagonal / Tridiagonal storage: the stored diagonals packed in one buffer (fdb_plan_create_banded) */
+  FDB_J_DIAGONALS = 5, /* J::Diagonal / Bidiagonal / Tridiagonal storage: the stored diagonals packed in one buffer (fdb_plan_create_banded) */
+  FDB_J_BLOCK_DENSE = 6 /* J::BlockBandedMatrix data, one column-major slab per block column (fdb_plan_create_block_dense):
+                           entry (r, c) of block (K, J), 0-based, at slot start_J + c*h_J + (rowoff_J(K) + r), where
+                           h_J = sum of the sizes of block rows max(0, J-u)..min(N-1, J+l), start_J = sum_{J'<J} h_J'*cb[J']
+                           and rowoff_J(K) = the sizes of block rows max(0, J-u)..K-1 */
 } fdb_jkind;
 
 /*
@@ -151,7 +155,7 @@ double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep,
 /* ---- plans: the per-(pattern, colorvec, fdtype) state the reference rebuilds on every call
  *      (jacobians.jl:515-535: colour reshape, findstructralnz, same-pattern test) ---- */
 
-/* Which plans each call takes.  Coloured plans: fdb_plan_create_csc / _coo / _banded / _block_banded; dense plans:
+/* Which plans each call takes.  Coloured plans: fdb_plan_create_csc / _coo / _banded / _block_banded / _block_dense; dense plans:
  * fdb_plan_create_dense / _dense_colorvec; out-of-place plans: fdb_oop_plan_create_*.  Any other plan is refused with
  * FDB_ERR_INVALID (FDB_ERR_UNSUPPORTED where noted) before the call allocates, launches or calls f.
  *   fdb_jacobian, fdb_jacobian_host   coloured and dense plans, fdtype forward / central
@@ -226,6 +230,24 @@ fdb_status fdb_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t
 fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
                                         int64_t lam, int64_t mu, int64_t ldata, const int64_t *colorvec,
                                         const fdb_plan_opts *opts);
+
+/* sparsity::BlockBandedMatrix with square blocks, J the same structure: ext/FiniteDiffBlockBandedMatricesExt.jl:44-68
+ * (every row of every block in blockcolrange(J), for every column of the colour).
+ *   blocks: nblocks block sizes (Int64, host or device; the column sizes are the row sizes, as the hook takes both from
+ *   axes(Jac, 1)); n = m = sum(blocks).  (l, u) block bandwidths, >= 0 (bandwidths of nblocks or more mean nblocks).
+ *   J is BlockBandedMatrices' storage of a BlockBandedMatrix (a BlockSkylineMatrix with constant block bandwidths):
+ *   FDB_J_BLOCK_DENSE above, j_len = sum_J h_J*cb[J] slots, every one a structural entry.  ldata >= j_len doubles.
+ * Plan-time host work is O(nblocks); the plan keeps the block offsets and the slab starts on the device and reads no
+ * index stream.  Every call writes every one of the j_len slots exactly once — the quotient in columns with a valid
+ * colour, +0.0 in the others — with the values of the slot-addressed route (fdb_plan_create_coo with FDB_J_SLOTS on the
+ * hook's entry set); slots [j_len, ldata) are not touched.  For uniform blocks of size b the colouring of
+ * ArrayInterface.matrix_colors, (J mod (l+u+1))*b + j + 1 for column j of block J, is detected and then read in closed
+ * form.  opts, rank plans and fdb_plan_set_peers (FDB_ERR_UNSUPPORTED) as for fdb_plan_create_block_banded.  Negative
+ * sizes or bandwidths, ldata < j_len, a NULL blocks with nblocks > 0: FDB_ERR_INVALID; a block column of more than 2^32
+ * slots: FDB_ERR_UNSUPPORTED.  fdb_plan_info: jkind FDB_J_BLOCK_DENSE, n_entries = j_len, alg_bytes_scatter =
+ * moved_bytes_scatter = 8*j_len + 16*n*C. */
+fdb_status fdb_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                       int64_t ldata, const int64_t *colorvec, const fdb_plan_opts *opts);
 
 /* sparsity === nothing: dense column branch jacobians.jl:548-557,590-598 (colorvec = 1:n; per-component step).
  * With world>1 the columns are block-partitioned: this rank computes columns [col_begin, col_end) (0-based, see
@@ -336,6 +358,10 @@ fdb_status fdb_group_create_dense(fdb_group **group, int n_devices, const int *d
 fdb_status fdb_group_create_block_banded(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
                                          const int64_t *blocks, int64_t l, int64_t u, int64_t lam, int64_t mu, int64_t ldata,
                                          const int64_t *colorvec, const fdb_plan_opts *opts);
+/* block-dense groups: as block-banded groups, into the root's BlockBandedMatrix storage */
+fdb_status fdb_group_create_block_dense(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                        const int64_t *blocks, int64_t l, int64_t u, int64_t ldata, const int64_t *colorvec,
+                                        const fdb_plan_opts *opts);
 fdb_status fdb_group_destroy(fdb_group *group);
 fdb_status fdb_group_size(const fdb_group *group, int *n_members);
 /* member i's plan (owned by the group): fdb_plan_info / fdb_plan_counters / fdb_plan_get_eps / fdb_plan_color_owner */
