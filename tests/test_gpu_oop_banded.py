@@ -8,7 +8,11 @@ central and complex mode; dir +-1 and 0.3; step overrides; f_in; cyclic, random 
 columns and maximum(colorvec) < 1; every band type, m != n, l or u = 0, bands wider than the matrix; m = 0; candidate
 counts at the 1024-entry tile boundaries; FDB_SM_COUNT=1; batches small enough for the candidate-copy path; groups of
 1-3 members (and two GPUs when present); the refusals before any f call; the calls check_call refuses; and a sparse result
-at n = 10^7 with its plan build time."""
+at n = 10^7 with its plan build time.
+
+The last section holds the band route to oop_oracle/ directly, with an f whose dependence is exactly the band, and dense
+results to the analytic derivative.  Results past 2^31 entries are not taken: the sparse result alone needs 16 bytes
+per entry and, with the f slabs, more than 60 GB."""
 import ctypes as C
 import time
 
@@ -367,3 +371,292 @@ def test_ten_million_columns(pkg):
     assert torch.equal(res[0].colptr, res[1].colptr) and torch.equal(res[0].rowval, res[1].rowval)
     assert torch.equal(res[0].nzval.view(torch.int64), res[1].nzval.view(torch.int64))
 
+
+
+# ------------------------------------------------------------------------------------------------ held to oop_oracle
+# The comparisons above hold the band route to the CSC route, with an f whose dependence is not the band.  Here f is the
+# ELL rows function of test_gpu_oop_random.py built so that row r reads exactly the band columns max(0, r-l) ..
+# min(n-1, r+u), in random order, with coefficients in +-[0.5, 2] of which about one in ten is exactly 0: those entries'
+# quotients are exactly +-0 (-0.0 with dir = -1), dropped from a sparse result and +0.0 in a dense one.  Each case runs
+# the band sparsity object on the device through run_csc and the restatement oop_oracle/ on the CSC of the band's entry
+# set, bit for bit, with the same f calls; dense results are also held to the analytic derivative.
+import test_gpu_oop_random as OR  # noqa: E402
+from test_gpu_structured_fill import analytic_tolerance, ell_derivative  # noqa: E402
+
+
+def band_entries(m, n, l, u):
+    """(rows, cols), 0-based, of the band's entries in storage order (column-major, rows ascending)"""
+    cols = [np.arange(max(0, c - u), min(m - 1, c + l) + 1, dtype=np.int64) for c in range(n)]
+    r = np.concatenate(cols) if cols else np.zeros(0, np.int64)
+    c = np.repeat(np.arange(n, dtype=np.int64), [len(v) for v in cols])
+    return r, c
+
+
+def band_cp_rv(m, n, l, u):
+    r, c = band_entries(m, n, l, u)
+    cp = np.concatenate([[0], np.cumsum(np.bincount(c, minlength=n))]).astype(np.int64) + 1
+    return cp, r + 1
+
+
+def band_ell(m, n, l, u, seed, zero_share=0.1):
+    """row r reads exactly the band columns of row r in random order; coefficients +-[0.5, 2], about zero_share of them
+    exactly 0 (padding repeats the row's first column with coefficient 0)"""
+    rng = np.random.default_rng(seed)
+    # row r of a band holds the columns c with r - l <= c <= r + u
+    rows = [np.arange(max(0, r - l), min(n - 1, r + u) + 1) for r in range(m)]
+    assert all(len(v) for v in rows), "a row without a band column"
+    K = max(len(v) for v in rows)
+    cols = np.zeros((K, m), np.int64)
+    coef = np.zeros((K, m))
+    for r, v in enumerate(rows):
+        v = rng.permutation(v)
+        cols[:, r] = v[0]
+        cols[:len(v), r] = v
+        a = rng.uniform(0.5, 2.0, len(v)) * np.where(rng.random(len(v)) < 0.5, -1.0, 1.0)
+        a[rng.random(len(v)) < zero_share] = 0.0
+        coef[:len(v), r] = a
+    return OR.Ell(cols, coef)
+
+
+def check_band_dense(J, ell, x, cv, eps, fd, m, n, l, u, what):
+    """Every element outside the band, and every band entry of a column without a valid colour, is +0.0 by bit pattern;
+    every band entry of a coloured column is within the analytic tolerance of d f_r / d x_c (valid colourings only)."""
+    J = np.asarray(J)
+    assert J.shape == (m, n), what
+    r, c = band_entries(m, n, l, u)
+    inside = np.zeros((m, n), bool)
+    inside[r, c] = True
+    assert np.all(J[~inside].view(np.uint64) == 0), f"{what}: an element outside the band is not +0.0"
+    k = cv[c] - 1
+    live = k >= 0
+    assert np.all(J[r[~live], c[~live]].view(np.uint64) == 0), f"{what}: a column without a colour is not +0.0"
+    r, c, k = r[live], c[live], k[live]
+    d, S, T = ell_derivative(ell.cols.astype(np.int64), ell.coef, r, c, x)
+    tol = analytic_tolerance(fd, None if fd == "complex" else np.asarray(eps)[k], S, T, ell.K)
+    v = J[r, c]
+    bad = np.flatnonzero(~(np.abs(v - d) <= tol))
+    assert bad.size == 0, (f"{what}: {bad.size} band entries off the derivative; first ({r[bad[0]]}, {c[bad[0]]}): "
+                           f"{v[bad[0]]!r} vs {d[bad[0]]!r}")
+    assert np.all(J[r, c][d == 0].view(np.uint64) == 0), f"{what}: a zero derivative is not +0.0"
+
+
+def band_x(n, seed):
+    rng = np.random.default_rng(seed)
+    return rng.uniform(0.5, 1.5, n) * np.where(rng.random(n) < 0.5, -1.0, 1.0)
+
+
+def run_band(pkg, oracle, sp, m, n, l, u, cv, *, fd="forward", sparse=True, seed=0, analytic=True, nan=False, what="",
+             **kw):
+    """run_csc with the band object on the device and the CSC of its entries in the restatement; the dense result's
+    analytic check (only for valid colourings, and x without NaN; nan: one NaN component, kept by the compaction)"""
+    ell = kw.pop("ell", None) or band_ell(m, n, l, u, seed)
+    x = band_x(n, seed + 1)
+    if nan:
+        x[n // 2] = np.nan
+        analytic = False
+    cp, rv = band_cp_rv(m, n, l, u)
+    res, plan = OR.run_csc(pkg, oracle, ell, x, cp, rv, cv, fd=fd, sparse=sparse, band=sp, what=what, **kw)
+    assert plan is None or plan.info()["n_entries"] == len(rv), what
+    if res is not None and not sparse and analytic and kw.get("steps", (None, None)) == (None, None):
+        eps = None if fd == "complex" else plan.eps()
+        check_band_dense(res.cpu().numpy(), ell, x, cv, eps, fd, m, n, l, u, what)
+    return res, plan, ell, x
+
+
+def _oracle_types(pkg, n):
+    """(name, band object, m, l, u): every row of each holds at least one band column"""
+    return [
+        ("banded 2,1", pkg.BandedMatrix(n, n, 2, 1), n, 2, 1),
+        ("banded m > n", pkg.BandedMatrix(n + 3, n, 3, 1), n + 3, 3, 1),
+        ("banded m < n", pkg.BandedMatrix(n - 4, n, 0, 2), n - 4, 0, 2),
+        ("banded l = 0", pkg.BandedMatrix(n, n, 0, 3), n, 0, 3),
+        ("banded u = 0", pkg.BandedMatrix(n, n, 4, 0), n, 4, 0),
+        ("banded wider than the matrix", pkg.BandedMatrix(n, n, n + 3, 2 * n), n, n + 3, 2 * n),
+        ("diagonal", pkg.Diagonal(n), n, 0, 0),
+        ("bidiagonal U", pkg.Bidiagonal(n, "U"), n, 0, 1),
+        ("bidiagonal L", pkg.Bidiagonal(n, "L"), n, 1, 0),
+        ("symtridiagonal", pkg.SymTridiagonal(n), n, 1, 1),
+    ]
+
+
+@pytest.mark.parametrize("fd", ["forward", "central", "complex"])
+@pytest.mark.parametrize("sparse", [False, True], ids=["dense", "sparse"])
+def test_band_types_against_the_oracle(pkg, oracle, fd, sparse):
+    for n in (5, 37, 130):
+        for name, sp, m, l, u in _oracle_types(pkg, n):
+            cv = _valid_cv(n, l, u, m)
+            what = f"{name} n={n} {fd} sparse={sparse}"
+            res, _, ell, x = run_band(pkg, oracle, sp, m, n, l, u, cv, fd=fd, sparse=sparse, seed=n, what=what)
+            if not sparse:
+                # the dense prototype takes the same values
+                xd = torch.from_numpy(x).cuda()
+                f, _ = ell.native(pkg, fd == "complex")
+                proto = torch.full((n, m), float("nan"), dtype=torch.float64, device="cuda").t()
+                cache = pkg.JacobianCache(xd, torch.zeros(m, dtype=torch.float64, device="cuda"), fd)
+                got = pkg.finite_difference_jacobian(f, xd, cache, colorvec=cv, sparsity=sp, jac_prototype=proto)
+                torch.cuda.synchronize()
+                assert_same_bits(got.cpu().numpy(), res.cpu().numpy(), f"{what}: dense prototype")
+
+
+BAND_OPTIONS = [("dir+", dict(dir=1.0)), ("dir-", dict(dir=-1.0)), ("steps", dict(steps=(1e-5, 1e-9))),
+                ("abs0", dict(steps=(None, 0.0))), ("f_in", dict(f_in=True)), ("f_in dir-", dict(f_in=True, dir=-1.0)),
+                ("nan", dict(nan=True))]
+
+
+@pytest.mark.parametrize("opt", BAND_OPTIONS, ids=[o[0] for o in BAND_OPTIONS])
+@pytest.mark.parametrize("fd", ["forward", "central"])
+@pytest.mark.parametrize("sparse", [False, True], ids=["dense", "sparse"])
+def test_band_options_against_the_oracle(pkg, oracle, opt, fd, sparse):
+    name, kw = opt
+    if kw.get("f_in") and fd != "forward":
+        pytest.skip("f_in is the forward mode's f(x)")
+    n, m, l, u = 300, 290, 4, 3
+    cv = _valid_cv(n, l, u, m)
+    cv[::11] = 0
+    res, plan, ell, x = run_band(pkg, oracle, pkg.BandedMatrix(m, n, l, u), m, n, l, u, cv, fd=fd, sparse=sparse,
+                                 seed=17, what=f"{name} {fd} sparse={sparse}", **kw)
+    if sparse:
+        # the exact zeros (zero coefficients, columns without a colour) are dropped; NaN quotients are kept
+        assert res.nnz < len(band_entries(m, n, l, u)[0]), name
+        if kw.get("nan"):
+            assert np.isnan(res.nzval.cpu().numpy()).any(), name
+
+
+def _cyclic_many():
+    n, l, u = 3000, 700, 400
+    cv = _valid_cv(n, l, u, n)
+    assert cv.max() == 1101
+    return n, l, u, cv
+
+
+@pytest.mark.parametrize("fd", ["forward", "central", "complex"])
+def test_band_many_colours(pkg, oracle, fd):
+    """1101 cyclic colours (the closed form) and their relabelling (a 16-bit table), sparse against the restatement;
+    the dense result equals the sparse one scattered into +0.0 and meets the analytic check"""
+    n, l, u, cv = _cyclic_many()
+    ell = band_ell(n, n, l, u, 81)
+    sp = pkg.BandedMatrix(n, n, l, u)
+    for cvname, c in (("cyclic", cv), ("relabelled", 1102 - cv))[:2 if fd == "forward" else 1]:
+        what = f"C=1101 {cvname} {fd}"
+        res, plan, _, x = run_band(pkg, oracle, sp, n, n, l, u, c, fd=fd, sparse=True, seed=81, ell=ell, max_batch=4,
+                                   record=False, native_twin=True, what=what)
+        info = plan.info()
+        assert info["n_colors"] == 1101 and info["color_bits"] == 16, info
+        xd = torch.from_numpy(x).cuda()
+        f, _ = ell.native(pkg, fd == "complex")
+        cache = pkg.JacobianCache(xd, torch.zeros(n, dtype=torch.float64, device="cuda"), fd, max_batch=4)
+        J = pkg.finite_difference_jacobian(f, xd, cache, colorvec=c, sparsity=sp)
+        torch.cuda.synchronize()
+        h = _host_sparse(res)
+        want = np.zeros((n, n))
+        want[h[0], h[1]] = 0.0 + h[2]
+        assert_same_bits(J.cpu().numpy(), want, f"{what}: dense vs sparse")
+        check_band_dense(J.cpu().numpy(), ell, x, c, None if fd == "complex" else cache._last_plan.eps(), fd, n, n, l, u,
+                         what)
+
+
+def test_band_many_colours_identity(pkg, oracle):
+    """the identity colouring past 1024 colours, sparse result, on a narrow band (f runs once per column)"""
+    n, m, l, u = 1100, 1103, 3, 2
+    _, plan, _, _ = run_band(pkg, oracle, pkg.BandedMatrix(m, n, l, u), m, n, l, u, np.arange(1, n + 1), seed=83,
+                             max_batch=8, record=False, native_twin=True, what="identity n=1100")
+    assert plan.info()["n_colors"] == 1100 and plan.info()["color_bits"] == 16
+
+
+def _host_sparse(res):
+    cp = res.colptr.cpu().numpy()
+    cols = np.repeat(np.arange(len(cp) - 1), np.diff(cp))
+    return res.rowval.cpu().numpy() - 1, cols, res.nzval.cpu().numpy()
+
+
+@pytest.mark.parametrize("spread", [300, 70_000], ids=["16bit", "32bit"])
+@pytest.mark.parametrize("sparse", [False, True], ids=["dense", "sparse"])
+def test_band_wide_colour_tables(pkg, oracle, spread, sparse):
+    """colour ids spread to 300 or 70 000 (a valid colouring stays valid, so the dense result takes them too)"""
+    n, m, l, u = 60, 64, 4, 2
+    rng = np.random.default_rng(spread)
+    cv = _valid_cv(n, l, u, m)
+    cv[rng.random(n) < 0.1] = 0
+    cv = OR.spread_ids(cv, spread, rng)
+    assert cv.max() == spread
+    for fd in ("forward", "central"):
+        _, plan, _, _ = run_band(pkg, oracle, pkg.BandedMatrix(m, n, l, u), m, n, l, u, cv, fd=fd, sparse=sparse,
+                                 seed=spread, max_batch=8, record=False, native_twin=True,
+                                 dir=-1.0 if fd == "forward" else 1.0, what=f"spread {spread} {fd} sparse={sparse}")
+        assert plan.info()["color_bits"] == (16 if spread == 300 else 32)
+
+
+@pytest.mark.parametrize("fd", ["forward", "central", "complex"])
+def test_band_candidate_copy_against_the_oracle(pkg, oracle, fd):
+    n = 2000
+    for l, u in ((1, 1), (40, 33)):
+        cv = _valid_cv(n, l, u, n)
+        _, plan, _, _ = run_band(pkg, oracle, pkg.BandedMatrix(n, n, l, u), n, n, l, u, cv, fd=fd, seed=l,
+                                 max_batch=1, scratch=1, record=False, native_twin=True, what=f"copy l={l} u={u} {fd}")
+        assert plan.info()["n_groups"] > 1
+
+
+def band_tile_shapes():
+    """(E, m, n, l, u): band shapes with m != n, both bandwidths clipped at the matrix edges (head and tail columns of
+    varying length), and E candidates at and around the 1024-entry tile boundaries"""
+    def count(m, n, l, u):
+        c = np.arange(n)
+        return int(np.maximum(np.minimum(m - 1, c + l) - np.maximum(0, c - u) + 1, 0).sum())
+
+    out = []
+    for E in (1023, 1024, 1025, 2047, 2049):
+        found = next(((E, m, n, l, u) for n in range(60, 400) for d in (5, -3, 2, -1) for l in range(5, 16)
+                      for u in range(3, 16) for m in (n + d,) if count(m, n, l, u) == E), None)
+        assert found, E
+        out.append(found)
+    return out
+
+
+BAND_TILES = band_tile_shapes()
+
+
+@pytest.mark.parametrize("shape", BAND_TILES, ids=[f"E{s[0]}" for s in BAND_TILES])
+@pytest.mark.parametrize("sm", [None, 1])
+def test_band_tiles_against_the_oracle(pkg, oracle, shape, sm):
+    E, m, n, l, u = shape
+    cv = _valid_cv(n, l, u, m)
+    for fd in ("forward", "central"):
+        for sparse in (True, False):
+            _, plan, _, _ = run_band(pkg, oracle, pkg.BandedMatrix(m, n, l, u), m, n, l, u, cv, fd=fd, sparse=sparse,
+                                     seed=E, sm=sm, dir=-1.0, what=f"E={E} sm={sm} {fd} sparse={sparse}")
+            assert plan.info()["n_entries"] == E
+
+
+def _group_sets():
+    sets = [[0, 0], [0, 0, 0]]
+    if torch.cuda.is_available() and torch.cuda.device_count() >= 2:
+        sets.append([0, 1])
+    return sets
+
+
+@pytest.mark.parametrize("devs", _group_sets(), ids=lambda d: "-".join(map(str, d)))
+@pytest.mark.parametrize("sparse", [False, True], ids=["dense", "sparse"])
+def test_band_groups_against_the_oracle(pkg, oracle, fdist, devs, sparse):
+    """GroupJacobianOOP with colour-less columns: the group result is the one-device result, which is the restatement's"""
+    n, m, l, u = 400, 405, 6, 3
+    cv = _valid_cv(n, l, u, m)
+    cv[::7] = 0
+    sp = pkg.BandedMatrix(m, n, l, u)
+    for fd in ("forward", "central"):
+        for partition in (0, 1):
+            what = f"group {devs} {fd} sparse={sparse} partition={partition}"
+            single, plan, ell, x = run_band(pkg, oracle, sp, m, n, l, u, cv, fd=fd, sparse=sparse, seed=91,
+                                            record=False, what=what)
+            xd = torch.from_numpy(x).cuda(devs[0])
+            proto = sparse_proto(pkg, m, n) if sparse else None
+            with torch.cuda.device(devs[0]):
+                g = fdist.GroupJacobianOOP(devs, fd, colorvec=cv, sparsity=sp, jac_prototype=proto, partition=partition)
+                members = [ell.native(pkg, device=f"cuda:{d}") for d in devs]
+                try:
+                    res = g.run([f for f, _ in members], xd)
+                    torch.cuda.synchronize()
+                finally:
+                    g.close()
+            assert_same_tuple(host(res), host(single), f"{what}: against one device")
+            Cn = int(cv.max())
+            assert sum(ctx.calls for _, ctx in members) == (2 * Cn if fd == "central" else Cn + 1), what

@@ -158,10 +158,11 @@ def make_x(rng, n, nan=False):
 
 # ------------------------------------------------------------------------------------------------ one coloured case
 def run_csc(pkg, oracle, ell, x, cp, rv, cv, *, fd="forward", sparse=True, dir=1.0, steps=(None, None), f_in=False,
-            max_batch=1, scratch=0, sm=None, record=True, native_twin=False, what=""):
+            max_batch=1, scratch=0, sm=None, record=True, native_twin=False, band=None, what=""):
     """The device's finite_difference_jacobian(f, x, cache, f_in; sparsity, colorvec[, jac_prototype]) with the native
     ELL function, compared with the restatement; returns (device result, plan).  An invalid colouring with a dense result
-    must raise on both sides."""
+    must raise on both sides.  band: a band sparsity object (BandedMatrix, Diagonal, ...) handed to the device instead of
+    the CSC (cp, rv), which must then be the CSC of its entry set; the restatement still receives (cp, rv)."""
     m, n = ell.m, len(x)
     complex_ = fd == "complex"
     f, ctx = ell.native(pkg, complex_)
@@ -169,7 +170,7 @@ def run_csc(pkg, oracle, ell, x, cp, rv, cv, *, fd="forward", sparse=True, dir=1
     x_before = xd.clone()
     S = pkg.SparseMatrixCSC(m, n, torch.from_numpy(cp), torch.from_numpy(rv),
                             torch.zeros(len(rv), dtype=torch.float64, device="cuda"))
-    tk = {"sparsity": S, "colorvec": cv}
+    tk = {"sparsity": S if band is None else band, "colorvec": cv}
     lk = {"sparsity": (m, n, cp, rv), "colorvec": cv}
     if sparse:
         tk["jac_prototype"] = S

@@ -1,5 +1,6 @@
-"""Block-banded (FDB_J_BLOCK_BAND) and diagonal-storage (FDB_J_DIAGONALS) Jacobians held to an f whose Jacobian fills
-the target's structure with distinct values.
+"""Block-banded (FDB_J_BLOCK_BAND), diagonal-storage (FDB_J_DIAGONALS) and block-dense (FDB_J_BLOCK_DENSE, a
+BlockBandedMatrix in its own storage) Jacobians held to an f whose Jacobian fills the target's structure with distinct
+values.
 
 The native tridiagonal and 5-point f's of the other files have constant coefficients: most structural slots of a
 block-banded target hold exactly +0.0 there, and the sub- and super-diagonal of diagonal storage hold the same value,
@@ -15,11 +16,13 @@ Every case checks four things on a NaN-prefilled buffer:
     in float64 from the coefficients (only for colourings that are valid for the structure), and none is exactly 0;
   * every slot outside the structure, and every slot of a column without a valid colour, is +0.0 by bit pattern;
 with the f call counts equal and x unchanged.  The slot of each (row, column) comes from decoders written from the
-documented storage layouts (block_band_entries, diagonal_entries), not from the mirror's findstructralnz.
+documented storage layouts (block_band_entries, diagonal_entries, block_dense_entries), not from the mirror's
+findstructralnz.  Block-dense storage also has every slot structural, so the COO route and the oracle cover all of J.
 
 IEEE edges (signed zeros, NaN / +-Inf in x, x near the ends of the fp64 range) are held to the COO route and the
-oracle only.  Slot offsets past 2^31 are taken by the block-banded kind (test_block_band_past_2_31, about 17 GB; it
-skips on a device with less free memory).  The diagonal kind is not taken past 2^31: its storage would need n of 7e8
+oracle only.  Slot offsets past 2^31 are taken by the block-banded kind (test_block_band_past_2_31, about 17 GB) and
+the block-dense kind (test_block_dense_past_2_31: one slab past 2^31, and slab starts past 2^31; about 20 GB each); they
+skip on a device with less free memory.  The diagonal kind is not taken past 2^31: its storage would need n of 7e8
 to 1e9 and, with the f slabs, more than 40 GB."""
 import ctypes as C
 
@@ -81,6 +84,31 @@ def block_band_entries(rb, l, u, lam, mu, dense_blocks=False):
                 slots.append(c * w + (K - J + u) * sw + (mu + k - jj))
     cat = lambda a: np.concatenate(a).astype(np.int64) if a else np.zeros(0, np.int64)
     return cat(rows), cat(cols), cat(slots), w * int(off[-1])
+
+
+def block_dense_entries(rb, l, u):
+    """(rows, cols, slots, length), 0-based, of a BlockBandedMatrix in BlockBandedMatrices' own storage, from the slot
+    formula of FDB_J_BLOCK_DENSE in include/fdjac_b200.h: entry (r, c) of block (K, J) sits at slot
+    start_J + c h_J + (rowoff_J(K) + r), with h_J the rows of block rows max(0, J-u)..min(N-1, J+l),
+    start_J = sum_{J'<J} h_J' cb[J'] and rowoff_J(K) the rows of block rows max(0, J-u)..K-1."""
+    off = np.concatenate([[0], np.cumsum(rb)]).astype(np.int64)
+    N = len(rb)
+    rows, cols, slots = [], [], []
+    start = 0
+    for J in range(N):
+        krange = range(max(0, J - u), min(N - 1, J + l) + 1)
+        h = sum(rb[K] for K in krange)
+        c = np.arange(rb[J], dtype=np.int64)
+        rowoff = 0
+        for K in krange:
+            r = np.arange(rb[K], dtype=np.int64)
+            rows.append(np.broadcast_to(off[K] + r, (len(c), len(r))).ravel())
+            cols.append(np.repeat(off[J] + c, len(r)))
+            slots.append((start + c[:, None] * h + rowoff + r[None, :]).ravel())
+            rowoff += rb[K]
+        start += h * rb[J]
+    cat = lambda a: np.concatenate(a).astype(np.int64) if a else np.zeros(0, np.int64)
+    return cat(rows), cat(cols), cat(slots), int(start)
 
 
 def diagonal_entries(kind, n):
@@ -147,16 +175,26 @@ class Ell:
         return s + 0.1 * (x0 * x0)
 
     def derivative(self, rows, cols, x):
-        """(d f_r / d x_c, S_r = sum of |terms| of row r, T_r = sum |coef| + 0.2 |x0|) at the entries (rows, cols)."""
-        n, K = self.n, self.K
-        coef = np.zeros(len(rows))
-        for p in range(K):
-            coef += np.where(self.cols[p, rows] == cols, self.coef[p, rows], 0.0)
-        x0 = x[self.cols[0, rows]]
-        d = coef + np.where(self.cols[0, rows] == cols, 0.2 * x0, 0.0)
-        terms = np.abs(self.coef * x[self.cols]).sum(axis=0) + 0.1 * x[self.cols[0]] ** 2
-        T = np.abs(self.coef).sum(axis=0) + 0.2 * np.abs(x[self.cols[0]])
-        return d, terms[rows], T[rows]
+        return ell_derivative(self.cols, self.coef, rows, cols, x)
+
+
+def ell_derivative(ecols, ecoef, rows, cols, x):
+    """For the ELL rows f (ecols, ecoef: [K][m], each column listed at most once per row with a nonzero coefficient):
+    (d f_r / d x_c, S_r = sum of |terms| of row r, T_r = sum |coef| + 0.2 |x0|) at the entries (rows, cols)."""
+    K, m = ecols.shape
+    n = len(x)
+    nz = ecoef != 0.0
+    key = np.broadcast_to(np.arange(m, dtype=np.int64), (K, m))[nz] * n + ecols[nz]
+    o = np.argsort(key, kind="stable")
+    key, val = key[o], ecoef[nz][o]
+    q = np.asarray(rows, np.int64) * n + cols
+    i = np.minimum(np.searchsorted(key, q), max(len(key) - 1, 0))
+    coef = np.where(key[i] == q, val[i], 0.0) if len(key) else np.zeros(len(rows))
+    x0 = x[ecols[0, rows]]
+    d = coef + np.where(ecols[0, rows] == cols, 0.2 * x0, 0.0)
+    terms = np.abs(ecoef * x[ecols]).sum(axis=0) + 0.1 * x[ecols[0]] ** 2
+    T = np.abs(ecoef).sum(axis=0) + 0.2 * np.abs(x[ecols[0]])
+    return d, terms[rows], T[rows]
 
 
 def analytic_tolerance(fdtype, eps, S, T, K):
@@ -690,6 +728,311 @@ def test_diagonal_group(pkg, api, fdist, devices, partition):
                 gj.close()
 
 
+# ------------------------------------------------------------------------------------------------ block-dense storage
+def bd_target(pkg, s, device=DEV):
+    rb, l, u = s
+    B = pkg.BlockSkylineMatrix(rb, rb, (l, u), device=device)
+    B.data.fill_(NAN)
+    return B
+
+
+def bd_run(pkg, api, s, st, ell, x, fdtype, cv, coo, f=None, f_in=None, run_kw=None, plan_kw=None, env=None):
+    """One Jacobian into a NaN-filled BlockSkylineMatrix, J and sparsity through the mirror: the block-dense plan, or
+    (coo=True) the slot-addressed COO plan on the decoder's entry list and the same buffer."""
+    B = bd_target(pkg, s)
+    ctx = None
+    if f is None:
+        f, ctx = ell.native(pkg, fdtype == "complex")
+    L = pkg._lib
+    plan_kw = plan_kw or {}
+    with fdb_env(**(env or {})):
+        cache = pkg.JacobianCache(x, fdtype, colorvec=cv, sparsity=B, **plan_kw)
+        if coo:
+            plan = _plan(pkg, api, B, B.n, 0, 0, L.FDB_J_SLOTS, st[3], cv, fdtype, plan_kw, st[0], st[1], st[2])
+            cache.plan_for = lambda *a: plan
+        pkg.finite_difference_jacobian_(B, f, x, cache, f_in, **(run_kw or {}))
+    torch.cuda.synchronize()
+    plan = cache._last_plan
+    info = plan.info()
+    assert info["jkind"] == (L.FDB_J_SLOTS if coo else L.FDB_J_BLOCK_DENSE)
+    assert info["j_len"] == st[3]
+    return B.data.cpu().numpy(), (ctx.calls if ctx is not None else None), plan
+
+
+def bd_case(pkg, api, oracle, s, fdtype, cv, valid, what, seed=0, run_kw=None, plan_kw=None, f_in=False, env=None,
+            ell=None, x_np=None, st=None):
+    rb, l, u = s
+    st = st or block_dense_entries(rb, l, u)
+    n = sum(rb)
+    ell = ell or Ell(n, st[0], st[1], seed)
+    x_np = host_x(n, seed + 1) if x_np is None else x_np
+    x = torch.from_numpy(x_np).to(DEV)
+    fin = torch.from_numpy(f_in_of(ell, x_np)).to(DEV) if f_in else None
+    out = {}
+    for coo in (False, True):
+        out[coo] = bd_run(pkg, api, s, st, ell, x, fdtype, cv, coo, f_in=fin, run_kw=run_kw, plan_kw=plan_kw, env=env)
+    assert_same_bits(x, x_np, f"{what}: x changed")
+    got, calls, plan = out[False]
+    assert_same_bits(got, out[True][0], f"{what}: vs COO route", allow_nan=False)
+    assert calls == out[True][1], what
+    kw = dict(run_kw or {}, **(plan_kw or {}))
+    eps = plan.eps()
+    ref, fcalls = oracle_run(oracle, st, n, ell, x_np, fdtype, cv, eps, kw, None if fin is None else fin.cpu().numpy(),
+                             False)
+    assert_same_bits(got, ref, f"{what}: vs oracle")
+    assert fcalls == calls, what
+    check_values(got, st, ell, x_np, cv, eps, fdtype, valid, what)
+    return got, plan
+
+
+# (name, (rb, l, u)): empty blocks leading, interior, trailing and all but one; l != u; bandwidths of nblocks or more;
+# uniform size-1 blocks (a tile spans hundreds of block columns: the unstaged search); uniform blocks (the closed form);
+# blocks spanning many 1024-slot tiles
+BD_STRUCTS = [
+    ("empty_lead", ([0, 0, 3, 5, 2, 4], 1, 1)),
+    ("empty_inner", ([4, 0, 0, 3, 6, 0, 5, 2], 2, 1)),
+    ("empty_trail", ([3, 5, 4, 0, 0], 1, 2)),
+    ("empty_but_one", ([0, 0, 7, 0, 0, 0], 2, 2)),
+    ("l_ne_u", ([3, 5, 2, 4, 6, 1, 3], 1, 3)),
+    ("wide_bands", ([3, 2, 4, 1, 5], 5, 7)),
+    ("size1", ([1] * 700, 1, 1)),
+    ("size1_w0", ([1] * 900, 0, 0)),
+    ("uniform6", ([6] * 40, 1, 1)),
+    ("big_blocks", ([300, 250, 0, 280], 1, 0)),
+]
+
+
+@pytest.mark.parametrize("name", [s[0] for s in BD_STRUCTS])
+@pytest.mark.parametrize("fdtype", ["forward", "central", "complex"])
+def test_block_dense_structures(pkg, api, oracle, name, fdtype):
+    s = dict(BD_STRUCTS)[name]
+    rb, l, u = s
+    st = block_dense_entries(rb, l, u)
+    n = sum(rb)
+    rng = np.random.default_rng(len(name) * 7 + FD[fdtype])
+    closed = bd_target(pkg, s, "cpu").matrix_colors()
+    ell = Ell(n, st[0], st[1], 13)
+    x_np = host_x(n, 14)
+    res = {}
+    for cvname, (cv, valid) in colorings(closed, n, st[0], st[1], rng, identity=n <= 1000).items():
+        res[cvname], plan = bd_case(pkg, api, oracle, s, fdtype, cv, valid, f"{name} {fdtype} {cvname}", ell=ell,
+                                    x_np=x_np, st=st)
+    assert_same_bits(res["relabelled"], res["matrix_colors"], f"{name} {fdtype}: relabelled vs closed form")
+
+
+@pytest.mark.parametrize("opt", BB_OPTIONS, ids=[o[0] for o in BB_OPTIONS])
+@pytest.mark.parametrize("fdtype", ["forward", "central"])
+def test_block_dense_options(pkg, api, oracle, opt, fdtype):
+    name, run_kw, plan_kw, f_in = opt
+    if f_in and fdtype != "forward":
+        pytest.skip("f_in is the forward mode's f(x)")
+    for sname in ("empty_inner", "uniform6"):
+        s = dict(BD_STRUCTS)[sname]
+        n = sum(s[0])
+        pk = dict(plan_kw)
+        if pk.get("scratch_bytes") == "2slabs":
+            pk["scratch_bytes"] = 8 * ((n + 1) & ~1) * 2
+        st = block_dense_entries(*s)
+        closed = bd_target(pkg, s, "cpu").matrix_colors()
+        for cvname, cv in (("matrix_colors", closed), ("relabelled", relabel(closed)),
+                           ("random", greedy_coloring(n, st[0], st[1], np.random.default_rng(3)))):
+            _, plan = bd_case(pkg, api, oracle, s, fdtype, cv, True, f"{sname} {fdtype} {name} {cvname}", seed=5,
+                              run_kw=run_kw, plan_kw=pk, f_in=f_in, st=st)
+            if name == "few_slabs" and int(cv.max()) > 2:
+                assert plan.info()["n_groups"] > 1
+
+
+@pytest.mark.parametrize("use_graph", [False, True])
+def test_block_dense_reused_plan(pkg, api, oracle, use_graph):
+    """One cache, x changed in place between Jacobians: the plan is reused (with use_graph, the graph is replayed)."""
+    s = dict(BD_STRUCTS)["empty_inner"]
+    st = block_dense_entries(*s)
+    n = sum(s[0])
+    ell = Ell(n, st[0], st[1], 43)
+    for cv in (bd_target(pkg, s, "cpu").matrix_colors(), greedy_coloring(n, st[0], st[1], np.random.default_rng(4))):
+        x = torch.empty(n, dtype=torch.float64, device=DEV)
+        B = bd_target(pkg, s)
+        f, ctx = ell.native(pkg)
+        cache = pkg.JacobianCache(x, "forward", colorvec=cv, sparsity=B, use_graph=use_graph)
+        plans = set()
+        for seed in (1, 2, 3):
+            x_np = host_x(n, seed)
+            x.copy_(torch.from_numpy(x_np))
+            B.data.fill_(NAN)
+            pkg.finite_difference_jacobian_(B, f, x, cache)
+            torch.cuda.synchronize()
+            got = B.data.cpu().numpy()
+            plans.add(id(cache._last_plan))
+            eps = cache._last_plan.eps()
+            ref, _ = oracle_run(oracle, st, n, ell, x_np, "forward", cv, eps, {}, None, False)
+            assert_same_bits(got, ref, f"reused {seed} graph={use_graph}", allow_nan=False)
+            check_values(got, st, ell, x_np, cv, eps, "forward", True, f"reused {seed}")
+        assert len(plans) == 1 and cache._last_plan.counters()["jacobians"] == 3
+        # a replayed graph does not call back into the host: the f! launches were captured with the first Jacobian
+        assert ctx.calls == (1 if use_graph else 3) * (1 + int(cv.max()))
+
+
+# uniform blocks of 400, l = u = 1: the closed form with 1200 colours (16-bit); the identity colouring on 1100 size-1
+# blocks; both past kSmemTable = 1024, so the scatter reads the step sizes and the group slots from global memory
+BD_MANY = [("closed_1200", ([400] * 3, 1, 1)), ("identity_1100", ([1] * 1100, 1, 1))]
+
+
+@pytest.mark.parametrize("case", BD_MANY, ids=[c[0] for c in BD_MANY])
+@pytest.mark.parametrize("fdtype", ["forward", "central", "complex"])
+def test_block_dense_many_colours(pkg, api, oracle, case, fdtype):
+    name, s = case
+    st = block_dense_entries(*s)
+    n = sum(s[0])
+    ell = Ell(n, st[0], st[1], 61)
+    x_np = host_x(n, 62)
+    closed = bd_target(pkg, s, "cpu").matrix_colors()
+    ident = np.arange(1, n + 1, dtype=np.int64)
+    cvs = [("matrix_colors", closed)] if name.startswith("closed") else [("identity", ident)]
+    if name.startswith("closed") and fdtype == "forward":
+        cvs.append(("relabelled", relabel(closed)))
+    res = {}
+    for cvname, cv in cvs:
+        res[cvname], plan = bd_case(pkg, api, oracle, s, fdtype, cv, True, f"{name} {fdtype} {cvname}", ell=ell,
+                                    x_np=x_np, st=st)
+        info = plan.info()
+        assert info["n_colors"] > 1024 and info["color_bits"] == 16, info
+    if "relabelled" in res:
+        assert_same_bits(res["relabelled"], res["matrix_colors"], f"{name} {fdtype}: relabelled vs closed form")
+    if fdtype == "forward":
+        # one f output per group: several launches, each with its own (l0, G) window over the global tables
+        for cvname, cv in cvs[:1]:
+            _, plan = bd_case(pkg, api, oracle, s, fdtype, cv, True, f"{name} groups {cvname}", ell=ell, x_np=x_np,
+                              st=st, plan_kw={"max_batch": 1, "scratch_bytes": 8 * ((n + 1) & ~1) * 300})
+            assert plan.info()["n_groups"] > 1
+
+
+@pytest.mark.parametrize("spread", [300, 70_000], ids=["16bit", "32bit"])
+def test_block_dense_wide_colour_tables(pkg, api, oracle, spread):
+    """Colour labels spread so that maximum(colorvec) needs a 16- or 32-bit table; small n (f runs once per label)."""
+    s = ([3, 0, 4, 2], 1, 1)
+    st = block_dense_entries(*s)
+    n = sum(s[0])
+    cv = greedy_coloring(n, st[0], st[1], np.random.default_rng(4)) * spread
+    cv[2] = -1
+    for fdtype in ("forward", "central") if spread < 65536 else ("forward",):
+        _, plan = bd_case(pkg, api, oracle, s, fdtype, cv, True, f"spread {spread} {fdtype}", seed=33, st=st)
+        assert plan.info()["color_bits"] == (16 if spread == 300 else 32)
+
+
+def bd_tile_spans(rb, l, u, tile=1024):
+    """The block columns each 1024-slot tile of the block-dense scatter spans (jhi - jlo + 1), found as the kernel
+    finds them: the last block column whose slab start is at or before the tile's first and last slot.  A span of up
+    to 256 (kBdStage) is staged in shared memory; a longer one searches the start table in global memory."""
+    B = np.asarray(rb, np.int64)
+    N = len(rb)
+    off = np.concatenate([[0], np.cumsum(B)])
+    h = np.array([off[min(N - 1, J + l) + 1] - off[max(0, J - u)] for J in range(N)], np.int64)
+    start = np.concatenate([[0], np.cumsum(h * B)])
+    total = int(start[-1])
+    s0 = np.arange(0, total, tile, dtype=np.int64)
+    s1 = np.minimum(s0 + tile, total) - 1
+    col = lambda s: np.searchsorted(start[:N], s, side="right") - 1
+    return col(s1) - col(s0) + 1
+
+
+# l = u = 0: slabs of b^2 slots.  Blocks of 2: every tile spans exactly 256 slabs (staged, at the limit); one block of 1
+# ahead of them: 257 (unstaged); [3, 1, 3, 1] + [2] * 251: 255 slabs of 9, 1, 9, 1 and 4 slots fill each tile exactly
+BD_STAGING = [("span255", ([3, 1, 3, 1] + [2] * 251) * 3, 255), ("span256", [2] * 600, 256),
+              ("span257", [1] + [2] * 600, 257)]
+
+
+@pytest.mark.parametrize("case", BD_STAGING, ids=[c[0] for c in BD_STAGING])
+@pytest.mark.parametrize("sm", [None, "1"])
+def test_block_dense_staging_boundary(pkg, api, oracle, case, sm):
+    name, rb, span = case
+    s = (rb, 0, 0)
+    spans = bd_tile_spans(rb, 0, 0)
+    assert spans[:-1].max() == span and spans.max() == span, spans
+    st = block_dense_entries(*s)
+    n = sum(rb)
+    closed = bd_target(pkg, s, "cpu").matrix_colors()
+    for cvname, cv in (("matrix_colors", closed), ("relabelled", relabel(closed))):
+        for fdtype in ("forward", "central"):
+            bd_case(pkg, api, oracle, s, fdtype, cv, True, f"{name} SM_COUNT={sm} {fdtype} {cvname}", seed=71,
+                    env={"SM_COUNT": sm}, st=st)
+
+
+@pytest.mark.parametrize("world,partition", [(2, 0), (2, 1), (3, 0), (3, 1), (4, 0), (4, 1)])
+def test_block_dense_rank_plans(pkg, api, oracle, world, partition):
+    """Each rank writes exactly the slots of its own colours' columns (rank 0 also those without a valid colour); the
+    merged buffer is the single plan's, which is the oracle's."""
+    s = dict(BD_STRUCTS)["l_ne_u"]
+    st = block_dense_entries(*s)
+    rows, cols, slots, length = st
+    n = sum(s[0])
+    ell = Ell(n, rows, cols, 73)
+    x_np = host_x(n, 74)
+    x = torch.from_numpy(x_np).to(DEV)
+    closed = bd_target(pkg, s, "cpu").matrix_colors()
+    inval = greedy_coloring(n, rows, cols, np.random.default_rng(world))
+    inval[::5] = 0
+    for cvname, cv in (("matrix_colors", closed), ("invalid", inval)):
+        one, _, plan1 = bd_run(pkg, api, s, st, ell, x, "forward", cv, False)
+        ref, _ = oracle_run(oracle, st, n, ell, x_np, "forward", cv, plan1.eps(), {}, None, False)
+        assert_same_bits(one, ref, f"{cvname}: one plan vs oracle")
+        col_of_slot = np.empty(length, np.int64)
+        col_of_slot[slots] = cols
+        merged = np.full(length, np.nan)
+        for rank in range(world):
+            f, ctx = ell.native(pkg)
+            got, _, plan = bd_run(pkg, api, s, st, ell, x, "forward", cv, False, f=f,
+                                  plan_kw={"rank": rank, "world": world, "partition": partition})
+            owner = plan.color_owner()
+            k = cv[col_of_slot] - 1
+            valid = (k >= 0) & (k < len(owner))
+            mine = np.zeros(length, bool)
+            mine[valid] = owner[k[valid]] == rank
+            if rank == 0:
+                mine |= ~valid
+            what = f"{cvname} world={world} partition={partition} rank {rank}"
+            assert np.isnan(got[~mine]).all(), what
+            assert_same_bits(got[mine], one[mine], what, allow_nan=False)
+            merged[mine] = got[mine]
+            assert ctx.calls == 1 + int(np.sum(owner == rank)), what
+        assert_same_bits(merged, ref, f"{cvname} world={world}: merged vs oracle", allow_nan=False)
+
+
+@pytest.mark.parametrize("devices", device_sets(), ids=lambda d: "-".join(map(str, d)))
+@pytest.mark.parametrize("partition", [0, 1], ids=["round_robin", "lpt"])
+def test_block_dense_group(pkg, api, oracle, fdist, devices, partition):
+    root = torch.device("cuda", devices[0])
+    for sname in ("empty_inner", "uniform6"):
+        s = dict(BD_STRUCTS)[sname]
+        st = block_dense_entries(*s)
+        n = sum(s[0])
+        ell = Ell(n, st[0], st[1], 53)
+        x_np = host_x(n, 54)
+        x = torch.from_numpy(x_np).to(root)
+        closed = bd_target(pkg, s, "cpu").matrix_colors()
+        inval = closed.copy()
+        inval[::4] = 0
+        for fdtype in ("forward", "central"):
+            for cvname, cv in (("matrix_colors", closed), ("invalid", inval)):
+                BG = bd_target(pkg, s, root)
+                fns = [ell.native(pkg) for _ in devices]
+                gj = fdist.GroupJacobian(BG, cv, fdtype, devices, partition=partition)
+                assert gj.plans[0].info()["jkind"] == pkg._lib.FDB_J_BLOCK_DENSE
+                gj.run([f for f, _ in fns], x)
+                gj.synchronize()
+                what = f"{sname} {devices} {fdtype} {cvname} partition={partition}"
+                got = BG.data.cpu().numpy()
+                eps = gj.plans[0].eps()
+                ref, fcalls = oracle_run(oracle, st, n, ell, x_np, fdtype, cv, eps, {}, None, False)
+                assert_same_bits(got, ref, f"{what}: vs oracle", allow_nan=False)
+                check_values(got, st, ell, x_np, cv, eps, fdtype, True, what)
+                owner = gj.plans[0].color_owner()
+                for i, (_, ctx) in enumerate(fns):
+                    own = int(np.sum(owner == i))
+                    assert ctx.calls == (1 + own if fdtype == "forward" else 2 * own), (what, i)
+                assert sum(ctx.calls for _, ctx in fns) == fcalls + (len(devices) - 1 if fdtype == "forward" else 0), what
+                gj.close()
+
+
 # ------------------------------------------------------------------------------------------------ IEEE edges
 class SignF:
     """The ELL gather plus copysign(0.5, x_r), as a torch callback and its numpy twin with the same operations in the
@@ -732,7 +1075,8 @@ def edge_x(kind, cv, seed):
 
 EDGES = ["signed_zeros", "nan", "+inf", "-inf", "sq_overflow", "norm_inf", "sq_zero", "mixed"]
 EDGE_TARGETS = [("bb", ([20, 0, 17, 23, 0, 20] * 4, 1, 1, 1, 1, False)), ("bb", ([24] * 25, 1, 0, 2, 1, False)),
-                ("bidiag_U", None), ("bidiag_L", None), ("tri", None), ("dense_symtri", None)]
+                ("bidiag_U", None), ("bidiag_L", None), ("tri", None), ("dense_symtri", None),
+                ("block_dense", ([20, 0, 17, 23, 0, 20] * 2, 1, 1))]
 
 
 @pytest.mark.parametrize("edge", EDGES)
@@ -744,6 +1088,10 @@ def test_ieee_edges(pkg, api, oracle, edge, target, fdtype, dir):
         st = block_band_entries(*s[:5])
         n = sum(s[0])
         closed = bb_target(pkg, s, "cpu").matrix_colors()
+    elif kind == "block_dense":
+        st = block_dense_entries(*s)
+        n = sum(s[0])
+        closed = bd_target(pkg, s, "cpu").matrix_colors()
     else:
         n = 600
         st = diagonal_entries(kind, n)
@@ -765,6 +1113,8 @@ def test_ieee_edges(pkg, api, oracle, edge, target, fdtype, dir):
                 f, ctx = ell.native(pkg)
             if kind == "bb":
                 got, _, plan = bb_run(pkg, api, s, ell, x, fdtype, cv, coo, f=f, run_kw=kw)
+            elif kind == "block_dense":
+                got, _, plan = bd_run(pkg, api, s, st, ell, x, fdtype, cv, coo, f=f, run_kw=kw)
             else:
                 got, plan = dg_run(pkg, api, kind, n, st, f, x, fdtype, cv, coo, run_kw=kw)
             out[coo] = (got, plan, ctx and ctx.calls)
@@ -857,3 +1207,99 @@ def test_block_band_past_2_31(pkg):
     finally:
         del B
         torch.cuda.empty_cache()
+
+
+def tridiag_colour_sum(rows, c, cv, n):
+    """J value of (row, column) under the native tridiagonal f and colouring cv: the sum of f_r's coefficients (-2 at r,
+    1 at r - 1 and r + 1) over the columns of c's colour (any colouring, valid or not)."""
+    want = np.zeros(len(rows))
+    for dc, coef in ((-1, 1.0), (0, -2.0), (1, 1.0)):
+        o = rows + dc
+        ok = (o >= 0) & (o < n)
+        want += np.where(ok & (cv[np.clip(o, 0, n - 1)] == cv[c]), coef, 0.0)
+    return want
+
+
+# (a) one block of 46 400: a slab of 2 152 960 000 slots, so offsets inside one slab pass 2^31; (b) 700 blocks of 1024
+# with l = u = 1: 2.2e9 slots, so the slab starts pass 2^31
+BD_PAST = [("one_slab", [46_400], 0, 0), ("slab_starts", [1024] * 700, 1, 1)]
+
+
+@pytest.mark.parametrize("case", BD_PAST, ids=[c[0] for c in BD_PAST])
+def test_block_dense_past_2_31(pkg, case):
+    """Block-dense storage past 2^31 slots (about 17.6 GB of J and 2 GiB of f outputs).  Slots sampled below 2^31, across
+    it, above it and at the end are decoded with the header's slot formula in int64 and checked against the closed-form
+    sum of the tridiagonal f's coefficients over the colour of their column; J is prefilled with NaN."""
+    name, rb, l, u = case
+    n = sum(rb)
+    N = len(rb)
+    off = np.concatenate([[0], np.cumsum(rb)]).astype(np.int64)
+    K0 = np.maximum(np.arange(N) - u, 0)
+    K1 = np.minimum(np.arange(N) + l, N - 1)
+    h = off[K1 + 1] - off[K0]
+    start = np.concatenate([[0], np.cumsum(h * np.asarray(rb, np.int64))])
+    total = int(start[-1])
+    assert total > 2 ** 31
+    if name == "one_slab":
+        assert total > 2 ** 31 and total < 2 ** 32
+    free, _ = torch.cuda.mem_get_info()
+    need = 8 * total + (2 << 30) + 2e9
+    if free < need:
+        pytest.skip(f"needs about {need / 1e9:.0f} GB of free device memory, {free / 1e9:.1f} GB free")
+    rng = np.random.default_rng(37)
+    s = np.unique(np.concatenate([np.arange(2 ** 31 - 5000, 2 ** 31 + 5000), rng.integers(2 ** 31, total, 200_000),
+                                  rng.integers(0, 2 ** 31, 100_000), np.arange(total - 3000, total),
+                                  np.arange(0, 2000)]))
+    J = np.searchsorted(start[:N], s, side="right") - 1
+    rel = s - start[J]
+    col = off[J] + rel // h[J]
+    row = off[K0[J]] + rel % h[J]
+    B = pkg.BlockSkylineMatrix(rb, rb, (l, u), device=DEV)
+    assert B.j_len == total
+    x = torch.empty(n, dtype=torch.float64, device=DEV)
+    pkg._lib.synth().fdbs_fill_x(x.data_ptr(), n, 0x2B32, None)
+    closed = B.matrix_colors()
+    cvs = [("matrix_colors", closed), ("mod3", np.arange(n) % 3 + 1)] if name == "one_slab" else \
+        [("matrix_colors", closed), ("relabelled", relabel(closed))]
+    try:
+        got = {}
+        for cvname, cv in cvs:
+            B.data.fill_(NAN)
+            ctx = pkg._lib.TridiagCtx(n, 0)
+            f = pkg.NativeFn(C.cast(pkg._lib.synth().fdbs_tridiag, C.c_void_p).value, ctx)
+            cache = pkg.JacobianCache(x, "forward", colorvec=cv, sparsity=B, scratch_bytes=2 << 30)
+            pkg.finite_difference_jacobian_(B, f, x, cache)
+            torch.cuda.synchronize()
+            info = cache._last_plan.info()
+            assert info["jkind"] == pkg._lib.FDB_J_BLOCK_DENSE and info["j_len"] == total
+            assert ctx.calls == 1 + int(cv.max())
+            v = B.data[torch.from_numpy(s).to(DEV)].cpu().numpy()
+            del cache
+            want = tridiag_colour_sum(row, col, cv, n)
+            np.testing.assert_allclose(v, want, rtol=1e-6, atol=1e-6, err_msg=f"{name} {cvname}")
+            assert np.all(v[want == 0].view(np.uint64) == 0), f"{name} {cvname}: a zero slot is not +0.0"
+            got[cvname] = v
+        if "relabelled" in got:
+            assert_same_bits(got["relabelled"], got["matrix_colors"], "relabelled vs closed form past 2^31")
+    finally:
+        del B
+        torch.cuda.empty_cache()
+
+
+def test_block_dense_slab_limit(pkg, api):
+    """A block column may hold up to 2^32 - 1 slots: one block of 65 535 (4 294 836 225 slots) makes a plan, one of
+    65 536 (2^32) is refused.  No J is needed to create the plan."""
+    L = pkg._lib
+    for b, want in ((65_535, L.FDB_OK), (65_536, L.FDB_ERR_UNSUPPORTED)):
+        blocks = np.array([b], np.int64)
+        h = C.c_void_p()
+        o = api._opts(FD["forward"], 0)
+        st = L.lib().fdb_plan_create_block_dense(C.byref(h), 1, blocks.ctypes.data, 0, 0, b * b, None, C.byref(o))
+        assert st == want, (b, st, L.lib().fdb_last_error())
+        if st == L.FDB_OK:
+            plan = pkg.Plan(h.value)
+            info = plan.info()
+            assert info["jkind"] == L.FDB_J_BLOCK_DENSE and info["j_len"] == b * b > 2 ** 31
+            del plan
+        else:
+            assert not h.value

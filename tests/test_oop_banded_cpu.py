@@ -263,3 +263,80 @@ def test_the_typeerrors_that_stay(pkg, api):
     for proto in structured_protos:
         with pytest.raises(TypeError):
             api._oop_kind(pkg.BandedMatrix(n, n, 1, 1, device="cpu"), proto)
+
+
+# ---- the f and the checks of the oracle-held band tests (tests/test_gpu_oop_banded.py) ----
+def _oracle_shapes():
+    return [(37, 37, 2, 1), (40, 37, 3, 1), (33, 37, 0, 2), (37, 37, 40, 74), (37, 37, 0, 0), (290, 300, 4, 3)]
+
+
+@pytest.mark.parametrize("n,m,l,u", [(n, m, l, u) for m, n, l, u in _oracle_shapes()])
+def test_band_ell_reads_exactly_the_band(n, m, l, u):
+    from test_gpu_oop_banded import band_cp_rv, band_ell, band_entries
+    r, c = band_entries(m, n, l, u)
+    assert list(zip(r.tolist(), c.tolist())) == entries(m, n, l, u)
+    cp, rv = band_cp_rv(m, n, l, u)
+    assert np.array_equal(rv - 1, r) and np.array_equal(np.repeat(np.arange(n), np.diff(cp)), c)
+    ell = band_ell(m, n, l, u, 3)
+    listed = {(i, int(ell.cols[p, i])) for p in range(ell.K) for i in range(m)}
+    assert listed == set(zip(r.tolist(), c.tolist()))
+    nz = ell.coef[ell.coef != 0]
+    assert np.all(np.abs(nz) >= 0.5) and np.all(np.abs(nz) <= 2.0)
+    if len(r) > 500:
+        share = 1 - np.count_nonzero(ell.coef) / len(r)
+        assert 0.05 < share < 0.15, share
+
+
+def test_band_tile_shapes_reach_their_boundaries():
+    from test_gpu_oop_banded import BAND_TILES, band_entries
+    assert [s[0] for s in BAND_TILES] == [1023, 1024, 1025, 2047, 2049]
+    for E, m, n, l, u in BAND_TILES:
+        assert m != n and len(band_entries(m, n, l, u)[0]) == E
+        lens = np.diff(band_cp_rv_of(m, n, l, u))
+        assert lens[0] < lens.max() and lens[-1] < lens.max(), (E, m, n, l, u)       # clipped head and tail columns
+
+
+def band_cp_rv_of(m, n, l, u):
+    from test_gpu_oop_banded import band_cp_rv
+    return band_cp_rv(m, n, l, u)[0]
+
+
+@pytest.mark.parametrize("fd,dir", [("forward", 1.0), ("forward", -1.0), ("central", 1.0), ("central", -1.0),
+                                    ("complex", 1.0)])
+def test_oracle_within_the_band_check(pkg, oracle, fd, dir):
+    """The restatement on the band f lands within the analytic tolerance, its exact zeros (zero coefficients) give +0.0
+    in the dense result; a swapped entry, an entry moved out of the band, and a -0.0 left in place of a structural zero
+    each fail check_band_dense."""
+    from oop_oracle import fd_oop_oracle as OO
+    from test_gpu_oop_banded import _valid_cv, band_cp_rv, band_ell, band_x, check_band_dense
+    from test_gpu_oop_random import Twin
+    m, n, l, u = 66, 64, 4, 2
+    ell = band_ell(m, n, l, u, 5)
+    x = band_x(n, 6)
+    cp, rv = band_cp_rv(m, n, l, u)
+    cv = _valid_cv(n, l, u, m)
+    cv[::9] = 0
+    C_ = int(cv.max())
+    eps = None if fd == "complex" else np.full(C_, (1e-7 if fd == "forward" else 6e-6) * dir)
+    kw = {} if fd == "complex" else {"dir": dir, "eps_override": list(eps)}
+    want = OO.jacobian_oop(Twin(ell, oracle, fd == "complex"), x, fd, None, sparsity=(m, n, cp, rv), colorvec=cv,
+                           jac_prototype=("sparse", m, n), **kw)
+    J = np.zeros((m, n))
+    cols = np.repeat(np.arange(n), np.diff(want[3]))
+    J[want[4] - 1, cols] = 0.0 + want[5]
+    assert len(want[4]) < len(rv)                            # the exact zeros were dropped
+    check_band_dense(J, ell, x, cv, eps, fd, m, n, l, u, "restatement")
+    # a structural zero: a zero coefficient outside the row's slot 0, in a coloured column
+    z = [(i, int(ell.cols[p, i])) for p in range(1, ell.K) for i in range(m)
+         if ell.coef[p, i] == 0 and cv[ell.cols[p, i]] >= 1 and ell.cols[p, i] != ell.cols[0, i]]
+    assert z
+    r0, c0 = z[0]
+    c1 = next(c for c in range(max(0, r0 - l), min(n - 1, r0 + u) + 1) if J[r0, c] != 0 and J[r0, c] != J[r0, c0])
+    out = (r0 + l + 1, c0) if r0 + l + 1 < m and r0 + l + 1 > c0 + l else (0, n - 1)
+    for what, edit in (("-0.0 left", lambda A: A.__setitem__((r0, c0), -0.0)),
+                       ("swapped", lambda A: A.__setitem__(([r0, r0], [c0, c1]), A[[r0, r0], [c1, c0]])),
+                       ("moved out", lambda A: A.__setitem__(out, A[r0, c1]))):
+        bad = J.copy()
+        edit(bad)
+        with pytest.raises(AssertionError):
+            check_band_dense(bad, ell, x, cv, eps, fd, m, n, l, u, what)
