@@ -1324,11 +1324,26 @@ def _oop_band(sparsity):
     return None
 
 
+def _oop_block(sparsity):
+    """("block_banded", (l, u, lam, mu)) or ("block_dense", (l, u)) for a block sparsity the out-of-place Jacobian takes
+    in closed form (a BandedBlockBandedMatrix, BlockBandedMatrix included, or a BlockSkylineMatrix, with square blocks and
+    non-negative bandwidths), else None.  Its result is sparse only."""
+    if isinstance(sparsity, BandedBlockBandedMatrix) and min(sparsity.l, sparsity.u, sparsity.lam, sparsity.mu) >= 0 \
+            and sparsity.rb == sparsity.cb:
+        return "block_banded", (sparsity.l, sparsity.u, sparsity.lam, sparsity.mu)
+    if isinstance(sparsity, BlockSkylineMatrix) and min(sparsity.l, sparsity.u) >= 0 and sparsity.rb == sparsity.cb:
+        return "block_dense", (sparsity.l, sparsity.u)
+    return None
+
+
 def _oop_kind(sparsity, jac_prototype):
     """(result kind, m, ncols) the pair (sparsity, jac_prototype) gives; m / ncols None where f and colorvec decide."""
-    if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC) and _oop_band(sparsity) is None:
+    block = _oop_block(sparsity) is not None and isinstance(jac_prototype, SparseMatrixCSC)
+    if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC) and _oop_band(sparsity) is None and not block:
         raise TypeError(f"not built: sparsity of type {type(sparsity).__name__} in the out-of-place Jacobian "
-                        "(SparseMatrixCSC, BandedMatrix with l, u >= 0, Diagonal, Bidiagonal, SymTridiagonal or None)")
+                        "(SparseMatrixCSC, BandedMatrix with l, u >= 0, Diagonal, Bidiagonal, SymTridiagonal or None; "
+                        "BandedBlockBandedMatrix and BlockSkylineMatrix with square blocks and a SparseMatrixCSC "
+                        "jac_prototype)")
     if jac_prototype is not None:
         if isinstance(jac_prototype, SparseMatrixCSC):
             pm, pn = jac_prototype.shape
@@ -1355,6 +1370,11 @@ def _oop_plan_route(kind, sparsity, colorvec, pn, m, n):
     band = _oop_band(sparsity)
     if band is not None:
         return "banded", (m, n, band[0], band[1], cvp, kind, max(m, 1)), [k0]
+    block = _oop_block(sparsity)
+    if block is not None:
+        suffix, bw = block
+        blocks = np.asarray(sparsity.rb, dtype=np.int64)
+        return suffix, (len(blocks), blocks.ctypes.data if len(blocks) else None, *bw, cvp, kind, max(m, 1)), [k0, blocks]
     if sparsity is not None:
         cp, k1 = _index_ptr(sparsity.colptr)
         rv, k2 = _index_ptr(sparsity.rowval)
@@ -1447,6 +1467,10 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
         band / as for CSC           the same results for a BandedMatrix (l, u >= 0), Diagonal, Bidiagonal or SymTridiagonal
                                     sparsity, whose structural entries are the in-matrix band (l, u): a closed-form plan
                                     (fdb_oop_plan_create_banded) builds no entry list
+        block / SparseMatrixCSC     the sparse result for a BandedBlockBandedMatrix (BlockBandedMatrix included) or
+                                    BlockSkylineMatrix sparsity with square blocks, whose structural entries are those of
+                                    findstructralnz: closed-form plans (fdb_oop_plan_create_block_banded / _block_dense)
+                                    build no entry list; a dense result of a block sparsity is not built
     A sparse result is sized to the kept entries: reading that count is the call's one host synchronisation (when most
     candidates were dropped its rowval / nzval are copied into storage of their own size).  Other sparsity / prototype
     types and complex-valued results raise TypeError (not built).
@@ -1464,7 +1488,8 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
             stream = _stream(stream, x.device)
             if isinstance(f, NativeFn):
                 sp = None if sparsity is _DEFAULT else sparsity
-                m = sp.shape[0] if isinstance(sp, SparseMatrixCSC) or _oop_band(sp) is not None else (
+                m = sp.shape[0] if isinstance(sp, SparseMatrixCSC) or _oop_band(sp) is not None or \
+                    _oop_block(sp) is not None else (
                     jac_prototype.shape[0] if jac_prototype is not None else xv.numel())
                 xin = xv.to(torch.complex128) if _fdtype_code(fd) == L.FDB_COMPLEX else xv
                 fx = torch.empty(m, dtype=xin.dtype, device=x.device)

@@ -296,6 +296,7 @@ struct fdb_plan {
     int32_t *tile_col = nullptr;      // sparse result of a CSC sparsity: first column starting in each tile
     bool fused = false;               // sparse result, every colour's f! output resident: quotient + compaction fused
     int64_t band_nnz = 0;             // result of a band sparsity: |E|, every in-matrix band entry (colors.E counts coloured ones)
+    int64_t *block_start = nullptr;   // result of a block-banded sparsity: [nblocks + 1] first entry of every block column of E
   } oop;
   // side stream and events: coloured plans.  Forward mode runs the eps pass beside f(x) on the side stream; with
   // double_buffer, two output buffers let a group's scatter overlap the next group's f!

@@ -63,6 +63,53 @@ static int64_t oop_candidates(const fdb_plan *P) {
 // the entry set of a band plan (its bandwidths are clamped to the matrix at creation)
 static BandShape oop_band_shape(const fdb_plan *P) { return make_band_shape(P->m, P->n, P->band.l, P->band.u); }
 
+// the entry set of a block-banded or block-dense plan (kernels_oop.cuh, BlockShape)
+static BlockShape oop_block_shape(const fdb_plan *P) {
+  const auto &bb = P->block_band;
+  BlockShape b{};
+  b.boff = bb.off;
+  b.start = P->jkind == FDB_J_BLOCK_DENSE ? bb.start : P->oop.block_start;
+  b.jcolor = P->colors.jcolor;
+  b.n = P->n; b.lam = bb.lam; b.mu = bb.mu; b.u_full = P->band.u; b.w = bb.w;
+  b.nblocks = bb.nblocks;
+  b.l = (int32_t)std::min<int64_t>(P->band.l, bb.nblocks);
+  b.u = (int32_t)std::min<int64_t>(P->band.u, bb.nblocks);
+  b.bs = bb.bs;
+  b.block_cyclic = bb.cyclic ? 1 : 0;
+  b.bw = make_fastdiv((uint32_t)(P->band.l + P->band.u + 1));
+  b.sw = make_fastdiv((uint32_t)(bb.lam + bb.mu + 1));
+  return b;
+}
+
+// A block sparsity gives the sparse result only: a dense one would cost the m x n zero fill that the CSC route's entry
+// list already undercuts at any size where it fits
+static fdb_status oop_block_result(int result_kind, const char *what) {
+  if (result_kind == FDB_OOP_DENSE)
+    return fail(FDB_ERR_UNSUPPORTED, "not built: a dense out-of-place result of a %s sparsity (give a sparse prototype, "
+                                     "or a CSC sparsity)", what);
+  if (result_kind != FDB_OOP_SPARSE)
+    return fail(FDB_ERR_INVALID, "a %s sparsity gives a sparse (FDB_OOP_SPARSE) result", what);
+  return FDB_OK;
+}
+
+// The out-of-place form of an in-place block plan: the sparse result over its |E| = colors.E candidates
+static fdb_status oop_block_finish(PlanPtr &owner, fdb_plan **plan) {
+  fdb_plan *P = owner.get();
+  P->oop.on = 1;
+  P->oop.kind = FDB_OOP_SPARSE;
+  P->oop.ncols = P->n;
+  // many colours: the step sizes from the per-colour column lists, in the CSC plan's summation order
+  if (P->colors.C > kEpsRegColors) TRY(build_color_lists(P));
+  if (P->rank == 0) {
+    // one group of resident f! outputs on one rank: the compaction forms the quotients itself; otherwise the colour loop's
+    // block scatter writes the candidates in the in-place layout (every rank into the root's buffer)
+    P->oop.fused = P->scratch.n_groups <= 1 && P->world == 1;
+    TRY(oop_alloc_sparse(P, P->colors.E, P->oop.fused ? 0 : P->j_len));
+  }
+  *plan = owner.release();
+  return FDB_OK;
+}
+
 extern "C" {
 
 fdb_status fdb_oop_plan_create_csc(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval,
@@ -166,6 +213,58 @@ fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int
   return FDB_OK;
 }
 
+// BandedBlockBandedMatrix with square blocks: the in-place block-banded plan (block offsets, cyclic-colour detection)
+// plus the entries of E before every block column.  Host work O(nblocks).
+fdb_status fdb_oop_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                            int64_t lam, int64_t mu, const int64_t *colorvec, int result_kind, int64_t ldJ,
+                                            const fdb_plan_opts *opts) {
+  (void)ldJ;   // a sparse result has no leading dimension
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  TRY(oop_block_result(result_kind, "block-banded"));
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
+  fdb_plan_opts o = oop_opts(opts);
+  fdb_plan *raw = nullptr;
+  // the candidate buffer of a kCopy plan is the in-place band data: ldata is the plan's own
+  TRY(fdb_plan_create_block_banded(&raw, nblocks, blocks, l, u, lam, mu, INT64_MAX, colorvec, &o));
+  PlanPtr owner(raw);
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  if (P->n == 0) return fail(FDB_ERR_INVALID, "maximum(colorvec) of an empty colorvec: the reference throws");
+  const int32_t N = P->block_band.nblocks;
+  std::vector<int64_t> st((size_t)N + 1, 0);
+  {
+    DevBuf<int64_t> d_cnt;
+    TRY(d_cnt.alloc((size_t)N));
+    const BlockShape b = oop_block_shape(P);
+    block_band_col_counts<<<P->grid(N), kThreads>>>(b.boff, N, b.l, b.u, b.lam, b.mu, d_cnt.get());
+    CU(cudaGetLastError());
+    TRY(read_back(st.data() + 1, d_cnt.get(), (size_t)N, "block-column entry counts"));
+  }
+  for (int32_t J = 0; J < N; ++J) st[(size_t)J + 1] += st[(size_t)J];
+  TRY(P->alloc_t(&P->oop.block_start, (size_t)N + 1));
+  CU(cudaMemcpy(P->oop.block_start, st.data(), ((size_t)N + 1) * 8, cudaMemcpyHostToDevice));
+  return oop_block_finish(owner, plan);
+}
+
+// BlockSkylineMatrix (BlockBandedMatrices' BlockBandedMatrix) with square blocks: the in-place block-dense plan, whose slab
+// starts are the block-column starts of E.  Host work O(nblocks).
+fdb_status fdb_oop_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                           const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
+  (void)ldJ;
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  TRY(oop_block_result(result_kind, "block-dense"));
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
+  fdb_plan_opts o = oop_opts(opts);
+  fdb_plan *raw = nullptr;
+  TRY(fdb_plan_create_block_dense(&raw, nblocks, blocks, l, u, INT64_MAX, colorvec, &o));
+  PlanPtr owner(raw);
+  DeviceGuard g(owner->device);
+  if (owner->n == 0) return fail(FDB_ERR_INVALID, "maximum(colorvec) of an empty colorvec: the reference throws");
+  return oop_block_finish(owner, plan);
+}
+
 fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colorvec, int64_t ncols_out,
                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
   if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
@@ -237,7 +336,8 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
   double *J = base + P->columns.begin * P->ldJ;   // dense branch: this rank's column block
   DeviceGuard g(P->device);
   // a sparse result whose colorvec has no valid colour: nobody scatters, and the candidates are the zeros of rank 0
-  const int64_t cand_len = P->sp_kind == SP_BANDED ? P->j_len : P->colors.E;   // band data: every column's slots
+  // band and block-band data: every column's slots
+  const int64_t cand_len = P->sp_kind == SP_BANDED || P->sp_kind == SP_BLOCKBAND ? P->j_len : P->colors.E;
   if (P->oop.kind == FDB_OOP_SPARSE && !full && P->world > 1 && P->colors.local.empty() && cand_len > 0)
     CU(cudaMemsetAsync(J, 0, (size_t)cand_len * 8, s));
   if ((P->n > 0 && !d_x) || (P->j_len > 0 && !J)) return fail(FDB_ERR_INVALID, "NULL x or J");
@@ -284,7 +384,7 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
 // them (the full candidate count and maximum(colorvec)), fused with the quotients when one plan holds every f! output.
 static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const double *d_fx, const double *d_f_in,
                                   cudaStream_t s) {
-  const bool full = P->sp_kind == SP_NONE, band = P->sp_kind == SP_BANDED;
+  const bool full = P->sp_kind == SP_NONE, band = P->sp_kind == SP_BANDED, block = P->sp_kind == SP_BLOCKBAND;
   const int64_t candidates = oop_candidates(P);
   DeviceGuard g(P->device);
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
@@ -302,6 +402,24 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
     kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a, cs...);
   };
   if (full) go(oop_compact<true, kCopy, uint8_t>);
+  else if (block) {
+    // the candidates from the block scatters' buffer (kCopy), or the quotients from the resident f! outputs
+    const BlockShape b = oop_block_shape(P);
+    const bool dense = P->jkind == FDB_J_BLOCK_DENSE;
+    if (!P->oop.fused) {
+      if (dense) go(oop_compact_block_dense<kCopy, uint8_t>, b);
+      else go(oop_compact_block_band<kCopy, uint8_t>, b);
+    } else {
+      TRY(dispatch_mode(P->fdtype, [&](auto mode) {
+        return dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
+          constexpr int M = decltype(mode)::value;
+          if (dense) go(oop_compact_block_dense<M, decltype(tag)>, b);
+          else go(oop_compact_block_band<M, decltype(tag)>, b);
+          return FDB_OK;
+        });
+      }));
+    }
+  }
   else if (band && !P->oop.fused) go(oop_compact_band<kCopy, TableColors<uint8_t>>, TableColors<uint8_t>{nullptr});
   else if (band) TRY(dispatch_mode(P->fdtype, [&](auto mode) {
     return dispatch_ct(P->colors.bits, [&](auto tag) {
@@ -375,6 +493,22 @@ fdb_status fdb_group_create_oop_banded(fdb_group **group, int n_devices, const i
                                        const fdb_plan_opts *opts) {
   return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
     return fdb_oop_plan_create_banded(p, m, n, l, u, colorvec, result_kind, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_create_oop_block_banded(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                            const int64_t *blocks, int64_t l, int64_t u, int64_t lam, int64_t mu,
+                                            const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_block_banded(p, nblocks, blocks, l, u, lam, mu, colorvec, result_kind, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_create_oop_block_dense(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                           const int64_t *blocks, int64_t l, int64_t u, const int64_t *colorvec,
+                                           int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_block_dense(p, nblocks, blocks, l, u, colorvec, result_kind, ldJ, o);
   });
 }
 

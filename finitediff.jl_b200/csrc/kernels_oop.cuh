@@ -10,6 +10,7 @@
 #pragma once
 #include "common.cuh"
 #include "kernels_scatter.cuh"
+#include "kernels_blockband.cuh"
 
 namespace fdb {
 
@@ -59,8 +60,10 @@ oop_dense_finish(double *__restrict__ J, int64_t ldJ, int64_t m, int64_t C, int6
 //   kFormBand: the in-matrix band (l, u) of an m x n matrix, column-major and row-sorted, in closed form (BandShape): no
 //              row, colour-per-entry or column-start stream.  kCopy reads the candidates in band-data layout (slot u + r - c
 //              of column c, stride l + u + 1), as the in-place band scatter writes them.
+//   kFormBlockBand / kFormBlockDense: the entry set of a BandedBlockBandedMatrix / BlockSkylineMatrix with square blocks,
+//              in closed form from the block offsets (BlockShape, BlockBandForm, BlockDenseForm below).
 constexpr uint64_t kLbAggregate = 1ull << 62, kLbPrefix = 2ull << 62, kLbValue = (1ull << 62) - 1;
-enum { kFormCsc = 0, kFormFull = 1, kFormBand = 2 };
+enum { kFormCsc = 0, kFormFull = 1, kFormBand = 2, kFormBlockBand = 3, kFormBlockDense = 4 };
 
 // The in-matrix band E(m, n, l, u) = {(r, c) : -u <= r - c <= l, 0 <= r < m, 0 <= c < n} (0-based), l, u >= 0, clamped to
 // l <= m - 1, u <= n - 1 (the same set).  Column c holds rows max(0, c - u) .. min(m - 1, c + l); columns c >= m + u are
@@ -169,9 +172,11 @@ oop_tile_first_col(const int32_t *__restrict__ colptr32, int64_t ncols, int64_t 
 }
 
 // The compaction over candidates of structure FORM.  CS: the colour source, of the entry (kFormCsc: TableColors over
-// ecolor) or of the column (kFormBand); unused by kCopy.
+// ecolor) or of the column (kFormBand); unused by kCopy.  The block forms pass their form object (BlockBandForm,
+// BlockDenseForm), which stages each tile's block geometry and gives every candidate its row, source slot and colour.
 template <int FORM, int MODE, typename CS>
 __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs) {
+  constexpr bool kBlock = FORM == kFormBlockBand || FORM == kFormBlockDense;
   constexpr int kWarps = kThreads / 32, kRounds = kTile / kThreads;
   __shared__ uint32_t s_mask[kRounds * kWarps];
   __shared__ uint32_t s_pre[kRounds * kWarps + 1];
@@ -191,6 +196,7 @@ __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs
     const int64_t tile = s_tile;
     if (tile >= ntiles) return;
     const int64_t t0 = tile * kTile;
+    if constexpr (kBlock) cs.begin_tile(a.E, t0);   // (synchronises the block)
     // element (round u, warp w, lane) = t0 + u*kThreads + w*32 + lane: (u, w, lane) order is storage order
     double v[kRounds];
     int32_t r[kRounds];
@@ -198,27 +204,42 @@ __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs
     for (int u = 0; u < kRounds; ++u) {
       const int64_t e = t0 + u * kThreads + threadIdx.x;
       const bool in = e < a.E;
-      int64_t bc = 0, br = 0;                      // kFormBand: the candidate's column and row
-      if (FORM == kFormBand) {
-        if (in) band_locate(a.band, e, bc, br);
-        r[u] = (int32_t)br;
-      } else if (FORM == kFormFull) {
-        r[u] = in ? (int32_t)(e % a.m) : 0;
-      } else {
-        r[u] = in ? __ldcs(a.row32 + e) : 0;
-      }
-      if (MODE == kCopy) {
-        const int64_t src = FORM == kFormBand ? bc * a.band.w + a.band.u + br - bc : e;
-        v[u] = in ? __ldcs(a.vals + src) : 0.0;
-      } else {
+      if constexpr (kBlock) {
+        // the form gives the row, the slot of the candidate buffer (kCopy) and the colour of the column (quotients)
+        int32_t row = 0;
+        int64_t src = e;
         uint32_t k = 0xFFFFFFFFu;
-        if constexpr (FORM == kFormBand) { if (in) k = cs.at(bc); }
-        else if (in) k = (uint32_t)cs.p[e];
-        // a column without a valid colour is never perturbed: its entries are 0 and dropped
-        v[u] = k < (uint32_t)a.ncolors
-                   ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, r[u],
-                                       __ldg(a.eps + k))
-                   : 0.0;
+        if (in) cs.template locate<MODE != kCopy>(e, row, src, k);
+        r[u] = row;
+        if (MODE == kCopy) v[u] = in ? __ldcs(a.vals + src) : 0.0;
+        else
+          v[u] = k < (uint32_t)a.ncolors
+                     ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx,
+                                         row, __ldg(a.eps + k))
+                     : 0.0;
+      } else {
+        int64_t bc = 0, br = 0;                      // kFormBand: the candidate's column and row
+        if (FORM == kFormBand) {
+          if (in) band_locate(a.band, e, bc, br);
+          r[u] = (int32_t)br;
+        } else if (FORM == kFormFull) {
+          r[u] = in ? (int32_t)(e % a.m) : 0;
+        } else {
+          r[u] = in ? __ldcs(a.row32 + e) : 0;
+        }
+        if (MODE == kCopy) {
+          const int64_t src = FORM == kFormBand ? bc * a.band.w + a.band.u + br - bc : e;
+          v[u] = in ? __ldcs(a.vals + src) : 0.0;
+        } else {
+          uint32_t k = 0xFFFFFFFFu;
+          if constexpr (FORM == kFormBand) { if (in) k = cs.at(bc); }
+          else if (in) k = (uint32_t)cs.p[e];
+          // a column without a valid colour is never perturbed: its entries are 0 and dropped
+          v[u] = k < (uint32_t)a.ncolors
+                     ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, r[u],
+                                         __ldg(a.eps + k))
+                     : 0.0;
+        }
       }
       const uint32_t mk = __ballot_sync(0xffffffffu, v[u] != 0.0);   // NaN != 0.0 is true: NaN is kept
       if (lane == 0) s_mask[u * kWarps + w] = mk;
@@ -280,11 +301,15 @@ __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs
     const bool last = tile == ntiles - 1;
     const int64_t t1 = last ? a.E + 1 : t0 + kTile;
     // first column that starts at or after t0 (kFormFull: ceil(t0 / m), at most C since t0 < E = C*m)
-    const int64_t clo = FORM == kFormFull   ? (t0 + a.m - 1) / a.m
-                        : FORM == kFormBand ? band_first_col(a.band, t0)
-                                            : (int64_t)__ldg(a.tile_col + tile);
+    int64_t clo;
+    if constexpr (kBlock) clo = cs.first_col(t0);
+    else clo = FORM == kFormFull   ? (t0 + a.m - 1) / a.m
+               : FORM == kFormBand ? band_first_col(a.band, t0)
+                                   : (int64_t)__ldg(a.tile_col + tile);
     for (int64_t c = clo + threadIdx.x; c <= a.ncols; c += kThreads) {
-      const int64_t p = compact_col_start<FORM>(a, c);
+      int64_t p;
+      if constexpr (kBlock) p = cs.col_start(a.E, c);
+      else p = compact_col_start<FORM>(a, c);
       if (p >= t1) break;
       const int64_t q = p - t0;                      // position inside the tile, 0..1024
       int64_t before;
@@ -312,6 +337,252 @@ template <int MODE, typename CS>
 __global__ void __launch_bounds__(kThreads)
 oop_compact_band(const CompactArgs a, const CS cs) {
   compact_tiles<kFormBand, MODE>(a, cs);
+}
+
+// ---- the block forms ----
+// The entry set E of a block structure with square blocks (block K has rows and columns boff[K] .. boff[K+1] - 1), in
+// column-major, row-sorted order.  Column j of block column J holds, for every block row K in K0(J) = max(0, J-u) ..
+// K1(J) = min(N-1, J+l) in turn:
+//   kFormBlockBand  (BandedBlockBandedMatrix) the sub-band rows max(0, j-mu) .. min(m_K-1, j+lam) of block (K, J).  The
+//                   entries of block (K, J) in its columns before j number band_col_start(m_K, lam, mu, j), so column j
+//                   starts at start[J] + sum_K band_col_start(m_K, lam, mu, j);
+//   kFormBlockDense (BlockSkylineMatrix) every row of those blocks, one contiguous range of height h_J: the slab storage
+//                   order of the in-place block-dense plan is this order, and candidate e is slot e.
+// start[J] is the first entry of block column J (nblocks + 1 values: the only table besides the block offsets).  Every
+// column holds at least its diagonal entry, so a tile of kTile candidates spans at most kTile columns.
+struct BlockShape {
+  const int32_t *boff;         // [nblocks + 1] first row / column of every block, 0-based
+  const int64_t *start;        // [nblocks + 1] first entry of every block column
+  const void *jcolor;          // [n] colour of column c (CT); not read with block_cyclic
+  int64_t n, lam, mu, u_full;  // u_full: the block upper bandwidth as given (band-data slot of kCopy)
+  int64_t w;                   // kFormBlockBand: band-data slots per column, (l+u+1)(lam+mu+1)
+  int32_t nblocks, l, u;       // l, u clamped to nblocks (the same structure)
+  int32_t bs;                  // kFormBlockDense with block_cyclic: the uniform block size
+  int32_t block_cyclic;        // the colour is the block-cyclic closed form of matrix_colors: no colour stream
+  FastDiv bw, sw;              // l+u+1 and lam+mu+1 as given (the cyclic colour's periods)
+};
+
+// entries of E in columns 0 .. j-1 of block column J (kFormBlockBand): at most l+u+1 closed forms
+__host__ __device__ __forceinline__ int64_t bb_col_offset(const int32_t *boff, int32_t nblocks, int32_t l, int32_t u,
+                                                          int64_t lam, int64_t mu, int32_t J, int64_t j) {
+  const int32_t K0 = J - u > 0 ? J - u : 0, K1 = J + l < nblocks - 1 ? J + l : nblocks - 1;
+  int64_t s = 0;
+  for (int32_t K = K0; K <= K1; ++K) s += band_col_start((int64_t)boff[K + 1] - boff[K], lam, mu, j);
+  return s;
+}
+
+// the block column holding candidate e: the largest J with start[J] <= e (an empty block column shares its start with
+// the next one)
+__device__ __forceinline__ int32_t blk_column_of(const BlockShape &b, int32_t lo, int32_t hi, int64_t e) {
+  while (lo < hi) {
+    const int32_t mid = (int32_t)(((uint32_t)lo + (uint32_t)hi + 1u) >> 1);
+    if (__ldg(b.start + mid) <= e) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+template <typename CT>
+__device__ __forceinline__ uint32_t blk_table_color(const BlockShape &b, int64_t c) {
+  return (uint32_t)__ldg(reinterpret_cast<const CT *>(b.jcolor) + c);
+}
+
+// Block-banded: each tile stages the starts of the columns it spans (c_lo .. c_lo + nc, the last one the start of the
+// column after the tile's last), found once per tile from the closed form; a candidate then finds its column by a search
+// of that table in shared memory and its block and row by walking the blocks of the column.
+struct BlockBandTile {
+  int64_t cs[kTile + 1];       // start of column c_lo + i
+  int32_t cj[kTile + 1];       // its block column
+  int64_t c_lo, c_hi;          // the columns of the tile's first and last candidates (at most kTile columns)
+  int32_t jlo, jhi;            // their block columns
+  __device__ __forceinline__ int32_t nc() const { return (int32_t)(c_hi - c_lo) + 1; }
+};
+
+template <typename CT>
+struct BlockBandForm {
+  BlockShape b;
+  BlockBandTile *t;
+
+  // column of candidate e and its block column: a search over the block-column starts, then over the closed form
+  __device__ __forceinline__ void column_of(int64_t e, int64_t &c, int32_t &J) const {
+    J = blk_column_of(b, 0, b.nblocks - 1, e);
+    const int64_t rel = e - __ldg(b.start + J);
+    int64_t lo = 0, hi = (int64_t)__ldg(b.boff + J + 1) - __ldg(b.boff + J) - 1;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (bb_col_offset(b.boff, b.nblocks, b.l, b.u, b.lam, b.mu, J, mid) <= rel) lo = mid;
+      else hi = mid - 1;
+    }
+    c = __ldg(b.boff + J) + lo;
+  }
+
+  __device__ __forceinline__ void begin_tile(int64_t E, int64_t t0) const {
+    if (threadIdx.x < 2) {
+      int64_t c;
+      int32_t J;
+      column_of(threadIdx.x == 0 ? t0 : (t0 + kTile < E ? t0 + kTile : E) - 1, c, J);
+      if (threadIdx.x == 0) { t->c_lo = c; t->jlo = J; }
+      else { t->c_hi = c; t->jhi = J; }
+    }
+    __syncthreads();
+    const int64_t c_lo = t->c_lo;
+    const int32_t nc = t->nc(), jlo = t->jlo, jhi = t->jhi;
+    for (int i = threadIdx.x; i <= nc; i += kThreads) {
+      const int64_t c = c_lo + i;
+      int64_t s = E;
+      int32_t J = jhi;
+      if (c < b.n) {
+        J = i < nc ? bb_block_of(b.boff, jlo, jhi, (int32_t)c) : bb_block_of(b.boff, jhi, b.nblocks - 1, (int32_t)c);
+        s = __ldg(b.start + J) + bb_col_offset(b.boff, b.nblocks, b.l, b.u, b.lam, b.mu, J, c - __ldg(b.boff + J));
+      }
+      t->cs[i] = s;
+      t->cj[i] = J;
+    }
+    __syncthreads();
+  }
+
+  template <bool COLOR>
+  __device__ __forceinline__ void locate(int64_t e, int32_t &row, int64_t &src, uint32_t &k) const {
+    int32_t lo = 0, hi = t->nc() - 1;                   // the last staged column starting at or before e
+    while (lo < hi) {
+      const int32_t mid = (lo + hi + 1) >> 1;
+      if (t->cs[mid] <= e) lo = mid;
+      else hi = mid - 1;
+    }
+    const int64_t c = t->c_lo + lo;
+    const int32_t J = t->cj[lo];
+    const int64_t j = c - __ldg(b.boff + J);
+    int64_t q = e - t->cs[lo];                          // position inside the column
+    const int32_t K0 = J - b.u > 0 ? J - b.u : 0, K1 = J + b.l < b.nblocks - 1 ? J + b.l : b.nblocks - 1;
+    const int64_t rlo = j - b.mu > 0 ? j - b.mu : 0;    // first sub-band row of column j in every block
+    int32_t K = K0;
+    for (;; ++K) {                                      // the block row of the q-th entry of the column
+      const int64_t rK = __ldg(b.boff + K), mK = (int64_t)__ldg(b.boff + K + 1) - rK;
+      const int64_t rhi = j + b.lam < mK - 1 ? j + b.lam : mK - 1;
+      const int64_t cnt = rhi >= rlo ? rhi - rlo + 1 : 0;
+      if (q < cnt || K == K1) { row = (int32_t)(rK + rlo + q); break; }
+      q -= cnt;
+    }
+    // entry (k, j) of block (K, J), k = rlo + q: slot (K - J + u)(lam + mu + 1) + (mu + k - j) of column c
+    src = c * b.w + ((int64_t)K - J + b.u_full) * (b.lam + b.mu + 1) + (b.mu + rlo + q - j);
+    if (COLOR)
+      k = b.block_cyclic ? b.bw.mod((uint32_t)J) * b.sw.d + b.sw.mod((uint32_t)j) : blk_table_color<CT>(b, c);
+  }
+
+  // the first column that starts at or after t0, and the start of column c >= it (every column the tile's colptr pass
+  // reaches is staged: a later one starts after the tile)
+  __device__ __forceinline__ int64_t first_col(int64_t t0) const { return t->cs[0] == t0 ? t->c_lo : t->c_lo + 1; }
+  __device__ __forceinline__ int64_t col_start(int64_t E, int64_t c) const {
+    const int64_t i = c - t->c_lo;
+    return i <= t->nc() ? t->cs[i] : E;
+  }
+};
+
+// Block-dense: the staging of diff_scatter_block_dense (the tile's first and last block columns, and the geometry of
+// up to kBdStage block columns between them in shared memory); candidate e is slot e, and its column and row come from
+// (e - start_J) / h_J.
+struct BlockDenseTile {
+  int64_t start[kBdStage];
+  int32_t h[kBdStage], row0[kBdStage], col0[kBdStage];
+  int32_t jlo, jhi;
+};
+
+template <typename CT>
+struct BlockDenseForm {
+  BlockShape b;
+  BlockDenseTile *t;
+
+  __device__ __forceinline__ void slab(int32_t J, int32_t &h, int32_t &row0) const {
+    const int32_t K0 = J - b.u > 0 ? J - b.u : 0, K1 = J + b.l < b.nblocks - 1 ? J + b.l : b.nblocks - 1;
+    row0 = __ldg(b.boff + K0);
+    h = __ldg(b.boff + K1 + 1) - row0;
+  }
+
+  __device__ __forceinline__ void begin_tile(int64_t E, int64_t t0) const {
+    if (threadIdx.x < 2) {
+      const int64_t s = threadIdx.x == 0 ? t0 : (t0 + kTile < E ? t0 + kTile : E) - 1;
+      const int32_t J = blk_column_of(b, 0, b.nblocks - 1, s);
+      if (threadIdx.x == 0) t->jlo = J;
+      else t->jhi = J;
+    }
+    __syncthreads();
+    const int32_t jlo = t->jlo, jhi = t->jhi;
+    if (jhi - jlo < kBdStage && threadIdx.x <= jhi - jlo) {
+      const int32_t J = jlo + threadIdx.x;
+      t->start[threadIdx.x] = __ldg(b.start + J);
+      slab(J, t->h[threadIdx.x], t->row0[threadIdx.x]);
+      t->col0[threadIdx.x] = __ldg(b.boff + J);
+    }
+    __syncthreads();
+  }
+
+  // block column, its start, height, first row and first column of candidate e
+  __device__ __forceinline__ void geometry(int64_t e, int32_t &J, int64_t &st, int32_t &h, int32_t &row0,
+                                           int32_t &col0) const {
+    const int32_t jlo = t->jlo, jhi = t->jhi;
+    if (jhi - jlo < kBdStage) {
+      const int32_t i = bd_column_of(t->start, 0, jhi - jlo, e);
+      J = jlo + i; st = t->start[i]; h = t->h[i]; row0 = t->row0[i]; col0 = t->col0[i];
+    } else {
+      J = blk_column_of(b, jlo, jhi, e);
+      st = __ldg(b.start + J);
+      slab(J, h, row0);
+      col0 = __ldg(b.boff + J);
+    }
+  }
+
+  template <bool COLOR>
+  __device__ __forceinline__ void locate(int64_t e, int32_t &row, int64_t &src, uint32_t &k) const {
+    int32_t J, h, row0, col0;
+    int64_t st;
+    geometry(e, J, st, h, row0, col0);
+    const uint32_t rel = (uint32_t)(e - st);           // < h cb[J] <= 2^32 (the plan refuses larger slabs)
+    const uint32_t j = rel / (uint32_t)h;
+    row = row0 + (int32_t)(rel - j * (uint32_t)h);
+    src = e;
+    if (COLOR) k = b.block_cyclic ? b.bw.mod((uint32_t)J) * (uint32_t)b.bs + j : blk_table_color<CT>(b, col0 + (int64_t)j);
+  }
+
+  __device__ __forceinline__ int64_t first_col(int64_t t0) const {
+    int32_t J, h, row0, col0;
+    int64_t st;
+    geometry(t0, J, st, h, row0, col0);
+    const uint32_t rel = (uint32_t)(t0 - st), j = rel / (uint32_t)h;
+    return col0 + (int64_t)j + (rel == j * (uint32_t)h ? 0 : 1);
+  }
+  // column c >= first_col(t0): in block columns jlo .. jhi, or after the tile (its start is at least start[jhi + 1])
+  __device__ __forceinline__ int64_t col_start(int64_t E, int64_t c) const {
+    if (c >= b.n) return E;
+    const int32_t jhi = t->jhi;
+    if (c >= __ldg(b.boff + jhi + 1)) return __ldg(b.start + jhi + 1);
+    const int32_t J = bb_block_of(b.boff, t->jlo, jhi, (int32_t)c);
+    int32_t h, row0;
+    slab(J, h, row0);
+    return __ldg(b.start + J) + (c - __ldg(b.boff + J)) * (int64_t)h;
+  }
+};
+
+// BandedBlockBandedMatrix (kFormBlockBand) and BlockSkylineMatrix (kFormBlockDense) entry sets; colours of type CT
+template <int MODE, typename CT>
+__global__ void __launch_bounds__(kThreads)
+oop_compact_block_band(const CompactArgs a, const BlockShape b) {
+  __shared__ BlockBandTile s_t;
+  compact_tiles<kFormBlockBand, MODE>(a, BlockBandForm<CT>{b, &s_t});
+}
+
+template <int MODE, typename CT>
+__global__ void __launch_bounds__(kThreads)
+oop_compact_block_dense(const CompactArgs a, const BlockShape b) {
+  __shared__ BlockDenseTile s_t;
+  compact_tiles<kFormBlockDense, MODE>(a, BlockDenseForm<CT>{b, &s_t});
+}
+
+// Plan time, block-banded result: the entries of E in every block column, sum_K band_col_start(m_K, lam, mu, cb[J])
+__global__ void __launch_bounds__(kThreads)
+block_band_col_counts(const int32_t *__restrict__ boff, int32_t nblocks, int32_t l, int32_t u, int64_t lam, int64_t mu,
+                      int64_t *__restrict__ cnt) {
+  for (int32_t J = blockIdx.x * kThreads + threadIdx.x; J < nblocks; J += gridDim.x * kThreads)
+    cnt[J] = bb_col_offset(boff, nblocks, l, u, lam, mu, J, (int64_t)boff[J + 1] - boff[J]);
 }
 
 // J[r + c ldJ] += 0.0 over the band entries of the columns whose colour this rank owns, for a zero-filled dense J that

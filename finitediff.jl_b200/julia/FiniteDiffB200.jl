@@ -1023,6 +1023,39 @@ function oop_band_plan(anchor, band, kind::Cint, colorvec, fd::Cint)
     end
 end
 
+# block sparsities the out-of-place Jacobian takes in closed form (fdb_oop_plan_create_block_banded / _block_dense): their
+# structural entries are those the in-place block plans write.  Only the sparse result is built.
+oopblock(A::Union{DeviceBlockBanded, DeviceBlockDense}) = A
+oopblock(A) = nothing
+
+function oop_block_plan(anchor, B::DeviceBlockBanded, kind::Cint, colorvec, fd::Cint)
+    cached_plan(anchor, (:oop_block_banded, kind, B.blocks, B.l, B.u, B.lam, B.mu, color_key(colorvec), fd)) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd))
+        cptr, croot = color_arg(colorvec, sum(B.blocks))
+        GC.@preserve croot B begin
+            check(ccall((:fdb_oop_plan_create_block_banded, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Ptr{Int64}, Int64, Int64, Int64, Int64, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+                h, length(B.blocks), pointer(B.blocks), B.l, B.u, B.lam, B.mu, cptr, kind, max(sum(B.blocks), 1), opts))
+        end
+        Plan(h[], croot)
+    end
+end
+
+function oop_block_plan(anchor, B::DeviceBlockDense, kind::Cint, colorvec, fd::Cint)
+    cached_plan(anchor, (:oop_block_dense, kind, B.blocks, B.l, B.u, color_key(colorvec), fd)) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd))
+        cptr, croot = color_arg(colorvec, sum(B.blocks))
+        GC.@preserve croot B begin
+            check(ccall((:fdb_oop_plan_create_block_dense, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Ptr{Int64}, Int64, Int64, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+                h, length(B.blocks), pointer(B.blocks), B.l, B.u, cptr, kind, max(sum(B.blocks), 1), opts))
+        end
+        Plan(h[], croot)
+    end
+end
+
 """
     finite_difference_jacobian(f, x::CuVector{Float64}, cache::JacobianCache, f_in = nothing;
                                relstep, absstep, colorvec, sparsity, jac_prototype, dir)
@@ -1030,7 +1063,8 @@ end
 `src/jacobians.jl:277-429` on the device.  The result follows (sparsity, jac_prototype) as `J + Ji` does in the reference:
 a dense `CuMatrix` (raw quotients without either, `0.0 + dx` with a dense prototype or a CSC sparsity) or, with a sparse
 prototype, a `DeviceCSC` holding the entries whose value is not ±0.0 (its pattern is copied back to the host: reading the
-kept count is the call's one synchronisation).  `cache.x1` receives a copy of x (:293-295).
+kept count is the call's one synchronisation).  A `DeviceBlockBanded` or `DeviceBlockDense` sparsity takes a sparse
+prototype only (a dense result of it throws `ArgumentError`).  `cache.x1` receives a copy of x (:293-295).
 """
 function finite_difference_jacobian(f, x::CuVector{Float64},
         cache::JacobianCache{T1, T2, T3, T4, cType, sType, fdtype, returntype}, f_in = nothing;
@@ -1039,8 +1073,13 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     cache.x1 === x || copyto!(cache.x1, x)
     n = length(x)
     band = sparsity === nothing ? nothing : oopband(sparsity)
-    sp = sparsity === nothing || band !== nothing ? nothing : hostcsc(sparsity)
-    m = band !== nothing ? band[1] : sp !== nothing ? size(sp, 1) : (f_in !== nothing ? length(f_in) : length(cache.fx))
+    block = sparsity === nothing ? nothing : oopblock(sparsity)
+    sp = sparsity === nothing || band !== nothing || block !== nothing ? nothing : hostcsc(sparsity)
+    m = band !== nothing ? band[1] : block !== nothing ? size(block, 1) : sp !== nothing ? size(sp, 1) :
+        (f_in !== nothing ? length(f_in) : length(cache.fx))
+    block !== nothing && !(jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC) &&
+        throw(ArgumentError("not built: a dense out-of-place result of a $(typeof(block)) sparsity (give a sparse " *
+                            "jac_prototype, or a CSC sparsity)"))
     if jac_prototype === nothing
         kind, ncols = sp === nothing && band === nothing ? (FDB_OOP_RAW, 0) : (FDB_OOP_DENSE, n)
     elseif jac_prototype isa AbstractMatrix && !(jac_prototype isa SparseMatrixCSC)
@@ -1050,6 +1089,7 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     end
     fd = fdcode(fdtype)
     plan = band !== nothing ? oop_band_plan(cache, band, kind, colorvec, fd) :
+           block !== nothing ? oop_block_plan(cache, block, kind, colorvec, fd) :
            oop_plan(sp === nothing ? cache : sp.colptr, sp, m, n, kind, ncols, colorvec, fd)
     pinfo = info(plan)
     kind == FDB_OOP_RAW && (ncols = pinfo.n_local_colors)
@@ -1057,7 +1097,7 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     J = nothing
     colptr = rowval = nzval = nnz = nothing
     if kind == FDB_OOP_SPARSE
-        cap = sp === nothing && band === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
+        cap = sp === nothing && band === nothing && block === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
         colptr, rowval = CuVector{Int64}(undef, ncols + 1), CuVector{Int64}(undef, max(cap, 1))
         nzval, nnz = CuVector{Float64}(undef, max(cap, 1)), CuVector{Int64}(undef, 1)
         out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), cap, pointer(nnz)))
@@ -1148,6 +1188,40 @@ function group_oop_banded(sparsity, colorvec, fdtype, devices::Vector{Cint}; jac
             h, length(devices), pointer(devices), m, n, l, u, cptr, kind, max(m, 1), opts))
     end
     oop_group_result(h, devices, croot, kind, m, n, n, fdtype)
+end
+
+# sparsity: a DeviceBlockBanded / DeviceBlockDense; jac_prototype: a sparse one (the dense result is not built)
+function group_oop_block_banded(B::DeviceBlockBanded, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC ||
+        throw(ArgumentError("not built: a dense out-of-place result of a block-banded sparsity"))
+    n = sum(B.blocks)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve B croot devices begin
+        check(ccall((:fdb_group_create_oop_block_banded, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Ptr{Int64}, Int64, Int64, Int64, Int64, Ptr{Int64}, Cint, Int64,
+                Ref{PlanOpts}),
+            h, length(devices), pointer(devices), length(B.blocks), pointer(B.blocks), B.l, B.u, B.lam, B.mu, cptr,
+            FDB_OOP_SPARSE, max(n, 1), opts))
+    end
+    oop_group_result(h, devices, croot, FDB_OOP_SPARSE, n, n, n, fdtype)
+end
+
+function group_oop_block_dense(B::DeviceBlockDense, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC ||
+        throw(ArgumentError("not built: a dense out-of-place result of a block-dense sparsity"))
+    n = sum(B.blocks)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve B croot devices begin
+        check(ccall((:fdb_group_create_oop_block_dense, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Ptr{Int64}, Int64, Int64, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), length(B.blocks), pointer(B.blocks), B.l, B.u, cptr, FDB_OOP_SPARSE,
+            max(n, 1), opts))
+    end
+    oop_group_result(h, devices, croot, FDB_OOP_SPARSE, n, n, n, fdtype)
 end
 
 # sparsity === nothing: m rows (length of f(x)), n = length(x)

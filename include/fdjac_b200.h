@@ -515,13 +515,22 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   colouring's conflicts on the device at plan time (skipped for a cyclic colouring with more than l + u colours, which has
  *   none).  A sparse result is compacted from the resident f! outputs in closed form, or, when they come in several groups
  *   or ranks, from candidates the band scatter wrote in band-data layout.
+ * fdb_oop_plan_create_block_banded / fdb_oop_plan_create_block_dense: the sparsity is the entry set E of a square-block
+ *   BandedBlockBandedMatrix (block bandwidths (l, u), sub-block bandwidths (lam, mu): rows max(0, j-mu) .. min(m_K-1, j+lam)
+ *   of every block (K, J) with K in blockcolrange(J)) or BlockSkylineMatrix (every row of those blocks; BlockBandedMatrices'
+ *   BlockBandedMatrix), `blocks` the nblocks block sizes as for fdb_plan_create_block_banded / _block_dense.  Only
+ *   result_kind FDB_OOP_SPARSE is built (ldJ is ignored): the same result, status and f! calls as fdb_oop_plan_create_csc
+ *   given the CSC of E, for any colorvec.  FDB_OOP_DENSE is FDB_ERR_UNSUPPORTED and FDB_OOP_RAW FDB_ERR_INVALID; sizes,
+ *   bandwidths and the block list are refused as by the in-place block creators.  Host work is O(nblocks) plus reading the
+ *   colorvec, and no entry, row or column-start list exists: the compaction finds each candidate's column and row from the
+ *   block offsets and one table of nblocks + 1 block-column starts.  Candidate counts may pass 2^31.
  * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans (rank plans below).
  * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
  *   dense kinds: out->J (device, ldJ of the plan; the whole result, rank plans included);
  *   FDB_OOP_SPARSE: out->colptr [ncols + 1], out->rowval / out->nzval [out->cap >= the candidate count: nnz of the sparsity,
  *   or m*C], Int64 1-based; the kept count goes to the device scalar *out->nnz (stream-ordered, no host sync).
  * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a sparsity,
- * |E| with a band).
+ * |E| with a band or a block structure).
  *
  * Rank plans (opts.rank / opts.world, world in 2..64).  A rank evaluates only the colours it owns: the colour partition of
  * the in-place plans (opts.partition: round-robin or LPT, fdb_plan_color_owner) with a sparsity, the contiguous column
@@ -538,6 +547,9 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   FDB_OOP_DENSE, band         as for a CSC sparsity, the + 0.0 in closed form over its own colours' band entries;
  *   FDB_OOP_SPARSE, band        its colours' columns of the band data into the root's buffer (rank 0 also writes the zeros
  *                               of columns without a valid colour); the root then compacts every band entry into `out`;
+ *   FDB_OOP_SPARSE, block       its colours' columns into the root's buffer in the in-place layout (band data for
+ *                               block-banded, slabs for block-dense; rank 0 also writes the zeros of columns without a valid
+ *                               colour); the root then compacts every entry of E into `out`;
  *   FDB_OOP_SPARSE, no sparsity its column block of the m x C candidates at offset col_begin*m; the root then compacts all
  *                               m*C of them.
  * Per rank: forward mode without d_f_in evaluates f(x) first, then its own colours ascending; central f(x+) then f(x-) per
@@ -564,6 +576,11 @@ fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, cons
                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_oop_plan_create_banded(fdb_plan **plan, int64_t m, int64_t n, int64_t l, int64_t u, const int64_t *colorvec,
                                       int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_oop_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                            int64_t lam, int64_t mu, const int64_t *colorvec, int result_kind, int64_t ldJ,
+                                            const fdb_plan_opts *opts);
+fdb_status fdb_oop_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
+                                           const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_jacobian_oop(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream);
 fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
@@ -588,6 +605,12 @@ fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const in
 fdb_status fdb_group_create_oop_banded(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n, int64_t l,
                                        int64_t u, const int64_t *colorvec, int result_kind, int64_t ldJ,
                                        const fdb_plan_opts *opts);
+fdb_status fdb_group_create_oop_block_banded(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                            const int64_t *blocks, int64_t l, int64_t u, int64_t lam, int64_t mu,
+                                            const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_group_create_oop_block_dense(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
+                                           const int64_t *blocks, int64_t l, int64_t u, const int64_t *colorvec,
+                                           int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_group_jacobian_oop(fdb_group *group, fdb_fn f, void *const *ctx, const double *d_x, const fdb_oop_out *out,
                                   double *d_fx, const double *d_f_in, double relstep, double absstep, double dir,
                                   void *stream);
