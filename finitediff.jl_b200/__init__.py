@@ -14,7 +14,7 @@ The directory name contains a dot, so it is imported through _bootstrap.py (repo
 `finitediff_jl_b200`.
 """
 from . import _lib  # noqa: F401
-from .api import (BandedBlockBandedMatrix, BandedMatrix, BlockBandedMatrix, BlockSkylineMatrix, DenseColumnBlock, JacobianCache, JVPCache, NativeFn, Plan, SparseMatrixCSC, Tridiagonal, compute_epsilon,
+from .api import (BandedBlockBandedMatrix, BandedMatrix, BlockBandedMatrix, BlockSkylineMatrix, DenseColumnBlock, JacobianCache, JVPCache, NativeFn, Plan, SparseMatrixCSC, SparseMatrixCSR, Tridiagonal, compute_epsilon,
                   Diagonal, Bidiagonal, SymTridiagonal,
                   default_relstep, finite_difference_jacobian_, finite_difference_jacobian_b, finite_difference_jvp_,
                   check_coloring, make_plan, matrix_colors, pinned_empty, resize_, zeros_colmajor,
@@ -23,7 +23,7 @@ from .api import (BandedBlockBandedMatrix, BandedMatrix, BlockBandedMatrix, Bloc
                   DerivativeCache, finite_difference_derivative_, finite_difference_derivative,
                   finite_difference_jacobian, finite_difference_jvp)
 
-__all__ = ["BandedBlockBandedMatrix", "BandedMatrix", "BlockBandedMatrix", "BlockSkylineMatrix", "DenseColumnBlock", "JacobianCache", "JVPCache", "finite_difference_jvp_", "NativeFn", "Plan", "SparseMatrixCSC", "Tridiagonal", "compute_epsilon",
+__all__ = ["BandedBlockBandedMatrix", "BandedMatrix", "BlockBandedMatrix", "BlockSkylineMatrix", "DenseColumnBlock", "JacobianCache", "JVPCache", "finite_difference_jvp_", "NativeFn", "Plan", "SparseMatrixCSC", "SparseMatrixCSR", "Tridiagonal", "compute_epsilon",
            "Diagonal", "Bidiagonal", "SymTridiagonal",
            "default_relstep", "finite_difference_jacobian_", "finite_difference_jacobian_b", "make_plan", "matrix_colors", "check_coloring",
            "pinned_empty", "resize_", "zeros_colmajor", "HessianCache", "finite_difference_hessian_",

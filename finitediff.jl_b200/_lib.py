@@ -17,6 +17,7 @@ FDB_OK, FDB_ERR_INVALID, FDB_ERR_CUDA, FDB_ERR_CALLBACK, FDB_ERR_NOMEM, FDB_ERR_
 FDB_FORWARD, FDB_CENTRAL, FDB_COMPLEX, FDB_HCENTRAL = 0, 1, 2, 3
 FDB_J_CSC_NZVAL, FDB_J_DENSE, FDB_J_BAND, FDB_J_SLOTS, FDB_J_BLOCK_BAND, FDB_J_DIAGONALS = 0, 1, 2, 3, 4, 5
 FDB_J_BLOCK_DENSE = 6
+FDB_J_CSR = 7
 FDB_OOP_RAW, FDB_OOP_DENSE, FDB_OOP_SPARSE = 0, 1, 2
 # FDB_STEP_DEFAULT: relstep / absstep keyword not given (any other value, 0 included, is used as passed)
 STEP_DEFAULT = float("nan")
@@ -76,6 +77,7 @@ ABI_SYMBOLS = {
     "fdb_plan_create_banded": (_int, [_PP, _i64, _i64, _i64, _i64, _int, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_block_banded": (_int, [_PP, _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_block_dense": (_int, [_PP, _i64, _vp, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
+    "fdb_plan_create_csr": (_int, [_PP, _i64, _i64, _vp, _vp, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_create_dense": (_int, [_PP, _i64, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_plan_create_dense_colorvec": (_int, [_PP, _i64, _i64, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_plan_destroy": (_int, [_vp]),
@@ -94,6 +96,7 @@ ABI_SYMBOLS = {
     "fdb_color_eps": (_int, [_vp, _vp, _f64, _f64, _f64, _vp, _vp]),
     "fdb_plan_set_external_eps": (_int, [_vp, _vp]),
     "fdb_group_create_csc": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _vp, _vp, _int, _vp, _vp, _i64, _vp, C.POINTER(PlanOpts)]),
+    "fdb_group_create_csr": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _vp, _vp, _vp, C.POINTER(PlanOpts)]),
     "fdb_group_create_banded": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _i64, _i64, _int, _i64, _vp, C.POINTER(PlanOpts)]),
     "fdb_group_create_dense": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_group_create_block_banded": (_int, [_PP, _int, C.POINTER(_int), _i64, _vp, _i64, _i64, _i64, _i64, _i64, _vp,
@@ -112,6 +115,8 @@ ABI_SYMBOLS = {
     "fdb_matrix_colors_banded": (_int, [_i64, _i64, _i64, _vp, _vp]),
     "fdb_matrix_colors_csc": (_int, [_i64, _i64, _vp, _vp, _vp, C.POINTER(_i64), C.POINTER(_i64)]),
     "fdb_check_coloring_csc": (_int, [_i64, _i64, _vp, _vp, _vp, C.POINTER(_i64)]),
+    "fdb_matrix_colors_csr": (_int, [_i64, _i64, _vp, _vp, _vp, C.POINTER(_i64), C.POINTER(_i64)]),
+    "fdb_check_coloring_csr": (_int, [_i64, _i64, _vp, _vp, _vp, C.POINTER(_i64)]),
     "fdb_jvp_plan_create": (_int, [_PP, _i64, _i64, C.POINTER(PlanOpts)]),
     "fdb_jvp": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f64, _f64, _f64, _vp]),
     "fdb_oop_plan_create_csc": (_int, [_PP, _i64, _i64, _vp, _vp, _vp, _int, _i64, C.POINTER(PlanOpts)]),

@@ -32,7 +32,7 @@ from . import _lib as L
 
 __all__ = [
     "SparseMatrixCSC", "BandedMatrix", "Tridiagonal", "Diagonal", "Bidiagonal", "SymTridiagonal", "BandedBlockBandedMatrix",
-    "BlockSkylineMatrix", "DenseColumnBlock", "NativeFn", "JacobianCache", "Plan",
+    "BlockSkylineMatrix", "DenseColumnBlock", "SparseMatrixCSR", "NativeFn", "JacobianCache", "Plan",
     "finite_difference_jacobian_", "finite_difference_jacobian_b", "resize_", "default_relstep", "compute_epsilon",
     "zeros_colmajor", "pinned_empty", "HessianCache", "finite_difference_hessian_", "finite_difference_hessian",
     "GradientCache", "finite_difference_gradient_", "finite_difference_gradient", "DerivativeCache",
@@ -196,6 +196,56 @@ class SparseMatrixCSC:
         nz = self.nzval.cpu().numpy() if isinstance(self.nzval, torch.Tensor) else np.asarray(self.nzval)
         import scipy.sparse as sp
         return sp.csc_matrix((nz, rv, cp), shape=(self.m, self.n)).toarray()
+
+
+class SparseMatrixCSR:
+    """Mirror of a row-compressed sparse matrix (CUDA.jl's CuSparseMatrixCSR{Float64} with Int64 indices, the input format
+    of cuSPARSE, cuDSS and AMGX): m, n, rowptr[m+1], colval[nnz] (Int64, 1-based), nzval[nnz] (float64).  Columns within a
+    row may come in any order and an (r, c) may repeat: each stored entry is its own slot of nzval."""
+
+    def __init__(self, m, n, rowptr, colval, nzval):
+        self.m, self.n = int(m), int(n)
+        self.rowptr, self.colval, self.nzval = rowptr, colval, nzval
+
+    @property
+    def shape(self):
+        return (self.m, self.n)
+
+    @property
+    def nnz(self):
+        return int(self.colval.shape[0]) if hasattr(self.colval, "shape") else len(self.colval)
+
+    @staticmethod
+    def from_scipy(A, device="cuda", index_device=None):
+        """The CSR of A as scipy stores it: its column order within a row (and its duplicates) are kept."""
+        import scipy.sparse as sp
+        A = A if sp.isspmatrix_csr(A) or isinstance(A, sp.csr_array) else sp.csr_matrix(A)
+        rowptr = torch.from_numpy(A.indptr.astype(np.int64) + 1)
+        colval = torch.from_numpy(A.indices.astype(np.int64) + 1)
+        if index_device is not None:
+            rowptr, colval = rowptr.to(index_device), colval.to(index_device)
+        nz = torch.zeros(A.nnz, dtype=torch.float64, device=device) if device != "host" else np.zeros(A.nnz)
+        return SparseMatrixCSR(A.shape[0], A.shape[1], rowptr, colval, nz)
+
+    def similar(self):
+        nz = torch.empty_like(self.nzval) if isinstance(self.nzval, torch.Tensor) else np.empty_like(self.nzval)
+        return SparseMatrixCSR(self.m, self.n, self.rowptr, self.colval, nz)
+
+    def findstructralnz(self):
+        """(rows, cols), 1-based, one per stored entry in storage order: the entry list of the slot route, whose slots
+        are 1:nnz."""
+        rp = np.asarray(self.rowptr.cpu() if isinstance(self.rowptr, torch.Tensor) else self.rowptr, dtype=np.int64)
+        cv = np.asarray(self.colval.cpu() if isinstance(self.colval, torch.Tensor) else self.colval, dtype=np.int64)
+        rows = np.repeat(np.arange(1, self.m + 1, dtype=np.int64), np.diff(rp))
+        return rows, cv.copy()
+
+    def to_dense(self) -> np.ndarray:
+        """Dense copy; a repeated (r, c) shows the value of its last slot."""
+        rows, cols = self.findstructralnz()
+        nz = self.nzval.cpu().numpy() if isinstance(self.nzval, torch.Tensor) else np.asarray(self.nzval)
+        out = np.zeros((self.m, self.n))
+        out[rows - 1, cols - 1] = nz[: len(rows)]
+        return out
 
 
 class BandedMatrix:
@@ -777,6 +827,8 @@ def _plan_route(J, sparsity, colorvec):
         # Diagonal / Bidiagonal / SymTridiagonal sparsity: the banded plan with the band (l, u) of the type, into the packed
         # diagonal storage of the same type or into a dense J
         return "banded", (*diag_route, cv_ptr), keep
+    if isinstance(J, SparseMatrixCSR) and not isinstance(sparsity, SparseMatrixCSR):
+        raise TypeError(f"not built: a SparseMatrixCSR J with a {type(sparsity).__name__} sparsity")
     if sparsity is None:
         # dense column branch (jacobians.jl:548-557): column i of J from perturbing component i, colorvec = 1:n.
         # With sparsity === nothing and any OTHER colorvec the reference loops color_i in 1:maximum(colorvec) and
@@ -804,6 +856,22 @@ def _plan_route(J, sparsity, colorvec):
                 raise ValueError("size(J) != size(sparsity)")
             return "csc", (m, n, cp, rv, L.FDB_J_DENSE, None, None, ld, cv_ptr), keep
         raise TypeError(f"unsupported J type {type(J)} for a SparseMatrixCSC sparsity")
+    if isinstance(sparsity, SparseMatrixCSR):
+        if isinstance(J, SparseMatrixCSR):
+            # J's own pattern: the nzval scatter (rowptr / colval / nzval as the solver holds them)
+            if not (J is sparsity or (J.rowptr is sparsity.rowptr and J.colval is sparsity.colval) or _same_csr(J, sparsity)):
+                raise TypeError("not built: a SparseMatrixCSR J with a different pattern than its sparsity")
+            rp, k1 = _index_ptr(J.rowptr)
+            cv, k2 = _index_ptr(J.colval)
+            return "csr", (J.m, J.n, rp, cv, cv_ptr), keep + [k1, k2]
+        if isinstance(J, torch.Tensor):
+            rows, cols = sparsity.findstructralnz()
+            m, nn, ld = _dense_ld(J)
+            if (m, nn) != (sparsity.m, sparsity.n):
+                raise ValueError("size(J) != size(sparsity)")
+            return "coo", (m, nn, len(rows), rows.ctypes.data, cols.ctypes.data, L.FDB_J_DENSE, None, ld, cv_ptr), \
+                keep + [rows, cols]
+        raise TypeError(f"not built: J of type {type(J).__name__} with a SparseMatrixCSR sparsity")
     if isinstance(sparsity, BandedMatrix):
         if isinstance(J, BandedMatrix):
             if (J.l, J.u) != (sparsity.l, sparsity.u):
@@ -874,6 +942,13 @@ def _plan_route(J, sparsity, colorvec):
         keep + [rows, cols, slots]
 
 
+def _same_csr(A, B) -> bool:
+    """A and B are CSRs with the same size, row pointer and columns (the same pattern in the same storage order)."""
+    def host(a):
+        return np.asarray(a.cpu() if isinstance(a, torch.Tensor) else a, dtype=np.int64)
+    return A.shape == B.shape and np.array_equal(host(A.rowptr), host(B.rowptr)) and np.array_equal(host(A.colval), host(B.colval))
+
+
 def make_plan(J, sparsity, colorvec, fdtype, x_len: int, device, **plan_kw) -> Plan:
     """Create the fdb_plan for (typeof(J), sparsity, colorvec, fdtype) by the creator _plan_route chooses."""
     kind, args, keep = _plan_route(J, sparsity, colorvec)
@@ -932,12 +1007,12 @@ def _diagonals_route(J, sparsity):
 
 def _has_sparsestruct(J) -> bool:
     """ArrayInterface.has_sparsestruct(J) as used at jacobians.jl:455."""
-    return isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix)
-                      + _LA_BANDED)
+    return isinstance(J, (SparseMatrixCSC, SparseMatrixCSR, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix,
+                          BlockSkylineMatrix) + _LA_BANDED)
 
 
 def _j_values(J):
-    if isinstance(J, SparseMatrixCSC):
+    if isinstance(J, (SparseMatrixCSC, SparseMatrixCSR)):
         return J.nzval
     if isinstance(J, BandedMatrix):
         return J.data
@@ -953,6 +1028,8 @@ def _j_values(J):
 def _j_key(J):
     if isinstance(J, SparseMatrixCSC):
         return ("csc", J.m, J.n, _index_key(J.colptr), _index_key(J.rowval))
+    if isinstance(J, SparseMatrixCSR):
+        return ("csr", J.m, J.n, _index_key(J.rowptr), _index_key(J.colval))
     if isinstance(J, BandedMatrix):
         return ("band", J.m, J.n, J.l, J.u)
     if isinstance(J, Tridiagonal):
@@ -979,7 +1056,8 @@ def _j_key(J):
 def _sp_key(sp):
     if sp is None:
         return None
-    if isinstance(sp, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix) + _LA_BANDED):
+    if isinstance(sp, (SparseMatrixCSC, SparseMatrixCSR, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix,
+                       BlockSkylineMatrix) + _LA_BANDED):
         return _j_key(sp)
     if isinstance(sp, torch.Tensor):
         return ("proto", sp.data_ptr(), tuple(sp.shape), sp._version)
@@ -1088,6 +1166,7 @@ def matrix_colors(A, device=None) -> torch.Tensor:
     `colorvec`.  Tridiagonal and SymTridiagonal -> 1,2,3,...; Diagonal -> all 1; Bidiagonal -> 1,2,1,2,...;
     BandedMatrix(l,u) -> cycle 1:(l+u+1) (ArrayInterface's closed forms);
     SparseMatrixCSC -> a valid distance-2 column colouring (deterministic Jones-Plassmann, fdb_matrix_colors_csc);
+    SparseMatrixCSR -> the same colouring of the same matrix (fdb_matrix_colors_csr);
     dense tensors -> 1:n (ArrayInterface: eachindex of the columns)."""
     lib = L.lib()
     if isinstance(A, Tridiagonal):
@@ -1100,15 +1179,17 @@ def matrix_colors(A, device=None) -> torch.Tensor:
     elif isinstance(A, BandedMatrix):
         n, l, u = A.n, A.l, A.u
         dev = (A.data.device if isinstance(A.data, torch.Tensor) and A.data.is_cuda else torch.device("cuda")) if device is None else torch.device(device)
-    elif isinstance(A, SparseMatrixCSC):
+    elif isinstance(A, (SparseMatrixCSC, SparseMatrixCSR)):
         dev = torch.device("cuda") if device is None else torch.device(device)
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         out = torch.zeros(max(A.n, 1), dtype=torch.int64, device=dev)
-        cp, k1 = _index_ptr(A.colptr)
-        rv, k2 = _index_ptr(A.rowval)
+        csr = isinstance(A, SparseMatrixCSR)
+        cp, k1 = _index_ptr(A.rowptr if csr else A.colptr)
+        rv, k2 = _index_ptr(A.colval if csr else A.rowval)
         nc, nr = C.c_int64(), C.c_int64()
-        _call(dev, (), lib.fdb_matrix_colors_csc, A.m, A.n, cp, rv, out.data_ptr(), C.byref(nc), C.byref(nr))
+        _call(dev, (), lib.fdb_matrix_colors_csr if csr else lib.fdb_matrix_colors_csc, A.m, A.n, cp, rv, out.data_ptr(),
+              C.byref(nc), C.byref(nr))
         out = out[: A.n]
         out.n_colors, out.n_rounds = nc.value, nr.value
         return out
@@ -1126,13 +1207,15 @@ def matrix_colors(A, device=None) -> torch.Tensor:
     return out[:n]
 
 
-def check_coloring(A: "SparseMatrixCSC", colorvec) -> int:
-    """Number of (row, colour) collisions of `colorvec` on the CSC pattern (0 = valid for the decompression)."""
-    cp, k1 = _index_ptr(A.colptr)
-    rv, k2 = _index_ptr(A.rowval)
+def check_coloring(A: "SparseMatrixCSC | SparseMatrixCSR", colorvec) -> int:
+    """Number of (row, colour) collisions of `colorvec` on the CSC or CSR pattern (0 = valid for the decompression)."""
+    csr = isinstance(A, SparseMatrixCSR)
+    cp, k1 = _index_ptr(A.rowptr if csr else A.colptr)
+    rv, k2 = _index_ptr(A.colval if csr else A.rowval)
     cv, k3 = _index_ptr(colorvec)
     out = C.c_int64()
-    L.check(L.lib().fdb_check_coloring_csc(A.m, A.n, cp, rv, cv, C.byref(out)))
+    fn = L.lib().fdb_check_coloring_csr if csr else L.lib().fdb_check_coloring_csc
+    L.check(fn(A.m, A.n, cp, rv, cv, C.byref(out)))
     return out.value
 
 
@@ -1597,7 +1680,8 @@ def finite_difference_jvp(f, x, v, cache=None, f_in=None, *, relstep=None, absst
 
 
 def _shape_of(J):
-    if isinstance(J, (SparseMatrixCSC, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix, DenseColumnBlock)
+    if isinstance(J, (SparseMatrixCSC, SparseMatrixCSR, BandedMatrix, Tridiagonal, BandedBlockBandedMatrix, BlockSkylineMatrix,
+                      DenseColumnBlock)
                   + _LA_BANDED):
         return J.shape
     if isinstance(J, torch.Tensor):

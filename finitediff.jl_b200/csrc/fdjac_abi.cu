@@ -33,6 +33,7 @@
 #include "kernels_derivative.cuh"
 #include "kernels_blockband.cuh"
 #include "kernels_diagonals.cuh"
+#include "kernels_csr.cuh"
 
 using namespace fdb;
 
@@ -62,7 +63,7 @@ static fdb_status fail(fdb_status st, const char *fmt, ...) {
     if (s__ != FDB_OK) return s__;   \
   } while (0)
 
-enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7, SP_DERIV = 8, SP_BLOCKBAND = 9 };
+enum { SP_NONE = 0, SP_CSC = 1, SP_COO = 3, SP_BANDED = 4, SP_JVP = 5, SP_EPS = 6, SP_HESS = 7, SP_DERIV = 8, SP_BLOCKBAND = 9, SP_CSR = 10 };
 
 // Device memory that lives while a plan or a colouring is built: freed when it goes out of scope, unless release()
 // hands it to a plan that keeps it (fdb_plan::adopt).  Declared after the builder's DeviceGuard, it is freed on the
@@ -261,6 +262,11 @@ struct fdb_plan {
     bool cyclic = false;              // colorvec is the block-cyclic closed form of matrix_colors
     int64_t *start = nullptr;         // block-dense: [nblocks + 1] first slot of every block column's slab
   } block_band;
+  // CSR plans (kernels_csr.cuh): the row pointer and the columns, 0-based int32, on the device
+  struct Csr {
+    int32_t *rowptr = nullptr;        // [m + 1]
+    int32_t *colval = nullptr;        // [nnz]
+  } csr;
   // dense plans: this rank's column block [begin, end) and its steps
   struct Columns {
     int64_t begin = 0, end = 0;
@@ -422,7 +428,7 @@ static fdb_status check_call(const fdb_plan *P, Call c) {
   using K = Call;
   const int k = P->sp_kind;
   const bool cplx = P->fdtype == FDB_COMPLEX;
-  const bool colored = k == SP_CSC || k == SP_COO || k == SP_BANDED || k == SP_BLOCKBAND;   // coloured Jacobian plans
+  const bool colored = k == SP_CSC || k == SP_COO || k == SP_BANDED || k == SP_BLOCKBAND || k == SP_CSR;   // coloured Jacobian plans
   const bool jac = c == K::jacobian || c == K::jacobian_complex, oop = c == K::jacobian_oop || c == K::jacobian_oop_complex;
   const bool group = c == K::group_jacobian || c == K::group_jacobian_oop;
   const fdb_status INV = FDB_ERR_INVALID;
@@ -1381,6 +1387,69 @@ fdb_status fdb_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const i
   return finish_plan(owner, plan);
 }
 
+// J a CSR matrix (rowptr, colval, nzval) with the sparsity's own pattern: the nzval scatter of kernels_csr.cuh.  The
+// plan keeps the row pointer and the columns as 0-based int32; J is never zero-filled.
+fdb_status fdb_plan_create_csr(fdb_plan **plan, int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval,
+                               const int64_t *colorvec, const fdb_plan_opts *opts) {
+  PlanPtr owner;
+  TRY(new_plan(plan, owner, opts, m, n));
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  if (!rowptr) return fail(FDB_ERR_INVALID, "rowptr is NULL");
+  P->sp_kind = SP_CSR;
+  P->jkind = FDB_J_CSR;
+  // nnz = rowptr[m]-1: read the first and last elements wherever they live, then check the whole pointer on the device
+  I64View rp, cv;
+  TRY(view_i64(rowptr, m + 1, rp));
+  int64_t first = 1, last = 1;
+  TRY(read_back(&first, rp.d, 1, "reading rowptr[1]"));
+  TRY(read_back(&last, rp.d + m, 1, "reading rowptr[m+1]"));
+  if (first != 1) return fail(FDB_ERR_INVALID, "rowptr[1]=%lld: a CSR row pointer starts at 1", (long long)first);
+  const int64_t nnz = last - 1;
+  if (nnz < 0) return fail(FDB_ERR_INVALID, "rowptr is not a valid CSR row pointer (must start at 1, be non-decreasing, end at nnz+1)");
+  {
+    DevBuf<uint32_t> d_err;
+    TRY(d_err.alloc(1));
+    CU(cudaMemset(d_err.get(), 0, 4));
+    validate_colptr<<<P->grid(m + 1), kThreads>>>(rp.d, m, nnz, d_err.get());
+    uint32_t h = 0;
+    TRY(read_back(&h, d_err.get(), 1, "CSR row pointer"));
+    if (h) return fail(FDB_ERR_INVALID, "rowptr is not a valid CSR row pointer (must start at 1, be non-decreasing, end at nnz+1)");
+  }
+  if (nnz > 0x7FFFFFF0LL) return fail(FDB_ERR_UNSUPPORTED, "nnz=%lld unsupported (must be in [0, 2^31))", (long long)nnz);
+  if (nnz > 0 && !colval) return fail(FDB_ERR_INVALID, "colval is NULL");
+  TRY(view_i64(colval, nnz, cv));
+  P->colors.E = nnz;
+  P->j_len = nnz;
+  TRY(setup_colors(P, colorvec));
+  DevBuf<uint32_t> d_err;
+  DevBuf<unsigned long long> d_cnt;
+  TRY(d_err.alloc(1));
+  TRY(d_cnt.alloc(std::max<int32_t>(P->colors.C, 1)));
+  CU(cudaMemset(d_err.get(), 0, 4));
+  CU(cudaMemset(d_cnt.get(), 0, (size_t)std::max<int32_t>(P->colors.C, 1) * 8));
+  TRY(P->alloc_t(&P->csr.rowptr, (size_t)m + 1));
+  TRY(P->alloc_t(&P->csr.colval, (size_t)std::max<int64_t>(nnz, 1)));
+  csr_rowptr32<<<P->grid(m + 1), kThreads>>>(rp.d, m, P->csr.rowptr);
+  if (nnz > 0) {
+    TRY(dispatch_ct(P->colors.bits, [&](auto tag) -> fdb_status {
+      using CT = decltype(tag);
+      const size_t hsm = P->colors.C <= kPlanSmemColors ? (size_t)std::max<int32_t>(P->colors.C, 1) * sizeof(unsigned int) : 0;
+      csr_plan_pass<CT><<<P->grid(nnz), kThreads, hsm>>>(cv.d, n, nnz, (const CT *)P->colors.jcolor, P->colors.C, P->csr.colval,
+                                                        d_cnt.get(), d_err.get());
+      CU(cudaGetLastError());
+      return FDB_OK;
+    }));
+  }
+  TRY(read_plan_err(d_err.get(), "CSR sparsity"));
+  std::vector<unsigned long long> cnt(std::max<int32_t>(P->colors.C, 1), 0);
+  if (P->colors.C > 0) TRY(read_back(cnt.data(), d_cnt.get(), (size_t)P->colors.C, "colour counts"));
+  TRY(finish_colored_plan(P, opts, cnt));
+  // the CSC plan's SURVEY.md §8(d) model: B_alg = 32*nnz + 16*n + 8 (valid colouring; Int64 indices as at the ABI)
+  P->alg_bytes = 32 * nnz + 16 * n + 8;
+  return finish_plan(owner, plan);
+}
+
 // dense column branch over the leading `ncols` components (ncols == n for the default colorvec = 1:n)
 static fdb_status create_dense(fdb_plan **plan, int64_t m, int64_t n, int64_t ldJ, int64_t ncols, const fdb_plan_opts *opts) {
   PlanPtr owner;
@@ -1530,6 +1599,14 @@ fdb_status fdb_plan_info(const fdb_plan *P, fdb_plan_info_t *info) {
         else if (P->staged.on)   // 16-bit row offsets; every slab row and f(x) row staged once
           info->moved_bytes_scatter = P->colors.E * (2 + (P->staged.packed ? 0 : ct) + 8) + staged_rows;
       }
+    } else if (P->sp_kind == SP_CSR) {
+      // every launch streams the columns, the row pointer and (unless cyclic) the column colours; the entries it owns
+      // gather their slab rows and store their slot once
+      const int64_t launches = std::max<int64_t>(P->scratch.n_groups, 1);
+      const int64_t C = std::max<int32_t>(P->colors.C, 1);
+      const int64_t owned = P->world > 1 ? P->colors.E * (int64_t)P->colors.local.size() / C : P->colors.E;   // approx. share
+      info->moved_bytes_scatter = launches * (4 * P->colors.E + 4 * (P->m + 1) + (P->colors.cyclic ? 0 : P->n * ct)) +
+                                  owned * (8 * slabs_read + 8) + fx_once;
     } else {
       info->moved_bytes_scatter = P->alg_bytes;
     }
@@ -1653,13 +1730,14 @@ static fdb_status zero_J(const fdb_plan *P, double *J, cudaStream_t s) {
 // How a coloured plan turns a group's f! outputs into J: one launcher per family (scatter_lists ... scatter_entries), and
 // none for an out-of-place sparse result whose compaction forms the quotients itself (fdjac_oop.cuh).  Fixed once the
 // plan is built, but derived rather than stored: the out-of-place creators set oop.fused after the in-place creator.
-enum class Scatter { none, lists, block_band, block_dense, diagonals, band, entries };
+enum class Scatter { none, lists, block_band, block_dense, diagonals, band, csr, entries };
 
 static Scatter scatter_family(const fdb_plan *P) {
   if (P->oop.fused) return Scatter::none;
   if (P->sp_kind == SP_CSC && P->entries.strategy == 1) return Scatter::lists;
   if (P->sp_kind == SP_BLOCKBAND) return P->jkind == FDB_J_BLOCK_DENSE ? Scatter::block_dense : Scatter::block_band;
   if (P->sp_kind == SP_BANDED) return P->jkind == FDB_J_DIAGONALS ? Scatter::diagonals : Scatter::band;
+  if (P->sp_kind == SP_CSR) return Scatter::csr;
   return Scatter::entries;
 }
 
@@ -1668,7 +1746,7 @@ static Scatter scatter_family(const fdb_plan *P) {
 // out-of-place plan stores no candidate, and its candidate buffer is not J-sized: nothing to fill.
 static bool scatter_defines_J(const fdb_plan *P, int64_t colours) {
   const Scatter f = scatter_family(P);
-  if (f == Scatter::none || f == Scatter::block_band || f == Scatter::block_dense) return true;
+  if (f == Scatter::none || f == Scatter::block_band || f == Scatter::block_dense || f == Scatter::csr) return true;
   if (f == Scatter::band && P->jkind != FDB_J_BAND) return false;   // a dense J
   if ((f == Scatter::lists || f == Scatter::entries) && P->entries.dest != nullptr) return false;   // explicit destinations
   return colours > 0;
@@ -1902,6 +1980,30 @@ static fdb_status scatter_diagonals(const ScatterGroup &g) {
   });
 }
 
+// CSR nzval: every entry of the columns of the group's colours, and (first group of rank 0) of the columns without a
+// valid colour: storage order, row from the row pointer
+template <typename CT, int MODE>
+static fdb_status scatter_csr(const ScatterGroup &g) {
+  fdb_plan *P = g.P;
+  CsrArgs a{};
+  a.rowptr = P->csr.rowptr; a.colval = P->csr.colval; a.fx = g.fx; a.Fp = g.Fp; a.Fm = g.Fm; a.eps = P->steps.eps;
+  a.local_of = P->colors.local_of; a.J = g.J; a.ldF = g.ldF;
+  a.m = (int32_t)P->m; a.nnz = (int32_t)P->j_len;
+  a.C = P->colors.C; a.l0 = (int32_t)g.l0; a.G = (int32_t)g.G;
+  // single group on a single rank: every valid colour is resident at its own slab (the first group of rank 0)
+  a.full = P->scratch.n_groups == 1 && P->world == 1 ? 1 : 0;
+  a.write_other = g.first ? 1 : 0;
+  const size_t sm = color_table_smem(P);
+  const int64_t tiles = (P->j_len + kCsrTile - 1) / kCsrTile;
+  ScatterTimer tm(P, g.s);
+  return dispatch_colors<CT>(P, [&](auto cs) -> fdb_status {
+    using CS = decltype(cs);
+    const int grid = oversubscribed_grid(P, diff_scatter_csr<CS, MODE>, sm, tiles, 16);
+    diff_scatter_csr<CS, MODE><<<grid, kThreads, sm, g.s>>>(a, cs);
+    return FDB_OK;
+  });
+}
+
 // band data or a dense J of a banded sparsity: one timed region per group, the pre-division pass (when used) and the
 // band kernel
 template <typename CT, int MODE>
@@ -2023,9 +2125,10 @@ static fdb_status scatter(Scatter family, const ScatterGroup &g) {
   // colour-major lists: rank 0 zeroes the entries of the columns without a valid colour with its first group; owning no
   // colour, it does so only where this call does not zero-fill J (peer stores, a shared J)
   if (family == Scatter::lists && g.first && (g.G > 0 || P->peers.n > 0 || P->shared_J)) zero_uncoloured_slots(g);
-  // a rank that owns no colour launches the block-banded or block-dense scatter of rank 0 alone: the columns without a
-  // valid colour
-  if (g.G == 0 && !((family == Scatter::block_band || family == Scatter::block_dense) && g.first)) return FDB_OK;
+  // a rank that owns no colour launches the block-banded, block-dense or CSR scatter of rank 0 alone: the columns without
+  // a valid colour
+  const bool self_defining = family == Scatter::block_band || family == Scatter::block_dense || family == Scatter::csr;
+  if (g.G == 0 && !(self_defining && g.first)) return FDB_OK;
   switch (family) {   // (a group has a colour: C > 0 and n > 0, so band and diagonal storage have slots)
     case Scatter::none: return FDB_OK;
     case Scatter::lists:
@@ -2035,6 +2138,7 @@ static fdb_status scatter(Scatter family, const ScatterGroup &g) {
     case Scatter::block_dense: if (P->j_len == 0) return FDB_OK; TRY((scatter_block_dense<CT, MODE>(g))); break;
     case Scatter::diagonals: TRY((scatter_diagonals<CT, MODE>(g))); break;
     case Scatter::band: TRY((scatter_band<CT, MODE>(g))); break;
+    case Scatter::csr: if (P->j_len == 0) return FDB_OK; TRY((scatter_csr<CT, MODE>(g))); break;
     case Scatter::entries: if (P->colors.E == 0) return FDB_OK; TRY((scatter_entries<CT, MODE>(g))); break;
   }
   P->cnt.kernel_launches += 1;

@@ -215,6 +215,13 @@ fdb_status fdb_group_create_block_dense(fdb_group **group, int n_devices, const 
   });
 }
 
+fdb_status fdb_group_create_csr(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_plan_create_csr(p, m, n, rowptr, colval, colorvec, o);
+  });
+}
+
 fdb_status fdb_group_destroy(fdb_group *group) {
   free_group(group);
   return FDB_OK;
@@ -454,6 +461,57 @@ fdb_status fdb_check_coloring_csc(int64_t m, int64_t n, const int64_t *colptr, c
   TRY(read_back(&h, d_c.get(), 1, "conflict count"));
   *n_conflicts = (int64_t)h;
   return FDB_OK;
+}
+
+}  // extern "C"
+
+// The CSC (Int64, 1-based, device) of a CSR pattern (rowptr[m+1], colval[nnz], Int64 1-based, host or device): the CSR
+// read as the CSC of the transpose, whose row-compressed form build_csr_pattern builds.
+struct CscOfCsr {
+  DevBuf<int64_t> colptr, rowval;
+};
+
+static fdb_status csc_of_csr(int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval, CscOfCsr &out) {
+  if (!rowptr) return fail(FDB_ERR_INVALID, "rowptr is NULL");
+  CsrPattern T;
+  if (build_csr_pattern(n, m, rowptr, colval, T) != FDB_OK)
+    return fail(FDB_ERR_INVALID, "invalid CSR pattern (%s)", fdb_last_error());
+  TRY(out.colptr.alloc((size_t)n + 1));
+  TRY(out.rowval.alloc((size_t)std::max<int64_t>(T.nnz, 1)));
+  const int gb = (int)std::max<int64_t>(1, std::min<int64_t>((std::max<int64_t>(T.nnz, n + 1) + kThreads - 1) / kThreads, 132 * 16));
+  widen_index<<<gb, kThreads>>>(T.rowptr.get(), n + 1, out.colptr.get());
+  if (T.nnz > 0) widen_index<<<gb, kThreads>>>(T.rcols.get(), T.nnz, out.rowval.get());
+  CU(cudaDeviceSynchronize());
+  return FDB_OK;
+}
+
+extern "C" {
+
+// the colouring of fdb_matrix_colors_csc on the same matrix: it depends on the pattern alone
+fdb_status fdb_matrix_colors_csr(int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval, int64_t *d_colorvec,
+                                 int64_t *n_colors, int64_t *n_rounds) {
+  if (n > 0 && !d_colorvec) return fail(FDB_ERR_INVALID, "colorvec is NULL");
+  int dev = 0;
+  TRY(check_device(nullptr, &dev));
+  if (n_colors) *n_colors = 0;
+  if (n_rounds) *n_rounds = 0;
+  if (n == 0) return FDB_OK;
+  CscOfCsr T;
+  TRY(csc_of_csr(m, n, rowptr, colval, T));
+  return fdb_matrix_colors_csc(m, n, T.colptr.get(), T.rowval.get(), d_colorvec, n_colors, n_rounds);
+}
+
+fdb_status fdb_check_coloring_csr(int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec,
+                                  int64_t *n_conflicts) {
+  if (!n_conflicts) return fail(FDB_ERR_INVALID, "NULL argument");
+  *n_conflicts = 0;
+  int dev = 0;
+  TRY(check_device(nullptr, &dev));
+  if (n == 0 || m == 0) return FDB_OK;
+  if (!colorvec) return FDB_OK;                     // 1:n: every column its own colour
+  CscOfCsr T;
+  TRY(csc_of_csr(m, n, rowptr, colval, T));
+  return fdb_check_coloring_csc(m, n, T.colptr.get(), T.rowval.get(), colorvec, n_conflicts);
 }
 
 }  // extern "C"

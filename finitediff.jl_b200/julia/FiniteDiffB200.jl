@@ -149,6 +149,22 @@ end
 Base.size(J::DeviceBlockDense) = (sum(J.blocks), sum(J.blocks))
 Base.size(J::DeviceBlockDense, d) = sum(J.blocks)
 
+# A row-compressed sparse matrix on the device (the format of cuSPARSE, cuDSS and AMGX): Int64 1-based row pointer and
+# columns on the device, nzval the Jacobian's values (FDB_J_CSR: J and the sparsity are this one pattern)
+struct DeviceCSR
+    m::Int
+    n::Int
+    rowptr::CuVector{Int64}                  # m + 1
+    colval::CuVector{Int64}                  # nnz
+    nzval::CuVector{Float64}                 # nnz
+end
+Base.size(J::DeviceCSR) = (J.m, J.n)
+Base.size(J::DeviceCSR, d) = d == 1 ? J.m : J.n
+# CUDA.jl's CuSparseMatrixCSR{Float64}: its Cint indices are widened on the device once per wrapper; nzVal is aliased, so
+# the Jacobian is written in place into the matrix the solver holds
+DeviceCSR(A::CUDA.CUSPARSE.CuSparseMatrixCSR{Float64}) =
+    DeviceCSR(size(A, 1), size(A, 2), CuVector{Int64}(A.rowPtr), CuVector{Int64}(A.colVal), A.nzVal)
+
 struct DeviceTridiagonal                     # LinearAlgebra.Tridiagonal(dl, d, du): one buffer [dl; d; du]
     n::Int
     buf::CuVector{Float64}                   # 3n - 2
@@ -347,6 +363,24 @@ function plan_block_dense(J::DeviceBlockDense, colorvec, fd::Cint; kw...)
     end
 end
 
+# J and sparsity one CSR pattern: the nzval scatter, indices read from the device (ext/FiniteDiffSparseArraysExt.jl:20-28 on a
+# row-compressed target)
+function plan_csr(J::DeviceCSR, colorvec, fd::Cint; kw...)
+    key = (:csr, J.m, J.n, objectid(J.rowptr), objectid(J.colval), color_key(colorvec), fd, values(kw))
+    cached_plan(J.nzval, key) do
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd; kw...))
+        cptr, croot = color_arg(colorvec, J.n)
+        rowptr, colval = J.rowptr, J.colval
+        GC.@preserve rowptr colval croot begin
+            check(ccall((:fdb_plan_create_csr, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Ptr{Int64}, Ref{PlanOpts}),
+                h, J.m, J.n, pointer(rowptr), pointer(colval), cptr, opts))
+        end
+        Plan(h[], (rowptr, colval, croot))
+    end
+end
+
 # sparsity === nothing: dense column branch; a non-default colorvec reproduces jacobians.jl:547-557 as written
 function plan_dense(anchor, m::Integer, n::Integer, ldJ::Integer, colorvec, fd::Cint; kw...)
     key = (:dense, m, n, ldJ, color_key(colorvec), fd, values(kw))
@@ -435,7 +469,7 @@ function run_plan!(plan::Plan, jvals::CuArray{Float64}, f, x::CuVector{Float64},
     nothing                                  # jacobians.jl:652
 end
 
-const DeviceJ = Union{DeviceCSC, DeviceBanded, DeviceBlockBanded, DeviceBlockDense, DeviceTridiagonal, DeviceDiagonal, DeviceBidiagonal,
+const DeviceJ = Union{DeviceCSC, DeviceCSR, DeviceBanded, DeviceBlockBanded, DeviceBlockDense, DeviceTridiagonal, DeviceDiagonal, DeviceBidiagonal,
     CuMatrix{Float64}}
 
 ld(J::CuMatrix) = max(stride(J, 2), size(J, 1), 1)
@@ -446,6 +480,11 @@ function plan_for(J::DeviceCSC, sp, colorvec, fd)
     sph = sp isa DeviceCSC ? sp.host : sp
     sph isa SparseMatrixCSC || throw(ArgumentError("a DeviceCSC Jacobian needs a SparseMatrixCSC sparsity"))
     (plan_csc(sph, J.host, 0, colorvec, fd), J.nzval)
+end
+function plan_for(J::DeviceCSR, sp, colorvec, fd)
+    (sp === J || (sp isa DeviceCSR && sp.rowptr === J.rowptr && sp.colval === J.colval)) ||
+        throw(ArgumentError("not built: a DeviceCSR Jacobian with another sparsity than its own pattern"))
+    (plan_csr(J, colorvec, fd), J.nzval)
 end
 function plan_for(J::DeviceBanded, sp, colorvec, fd)
     (sp isa DeviceBanded && (sp.l, sp.u) == (J.l, J.u)) || throw(ArgumentError("J and sparsity must have the same bandwidths"))
@@ -807,6 +846,19 @@ function group_block_dense(J::DeviceBlockDense, colorvec, fdtype, devices::Vecto
             h, length(devices), pointer(devices), length(blocks), pointer(blocks), J.l, J.u, length(J.data), cptr, opts))
     end
     Group(h[], length(devices), (blocks, croot))
+end
+
+function group_csr(J::DeviceCSR, colorvec, fdtype, devices::Vector{Cint}; kw...)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, J.n)
+    rowptr, colval = J.rowptr, J.colval
+    GC.@preserve rowptr colval croot devices begin
+        check(ccall((:fdb_group_create_csr, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Ptr{Int64}, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), J.m, J.n, pointer(rowptr), pointer(colval), cptr, opts))
+    end
+    Group(h[], length(devices), (rowptr, colval, croot))
 end
 
 function group_dense(J::CuMatrix{Float64}, fdtype, devices::Vector{Cint}; kw...)

@@ -60,10 +60,12 @@ typedef enum {
   FDB_J_SLOTS = 3,     /* structured J (e.g. Tridiagonal): explicit 1-based slot per structural entry (iteration_utils.jl:25-32) */
   FDB_J_BLOCK_BAND = 4, /* J::BandedBlockBandedMatrix band data, (l+u+1)(lam+mu+1) slots per column (fdb_plan_create_block_banded) */
   FDB_J_DIAGONALS = 5, /* J::Diagonal / Bidiagonal / Tridiagonal storage: the stored diagonals packed in one buffer (fdb_plan_create_banded) */
-  FDB_J_BLOCK_DENSE = 6 /* J::BlockBandedMatrix data, one column-major slab per block column (fdb_plan_create_block_dense):
+  FDB_J_BLOCK_DENSE = 6, /* J::BlockBandedMatrix data, one column-major slab per block column (fdb_plan_create_block_dense):
                            entry (r, c) of block (K, J), 0-based, at slot start_J + c*h_J + (rowoff_J(K) + r), where
                            h_J = sum of the sizes of block rows max(0, J-u)..min(N-1, J+l), start_J = sum_{J'<J} h_J'*cb[J']
                            and rowoff_J(K) = the sizes of block rows max(0, J-u)..K-1 */
+  FDB_J_CSR = 7         /* J is the nzval of a CSR matrix with the sparsity's own pattern: entry s of row r, column colval[s],
+                           at nzval[s] (fdb_plan_create_csr) */
 } fdb_jkind;
 
 /*
@@ -155,7 +157,7 @@ double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep,
 /* ---- plans: the per-(pattern, colorvec, fdtype) state the reference rebuilds on every call
  *      (jacobians.jl:515-535: colour reshape, findstructralnz, same-pattern test) ---- */
 
-/* Which plans each call takes.  Coloured plans: fdb_plan_create_csc / _coo / _banded / _block_banded / _block_dense; dense plans:
+/* Which plans each call takes.  Coloured plans: fdb_plan_create_csc / _coo / _banded / _block_banded / _block_dense / _csr; dense plans:
  * fdb_plan_create_dense / _dense_colorvec; out-of-place plans: fdb_oop_plan_create_*.  Any other plan is refused with
  * FDB_ERR_INVALID (FDB_ERR_UNSUPPORTED where noted) before the call allocates, launches or calls f.
  *   fdb_jacobian, fdb_jacobian_host   coloured and dense plans, fdtype forward / central
@@ -248,6 +250,24 @@ fdb_status fdb_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, const 
  * moved_bytes_scatter = 8*j_len + 16*n*C. */
 fdb_status fdb_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
                                        int64_t ldata, const int64_t *colorvec, const fdb_plan_opts *opts);
+
+/* sparsity and J: one CSR matrix (m x n, rowptr[m+1], colval[nnz]; Int64, 1-based, host or device), J its nzval — the generic
+ * J[r, c] = v hook (ext/FiniteDiffSparseArraysExt.jl:20-28, iteration_utils.jl:25-32) on a row-compressed target, the format
+ * GPU sparse solvers take.  Columns within a row may come in any order; a repeated (r, c) is allowed and each of its slots
+ * gets the value.  Every call writes every one of the nnz slots exactly once — the quotient of the column's colour, +0.0
+ * when the column has no valid colour — so J is never zero-filled; slots past nnz are not touched.  Values, f! calls and
+ * f! points are those of the slot route (fdb_plan_create_coo with FDB_J_SLOTS, the CSR's rows and columns and slots 1..nnz)
+ * on the same buffer, for any colouring.  opts as for the other coloured plans (forward / central / complex, max_batch,
+ * scratch_bytes, no_drift, use_graph, rank / world / partition, shared_j, fdb_color_eps, fdb_plan_set_external_eps);
+ * fdb_plan_set_peers is FDB_ERR_UNSUPPORTED.  A rank plan writes the slots of its own colours (rank 0 also those of the
+ * columns without a valid colour), so the ranks together write every slot once and nobody zero-fills J.  A NULL rowptr,
+ * rowptr[1] != 1, a decreasing rowptr, a column outside 1..n or negative sizes: FDB_ERR_INVALID; nnz >= 2^31:
+ * FDB_ERR_UNSUPPORTED; both before any f! call.  fdb_plan_info: jkind FDB_J_CSR, n_entries = j_len = nnz,
+ * alg_bytes_scatter = 32*nnz + 16*n + 8 (as for CSC), moved_bytes_scatter = G*(4*nnz + 4*(m+1) + |colour|*n) + E_own*(8*slabs_read
+ * + 8) [+ 8m, forward] with G scatter launches (n_groups), |colour| = 0 for a cyclic colouring and E_own the entries of the
+ * rank's colours (nnz on one rank). */
+fdb_status fdb_plan_create_csr(fdb_plan **plan, int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval,
+                               const int64_t *colorvec, const fdb_plan_opts *opts);
 
 /* sparsity === nothing: dense column branch jacobians.jl:548-557,590-598 (colorvec = 1:n; per-component step).
  * With world>1 the columns are block-partitioned: this rank computes columns [col_begin, col_end) (0-based, see
@@ -362,6 +382,10 @@ fdb_status fdb_group_create_block_banded(fdb_group **group, int n_devices, const
 fdb_status fdb_group_create_block_dense(fdb_group **group, int n_devices, const int *devices, int64_t nblocks,
                                         const int64_t *blocks, int64_t l, int64_t u, int64_t ldata, const int64_t *colorvec,
                                         const fdb_plan_opts *opts);
+/* CSR groups: member i writes the slots of its own colours straight into the root's nzval, member 0 also those of the
+ * columns without a valid colour; J is never zero-filled. */
+fdb_status fdb_group_create_csr(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec, const fdb_plan_opts *opts);
 fdb_status fdb_group_destroy(fdb_group *group);
 fdb_status fdb_group_size(const fdb_group *group, int *n_members);
 /* member i's plan (owned by the group): fdb_plan_info / fdb_plan_counters / fdb_plan_get_eps / fdb_plan_color_owner */
@@ -394,11 +418,18 @@ fdb_status fdb_sync_destroy(fdb_sync *sync);
  *        csc      a valid distance-2 colouring of the columns (no two columns of one colour share a row) by a
  *                 deterministic Jones-Plassmann sweep; the result depends on the pattern alone.  colptr / rowval: Int64,
  *                 1-based, host or device.  n_colors / n_rounds (host, nullable) receive maximum(colorvec) / sweeps.
- *        check    number of (row, colour) collisions of a colouring (0 = valid for this path's decompression). */
+ *        check    number of (row, colour) collisions of a colouring (0 = valid for this path's decompression).
+ *        csr      the same two operations on a CSR pattern (rowptr[m+1], colval[nnz]; Int64, 1-based, host or device): the
+ *                 column -> rows adjacency is built on the device, and the colorvec equals fdb_matrix_colors_csc's on the
+ *                 same matrix element for element. */
 fdb_status fdb_matrix_colors_banded(int64_t n, int64_t l, int64_t u, int64_t *d_colorvec, void *stream);
 fdb_status fdb_matrix_colors_csc(int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval, int64_t *d_colorvec,
                                  int64_t *n_colors, int64_t *n_rounds);
 fdb_status fdb_check_coloring_csc(int64_t m, int64_t n, const int64_t *colptr, const int64_t *rowval, const int64_t *colorvec,
+                                  int64_t *n_conflicts);
+fdb_status fdb_matrix_colors_csr(int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval, int64_t *d_colorvec,
+                                 int64_t *n_colors, int64_t *n_rounds);
+fdb_status fdb_check_coloring_csr(int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec,
                                   int64_t *n_conflicts);
 
 /* ---- Jacobian-vector product: finite_difference_jvp!(jvp, f, x, v, cache::JVPCache, f_in; relstep, absstep, dir)
