@@ -125,9 +125,11 @@ ABI_SYMBOLS = {
     "fdb_oop_plan_create_block_banded": (_int, [_PP, _i64, _vp, _i64, _i64, _i64, _i64, _vp, _int, _i64,
                                                 C.POINTER(PlanOpts)]),
     "fdb_oop_plan_create_block_dense": (_int, [_PP, _i64, _vp, _i64, _i64, _vp, _int, _i64, C.POINTER(PlanOpts)]),
+    "fdb_oop_plan_create_csr": (_int, [_PP, _i64, _i64, _vp, _vp, _vp, _int, _i64, C.POINTER(PlanOpts)]),
     "fdb_jacobian_oop": (_int, [_vp, _vp, _vp, _vp, C.POINTER(OopOut), _vp, _vp, _f64, _f64, _f64, _vp]),
     "fdb_jacobian_oop_complex": (_int, [_vp, _vp, _vp, _vp, C.POINTER(OopOut), _vp]),
     "fdb_group_create_oop_csc": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _vp, _vp, _vp, _int, _i64, C.POINTER(PlanOpts)]),
+    "fdb_group_create_oop_csr": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _vp, _vp, _vp, _int, _i64, C.POINTER(PlanOpts)]),
     "fdb_group_create_oop_dense": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _vp, _i64, _int, _i64, C.POINTER(PlanOpts)]),
     "fdb_group_create_oop_banded": (_int, [_PP, _int, C.POINTER(_int), _i64, _i64, _i64, _i64, _vp, _int, _i64,
                                            C.POINTER(PlanOpts)]),

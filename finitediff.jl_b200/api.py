@@ -1122,16 +1122,19 @@ class JacobianCache:
         return _cached_plan(self, key, lambda: make_plan(J, sparsity, None if default_cv else colorvec, self.fdtype, x_len,
                                                          self.x1.device, **self._plan_kw))
 
-    def _oop_plan_for(self, kind, sparsity, colorvec, pn, m, n, device) -> Plan:
-        """The out-of-place plan (finite_difference_jacobian) for a result of `kind` with m rows and n = length(x); of
-        the plan keywords it takes max_batch and scratch_bytes."""
+    def _oop_plan_for(self, kind, sparsity, colorvec, pn, m, n, device, csr=False) -> Plan:
+        """The out-of-place plan (finite_difference_jacobian) for a result of `kind` with m rows and n = length(x) (csr:
+        a CSR result, which a CSC sparsity gives with a CSR prototype); of the plan keywords it takes max_batch and
+        scratch_bytes."""
         def create():
-            suffix, args, keep = _oop_plan_route(kind, sparsity, colorvec, pn, m, n)
+            suffix, args, keep = _oop_plan_route(kind, sparsity, colorvec, pn, m, n, csr)
             o = _opts(_fdtype_code(self.fdtype), _device_index(device),
                       **{k: v for k, v in self._plan_kw.items() if k in ("max_batch", "scratch_bytes")})
             with torch.cuda.device(device):
                 return Plan(_new_handle(f"fdb_oop_plan_create_{suffix}", *args, C.byref(o)).value)
         key = ("oop", kind, _sp_key(sparsity) if sparsity is not None else None, _index_key(colorvec), pn, m, n)
+        if csr:
+            key += ("csr",)
         return _cached_plan(self, key, create)
 
     def invalidate(self):
@@ -1419,8 +1422,23 @@ def _oop_block(sparsity):
     return None
 
 
+def _oop_csr(sparsity, jac_prototype):
+    """True when (sparsity, jac_prototype) gives a CSR result: a SparseMatrixCSR prototype with a SparseMatrixCSR or a
+    SparseMatrixCSC sparsity (fdb_oop_plan_create_csr).  Every other pairing with a CSR on either side is not built."""
+    return isinstance(jac_prototype, SparseMatrixCSR) and isinstance(sparsity, (SparseMatrixCSR, SparseMatrixCSC))
+
+
 def _oop_kind(sparsity, jac_prototype):
     """(result kind, m, ncols) the pair (sparsity, jac_prototype) gives; m / ncols None where f and colorvec decide."""
+    if isinstance(sparsity, SparseMatrixCSR) or isinstance(jac_prototype, SparseMatrixCSR):
+        if not _oop_csr(sparsity, jac_prototype):
+            raise TypeError(f"not built: a {type(sparsity).__name__} sparsity with a {type(jac_prototype).__name__} "
+                            "jac_prototype in the out-of-place Jacobian (a SparseMatrixCSR result takes a "
+                            "SparseMatrixCSR or SparseMatrixCSC sparsity and a SparseMatrixCSR jac_prototype)")
+        if jac_prototype.shape != sparsity.shape:
+            raise ValueError(f"jac_prototype is {jac_prototype.shape[0]}x{jac_prototype.shape[1]} but sparsity is "
+                             f"{sparsity.shape[0]}x{sparsity.shape[1]}")
+        return L.FDB_OOP_SPARSE, int(jac_prototype.shape[0]), int(jac_prototype.shape[1])
     block = _oop_block(sparsity) is not None and isinstance(jac_prototype, SparseMatrixCSC)
     if sparsity is not None and not isinstance(sparsity, SparseMatrixCSC) and _oop_band(sparsity) is None and not block:
         raise TypeError(f"not built: sparsity of type {type(sparsity).__name__} in the out-of-place Jacobian "
@@ -1445,11 +1463,29 @@ def _oop_kind(sparsity, jac_prototype):
     return L.FDB_OOP_RAW, None, None
 
 
-def _oop_plan_route(kind, sparsity, colorvec, pn, m, n):
+def _csr_of_csc(A):
+    """(rowptr, colval), Int64 and 1-based on the host: the CSR of a CSC pattern's entry set (scipy's O(nnz) transpose;
+    every stored entry kept, rows in order and columns ascending within a row)."""
+    import scipy.sparse as sps
+    cp = np.asarray(A.colptr.cpu() if isinstance(A.colptr, torch.Tensor) else A.colptr, dtype=np.int64) - 1
+    nnz = int(cp[-1]) if len(cp) else 0
+    rv = np.asarray(A.rowval.cpu() if isinstance(A.rowval, torch.Tensor) else A.rowval, dtype=np.int64)[:nnz] - 1
+    T = sps.csc_matrix((np.ones(nnz, dtype=np.int8), rv, cp), shape=(A.m, A.n)).tocsr()
+    return T.indptr.astype(np.int64) + 1, T.indices.astype(np.int64) + 1
+
+
+def _oop_plan_route(kind, sparsity, colorvec, pn, m, n, csr=False):
     """(suffix, args, keep) of the out-of-place plan for a result of `kind` with m rows and n = length(x): it is made by
     fdb_oop_plan_create_<suffix>(&h, *args, &opts) (or fdb_group_create_oop_<suffix>(&h, n_devices, devices, *args,
-    &opts)), and `keep` holds the host arrays the pointers in args point into."""
+    &opts)), and `keep` holds the host arrays the pointers in args point into.  csr: a CSR result (_oop_csr), whose plan
+    takes the CSR of the sparsity's entry set."""
     cvp, k0 = _index_ptr(None if _is_identity_colorvec(colorvec, n) else colorvec)
+    if csr:
+        rowptr, colval = (sparsity.rowptr, sparsity.colval) if isinstance(sparsity, SparseMatrixCSR) else \
+            _csr_of_csc(sparsity)
+        rp, k1 = _index_ptr(rowptr)
+        cv, k2 = _index_ptr(colval)
+        return "csr", (m, n, rp, cv, cvp, kind, max(m, 1)), [k0, k1, k2]
     band = _oop_band(sparsity)
     if band is not None:
         return "banded", (m, n, band[0], band[1], cvp, kind, max(m, 1)), [k0]
@@ -1498,16 +1534,17 @@ def _oop_fin_ptr(f_in, fd, m):
 class _OopOutput:
     """Device storage of an out-of-place result and the fdb_oop_out naming it.  ncols: the prototype's columns, else
     the quotient columns C = maximum(colorvec) of the whole result (dense branch); a sparse result holds up to m*C
-    candidates without a sparsity and nnz(sparsity) = n_entries with one."""
+    candidates without a sparsity and nnz(sparsity) = n_entries with one.  csr: a CSR result, whose pointer holds the
+    m + 1 row starts and whose stored indices are columns."""
 
-    def __init__(self, kind, sparsity, pn, m, C, n_entries, dev):
-        self.kind, self.m, self.dev = kind, m, dev
+    def __init__(self, kind, sparsity, pn, m, C, n_entries, dev, csr=False):
+        self.kind, self.m, self.dev, self.csr = kind, m, dev, csr
         self.ncols = pn if pn is not None else C
         self.out = L.OopOut()
         self.dense = None
         if kind == L.FDB_OOP_SPARSE:
             self.cap = m * C if sparsity is None else n_entries
-            self.colptr = torch.empty(self.ncols + 1, dtype=torch.int64, device=dev)
+            self.colptr = torch.empty((m if csr else self.ncols) + 1, dtype=torch.int64, device=dev)
             self.rowval = torch.empty(max(self.cap, 1), dtype=torch.int64, device=dev)
             self.nzval = torch.empty(max(self.cap, 1), dtype=torch.float64, device=dev)
             self.nnz = torch.empty(1, dtype=torch.int64, device=dev)
@@ -1519,8 +1556,9 @@ class _OopOutput:
             self.out.J = self.dense.data_ptr() if self.dense.numel() else _fx_ptr(self.dense)  # m = 0: nothing is written
 
     def result(self, stream):
-        """The dense tensor, or the SparseMatrixCSC sized to the kept entries (reading that count is the one host sync;
-        when most candidates were dropped its rowval / nzval are copied into storage of their own size)."""
+        """The dense tensor, or the SparseMatrixCSC (SparseMatrixCSR) sized to the kept entries (reading that count is the
+        one host sync; when most candidates were dropped its stored indices and nzval are copied into storage of their
+        own size)."""
         if self.kind != L.FDB_OOP_SPARSE:
             return self.dense
         _call(self.dev, (), L.lib().fdb_stream_sync, C.c_void_p(stream))
@@ -1528,6 +1566,8 @@ class _OopOutput:
         rowval, nzval = self.rowval[:nnz], self.nzval[:nnz]
         if 2 * nnz < self.cap:
             rowval, nzval = rowval.clone(), nzval.clone()
+        if self.csr:
+            return SparseMatrixCSR(self.m, self.ncols, self.colptr, rowval, nzval)
         return SparseMatrixCSC(self.m, self.ncols, self.colptr, rowval, nzval)
 
 
@@ -1554,9 +1594,14 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
                                     BlockSkylineMatrix sparsity with square blocks, whose structural entries are those of
                                     findstructralnz: closed-form plans (fdb_oop_plan_create_block_banded / _block_dense)
                                     build no entry list; a dense result of a block sparsity is not built
+        CSR / SparseMatrixCSR       SparseMatrixCSR (fdb_oop_plan_create_csr): the sparsity's stored entries whose value
+                                    is not +-0.0 (NaN kept), rows in order and each row in the sparsity's own storage
+                                    order; the values are the CSC route's bit for bit
+        CSC / SparseMatrixCSR       the same, for the CSR of the CSC's entry set (built on the host in O(nnz))
     A sparse result is sized to the kept entries: reading that count is the call's one host synchronisation (when most
     candidates were dropped its rowval / nzval are copied into storage of their own size).  Other sparsity / prototype
-    types and complex-valued results raise TypeError (not built).
+    types (a CSR sparsity with any other prototype, a CSR prototype with any other sparsity) and complex-valued results
+    raise TypeError (not built).
     Rows of the result: size(sparsity, 1) or size(jac_prototype, 1) when given; else those of f(x) — forward mode with a
     Python f evaluates it first, as the reference does (:299-300), and passes it on as f_in — or of f_in; else length of
     cache.fx (central and complex mode, and a NativeFn, whose output length the mirror cannot see before the device calls
@@ -1571,7 +1616,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
             stream = _stream(stream, x.device)
             if isinstance(f, NativeFn):
                 sp = None if sparsity is _DEFAULT else sparsity
-                m = sp.shape[0] if isinstance(sp, SparseMatrixCSC) or _oop_band(sp) is not None or \
+                m = sp.shape[0] if isinstance(sp, (SparseMatrixCSC, SparseMatrixCSR)) or _oop_band(sp) is not None or \
                     _oop_block(sp) is not None else (
                     jac_prototype.shape[0] if jac_prototype is not None else xv.numel())
                 xin = xv.to(torch.complex128) if _fdtype_code(fd) == L.FDB_COMPLEX else xv
@@ -1599,6 +1644,7 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
     colorvec = cache.colorvec if colorvec is None else colorvec                           # :284
     sparsity = cache.sparsity if sparsity is _DEFAULT else sparsity                       # :285
     kind, pm, pn = _oop_kind(sparsity, jac_prototype)
+    csr = _oop_csr(sparsity, jac_prototype)
     xv = x.reshape(-1)
     if not xv.is_contiguous():
         xv = xv.contiguous()
@@ -1607,8 +1653,8 @@ def finite_difference_jacobian(f, x, cache=None, f_in=None, returntype=None, *, 
         cache.x1.reshape(-1).copy_(xv)
     f_in, m = _oop_rows(f, x, fd, f_in, cache.fx.numel(), sparsity, pm, n)
     dev = x.device
-    plan = cache._oop_plan_for(kind, sparsity, colorvec, pn, m, n, dev)
-    res = _OopOutput(kind, sparsity, pn, m, plan.dense_range()[1], plan.info()["n_entries"], dev)
+    plan = cache._oop_plan_for(kind, sparsity, colorvec, pn, m, n, dev, csr)
+    res = _OopOutput(kind, sparsity, pn, m, plan.dense_range()[1], plan.info()["n_entries"], dev, csr)
     addr, ctx, pyfn = _as_fn(f, m, n, dev, 1, fd == L.FDB_COMPLEX, oop=True)
     stream = _stream(stream, dev)
     fin_ptr = _oop_fin_ptr(f_in, fd, m)

@@ -81,8 +81,8 @@ static BlockShape oop_block_shape(const fdb_plan *P) {
   return b;
 }
 
-// A block sparsity gives the sparse result only: a dense one would cost the m x n zero fill that the CSC route's entry
-// list already undercuts at any size where it fits
+// A block or CSR sparsity gives the sparse result only: a dense one would cost the m x n zero fill that the CSC route's
+// entry list already undercuts at any size where it fits
 static fdb_status oop_block_result(int result_kind, const char *what) {
   if (result_kind == FDB_OOP_DENSE)
     return fail(FDB_ERR_UNSUPPORTED, "not built: a dense out-of-place result of a %s sparsity (give a sparse prototype, "
@@ -92,7 +92,7 @@ static fdb_status oop_block_result(int result_kind, const char *what) {
   return FDB_OK;
 }
 
-// The out-of-place form of an in-place block plan: the sparse result over its |E| = colors.E candidates
+// The out-of-place form of an in-place block or CSR plan: the sparse result over its |E| = colors.E candidates
 static fdb_status oop_block_finish(PlanPtr &owner, fdb_plan **plan) {
   fdb_plan *P = owner.get();
   P->oop.on = 1;
@@ -265,6 +265,34 @@ fdb_status fdb_oop_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, con
   return oop_block_finish(owner, plan);
 }
 
+// A CSR sparsity: the in-place CSR plan (row pointer and columns as 0-based int32) plus, at the root, the first row
+// starting in every compaction tile.  The result is a CSR in the sparsity's own storage order.
+fdb_status fdb_oop_plan_create_csr(fdb_plan **plan, int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval,
+                                   const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
+  (void)ldJ;   // a sparse result has no leading dimension
+  if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
+  *plan = nullptr;
+  TRY(oop_block_result(result_kind, "CSR"));
+  if (n == 0) return fail(FDB_ERR_INVALID, "maximum(colorvec) of an empty colorvec: the reference throws");
+  if (opts && opts->world > 64) return fail(FDB_ERR_INVALID, "out-of-place plans take world <= 64");
+  fdb_plan_opts o = oop_opts(opts);
+  fdb_plan *raw = nullptr;
+  TRY(fdb_plan_create_csr(&raw, m, n, rowptr, colval, colorvec, &o));
+  PlanPtr owner(raw);
+  fdb_plan *P = owner.get();
+  DeviceGuard g(P->device);
+  if (P->rank == 0) {
+    const int64_t ntiles = (P->colors.E + kTile - 1) / kTile;
+    TRY(P->alloc_t(&P->oop.tile_col, (size_t)std::max<int64_t>(ntiles, 1)));
+    if (ntiles > 0) {
+      oop_tile_first_col<<<P->grid(ntiles), kThreads>>>(P->csr.rowptr, m, ntiles, P->oop.tile_col);
+      CU(cudaGetLastError());
+      CU(cudaDeviceSynchronize());
+    }
+  }
+  return oop_block_finish(owner, plan);
+}
+
 fdb_status fdb_oop_plan_create_dense(fdb_plan **plan, int64_t m, int64_t n, const int64_t *colorvec, int64_t ncols_out,
                                      int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
   if (!plan) return fail(FDB_ERR_INVALID, "plan output pointer is NULL");
@@ -385,6 +413,7 @@ static fdb_status oop_member(fdb_plan *P, fdb_fn f, void *ctx, const double *d_x
 static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const double *d_fx, const double *d_f_in,
                                   cudaStream_t s) {
   const bool full = P->sp_kind == SP_NONE, band = P->sp_kind == SP_BANDED, block = P->sp_kind == SP_BLOCKBAND;
+  const bool csr = P->sp_kind == SP_CSR;
   const int64_t candidates = oop_candidates(P);
   DeviceGuard g(P->device);
   const int64_t ntiles = (candidates + kTile - 1) / kTile;
@@ -398,10 +427,22 @@ static fdb_status oop_root_finish(fdb_plan *P, const fdb_oop_out *out, const dou
   a.colptr = out->colptr; a.rowval = out->rowval; a.nzval = out->nzval; a.nnz = out->nnz;
   a.state = P->oop.state; a.claim = P->oop.state + ntiles; a.tile_col = P->oop.tile_col;
   if (band) a.band = oop_band_shape(P);
+  // a CSR result: the columns are the stored index and the row starts the pointer written (out->colptr gets m + 1)
+  if (csr) { a.row32 = P->csr.colval; a.colptr32 = P->csr.rowptr; a.ncols = P->m; }
   auto go = [&](auto kern, auto... cs) {
     kern<<<resident_grid(P, kern, 0, std::max<int64_t>(ntiles, 1)), kThreads, 0, s>>>(a, cs...);
   };
   if (full) go(oop_compact<true, kCopy, uint8_t>);
+  else if (csr && P->oop.fused) TRY(dispatch_mode(P->fdtype, [&](auto mode) {
+    return dispatch_ct(P->colors.bits, [&](auto tag) {
+      return dispatch_colors<decltype(tag)>(P, [&](auto cs) -> fdb_status {
+        go(oop_compact_csr<decltype(mode)::value, decltype(cs)>, cs);
+        return FDB_OK;
+      });
+    });
+  }));
+  // the candidates the CSR scatters wrote in slot order: the CSC copy over (colval, rowptr) is the CSR copy
+  else if (csr) go(oop_compact<false, kCopy, uint8_t>);
   else if (block) {
     // the candidates from the block scatters' buffer (kCopy), or the quotients from the resident f! outputs
     const BlockShape b = oop_block_shape(P);
@@ -509,6 +550,14 @@ fdb_status fdb_group_create_oop_block_dense(fdb_group **group, int n_devices, co
                                            int result_kind, int64_t ldJ, const fdb_plan_opts *opts) {
   return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
     return fdb_oop_plan_create_block_dense(p, nblocks, blocks, l, u, colorvec, result_kind, ldJ, o);
+  });
+}
+
+fdb_status fdb_group_create_oop_csr(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                    const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec, int result_kind,
+                                    int64_t ldJ, const fdb_plan_opts *opts) {
+  return group_create(group, n_devices, devices, opts, [&](int, const fdb_plan_opts *o, fdb_plan **p) {
+    return fdb_oop_plan_create_csr(p, m, n, rowptr, colval, colorvec, result_kind, ldJ, o);
   });
 }
 

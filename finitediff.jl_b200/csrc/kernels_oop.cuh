@@ -11,6 +11,7 @@
 #include "common.cuh"
 #include "kernels_scatter.cuh"
 #include "kernels_blockband.cuh"
+#include "kernels_csr.cuh"
 
 namespace fdb {
 
@@ -62,8 +63,12 @@ oop_dense_finish(double *__restrict__ J, int64_t ldJ, int64_t m, int64_t C, int6
 //              of column c, stride l + u + 1), as the in-place band scatter writes them.
 //   kFormBlockBand / kFormBlockDense: the entry set of a BandedBlockBandedMatrix / BlockSkylineMatrix with square blocks,
 //              in closed form from the block offsets (BlockShape, BlockBandForm, BlockDenseForm below).
+//   kFormCsr:  a CSR pattern's entries in row order (CsrForm below): candidate e is slot e, row32[e] its 0-based column
+//              (the stored minor index), colptr32 the 0-based row pointer and ncols = m, so the pointer pass below writes
+//              the row starts.  Only the quotient modes use it: kCopy has no use for the row, and the kFormCsc pass over
+//              (colval, rowptr) is already the CSR copy.
 constexpr uint64_t kLbAggregate = 1ull << 62, kLbPrefix = 2ull << 62, kLbValue = (1ull << 62) - 1;
-enum { kFormCsc = 0, kFormFull = 1, kFormBand = 2, kFormBlockBand = 3, kFormBlockDense = 4 };
+enum { kFormCsc = 0, kFormFull = 1, kFormBand = 2, kFormBlockBand = 3, kFormBlockDense = 4, kFormCsr = 5 };
 
 // The in-matrix band E(m, n, l, u) = {(r, c) : -u <= r - c <= l, 0 <= r < m, 0 <= c < n} (0-based), l, u >= 0, clamped to
 // l <= m - 1, u <= n - 1 (the same set).  Column c holds rows max(0, c - u) .. min(m - 1, c + l); columns c >= m + u are
@@ -136,15 +141,15 @@ struct CompactArgs {
   const double *Fp, *Fm, *fx, *eps;   // resident f! outputs [C][ldF], central minus outputs, f(x), step sizes [C]
   int64_t ldF;               // doubles between two colours' outputs
   int32_t ncolors;
-  const int32_t *row32;      // [E] 0-based rows (kFormCsc)
-  const int32_t *colptr32;   // [ncols + 1] 0-based column starts (kFormCsc)
+  const int32_t *row32;      // [E] 0-based rows (kFormCsc; kFormCsr: columns)
+  const int32_t *colptr32;   // [ncols + 1] 0-based column starts (kFormCsc; kFormCsr: row starts, ncols = m)
   int64_t E, m, C, ncols;
   int64_t *colptr, *rowval;  // outputs: [ncols + 1], [<= E]  (1-based)
   double *nzval;             // [<= E]
   int64_t *nnz;              // kept count
   unsigned long long *state; // [ntiles] look-back words, zeroed before the launch
   unsigned long long *claim; // tile counter, zeroed before the launch
-  const int32_t *tile_col;   // [ntiles] first column starting at or after the tile's first entry (kFormCsc)
+  const int32_t *tile_col;   // [ntiles] first column (kFormCsr: row) starting at or after the tile's first entry
   BandShape band;            // kFormBand
 };
 
@@ -197,6 +202,7 @@ __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs
     if (tile >= ntiles) return;
     const int64_t t0 = tile * kTile;
     if constexpr (kBlock) cs.begin_tile(a.E, t0);   // (synchronises the block)
+    if constexpr (FORM == kFormCsr) cs.begin_tile(a, t0);
     // element (round u, warp w, lane) = t0 + u*kThreads + w*32 + lane: (u, w, lane) order is storage order
     double v[kRounds];
     int32_t r[kRounds];
@@ -217,6 +223,20 @@ __device__ __forceinline__ void compact_tiles(const CompactArgs &a, const CS &cs
                      ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx,
                                          row, __ldg(a.eps + k))
                      : 0.0;
+      } else if constexpr (FORM == kFormCsr) {
+        // the stored index is the column; the quotient is read at the entry's row
+        int32_t row = 0, c = 0;
+        uint32_t k = 0xFFFFFFFFu;
+        if (in) {
+          c = __ldcs(a.row32 + e);
+          row = cs.row_of(a, (int32_t)e);
+          k = cs.colors.at(c);
+        }
+        r[u] = c;
+        v[u] = k < (uint32_t)a.ncolors
+                   ? fd_quotient<MODE>(a.Fp + (int64_t)k * a.ldF, MODE == kCentral ? a.Fm + (int64_t)k * a.ldF : a.fx, row,
+                                       __ldg(a.eps + k))
+                   : 0.0;
       } else {
         int64_t bc = 0, br = 0;                      // kFormBand: the candidate's column and row
         if (FORM == kFormBand) {
@@ -575,6 +595,50 @@ __global__ void __launch_bounds__(kThreads)
 oop_compact_block_dense(const CompactArgs a, const BlockShape b) {
   __shared__ BlockDenseTile s_t;
   compact_tiles<kFormBlockDense, MODE>(a, BlockDenseForm<CT>{b, &s_t});
+}
+
+// ---- the CSR form ----
+// A CSR pattern's entries in storage order (row order; columns within a row, repeats included, as stored).  The row of a
+// candidate is found as diff_scatter_csr finds it: the tile's first and last rows by a search of the row pointer, once;
+// their starts staged in shared memory when the tile spans at most kTile rows, and searched there; otherwise (long runs
+// of empty rows) rowptr[rlo..rhi] is searched in global memory.
+struct CsrTile {
+  int32_t ptr[kTile];          // row starts rowptr[rlo .. rhi], staged
+  int32_t rlo, rhi;
+};
+
+template <typename CS>
+struct CsrForm {
+  CS colors;                   // the colour of a column: the cyclic closed form or the table
+  CsrTile *t;
+
+  __device__ __forceinline__ void begin_tile(const CompactArgs &a, int64_t t0) const {
+    if (threadIdx.x < 2) {
+      const int64_t s = threadIdx.x == 0 ? t0 : (t0 + kTile < a.E ? t0 + kTile : a.E) - 1;
+      const int32_t r = csr_row_of(a.colptr32, 0, (int32_t)a.ncols - 1, (int32_t)s);
+      if (threadIdx.x == 0) t->rlo = r;
+      else t->rhi = r;
+    }
+    __syncthreads();
+    const int32_t rlo = t->rlo, rhi = t->rhi;
+    if (rhi - rlo < kTile)
+      for (int i = threadIdx.x; i <= rhi - rlo; i += kThreads) t->ptr[i] = __ldg(a.colptr32 + rlo + i);
+    __syncthreads();
+  }
+
+  __device__ __forceinline__ int32_t row_of(const CompactArgs &a, int32_t e) const {
+    const int32_t rlo = t->rlo, rhi = t->rhi;
+    return rhi - rlo < kTile ? rlo + csr_row_of(t->ptr, 0, rhi - rlo, e) : csr_row_of(a.colptr32, rlo, rhi, e);
+  }
+};
+
+// A CSR pattern (kFormCsr), per-column colours from CS; quotient modes only
+template <int MODE, typename CS>
+__global__ void __launch_bounds__(kThreads)
+oop_compact_csr(const CompactArgs a, const CS cs) {
+  static_assert(MODE != kCopy, "the CSR copy is oop_compact<false, kCopy> over (colval, rowptr)");
+  __shared__ CsrTile s_t;
+  compact_tiles<kFormCsr, MODE>(a, CsrForm<CS>{cs, &s_t});
 }
 
 // Plan time, block-banded result: the entries of E in every block column, sum_K band_col_start(m_K, lam, mu, cb[J])

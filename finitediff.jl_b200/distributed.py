@@ -420,6 +420,7 @@ class GroupJacobianOOP(_Group):
         self._set_devices(devices)
         self.fdtype, self.colorvec, self.sparsity, self.jac_prototype = fdtype, colorvec, sparsity, jac_prototype
         self.kind, self.pm, self.pn = api._oop_kind(sparsity, jac_prototype)
+        self.csr = api._oop_csr(sparsity, jac_prototype)
         self._code = api._fdtype_code(fdtype)
         self._plan_kw = plan_kw
         self._key = None
@@ -430,7 +431,8 @@ class GroupJacobianOOP(_Group):
         if self._key is not None:
             self.close()
         o = api._opts(self._code, self.devices[0], **self._plan_kw)
-        suffix, args, self._keep = api._oop_plan_route(self.kind, self.sparsity, self.colorvec, self.pn, m, n)
+        suffix, args, self._keep = api._oop_plan_route(self.kind, self.sparsity, self.colorvec, self.pn, m, n,
+                                                            self.csr)
         with torch.cuda.device(self.root):
             self._create(f"oop_{suffix}", o, *args)
         self._key = (m, n)
@@ -441,7 +443,8 @@ class GroupJacobianOOP(_Group):
         devices[0]) is never modified.  In forward mode without f_in, f(x) is evaluated once, by fs[0] at the root, and
         passed on as f_in (jacobians.jl:299-300), so the members evaluate only their colours.  Rows of the result: those
         of the sparsity or prototype, else of f_in or f(x), else length(x).  Returns what finite_difference_jacobian
-        returns: a dense column-major tensor, or a SparseMatrixCSC sized to the kept entries (one host sync)."""
+        returns: a dense column-major tensor, or a SparseMatrixCSC (SparseMatrixCSR with a CSR prototype) sized to the kept
+        entries (one host sync)."""
         if not api._is_cuda(x) or x.dtype != torch.float64 or x.device != self.root:
             raise TypeError(f"x must be a float64 CUDA tensor on {self.root}")
         if len(fs) != len(self.devices):
@@ -456,7 +459,7 @@ class GroupJacobianOOP(_Group):
                 api._native_call(fs[0], f_in, xv, stream)
         self._build(m, n)
         res = api._OopOutput(self.kind, self.sparsity, self.pn, m, self.plans[-1].dense_range()[1],
-                             self.plans[0].info()["n_entries"], self.root)
+                             self.plans[0].info()["n_entries"], self.root, self.csr)
         addr, ctxs, pyfns = self._member_fns(fs, m, n, oop=True)
         api._call(self.root, pyfns, L.lib().fdb_group_jacobian_oop, self._h, addr, ctxs, xv.data_ptr(), C.byref(res.out),
                   None, api._oop_fin_ptr(f_in, self._code, m), *api._steps(relstep, absstep), float(dir),

@@ -1108,6 +1108,47 @@ function oop_block_plan(anchor, B::DeviceBlockDense, kind::Cint, colorvec, fd::C
     end
 end
 
+# CSR results (fdb_oop_plan_create_csr): a DeviceCSR prototype with a DeviceCSR sparsity, or with a CSC one whose entry set
+# is converted to CSR.  oopcsr gives the pattern the plan is made from (the DeviceCSR, or the host SparseMatrixCSC), else
+# nothing; every other pairing with a DeviceCSR on either side throws ArgumentError, and a prototype of another size
+# DimensionMismatch (the mirror's ValueError).
+function oopcsr(sparsity, jac_prototype)
+    sparsity isa DeviceCSR || jac_prototype isa DeviceCSR || return nothing
+    jac_prototype isa DeviceCSR && sparsity isa Union{DeviceCSR, SparseMatrixCSC, DeviceCSC} ||
+        throw(ArgumentError("not built: a $(typeof(sparsity)) sparsity with a $(typeof(jac_prototype)) jac_prototype " *
+                            "(a DeviceCSR result takes a DeviceCSR, DeviceCSC or SparseMatrixCSC sparsity)"))
+    size(jac_prototype) == size(sparsity) ||
+        throw(DimensionMismatch("jac_prototype is $(size(jac_prototype)) but sparsity is $(size(sparsity))"))
+    sparsity isa DeviceCSR ? sparsity : hostcsc(sparsity)
+end
+
+# the arrays that identify a CSR result's pattern (the plan cache's anchor and key), and the CSR arrays the plan takes:
+# a DeviceCSR's own, or the CSR of a CSC's entry set (copy(transpose(A)): O(nnz), every stored entry kept, columns
+# ascending in a row), built only when a plan is made
+csrid(A::DeviceCSR) = (A.rowptr, A.colval)
+csrid(A::SparseMatrixCSC) = (A.colptr, A.rowval)
+csrarrays(A::DeviceCSR) = (A.rowptr, A.colval)
+function csrarrays(A::SparseMatrixCSC)
+    T = copy(transpose(A))
+    (CuVector{Int64}(T.colptr), CuVector{Int64}(T.rowval))
+end
+
+function oop_csr_plan(src, m::Integer, n::Integer, colorvec, fd::Cint)
+    anchor, second = csrid(src)
+    cached_plan(anchor, (:oop_csr, m, n, objectid(second), color_key(colorvec), fd)) do
+        rowptr, colval = csrarrays(src)
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        opts = Ref(PlanOpts(fd))
+        cptr, croot = color_arg(colorvec, n)
+        GC.@preserve croot rowptr colval begin
+            check(ccall((:fdb_oop_plan_create_csr, libfdjac), Cint,
+                (Ref{Ptr{Cvoid}}, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+                h, m, n, pointer(rowptr), pointer(colval), cptr, FDB_OOP_SPARSE, max(m, 1), opts))
+        end
+        Plan(h[], (rowptr, colval, croot))
+    end
+end
+
 """
     finite_difference_jacobian(f, x::CuVector{Float64}, cache::JacobianCache, f_in = nothing;
                                relstep, absstep, colorvec, sparsity, jac_prototype, dir)
@@ -1116,7 +1157,9 @@ end
 a dense `CuMatrix` (raw quotients without either, `0.0 + dx` with a dense prototype or a CSC sparsity) or, with a sparse
 prototype, a `DeviceCSC` holding the entries whose value is not ±0.0 (its pattern is copied back to the host: reading the
 kept count is the call's one synchronisation).  A `DeviceBlockBanded` or `DeviceBlockDense` sparsity takes a sparse
-prototype only (a dense result of it throws `ArgumentError`).  `cache.x1` receives a copy of x (:293-295).
+prototype only (a dense result of it throws `ArgumentError`).  A `DeviceCSR` prototype with a `DeviceCSR`, `DeviceCSC` or
+`SparseMatrixCSC` sparsity gives a `DeviceCSR` of the kept entries, rows in order and each row in the sparsity's storage
+order (fdb_oop_plan_create_csr; a CSC sparsity is converted on the host).  `cache.x1` receives a copy of x (:293-295).
 """
 function finite_difference_jacobian(f, x::CuVector{Float64},
         cache::JacobianCache{T1, T2, T3, T4, cType, sType, fdtype, returntype}, f_in = nothing;
@@ -1124,15 +1167,18 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
         jac_prototype = nothing, dir = true) where {T1, T2, T3, T4, cType, sType, fdtype, returntype}
     cache.x1 === x || copyto!(cache.x1, x)
     n = length(x)
-    band = sparsity === nothing ? nothing : oopband(sparsity)
-    block = sparsity === nothing ? nothing : oopblock(sparsity)
-    sp = sparsity === nothing || band !== nothing || block !== nothing ? nothing : hostcsc(sparsity)
-    m = band !== nothing ? band[1] : block !== nothing ? size(block, 1) : sp !== nothing ? size(sp, 1) :
-        (f_in !== nothing ? length(f_in) : length(cache.fx))
+    csr = oopcsr(sparsity, jac_prototype)
+    band = sparsity === nothing || csr !== nothing ? nothing : oopband(sparsity)
+    block = sparsity === nothing || csr !== nothing ? nothing : oopblock(sparsity)
+    sp = sparsity === nothing || band !== nothing || block !== nothing || csr !== nothing ? nothing : hostcsc(sparsity)
+    m = csr !== nothing ? size(sparsity, 1) : band !== nothing ? band[1] : block !== nothing ? size(block, 1) :
+        sp !== nothing ? size(sp, 1) : (f_in !== nothing ? length(f_in) : length(cache.fx))
     block !== nothing && !(jac_prototype isa SparseMatrixCSC || jac_prototype isa DeviceCSC) &&
         throw(ArgumentError("not built: a dense out-of-place result of a $(typeof(block)) sparsity (give a sparse " *
                             "jac_prototype, or a CSC sparsity)"))
-    if jac_prototype === nothing
+    if csr !== nothing
+        kind, ncols = FDB_OOP_SPARSE, n
+    elseif jac_prototype === nothing
         kind, ncols = sp === nothing && band === nothing ? (FDB_OOP_RAW, 0) : (FDB_OOP_DENSE, n)
     elseif jac_prototype isa AbstractMatrix && !(jac_prototype isa SparseMatrixCSC)
         kind, ncols = FDB_OOP_DENSE, size(jac_prototype, 2)
@@ -1140,7 +1186,8 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
         kind, ncols = FDB_OOP_SPARSE, size(hostcsc(jac_prototype), 2)
     end
     fd = fdcode(fdtype)
-    plan = band !== nothing ? oop_band_plan(cache, band, kind, colorvec, fd) :
+    plan = csr !== nothing ? oop_csr_plan(csr, m, n, colorvec, fd) :
+           band !== nothing ? oop_band_plan(cache, band, kind, colorvec, fd) :
            block !== nothing ? oop_block_plan(cache, block, kind, colorvec, fd) :
            oop_plan(sp === nothing ? cache : sp.colptr, sp, m, n, kind, ncols, colorvec, fd)
     pinfo = info(plan)
@@ -1149,8 +1196,10 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     J = nothing
     colptr = rowval = nzval = nnz = nothing
     if kind == FDB_OOP_SPARSE
-        cap = sp === nothing && band === nothing && block === nothing ? m * pinfo.n_local_colors : pinfo.n_entries
-        colptr, rowval = CuVector{Int64}(undef, ncols + 1), CuVector{Int64}(undef, max(cap, 1))
+        cap = sp === nothing && band === nothing && block === nothing && csr === nothing ? m * pinfo.n_local_colors :
+              pinfo.n_entries
+        # a CSR result: colptr receives the m + 1 row starts and rowval the columns
+        colptr, rowval = CuVector{Int64}(undef, (csr === nothing ? ncols : m) + 1), CuVector{Int64}(undef, max(cap, 1))
         nzval, nnz = CuVector{Float64}(undef, max(cap, 1)), CuVector{Int64}(undef, 1)
         out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), cap, pointer(nnz)))
     else
@@ -1178,6 +1227,7 @@ function finite_difference_jacobian(f, x::CuVector{Float64},
     check(rc)
     kind == FDB_OOP_SPARSE || return m == 0 ? J[1:0, :] : J
     k = Int(Array(nnz)[1])                                     # the one host synchronisation
+    csr === nothing || return DeviceCSR(m, n, colptr, rowval[1:k], nzval[1:k])
     host = SparseMatrixCSC(m, ncols, Array(colptr), Array(rowval[1:k]), zeros(k))
     DeviceCSC(host, nzval[1:k])
 end
@@ -1194,6 +1244,7 @@ mutable struct OopGroup
     ncols::Int         # columns of the result (the prototype's, else maximum(colorvec))
     cap::Int           # candidate entries of a sparse result
     fdtype::Any
+    csr::Bool          # a DeviceCSR result (group_oop_csr): the pointer holds the m + 1 row starts
 end
 
 function oop_group_result(h, devices, roots, kind, m, n, ncols, fdtype)
@@ -1206,7 +1257,7 @@ function oop_group_result(h, devices, roots, kind, m, n, ncols, fdtype)
     b, e = Ref{Int64}(0), Ref{Int64}(0)
     check(ccall((:fdb_plan_dense_range, libfdjac), Cint, (Ptr{Cvoid}, Ref{Int64}, Ref{Int64}), pl[], b, e))
     kind == FDB_OOP_RAW && (ncols = e[])                       # C of the whole result: where the last block ends
-    OopGroup(g, kind, m, n, ncols, i0[].n_entries, fdtype)
+    OopGroup(g, kind, m, n, ncols, i0[].n_entries, fdtype, false)
 end
 
 # sparsity: a CSC pattern (SparseMatrixCSC or DeviceCSC); jac_prototype: nothing, a dense matrix or a sparse one
@@ -1276,6 +1327,23 @@ function group_oop_block_dense(B::DeviceBlockDense, colorvec, fdtype, devices::V
     oop_group_result(h, devices, croot, FDB_OOP_SPARSE, n, n, n, fdtype)
 end
 
+# sparsity: a DeviceCSR, or a CSC pattern (converted on the host); jac_prototype: a DeviceCSR of the same size
+function group_oop_csr(sparsity, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
+    rowptr, colval = csrarrays(oopcsr(sparsity, jac_prototype))
+    m, n = size(sparsity)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    opts = Ref(PlanOpts(fdcode(fdtype); kw...))
+    cptr, croot = color_arg(colorvec, n)
+    GC.@preserve rowptr colval croot devices begin
+        check(ccall((:fdb_group_create_oop_csr, libfdjac), Cint,
+            (Ref{Ptr{Cvoid}}, Cint, Ptr{Cint}, Int64, Int64, CuPtr{Int64}, CuPtr{Int64}, Ptr{Int64}, Cint, Int64, Ref{PlanOpts}),
+            h, length(devices), pointer(devices), m, n, pointer(rowptr), pointer(colval), cptr, FDB_OOP_SPARSE, max(m, 1), opts))
+    end
+    g = oop_group_result(h, devices, (rowptr, colval, croot), FDB_OOP_SPARSE, m, n, n, fdtype)
+    g.csr = true
+    g
+end
+
 # sparsity === nothing: m rows (length of f(x)), n = length(x)
 function group_oop_dense(m::Integer, n::Integer, colorvec, fdtype, devices::Vector{Cint}; jac_prototype = nothing, kw...)
     if jac_prototype === nothing
@@ -1312,7 +1380,7 @@ function group_jacobian(g::OopGroup, fs::Vector, x::CuVector{Float64}; f_in = no
     J = nothing
     colptr = rowval = nzval = nnz = nothing
     if g.kind == FDB_OOP_SPARSE
-        colptr, rowval = CuVector{Int64}(undef, g.ncols + 1), CuVector{Int64}(undef, max(g.cap, 1))
+        colptr, rowval = CuVector{Int64}(undef, (g.csr ? g.m : g.ncols) + 1), CuVector{Int64}(undef, max(g.cap, 1))
         nzval, nnz = CuVector{Float64}(undef, max(g.cap, 1)), CuVector{Int64}(undef, 1)
         out = Ref(OopOut(CU_NULL, pointer(colptr), pointer(rowval), pointer(nzval), g.cap, pointer(nnz)))
     else
@@ -1334,6 +1402,7 @@ function group_jacobian(g::OopGroup, fs::Vector, x::CuVector{Float64}; f_in = no
     check(rc)
     g.kind == FDB_OOP_SPARSE || return g.m == 0 ? J[1:0, :] : J
     k = Int(Array(nnz)[1])                                     # the one host synchronisation
+    g.csr && return DeviceCSR(g.m, g.n, colptr, rowval[1:k], nzval[1:k])
     host = SparseMatrixCSC(g.m, g.ncols, Array(colptr), Array(rowval[1:k]), zeros(k))
     DeviceCSC(host, nzval[1:k])
 end

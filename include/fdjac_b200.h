@@ -164,8 +164,8 @@ double fdb_compute_epsilon(int fdtype, double x, double relstep, double absstep,
  *   fdb_jacobian_complex              coloured and dense plans, fdtype complex
  *   fdb_jacobian_oop                  out-of-place plans, fdtype forward / central
  *   fdb_jacobian_oop_complex          out-of-place plans, fdtype complex
- *   fdb_color_eps                     coloured plans (out-of-place CSC included) and step-size plans
- *   fdb_plan_set_external_eps         coloured plans (out-of-place CSC included)
+ *   fdb_color_eps                     coloured plans (out-of-place CSC, band, block and CSR included) and step-size plans
+ *   fdb_plan_set_external_eps         coloured plans (out-of-place CSC, band, block and CSR included)
  *   fdb_plan_set_peers                CSC, COO, JVP and step-size plans (else FDB_ERR_UNSUPPORTED)
  *   fdb_plan_color_owner              every plan but dense, Hessian and derivative plans
  *   fdb_plan_get_eps                  every plan but derivative plans
@@ -555,13 +555,24 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   bandwidths and the block list are refused as by the in-place block creators.  Host work is O(nblocks) plus reading the
  *   colorvec, and no entry, row or column-start list exists: the compaction finds each candidate's column and row from the
  *   block offsets and one table of nblocks + 1 block-column starts.  Candidate counts may pass 2^31.
+ * fdb_oop_plan_create_csr: the sparsity is one CSR pattern (m x n, rowptr[m+1], colval[nnz]; Int64, 1-based, host or
+ *   device), and the result a CSR.  Only result_kind FDB_OOP_SPARSE is built (ldJ is ignored); FDB_OOP_DENSE is
+ *   FDB_ERR_UNSUPPORTED and FDB_OOP_RAW FDB_ERR_INVALID; sizes, the row pointer, the columns and nnz >= 2^31 are refused
+ *   as by fdb_plan_create_csr.  The candidates are the stored entries, one per slot; a candidate is kept when its value is
+ *   not +-0.0 (NaN is kept), and each kept value is bit-identical to what fdb_oop_plan_create_csc gives for the same
+ *   (row, column) on the CSC of the same entry set.  Rows come in order and, within a row, the kept entries keep the
+ *   pattern's own storage order (unsorted columns stay unsorted; a repeated (r, c) gives two entries of one value), so for
+ *   rows of sorted, distinct columns the result is the CSC route's result converted to CSR.  f! calls and points are the
+ *   CSC route's.  With more than 8 colours the step sizes come from per-colour column lists, as the CSC plan's do.
  * n = 0 is FDB_ERR_INVALID (maximum of an empty colorvec throws).  opts as for the in-place plans (rank plans below).
  * fdb_jacobian_oop / fdb_jacobian_oop_complex write the result to `out`:
  *   dense kinds: out->J (device, ldJ of the plan; the whole result, rank plans included);
  *   FDB_OOP_SPARSE: out->colptr [ncols + 1], out->rowval / out->nzval [out->cap >= the candidate count: nnz of the sparsity,
  *   or m*C], Int64 1-based; the kept count goes to the device scalar *out->nnz (stream-ordered, no host sync).
- * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a sparsity,
- * |E| with a band or a block structure).
+ *   A CSR plan writes the same fields in row-compressed form: out->colptr receives the m + 1 row starts and out->rowval
+ *   the column of every kept entry (Int64, 1-based), with out->cap >= nnz.
+ * fdb_plan_info(...).n_entries is the candidate count of the whole result (m*C on the dense branch, nnz with a CSC or CSR
+ * sparsity, |E| with a band or a block structure); a CSR plan reports jkind FDB_J_CSR.
  *
  * Rank plans (opts.rank / opts.world, world in 2..64).  A rank evaluates only the colours it owns: the colour partition of
  * the in-place plans (opts.partition: round-robin or LPT, fdb_plan_color_owner) with a sparsity, the contiguous column
@@ -581,6 +592,9 @@ fdb_status fdb_derivative_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, double 
  *   FDB_OOP_SPARSE, block       its colours' columns into the root's buffer in the in-place layout (band data for
  *                               block-banded, slabs for block-dense; rank 0 also writes the zeros of columns without a valid
  *                               colour); the root then compacts every entry of E into `out`;
+ *   FDB_OOP_SPARSE, CSR         its colours' candidate quotients, in slot order, into the root's candidate buffer (rank 0
+ *                               also writes the zeros of columns without a valid colour); the root then compacts all nnz
+ *                               candidates into `out`;
  *   FDB_OOP_SPARSE, no sparsity its column block of the m x C candidates at offset col_begin*m; the root then compacts all
  *                               m*C of them.
  * Per rank: forward mode without d_f_in evaluates f(x) first, then its own colours ascending; central f(x+) then f(x-) per
@@ -612,6 +626,8 @@ fdb_status fdb_oop_plan_create_block_banded(fdb_plan **plan, int64_t nblocks, co
                                             const fdb_plan_opts *opts);
 fdb_status fdb_oop_plan_create_block_dense(fdb_plan **plan, int64_t nblocks, const int64_t *blocks, int64_t l, int64_t u,
                                            const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_oop_plan_create_csr(fdb_plan **plan, int64_t m, int64_t n, const int64_t *rowptr, const int64_t *colval,
+                                   const int64_t *colorvec, int result_kind, int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_jacobian_oop(fdb_plan *plan, fdb_fn f, void *ctx, const double *d_x, const fdb_oop_out *out, double *d_fx,
                             const double *d_f_in, double relstep, double absstep, double dir, void *stream);
 fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const double *d_x, const fdb_oop_out *out,
@@ -629,6 +645,9 @@ fdb_status fdb_jacobian_oop_complex(fdb_plan *plan, fdb_fn_c f, void *ctx, const
  * group, return FDB_ERR_INVALID before any launch. */
 fdb_status fdb_group_create_oop_csc(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
                                     const int64_t *colptr, const int64_t *rowval, const int64_t *colorvec, int result_kind,
+                                    int64_t ldJ, const fdb_plan_opts *opts);
+fdb_status fdb_group_create_oop_csr(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
+                                    const int64_t *rowptr, const int64_t *colval, const int64_t *colorvec, int result_kind,
                                     int64_t ldJ, const fdb_plan_opts *opts);
 fdb_status fdb_group_create_oop_dense(fdb_group **group, int n_devices, const int *devices, int64_t m, int64_t n,
                                       const int64_t *colorvec, int64_t ncols_out, int result_kind, int64_t ldJ,
